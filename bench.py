@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- BM25 queries/s of the batched posting-traversal path (BASELINE.json configs[1]):
-10M-doc synthetic Zipf corpus, 1024 three-term disjunctive queries, top-100, on N B200s.
+10M-doc synthetic Zipf corpus, 1024 three-term disjunctive queries, top-100, on N H100s.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload bm25|conj|knn|hybrid]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload bm25|conj|knn|hybrid] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the hot path over the 1024-query batch. `value` = whole-job queries/s with the compiled batch
@@ -13,9 +13,16 @@ BM25 statistics all-reduced at build time); every step ends with ONE NCCL all-ga
 
 Every number is gated: before timing, the results of the first `--cpu-sample` queries are compared bit for bit with the CPU
 oracle (at N > 1 the MERGED page against the oracle run on the whole corpus by rank 0). The default N = 1 line also carries
-`extra.conj` (configs[2]) and `extra.knn` (configs[3]), each with its own gate and roofline.
+`extra.conj` (configs[2]) and `extra.knn` (configs[3]), each with its own gate and roofline; every leg times --steps steps.
+
+--dump-outputs DIR writes, after the timed steps, the page the timed path returned in its last step (doc ids, scores, hit
+counts, ...) as DIR/<name>.npy in float64 (float32 for scores), so that two builds can be compared output for output: the
+inputs are generated from fixed seeds and are the same in every run with the same arguments.
+A totalHits whose relation is GREATER_THAN_OR_EQUAL_TO (flags bit 0) is a lower bound that depends on the pruning order;
+compare it only where the relation is EQUAL_TO.
 """
 import argparse
+import atexit
 import ctypes
 import json
 import os
@@ -54,26 +61,30 @@ def parse():
     ap.add_argument("--hybrid-dims", type=int, default=128)
     ap.add_argument("--vectors", type=int, default=1_000_000)
     ap.add_argument("--dims", type=int, default=768)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's results as DIR/<name>.npy (float32 / float64)")
     return ap.parse_args()
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: {name: array} of what the timed path returned in its last step. Integer arrays (doc ids, counts, totalHits,
+    flags) are stored as float64, which holds them exactly; float scores stay float32."""
+    if not out_dir:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    conv = {n: np.ascontiguousarray(a, dtype=np.float32 if np.asarray(a).dtype == np.float32 else np.float64) for n, a in arrays.items()}
+    total = sum(a.nbytes for a in conv.values())
+    assert total <= DUMP_LIMIT_BYTES, f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT_BYTES}-byte limit"
+    for n, a in conv.items():
+        np.save(os.path.join(out_dir, f"{n}.npy"), a)
+
+
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            p = json.load(f)
-        return p, "measured (MEASURED_PEAKS.json)"
-    except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback (B200_PROFILING.md)"
-
-
-def static_traffic(name):
-    """Physical DRAM bytes per launch from the committed ncu --set full capture of this exact workload (a STATIC figure:
-    the bench cannot run under the profiler). Returns (bytes, source) or (None, None)."""
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))[name]
-        return tr["dram_bytes_read"] + tr["dram_bytes_write"], "static: profiles/r2_traffic.json (%s)" % tr["source"]
-    except Exception:
-        return None, None
+    """Data-sheet peaks of the H100 SXM at 700 W (a power-capped card runs below them; `clocks` in the line shows it)."""
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (700 W; dense bf16)"
 
 
 class ClockSampler:
@@ -90,6 +101,7 @@ class ClockSampler:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-lms", "20",
                                           "-i", str(self.device)], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True,
                                          bufsize=1)
+            atexit.register(self.proc.kill)   # never outlives the bench, even when a gate fails mid-run
             threading.Thread(target=self._read, daemon=True).start()
         except Exception:
             self.proc = None
@@ -221,12 +233,12 @@ def workload_config(args, kind="bm25"):
     return {"workload": "configs[1]: 10M-doc synthetic Zipf postings, 1024-query disjunctive BM25 top-100",
             "docs": args.docs, "vocab": args.vocab, "batch": args.nq, "terms_per_query": 3, "top_k": args.topk,
             "total_hits_threshold": args.threshold, "sharding": f"doc-range x{args.gpus}",
-            "l2": "posting image (GBs) >> 126 MB L2; no flush needed"}
+            "l2": "posting image (GBs) >> 50 MB L2; no flush needed"}
 
 
 # ---------------------------------------------------------------------------------------------- conj leg (configs[2])
 
-def conj_leg(args, searcher, sh, stream, steps, threads, n_sample):
+def conj_leg(args, searcher, sh, stream, steps, threads, n_sample, dump=None):
     """configs[2] on the resident index: gate vs the exhaustive oracle, kernel time, SURVEY 8d byte formula
     sum_q [ sum_t df(t) * 8 B + |intersection_q| * (T + 4) B ]."""
     import torch
@@ -240,7 +252,11 @@ def conj_leg(args, searcher, sh, stream, steps, threads, n_sample):
     inter = searcher.search_batch(make_conj_queries(args.nq, args.vocab, with_filter=False), RelevanceCollector(1, INT_MAX)).total_hits
     batch = searcher.prepare(queries, coll)
     stats = batch.stats()
-    kernel_ms, merge_ms, step_ms = time_batch(batch, stream, steps)
+    kernel_ms, merge_ms, step_ms = time_batch(batch, stream, steps, args.warmup)
+    if dump is not None:
+        r = batch.fetch(stream)
+        dump.update({"conj_docs": r.docs, "conj_scores": r.scores, "conj_counts": r.counts, "conj_total_hits": r.total_hits,
+                     "conj_relation": r.relation})
     batch.close()
     # e2e: the one-shot C-ABI call with HOST query buffers (compiled once, as a serving adaptor would cache them) and host results
     from nrtsearch_b200.search import compile_queries
@@ -277,8 +293,8 @@ def conj_leg(args, searcher, sh, stream, steps, threads, n_sample):
 
 # ---------------------------------------------------------------------------------------------- kNN (configs[3])
 
-def knn_leg(args, rank, world, local_rank, steps, warmup):
-    """configs[3]: 1M x 768 fp32 vectors, batch-1024 cosine top-100; exact search (tcgen05 bf16 candidate stage, fp64
+def knn_leg(args, rank, world, local_rank, steps, warmup, dump=None, prefix=""):
+    """configs[3]: 1M x 768 fp32 vectors, batch-1024 cosine top-100; exact search (wgmma bf16 candidate stage, fp64
     re-score, rank-safety certificate). world > 1: the corpus is row-partitioned, every rank searches its shard, ONE
     all-gather of the packed results, TopDocs.merge on the device."""
     import torch
@@ -353,6 +369,8 @@ def knn_leg(args, rank, world, local_rank, steps, warmup):
         wd, ws, wc = oracle.knn_exact(whole, ix.SIM_COSINE, queries[:ns], k, n_threads=threads)
         cpu_qps = ns / (time.perf_counter() - t0)
         gd, gs = out[0], out[1]
+        if dump is not None:
+            dump.update({prefix + "docs": out[0], prefix + "scores": out[1], prefix + "counts": out[2]})
         recall = float(np.mean([len(set(gd[q]) & set(wd[q])) / k for q in range(ns)]))
         bad = [q for q in range(ns) if not np.array_equal(gd[q], wd[q])]
         for q in bad:   # ids may differ only inside a score tie band (1e-5 relative), as in tests/test_gpu_knn.py
@@ -373,9 +391,9 @@ def knn_leg(args, rank, world, local_rank, steps, warmup):
                 "gate": {"queries": ns, "ids_equal_oracle": ns - len(bad), "tie_band_only": len(bad), "scores_rtol": 1e-5},
                 "certificate": {"uncertified_queries": uncert, "of": nq,
                                 "rule": "every vector outside the k' = 4k candidate list proven below the k-th exact score with the bf16 error bound 2^-7 |q||d|; rejected queries re-run exactly"},
-                "roofline": {"bound": "tensor", "kernel": "knn_gemm_bf16_db_kernel (tcgen05 UMMA, 256x128 tiles double-buffered in TMEM, TMA operand ring, 16 epilogue warps with the fused top-k' threshold filter)",
+                "roofline": {"bound": "tensor", "kernel": "knn_gemm_bf16_kernel (wgmma m64n128k16, 128x128 tiles, 3-stage TMA operand ring, two consumer warpgroups, fused top-k' threshold filter)",
                              "achieved": ach, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / pk["bf16_tflops"], "traffic": None,
-                             "peak_source": src + " burst", "gemm_ms": gemm_ms, "select_ms": float(np.mean(sel)), "rescore_ms": float(np.mean(resc))},
+                             "peak_source": src, "gemm_ms": gemm_ms, "select_ms": float(np.mean(sel)), "rescore_ms": float(np.mean(resc))},
                 "cpu_baseline": {"value": cpu_qps, "unit": "queries/s", "cores": threads, "kind": "port",
                                  "sample": f"{ns} queries, exact fp64 brute force (oracle/oracle.c), same corpus"},
                 "clocks": clocks}
@@ -500,7 +518,7 @@ def run_hybrid(args, rank, world, local_rank):
     sampler.mark_begin()
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        step()
+        last = step()
     barrier()
     wall = (time.perf_counter() - t0) / args.steps
     sampler.mark_end()
@@ -511,6 +529,8 @@ def run_hybrid(args, rank, world, local_rank):
         wall = float(t[0])
     if rank == 0:
         stats = batch.stats()
+        (bd, bs, bc, bt), _, _ = last
+        dump_outputs(args.dump_outputs, {"docs": bd, "scores": bs, "counts": bc, "total": np.asarray(bt)})
         print(json.dumps({
             "metric": "hybrid BM25 + kNN + weighted-RRF queries/sec (batch 1024, doc-sharded)", "value": nq / wall, "unit": "queries/s",
             "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": wall * 1e3, "higher_is_better": True,
@@ -596,8 +616,10 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     dev = torch.device("cuda", local_rank)
     if args.workload == "knn":
-        line = knn_leg(args, rank, world, local_rank, args.steps, args.warmup)
+        dump = {}
+        line = knn_leg(args, rank, world, local_rank, args.steps, args.warmup, dump)
         if rank == 0:
+            dump_outputs(args.dump_outputs, dump)
             print(json.dumps(line))
         if world > 1:
             dist.destroy_process_group()
@@ -675,6 +697,10 @@ def main():
     barrier()
     sampler.mark_end()
     clocks = sampler.stop() if rank == 0 else None
+    dump = {}
+    if rank == 0 and args.dump_outputs:   # the page of the last timed step (the merged one at N > 1)
+        dd, ds, dc, df, dt = pg.unpack(pg.merged if world > 1 else pg.local)
+        dump.update({"docs": dd, "scores": ds, "counts": dc, "flags": df, "total_hits": dt})
     ms = e0.elapsed_time(e1)
     kernel_ms = batch.stage_ms(0)
     merge_ms = batch.stage_ms(1)
@@ -694,7 +720,7 @@ def main():
     exh_ms = None
     if args.threshold != INT_MAX and not conj:
         bex = searcher.prepare(queries, RelevanceCollector(args.topk, INT_MAX))
-        exh_ms, _, _ = time_batch(bex, stream, 5, warmup=2)
+        exh_ms, _, _ = time_batch(bex, stream, args.steps, args.warmup)
         bex.close()
         if world > 1:
             t = torch.tensor([exh_ms], device=dev, dtype=torch.float64)
@@ -738,14 +764,14 @@ def main():
 
     extra = None
     if rank == 0 and world == 1 and not conj and not args.no_extra:
-        extra = {"conj": conj_leg(args, searcher, sh, stream, max(5, args.steps // 2), threads, min(256, n_sample))}
+        extra = {"conj": conj_leg(args, searcher, sh, stream, args.steps, threads, min(256, n_sample), dump if args.dump_outputs else None)}
     batch.close()
     gix.close()
     if rank == 0 and world == 1 and not conj and not args.no_extra:
         del sh
         ctx.close()
         ctx = None
-        extra["knn"] = knn_leg(args, 0, 1, local_rank, max(5, args.steps // 4), 2)
+        extra["knn"] = knn_leg(args, 0, 1, local_rank, args.steps, args.warmup, dump if args.dump_outputs else None, "knn_")
 
     if rank == 0:
         pk, peak_src = peaks()
@@ -755,11 +781,6 @@ def main():
             alg_bytes = per_gpu_postings * 8 + nq * k * 8   # + the intersection gathers, reported by the default line's extra.conj
         else:
             alg_bytes = per_gpu_postings * ALG_BYTES_PER_POSTING + nq * k * 8   # per launch (per GPU)
-        traffic, traffic_src = (None, None)
-        exh_traffic = None
-        if world == 1 and not conj and args.docs == 10_000_000 and args.vocab == 1_000_000 and nq == 1024 and k == 100 and args.threshold == 1000:
-            traffic, traffic_src = static_traffic("posting_probe_kernel<simple> TOP_SCORES")
-            exh_traffic, _ = static_traffic("posting_probe_kernel<simple> COMPLETE")
         achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
         kernel_name = ("posting_probe_kernel<generic>" if conj else "posting_probe_kernel<simple>") + \
             " (persistent, data-parallel over the driver postings: 2-bit tf-plane gathers / granule-narrowed searches of TMA-staged lists, MAXSCORE roles, BM25 + exact top-k)"
@@ -774,21 +795,19 @@ def main():
             "roofline": {"bound": "hbm", "kernel": kernel_name,
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "frac_kind": "effective: ALGORITHMIC bytes of every posting of the batch (9 B each, SURVEY.md 8d) / kernel time; MAXSCORE lets the kernel skip most of them, as the reference does",
-                         "traffic": traffic, "traffic_source": traffic_src,
-                         "physical_frac": None if traffic is None else traffic / (kernel_ms * 1e-3) / 1e9 / peak,
                          "peak_source": peak_src, "kernel_ms": kernel_ms, "merge_ms": merge_ms,
                          "alg_bytes_per_launch": alg_bytes, "alg_postings_per_launch": per_gpu_postings,
                          "mode": ("TOP_SCORES (totalHitsThreshold %d, the reference default)" % args.threshold) if args.threshold != INT_MAX else "COMPLETE (exact counts)",
                          "exhaustive": None if exh_ms is None else
                                        {"mode": "ScoreMode.COMPLETE: exact totalHits for every query (inclusion by ownership; a dense non-essential list contributes its posting count unread)",
                                         "kernel_ms": exh_ms, "achieved": alg_bytes / (exh_ms * 1e-3) / 1e9,
-                                        "frac": alg_bytes / (exh_ms * 1e-3) / 1e9 / peak, "traffic": exh_traffic,
-                                        "physical_frac": None if exh_traffic is None else exh_traffic / (exh_ms * 1e-3) / 1e9 / peak}},
+                                        "frac": alg_bytes / (exh_ms * 1e-3) / 1e9 / peak}},
             "cpu_baseline": cpu,
             "clocks": clocks,
             "index": {"postings": n_postings, "device_bytes": dev_bytes, "build_s": build_s, "work_items": stats["work_items"]},
             "extra": extra,
         }
+        dump_outputs(args.dump_outputs, dump)
         print(json.dumps(line))
     if ctx is not None:
         ctx.close()

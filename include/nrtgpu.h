@@ -1,5 +1,5 @@
 /*
- * nrtgpu.h -- C ABI of the B200-native query-execution engine that drops in behind nrtsearch's
+ * nrtgpu.h -- C ABI of the H100-native query-execution engine that drops in behind nrtsearch's
  * SearchHandler / SearchRequestProcessor (reference = Yelp/nrtsearch @ 59c38655, Lucene 10.4.0).
  *
  * The reference has NO native seam for query execution (it is pure Java over lucene-core); the
@@ -309,7 +309,7 @@ int nrtgpu_search_knn(nrtgpu_index* ix, const float* queries, int32_t nq, int32_
                       void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts);
 
 /* same search, plus the device time (ms, CUDA events on `stream`) of its three stages:
- * stage_ms[0] candidate GEMM (tcgen05 bf16 when dims % 8 == 0), [1] per-query select, [2] exact fp64 re-score */
+ * stage_ms[0] candidate GEMM (wgmma bf16 when dims % 8 == 0), [1] per-query select, [2] exact fp64 re-score */
 int nrtgpu_search_knn_timed(nrtgpu_index* ix, const float* queries, int32_t nq, int32_t k, void* stream,
                             int32_t* out_docs, float* out_scores, int32_t* out_counts, float* stage_ms);
 

@@ -1,4 +1,4 @@
-"""nrtsearch_b200 -- B200-native query-execution engine behind nrtsearch's search path.
+"""nrtsearch_b200 -- H100-native query-execution engine behind nrtsearch's search path.
 
 Only what the hot path needs: csrc/ (CUDA kernels + the C ABI of include/nrtgpu.h), the host-side
 mirror of the reference's query/collector interface (search.py) and the shard description +

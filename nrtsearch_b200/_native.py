@@ -1,6 +1,6 @@
 """ctypes bindings of the in-tree native libraries.
 
-libnrtgpu.so   -- the CUDA engine behind include/nrtgpu.h (sm_100a). There is NO fallback: if the
+libnrtgpu.so   -- the CUDA engine behind include/nrtgpu.h (sm_90a). There is NO fallback: if the
                   library is missing or no CUDA device is present, calls raise NrtGpuError.
 libnrtsynth.so -- host-side deterministic corpus/query generators (bench + tests inputs).
 """

@@ -1,10 +1,12 @@
 // Tensor-core candidate stage of the kNN path: S[q, d] = <Q[q,:], D[d,:]> for a chunk of the corpus, bf16 inputs,
-// fp32 accumulation in TMEM, hand-written for sm_100a:
-//   * operands are staged by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) through a 4-stage mbarrier pipeline,
-//   * one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (UMMA 128 x 256 x 16) on shared-memory descriptors,
-//   * the 128 x 256 fp32 accumulator lives in TMEM (256 columns) and is read back with tcgen05.ld.32x32b.x32 by four
-//     epilogue warps, which apply the similarity's monotone transform (cosine: / |d|, l2: 2 dot - |d|^2) and store the
-//     approximate scores for the per-query select (knn_select_kernel). The exact fp64 re-score (knn_rescore_kernel)
+// fp32 accumulation in registers, hand-written for sm_90a:
+//   * operands are staged by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) through a 3-stage mbarrier ring; thread 0
+//     refills a stage once all eight warps have released it,
+//   * two consumer warpgroups issue wgmma.mma_async m64n128k16 (bf16 -> f32) on shared-memory descriptors, each owning
+//     64 query rows of the 128 x 128 output tile,
+//   * the epilogue reads the accumulators from registers and applies the similarity's monotone transform (cosine: / |d|,
+//     l2: 2 dot - |d|^2): unfused, it stores the approximate scores for the per-query select (knn_select_kernel); fused,
+//     it keeps only the values at or above the query's running k'-th best. The exact fp64 re-score (knn_rescore_kernel)
 //     restores oracle arithmetic for the surviving candidates, so bf16 only affects which k' = 4k candidates survive.
 // Replaces the GEMM-shaped part of ExactVectorQuery's scan
 // (reference src/main/java/com/yelp/nrtsearch/server/query/vector/ExactVectorQuery.java:137-173).
@@ -17,21 +19,29 @@
 namespace nrtgpu {
 namespace tc {
 
-#ifndef NRT_GEMM_STAGES
-#define NRT_GEMM_STAGES 2
-#endif
-constexpr int BM = 128, BN = 256, BK = 64, kStages = NRT_GEMM_STAGES, kUmmaK = 16;
-constexpr int kGemmCtasPerSm = kStages <= 2 ? 2 : 1;   // 2 x (2 stages x 48 KB) fit one SM: the epilogue of one CTA overlaps the mainloop of the other
-constexpr int kGemmThreads = 256;   // warp 0: TMA producer, warp 1: TMEM alloc + MMA issuer, warps 4-7: epilogue
+constexpr int BM = 128, BN = 128, BK = 64, kStages = 3, kWgmmaK = 16;
+constexpr int kGemmThreads = 256;   // two consumer warpgroups, 64 query rows each
+constexpr int kGemmCtasPerSm = 2;   // two CTAs' shared memory fit one SM: the epilogue of one overlaps the mainloop of the other
 constexpr uint32_t kABytes = BM * BK * 2, kBBytes = BN * BK * 2, kStageBytes = kABytes + kBBytes;
-constexpr uint32_t kTmemCols = 256;
-constexpr size_t kGemmSmem = (size_t)kStages * kStageBytes + 1024 /*alignment slack*/ + 256 /*barriers*/;
+// Fused epilogue: a row's survivors of the tile are buffered in shared memory and appended to the query's chunk list with
+// ONE global atomicAdd per row (a returning atomic per survivor costs a round trip to L2 each); survivors past kRowCap in
+// one tile, rare once the threshold is warm, go out one atomic each.
+constexpr int kRowCap = 8;
+struct GemmSmemTail {
+  uint64_t full[kStages], empty[kStages];
+  float2 ab[BN];                 // (a, b) of the tile's vectors
+  int cnt[BM];                   // survivors per row of the tile
+  uint64_t surv[BM * kRowCap];
+};
+constexpr size_t kGemmSmem = (size_t)kStages * kStageBytes + sizeof(GemmSmemTail) + 1024 /*alignment slack*/;
+static_assert(kGemmCtasPerSm * (kGemmSmem + 1024) <= 233472, "kNN GEMM shared memory exceeds two CTAs per SM");
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void bar_init(uint64_t* b, uint32_t c) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s_u32(b)), "r"(c) : "memory"); }
 __device__ __forceinline__ void bar_expect_tx(uint64_t* b, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s_u32(b)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void bar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(b)) : "memory"); }
 __device__ __forceinline__ void bar_wait(uint64_t* b, uint32_t parity) {
   uint32_t ok;
   do {
@@ -43,21 +53,38 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(s_u32(dst)), "l"(map), "r"(s_u32(bar)), "r"(crd0), "r"(crd1) : "memory");
 }
-// shared-memory matrix descriptor, K-major, 128-byte swizzle (cute SmemDescriptor: start>>4 | LBO 1 | SBO 1024 B | version 1 | SW128)
+// wgmma shared-memory matrix descriptor, K-major, 128-byte swizzle: start >> 4 | LBO 1 (unused for swizzled K-major) |
+// SBO 1024 B (8 rows x 128 B) | layout SWIZZLE_128B. The tile bases are 1024-byte aligned, so the base offset is 0.
 __device__ __forceinline__ uint64_t make_smem_desc(const void* p) {
   uint64_t d = (uint64_t)((s_u32(p) >> 4) & 0x3fffu);
-  d |= (uint64_t)1 << 16;              // leading byte offset (unused for swizzled K-major; canonical value 1)
-  d |= (uint64_t)(1024 >> 4) << 32;    // stride byte offset: 8 rows x 128 B
-  d |= (uint64_t)1 << 46;              // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;              // SWIZZLE_128B
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_c, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_c), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s_u32(bar)) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both operands K-major bf16 in shared memory, D fp32 in registers
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
+      "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, "
+      "%42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, "
+      "%62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
 }
 
 struct GemmParams {
@@ -75,603 +102,102 @@ struct GemmParams {
   const uint8_t* filter;  // per DOC 0/1 or NULL
   const int32_t* vec_docs;  // ordinal -> doc or NULL
   const uint32_t* live_bits;  // liveDocs bitmap or NULL
-  int debug;              // experiments only (NRTGPU_KNN_DEBUG): 1 = the epilogue drops every value (mainloop-only timing)
 };
 
-// one 32-column slice of an accumulator row: store the approximate scores (unfused) or keep the survivors (fused)
-__device__ __forceinline__ void epilogue_slice(const GemmParams& P, const uint32_t (&v)[32], int gq, int n0, int c) {
-  if (gq < P.M) {
-    if (P.S) {   // unfused: store the approximate scores
-      float* out = P.S + (size_t)gq * P.ldS + n0 + c * 32;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int gd = n0 + c * 32 + j;
-        if (gd < P.N) {
-          float x = __uint_as_float(v[j]);
-          if (P.sim == NRTGPU_SIM_COSINE) x = x * rsqrtf(fmaxf(P.dnorm2[gd], 1e-30f));
-          else if (P.sim == NRTGPU_SIM_L2) x = 2.0f * x - P.dnorm2[gd];
-          out[j] = x;
-        }
-      }
-    } else {     // fused top-k': keep only values that can still enter the query's best k'
-      const float th = P.theta[gq];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int gd = n0 + c * 32 + j;
-        const float2 ab = __ldg(P.ab + min(gd, P.N - 1));
-        const float x = fmaf(ab.x, __uint_as_float(v[j]), ab.y);
-        if (gd < P.N && x >= th) {
-          const int ord = P.n_base + gd;
-          bool ok = true;
-          if (P.filter || P.live_bits) {
-            const int doc = P.vec_docs ? P.vec_docs[ord] : ord;
-            if (P.filter) ok = P.filter[doc] != 0;
-            if (ok && P.live_bits) ok = (P.live_bits[doc >> 5] >> (doc & 31)) & 1u;
-          }
-          if (ok) {
-            const int pos = atomicAdd(P.cc_cnt + gq, 1);
-            if (pos < P.cc_cap) P.cc[(size_t)gq * P.cc_cap + pos] = make_key(x, ord);
-          }
-        }
-      }
-    }
-  }
-}
-
-// fused top-k' epilogue of one 32-column slice with the tile's (a, b) pairs staged in shared memory (one broadcast LDS.64
-// per column instead of a global load per element: the profile of the first 256 x 256 build had 40 % of its stall samples
-// on those loads, the tensor pipe waiting for the epilogue to hand the accumulators back)
-// Survivors of a row are buffered in shared memory (kSurvBuf keys per row, column-major so the lanes of a warp do not
-// collide) and appended to the query's chunk list with ONE atomicAdd per flush: a returning atomic per survivor cost every
-// warp a ~1 us round trip at ~30 columns per tile (different lanes survive at different columns), 2/3 of the kernel's time.
-constexpr int kSurvBuf = 4;
-constexpr int kSurvRows = 512;   // one buffer column per epilogue thread of the 256 x 256 kernel
-__device__ __forceinline__ void surv_flush(const GemmParams& P, uint64_t* surv, int row, int gq, int& nbuf) {
-  if (nbuf == 0) return;
-  const int pos = atomicAdd(P.cc_cnt + gq, nbuf);
-  for (int i = 0; i < nbuf; ++i)
-    if (pos + i < P.cc_cap) P.cc[(size_t)gq * P.cc_cap + pos + i] = surv[i * kSurvRows + row];
-  nbuf = 0;
-}
-
-__device__ __forceinline__ void epilogue_slice_fused(const GemmParams& P, const uint32_t (&v)[32], uint32_t ab_smem /*shared-space address of the tile's [BN] float2*/,
-                                                     float th, int gq, int n0, int c, uint64_t* surv, int row, int& nbuf) {
-  const int lim = gq < P.M ? P.N - (n0 + c * 32) : 0;   // columns of this slice inside the chunk (rows past M: none)
-  // branch-free pass: which of the 32 values can still enter the query's best k'? (two (a, b) pairs per LDS.128)
-  uint32_t mask = 0u;
-  const uint32_t sb = ab_smem + (uint32_t)(c * 32) * 8u;
-#pragma unroll
-  for (int j = 0; j < 32; j += 2) {
-    float a0, b0, a1, b1;
-    asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(a0), "=f"(b0), "=f"(a1), "=f"(b1) : "r"(sb + (uint32_t)j * 8u));
-    const float x0 = fmaf(a0, __uint_as_float(v[j]), b0), x1 = fmaf(a1, __uint_as_float(v[j + 1]), b1);
-    mask |= (x0 >= th ? 1u : 0u) << j;
-    mask |= (x1 >= th ? 1u : 0u) << (j + 1);
-  }
-  if (lim < 32) mask &= lim > 0 ? ((1u << lim) - 1u) : 0u;
-  // columns in which ANY row of the warp has a survivor (about 4 of the 32 once the threshold is warm): only those are walked
-  const uint32_t warp_mask = __reduce_or_sync(0xffffffffu, mask);
-  if (warp_mask == 0u) return;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    if (!((warp_mask >> j) & 1u)) continue;   // warp-uniform
-    if (!((mask >> j) & 1u)) continue;
-    float a, b;
-    asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a), "=f"(b) : "r"(sb + (uint32_t)j * 8u));
-    const float x = fmaf(a, __uint_as_float(v[j]), b);
-    const int ord = P.n_base + n0 + c * 32 + j;
-    bool ok = true;
-    if (P.filter || P.live_bits) {
-      const int doc = P.vec_docs ? P.vec_docs[ord] : ord;
-      if (P.filter) ok = P.filter[doc] != 0;
-      if (ok && P.live_bits) ok = (P.live_bits[doc >> 5] >> (doc & 31)) & 1u;
-    }
-    if (ok) {
-      surv[nbuf * kSurvRows + row] = make_key(x, ord);
-      if (++nbuf == kSurvBuf) surv_flush(P, surv, row, gq, nbuf);
-    }
-  }
-}
-
+// One 128 x 128 output tile per CTA; grid = query tiles x corpus tiles, query tiles varying fastest so that the CTAs sharing
+// a corpus tile run together and the tile is fetched from HBM once and served to the other query tiles by L2.
 __global__ void __launch_bounds__(kGemmThreads, kGemmCtasPerSm)
 knn_gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams P) {
   extern __shared__ uint8_t gemm_raw[];
   uint8_t* base = (uint8_t*)(((uintptr_t)gemm_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* smA = base;
   uint8_t* smB = base + (size_t)kStages * kABytes;
-  uint64_t* full_bar = (uint64_t*)(base + (size_t)kStages * kStageBytes);
-  uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint32_t* tmem_ptr = (uint32_t*)(tmem_full + 1);
+  GemmSmemTail& T = *(GemmSmemTail*)(base + (size_t)kStages * kStageBytes);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // query tiles vary fastest: the CTAs that share a corpus tile run together, so it is fetched from HBM once and
-  // served to the other query tiles by L2
-  const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const int m_tiles = (P.M + BM - 1) / BM;
+  const int m0 = (int)(blockIdx.x % m_tiles) * BM, n0 = (int)(blockIdx.x / m_tiles) * BN;
   const int num_kb = (P.K + BK - 1) / BK;
+  const bool fused = P.S == nullptr;
 
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { bar_init(&full_bar[s], 1); bar_init(&empty_bar[s], 1); }
-    bar_init(tmem_full, 1);
+    for (int s = 0; s < kStages; ++s) { bar_init(&T.full[s], 1); bar_init(&T.empty[s], kGemmThreads / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   }
-  if (warp == 1) {   // one warp allocates the accumulator columns and publishes the TMEM base address
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr)), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  if (fused && tid < BN) T.ab[tid] = __ldg(P.ab + min(n0 + tid, P.N - 1));
+  if (tid < BM) T.cnt[tid] = 0;
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {   // ===== TMA producer
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kStages;
-        bar_wait(&empty_bar[s], ((kb / kStages) & 1) ^ 1);
-        bar_expect_tx(&full_bar[s], kStageBytes);
-        tma_load_2d(smA + (size_t)s * kABytes, &tmA, &full_bar[s], kb * BK, m0);
-        tma_load_2d(smB + (size_t)s * kBBytes, &tmB, &full_bar[s], kb * BK, P.n_base + n0);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {   // ===== MMA issuer (single thread)
-      // instruction descriptor (cute UMMA::InstrDescriptor): D = F32, A = B = BF16, both K-major, N >> 3, M >> 4
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kStages;
-        bar_wait(&full_bar[s], (kb / kStages) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t da = make_smem_desc(smA + (size_t)s * kABytes), db = make_smem_desc(smB + (size_t)s * kBBytes);
-#pragma unroll
-        for (int k = 0; k < BK / kUmmaK; ++k)   // advance 16 bf16 = 32 B inside the 128 B swizzle atom: +2 in the address field
-          umma_f16(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (uint32_t)((kb | k) != 0));
-        umma_commit(&empty_bar[s]);   // frees the smem stage when these MMAs retire
-      }
-      umma_commit(tmem_full);         // accumulator complete
-    }
-  } else if (warp >= 4) {             // ===== epilogue: TMEM -> registers -> global
-    const int quad = warp & 3;        // TMEM lane quadrant this warp may access
-    const int row = quad * 32 + lane;
-    bar_wait(tmem_full, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int gq = m0 + row;
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t v[32];
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(c * 32);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-            "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-            "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-            "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-          : "r"(taddr) : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      epilogue_slice(P, v, gq, n0, c);
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
-  }
-}
-
-// ---- persistent variant: one CTA per SM loops over output tiles; the TMA ring keeps streaming across tiles and the
-// accumulator is double buffered in TMEM (2 x 256 columns), so the epilogue of tile i overlaps the MMAs of tile i+1.
-constexpr int kPStages = 4;
-constexpr uint32_t kPTmemCols = 512;
-constexpr size_t kPGemmSmem = (size_t)kPStages * kStageBytes + 1024 + 256;
-
-__global__ void __launch_bounds__(kGemmThreads, 1)
-knn_gemm_bf16_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams P) {
-  extern __shared__ uint8_t gemm_raw[];
-  uint8_t* base = (uint8_t*)(((uintptr_t)gemm_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* smA = base;
-  uint8_t* smB = base + (size_t)kPStages * kABytes;
-  uint64_t* full_bar = (uint64_t*)(base + (size_t)kPStages * kStageBytes);
-  uint64_t* empty_bar = full_bar + kPStages;
-  uint64_t* tmem_full = empty_bar + kPStages;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;         // [2]
-  uint32_t* tmem_ptr = (uint32_t*)(tmem_empty + 2);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m_tiles = (P.M + BM - 1) / BM, n_tiles = (P.N + BN - 1) / BN;
-  const int total = m_tiles * n_tiles;
-  const int num_kb = (P.K + BK - 1) / BK;
-
   if (tid == 0) {
-    for (int s = 0; s < kPStages; ++s) { bar_init(&full_bar[s], 1); bar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { bar_init(&tmem_full[a], 1); bar_init(&tmem_empty[a], 128); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr)), "r"(kPTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {   // ===== TMA producer: one continuous stream of k-blocks over all tiles of this CTA
-      int it = 0;
-      for (int t = blockIdx.x; t < total; t += gridDim.x) {
-        const int m0 = (t % m_tiles) * BM, n0 = (t / m_tiles) * BN;   // query tiles vary fastest (corpus tile shared via L2)
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kPStages;
-          bar_wait(&empty_bar[s], ((it / kPStages) & 1) ^ 1);
-          bar_expect_tx(&full_bar[s], kStageBytes);
-          tma_load_2d(smA + (size_t)s * kABytes, &tmA, &full_bar[s], kb * BK, m0);
-          tma_load_2d(smB + (size_t)s * kBBytes, &tmB, &full_bar[s], kb * BK, P.n_base + n0);
-        }
-      }
+    for (int kb = 0; kb < num_kb && kb < kStages; ++kb) {
+      bar_expect_tx(&T.full[kb], kStageBytes);
+      tma_load_2d(smA + (size_t)kb * kABytes, &tmA, &T.full[kb], kb * BK, m0);
+      tma_load_2d(smB + (size_t)kb * kBBytes, &tmB, &T.full[kb], kb * BK, P.n_base + n0);
     }
-  } else if (warp == 1) {
-    if (lane == 0) {   // ===== MMA issuer
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      int it = 0, lt = 0;
-      for (int t = blockIdx.x; t < total; t += gridDim.x, ++lt) {
-        const int acc = lt & 1;
-        bar_wait(&tmem_empty[acc], ((lt >> 1) & 1) ^ 1);   // the epilogue has drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tacc = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kPStages;
-          bar_wait(&full_bar[s], (it / kPStages) & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da = make_smem_desc(smA + (size_t)s * kABytes), db = make_smem_desc(smB + (size_t)s * kBBytes);
+  }
+
+  float d[64];
 #pragma unroll
-          for (int k = 0; k < BK / kUmmaK; ++k)
-            umma_f16(tacc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (uint32_t)((kb | k) != 0));
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tmem_full[acc]);
-      }
-    }
-  } else if (warp >= 4) {   // ===== epilogue warps
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    int lt = 0;
-    for (int t = blockIdx.x; t < total; t += gridDim.x, ++lt) {
-      const int acc = lt & 1;
-      const int m0 = (t % m_tiles) * BM, n0 = (t / m_tiles) * BN;
-      const int gq = m0 + row;
-      bar_wait(&tmem_full[acc], (lt >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + c * 32);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (c == BN / 32 - 1) {   // every column of this accumulator is in registers: hand it back to the MMA warp
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(&tmem_empty[acc])) : "memory");
-        }
-        epilogue_slice(P, v, gq, n0, c);
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kPTmemCols) : "memory");
-  }
-}
-
-// ---- 256 x 256 variant (default): one persistent CTA per SM, TWO 128 x 256 accumulators (all 512 TMEM columns) fed by the
-// same corpus tile -- 64 KB of operands per k-block for 2 x the flops of the 128 x 256 kernel (48 KB), i.e. a third less
-// L2 -> SM traffic per flop, which is what bounded the smaller tile (profiles/r1_final_counters.md: tensor pipe 18 %, L2 hit
-// 82 %) -- and a 3-stage TMA ring that keeps streaming across tiles. Warp 0 = TMA producer, warp 1 = MMA issuer (two
-// tcgen05.mma per 16-wide k-step), warps 4-11 = epilogue (warp w reads TMEM lane quadrant w % 4 of accumulator (w - 4) / 4).
-constexpr int BM2 = 256;
-
-constexpr int kStages2 = 3;
-constexpr int kGemm2Threads = 640;   // warps 0 / 1: TMA / MMA, warps 4-19: epilogue (two warps per TMEM lane quadrant and accumulator, half the columns each)
-constexpr int kEpi2Threads = 512;
-constexpr uint32_t kA2Bytes = BM2 * BK * 2, kStage2Bytes = kA2Bytes + kBBytes;
-constexpr uint32_t kTmem2Cols = 512;
-constexpr size_t kGemm2Smem = (size_t)kStages2 * kStage2Bytes + 1024 + 256 + 2 * BN * sizeof(float2) + (size_t)kSurvBuf * kSurvRows * sizeof(uint64_t);
-
-__global__ void __launch_bounds__(kGemm2Threads, 1)
-knn_gemm_bf16_256_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams P) {
-  extern __shared__ uint8_t gemm_raw[];
-  uint8_t* base = (uint8_t*)(((uintptr_t)gemm_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* smA = base;
-  uint8_t* smB = base + (size_t)kStages2 * kA2Bytes;
-  uint64_t* full_bar = (uint64_t*)(base + (size_t)kStages2 * kStage2Bytes);
-  uint64_t* empty_bar = full_bar + kStages2;
-  uint64_t* tmem_full = empty_bar + kStages2;
-  uint64_t* tmem_empty = tmem_full + 1;
-  uint32_t* tmem_ptr = (uint32_t*)(tmem_empty + 1);
-  float2* ab_s = (float2*)(base + (size_t)kStages2 * kStage2Bytes + 256);   // [2][BN] (a, b) of the tile's vectors, double buffered
-  uint64_t* surv = (uint64_t*)(ab_s + 2 * BN);                                // [kSurvBuf][BM2] survivor keys per accumulator row
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m_tiles = (P.M + BM2 - 1) / BM2, n_tiles = (P.N + BN - 1) / BN;
-  const int total = m_tiles * n_tiles;
-  const int num_kb = (P.K + BK - 1) / BK;
-  // Tile order: t = blockIdx.x, + gridDim.x, ... in the m-fastest numbering. The host makes the grid a multiple of the query
-  // tiles when it can, so a CTA keeps ONE query tile for the whole launch (t % m_tiles is constant): an epilogue thread then
-  // serves the same query all along and appends its survivors with one atomic per full buffer, not one per tile.
-
-  if (tid == 0) {
-    for (int s = 0; s < kStages2; ++s) { bar_init(&full_bar[s], 1); bar_init(&empty_bar[s], 1); }
-    bar_init(tmem_full, 1); bar_init(tmem_empty, kEpi2Threads);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr)), "r"(kTmem2Cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {   // ===== TMA producer: one continuous stream of k-blocks over all tiles of this CTA
-      int it = 0;
-      for (int t = blockIdx.x; t < total; t += gridDim.x) {
-        const int m0 = (t % m_tiles) * BM2, n0 = (t / m_tiles) * BN;   // query tiles vary fastest (corpus tile shared via L2)
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kStages2;
-          bar_wait(&empty_bar[s], ((it / kStages2) & 1) ^ 1);
-          bar_expect_tx(&full_bar[s], kStage2Bytes);
-          tma_load_2d(smA + (size_t)s * kA2Bytes, &tmA, &full_bar[s], kb * BK, m0);
-          tma_load_2d(smB + (size_t)s * kBBytes, &tmB, &full_bar[s], kb * BK, P.n_base + n0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {   // ===== MMA issuer
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      int it = 0, lt = 0;
-      for (int t = blockIdx.x; t < total; t += gridDim.x, ++lt) {
-        bar_wait(tmem_empty, (lt & 1) ^ 1);   // the epilogue has drained both accumulators of the previous tile
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kStages2;
-          bar_wait(&full_bar[s], (it / kStages2) & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da0 = make_smem_desc(smA + (size_t)s * kA2Bytes);
-          const uint64_t da1 = make_smem_desc(smA + (size_t)s * kA2Bytes + 128 * BK * 2);   // query rows 128..255 of the tile
-          const uint64_t db = make_smem_desc(smB + (size_t)s * kBBytes);
+  for (int i = 0; i < 64; ++i) d[i] = 0.0f;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % kStages;
+    bar_wait(&T.full[s], (kb / kStages) & 1);
+    const uint64_t da = make_smem_desc(smA + (size_t)s * kABytes + wg * 64 * 128);   // this warpgroup's 64 query rows
+    const uint64_t db = make_smem_desc(smB + (size_t)s * kBBytes);
+    wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BK / kUmmaK; ++k) {
-            umma_f16(tmem_base, da0 + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (uint32_t)((kb | k) != 0));
-            umma_f16(tmem_base + (uint32_t)BN, da1 + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (uint32_t)((kb | k) != 0));
+    for (int k = 0; k < BK / kWgmmaK; ++k)   // advance 16 bf16 = 32 B inside the 128 B swizzle atom: +2 in the address field
+      wgmma_m64n128k16(d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+    wgmma_commit();
+    wgmma_wait<1>();   // the MMAs of k-block kb - 1 have retired: its stage can be refilled
+    if (kb > 0) {
+      const int ps = (kb - 1) % kStages;
+      if (lane == 0) bar_arrive(&T.empty[ps]);
+      if (tid == 0 && kb - 1 + kStages < num_kb) {
+        const int nk = kb - 1 + kStages;
+        bar_wait(&T.empty[ps], ((kb - 1) / kStages) & 1);
+        bar_expect_tx(&T.full[ps], kStageBytes);
+        tma_load_2d(smA + (size_t)ps * kABytes, &tmA, &T.full[ps], nk * BK, m0);
+        tma_load_2d(smB + (size_t)ps * kBBytes, &tmB, &T.full[ps], nk * BK, P.n_base + n0);
+      }
+      __syncwarp();
+    }
+  }
+  wgmma_wait<0>();
+
+  // accumulator layout of m64nNk16: d[4 j + 2 i + e] is row 16 (warp % 4) + lane / 4 + 8 i, column 8 j + 2 (lane % 4) + e
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = row0 + 8 * i, gq = m0 + row;
+    if (gq >= P.M) continue;
+    if (!fused) {   // unfused: store the approximate scores
+      float* out = P.S + (size_t)gq * P.ldS + n0;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * j + c0 + e, gd = n0 + c;
+          if (gd < P.N) {
+            float x = d[4 * j + 2 * i + e];
+            if (P.sim == NRTGPU_SIM_COSINE) x = x * rsqrtf(fmaxf(P.dnorm2[gd], 1e-30f));
+            else if (P.sim == NRTGPU_SIM_L2) x = 2.0f * x - P.dnorm2[gd];
+            out[c] = x;
           }
-          umma_commit(&empty_bar[s]);
         }
-        umma_commit(tmem_full);
-      }
-    }
-  } else if (warp >= 4) {   // ===== epilogue warps
-    const int quad = warp & 3, half = ((warp - 4) >> 2) & 1, chalf = (warp - 4) >> 3;   // TMEM lane quadrant, accumulator, column half
-    const int row = half * 128 + quad * 32 + lane;
-    const int et = tid - 128;   // epilogue thread 0..511: its own survivor buffer column
-    int lt = 0;
-    int nbuf = 0, prev_gq = -1;   // survivors buffered for query prev_gq, flushed at the start of the next tile
-    for (int t = blockIdx.x; t < total; t += gridDim.x, ++lt) {
-      const int m0 = (t % m_tiles) * BM2, n0 = (t / m_tiles) * BN;
-      const int gq = m0 + row;
-      const bool fused = P.S == nullptr;
-      float2* abt = ab_s + (lt & 1) * BN;
-      float th = 0.0f;
-      if (fused) {   // stage the tile's (a, b) pairs (256 epilogue threads, one pair each) while the MMAs run
-        if (et < BN) abt[et] = __ldg(P.ab + min(n0 + et, P.N - 1));
-        th = gq < P.M ? P.theta[gq] : 0.0f;
-        asm volatile("bar.sync 1, 512;" ::: "memory");   // epilogue warps only; a thread is at most one tile ahead, so the
-                                                         // other buffer is not being read any more when it is rewritten
-        // survivors buffered for ANOTHER query (the CTA moved to a different query tile) go out now, while this tile's MMAs run
-        if (prev_gq >= 0 && prev_gq != gq) surv_flush(P, surv, et, prev_gq, nbuf);
-      }
-      bar_wait(tmem_full, lt & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-      for (int c = chalf * (BN / 64); c < (chalf + 1) * (BN / 64); ++c) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(half * BN + c * 32);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (c == (chalf + 1) * (BN / 64) - 1) {   // this thread's last slice is in registers: hand TMEM back to the MMA warp
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(tmem_empty)) : "memory");
-        }
-        if (P.debug & 1) continue;
-        if (fused) epilogue_slice_fused(P, v, s_u32(abt), th, gq, n0, c, surv, et, nbuf);
-        else epilogue_slice(P, v, gq, n0, c);
-      }
-      prev_gq = (fused && gq < P.M) ? gq : -1;
-    }
-    if (prev_gq >= 0) surv_flush(P, surv, et, prev_gq, nbuf);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmem2Cols) : "memory");
-  }
-}
-
-// ---- 256 x 128 tiles, DOUBLE-BUFFERED in TMEM (default): buffer b holds the two 128 x 128 accumulators of a tile (query rows
-// 0-127 and 128-255 against the same 128 corpus vectors) in columns [256 b, 256 b + 256); the MMAs of tile t + 1 run into the
-// other buffer while the 16 epilogue warps drain tile t, so the fused top-k' epilogue (the bottleneck of the single-buffered
-// 256 x 256 kernel: mainloop alone 1.14 ms = 82 % of the tensor peak, with epilogue 2.3 ms) leaves the critical path. A
-// survivor's value is re-read from TMEM by a one-column tcgen05.ld (warp-uniform loop over the columns in which any row
-// survives) instead of 32 predicated blocks. 4-stage TMA ring of 48 KB k-blocks.
-constexpr int BN3 = 128;
-constexpr int kStages3 = 4;
-constexpr uint32_t kB3Bytes = BN3 * BK * 2, kStage3Bytes = kA2Bytes + kB3Bytes;
-constexpr size_t kGemm3Smem = (size_t)kStages3 * kStage3Bytes + 1024 + 256 + 2 * BN3 * sizeof(float2) + (size_t)kSurvBuf * kSurvRows * sizeof(uint64_t);
-
-__global__ void __launch_bounds__(kGemm2Threads, 1)
-knn_gemm_bf16_db_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams P) {
-  extern __shared__ uint8_t gemm_raw[];
-  uint8_t* base = (uint8_t*)(((uintptr_t)gemm_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* smA = base;
-  uint8_t* smB = base + (size_t)kStages3 * kA2Bytes;
-  uint64_t* full_bar = (uint64_t*)(base + (size_t)kStages3 * kStage3Bytes);
-  uint64_t* empty_bar = full_bar + kStages3;
-  uint64_t* tmem_full = empty_bar + kStages3;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;         // [2]
-  uint32_t* tmem_ptr = (uint32_t*)(tmem_empty + 2);
-  float2* ab_s = (float2*)(base + (size_t)kStages3 * kStage3Bytes + 256);   // [2][BN3]
-  uint64_t* surv = (uint64_t*)(ab_s + 2 * BN3);                              // [kSurvBuf][512]
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m_tiles = (P.M + BM2 - 1) / BM2, n_tiles = (P.N + BN3 - 1) / BN3;
-  const int total = m_tiles * n_tiles;
-  const int num_kb = (P.K + BK - 1) / BK;
-
-  if (tid == 0) {
-    for (int s = 0; s < kStages3; ++s) { bar_init(&full_bar[s], 1); bar_init(&empty_bar[s], 1); }
-    for (int b = 0; b < 2; ++b) { bar_init(&tmem_full[b], 1); bar_init(&tmem_empty[b], kEpi2Threads); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_ptr)), "r"(kTmem2Cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {   // ===== TMA producer
-      int it = 0;
-      for (int t = blockIdx.x; t < total; t += gridDim.x) {
-        const int m0 = (t % m_tiles) * BM2, n0 = (t / m_tiles) * BN3;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kStages3;
-          bar_wait(&empty_bar[s], ((it / kStages3) & 1) ^ 1);
-          bar_expect_tx(&full_bar[s], kStage3Bytes);
-          tma_load_2d(smA + (size_t)s * kA2Bytes, &tmA, &full_bar[s], kb * BK, m0);
-          tma_load_2d(smB + (size_t)s * kB3Bytes, &tmB, &full_bar[s], kb * BK, P.n_base + n0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {   // ===== MMA issuer
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN3 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      int it = 0, lt = 0;
-      for (int t = blockIdx.x; t < total; t += gridDim.x, ++lt) {
-        const int b = lt & 1;
-        bar_wait(&tmem_empty[b], ((lt >> 1) & 1) ^ 1);   // the epilogue has drained this buffer (two tiles ago)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t acc0 = tmem_base + (uint32_t)(b * 2 * BN3), acc1 = acc0 + (uint32_t)BN3;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kStages3;
-          bar_wait(&full_bar[s], (it / kStages3) & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da0 = make_smem_desc(smA + (size_t)s * kA2Bytes);
-          const uint64_t da1 = make_smem_desc(smA + (size_t)s * kA2Bytes + 128 * BK * 2);
-          const uint64_t db = make_smem_desc(smB + (size_t)s * kB3Bytes);
+    } else {        // fused top-k': keep only values that can still enter the query's best k'
+      const float th = P.theta[gq];
 #pragma unroll
-          for (int k = 0; k < BK / kUmmaK; ++k) {
-            umma_f16(acc0, da0 + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (uint32_t)((kb | k) != 0));
-            umma_f16(acc1, da1 + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (uint32_t)((kb | k) != 0));
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tmem_full[b]);
-      }
-    }
-  } else if (warp >= 4) {   // ===== epilogue warps
-    const int quad = warp & 3, half = ((warp - 4) >> 2) & 1, chalf = (warp - 4) >> 3;   // TMEM lane quadrant, accumulator, column half
-    const int row = half * 128 + quad * 32 + lane;
-    const int et = tid - 128;
-    const bool fused = P.S == nullptr;
-    int lt = 0;
-    int nbuf = 0, prev_gq = -1;
-    for (int t = blockIdx.x; t < total; t += gridDim.x, ++lt) {
-      const int b = lt & 1;
-      const int m0 = (t % m_tiles) * BM2, n0 = (t / m_tiles) * BN3;
-      const int gq = m0 + row;
-      float2* abt = ab_s + b * BN3;
-      float th = 0.0f;
-      if (fused) {
-        if (et < BN3) abt[et] = __ldg(P.ab + min(n0 + et, P.N - 1));
-        th = gq < P.M ? P.theta[gq] : 0.0f;
-        asm volatile("bar.sync 1, 512;" ::: "memory");
-        if (prev_gq >= 0 && prev_gq != gq) surv_flush(P, surv, et, prev_gq, nbuf);
-      }
-      bar_wait(&tmem_full[b], (lt >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t lane_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(b * 2 * BN3 + half * BN3);
-#pragma unroll 1
-      for (int c = chalf * (BN3 / 64); c < (chalf + 1) * (BN3 / 64); ++c) {
-        uint32_t v[32];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(lane_addr + (uint32_t)(c * 32)) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (P.debug & 1) continue;
-        if (!fused) { epilogue_slice(P, v, gq, n0, c); continue; }
-        // branch-free pass over the slice: which values can still enter the query's best k'?
-        const int lim = gq < P.M ? P.N - (n0 + c * 32) : 0;
-        uint32_t mask = 0u;
-        const uint32_t sb = s_u32(abt) + (uint32_t)(c * 32) * 8u;
+      for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          float a0, b0, a1, b1;
-          asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(a0), "=f"(b0), "=f"(a1), "=f"(b1) : "r"(sb + (uint32_t)j * 8u));
-          const float x0 = fmaf(a0, __uint_as_float(v[j]), b0), x1 = fmaf(a1, __uint_as_float(v[j + 1]), b1);
-          mask |= (x0 >= th ? 1u : 0u) << j;
-          mask |= (x1 >= th ? 1u : 0u) << (j + 1);
-        }
-        if (lim < 32) mask &= lim > 0 ? ((1u << lim) - 1u) : 0u;
-        // survivors: warp-uniform walk over the columns in which any row survives; the value comes back by a one-column TMEM load
-        uint32_t warp_mask = __reduce_or_sync(0xffffffffu, mask);
-        while (warp_mask) {
-          const int j = __ffs(warp_mask) - 1;
-          warp_mask &= warp_mask - 1u;
-          uint32_t vj;
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(vj) : "r"(lane_addr + (uint32_t)(c * 32 + j)) : "memory");
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if ((mask >> j) & 1u) {
-            const float2 ab = abt[c * 32 + j];
-            const float x = fmaf(ab.x, __uint_as_float(vj), ab.y);
-            const int ord = P.n_base + n0 + c * 32 + j;
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * j + c0 + e, gd = n0 + c;
+          const float2 ab = T.ab[c];
+          const float x = fmaf(ab.x, d[4 * j + 2 * i + e], ab.y);
+          if (gd < P.N && x >= th) {
+            const int ord = P.n_base + gd;
             bool ok = true;
             if (P.filter || P.live_bits) {
               const int doc = P.vec_docs ? P.vec_docs[ord] : ord;
@@ -679,24 +205,30 @@ knn_gemm_bf16_db_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
               if (ok && P.live_bits) ok = (P.live_bits[doc >> 5] >> (doc & 31)) & 1u;
             }
             if (ok) {
-              surv[nbuf * kSurvRows + et] = make_key(x, ord);
-              if (++nbuf == kSurvBuf) surv_flush(P, surv, et, gq, nbuf);
+              const uint64_t key = make_key(x, ord);
+              const int pos = atomicAdd(&T.cnt[row], 1);
+              if (pos < kRowCap) {
+                T.surv[row * kRowCap + pos] = key;
+              } else {
+                const int gp = atomicAdd(P.cc_cnt + gq, 1);
+                if (gp < P.cc_cap) P.cc[(size_t)gq * P.cc_cap + gp] = key;
+              }
             }
           }
         }
-      }
-      // this thread is done with the buffer: hand it back to the MMA warp
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(&tmem_empty[b])) : "memory");
-      prev_gq = (fused && gq < P.M) ? gq : -1;
     }
-    if (prev_gq >= 0) surv_flush(P, surv, et, prev_gq, nbuf);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmem2Cols) : "memory");
+  if (fused) {   // one append per row of the tile
+    __syncthreads();
+    const int gq = m0 + tid;
+    if (tid < BM && gq < P.M) {
+      const int n = min(T.cnt[tid], kRowCap);
+      if (n > 0) {
+        const int pos = atomicAdd(P.cc_cnt + gq, n);
+        for (int i = 0; i < n; ++i)
+          if (pos + i < P.cc_cap) P.cc[(size_t)gq * P.cc_cap + pos + i] = T.surv[tid * kRowCap + i];
+      }
+    }
   }
 }
 

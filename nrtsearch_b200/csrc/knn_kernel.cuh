@@ -408,7 +408,7 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
                            int32_t* out_counts, const __nv_bfloat16* d_vec_bf16 = nullptr,
                            const CUtensorMap* tm_corpus = nullptr, float* stage_ms = nullptr, const float2* d_ab = nullptr,
                            KnnScratch* sc = nullptr, const uint32_t* d_live_bits = nullptr, float dmax = 0.0f,
-                           int32_t* n_uncertified = nullptr, const CUtensorMap* tm_corpus128 = nullptr) {
+                           int32_t* n_uncertified = nullptr) {
   KnnScratch local_scratch;   // only when the caller brings none (freed on return)
   if (!sc) sc = &local_scratch;
   const bool use_tc = d_vec_bf16 != nullptr && tm_corpus != nullptr && d_ab != nullptr;
@@ -449,16 +449,13 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
   NRT_CUDA_TRY(cudaMemcpyAsync(dQ, h_queries, (size_t)nq * dims * sizeof(float), cudaMemcpyHostToDevice, st));
   NRT_CUDA_TRY(cudaMemsetAsync(dCn, 0, (size_t)nq * sizeof(int32_t), st));
   __nv_bfloat16* dQb = nullptr;
-  CUtensorMap tmQ, tmQ256s;
-  const CUtensorMap* tmQ256 = nullptr;
+  CUtensorMap tmQ;
   if (use_tc) {
     NRT_KNN_GET(13, dQb, (size_t)nq * dims * sizeof(__nv_bfloat16));
     tc::f32_to_bf16_kernel<<<256, 256, 0, st>>>(dQ, dQb, (size_t)nq * dims);
     NRT_CUDA_TRY(cudaGetLastError());
     int rc = tc::make_tensor_map_bf16(&tmQ, dQb, (uint64_t)nq, (uint64_t)dims, tc::BM);
     if (rc) return rc;
-    if ((rc = tc::make_tensor_map_bf16(&tmQ256s, dQb, (uint64_t)nq, (uint64_t)dims, tc::BM2))) return rc;
-    tmQ256 = &tmQ256s;
   }
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   float gemm_ms = 0.f, select_ms = 0.f;
@@ -475,34 +472,8 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
       tc::GemmParams G; G.M = nq; G.N = nc; G.K = dims; G.n_base = base; G.dnorm2 = d_norm2 + base; G.ab = d_ab + base; G.sim = sim & 0xff;
       G.S = (fused && !warm_chunk) ? nullptr : dS; G.ldS = fused ? warm : chunk;
       G.theta = dTheta; G.cc = dCC; G.cc_cnt = dCCn; G.cc_cap = cc_cap; G.filter = dF; G.vec_docs = d_vec_docs; G.live_bits = d_live_bits;
-      { static const int dbg = [] { const char* e = getenv("NRTGPU_KNN_DEBUG"); return e ? atoi(e) : 0; }(); G.debug = dbg; }
-      // default: one tile per CTA, 2 CTAs/SM (measured 4.9 ms at C4); the persistent double-buffered variant measured
-      // 7.5 ms -- both are bound by L2 -> SM operand traffic (48 KB per 128x256x64 k-block), see DESIGN.md 4.3
-      // NRTGPU_KNN_GEMM: "256" (default) = persistent 256 x 256 tiles, two TMEM accumulators; "128" = one 128 x 256 tile per
-      // CTA, 2 CTAs / SM (round 1); "p128" = persistent 128 x 256 with a double-buffered accumulator
-      // "db" (default) = 256 x 128 tiles double-buffered in TMEM
-      static const int gemm_kind = [] { const char* e = getenv("NRTGPU_KNN_GEMM"); return !e ? 3 : (e[0] == 'p' ? 1 : (e[0] == '1' ? 0 : (e[0] == '2' ? 2 : 3))); }();
-      static int sm_count = 0;
-      if (!sm_count) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev); }
-      if (gemm_kind == 3 && tmQ256 && tm_corpus128) {
-        const int m_tiles = (nq + tc::BM2 - 1) / tc::BM2;
-        const int tiles = m_tiles * ((nc + tc::BN3 - 1) / tc::BN3);
-        int grid = tiles < sm_count ? tiles : sm_count;
-        if (m_tiles <= grid) grid = grid / m_tiles * m_tiles;
-        tc::knn_gemm_bf16_db_kernel<<<grid, tc::kGemm2Threads, tc::kGemm3Smem, st>>>(*tmQ256, *tm_corpus128, G);
-      } else if (gemm_kind >= 2 && tmQ256) {
-        const int m_tiles = (nq + tc::BM2 - 1) / tc::BM2;
-        const int tiles = m_tiles * ((nc + tc::BN - 1) / tc::BN);
-        int grid = tiles < sm_count ? tiles : sm_count;
-        if (m_tiles <= grid) grid = grid / m_tiles * m_tiles;   // every CTA keeps one query tile (see the kernel's tile order)
-        tc::knn_gemm_bf16_256_kernel<<<grid, tc::kGemm2Threads, tc::kGemm2Smem, st>>>(*tmQ256, *tm_corpus, G);
-      } else if (gemm_kind != 1) {
-        dim3 grid((nq + tc::BM - 1) / tc::BM, (nc + tc::BN - 1) / tc::BN);
-        tc::knn_gemm_bf16_kernel<<<grid, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *tm_corpus, G);
-      } else {
-        const int tiles = ((nq + tc::BM - 1) / tc::BM) * ((nc + tc::BN - 1) / tc::BN);
-        tc::knn_gemm_bf16_persistent_kernel<<<tiles < sm_count ? tiles : sm_count, tc::kGemmThreads, tc::kPGemmSmem, st>>>(tmQ, *tm_corpus, G);
-      }
+      const int tiles = ((nq + tc::BM - 1) / tc::BM) * ((nc + tc::BN - 1) / tc::BN);
+      tc::knn_gemm_bf16_kernel<<<tiles, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *tm_corpus, G);
     } else {
       dim3 grid((nc + kKnnTile - 1) / kKnnTile, (nq + kKnnTile - 1) / kKnnTile);
       knn_dot_tile_kernel<<<grid, 256, 0, st>>>(dQ, d_vec + (size_t)base * dims, d_norm2 + base, nq, nc, dims, sim & 0xff, dS, chunk);
@@ -534,7 +505,7 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
     if (ovf) {
       if (stage_ms) for (auto& e : ev) cudaEventDestroy(e);
       return knn_search_host(d_vec, d_norm2, d_vec_docs, n, dims, sim, doc_base, n_docs, h_queries, nq, k, h_boosts, h_filter, st,
-                             out_docs, out_scores, out_counts, nullptr, nullptr, stage_ms, nullptr, sc, d_live_bits, dmax, n_uncertified, nullptr);
+                             out_docs, out_scores, out_counts, nullptr, nullptr, stage_ms, nullptr, sc, d_live_bits, dmax, n_uncertified);
     }
   }
   if (stage_ms) NRT_CUDA_TRY(cudaEventRecord(ev[0], st));

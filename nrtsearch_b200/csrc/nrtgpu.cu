@@ -1,4 +1,4 @@
-// nrtgpu.cu -- C ABI (include/nrtgpu.h) of the B200 query-execution engine: context, HBM index image,
+// nrtgpu.cu -- C ABI (include/nrtgpu.h) of the H100 query-execution engine: context, HBM index image,
 // batch compilation, kernel launches. No CPU fallback: every entry point needs a CUDA device.
 #include "../../include/nrtgpu.h"
 #include "bool_kernel.cuh"
@@ -198,8 +198,7 @@ struct nrtgpu_index {
   bool vec_is_byte = false;   // byte vector field (ByteVectorFieldDef): same image, byte score mapping
   DevBuf<float> vectors;
   DevBuf<__nv_bfloat16> vec_bf16;   // bf16 copy of the corpus for the tensor-core candidate stage (dims % 8 == 0)
-  CUtensorMap vec_tmap;             // TMA tensor map over vec_bf16 (256-row boxes)
-  CUtensorMap vec_tmap128;          // ... (128-row boxes: the double-buffered GEMM's corpus tile)
+  CUtensorMap vec_tmap;             // TMA tensor map over vec_bf16 (boxes of one GEMM corpus tile)
   DevBuf<float2> vec_ab;            // per-vector (a, b) of the approximate score a * dot + b
   bool vec_tc = false;
   float vec_dmax = 0.0f;    // largest vector magnitude (error bound of the kNN candidate-stage certificate)
@@ -355,7 +354,7 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   NRT_CUDA_TRY(cudaSetDevice(device_id));
   cudaDeviceProp prop;
   NRT_CUDA_TRY(cudaGetDeviceProperties(&prop, device_id));
-  if (prop.major < 10) NRT_FAIL(NRTGPU_ERR_CUDA, "nrtgpu_init: device is not sm_100 class (kernels are built for sm_100a only)");
+  if (prop.major != 9 || prop.minor != 0) NRT_FAIL(NRTGPU_ERR_CUDA, "nrtgpu_init: device is not sm_90 (kernels are built for sm_90a only)");
   std::unique_ptr<nrtgpu_ctx> c(new nrtgpu_ctx);   // released to the caller only when every attribute call succeeded
   c->device = device_id;
   c->sm_count = prop.multiProcessorCount;
@@ -383,9 +382,6 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   NRT_PROBE_ATTR(true, false) NRT_PROBE_ATTR(false, false) NRT_PROBE_ATTR(true, true) NRT_PROBE_ATTR(false, true)
 #undef NRT_PROBE_ATTR
   NRT_CUDA_TRY(cudaFuncSetAttribute(tc::knn_gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kGemmSmem));
-  NRT_CUDA_TRY(cudaFuncSetAttribute(tc::knn_gemm_bf16_db_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kGemm3Smem));
-  NRT_CUDA_TRY(cudaFuncSetAttribute(tc::knn_gemm_bf16_256_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kGemm2Smem));
-  NRT_CUDA_TRY(cudaFuncSetAttribute(tc::knn_gemm_bf16_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kPGemmSmem));
   *out = c.release();
   return NRTGPU_OK;
 }
@@ -637,7 +633,6 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
       tc::f32_to_bf16_kernel<<<1024, 256>>>(ix->vectors.p, ix->vec_bf16.p, (size_t)d->vec_count * d->vec_dims);
       NRT_CUDA_TRY(cudaGetLastError());
       if ((rc = tc::make_tensor_map_bf16(&ix->vec_tmap, ix->vec_bf16.p, (uint64_t)d->vec_count, (uint64_t)d->vec_dims, tc::BN))) return rc;
-      if ((rc = tc::make_tensor_map_bf16(&ix->vec_tmap128, ix->vec_bf16.p, (uint64_t)d->vec_count, (uint64_t)d->vec_dims, tc::BN3))) return rc;
       if ((rc = ix->vec_ab.alloc((size_t)d->vec_count))) return rc;
       knn_ab_kernel<<<(d->vec_count + 255) / 256, 256>>>(ix->vec_norm2.p, d->vec_count, d->vec_similarity, ix->vec_ab.p);
       NRT_CUDA_TRY(cudaGetLastError());
@@ -1674,7 +1669,7 @@ int nrtgpu_search_knn(nrtgpu_index* ix, const float* queries, int32_t nq, int32_
   return knn_search_host(ix->vectors.p, ix->vec_norm2.p, ix->vec_docs.p, ix->vec_count, ix->vec_dims, ix->vec_sim | (ix->vec_is_byte ? kKnnByteFlag : 0),
                          ix->doc_base, ix->n_docs, queries, nq, k, boosts, filter, (cudaStream_t)stream, out_docs,
                          out_scores, out_counts, tcp ? ix->vec_bf16.p : nullptr, tcp ? &ix->vec_tmap : nullptr, nullptr, ix->vec_ab.p,
-                         &ix->knn_scratch, ix->live_bits.p, ix->vec_dmax, &ix->knn_last_uncertified, tcp ? &ix->vec_tmap128 : nullptr);
+                         &ix->knn_scratch, ix->live_bits.p, ix->vec_dmax, &ix->knn_last_uncertified);
 }
 
 int nrtgpu_search_knn_timed(nrtgpu_index* ix, const float* queries, int32_t nq, int32_t k, void* stream, int32_t* out_docs,
@@ -1688,7 +1683,7 @@ int nrtgpu_search_knn_timed(nrtgpu_index* ix, const float* queries, int32_t nq, 
   return knn_search_host(ix->vectors.p, ix->vec_norm2.p, ix->vec_docs.p, ix->vec_count, ix->vec_dims, ix->vec_sim | (ix->vec_is_byte ? kKnnByteFlag : 0),
                          ix->doc_base, ix->n_docs, queries, nq, k, nullptr, nullptr, (cudaStream_t)stream, out_docs,
                          out_scores, out_counts, tcp ? ix->vec_bf16.p : nullptr, tcp ? &ix->vec_tmap : nullptr, stage_ms, ix->vec_ab.p,
-                         &ix->knn_scratch, ix->live_bits.p, ix->vec_dmax, &ix->knn_last_uncertified, tcp ? &ix->vec_tmap128 : nullptr);
+                         &ix->knn_scratch, ix->live_bits.p, ix->vec_dmax, &ix->knn_last_uncertified);
 }
 
 int32_t nrtgpu_knn_last_uncertified(const nrtgpu_index* ix) { return ix ? ix->knn_last_uncertified : 0; }

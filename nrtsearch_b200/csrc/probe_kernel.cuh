@@ -5,7 +5,7 @@
 //   ReqExclBulkScorer / ReqOptSumScorer (MUST_NOT and optional clauses looked up per candidate)
 // behind IndexSearcher.search (reference src/main/java/com/yelp/nrtsearch/server/handler/SearchHandler.java:1412).
 //
-// Design (B200-first, nothing like the per-document iterator chain of the reference):
+// Design (GPU-first, nothing like the per-document iterator chain of the reference):
 //   * work item = (query, doc slice, part), claimed from an atomic queue by PERSISTENT CTAs (3 or 4 per SM): no per-CTA
 //     launch cost; slice-major so that the CTAs resident together probe the same doc range of the dense tf planes in
 //     L2; a heavy (query, slice) is split into 2..16 parts so that no item is a large share of the launch; warm-up

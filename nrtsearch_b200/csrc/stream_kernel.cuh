@@ -131,7 +131,7 @@ struct alignas(128) StreamSmem {
   uint64_t tab_bar;
   unsigned long long theta;
 };
-static_assert(sizeof(StreamSmem) <= (kCtasPerSm == 1 ? 232448 : 115712), "StreamSmem exceeds the shared memory budget of sm_100");
+static_assert(sizeof(StreamSmem) <= (kCtasPerSm == 1 ? 232448 : 115712), "StreamSmem exceeds the shared memory budget of sm_90");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

@@ -2,8 +2,10 @@
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -49,12 +51,17 @@ def build(force: bool = False) -> str:
 
 def _native_so() -> str:
     """liboracle.so rebuilt with -O3 -march=native for the host it runs on (bench.py's cpu_baseline / reference arm: the
-    portable build that travels to the GPU box is -march=x86-64-v2). Same sources, same results (-ffp-contract=off, no
-    fast-math); falls back to the portable build when no compiler is present."""
-    so = os.path.join(_HERE, "liboracle_native.so")
+    portable in-tree build is -march=x86-64-v2). Same sources, same results (-ffp-contract=off, no fast-math); falls back
+    to the portable build when no compiler is present. The build goes to the temporary directory, keyed by the sources'
+    hash, so that the tree stays untouched (it may be read-only)."""
     src = [os.path.join(_HERE, f) for f in ("oracle.c", "oracle.h")]
     try:
-        if not os.path.exists(so) or any(os.path.getmtime(x) > os.path.getmtime(so) for x in src):
+        h = hashlib.sha256()
+        for x in src:
+            with open(x, "rb") as f:
+                h.update(f.read())
+        so = os.path.join(tempfile.gettempdir(), f"liboracle_native-{os.getuid()}-{h.hexdigest()[:16]}.so")
+        if not os.path.exists(so):
             tmp = so + f".{os.getpid()}.tmp"
             subprocess.check_call(["gcc", "-O3", "-march=native", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-fopenmp", "-std=c11",
                                    "-shared", "-o", tmp, src[0], "-lm"], stderr=subprocess.DEVNULL)

@@ -6,8 +6,8 @@
  * --impl reference legs use it, as the checker / reported CPU baseline.
  *
  * The arithmetic lives in org.apache.lucene:lucene-core:10.4.0
- * (reference gradle/libs.versions.toml:7,42), which is NOT vendored under
- * /root/reference; it is restated here from Lucene's published algorithm and
+ * (reference gradle/libs.versions.toml:7,42), which is NOT vendored in the
+ * reference (Yelp/nrtsearch); it is restated here from Lucene's published algorithm and
  * anchored on the reference's own call sites and known-answer tests:
  *   - BM25 term score: pinned bit-exactly by
  *       src/test/java/com/yelp/nrtsearch/server/query/multifunction/MultiFunctionScoreQueryTest.java:139
