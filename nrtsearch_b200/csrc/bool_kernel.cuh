@@ -21,6 +21,7 @@
 // used here only to drop hits that provably cannot enter the top-k (results stay exact).
 #pragma once
 #include "common.cuh"
+#include "../../include/nrtgpu.h"
 
 namespace nrtgpu {
 

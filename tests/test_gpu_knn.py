@@ -3,7 +3,9 @@ reference VectorFieldDefTest.java:1886-2117 compares exact search with brute for
 import numpy as np
 import pytest
 
+import knn_harness as kh
 import oracle
+from nrtsearch_b200 import _native
 from nrtsearch_b200 import index as ix
 from nrtsearch_b200.index import HostShard, TextField
 from nrtsearch_b200.search import GpuIndex, GpuIndexSearcher
@@ -11,9 +13,9 @@ from nrtsearch_b200.search import GpuIndex, GpuIndexSearcher
 pytestmark = pytest.mark.gpu
 
 
-def vec_shard(vectors, sim, vec_docs=None, n_docs=None, live_docs=None):
+def vec_shard(vectors, sim, vec_docs=None, n_docs=None, live_docs=None, doc_base=0):
     n = len(vectors) if n_docs is None else n_docs
-    return HostShard(n_docs=n, doc_base=0, term_off=np.zeros(1, np.int64), post_docs=np.zeros(0, np.int32),
+    return HostShard(n_docs=n, doc_base=doc_base, term_off=np.zeros(1, np.int64), post_docs=np.zeros(0, np.int32),
                      post_freqs=np.zeros(0, np.int32), fields=[], vectors=vectors, vec_similarity=sim, vec_docs=vec_docs,
                      live_docs=live_docs)
 
@@ -36,6 +38,34 @@ def check(gd, gs, gc, wd, ws, wc, rtol=1e-5):
                 assert abs(ws[q, pos[d]] - ws[q, i]) <= rtol * abs(ws[q, i]), (q, i, d)
             else:          # swapped with a doc just outside the oracle's list: only legal at the boundary tie
                 assert abs(gs[q, i] - ws[q, n - 1]) <= rtol * abs(ws[q, n - 1]), (q, i, d)
+
+
+def kprime(k, tensor_core=True):
+    """Candidates kept per query by knn_search_host: 4k (at least 128) for the bf16 stage, 2k (at least 64) for fp32."""
+    kp = max(128, 4 * k) if tensor_core else max(64, 2 * k)
+    return min(kp, 4096 - 256)
+
+
+def assert_certifiable(corpus, queries, sim, k, tensor_core=True, eligible=None):
+    """The exact gap between every query's k-th and k'-th best candidate scores (among eligible vectors) clearly
+    exceeds the candidate stage's error bound, so a correct candidate stage must certify every query: the bf16 bound
+    2^-7 (1 + 1e-3) |q| dmax (twice that for l2, |q| for cosine), or dims * 2^-23 for the fp32 stage."""
+    corpus = np.asarray(corpus, np.float64)
+    kp = kprime(k, tensor_core)
+    n_ok = len(corpus) if eligible is None else int(np.count_nonzero(eligible))
+    assert n_ok > kp, "the candidate list must be full for the certificate to matter"
+    eps = (2.0**-7 if tensor_core else corpus.shape[1] * 2.0**-23) * (1 + 1e-3)
+    dmax = np.linalg.norm(corpus, axis=1).max()
+    for q0 in range(0, len(queries), 16):
+        qs = np.asarray(queries[q0:q0 + 16], np.float64)
+        a = kh.approx_reference(qs, corpus, sim)
+        if eligible is not None:
+            a[:, ~np.asarray(eligible, bool)] = -np.inf
+        top = -np.partition(-a, [k - 1, kp - 1], axis=1)
+        gap = top[:, k - 1] - top[:, kp - 1]
+        qn = np.linalg.norm(qs, axis=1)
+        bound = eps * qn * ({ix.SIM_L2: 2 * dmax, ix.SIM_COSINE: 1.0}.get(sim, dmax))
+        assert (gap > 3 * bound).all(), np.min(gap / bound)
 
 
 @pytest.mark.parametrize("sim", [ix.SIM_L2, ix.SIM_COSINE, ix.SIM_MIP])
@@ -163,3 +193,95 @@ def test_knn_normalized_cosine(gpu_ctx):
     check(gd, gs, gc, wd, ws, wc)
     cd, cs, cc = oracle.knn_exact(raw, ix.SIM_COSINE, queries, 30)   # and it IS cosine similarity of the raw vectors
     np.testing.assert_allclose(gs, cs, rtol=2e-5)
+
+
+def knn_run(ctx, shard, queries, k, **kw):
+    """GpuIndexSearcher.knn on a fresh index image; also returns how many queries took the exact fallback."""
+    gix = GpuIndex(ctx, shard)
+    try:
+        gd, gs, gc = GpuIndexSearcher(gix).knn(queries, k, **kw)
+        unc = _native.gpu_lib().nrtgpu_knn_last_uncertified(gix.handle)
+    finally:
+        gix.close()
+    return gd, gs, gc, unc
+
+
+def test_knn_fused_chunk_schedule(gpu_ctx):
+    """500K vectors: the 32K unfused warm chunk, then fused chunks of 64K, 128K, 256K and a partial second 256K chunk
+    ending inside a 128-vector tile; filter, deletes and boosts; 300 queries = three 128-row query tiles. Certified:
+    the fused candidate stage alone must find the oracle's page."""
+    n, dims, k, nq = 500_000, 16, 10, 300
+    corpus = ix.synth_vectors(n, dims)
+    queries = ix.synth_vectors(nq, dims, seed=ix.SEED_VQUERIES)
+    rng = np.random.default_rng(21)
+    live = (rng.random(n) < 0.9).astype(np.uint8)
+    flt = (rng.random(n) < 0.8).astype(np.uint8)
+    boosts = rng.uniform(0.5, 2.0, nq).astype(np.float32)
+    assert_certifiable(corpus, queries, ix.SIM_MIP, k, eligible=(live & flt) != 0)
+    gd, gs, gc, unc = knn_run(gpu_ctx, vec_shard(corpus, ix.SIM_MIP, live_docs=live), queries, k, boosts=boosts,
+                              filter_docs=flt)
+    wd, ws, wc = oracle.knn_exact(corpus, ix.SIM_MIP, queries, k, filter_docs=flt, boosts=boosts, live_docs=live)
+    check(gd, gs, gc, wd, ws, wc)
+    assert unc == 0, unc
+
+
+@pytest.mark.parametrize("k", [256, 257, 1024])
+def test_knn_unfused_multi_chunk(gpu_ctx, k):
+    """k' = 4k > 1024 turns the fused epilogue off (k = 257: k' = 1028; k = 1024 = kMaxTopK: k' capped at 3840); k = 256
+    is the last fused k. 150K vectors = three 64K chunks of stored scores, the last one partial."""
+    n, dims, nq = 150_000, 32, 130
+    corpus = ix.synth_vectors(n, dims)
+    queries = ix.synth_vectors(nq, dims, seed=ix.SEED_VQUERIES)
+    assert_certifiable(corpus, queries, ix.SIM_COSINE, k)
+    gd, gs, gc, unc = knn_run(gpu_ctx, vec_shard(corpus, ix.SIM_COSINE), queries, k)
+    wd, ws, wc = oracle.knn_exact(corpus, ix.SIM_COSINE, queries, k)
+    check(gd, gs, gc, wd, ws, wc)
+    assert unc == 0, unc
+
+
+@pytest.mark.parametrize("dims, sim, force", [(3, ix.SIM_COSINE, False), (100, ix.SIM_L2, False), (96, ix.SIM_MIP, True)])
+def test_knn_simt_candidate_stage(gpu_ctx, monkeypatch, dims, sim, force):
+    """knn_dot_tile_kernel: dims % 8 != 0 (no TMA row pitch) or NRTGPU_KNN_SIMT=1; two 32K chunks."""
+    if force:
+        monkeypatch.setenv("NRTGPU_KNN_SIMT", "1")
+    n, k, nq = 40_000, 10, 70
+    corpus = ix.synth_vectors(n, dims)
+    queries = ix.synth_vectors(nq, dims, seed=ix.SEED_VQUERIES)
+    assert_certifiable(corpus, queries, sim, k, tensor_core=False)
+    gd, gs, gc, unc = knn_run(gpu_ctx, vec_shard(corpus, sim), queries, k)
+    wd, ws, wc = oracle.knn_exact(corpus, sim, queries, k)
+    check(gd, gs, gc, wd, ws, wc)
+    assert unc == 0, unc
+
+
+def test_knn_fused_overflow_reruns_without_fusion(gpu_ctx):
+    """A filter rejecting every vector of the 32K warm chunk leaves every threshold at -inf, so all 65 536 vectors of
+    the first fused chunk survive and overflow the 3072-key chunk buffer: the search reruns on the fp32 stage."""
+    n, dims, k = 100_000, 64, 10
+    corpus = ix.synth_vectors(n, dims)
+    queries = ix.synth_vectors(20, dims, seed=ix.SEED_VQUERIES)
+    flt = (np.arange(n) >= 32768).astype(np.uint8)
+    gd, gs, gc, _ = knn_run(gpu_ctx, vec_shard(corpus, ix.SIM_L2), queries, k, filter_docs=flt)
+    wd, ws, wc = oracle.knn_exact(corpus, ix.SIM_L2, queries, k, filter_docs=flt)
+    check(gd, gs, gc, wd, ws, wc)
+    assert (gd >= 32768).all()
+
+
+def test_knn_sparse_vec_docs_and_doc_base(gpu_ctx):
+    """A sparse vector field (vec_docs: ascending ordinal -> doc over twice as many docs) in a leaf with doc_base != 0;
+    filter and deletes are per doc. The oracle searches ordinals: filter and live map to ordinals, its ordinals to docs."""
+    n_vec, dims, k, nq, doc_base = 70_000, 32, 20, 40, 1_000_000
+    n_docs = 2 * n_vec
+    rng = np.random.default_rng(33)
+    vec_docs = np.sort(rng.choice(n_docs, n_vec, replace=False)).astype(np.int32)
+    corpus = ix.synth_vectors(n_vec, dims)
+    queries = ix.synth_vectors(nq, dims, seed=ix.SEED_VQUERIES)
+    live = (rng.random(n_docs) < 0.9).astype(np.uint8)
+    flt = (rng.random(n_docs) < 0.85).astype(np.uint8)
+    assert_certifiable(corpus, queries, ix.SIM_COSINE, k, eligible=(live[vec_docs] & flt[vec_docs]) != 0)
+    shard = vec_shard(corpus, ix.SIM_COSINE, vec_docs=vec_docs, n_docs=n_docs, live_docs=live, doc_base=doc_base)
+    gd, gs, gc, unc = knn_run(gpu_ctx, shard, queries, k, filter_docs=flt)
+    wo, ws, wc = oracle.knn_exact(corpus, ix.SIM_COSINE, queries, k, filter_docs=flt[vec_docs], live_docs=live[vec_docs])
+    wd = np.where(np.arange(k)[None, :] < wc[:, None], vec_docs[np.clip(wo, 0, n_vec - 1)] + doc_base, 0)
+    check(gd, gs, gc, wd, ws, wc)
+    assert unc == 0, unc
