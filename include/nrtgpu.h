@@ -316,6 +316,32 @@ int nrtgpu_search_knn_timed(nrtgpu_index* ix, const float* queries, int32_t nq, 
 /* number of queries of the most recent kNN call on this index that took the exact fallback */
 int32_t nrtgpu_knn_last_uncertified(const nrtgpu_index* ix);
 
+/* Exact kNN in which every query has its own filter query (KnnQuery.filter, reference KnnUtils.java:135-155). The filters
+ * are flat BooleanQuerys in the same clause format as nrtgpu_search_bool, and they are evaluated on the device.
+ *   filters[n_filters]: clause ranges into filter_clauses. Only matching counts: boosts and scores are ignored.
+ *   filter_of[nq]: index into filters, or -1 for no filter. Queries that share a filter pass the same index, and
+ *   each filter is evaluated once per call.
+ * Deleted docs never match. Results are as for nrtgpu_search_knn: the exact top-k among the docs that match the query's
+ * filter, so counts[q] < k when fewer match. Matching follows the boolean path: an empty clause range matches nothing, as an
+ * empty BooleanQuery does; so does a query of MUST_NOT clauses only.
+ * NRTGPU_ERR_INVALID: has_after on a filter, a filter_of entry or clause id out of range, an index without vectors, k outside
+ * 1..1024. NRTGPU_ERR_UNSUPPORTED: a filter shape outside the boolean path (more than 16 clauses or 8 term clauses); the
+ * byte filter of nrtgpu_search_knn still serves it.
+ * A query whose filter matches at most 1/320 of the vectors is scored exactly over those docs only; the others go through
+ * the candidate GEMM with the filter applied. The first path needs one vector per doc in doc order (ascending vec_docs, as
+ * Lucene assigns vector ordinals); on a shard whose vec_docs is not strictly ascending every query takes the second.
+ * Device scratch is bounded: the filter bitmaps of one call (one row of n_docs / 8 bytes per distinct filter) are capped at
+ * 128 MB, and a call with more distinct filters runs in groups of queries whose rows fit; the term bitmaps they are built
+ * from are capped at another 128 MB. nrtgpu_knn_last_uncertified counts this call's exact fallbacks. */
+int nrtgpu_search_knn_filtered(nrtgpu_index* ix, const float* queries, int32_t nq, int32_t k, const float* boosts,
+                               const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses,
+                               const nrtgpu_query* filters, int32_t n_filters, const int32_t* filter_of,
+                               void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts);
+
+/* of the most recent nrtgpu_search_knn_filtered call on this index: queries scored over their filter's docs only (the rest
+ * took the candidate GEMM), and the device time of the filter evaluation in ms (either pointer may be NULL) */
+int nrtgpu_knn_filter_stats(const nrtgpu_index* ix, int32_t* out_gather_queries, float* out_filter_ms);
+
 /* TopDocs.merge over `n_lists` per-shard lists resident on the DEVICE (the receive buffer of the NCCL
  * all-gather): docs/scores [n_lists][nq][top_k], counts [n_lists][nq]; outputs on the device. */
 int nrtgpu_merge_topk_device(nrtgpu_ctx* ctx, int32_t n_lists, int32_t nq, int32_t top_k,

@@ -27,6 +27,12 @@ public final class NrtGpu {
       long index, ByteBuffer queries, int nq, int k, ByteBuffer boosts, ByteBuffer filter,
       ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts);
 
+  /** kNN with one filter query per query vector (KnnQuery.filter); filterOf[q] indexes filters, -1 = none. */
+  public static native int searchKnnFiltered(
+      long index, ByteBuffer queries, int nq, int k, ByteBuffer boosts, ByteBuffer filterClauses,
+      int nFilterClauses, ByteBuffer filters, int nFilters, ByteBuffer filterOf, ByteBuffer outDocs,
+      ByteBuffer outScores, ByteBuffer outCounts);
+
   public static native int blendRrf(
       long ctx, int nRetrievers, int nq, int topIn, ByteBuffer docs, ByteBuffer counts,
       ByteBuffer boosts, int rankConstant, int topOut, ByteBuffer outDocs, ByteBuffer outScores,

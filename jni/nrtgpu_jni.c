@@ -54,6 +54,16 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchKnn(
                                      (const float*)ADDR(env, boosts), (const uint8_t*)ADDR(env, filter), NULL,
                                      (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores), (int32_t*)ADDR(env, outCounts)));
 }
+/* filterClauses / filters: direct buffers laid out as nrtgpu_clause[] / nrtgpu_query[]; filterOf: int32 per query (-1 = none) */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchKnnFiltered(
+    JNIEnv* env, jclass c, jlong ix, jobject queries, jint nq, jint k, jobject boosts, jobject filterClauses,
+    jint nFilterClauses, jobject filters, jint nFilters, jobject filterOf, jobject outDocs, jobject outScores, jobject outCounts) {
+  return fail(env, nrtgpu_search_knn_filtered((nrtgpu_index*)(intptr_t)ix, (const float*)ADDR(env, queries), nq, k,
+                                              (const float*)ADDR(env, boosts), (const nrtgpu_clause*)ADDR(env, filterClauses),
+                                              nFilterClauses, (const nrtgpu_query*)ADDR(env, filters), nFilters,
+                                              (const int32_t*)ADDR(env, filterOf), NULL, (int32_t*)ADDR(env, outDocs),
+                                              (float*)ADDR(env, outScores), (int32_t*)ADDR(env, outCounts)));
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_blendRrf(
     JNIEnv* env, jclass c, jlong ctx, jint nRetrievers, jint nq, jint topIn, jobject docs, jobject counts, jobject boosts,
     jint rankConstant, jint topOut, jobject outDocs, jobject outScores, jobject outCounts, jobject outTotal) {

@@ -97,6 +97,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_batch_run", "nrtgpu_batch_fetch", "nrtgpu_batch_device_results", "nrtgpu_batch_stats",
     "nrtgpu_batch_stage_ms", "nrtgpu_batch_reset_timing", "nrtgpu_batch_bind_output", "nrtgpu_batch_free", "nrtgpu_search_knn", "nrtgpu_search_knn_timed", "nrtgpu_merge_topk_device",
     "nrtgpu_blend_rrf", "nrtgpu_blend_scores", "nrtgpu_rescore_combine", "nrtgpu_knn_last_uncertified", "nrtgpu_packed_words", "nrtgpu_search_sorted", "nrtgpu_search_bool_aggs", "nrtgpu_score_docs", "nrtgpu_rescore_query", "nrtgpu_fetch_columns", "nrtgpu_index_set_live_docs", "nrtgpu_index_update_stats", "nrtgpu_searcher_create", "nrtgpu_searcher_search_bool", "nrtgpu_searcher_close", "nrtgpu_batcher_create", "nrtgpu_batcher_submit", "nrtgpu_batcher_stats", "nrtgpu_batcher_close", "nrtgpu_search_bool_ex", "nrtgpu_search_bool_packed", "nrtgpu_batch_set_limits", "nrtgpu_batch_fetch_ex", "nrtgpu_batch_bind_packed", "nrtgpu_merge_topk_packed",
+    "nrtgpu_search_knn_filtered", "nrtgpu_knn_filter_stats",
 ]
 
 _gpu = None
@@ -167,6 +168,10 @@ def gpu_lib() -> C.CDLL:
         lib.nrtgpu_merge_topk_packed.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.nrtgpu_knn_last_uncertified.argtypes = [C.c_void_p]
         lib.nrtgpu_knn_last_uncertified.restype = C.c_int32
+        lib.nrtgpu_search_knn_filtered.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(Clause),
+                                                   C.c_int32, C.POINTER(Query), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p]
+        lib.nrtgpu_knn_filter_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float)]
         lib.nrtgpu_merge_topk_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 7
         lib.nrtgpu_blend_rrf.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -102,12 +102,18 @@ struct GemmParams {
   const uint8_t* filter;  // per DOC 0/1 or NULL
   const int32_t* vec_docs;  // ordinal -> doc or NULL
   const uint32_t* live_bits;  // liveDocs bitmap or NULL
+  // per-query filter rows (KnnQuery.filter): query q keeps doc d iff bit d of row qrow[q] is set; qrow[q] < 0 = no filter
+  const uint32_t* qfilter = nullptr;   // [n_rows][qwords]
+  const int32_t* qrow = nullptr;       // [M] or NULL
+  int qwords = 0;
 };
 
 // One 128 x 128 output tile per CTA; grid = query tiles x corpus tiles, query tiles varying fastest so that the CTAs sharing
 // a corpus tile run together and the tile is fetched from HBM once and served to the other query tiles by L2.
-__global__ void __launch_bounds__(kGemmThreads, kGemmCtasPerSm)
-knn_gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams P) {
+// kRows: the fused epilogue also applies the per-query filter rows (P.qfilter / P.qrow); a separate instantiation keeps the
+// epilogue of unfiltered batches exactly as it was.
+template <bool kRows>
+__device__ __forceinline__ void knn_gemm_bf16_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& P) {
   extern __shared__ uint8_t gemm_raw[];
   uint8_t* base = (uint8_t*)(((uintptr_t)gemm_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* smA = base;
@@ -189,6 +195,8 @@ knn_gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
         }
     } else {        // fused top-k': keep only values that can still enter the query's best k'
       const float th = P.theta[gq];
+      const uint32_t* qf = nullptr;   // read once per accumulator row
+      if constexpr (kRows) { const int qr = P.qrow[gq]; if (qr >= 0) qf = P.qfilter + (size_t)qr * P.qwords; }
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
@@ -199,10 +207,11 @@ knn_gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
           if (gd < P.N && x >= th) {
             const int ord = P.n_base + gd;
             bool ok = true;
-            if (P.filter || P.live_bits) {
+            if (P.filter || P.live_bits || (kRows && qf)) {
               const int doc = P.vec_docs ? P.vec_docs[ord] : ord;
               if (P.filter) ok = P.filter[doc] != 0;
               if (ok && P.live_bits) ok = (P.live_bits[doc >> 5] >> (doc & 31)) & 1u;
+              if (kRows && ok && qf) ok = (qf[doc >> 5] >> (doc & 31)) & 1u;
             }
             if (ok) {
               const uint64_t key = make_key(x, ord);
@@ -230,6 +239,16 @@ knn_gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(kGemmThreads, kGemmCtasPerSm)
+knn_gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams P) {
+  knn_gemm_bf16_body<false>(tmA, tmB, P);
+}
+// the same with per-query filter rows
+__global__ void __launch_bounds__(kGemmThreads, kGemmCtasPerSm)
+knn_gemm_bf16_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams P) {
+  knn_gemm_bf16_body<true>(tmA, tmB, P);
 }
 
 __global__ void f32_to_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* __restrict__ out, size_t n) {

@@ -118,6 +118,8 @@ struct KnnSelectLaunch {
   uint64_t* cand;          // [nq][kprime] sorted desc keys (approx score, ord)
   int32_t* cand_cnt;       // [nq]
   float* theta_out;        // optional [nq]: the k'-th best approximate score once the list is full (threshold of the fused chunks)
+  // per-query filter rows: query q keeps doc d iff bit d of row qrow[q] is set; qrow[q] < 0 = no filter
+  const uint32_t* qfilter = nullptr; const int32_t* qrow = nullptr; int qwords = 0;
 };
 
 __global__ void __launch_bounds__(kKnnSelThreads) knn_select_kernel(KnnSelectLaunch L) {
@@ -125,6 +127,8 @@ __global__ void __launch_bounds__(kKnnSelThreads) knn_select_kernel(KnnSelectLau
   __shared__ int count;
   __shared__ unsigned long long theta;
   const int q = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+  const int qr = L.qrow ? L.qrow[q] : -1;
+  const uint32_t* qf = qr >= 0 ? L.qfilter + (size_t)qr * L.qwords : nullptr;
   int have = L.cand_cnt[q];
   for (int i = tid; i < have; i += kKnnSelThreads) buf[i] = L.cand[(size_t)q * L.kprime + i];
   if (tid == 0) { count = have; theta = (have == L.kprime) ? L.cand[(size_t)q * L.kprime + L.kprime - 1] : 0ull; }
@@ -148,10 +152,11 @@ __global__ void __launch_bounds__(kKnnSelThreads) knn_select_kernel(KnnSelectLau
     if (i < L.n_chunk) {
       int ord = L.chunk_base + i;
       bool ok = true;
-      if (L.filter || L.live_bits) {
+      if (L.filter || L.live_bits || qf) {
         const int doc = L.vec_docs ? L.vec_docs[ord] : ord;
         if (L.filter) ok = L.filter[doc] != 0;
         if (ok && L.live_bits) ok = (L.live_bits[doc >> 5] >> (doc & 31)) & 1u;
+        if (ok && qf) ok = (qf[doc >> 5] >> (doc & 31)) & 1u;
       }
       if (ok) { key = make_key(L.S[(size_t)q * L.ldS + i], ord); is_cand = key > theta; }
     }
@@ -297,6 +302,11 @@ struct KnnExactLaunch {
   int k, n_chunks;
   uint64_t* keys;              // [n_sel][n_chunks][k]
   int32_t* cnt;                // [n_sel][n_chunks]
+  // per-query filter rows: query q keeps doc d iff bit d of row qrow[q] is set; qrow[q] < 0 = no filter
+  const uint32_t* qfilter = nullptr; const int32_t* qrow = nullptr; int qwords = 0;
+  // optional gather mode: a query with filter row r scores only the ord_cnt[r] ordinals ords[ord_begin[r] ..] of its row's
+  // docs instead of every vector (chunk c covers list entries [c * kKnnExactChunk, (c + 1) * kKnnExactChunk))
+  const int32_t* ords = nullptr; const int64_t* ord_begin = nullptr; const int32_t* ord_cnt = nullptr;
 };
 
 __global__ void __launch_bounds__(256) knn_exact_chunk_kernel(KnnExactLaunch L) {
@@ -305,16 +315,20 @@ __global__ void __launch_bounds__(256) knn_exact_chunk_kernel(KnnExactLaunch L) 
   const int q = L.qsel[sel];
   const float* qv = L.Q + (size_t)q * L.dims;
   const float boost = L.boosts ? L.boosts[q] : 1.0f;
+  const int qr = L.qrow ? L.qrow[q] : -1;
+  const uint32_t* qf = qr >= 0 ? L.qfilter + (size_t)qr * L.qwords : nullptr;
+  const int32_t* list = (L.ords && qr >= 0) ? L.ords + L.ord_begin[qr] : nullptr;
   const int base = chunk * kKnnExactChunk;
-  const int m = min(kKnnExactChunk, L.n - base);
+  const int m = min(kKnnExactChunk, (list ? L.ord_cnt[qr] : L.n) - base);
   for (int c = warp; c < kKnnExactChunk; c += 8) {
     uint64_t key = 0ull;
     if (c < m) {
-      const int ord = base + c;
+      const int ord = list ? list[base + c] : base + c;
       const int doc = L.vec_docs ? L.vec_docs[ord] : ord;
       bool ok = true;
       if (L.filter) ok = L.filter[doc] != 0;
       if (ok && L.live_bits) ok = (L.live_bits[doc >> 5] >> (doc & 31)) & 1u;
+      if (ok && qf) ok = (qf[doc >> 5] >> (doc & 31)) & 1u;
       if (ok) {
         const float* dv = L.D + (size_t)ord * L.dims;
         double dot = 0, na = 0, nb = 0, d2 = 0;
@@ -384,7 +398,7 @@ __global__ void fill_f32_kernel(float* p, int n, float v) {
 // device scratch of one kNN call: slots grow on demand and are kept between calls (no cudaMalloc / cudaFree, which
 // synchronise the device, on the request path). The index owns one and serialises the calls that use it.
 struct KnnScratch {
-  static constexpr int kSlots = 16;
+  static constexpr int kSlots = 32;   // 0-16: knn_search_host, 17-27: per-query filters (knn_filter_kernel.cuh)
   void* p[kSlots] = {};
   size_t cap[kSlots] = {};
   ~KnnScratch() { for (auto q : p) if (q) cudaFree(q); }
@@ -400,15 +414,59 @@ struct KnnScratch {
 };
 #define NRT_KNN_GET(slot, ptr, bytes) do { int rc_ = sc->get((slot), (bytes), (void**)&(ptr)); if (rc_) return rc_; } while (0)
 
+// Exact evaluation of the queries sel[] (rows of X.Q) with the oracle's arithmetic over n_chunks chunks of kKnnExactChunk
+// vectors each (X.ords set: of their filter row's ordinal list); merge_slices_kernel merges the chunks' lists and the
+// pages overwrite rows sel[i] of the host outputs. X carries everything but qsel, n_chunks, keys and cnt.
+inline int knn_exact_host(KnnScratch* sc, cudaStream_t st, KnnExactLaunch X, int n_chunks, int doc_base,
+                          const std::vector<int32_t>& sel, int32_t* out_docs, float* out_scores, int32_t* out_counts) {
+  const int n_sel = (int)sel.size(), k = X.k;
+  int32_t *dSel = nullptr, *dCnt = nullptr, *dXD = nullptr, *dXC = nullptr; uint64_t* dKeys = nullptr; float* dXS = nullptr;
+  NRT_KNN_GET(15, dSel, (size_t)n_sel * sizeof(int32_t));
+  NRT_CUDA_TRY(cudaMemcpyAsync(dSel, sel.data(), (size_t)n_sel * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  // the slice lists can be large (n_sel * n_chunks * k keys): process the selected queries in groups that fit 256 MB
+  // (and the 65535 rows of a grid's y dimension)
+  const size_t per_q = (size_t)n_chunks * k * sizeof(uint64_t);
+  const int group = (int)std::max<size_t>(1, std::min<size_t>({(size_t)n_sel, ((size_t)256 << 20) / per_q, (size_t)65535}));
+  NRT_KNN_GET(5, dKeys, (size_t)group * per_q);   // slot 5 (the unfused score matrix) is free by now
+  NRT_KNN_GET(1, dCnt, (size_t)group * n_chunks * sizeof(int32_t) + (size_t)group * k * 8 + (size_t)group * 4);
+  dXD = dCnt + (size_t)group * n_chunks; dXS = (float*)(dXD + (size_t)group * k); dXC = (int32_t*)(dXS + (size_t)group * k);
+  std::vector<int32_t> hd((size_t)group * k), hc((size_t)group); std::vector<float> hs((size_t)group * k);
+  for (int g0 = 0; g0 < n_sel; g0 += group) {
+    const int gn = std::min(group, n_sel - g0);
+    X.qsel = dSel + g0; X.n_chunks = n_chunks; X.keys = dKeys; X.cnt = dCnt;
+    knn_exact_chunk_kernel<<<dim3((unsigned)n_chunks, (unsigned)gn), 256, 0, st>>>(X);
+    NRT_CUDA_TRY(cudaGetLastError());
+    MergeLaunch M; M.slice_keys = dKeys; M.slice_cnt = dCnt; M.n_lists = n_chunks; M.top_k = k; M.nq = gn; M.doc_base = doc_base;
+    M.out_docs = dXD; M.out_scores = dXS; M.out_counts = dXC;
+    M.total_hits = nullptr; M.pruned = nullptr; M.terminated = nullptr; M.terminate_after = 0; M.out_total = nullptr; M.out_flags = nullptr;
+    merge_slices_kernel<<<gn, kMergeThreads, 0, st>>>(M);
+    NRT_CUDA_TRY(cudaGetLastError());
+    NRT_CUDA_TRY(cudaMemcpyAsync(hd.data(), dXD, (size_t)gn * k * 4, cudaMemcpyDeviceToHost, st));
+    NRT_CUDA_TRY(cudaMemcpyAsync(hs.data(), dXS, (size_t)gn * k * 4, cudaMemcpyDeviceToHost, st));
+    NRT_CUDA_TRY(cudaMemcpyAsync(hc.data(), dXC, (size_t)gn * 4, cudaMemcpyDeviceToHost, st));
+    NRT_CUDA_TRY(cudaStreamSynchronize(st));
+    for (int i = 0; i < gn; ++i) {
+      const int q = sel[(size_t)(g0 + i)];
+      std::memcpy(out_docs + (size_t)q * k, hd.data() + (size_t)i * k, (size_t)k * 4);
+      std::memcpy(out_scores + (size_t)q * k, hs.data() + (size_t)i * k, (size_t)k * 4);
+      out_counts[q] = hc[(size_t)i];
+    }
+  }
+  return NRTGPU_OK;
+}
+
 // d_vec_bf16 / tm_corpus: bf16 copy of the corpus and its TMA tensor map (NULL => SIMT fp32 candidate stage).
 // stage_ms (optional): [0] = candidate GEMM kernels, [1] = select kernels, [2] = exact re-score (CUDA events on st).
+// d_qfilter / h_qrow (optional): per-query filter rows on the device, query q keeps doc d iff bit d of row h_qrow[q] is set
+// (h_qrow[q] < 0: no filter; ANDed with h_filter and the live docs).
 inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32_t* d_vec_docs, int n, int dims, int sim,
                            int doc_base, int n_docs, const float* h_queries, int nq, int k, const float* h_boosts,
                            const uint8_t* h_filter, cudaStream_t st, int32_t* out_docs, float* out_scores,
                            int32_t* out_counts, const __nv_bfloat16* d_vec_bf16 = nullptr,
                            const CUtensorMap* tm_corpus = nullptr, float* stage_ms = nullptr, const float2* d_ab = nullptr,
                            KnnScratch* sc = nullptr, const uint32_t* d_live_bits = nullptr, float dmax = 0.0f,
-                           int32_t* n_uncertified = nullptr) {
+                           int32_t* n_uncertified = nullptr, const uint32_t* d_qfilter = nullptr,
+                           const int32_t* h_qrow = nullptr, int qwords = 0) {
   KnnScratch local_scratch;   // only when the caller brings none (freed on return)
   if (!sc) sc = &local_scratch;
   const bool use_tc = d_vec_bf16 != nullptr && tm_corpus != nullptr && d_ab != nullptr;
@@ -446,6 +504,9 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
                   NRT_CUDA_TRY(cudaMemcpyAsync(dB, h_boosts, (size_t)nq * sizeof(float), cudaMemcpyHostToDevice, st)); }
   if (h_filter) { NRT_KNN_GET(12, dF, (size_t)n_docs);
                   NRT_CUDA_TRY(cudaMemcpyAsync(dF, h_filter, (size_t)n_docs, cudaMemcpyHostToDevice, st)); }
+  int32_t* dQrow = nullptr;
+  if (h_qrow) { NRT_KNN_GET(16, dQrow, (size_t)nq * sizeof(int32_t));
+                NRT_CUDA_TRY(cudaMemcpyAsync(dQrow, h_qrow, (size_t)nq * sizeof(int32_t), cudaMemcpyHostToDevice, st)); }
   NRT_CUDA_TRY(cudaMemcpyAsync(dQ, h_queries, (size_t)nq * dims * sizeof(float), cudaMemcpyHostToDevice, st));
   NRT_CUDA_TRY(cudaMemsetAsync(dCn, 0, (size_t)nq * sizeof(int32_t), st));
   __nv_bfloat16* dQb = nullptr;
@@ -472,8 +533,10 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
       tc::GemmParams G; G.M = nq; G.N = nc; G.K = dims; G.n_base = base; G.dnorm2 = d_norm2 + base; G.ab = d_ab + base; G.sim = sim & 0xff;
       G.S = (fused && !warm_chunk) ? nullptr : dS; G.ldS = fused ? warm : chunk;
       G.theta = dTheta; G.cc = dCC; G.cc_cnt = dCCn; G.cc_cap = cc_cap; G.filter = dF; G.vec_docs = d_vec_docs; G.live_bits = d_live_bits;
+      G.qfilter = d_qfilter; G.qrow = dQrow; G.qwords = qwords;
       const int tiles = ((nq + tc::BM - 1) / tc::BM) * ((nc + tc::BN - 1) / tc::BN);
-      tc::knn_gemm_bf16_kernel<<<tiles, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *tm_corpus, G);
+      if (dQrow) tc::knn_gemm_bf16_rows_kernel<<<tiles, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *tm_corpus, G);
+      else tc::knn_gemm_bf16_kernel<<<tiles, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *tm_corpus, G);
     } else {
       dim3 grid((nc + kKnnTile - 1) / kKnnTile, (nq + kKnnTile - 1) / kKnnTile);
       knn_dot_tile_kernel<<<grid, 256, 0, st>>>(dQ, d_vec + (size_t)base * dims, d_norm2 + base, nq, nc, dims, sim & 0xff, dS, chunk);
@@ -487,6 +550,7 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
     } else {
       KnnSelectLaunch S; S.S = dS; S.ldS = fused ? warm : chunk; S.n_chunk = nc; S.theta_out = fused ? dTheta : nullptr; S.chunk_base = base; S.filter = dF; S.live_bits = d_live_bits; S.vec_docs = d_vec_docs;
       S.kprime = kprime; S.nq = nq; S.cand = dC; S.cand_cnt = dCn;
+      S.qfilter = d_qfilter; S.qrow = dQrow; S.qwords = qwords;
       knn_select_kernel<<<nq, kKnnSelThreads, 0, st>>>(S);
     }
     NRT_CUDA_TRY(cudaGetLastError());
@@ -505,7 +569,8 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
     if (ovf) {
       if (stage_ms) for (auto& e : ev) cudaEventDestroy(e);
       return knn_search_host(d_vec, d_norm2, d_vec_docs, n, dims, sim, doc_base, n_docs, h_queries, nq, k, h_boosts, h_filter, st,
-                             out_docs, out_scores, out_counts, nullptr, nullptr, stage_ms, nullptr, sc, d_live_bits, dmax, n_uncertified);
+                             out_docs, out_scores, out_counts, nullptr, nullptr, stage_ms, nullptr, sc, d_live_bits, dmax, n_uncertified,
+                             d_qfilter, h_qrow, qwords);
     }
   }
   if (stage_ms) NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
@@ -537,39 +602,10 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
   for (int q = 0; q < nq; ++q) if (unsafe[(size_t)q]) sel.push_back(q);
   if (n_uncertified) *n_uncertified = (int32_t)sel.size();
   if (!sel.empty()) {
-    const int n_sel = (int)sel.size(), n_chunks = (n + kKnnExactChunk - 1) / kKnnExactChunk;
-    int32_t *dSel = nullptr, *dCnt = nullptr, *dXD = nullptr, *dXC = nullptr; uint64_t* dKeys = nullptr; float* dXS = nullptr;
-    NRT_KNN_GET(15, dSel, (size_t)n_sel * sizeof(int32_t));
-    NRT_CUDA_TRY(cudaMemcpyAsync(dSel, sel.data(), (size_t)n_sel * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    // the slice lists can be large (n_sel * n_chunks * k keys): process the selected queries in groups that fit 256 MB
-    const size_t per_q = (size_t)n_chunks * k * sizeof(uint64_t);
-    const int group = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_sel, ((size_t)256 << 20) / per_q));
-    NRT_KNN_GET(5, dKeys, (size_t)group * per_q);   // slot 5 (the unfused score matrix) is free by now
-    NRT_KNN_GET(1, dCnt, (size_t)group * n_chunks * sizeof(int32_t) + (size_t)group * k * 8 + (size_t)group * 4);
-    dXD = dCnt + (size_t)group * n_chunks; dXS = (float*)(dXD + (size_t)group * k); dXC = (int32_t*)(dXS + (size_t)group * k);
-    std::vector<int32_t> hd((size_t)group * k), hc((size_t)group); std::vector<float> hs((size_t)group * k);
-    for (int g0 = 0; g0 < n_sel; g0 += group) {
-      const int gn = std::min(group, n_sel - g0);
-      KnnExactLaunch X; X.Q = dQ; X.D = d_vec; X.n = n; X.dims = dims; X.sim = sim; X.qsel = dSel + g0; X.boosts = dB; X.filter = dF;
-      X.live_bits = d_live_bits; X.vec_docs = d_vec_docs; X.k = k; X.n_chunks = n_chunks; X.keys = dKeys; X.cnt = dCnt;
-      knn_exact_chunk_kernel<<<dim3((unsigned)n_chunks, (unsigned)gn), 256, 0, st>>>(X);
-      NRT_CUDA_TRY(cudaGetLastError());
-      MergeLaunch M; M.slice_keys = dKeys; M.slice_cnt = dCnt; M.n_lists = n_chunks; M.top_k = k; M.nq = gn; M.doc_base = doc_base;
-      M.out_docs = dXD; M.out_scores = dXS; M.out_counts = dXC;
-      M.total_hits = nullptr; M.pruned = nullptr; M.terminated = nullptr; M.terminate_after = 0; M.out_total = nullptr; M.out_flags = nullptr;
-      merge_slices_kernel<<<gn, kMergeThreads, 0, st>>>(M);
-      NRT_CUDA_TRY(cudaGetLastError());
-      NRT_CUDA_TRY(cudaMemcpyAsync(hd.data(), dXD, (size_t)gn * k * 4, cudaMemcpyDeviceToHost, st));
-      NRT_CUDA_TRY(cudaMemcpyAsync(hs.data(), dXS, (size_t)gn * k * 4, cudaMemcpyDeviceToHost, st));
-      NRT_CUDA_TRY(cudaMemcpyAsync(hc.data(), dXC, (size_t)gn * 4, cudaMemcpyDeviceToHost, st));
-      NRT_CUDA_TRY(cudaStreamSynchronize(st));
-      for (int i = 0; i < gn; ++i) {
-        const int q = sel[(size_t)(g0 + i)];
-        std::memcpy(out_docs + (size_t)q * k, hd.data() + (size_t)i * k, (size_t)k * 4);
-        std::memcpy(out_scores + (size_t)q * k, hs.data() + (size_t)i * k, (size_t)k * 4);
-        out_counts[q] = hc[(size_t)i];
-      }
-    }
+    KnnExactLaunch X; X.Q = dQ; X.D = d_vec; X.n = n; X.dims = dims; X.sim = sim; X.boosts = dB; X.filter = dF;
+    X.live_bits = d_live_bits; X.vec_docs = d_vec_docs; X.k = k;
+    X.qfilter = d_qfilter; X.qrow = dQrow; X.qwords = qwords;
+    return knn_exact_host(sc, st, X, (n + kKnnExactChunk - 1) / kKnnExactChunk, doc_base, sel, out_docs, out_scores, out_counts);
   }
   return NRTGPU_OK;
 }

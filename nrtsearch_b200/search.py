@@ -283,6 +283,31 @@ def compile_queries(queries: Sequence[object], search_after: Optional[Sequence[O
     return carr, len(flat), qarr, len(qs)
 
 
+def compile_filters(filter_queries: Sequence[Optional[object]], nq: int):
+    """Per-query kNN filter queries (KnnQuery.filter; None = no filter) -> (Clause[], n_clauses, Query[], n_filters,
+    filter_of int32[nq]) for nrtgpu_search_knn_filtered. Filters that compile to the same flat BooleanQuery, boosts aside
+    (a filter only matches), share one index, so the device evaluates each of them once per call."""
+    if len(filter_queries) != nq:
+        raise ValueError(f"filter_queries has {len(filter_queries)} entries for {nq} query vectors")
+    present = [i for i, f in enumerate(filter_queries) if f is not None]
+    filter_of = np.full(nq, -1, np.int32)
+    flat, qs, index_of = [], [], {}
+    if present:
+        carr, _, qarr, _ = compile_queries([filter_queries[i] for i in present])
+        for j, i in enumerate(present):
+            q = qarr[j]
+            cls = tuple((c.occur, c.kind, c.id, c.boost, c.lo, c.hi) for c in carr[q.clause_begin:q.clause_end])
+            key = (tuple(c[:3] + c[4:] for c in cls), q.min_should_match)
+            if key not in index_of:
+                index_of[key] = len(qs)
+                qs.append((len(flat), len(flat) + len(cls), q.min_should_match, 0, 0, 0.0))
+                flat.extend(cls)
+            filter_of[i] = index_of[key]
+    carr = (Clause * max(len(flat), 1))(*[Clause(*c) for c in flat])
+    qarr = (CQuery * max(len(qs), 1))(*[CQuery(*t) for t in qs])
+    return carr, len(flat), qarr, len(qs), filter_of
+
+
 class GpuContext:
     def __init__(self, device: int = 0):
         self._lib = _native.gpu_lib()
@@ -434,10 +459,12 @@ class GpuIndexSearcher:
         return out
 
     def knn_query(self, queries: np.ndarray, knn: KnnQuery, sim: int, boosts: Optional[np.ndarray] = None,
-                  filter_docs: Optional[np.ndarray] = None, stream: int = 0):
-        """KnnUtils.resolveKnnQueryAndBoost (:47-66) for a batch of query vectors under one KnnQuery configuration."""
+                  filter_docs: Optional[np.ndarray] = None, stream: int = 0,
+                  filter_queries: Optional[Sequence[Optional[object]]] = None):
+        """KnnUtils.resolveKnnQueryAndBoost (:47-66) for a batch of query vectors under one KnnQuery configuration;
+        filter_queries: the KnnQuery.filter of each query vector, or None (KnnUtils.java:135-155)."""
         knn.validate()
-        docs, scores, counts = self.knn(queries, knn.k, boosts, filter_docs, stream)
+        docs, scores, counts = self.knn(queries, knn.k, boosts, filter_docs, stream, filter_queries)
         if knn.similarity_threshold is not None:   # MinThresholdQuery: drop hits scoring below the threshold's score
             th = similarity_to_score(knn.similarity_threshold, sim, queries.shape[1])
             for q in range(len(counts)):
@@ -536,14 +563,24 @@ class GpuIndexSearcher:
         return self.search_batch([query], collector).top_docs(0)
 
     def knn(self, queries: np.ndarray, k: int, boosts: Optional[np.ndarray] = None,
-            filter_docs: Optional[np.ndarray] = None, stream: int = 0):
-        """Exact kNN (KnnUtils.resolveKnnQueryAndBoost with ExactVectorQuery semantics): returns docs, scores, counts."""
+            filter_docs: Optional[np.ndarray] = None, stream: int = 0, filter_queries: Optional[Sequence[Optional[object]]] = None):
+        """Exact kNN (KnnUtils.resolveKnnQueryAndBoost with ExactVectorQuery semantics): returns docs, scores, counts.
+        filter_docs: one 0/1 byte per doc, shared by the batch. filter_queries: one query object (KnnQuery.filter) or None per
+        query vector, evaluated on the device."""
         q = np.ascontiguousarray(queries, dtype=np.float32)
         nq = q.shape[0]
         docs = np.zeros((nq, k), np.int32)
         scores = np.zeros((nq, k), np.float32)
         counts = np.zeros(nq, np.int32)
         b = None if boosts is None else np.ascontiguousarray(boosts, dtype=np.float32)
+        if filter_queries is not None:
+            if filter_docs is not None:
+                raise ValueError("pass filter_docs or filter_queries, not both")
+            carr, ncl, qarr, nf, filter_of = compile_filters(filter_queries, nq)
+            check(self._lib.nrtgpu_search_knn_filtered(self.index.handle, q.ctypes.data, nq, k, None if b is None else b.ctypes.data,
+                                                       carr, ncl, qarr, nf, filter_of.ctypes.data, C.c_void_p(stream),
+                                                       docs.ctypes.data, scores.ctypes.data, counts.ctypes.data))
+            return docs, scores, counts
         f = None if filter_docs is None else np.ascontiguousarray(filter_docs, dtype=np.uint8)
         check(self._lib.nrtgpu_search_knn(self.index.handle, q.ctypes.data, nq, k,
                                           None if b is None else b.ctypes.data, None if f is None else f.ctypes.data,
