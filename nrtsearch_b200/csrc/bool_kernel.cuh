@@ -108,6 +108,11 @@ struct BoolLaunch {
   unsigned long long* total_hits;  // [nq]
   uint64_t* slice_keys;        // [nq][n_slices][top_k]
   int32_t* slice_cnt;          // [nq][n_slices]
+  // deadline, checked when a work item starts (deadline_passed, as in the probe kernel): a late item writes no keys,
+  // counts no hits and flags its query
+  long long deadline_ns;       // 0: no deadline; < 0: already expired
+  unsigned long long* clock0;
+  int32_t* timed_out;          // [nq]
 };
 
 // numeric range clause on one doc (IndexOrDocValuesQuery's doc-values side, reference IntFieldDef.java:124-158 inclusive
@@ -140,6 +145,7 @@ struct BoolSmem {
   DevClause cl[kMaxClauses];
   DevQuery q;
   int cand_count;
+  int skip;   // the work item started after the deadline
   unsigned long long theta;
 };
 
@@ -264,8 +270,11 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) 
       sm.q = L.queries[qi];
       sm.cand_count = 0;
       sm.theta = *(volatile unsigned long long*)&L.theta[qi];
+      sm.skip = L.deadline_ns && deadline_passed(L.deadline_ns, L.clock0);
+      if (sm.skip) L.timed_out[qi] = 1;
     }
     __syncthreads();
+    if (sm.skip) continue;   // (CTA-uniform) slice_cnt stays 0: the slice contributes no keys
     const int ncl = sm.q.n_clauses;
     if (tid < ncl) sm.cl[tid] = L.clauses[sm.q.clause_begin + tid];
     for (int i = tid; i < kWindowDocs; i += kThreads) sm.slots[i] = 0;

@@ -73,6 +73,18 @@ __device__ __forceinline__ int next_pow2(int x) {
   while (p < x) p <<= 1;
   return p;
 }
+
+// Deadline of a run (SearchCutoffWrapper): the first work item of the run stamps *clock0 with %globaltimer; an item
+// that starts more than deadline_ns later is late. deadline_ns < 0: the request's budget was spent before the launch.
+// Called by one thread per work item, only when a deadline is set (deadline_ns != 0).
+__device__ __forceinline__ bool deadline_passed(long long deadline_ns, unsigned long long* clock0) {
+  if (deadline_ns < 0) return true;
+  unsigned long long now;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+  unsigned long long t0 = atomicCAS(clock0, 0ull, now);
+  if (t0 == 0ull) t0 = now;
+  return now > t0 && now - t0 > (unsigned long long)deadline_ns;   // (another CTA may have stamped clock0 after this one read the timer)
+}
 #endif
 
 }  // namespace nrtgpu

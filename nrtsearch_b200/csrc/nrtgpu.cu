@@ -1094,6 +1094,10 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   NRT_CUDA_TRY(cudaMemsetAsync(b->pruned.p, 0, b->pruned.bytes(), st));
   NRT_CUDA_TRY(cudaMemsetAsync(b->terminated.p, 0, b->terminated.bytes(), st));
   if (b->work_counter.p) NRT_CUDA_TRY(cudaMemsetAsync(b->work_counter.p, 0, b->work_counter.bytes(), st));
+  if (b->limits_active) {   // every engine, and batches without work items: batch_fetch_impl reads timed_out of THIS run
+    NRT_CUDA_TRY(cudaMemsetAsync(b->clock0.p, 0, sizeof(unsigned long long), st));
+    NRT_CUDA_TRY(cudaMemsetAsync(b->timed_out.p, 0, b->timed_out.bytes(), st));
+  }
   const bool debug = b->ix->ctx->debug_modes;
   cudaEvent_t* ev = b->ev[b->runs_recorded % nrtgpu_batch::kEvRing];
   NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
@@ -1105,6 +1109,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
     L.n_work = b->n_work; L.n_slices = b->n_lists; L.top_k = b->top_k;
     L.theta = b->theta.p; L.total_hits = b->total_hits.p;
     L.slice_keys = b->slice_keys.p; L.slice_cnt = b->slice_cnt.p;
+    L.deadline_ns = b->limits_active ? b->deadline_ns : 0; L.clock0 = b->clock0.p; L.timed_out = b->timed_out.p;
     if (!b->wide_slots) {
       const int n_probe = b->n_probe_simple + b->n_probe_generic;
       if (n_probe > 0) {
@@ -1120,7 +1125,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         P.n_lists = b->n_lists; P.parts_max = b->parts_max; P.n_slices = b->n_slices; P.top_k = b->top_k; P.slice_docs = b->slice_docs; P.n_gran = b->n_gran;
         P.threshold = b->threshold; P.pruned = b->pruned.p; P.theta = L.theta; P.total_hits = L.total_hits;
         P.slice_keys = L.slice_keys; P.slice_cnt = L.slice_cnt;
-        P.deadline_ns = b->limits_active ? b->deadline_ns : 0; P.clock0 = b->clock0.p; P.timed_out = b->timed_out.p;
+        P.deadline_ns = L.deadline_ns; P.clock0 = L.clock0; P.timed_out = L.timed_out;
         P.terminate_after = b->ta_scalar; P.terminated = b->terminated.p;
         P.sort_kind = b->sort_kind; P.sort_reverse = b->sort_reverse;
         P.sort_codes = b->sort_kind == NRTGPU_SORT_COLUMN ? b->ix->col_code[(size_t)b->sort_column]->p : nullptr;
@@ -1149,10 +1154,6 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
           if ((rc_dbg = b->agg_launch.upload_async(&A, 1, st))) return rc_dbg;
           NRT_CUDA_TRY(cudaStreamSynchronize(st));   // A is a stack object
           P.aggs = b->agg_launch.p;
-        }
-        if (P.deadline_ns) {
-          NRT_CUDA_TRY(cudaMemsetAsync(b->clock0.p, 0, sizeof(unsigned long long), st));
-          NRT_CUDA_TRY(cudaMemsetAsync(b->timed_out.p, 0, b->timed_out.bytes(), st));
         }
         if (debug) {
           if (!b->probe_stats.p && (rc_dbg = b->probe_stats.alloc(32))) return rc_dbg;

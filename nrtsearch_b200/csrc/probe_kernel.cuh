@@ -401,16 +401,8 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       const int w = (int)atomicAdd(L.work_counter, 1u);
       sm.wi = w;
       sm.skip = 0;
-      if (L.deadline_ns && w < L.n_work) {
-        bool late = L.deadline_ns < 0;   // the request's budget was spent before the launch
-        if (!late) {
-          unsigned long long now;
-          asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-          unsigned long long t0 = atomicCAS(L.clock0, 0ull, now);
-          if (t0 == 0ull) t0 = now;
-          late = now > t0 && now - t0 > (unsigned long long)L.deadline_ns;   // (another CTA may have stamped clock0 after this one read the timer)
-        }
-        if (late) { sm.skip = 1; L.timed_out[L.work_query[w]] = 1; }   // drain the queue
+      if (L.deadline_ns && w < L.n_work && deadline_passed(L.deadline_ns, L.clock0)) {
+        sm.skip = 1; L.timed_out[L.work_query[w]] = 1;   // drain the queue
       }
     }
     __syncthreads();

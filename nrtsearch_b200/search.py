@@ -599,8 +599,12 @@ class GpuLeafSearcher:
         check(self._lib.nrtgpu_searcher_create(ctx.handle, arr, len(leaves), C.byref(h)))
         self.handle, self.leaves = h, list(leaves)
 
-    def search_batch(self, queries: Sequence[object], collector: RelevanceCollector, stream: int = 0) -> BatchResult:
-        carr, ncl, qarr, nq = compile_queries(queries)
+    def search_batch(self, queries: Sequence[object], collector: RelevanceCollector, stream: int = 0,
+                     search_after: Optional[Sequence[Optional[ScoreDoc]]] = None) -> BatchResult:
+        """search_after: one reader-wide ScoreDoc (or None) per query; every leaf pages after it (TopDocs.merge of the pages)."""
+        if search_after is None and collector.search_after is not None:
+            search_after = [collector.search_after] * len(queries)
+        carr, ncl, qarr, nq = compile_queries(queries, search_after)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
