@@ -98,8 +98,9 @@ typedef struct {
   const int64_t* const* column_offsets; /* NULL, or [n_columns]: a non-NULL entry makes column c MULTI-valued (SORTED_NUMERIC doc
                                        values, reference NumberFieldDef.java multiValued): int64[n_docs+1] offsets into columns[c],
                                        which then holds the flattened values, ascending within a doc. A range clause matches a doc
-                                       when ANY of its values lies in [lo, hi] (SortedNumericDocValuesRangeQuery). Sorting, terms /
-                                       min / max / sum collectors and fetch on such a column answer NRTGPU_ERR_UNSUPPORTED. */
+                                       when ANY of its values lies in [lo, hi] (SortedNumericDocValuesRangeQuery). nrtgpu_search_sorted,
+                                       terms / min / max / sum collectors and fetch on such a column answer NRTGPU_ERR_UNSUPPORTED;
+                                       nrtgpu_search_sorted_fields sorts on it (MIN / MAX selector). */
 } nrtgpu_shard_desc;
 
 int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* desc, nrtgpu_index** out);
@@ -184,7 +185,7 @@ int nrtgpu_search_bool_packed(nrtgpu_index* ix, const nrtgpu_clause* clauses, in
  * .../field/NumberFieldDef.java:266-278 = SortedNumericSortField(type, reverse) with missingValue from
  * getSortMissingValue(missingLast)). One sort key + the implicit doc-id tie-break (lower doc first), i.e. the Sort
  * [<numeric doc-value field>], [docid] or [docid reverse]; other sorts (several fields, score mixed in) return
- * NRTGPU_ERR_UNSUPPORTED. Values live in the column's sortable-long domain (the adaptor maps int/long directly and
+ * NRTGPU_ERR_UNSUPPORTED (nrtgpu_search_sorted_fields below serves them). Values live in the column's sortable-long domain (the adaptor maps int/long directly and
  * float/double through NumericUtils.floatToSortableInt / doubleToSortableLong, exactly as the range query bounds).
  *   missing_value: what a doc WITHOUT a value sorts as (Integer/Long.MIN|MAX_VALUE, -+Infinity in the sortable domain:
  *                  the reference picks MAX when missingLast, irrespective of `reverse`);
@@ -208,6 +209,46 @@ int nrtgpu_search_sorted(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
                          int32_t* out_docs, int64_t* out_sort_values, int32_t* out_counts,
                          int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
                          uint8_t* out_terminated_early);
+
+/* Sort on several fields (a Sort of 1..8 SortFields, SortParser.parseSort :54-92; Sortable.java:34-45). Each field is
+ *   NRTGPU_SORT_COLUMN  a numeric doc-value column (sortable-long domain), ascending unless reverse; a doc without a value
+ *                       sorts as missing_value; on a MULTI-valued column `selector` picks the doc's smallest (MIN, the
+ *                       default) or largest (MAX) value (SortedNumericSelector), ignored on a single-valued one;
+ *   NRTGPU_SORT_DOCID   the doc id, ascending unless reverse; the fields after it cannot decide anything and are ignored;
+ *   NRTGPU_SORT_SCORE   the BM25 score, higher first unless reverse (RelevanceComparator); FIRST position only.
+ * The implicit last tie-break is the doc id, ascending. An order (nrtgpu_sort_order) ranks every doc of the image under
+ * one Sort once (an O(n log n) device sort on `stream`); it depends on the columns only, so it stays valid across
+ * nrtgpu_index_set_live_docs and nrtgpu_index_update_stats: build one per (leaf, Sort) and reuse it for every request.
+ * It holds 8 bytes per doc of device memory (nrtgpu_sort_order_device_bytes) and must be closed before its index.
+ *   nrtgpu_sort_order_create: NRTGPU_ERR_INVALID for n_fields < 1, a bad kind or selector, a column out of range;
+ *                             NRTGPU_ERR_UNSUPPORTED for n_fields > 8 or a SCORE after the first position.
+ *   nrtgpu_search_sorted_fields: as nrtgpu_search_sorted (exact totalHits, the same limits and refusals) with the order's
+ *     Sort. out_sort_values [nq*top_k*n_fields] = FieldDoc.fields of every hit: a column's selected value or missing_value,
+ *     the global doc id for DOCID, the score's float bits zero-extended for SCORE (Float.floatToIntBits).
+ *     after_values [nq*n_fields] (same encoding) + nrtgpu_query.has_after / after_doc: a hit qualifies iff its field tuple
+ *     sorts strictly after the after tuple, or ties with it and has a greater global doc id than after_doc
+ *     (PagingFieldCollector); the values need not be held by any doc of this leaf.
+ *     NRTGPU_ERR_INVALID: an order of another index, has_after without after_values. */
+enum { NRTGPU_SORT_SCORE = 3 };
+enum { NRTGPU_SELECT_MIN = 0, NRTGPU_SELECT_MAX = 1 };
+typedef struct {
+  int32_t kind;          /* NRTGPU_SORT_COLUMN, NRTGPU_SORT_DOCID or NRTGPU_SORT_SCORE */
+  int32_t column;        /* NRTGPU_SORT_COLUMN: doc-value column id */
+  int32_t reverse;
+  int32_t selector;      /* NRTGPU_SELECT_MIN / _MAX (multi-valued columns) */
+  int64_t missing_value;
+} nrtgpu_sort_field;
+typedef struct nrtgpu_sort_order nrtgpu_sort_order;
+int nrtgpu_sort_order_create(nrtgpu_index* ix, const nrtgpu_sort_field* fields, int32_t n_fields, void* stream,
+                             nrtgpu_sort_order** out);
+int64_t nrtgpu_sort_order_device_bytes(const nrtgpu_sort_order* o);
+int nrtgpu_sort_order_close(nrtgpu_sort_order* o);
+int nrtgpu_search_sorted_fields(nrtgpu_index* ix, const nrtgpu_sort_order* order, const nrtgpu_clause* clauses,
+                                int32_t n_clauses, const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                const int64_t* after_values, const nrtgpu_search_limits* limits, void* stream,
+                                int32_t* out_docs, int64_t* out_sort_values, int32_t* out_counts,
+                                int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
+                                uint8_t* out_terminated_early);
 
 /* Aggregating "additional collectors" over ALL docs matching each query (ScoreMode.COMPLETE: RelevanceCollector.java:55-62
  * forces totalHitsThreshold = MAX when additional collectors exist; fan-out SearchCollectorManager.java:192-198):

@@ -25,6 +25,9 @@ public class GpuIndexSearcher extends MyIndexSearcher {
   private final long gpuIndex; // nrtgpu_index* of this reader version
   private final long batcher; // nrtgpu_batcher* bound to gpuIndex
   private final GpuQueryCompiler compiler; // term -> dense id dictionary built with the image
+  // nrtgpu_sort_order* of this leaf per Sort (key: its nrtgpu_sort_field records)
+  private final java.util.concurrent.ConcurrentHashMap<ByteBuffer, Long> sortOrders =
+      new java.util.concurrent.ConcurrentHashMap<>();
 
   protected GpuIndexSearcher(
       IndexReader reader,
@@ -45,6 +48,10 @@ public class GpuIndexSearcher extends MyIndexSearcher {
     GpuQueryCompiler.Compiled c = compiler.tryCompile(query, collectorManager);
     if (c == null) {
       return super.search(query, collectorManager); // not on the GPU path: Lucene
+    }
+    if (c.sortFields() != null) {
+      T sorted = searchSortedFields(c);
+      return sorted != null ? sorted : super.search(query, collectorManager);
     }
     int k = c.topK();
     ByteBuffer docs = direct(4 * k), scores = direct(4 * k), count = direct(4), total = direct(8);
@@ -73,7 +80,58 @@ public class GpuIndexSearcher extends MyIndexSearcher {
         diag.getInt(16));
   }
 
+  /**
+   * SortFieldCollector with a Sort of several fields (or a score / multi-valued field): one nrtgpu_sort_order per Sort,
+   * built on first use and kept with this leaf's image (it depends on the columns only). null = UNSUPPORTED: Lucene.
+   */
+  private <T> T searchSortedFields(GpuQueryCompiler.Compiled c) {
+    ByteBuffer fields = c.sortFields();
+    int nFields = c.numSortFields(), k = c.topK();
+    byte[] spec = new byte[24 * nFields];
+    fields.duplicate().get(spec);
+    long order;
+    try {
+      order =
+          sortOrders.computeIfAbsent(
+              java.nio.ByteBuffer.wrap(spec),
+              key -> {
+                ByteBuffer out = direct(8);
+                NrtGpu.sortOrderCreate(gpuIndex, fields, nFields, out);
+                return out.getLong(0);
+              });
+    } catch (UnsupportedOperationException e) {
+      return null;
+    }
+    ByteBuffer docs = direct(4 * k), values = direct(8 * k * nFields), count = direct(4), total = direct(8);
+    ByteBuffer relation = direct(1), hitTimeout = direct(1), terminated = direct(1);
+    try {
+      NrtGpu.searchSortedFields(
+          gpuIndex, order, c.clauses(), c.numClauses(), c.queries(), 1, k, 0, c.afterValues(), c.limits(), docs,
+          values, count, total, relation, hitTimeout, terminated);
+    } catch (UnsupportedOperationException e) {
+      return null;
+    }
+    int n = count.getInt(0);
+    int[] hitDocs = new int[n];
+    long[][] hitValues = new long[n][nFields];
+    for (int i = 0; i < n; ++i) {
+      hitDocs[i] = docs.getInt(4 * i);
+      for (int f = 0; f < nFields; ++f) {
+        hitValues[i][f] = values.getLong(8 * (i * nFields + f));
+      }
+    }
+    TotalHits.Relation rel =
+        relation.get(0) == 0
+            ? TotalHits.Relation.EQUAL_TO
+            : TotalHits.Relation.GREATER_THAN_OR_EQUAL_TO;
+    return c.toSortedResult(
+        new TotalHits(total.getLong(0), rel), hitDocs, hitValues, hitTimeout.get(0) != 0, terminated.get(0) != 0);
+  }
+
   public void close() {
+    for (long order : sortOrders.values()) {
+      NrtGpu.sortOrderClose(order);
+    }
     NrtGpu.batcherClose(batcher);
     NrtGpu.indexClose(gpuIndex);
   }
@@ -98,6 +156,33 @@ public class GpuIndexSearcher extends MyIndexSearcher {
       int totalHitsThreshold();
 
       <T> T toResult(TopDocs topDocs, double queueMs, double searchMs, int batchSize);
+
+      /** SortFieldCollector requests: nrtgpu_sort_field[numSortFields()], or null for relevance. */
+      default ByteBuffer sortFields() {
+        return null;
+      }
+
+      default int numSortFields() {
+        return 0;
+      }
+
+      default ByteBuffer queries() { // direct, one nrtgpu_query (has_after / after_doc of the FieldDoc)
+        return null;
+      }
+
+      default ByteBuffer afterValues() { // direct, numSortFields() int64 FieldDoc values, or null
+        return null;
+      }
+
+      default ByteBuffer limits() { // direct nrtgpu_search_limits, or null
+        return null;
+      }
+
+      /** TopFieldDocs from raw FieldDoc values (the compiler knows each field's type). */
+      default <T> T toSortedResult(
+          TotalHits totalHits, int[] docs, long[][] values, boolean hitTimeout, boolean terminatedEarly) {
+        throw new UnsupportedOperationException("sorted results");
+      }
     }
   }
 }

@@ -55,6 +55,20 @@ public final class NrtGpu {
       ByteBuffer outCounts, ByteBuffer outTotalHits, ByteBuffer outRelation,
       ByteBuffer outHitTimeout, ByteBuffer outTerminatedEarly);
 
+  /** fields = nFields nrtgpu_sort_field; the order handle is written to outOrder (8 bytes). */
+  public static native int sortOrderCreate(long index, ByteBuffer fields, int nFields, ByteBuffer outOrder);
+
+  public static native long sortOrderDeviceBytes(long order);
+
+  public static native int sortOrderClose(long order);
+
+  /** afterValues = nq * nFields FieldDoc values (or null); outSortValues = nq * topK * nFields. */
+  public static native int searchSortedFields(
+      long index, long order, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK,
+      int flags, ByteBuffer afterValues, ByteBuffer limits, ByteBuffer outDocs, ByteBuffer outSortValues,
+      ByteBuffer outCounts, ByteBuffer outTotalHits, ByteBuffer outRelation,
+      ByteBuffer outHitTimeout, ByteBuffer outTerminatedEarly);
+
   public static native int scoreDocs(
       long index, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int nHits,
       ByteBuffer docs, ByteBuffer counts, ByteBuffer outMatches, ByteBuffer outScores);

@@ -105,6 +105,31 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchSorted(
                                         (uint8_t*)ADDR(env, outRelation), (uint8_t*)ADDR(env, outHitTimeout),
                                         (uint8_t*)ADDR(env, outTerminatedEarly)));
 }
+/* fields: a direct ByteBuffer of nFields nrtgpu_sort_field; the order handle goes to outOrder (a direct ByteBuffer of 8 bytes) */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_sortOrderCreate(
+    JNIEnv* env, jclass c, jlong ix, jobject fields, jint nFields, jobject outOrder) {
+  return fail(env, nrtgpu_sort_order_create((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_sort_field*)ADDR(env, fields), nFields, NULL,
+                                            (nrtgpu_sort_order**)ADDR(env, outOrder)));
+}
+JNIEXPORT jlong JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_sortOrderDeviceBytes(JNIEnv* env, jclass c, jlong order) {
+  return (jlong)nrtgpu_sort_order_device_bytes((const nrtgpu_sort_order*)(intptr_t)order);
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_sortOrderClose(JNIEnv* env, jclass c, jlong order) {
+  return fail(env, nrtgpu_sort_order_close((nrtgpu_sort_order*)(intptr_t)order));
+}
+/* afterValues: nq * nFields int64 (FieldDoc.fields) or null */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchSortedFields(
+    JNIEnv* env, jclass c, jlong ix, jlong order, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
+    jobject afterValues, jobject limits, jobject outDocs, jobject outSortValues, jobject outCounts, jobject outTotalHits,
+    jobject outRelation, jobject outHitTimeout, jobject outTerminatedEarly) {
+  return fail(env, nrtgpu_search_sorted_fields((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_sort_order*)(intptr_t)order,
+                                               (const nrtgpu_clause*)ADDR(env, clauses), nClauses, (const nrtgpu_query*)ADDR(env, queries),
+                                               nq, topK, flags, (const int64_t*)ADDR(env, afterValues),
+                                               (const nrtgpu_search_limits*)ADDR(env, limits), NULL, (int32_t*)ADDR(env, outDocs),
+                                               (int64_t*)ADDR(env, outSortValues), (int32_t*)ADDR(env, outCounts),
+                                               (int64_t*)ADDR(env, outTotalHits), (uint8_t*)ADDR(env, outRelation),
+                                               (uint8_t*)ADDR(env, outHitTimeout), (uint8_t*)ADDR(env, outTerminatedEarly)));
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_scoreDocs(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject queries, jint nq, jint nHits, jobject docs,
     jobject counts, jobject outMatches, jobject outScores) {

@@ -71,6 +71,11 @@ class Sort(C.Structure):
                 ("missing_value", C.c_int64), ("after_values", C.c_void_p)]
 
 
+class SortField(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("column", C.c_int32), ("reverse", C.c_int32), ("selector", C.c_int32),
+                ("missing_value", C.c_int64)]
+
+
 class Diagnostics(C.Structure):
     _fields_ = [("queue_ms", C.c_double), ("search_ms", C.c_double), ("batch_size", C.c_int32), ("reserved", C.c_int32)]
 
@@ -98,6 +103,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_batch_stage_ms", "nrtgpu_batch_reset_timing", "nrtgpu_batch_bind_output", "nrtgpu_batch_free", "nrtgpu_search_knn", "nrtgpu_search_knn_timed", "nrtgpu_merge_topk_device",
     "nrtgpu_blend_rrf", "nrtgpu_blend_scores", "nrtgpu_rescore_combine", "nrtgpu_knn_last_uncertified", "nrtgpu_packed_words", "nrtgpu_search_sorted", "nrtgpu_search_bool_aggs", "nrtgpu_score_docs", "nrtgpu_rescore_query", "nrtgpu_fetch_columns", "nrtgpu_index_set_live_docs", "nrtgpu_index_update_stats", "nrtgpu_searcher_create", "nrtgpu_searcher_search_bool", "nrtgpu_searcher_close", "nrtgpu_batcher_create", "nrtgpu_batcher_submit", "nrtgpu_batcher_stats", "nrtgpu_batcher_close", "nrtgpu_search_bool_ex", "nrtgpu_search_bool_packed", "nrtgpu_batch_set_limits", "nrtgpu_batch_fetch_ex", "nrtgpu_batch_bind_packed", "nrtgpu_merge_topk_packed",
     "nrtgpu_search_knn_filtered", "nrtgpu_knn_filter_stats",
+    "nrtgpu_sort_order_create", "nrtgpu_sort_order_device_bytes", "nrtgpu_sort_order_close", "nrtgpu_search_sorted_fields",
 ]
 
 _gpu = None
@@ -142,7 +148,13 @@ def gpu_lib() -> C.CDLL:
                                                   C.c_int32, C.c_int32, C.POINTER(SearchLimits), C.c_void_p, C.c_void_p]
         lib.nrtgpu_search_sorted.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32,
                                              C.c_int32, C.POINTER(Sort), C.POINTER(SearchLimits), C.c_void_p] + [C.c_void_p] * 7
-        lib.nrtgpu_search_bool_aggs.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32,
+        lib.nrtgpu_sort_order_create.argtypes = [C.c_void_p, C.POINTER(SortField), C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]
+        lib.nrtgpu_sort_order_device_bytes.argtypes = [C.c_void_p]
+        lib.nrtgpu_sort_order_device_bytes.restype = C.c_int64
+        lib.nrtgpu_sort_order_close.argtypes = [C.c_void_p]
+        lib.nrtgpu_search_sorted_fields.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32,
+                                                    C.c_int32, C.c_int32, C.c_void_p, C.POINTER(SearchLimits), C.c_void_p] + [C.c_void_p] * 7
+        lib.nrtgpu_search_bool_aggs.argtypes =[C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32,
                                                 C.POINTER(Aggregation), C.c_int32, C.POINTER(AggregationResult), C.c_void_p] + [C.c_void_p] * 4
         lib.nrtgpu_score_docs.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

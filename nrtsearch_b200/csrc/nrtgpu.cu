@@ -236,6 +236,17 @@ struct nrtgpu_index {
   }
 };
 
+// a Sort of several fields ranked over one image (sort_kernel.cuh, sort_order_build)
+struct nrtgpu_sort_order {
+  const nrtgpu_index* ix = nullptr;
+  int32_t n_fields = 0;
+  bool score_first = false; int32_t score_reverse = 0;
+  int32_t n_rank = 0;                   // fields of the rank: after the leading SCORE, up to the first DOCID inclusive
+  SortFieldDev f[kMaxSortFields] = {};  // every field of the Sort (device pointers into the image)
+  DevBuf<int32_t> perm;                 // position -> doc
+  DevBuf<uint32_t> rank;                // doc -> position + 1
+};
+
 struct nrtgpu_batch;
 static void free_batch(nrtgpu_batch* b);
 struct nrtgpu_batch {
@@ -269,6 +280,7 @@ struct nrtgpu_batch {
   DevBuf<int64_t> after_values; DevBuf<int32_t> after_docs; DevBuf<uint32_t> sort_missing_code;
   DevBuf<int64_t> out_sort_values;
   std::vector<int32_t> h_after_docs;
+  const nrtgpu_sort_order* order = nullptr;   // nrtgpu_search_sorted_fields: the Sort's order (sort_kind COLUMN or kSortScoreRank)
   // additional collectors (aggregations)
   std::vector<nrtgpu_aggregation> aggs;
   DevBuf<unsigned int> agg_counts[kMaxAggs];
@@ -704,9 +716,10 @@ int nrtgpu_index_update_stats(nrtgpu_index* ix, const int64_t* term_df, const in
 static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
                        const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold,
                        int32_t flags, cudaStream_t st, const nrtgpu_sort* sort = nullptr, const nrtgpu_aggregation* aggs = nullptr,
-                       int32_t n_aggs = 0) {
+                       int32_t n_aggs = 0, const nrtgpu_sort_order* sort_order = nullptr, const int64_t* order_after = nullptr) {
   if (!ix || !queries || (n_clauses > 0 && !clauses)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: NULL argument");
   b->aggs.clear();
+  b->order = sort_order;
   if (n_aggs > 0) {
     if (!aggs || n_aggs > kMaxAggs) NRT_FAIL(NRTGPU_ERR_INVALID, "at most 8 aggregations per search");
     if (ix && ix->ctx->engine_stream) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "aggregations need the probe engine");
@@ -725,14 +738,19 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
     }
     total_hits_threshold = INT32_MAX;   // RelevanceCollector.java:55-62: additional collectors force exact collection
   }
-  const bool sorted = sort && sort->kind != NRTGPU_SORT_RELEVANCE;
-  b->sort_kind = sorted ? sort->kind : 0; b->sort_column = sorted ? sort->column : 0; b->sort_reverse = sorted ? (sort->reverse != 0) : 0;
-  b->sort_missing_value = sorted ? sort->missing_value : 0;
+  const bool sorted = (sort && sort->kind != NRTGPU_SORT_RELEVANCE) || sort_order;
+  if (sort_order) {   // fields-only order: the COLUMN key with the rank as its code; [score, ...]: kSortScoreRank
+    b->sort_kind = sort_order->score_first ? kSortScoreRank : NRTGPU_SORT_COLUMN; b->sort_column = 0;
+    b->sort_reverse = sort_order->score_first ? sort_order->score_reverse : 0; b->sort_missing_value = 0;
+  } else {
+    b->sort_kind = sorted ? sort->kind : 0; b->sort_column = sorted ? sort->column : 0; b->sort_reverse = sorted ? (sort->reverse != 0) : 0;
+    b->sort_missing_value = sorted ? sort->missing_value : 0;
+  }
   if (sorted) {
-    if (sort->kind != NRTGPU_SORT_COLUMN && sort->kind != NRTGPU_SORT_DOCID) NRT_FAIL(NRTGPU_ERR_INVALID, "bad sort kind");
-    if (sort->kind == NRTGPU_SORT_COLUMN && (sort->column < 0 || sort->column >= ix->n_columns))
+    if (!sort_order && sort->kind != NRTGPU_SORT_COLUMN && sort->kind != NRTGPU_SORT_DOCID) NRT_FAIL(NRTGPU_ERR_INVALID, "bad sort kind");
+    if (!sort_order && sort->kind == NRTGPU_SORT_COLUMN && (sort->column < 0 || sort->column >= ix->n_columns))
       NRT_FAIL(NRTGPU_ERR_INVALID, "sort column out of range (field does not support sorting: no doc values)");
-    if (sort->kind == NRTGPU_SORT_COLUMN && ix->col_multi[(size_t)sort->column]) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "sort on a multi-valued column");
+    if (!sort_order && sort->kind == NRTGPU_SORT_COLUMN && ix->col_multi[(size_t)sort->column]) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "sort on a multi-valued column");
     if (ix->ctx->engine_stream) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "sorted search needs the probe engine");
     total_hits_threshold = INT32_MAX;   // every match is visited: exact totalHits
   }
@@ -1007,21 +1025,41 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
     bool any_after = false;
     b->h_after_docs.assign((size_t)nq, 0);
     for (int qi = 0; qi < nq; ++qi) if (queries[qi].has_after) { any_after = true; b->h_after_docs[(size_t)qi] = queries[qi].after_doc; }
-    if (any_after && sort->kind == NRTGPU_SORT_COLUMN && !sort->after_values) NRT_FAIL(NRTGPU_ERR_INVALID, "sorted searchAfter needs after_values");
-    if ((rc = b->sort_missing_code.alloc(1))) return rc;
-    if ((rc = b->after_docs.upload_async(b->h_after_docs.data(), (size_t)nq, st))) return rc;
-    if (sort->after_values) { if ((rc = b->after_values.upload_async(sort->after_values, (size_t)nq, st))) return rc; }
-    else if ((rc = b->after_values.alloc((size_t)nq))) return rc;
-    SortAfterLaunch A;
-    A.queries = b->queries.p; A.nq = nq; A.after_docs = b->after_docs.p; A.after_values = b->after_values.p;
-    A.kind = sort->kind; A.reverse = sort->reverse != 0; A.doc_base = ix->doc_base; A.n_docs = ix->n_docs;
-    const bool col = sort->kind == NRTGPU_SORT_COLUMN;
-    A.distinct = col ? ix->col_distinct[(size_t)sort->column]->p : nullptr;
-    A.n_distinct = col ? ix->col_n_distinct[(size_t)sort->column] : 0;
-    A.missing_value = sort->missing_value; A.missing_code = b->sort_missing_code.p;
-    sort_after_kernel<<<(unsigned)((nq + 127) / 128), 128, 0, st>>>(A);
-    NRT_CUDA_TRY(cudaGetLastError());
-    if ((rc = b->out_sort_values.alloc((size_t)nq * top_k))) return rc;
+    if (sort_order) {
+      if (any_after && !order_after) NRT_FAIL(NRTGPU_ERR_INVALID, "sorted searchAfter needs after_values");
+      // (the COLUMN key reads a missing code; ranks are never 0, so it is never used)
+      if ((rc = b->sort_missing_code.alloc(1))) return rc;
+      NRT_CUDA_TRY(cudaMemsetAsync(b->sort_missing_code.p, 0, sizeof(uint32_t), st));
+      if ((rc = b->after_docs.upload_async(b->h_after_docs.data(), (size_t)nq, st))) return rc;
+      const size_t nv = (size_t)nq * sort_order->n_fields;
+      if (order_after) { if ((rc = b->after_values.upload_async(order_after, nv, st))) return rc; }
+      else if ((rc = b->after_values.alloc(nv))) return rc;
+      SortFieldsAfterLaunch A{};
+      A.queries = b->queries.p; A.nq = nq; A.after_docs = b->after_docs.p; A.after_values = b->after_values.p;
+      A.n_fields = sort_order->n_fields; A.score_first = sort_order->score_first ? 1 : 0; A.score_reverse = sort_order->score_reverse;
+      A.n_rank = sort_order->n_rank;
+      for (int i = 0; i < sort_order->n_rank; ++i) A.f[i] = sort_order->f[i + A.score_first];
+      A.perm = sort_order->perm.p; A.n_docs = ix->n_docs; A.doc_base = ix->doc_base;
+      if (any_after) sort_fields_after_kernel<<<(unsigned)((nq + 127) / 128), 128, 0, st>>>(A);
+      NRT_CUDA_TRY(cudaGetLastError());
+      if ((rc = b->out_sort_values.alloc(nv * top_k))) return rc;
+    } else {
+      if (any_after && sort->kind == NRTGPU_SORT_COLUMN && !sort->after_values) NRT_FAIL(NRTGPU_ERR_INVALID, "sorted searchAfter needs after_values");
+      if ((rc = b->sort_missing_code.alloc(1))) return rc;
+      if ((rc = b->after_docs.upload_async(b->h_after_docs.data(), (size_t)nq, st))) return rc;
+      if (sort->after_values) { if ((rc = b->after_values.upload_async(sort->after_values, (size_t)nq, st))) return rc; }
+      else if ((rc = b->after_values.alloc((size_t)nq))) return rc;
+      SortAfterLaunch A;
+      A.queries = b->queries.p; A.nq = nq; A.after_docs = b->after_docs.p; A.after_values = b->after_values.p;
+      A.kind = sort->kind; A.reverse = sort->reverse != 0; A.doc_base = ix->doc_base; A.n_docs = ix->n_docs;
+      const bool col = sort->kind == NRTGPU_SORT_COLUMN;
+      A.distinct = col ? ix->col_distinct[(size_t)sort->column]->p : nullptr;
+      A.n_distinct = col ? ix->col_n_distinct[(size_t)sort->column] : 0;
+      A.missing_value = sort->missing_value; A.missing_code = b->sort_missing_code.p;
+      sort_after_kernel<<<(unsigned)((nq + 127) / 128), 128, 0, st>>>(A);
+      NRT_CUDA_TRY(cudaGetLastError());
+      if ((rc = b->out_sort_values.alloc((size_t)nq * top_k))) return rc;
+    }
   }
   if ((rc = b->theta.alloc((size_t)nq))) return rc;
   if ((rc = b->total_hits.alloc((size_t)nq))) return rc;
@@ -1128,7 +1166,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         P.deadline_ns = L.deadline_ns; P.clock0 = L.clock0; P.timed_out = L.timed_out;
         P.terminate_after = b->ta_scalar; P.terminated = b->terminated.p;
         P.sort_kind = b->sort_kind; P.sort_reverse = b->sort_reverse;
-        P.sort_codes = b->sort_kind == NRTGPU_SORT_COLUMN ? b->ix->col_code[(size_t)b->sort_column]->p : nullptr;
+        P.sort_codes = b->order ? b->order->rank.p : b->sort_kind == NRTGPU_SORT_COLUMN ? b->ix->col_code[(size_t)b->sort_column]->p : nullptr;
         P.sort_missing_code = b->sort_missing_code.p;
         P.aggs = nullptr;
         if (!b->aggs.empty()) {
@@ -1249,7 +1287,17 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   M.known_hits = (b->use_probe && !b->ix->live_bits.p) ? b->known_hits.p : nullptr;
   merge_slices_kernel<<<b->nq, kMergeThreads, 0, st>>>(M);
   NRT_CUDA_TRY(cudaGetLastError());
-  if (b->sort_kind != NRTGPU_SORT_RELEVANCE) {   // FieldDoc values of the final hits; scores become NaN
+  if (b->order) {   // FieldDoc values of every field; score-first orders map ranks back to docs
+    const nrtgpu_sort_order* o = b->order;
+    SortFieldsValuesLaunch V{};
+    V.docs = b->o_docs(); V.counts = b->o_counts(); V.nq = b->nq; V.top_k = b->top_k; V.doc_base = b->ix->doc_base;
+    V.n_fields = o->n_fields; V.score_first = o->score_first ? 1 : 0; V.score_reverse = o->score_reverse;
+    for (int i = 0; i < o->n_fields; ++i) V.f[i] = o->f[i];
+    V.perm = o->perm.p; V.scores = b->o_scores(); V.out_values = b->out_sort_values.p;
+    const int n = b->nq * b->top_k;
+    sort_fields_values_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(V);
+    NRT_CUDA_TRY(cudaGetLastError());
+  } else if (b->sort_kind != NRTGPU_SORT_RELEVANCE) {   // FieldDoc values of the final hits; scores become NaN
     SortValuesLaunch V;
     V.docs = b->o_docs(); V.counts = b->o_counts(); V.nq = b->nq; V.top_k = b->top_k; V.doc_base = b->ix->doc_base; V.kind = b->sort_kind;
     const bool col = b->sort_kind == NRTGPU_SORT_COLUMN;
@@ -1480,7 +1528,8 @@ static int search_bool_impl(nrtgpu_index* ix, const nrtgpu_clause* clauses, int3
                             const nrtgpu_search_limits* limits, void* stream, int32_t* d_record, int32_t* out_docs, float* out_scores,
                             int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
                             uint8_t* out_terminated_early, const nrtgpu_sort* sort = nullptr, int64_t* out_sort_values = nullptr,
-                            const nrtgpu_aggregation* aggs = nullptr, int32_t n_aggs = 0, const nrtgpu_aggregation_result* agg_out = nullptr) {
+                            const nrtgpu_aggregation* aggs = nullptr, int32_t n_aggs = 0, const nrtgpu_aggregation_result* agg_out = nullptr,
+                            const nrtgpu_sort_order* order = nullptr, const int64_t* order_after = nullptr) {
   if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool: NULL index");
   // take a cached workspace (device buffers survive between calls: no cudaMalloc on the request path)
   nrtgpu_batch* b = nullptr;
@@ -1490,7 +1539,8 @@ static int search_bool_impl(nrtgpu_index* ix, const nrtgpu_clause* clauses, int3
   }
   if (!b) b = new nrtgpu_batch;
   b->bound_docs = nullptr; b->bound_scores = nullptr; b->bound_counts = nullptr; b->bound_total = nullptr; b->bound_flags = nullptr;
-  int rc = batch_build(b, ix, clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags, (cudaStream_t)stream, sort, aggs, n_aggs);
+  int rc = batch_build(b, ix, clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags, (cudaStream_t)stream, sort, aggs, n_aggs,
+                       order, order_after);
   if (!rc) rc = batch_set_limits(b, limits, (cudaStream_t)stream);
   if (!rc && d_record) rc = nrtgpu_batch_bind_packed(b, d_record);
   if (!rc) rc = nrtgpu_batch_run(b, stream);
@@ -1498,7 +1548,8 @@ static int search_bool_impl(nrtgpu_index* ix, const nrtgpu_clause* clauses, int3
     if (d_record) { cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream); if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); rc = NRTGPU_ERR_CUDA; } }
     else {
       if (out_sort_values && b->sort_kind != NRTGPU_SORT_RELEVANCE) {
-        cudaError_t e = cudaMemcpyAsync(out_sort_values, b->out_sort_values.p, (size_t)nq * top_k * sizeof(int64_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
+        const size_t nv = (size_t)nq * top_k * (order ? order->n_fields : 1);
+        cudaError_t e = cudaMemcpyAsync(out_sort_values, b->out_sort_values.p, nv * sizeof(int64_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
         if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); rc = NRTGPU_ERR_CUDA; }
       }
       if (!rc) rc = batch_fetch_impl(b, stream, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
@@ -1541,6 +1592,71 @@ int nrtgpu_search_sorted(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
   return search_bool_impl(ix, clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags, limits, stream, nullptr,
                           out_docs, nullptr, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early,
                           sort, out_sort_values);
+}
+
+int nrtgpu_sort_order_create(nrtgpu_index* ix, const nrtgpu_sort_field* fields, int32_t n_fields, void* stream, nrtgpu_sort_order** out) {
+  if (!ix || !fields || !out) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_sort_order_create: NULL argument");
+  if (n_fields < 1) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_sort_order_create: a Sort needs at least one field");
+  if (n_fields > kMaxSortFields) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nrtgpu_sort_order_create: more than 8 sort fields is not on the GPU path");
+  std::unique_ptr<nrtgpu_sort_order> o(new nrtgpu_sort_order);
+  o->ix = ix; o->n_fields = n_fields;
+  for (int i = 0; i < n_fields; ++i) {
+    const nrtgpu_sort_field& s = fields[i];
+    SortFieldDev& f = o->f[i];
+    f.kind = s.kind; f.reverse = s.reverse != 0; f.selector = s.selector; f.missing = s.missing_value;
+    if (s.kind == NRTGPU_SORT_COLUMN) {
+      if (s.column < 0 || s.column >= ix->n_columns) NRT_FAIL(NRTGPU_ERR_INVALID, "sort column out of range (field does not support sorting: no doc values)");
+      if (s.selector != NRTGPU_SELECT_MIN && s.selector != NRTGPU_SELECT_MAX) NRT_FAIL(NRTGPU_ERR_INVALID, "bad sort selector");
+      const size_t c = (size_t)s.column;
+      if (ix->col_multi[c]) { f.mv_off = ix->colmv_off[c]->p; f.c64 = ix->col64[c]->p; }
+      else {
+        f.c64 = ix->col64[c]->p; f.c32 = ix->col32[c]->p; f.has = ix->col_has[c]->p;
+        f.codes = ix->col_code[c]->p; f.distinct = ix->col_distinct[c]->p; f.n_distinct = ix->col_n_distinct[c];
+      }
+    } else if (s.kind == NRTGPU_SORT_SCORE) {
+      if (i > 0) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "a SCORE sort field is on the GPU path only in first position");
+      o->score_first = true; o->score_reverse = s.reverse != 0;
+    } else if (s.kind != NRTGPU_SORT_DOCID) NRT_FAIL(NRTGPU_ERR_INVALID, "bad sort field kind");
+  }
+  const int r0 = o->score_first ? 1 : 0;
+  int r1 = n_fields;   // the fields after the first DOCID cannot decide anything
+  for (int i = r0; i < n_fields; ++i) if (fields[i].kind == NRTGPU_SORT_DOCID) { r1 = i + 1; break; }
+  o->n_rank = r1 - r0;
+  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
+  const int32_t n = ix->n_docs;
+  int rc;
+  if ((rc = o->perm.alloc((size_t)std::max(n, 1))) || (rc = o->rank.alloc((size_t)std::max(n, 1)))) return rc;
+  o->perm.n = (size_t)n; o->rank.n = (size_t)n;
+  {
+    DevBuf<uint32_t> k32; DevBuf<uint64_t> k64;
+    if ((rc = k32.alloc((size_t)std::max(n, 1))) || (rc = k64.alloc((size_t)std::max(n, 1)))) return rc;
+    if ((rc = sort_order_build(o->f + r0, o->n_rank, n, ix->doc_base, (cudaStream_t)stream, o->perm.p, o->rank.p,
+                               k32.p, k64.p))) return rc;
+    NRT_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)stream));   // the scratch is freed on return
+  }
+  *out = o.release();
+  return NRTGPU_OK;
+}
+
+int64_t nrtgpu_sort_order_device_bytes(const nrtgpu_sort_order* o) { return o ? (int64_t)(o->perm.bytes() + o->rank.bytes()) : 0; }
+
+int nrtgpu_sort_order_close(nrtgpu_sort_order* o) {
+  if (!o) return NRTGPU_OK;
+  cudaSetDevice(o->ix->ctx->device);
+  delete o;
+  return NRTGPU_OK;
+}
+
+int nrtgpu_search_sorted_fields(nrtgpu_index* ix, const nrtgpu_sort_order* order, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags, const int64_t* after_values,
+                                const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs, int64_t* out_sort_values,
+                                int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
+                                uint8_t* out_terminated_early) {
+  if (!ix || !order) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_sorted_fields: NULL argument");
+  if (order->ix != ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_sorted_fields: the sort order was made on another index");
+  return search_bool_impl(ix, clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags, limits, stream, nullptr,
+                          out_docs, nullptr, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early,
+                          nullptr, out_sort_values, nullptr, 0, nullptr, order, after_values);
 }
 
 int nrtgpu_search_bool_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,

@@ -107,7 +107,7 @@ struct ProbeLaunch {
   // sort-by-field (generic instantiation): the key of a hit is (order-preserving code of its sort value, ~doc) instead
   // of (score, ~doc); see sort_kernel.cuh
   int32_t sort_kind, sort_reverse;
-  const uint32_t* sort_codes;    // [n_docs] codes of the sort column (0 = doc without a value)
+  const uint32_t* sort_codes;    // [n_docs] codes of the sort column (0 = doc without a value), or the 1-based ranks of a sort order
   const uint32_t* sort_missing_code;   // [1] code of the sort's missing value
   const AggLaunch* aggs;         // additional collectors (generic instantiation; device pointer, NULL: none)
   const unsigned long long* known_hits;   // optional [nq]: docs KNOWN to match (the longest list of a pure disjunction on a shard without
@@ -756,8 +756,11 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
           ++my_hits;
           if (L.aggs) agg_collect(*L.aggs, L.ix, qi, d);   // additional collectors see every matching doc
           uint64_t entry;
-          if (L.sort_kind == NRTGPU_SORT_RELEVANCE) entry = make_key(score, d);
-          else {   // TopFieldCollector: the key is the doc's sort value (order-preserving code), ties by doc id
+          if (L.sort_kind == NRTGPU_SORT_RELEVANCE || L.sort_kind == kSortScoreRank) {
+            entry = make_key(score, d);
+            // [score, ...] order: ties by the order's rank, which takes the doc's place; ordered(-s) == ~ordered(s) for reverse
+            if (L.sort_kind == kSortScoreRank) entry = make_key(L.sort_reverse ? -score : score, (int32_t)__ldg(L.sort_codes + d));
+          } else {   // TopFieldCollector: the key is the doc's sort value (order-preserving code), ties by doc id
             uint32_t code = 0;
             if (L.sort_kind == NRTGPU_SORT_COLUMN) { code = __ldg(L.sort_codes + d); if (code == 0u) code = sort_missing; }
             entry = ((uint64_t)sort_hi(L.sort_kind, L.sort_reverse, code, d) << 32) | (uint32_t)(~(uint32_t)d);

@@ -16,6 +16,7 @@
 #include <thrust/scan.h>
 #include <thrust/sequence.h>
 #include <thrust/sort.h>
+#include <thrust/system/cuda/execution_policy.h>
 #include "bool_kernel.cuh"
 
 namespace nrtgpu {
@@ -130,6 +131,156 @@ inline int sort_codes_build(const int64_t* c64, const int32_t* c32, const uint8_
   NRT_CUDA_TRY(cudaMemcpy(&last, rank_tmp + n_has - 1, sizeof(int32_t), cudaMemcpyDeviceToHost));
   *n_distinct_out = last;
   return NRTGPU_OK;
+}
+
+// ---- sort orders of several fields (nrtgpu_sort_order; Lucene Sort of 1..8 SortFields, TopFieldCollector) ----
+// An order ranks every doc of the leaf once: perm (position -> doc) and rank (doc -> position + 1) under the fields that
+// follow a leading SCORE, up to and including the first DOCID (fields after a DOCID cannot decide anything), then doc id
+// asc. The posting kernel keys a hit by its rank: hi = ~rank, lo = ~doc (the COLUMN key with the rank as its code), or,
+// for [score, ...], hi = the ordered score, lo = ~rank (kSortScoreRank; the merge decodes the rank as the "doc", and
+// sort_fields_values_kernel maps it back through perm). A score, a tie code and a doc would not fit 64 bits together;
+// the rank holds the doc tie-break, which is why SCORE must lead.
+constexpr int32_t kSortScoreRank = 4;   // internal sort kind of the posting kernels (beside NRTGPU_SORT_COLUMN / _DOCID)
+constexpr int kMaxSortFields = 8;
+
+struct SortFieldDev {
+  int32_t kind, reverse, selector, n_distinct;
+  int64_t missing;
+  const int64_t* c64; const int32_t* c32; const uint8_t* has;
+  const int64_t* mv_off;       // multi-valued column: per-doc offsets into c64 (values ascending within a doc)
+  const uint32_t* codes;       // single-valued column: order-preserving codes (0 = no value), with its distinct values
+  const uint64_t* distinct;
+};
+
+// the doc's value of one field: the column value (MIN / MAX selected on a multi-valued column) or missing; the global doc id
+__device__ __forceinline__ int64_t sort_field_value(const SortFieldDev& f, int32_t d, int32_t doc_base) {
+  if (f.kind == NRTGPU_SORT_DOCID) return (int64_t)d + doc_base;
+  if (f.mv_off) {
+    const int64_t a = f.mv_off[d], b = f.mv_off[d + 1];
+    return a == b ? f.missing : f.c64[f.selector == NRTGPU_SELECT_MAX ? b - 1 : a];
+  }
+  if (f.has && !f.has[d]) return f.missing;
+  return f.c32 ? (int64_t)f.c32[d] : f.c64[d];
+}
+// ascending key of a value under the field's direction
+__device__ __forceinline__ uint64_t sort_field_key(const SortFieldDev& f, int64_t v) { return sortable_u64(v) ^ (f.reverse ? ~0ull : 0ull); }
+
+// LSD pass keys, in the current perm order: 32-bit codes for single-valued columns, 64-bit keys otherwise
+__global__ void sort_order_keys32_kernel(SortFieldDev f, const int32_t* __restrict__ perm, int32_t n, uint32_t* __restrict__ keys) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint32_t c = f.codes[perm[i]];
+  if (c == 0u) c = sort_code_of(f.distinct, f.n_distinct, f.missing);
+  keys[i] = f.reverse ? ~c : c;
+}
+__global__ void sort_order_keys64_kernel(SortFieldDev f, const int32_t* __restrict__ perm, int32_t n, int32_t doc_base,
+                                         uint64_t* __restrict__ keys) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  keys[i] = sort_field_key(f, sort_field_value(f, perm[i], doc_base));
+}
+__global__ void sort_order_init_kernel(int32_t n, int32_t descending, int32_t* __restrict__ perm) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) perm[i] = descending ? n - 1 - i : i;
+}
+__global__ void sort_order_rank_kernel(const int32_t* __restrict__ perm, int32_t n, uint32_t* __restrict__ rank) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) rank[perm[i]] = (uint32_t)i + 1u;
+}
+
+// perm / rank of the fields f[0..n_f) (device pointers; scratch: n keys of each width). Stable LSD sorts on `st`, from the
+// last field to the first, starting from doc order (a trailing DOCID sets the start order instead of a pass).
+inline int sort_order_build(const SortFieldDev* f, int n_f, int32_t n, int32_t doc_base, cudaStream_t st, int32_t* perm,
+                            uint32_t* rank, uint32_t* keys32, uint64_t* keys64) {
+  if (n <= 0) return NRTGPU_OK;
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  const bool docid_last = n_f > 0 && f[n_f - 1].kind == NRTGPU_SORT_DOCID;
+  sort_order_init_kernel<<<grid, 256, 0, st>>>(n, docid_last && f[n_f - 1].reverse, perm);
+  NRT_CUDA_TRY(cudaGetLastError());
+  for (int i = n_f - (docid_last ? 2 : 1); i >= 0; --i) {
+    if (f[i].codes) {
+      sort_order_keys32_kernel<<<grid, 256, 0, st>>>(f[i], perm, n, keys32);
+      NRT_CUDA_TRY(cudaGetLastError());
+      thrust::stable_sort_by_key(thrust::cuda::par.on(st), keys32, keys32 + n, perm);
+    } else {
+      sort_order_keys64_kernel<<<grid, 256, 0, st>>>(f[i], perm, n, doc_base, keys64);
+      NRT_CUDA_TRY(cudaGetLastError());
+      thrust::stable_sort_by_key(thrust::cuda::par.on(st), keys64, keys64 + n, perm);
+    }
+  }
+  sort_order_rank_kernel<<<grid, 256, 0, st>>>(perm, n, rank);
+  NRT_CUDA_TRY(cudaGetLastError());
+  return NRTGPU_OK;
+}
+
+struct SortFieldsAfterLaunch {
+  DevQuery* queries; int32_t nq;
+  const int32_t* after_docs;      // [nq] global doc ids
+  const int64_t* after_values;    // [nq][n_fields]
+  int32_t n_fields;               // row length of after_values
+  int32_t score_first, score_reverse;
+  int32_t n_rank;                 // fields of the rank: f[0..n_rank) = after_values columns score_first .. score_first + n_rank
+  SortFieldDev f[kMaxSortFields];
+  const int32_t* perm; int32_t n_docs, doc_base;
+};
+
+// patches DevQuery::after_key (a hit qualifies iff key < after_key, PagingFieldCollector): pos = the docs of the leaf whose
+// (rank fields, global doc) tuple is <= (after values, after_doc), found by a binary search of perm; a doc qualifies on the
+// rank iff its rank (1-based) > pos. After values need not be held by any doc; after_doc may lie outside the leaf.
+__global__ void sort_fields_after_kernel(SortFieldsAfterLaunch S) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= S.nq || !S.queries[q].has_after) return;
+  const int64_t* av = S.after_values + (size_t)q * S.n_fields;
+  const int64_t after_doc = S.after_docs[q];
+  int lo = 0, hi = S.n_docs;   // first position whose tuple is > the after tuple
+  while (lo < hi) {
+    const int m = (lo + hi) >> 1;
+    const int32_t d = S.perm[m];
+    int c = 0;
+    for (int i = 0; i < S.n_rank && c == 0; ++i) {
+      const uint64_t kd = sort_field_key(S.f[i], sort_field_value(S.f[i], d, S.doc_base));
+      const uint64_t ka = sort_field_key(S.f[i], av[S.score_first + i]);
+      c = kd < ka ? -1 : (kd > ka ? 1 : 0);
+    }
+    if (c == 0) c = (int64_t)d + S.doc_base <= after_doc ? -1 : 1;
+    if (c < 0) lo = m + 1; else hi = m;
+  }
+  const uint32_t pos = (uint32_t)lo;
+  uint64_t key;
+  if (S.score_first) {
+    const uint32_t s = float_to_ordered(__uint_as_float((uint32_t)av[0])) ^ (S.score_reverse ? ~0u : 0u);
+    key = ((uint64_t)s << 32) | (uint32_t)~pos;
+  } else {
+    key = (uint64_t)(uint32_t)~pos << 32;
+  }
+  S.queries[q].after_key = key;
+}
+
+// FieldDoc.fields of the final hits ([nq][top_k][n_fields]); score-first orders: the merged "doc" is a rank, mapped back
+// to the doc through perm, and the score is recovered from the key's score word
+struct SortFieldsValuesLaunch {
+  int32_t* docs; const int32_t* counts; int32_t nq, top_k, doc_base, n_fields, score_first, score_reverse;
+  SortFieldDev f[kMaxSortFields];   // every field of the sort (a SCORE entry takes the hit's score)
+  const int32_t* perm;
+  float* scores; int64_t* out_values;
+};
+__global__ void sort_fields_values_kernel(SortFieldsValuesLaunch S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= S.nq * S.top_k) return;
+  const int q = i / S.top_k, r = i % S.top_k;
+  int64_t* out = S.out_values + (size_t)i * S.n_fields;
+  const float key_score = S.scores[i];
+  S.scores[i] = __int_as_float(0x7fc00000);   // NaN: TopFieldCollector does not track scores
+  if (r >= S.counts[q]) { for (int j = 0; j < S.n_fields; ++j) out[j] = 0; return; }
+  int32_t d = S.docs[i] - S.doc_base;
+  float score = 0.0f;
+  if (S.score_first) {
+    d = S.perm[d - 1];
+    S.docs[i] = d + S.doc_base;
+    score = S.score_reverse ? ordered_to_float(~float_to_ordered(key_score)) : key_score;
+  }
+  for (int j = 0; j < S.n_fields; ++j)
+    out[j] = S.f[j].kind == NRTGPU_SORT_SCORE ? (int64_t)__float_as_uint(score) : sort_field_value(S.f[j], d, S.doc_base);
 }
 
 }  // namespace nrtgpu

@@ -151,16 +151,20 @@ def double_to_sortable_long(d: float) -> int:
 
 @dataclass(frozen=True)
 class SortType:
-    """SortType of the search request for ONE sort field (SortParser.parseSort :54-95): a numeric doc-value column, or
-    "docid". field_type picks the missing value exactly as the reference's FieldDefs do (IntFieldDef.java:103,
-    LongFieldDef.java:103, FloatFieldDef.java:105, DoubleFieldDef.java:105): MAX / +Infinity when missing_last, else
-    MIN / -Infinity -- irrespective of reverse."""
-    field: object            # column id, or "docid"
+    """SortType of the search request for ONE sort field (SortParser.parseSort :54-95): a numeric doc-value column,
+    "docid" or "score" (higher scores first unless reverse). field_type picks the missing value exactly as the reference's
+    FieldDefs do (IntFieldDef.java:103, LongFieldDef.java:103, FloatFieldDef.java:105, DoubleFieldDef.java:105): MAX /
+    +Infinity when missing_last, else MIN / -Infinity -- irrespective of reverse. selector: which value of a multi-valued
+    column sorts the doc, "min" (the default) or "max" (NumberFieldDef.java:266-278, SortedNumericSelector)."""
+    field: object            # column id, "docid" or "score"
     reverse: bool = False
     missing_last: bool = False
     field_type: str = "long"   # int | long | float | double
+    selector: str = "min"
 
     def missing_value(self) -> int:
+        if self.field in ("docid", "score"):
+            return 0
         hi = self.missing_last
         if self.field_type == "int":
             return 2**31 - 1 if hi else -(2**31)
@@ -172,12 +176,20 @@ class SortType:
             return double_to_sortable_long(float("inf") if hi else float("-inf"))
         raise ValueError(f"field type {self.field_type} does not support sorting")
 
+    def c_field(self) -> _native.SortField:
+        if self.selector not in ("min", "max"):
+            raise ValueError(f"selector must be 'min' or 'max', not {self.selector!r}")
+        kind = 3 if self.field == "score" else 2 if self.field == "docid" else 1
+        return _native.SortField(kind, int(self.field) if kind == 1 else 0, 1 if self.reverse else 0,
+                                 1 if self.selector == "max" else 0, self.missing_value())
+
 
 @dataclass
 class SortFieldCollector:
-    """SortFieldCollector.java:44-105: numHitsToCollect + the query's Sort; searchAfter is a FieldDoc (value, doc)."""
+    """SortFieldCollector.java:44-105: numHitsToCollect + the query's Sort (one SortType, or a sequence of up to 8);
+    searchAfter is a FieldDoc (value, doc), or (values, doc) for a sequence."""
     num_hits_to_collect: int
-    sort: SortType = None
+    sort: object = None
     timeout_sec: float = 0.0
     terminate_after: int = 0
 
@@ -216,16 +228,19 @@ _VALUE_TYPE = {"int": 0, "long": 0, "float": 1, "double": 2}
 @dataclass
 class FieldDoc:
     doc: int
-    value: int   # fields[0], sortable-long domain
+    value: int = 0   # fields[0], sortable-long domain
+    values: Optional[Tuple[int, ...]] = None   # every field of a multi-field Sort (a row of SortedResult.sort_values)
 
 
 @dataclass
 class SortedResult:
     docs: np.ndarray          # int32 [nq, k]
-    sort_values: np.ndarray   # int64 [nq, k] FieldDoc.fields[0] of every hit
+    sort_values: np.ndarray   # int64 [nq, k] FieldDoc.fields[0] of every hit; [nq, k, n_fields] for a sequence of SortTypes
     counts: np.ndarray
     total_hits: np.ndarray
     relation: np.ndarray
+    hit_timeout: Optional[np.ndarray] = None        # uint8 [nq] (multi-field path)
+    terminated_early: Optional[np.ndarray] = None   # uint8 [nq] (multi-field path)
 
 
 def _f32(x: float) -> np.float32:
@@ -333,6 +348,19 @@ class GpuIndex:
         check(self._lib.nrtgpu_index_build(ctx.handle, C.byref(pinned.desc), C.byref(h)))
         self.handle = h
         self.n_docs, self.doc_base = shard.n_docs, shard.doc_base
+        self._orders = {}
+
+    def sort_order(self, fields: Sequence[SortType], stream: int = 0) -> C.c_void_p:
+        """The nrtgpu_sort_order of a Sort, built on first use and kept until close(): it depends on the columns only, so
+        deletes and statistics refreshes leave it valid."""
+        cf = [f.c_field() for f in fields]
+        key = tuple((f.kind, f.column, f.reverse, f.selector, f.missing_value) for f in cf)
+        if key not in self._orders:
+            arr = (_native.SortField * max(len(cf), 1))(*cf)
+            h = C.c_void_p()
+            check(self._lib.nrtgpu_sort_order_create(self.handle, arr, len(cf), C.c_void_p(stream), C.byref(h)))
+            self._orders[key] = h
+        return self._orders[key]
 
     def set_live_docs(self, live_docs: Optional[np.ndarray]):
         """Deletes of a new reader version (LeafReader.getLiveDocs): refreshed in place, no image rebuild."""
@@ -352,6 +380,9 @@ class GpuIndex:
 
     def close(self):
         if self.handle:
+            for h in self._orders.values():
+                self._lib.nrtgpu_sort_order_close(h)
+            self._orders.clear()
             self._lib.nrtgpu_index_close(self.handle)
             self.handle = None
 
@@ -479,6 +510,8 @@ class GpuIndexSearcher:
                       search_after: Optional[Sequence[Optional[FieldDoc]]] = None, stream: int = 0) -> SortedResult:
         """IndexSearcher.search(query, TopFieldCollectorManager(sort, numHits, after, threshold)) for a batch."""
         st = collector.sort
+        if not isinstance(st, SortType) or st.field == "score":
+            return self._search_sorted_fields(queries, collector, [st] if isinstance(st, SortType) else list(st), search_after, stream)
         after_sd = None if search_after is None else [None if a is None else ScoreDoc(a.doc, 0.0) for a in search_after]
         carr, ncl, qarr, nq = compile_queries(queries, after_sd)
         k = collector.num_hits_to_collect
@@ -496,6 +529,32 @@ class GpuIndexSearcher:
         check(self._lib.nrtgpu_search_sorted(self.index.handle, carr, ncl, qarr, nq, k, 0, C.byref(cs), None if lim is None else C.byref(lim),
                                              C.c_void_p(stream), out.docs.ctypes.data, out.sort_values.ctypes.data, out.counts.ctypes.data,
                                              out.total_hits.ctypes.data, out.relation.ctypes.data, None, None))
+        return out
+
+    def _search_sorted_fields(self, queries, collector: SortFieldCollector, fields: List[SortType],
+                              search_after: Optional[Sequence[Optional[FieldDoc]]], stream: int) -> SortedResult:
+        """A Sort of several fields (nrtgpu_search_sorted_fields) through the index's cached order of that Sort."""
+        order = self.index.sort_order(fields, stream)
+        nf = len(fields)
+        after_sd = None if search_after is None else [None if a is None else ScoreDoc(a.doc, 0.0) for a in search_after]
+        carr, ncl, qarr, nq = compile_queries(queries, after_sd)
+        k = collector.num_hits_to_collect
+        out = SortedResult(np.zeros((nq, k), np.int32), np.zeros((nq, k, nf), np.int64), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
+                           np.zeros(nq, np.uint8), np.zeros(nq, np.uint8), np.zeros(nq, np.uint8))
+        av = None
+        if search_after is not None:
+            av = np.zeros((nq, nf), np.int64)
+            for i, a in enumerate(search_after):
+                if a is not None:
+                    av[i] = a.values if a.values is not None else (a.value,)
+        lim = None
+        if collector.timeout_sec > 0 or collector.terminate_after > 0:
+            lim = SearchLimits(collector.timeout_sec, 0.0, 0, collector.terminate_after, 0)
+        check(self._lib.nrtgpu_search_sorted_fields(self.index.handle, order, carr, ncl, qarr, nq, k, 0,
+                                                    None if av is None else av.ctypes.data, None if lim is None else C.byref(lim),
+                                                    C.c_void_p(stream), out.docs.ctypes.data, out.sort_values.ctypes.data,
+                                                    out.counts.ctypes.data, out.total_hits.ctypes.data, out.relation.ctypes.data,
+                                                    out.hit_timeout.ctypes.data, out.terminated_early.ctypes.data))
         return out
 
     def search_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
