@@ -26,7 +26,7 @@
 namespace nrtgpu {
 
 constexpr int kMaxClauses = 16;     // clauses per flat BooleanQuery on the GPU path
-constexpr int kMaxTermSlots = 8;    // term clauses per query (u32 words: 4, u64 words: 8)
+constexpr int kMaxTermSlots = 8;    // term clauses per query: one tf byte each in the window kernel's 64-bit words
 constexpr int kWindowDocs = 16384;  // W
 constexpr int kSliceWindows = 64;   // windows per work item  => 1,048,576 docs per slice
 constexpr int kCandCap = 4096;      // candidate buffer (keys) per CTA, power of two
@@ -87,7 +87,7 @@ struct DevIndexView {
   const int64_t* const* colmv_off;  // [n_columns] multi-valued columns (SORTED_NUMERIC): doc d holds colmv_val[c][off[d] .. off[d + 1]),
   const int64_t* const* colmv_val;  //              ascending; NULL entry = single-valued column
   const uint32_t* live_bits;     // bitmap or NULL
-  const uint32_t* gran_tab;      // [n_rows][n_gran + 1] postings of the term below each stream-kernel granule (skip data)
+  const uint32_t* gran_tab;      // [n_rows][n_gran + 1] postings of the term below each 1024-doc granule boundary (skip data)
   int32_t n_gran;
   const uint8_t* dense_tf;       // [n_planes][dense_stride] min(freq, 255) per doc for the densest terms (0 = absent)
   int64_t dense_stride;
@@ -131,14 +131,8 @@ __device__ __forceinline__ bool range_matches(const DevIndexView& ix, int col, i
   return x >= lo && x <= hi;
 }
 
-template <typename SlotT>
-struct SlotTraits;
-template <> struct SlotTraits<uint32_t> { static constexpr int kSlots = 4; };
-template <> struct SlotTraits<uint64_t> { static constexpr int kSlots = 8; };
-
-template <typename SlotT>
 struct BoolSmem {
-  SlotT slots[kWindowDocs];
+  uint64_t slots[kWindowDocs];   // one tf byte per term slot
   uint64_t cand[kCandCap];
   uint32_t bounds[kMaxTermSlots][kSliceWindows + 1];
   float cache[kMaxTermSlots][256];
@@ -149,16 +143,19 @@ struct BoolSmem {
   unsigned long long theta;
 };
 
-template <typename SlotT>
-__device__ __forceinline__ uint32_t presence_mask(SlotT s) {
+// bit s set: byte s (term slot s) of a window word is non-zero
+__device__ __forceinline__ uint32_t presence_mask(uint64_t s) {
   uint32_t m = 0;
 #pragma unroll
-  for (int i = 0; i < SlotTraits<SlotT>::kSlots; ++i) m |= (((s >> (8 * i)) & 0xff) != 0 ? 1u : 0u) << i;
+  for (int i = 0; i < kMaxTermSlots; ++i) m |= (((s >> (8 * i)) & 0xff) != 0 ? 1u : 0u) << i;
   return m;
 }
 
-// exact tf of posting (clause c, doc) when the byte saturated: find the posting, then the exception list
-template <typename SlotT>
+// exact tf of posting (clause c, doc) when the byte saturated: find the posting, then the exception list.
+// Word is the tf word of the calling engine: uint64_t for the window kernel, uint32_t for the probe and collect kernels.
+// It only gives each engine its own out-of-line copy: one copy shared with the probe kernels costs the window kernel a
+// spilled register (8 more stack bytes, 4 bytes of spill stores and loads in ptxas -v).
+template <typename Word>
 __device__ __noinline__ float exact_freq_slow(const DevIndexView& ix, const DevClause& c, int32_t doc) {
   const int32_t* docs = ix.post_docs + c.post_base;
   int lo = 0, hi = c.n_post;
@@ -173,11 +170,10 @@ __device__ __noinline__ float exact_freq_slow(const DevIndexView& ix, const DevC
 // Evaluate the boolean constraints + score for one candidate doc. Returns false if the doc does not match.
 // Score combination follows Lucene's BooleanScorerSupplier: conjunction / disjunction sums are double,
 // required+optional is ReqOptSumScorer's float add (msm == 0) or ConjunctionScorer's double add (msm > 0).
-template <typename SlotT>
-__device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolSmem<SlotT>& sm, int32_t doc,
-                                             SlotT slot, float* out_score) {
+__device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolSmem& sm, int32_t doc,
+                                             uint64_t slot, float* out_score) {
   const DevQuery& q = sm.q;
-  uint32_t m = presence_mask<SlotT>(slot);
+  uint32_t m = presence_mask(slot);
   if ((m & q.req_term_mask) != q.req_term_mask) return false;
   if (m & q.not_term_mask) return false;
   if (ix.live_bits && !((ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
@@ -191,7 +187,7 @@ __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolS
       uint32_t b = (uint32_t)((slot >> (8 * c.slot)) & 0xff);
       present = b != 0;
       if (present && c.scoring) {
-        float f = (b == 255u) ? exact_freq_slow<SlotT>(ix, c, doc) : (float)b;
+        float f = (b == 255u) ? exact_freq_slow<uint64_t>(ix, c, doc) : (float)b;
         const uint8_t* nrm = ix.norms[c.field];
         uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
         s = bm25_score(c.weight, f, sm.cache[c.slot][nb]);
@@ -230,8 +226,7 @@ __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolS
 }
 
 // sort the candidate buffer, keep the best top_k, raise theta (local + global)
-template <typename SlotT>
-__device__ __forceinline__ void compact_candidates(BoolSmem<SlotT>& sm, int top_k, uint64_t* g_theta) {
+__device__ __forceinline__ void compact_candidates(BoolSmem& sm, int top_k, uint64_t* g_theta) {
   __syncthreads();
   int n = sm.cand_count;
   if (n > kCandCap) n = kCandCap;  // cannot happen (capacity invariant); defensive
@@ -255,10 +250,9 @@ __device__ __forceinline__ void compact_candidates(BoolSmem<SlotT>& sm, int top_
   __syncthreads();
 }
 
-template <typename SlotT>
 __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  BoolSmem<SlotT>& sm = *reinterpret_cast<BoolSmem<SlotT>*>(smem_raw);
+  BoolSmem& sm = *reinterpret_cast<BoolSmem*>(smem_raw);
   const int tid = threadIdx.x;
   const int lane = tid & 31;
 
@@ -324,7 +318,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) 
         for (uint32_t p = b0 + tid; p < b1; p += kThreads) {
           int32_t d = docs[p] - wbase;
           unsigned char f = scoring ? f8[p] : (unsigned char)1;
-          slot_bytes[(size_t)d * sizeof(SlotT) + s] = f;
+          slot_bytes[(size_t)d * sizeof(uint64_t) + s] = f;
         }
       }
       if (!any) continue;  // CTA-uniform: no postings in this window
@@ -362,9 +356,9 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) 
           const int s = sm.cl[c].slot;
           if (!((sm.q.driver_mask >> s) & 1u)) continue;
           // bytes of lower driver slots
-          SlotT below = 0;
-          for (int j = 0; j < s; ++j) if ((sm.q.driver_mask >> j) & 1u) below |= (SlotT)0xff << (8 * j);
-          const SlotT own = (SlotT)0xff << (8 * s);
+          uint64_t below = 0;
+          for (int j = 0; j < s; ++j) if ((sm.q.driver_mask >> j) & 1u) below |= (uint64_t)0xff << (8 * j);
+          const uint64_t own = (uint64_t)0xff << (8 * s);
           const uint32_t b0 = sm.bounds[s][w], b1 = sm.bounds[s][w + 1];
           const int32_t* docs = L.ix.post_docs + sm.cl[c].post_base;
           for (uint32_t p0 = b0; p0 < b1; p0 += kThreads) {
@@ -372,10 +366,10 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) 
             bool matched = false; int32_t doc = 0; float score = 0.0f;
             if (p < b1) {
               doc = docs[p];
-              SlotT v = sm.slots[doc - wbase];
+              uint64_t v = sm.slots[doc - wbase];
               if ((v & below) == 0 && (v & own) != 0) {
                 sm.slots[doc - wbase] = 0;
-                matched = evaluate_doc<SlotT>(L.ix, sm, doc, v, &score);
+                matched = evaluate_doc(L.ix, sm, doc, v, &score);
               }
             }
             offer(matched, doc, score);
@@ -389,9 +383,9 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) 
           int i = i0 + tid;
           bool matched = false; int32_t doc = wbase + i; float score = 0.0f;
           if (i < wlen) {
-            SlotT v = sm.slots[i];
+            uint64_t v = sm.slots[i];
             if (v) sm.slots[i] = 0;
-            matched = evaluate_doc<SlotT>(L.ix, sm, doc, v, &score);
+            matched = evaluate_doc(L.ix, sm, doc, v, &score);
           }
           offer(matched, doc, score);
           round_end();

@@ -2,7 +2,6 @@
 // batch compilation, kernel launches. No CPU fallback: every entry point needs a CUDA device.
 #include "../../include/nrtgpu.h"
 #include "bool_kernel.cuh"
-#include "stream_kernel.cuh"
 #include "probe_kernel.cuh"
 #include "sort_kernel.cuh"
 #include "collect_kernel.cuh"
@@ -77,6 +76,27 @@ __global__ void plane_fill_kernel(const int32_t* __restrict__ docs, const uint8_
   if (i < n) plane[docs[i]] = f8[i];
 }
 
+// index-time skip data: for every term with a long list, the number of its postings below each granule boundary
+struct GranTabLaunch {
+  const int32_t* post_docs;
+  const int64_t* row_off;   // [n_rows] first posting of the row's term
+  const int32_t* row_n;     // [n_rows] postings of the row's term
+  int32_t n_rows, n_gran, n_docs;
+  uint32_t* tab;            // [n_rows][n_gran + 1]
+};
+
+__global__ void gran_table_kernel(GranTabLaunch G) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)G.n_rows * (G.n_gran + 1)) return;
+  const int r = (int)(i / (G.n_gran + 1)), g = (int)(i % (G.n_gran + 1));
+  const int64_t target64 = (int64_t)g << v3::kLogGran;
+  const int32_t target = target64 > (int64_t)G.n_docs ? G.n_docs : (int32_t)target64;
+  const int32_t* docs = G.post_docs + G.row_off[r];
+  int lo = 0, hi = G.row_n[r];
+  while (lo < hi) { int mid = (lo + hi) >> 1; if (__ldg(docs + mid) < target) lo = mid + 1; else hi = mid; }
+  G.tab[i] = (uint32_t)lo;
+}
+
 namespace {
 
 // ---- SmallFloat.byte4ToInt (Lucene) : norm byte -> field length, for the BM25 length table ----
@@ -136,18 +156,14 @@ struct DevBuf {
 struct nrtgpu_ctx {
   int device = 0;
   int sm_count = 0;
-  bool engine_stream = false;   // NRTGPU_ENGINE=stream: round-1 window/stream kernel for every <= 4-term query (A/B runs)
   std::mutex hyb_mu;             // O(k) hybrid stages share one pooled device scratch (no cudaMalloc per call)
   DevBuf<int32_t> hyb_scratch;
   int64_t item_postings = 32768; // NRTGPU_ITEM_POSTINGS: floor of the postings a (query, slice) may hold before it is split into 2..16 parts
   int64_t item_share_full = 32;  // NRTGPU_ITEM_SHARE_FULL: the same for launches that visit every posting (ScoreMode.COMPLETE, generic clause evaluation)
   int64_t item_share = 12;       // NRTGPU_ITEM_SHARE: ... and it is split when it exceeds 1/share of the postings per resident CTA
-  int64_t warm_min_docs = 8ll * v2::kWarmGran * v2::kGran;   // NRTGPU_WARM_MIN_DOCS: shards below this size run without warm-up items
-  bool warm_sweep = true;        // NRTGPU_WARM=docs: warm-up items sweep the first 32K docs (round-2 first style) instead of the rarest list
+  int64_t warm_min_docs = 8ll * v3::kWarmGran * v3::kGran;   // NRTGPU_WARM_MIN_DOCS: shards below this size run without warm-up items
   int slice_gran = 512;          // NRTGPU_SLICE_GRAN: granules (1024 docs) per slice of the probe kernel, <= v3::kMaxSliceGran
   int probe_cfg = 0;             // NRTGPU_PROBE_CFG: 0 auto, 1 always A (3 CTAs / SM), 2 always B (4 CTAs / SM)
-  bool order_lpt = false;        // NRTGPU_ORDER=lpt: query-major work order, longest query first
-  bool order_by_cost = false;   // NRTGPU_ORDER=cost: round-1 work order (longest query first) instead of plane clusters
   bool debug_modes = false;     // NRTGPU_DEBUG_MODES=1: per-launch kernel statistics on stderr (adds a stream synchronisation)
 };
 
@@ -252,23 +268,18 @@ static void free_batch(nrtgpu_batch* b);
 struct nrtgpu_batch {
   nrtgpu_index* ix = nullptr;
   int32_t nq = 0, top_k = 0, n_slices = 0, n_work = 0;
-  int32_t n_lists = 0;         // per-query candidate lists the kernels fill: n_slices (+1: warm-up items of the stream path)
-  int32_t n_work_simple = 0;   // the first n_work_simple work items belong to pure single-field term disjunctions
-  // work list layout (<= 4-term batches): [probe simple | probe generic | stream (window kernel: no posting list can lead)]
-  int32_t n_probe_simple = 0, n_probe_generic = 0, n_stream = 0;
-  bool use_probe = false;
+  int32_t n_lists = 0;         // per-query candidate lists the kernels fill: n_slices * parts_max (+1: the warm-up items' list)
+  // work list layout of a probe batch: [probe simple | probe generic]
+  int32_t n_probe_simple = 0, n_probe_generic = 0;
   DevBuf<uint32_t> sbounds;            // probe kernel: [nq][4][n_slices * parts_max + 2] part-boundary posting offsets
   DevBuf<unsigned int> work_counter;   // probe kernel: queue heads [2]
   DevBuf<unsigned long long> probe_stats;
-  bool wide_slots = false;
+  bool wide_slots = false;     // more than 4 term clauses or top_k > 512: bool_window_kernel runs the whole batch
   bool exhaustive = true;
   int64_t alg_postings = 0;
   DevBuf<DevClause> clauses;
   DevBuf<DevQuery> queries;
   DevBuf<int32_t> work_query, work_slice;
-  DevBuf<uint32_t> gbounds;  // stream kernel: [nq][4][n_gran+1]
-  DevBuf<float> qtables;     // stream kernel: [nq][kQTabFloats] score + bound tables
-  DevBuf<unsigned long long> mode_stats;   // NRTGPU_DEBUG_MODES=1: cycles / work items per kernel mode
   DevBuf<int32_t> pruned;    // [nq] relation GTE flags
   DevBuf<int32_t> terminated; // [nq] terminateAfter cut the query short
   DevBuf<int32_t> timed_out;  // [nq] a work item of the query was skipped because the deadline had passed
@@ -379,24 +390,14 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   std::unique_ptr<nrtgpu_ctx> c(new nrtgpu_ctx);   // released to the caller only when every attribute call succeeded
   c->device = device_id;
   c->sm_count = prop.multiProcessorCount;
-  { const char* e = getenv("NRTGPU_ENGINE"); c->engine_stream = e && std::strcmp(e, "stream") == 0; }
   c->debug_modes = getenv("NRTGPU_DEBUG_MODES") != nullptr;
   { const char* e = getenv("NRTGPU_PROBE_CFG"); c->probe_cfg = e ? atoi(e) : 0; }
   { const char* e = getenv("NRTGPU_WARM_MIN_DOCS"); if (e && atoll(e) > 0) c->warm_min_docs = atoll(e); }
-  { const char* e = getenv("NRTGPU_WARM"); c->warm_sweep = !(e && std::strcmp(e, "docs") == 0); }
   { const char* e = getenv("NRTGPU_SLICE_GRAN"); if (e && atoi(e) >= 64) c->slice_gran = std::min(atoi(e), (int)v3::kMaxSliceGran); }
   { const char* e = getenv("NRTGPU_ITEM_POSTINGS"); if (e && atoll(e) > 0) c->item_postings = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE"); if (e && atoll(e) > 0) c->item_share = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE_FULL"); if (e && atoll(e) > 0) c->item_share_full = atoll(e); }
-  { const char* e = getenv("NRTGPU_ORDER"); c->order_by_cost = e && (std::strcmp(e, "cost") == 0 || std::strcmp(e, "lpt") == 0); c->order_lpt = e && std::strcmp(e, "lpt") == 0; }
-  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)sizeof(BoolSmem<uint32_t>)));
-  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)sizeof(BoolSmem<uint64_t>)));
-  NRT_CUDA_TRY(cudaFuncSetAttribute(v2::posting_stream_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)sizeof(v2::StreamSmem)));
-  NRT_CUDA_TRY(cudaFuncSetAttribute(v2::posting_stream_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)sizeof(v2::StreamSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
 #define NRT_PROBE_ATTR(S, D) \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasA, v3::kStageA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageA>))); \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasB, v3::kStageB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageB>)));
@@ -454,7 +455,7 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
   ix->field_doc_count.assign(d->field_doc_count, d->field_doc_count + d->n_fields);
   ix->field_sum_ttf.assign(d->field_sum_ttf, d->field_sum_ttf + d->n_fields);
   // postings
-  const size_t pad = 2 * (size_t)v2::kCH;   // whole TMA chunks may extend past the last posting
+  const size_t pad = (size_t)v3::kPostingPad;
   if ((rc = ix->post_docs.alloc((size_t)P + pad))) return rc;
   NRT_CUDA_TRY(cudaMemset(ix->post_docs.p, 0x7f, ((size_t)P + pad) * sizeof(int32_t)));
   if (P) NRT_CUDA_TRY(cudaMemcpy(ix->post_docs.p, d->post_docs, (size_t)P * sizeof(int32_t), cudaMemcpyHostToDevice));
@@ -503,11 +504,11 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
       NRT_CUDA_TRY(cudaGetLastError());
     }
   }
-  // skip data: posting offsets at every stream-kernel granule boundary for the lists long enough to make the
-  // per-batch lower_bound searches expensive (>= 4096 postings); a batch then copies the row instead of searching
+  // skip data: posting offsets at every 1024-doc granule boundary for the lists long enough to make the per-batch
+  // lower_bound searches expensive (>= 4096 postings); a batch then copies the row instead of searching
   ix->term_gran.assign((size_t)d->n_terms, -1);
   {
-    const int32_t n_gran = std::max<int32_t>(1, (int32_t)(((int64_t)d->n_docs + v2::kGran - 1) / v2::kGran));
+    const int32_t n_gran = std::max<int32_t>(1, (int32_t)(((int64_t)d->n_docs + v3::kGran - 1) / v3::kGran));
     std::vector<int64_t> row_off; std::vector<int32_t> row_n;
     const size_t max_rows = (size_t)((2ll << 30) / ((int64_t)(n_gran + 1) * 4));
     for (int32_t t = 0; t < d->n_terms && row_off.size() < max_rows; ++t) {
@@ -521,10 +522,10 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
       if ((rc = d_rn.upload(row_n.data(), row_n.size()))) return rc;
       const int64_t total = (int64_t)row_off.size() * (n_gran + 1);
       if ((rc = ix->gran_tab.alloc((size_t)total))) return rc;
-      v2::GranTabLaunch G;
+      GranTabLaunch G;
       G.post_docs = ix->post_docs.p; G.row_off = d_ro.p; G.row_n = d_rn.p; G.n_rows = (int32_t)row_off.size();
       G.n_gran = n_gran; G.n_docs = d->n_docs; G.tab = ix->gran_tab.p;
-      v2::gran_table_kernel<<<(unsigned)((total + 255) / 256), 256>>>(G);
+      gran_table_kernel<<<(unsigned)((total + 255) / 256), 256>>>(G);
       NRT_CUDA_TRY(cudaGetLastError());
       NRT_CUDA_TRY(cudaDeviceSynchronize());
     }
@@ -722,7 +723,6 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
   b->order = sort_order;
   if (n_aggs > 0) {
     if (!aggs || n_aggs > kMaxAggs) NRT_FAIL(NRTGPU_ERR_INVALID, "at most 8 aggregations per search");
-    if (ix && ix->ctx->engine_stream) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "aggregations need the probe engine");
     for (int i = 0; i < n_aggs; ++i) {
       const nrtgpu_aggregation& a = aggs[i];
       if (a.kind < NRTGPU_AGG_TERMS || a.kind > NRTGPU_AGG_SUM) NRT_FAIL(NRTGPU_ERR_INVALID, "bad aggregation kind");
@@ -751,7 +751,6 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
     if (!sort_order && sort->kind == NRTGPU_SORT_COLUMN && (sort->column < 0 || sort->column >= ix->n_columns))
       NRT_FAIL(NRTGPU_ERR_INVALID, "sort column out of range (field does not support sorting: no doc values)");
     if (!sort_order && sort->kind == NRTGPU_SORT_COLUMN && ix->col_multi[(size_t)sort->column]) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "sort on a multi-valued column");
-    if (ix->ctx->engine_stream) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "sorted search needs the probe engine");
     total_hits_threshold = INT32_MAX;   // every match is visited: exact totalHits
   }
   if (nq <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: nq must be > 0");
@@ -817,7 +816,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
         if (c.occur == NRTGPU_SHOULD) should_term_mask |= 1u << n_term;
         if (c.occur == NRTGPU_MUST) o.must_term_mask |= 1u << n_term;
         if (x.scoring) field0 = (field0 == -2 || field0 == f) ? f : -1;
-        if (x.scoring) b->alg_postings += x.n_post; else b->alg_postings += x.n_post;
+        b->alg_postings += x.n_post;
         ++n_term;
       } else if (c.kind == NRTGPU_RANGE_I64) {
         if (c.id < 0 || c.id >= ix->n_columns) NRT_FAIL(NRTGPU_ERR_INVALID, "column id out of range");
@@ -859,8 +858,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
       else o.after_key = make_key(q.after_score, (int32_t)local);
     }
   }
-  b->wide_slots = max_terms > 4 || top_k > v2::kMaxTopKStream;
-  b->use_probe = !b->wide_slots && !ix->ctx->engine_stream;
+  b->wide_slots = max_terms > 4 || top_k > v3::kMaxTopK;
   if (n_aggs > 0 && b->wide_slots) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "aggregations: more than 4 term clauses or top_k > 512 is not on the GPU path");
   if (sorted && b->wide_slots) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "sorted search: more than 4 term clauses or top_k > 512 is not on the GPU path");
   if (!b->wide_slots) {
@@ -868,10 +866,10 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
     // (probe kernel: slices of up to slice_gran granules -- NRTGPU_SLICE_GRAN, default and maximum 512: the MAXSCORE roles of an
     //  item are fixed when it starts, so larger slices prune with staler thresholds -- measured slower -- and smaller ones pay
     //  the per-item set-up more often)
-    const int64_t max_slice_docs = (!ix->ctx->engine_stream) ? (int64_t)ix->ctx->slice_gran * v2::kGran : (int64_t)v2::kSliceDocs;
+    const int64_t max_slice_docs = (int64_t)ix->ctx->slice_gran * v3::kGran;
     const int64_t n_sl = std::max<int64_t>(1, ((int64_t)ix->n_docs + max_slice_docs - 1) / max_slice_docs);
-    slice_docs = (((int64_t)ix->n_docs + n_sl - 1) / n_sl + v2::kGran - 1) / v2::kGran * v2::kGran;
-    if (slice_docs < v2::kGran) slice_docs = v2::kGran;
+    slice_docs = (((int64_t)ix->n_docs + n_sl - 1) / n_sl + v3::kGran - 1) / v3::kGran * v3::kGran;
+    if (slice_docs < v3::kGran) slice_docs = v3::kGran;
   }
   b->slice_docs = (int32_t)slice_docs;
   b->n_slices = (int32_t)std::max<int64_t>(1, ((int64_t)ix->n_docs + slice_docs - 1) / slice_docs);
@@ -886,7 +884,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
     if (dq[qi].dense_driver) cost[qi] += ix->n_docs;
   }
   std::stable_sort(order.begin(), order.end(), [&](int a, int c) { return cost[a] > cost[c]; });
-  if (b->use_probe && !ix->ctx->order_by_cost) {
+  if (!b->wide_slots) {
     // probe kernel: inside a slice, queries that share their densest tf plane are adjacent in the queue, so the plane's
     // bytes of the slice are gathered by CTAs that run together and stay in L2 between them (longer queries first inside
     // a cluster, clusters of the densest -- most shared -- planes first)
@@ -900,35 +898,27 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
     }
     std::stable_sort(order.begin(), order.end(), [&](int a, int c) { return ckey[(size_t)a] < ckey[(size_t)c]; });
   }
-  // pure disjunctions of scoring term clauses over one text field (no deletes) run in their own kernel instantiation
-  // (tf-pattern bound, deferred scoring, MAXSCORE): their work items come first
+  // pure disjunctions of scoring term clauses over one text field run in their own probe kernel instantiation
+  // (tf-pattern bound, deferred scoring, MAXSCORE): their work items come first. A wide batch (one launch) orders its
+  // work items the same way, but only on a shard without deletes.
   auto is_simple = [&](int qi) {
     const DevQuery& o = dq[(size_t)qi];
-    return !sorted && n_aggs == 0 && o.single_field >= 0 && !o.has_nonterm && !o.nonterm_scoring && (b->use_probe || ix->live_bits.p == nullptr) && o.n_req == 0 &&
+    return !sorted && n_aggs == 0 && o.single_field >= 0 && !o.has_nonterm && !o.nonterm_scoring && (!b->wide_slots || ix->live_bits.p == nullptr) && o.n_req == 0 &&
            o.not_term_mask == 0 && o.msm <= 1 && !o.dense_driver;
-  };
-  // 0: probe kernel, simple; 1: probe kernel, generic (a posting list leads); 2: window/stream kernel (no list can lead)
-  auto engine_class = [&](int qi) {
-    if (is_simple(qi)) return 0;
-    if (!b->use_probe) return 2;
-    return 1;   // the probe kernel also sweeps whole doc ranges when no posting list can lead (match-all / range-led queries)
   };
   std::vector<int32_t>& wq = b->h_wq; std::vector<int32_t>& ws = b->h_ws;
   wq.clear(); ws.clear();
   // warm-up items (large shards): a query first sweeps the leading kWarmGran granules of slice 0 as a work item of its
   // own, ahead of everything else, so that its other work items start with a threshold and a hit count (MAXSCORE can
-  // prune from the first slice on). Window kernel: TOP_SCORES mode, queries with a dense list; probe kernel: both score
-  // modes, every query whose lists are expected to hold 2 * top_k hits in those granules.
-  const bool warm_ok = !b->wide_slots && (b->use_probe || b->threshold < (int64_t)INT32_MAX) &&
-                       (int64_t)ix->n_docs >= (int64_t)ix->ctx->warm_min_docs;
+  // prune from the first slice on). Both score modes, every query whose lists are expected to hold 2 * top_k hits in
+  // those granules.
+  const bool warm_ok = !b->wide_slots && (int64_t)ix->n_docs >= (int64_t)ix->ctx->warm_min_docs;
   std::vector<uint8_t> has_warm((size_t)nq, 0);
   // probe kernel, pure disjunctions on a shard without deletes: the longest list is a lower bound of the matching docs
   // (pruning may start as soon as that exceeds totalHitsThreshold), and the warm-up SWEEPS the first 32K postings of the
-  // highest-bound (rarest) list over the whole shard instead of the first 32K docs (flags 4; NRTGPU_WARM=docs: old style)
+  // highest-bound (rarest) list over the whole shard instead of the first 32K docs (flags 4)
   b->h_known.assign((size_t)nq, 0ull);
-  const bool limits_may_apply = true;   // (terminateAfter counts collected hits only: the kernel never uses known_hits for it)
-  (void)limits_may_apply;
-  if (b->use_probe && !ix->live_bits.p && !sorted && n_aggs == 0)
+  if (!b->wide_slots && !ix->live_bits.p && !sorted && n_aggs == 0)
     for (int qi : order) {
       if (!is_simple(qi)) continue;
       int64_t mx = 0;
@@ -940,7 +930,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
       if (!is_simple(qi)) continue;
       // (not with searchAfter: a doc whose LOWER-BOUND key passes the after filter may in truth lie on an earlier page, and
       //  would be counted towards the k keys that justify the threshold)
-      if (b->use_probe && ix->ctx->warm_sweep && !dq[qi].has_after) {
+      if (!dq[qi].has_after) {
         int best = -1; float best_ub = -1.0f;
         for (int c = 0; c < dq[qi].n_clauses; ++c) {
           const DevClause& x = dc[(size_t)dq[qi].clause_begin + c];
@@ -951,24 +941,17 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
           continue;   // (has_warm stays 0: the query's slice-0 items cover the whole slice)
         }
       }
-      if (b->use_probe) {
-        if (cost[qi] * (int64_t)(v2::kWarmGran * v2::kGran) >= 2ll * top_k * (int64_t)ix->n_docs) has_warm[(size_t)qi] = 1;
-      } else {
-        for (int c = 0; c < dq[qi].n_clauses; ++c) {
-          const DevClause& x = dc[(size_t)dq[qi].clause_begin + c];
-          if (x.kind == NRTGPU_TERM && (int64_t)x.n_post * 64 >= (int64_t)ix->n_docs) has_warm[(size_t)qi] = 1;
-        }
-      }
+      if (cost[qi] * (int64_t)(v3::kWarmGran * v3::kGran) >= 2ll * top_k * (int64_t)ix->n_docs) has_warm[(size_t)qi] = 1;
       if (has_warm[(size_t)qi]) { wq.push_back(qi); ws.push_back(0 | (1 << 24)); }
     }
   }
   // heavy (query, slice) pairs are split into 2..16 parts of equal granule ranges, so that no single work item is a
   // large share of the launch (the longest item bounds the kernel time from below: what limits small shards)
-  const int gran_per_slice = (int)(slice_docs / v2::kGran);
-  const int n_gran_h = std::max<int>(1, (int)(((int64_t)ix->n_docs + v2::kGran - 1) / v2::kGran));
+  const int gran_per_slice = (int)(slice_docs / v3::kGran);
+  const int n_gran_h = std::max<int>(1, (int)(((int64_t)ix->n_docs + v3::kGran - 1) / v3::kGran));
   std::vector<uint8_t> lparts((size_t)nq, 0);
   int lp_max = 0;
-  if (b->use_probe) {
+  if (!b->wide_slots) {
     int64_t total_cost = 0;
     for (int qi : order) total_cost += cost[qi];
     const int64_t per_cta = total_cost / ((int64_t)v3::kCtasA * ix->ctx->sm_count);
@@ -994,26 +977,22 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
     const bool behind_warm = s == 0 && has_warm[(size_t)qi];
     for (int p = 0; p < P; ++p) {
       int lo = std::min(g_count, p * kfine * fine), hi = (p + 1) * kfine >= b->parts_max ? g_count : std::min(g_count, (p + 1) * kfine * fine);
-      if (behind_warm) lo = std::max(lo, std::min(g_count, (int)v2::kWarmGran));
+      if (behind_warm) lo = std::max(lo, std::min(g_count, (int)v3::kWarmGran));
       if (P > 1 && lo >= hi) continue;
       wq.push_back(qi); ws.push_back(s | (p << 16) | (lp << 20) | (behind_warm ? (2 << 24) : 0));
     }
   };
-  int32_t class_end[3] = {0, 0, 0};
-  for (int cls = 0; cls < 3; ++cls) {
-    if (ix->ctx->order_lpt && b->use_probe) {   // longest query first, its slices together (experiment: NRTGPU_ORDER=lpt)
-      for (int qi : order) if (engine_class(qi) == cls)
-        for (int s = 0; s < b->n_slices; ++s) push_items(qi, s);
-    } else {
-      for (int s = 0; s < b->n_slices; ++s)
-        for (int qi : order) if (engine_class(qi) == cls) push_items(qi, s);
-    }
-    class_end[cls] = (int32_t)wq.size();
+  // simple queries first (with the warm-up items ahead of them), then the generic ones; the generic probe instantiation
+  // also sweeps whole doc ranges when no posting list can lead (match-all / range-led queries)
+  int32_t n_simple_items = 0;
+  for (const bool simple : {true, false}) {
+    for (int s = 0; s < b->n_slices; ++s)
+      for (int qi : order) if (is_simple(qi) == simple) push_items(qi, s);
+    if (simple) n_simple_items = (int32_t)wq.size();
   }
   b->n_work = (int32_t)wq.size();
-  b->n_work_simple = class_end[0];
-  if (b->use_probe) { b->n_probe_simple = class_end[0]; b->n_probe_generic = class_end[1] - class_end[0]; b->n_stream = class_end[2] - class_end[1]; }
-  else { b->n_probe_simple = b->n_probe_generic = 0; b->n_stream = b->wide_slots ? 0 : b->n_work; }
+  b->n_probe_simple = b->wide_slots ? 0 : n_simple_items;
+  b->n_probe_generic = b->wide_slots ? 0 : b->n_work - n_simple_items;
   b->h_dc.swap(dc); b->h_dq.swap(dq);   // kept alive until the next compilation: the uploads below are asynchronous
   int rc;
   if ((rc = b->clauses.upload_async(b->h_dc.data(), b->h_dc.size(), st))) return rc;
@@ -1071,7 +1050,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
   if ((rc = b->pruned.alloc((size_t)nq))) return rc;
   if ((rc = b->terminated.alloc((size_t)nq))) return rc;
   if (!b->wide_slots) {
-    b->n_gran = (int32_t)(((int64_t)ix->n_docs + v2::kGran - 1) / v2::kGran);
+    b->n_gran = (int32_t)(((int64_t)ix->n_docs + v3::kGran - 1) / v3::kGran);
     if (b->n_gran < 1) b->n_gran = 1;
     if (b->n_probe_simple + b->n_probe_generic > 0) {
       // probe kernel: posting offsets of every (query, term slot) at the slice boundaries only (skip data for the long
@@ -1081,24 +1060,8 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
       if ((rc = b->work_counter.alloc(2))) return rc;
       v3::SliceBoundsLaunch S;
       S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_slices = b->n_slices;
-      S.slice_gran = b->slice_docs / v2::kGran; S.n_gran = b->n_gran; S.parts_max = b->parts_max; S.sbounds = b->sbounds.p;
+      S.slice_gran = b->slice_docs / v3::kGran; S.n_gran = b->n_gran; S.parts_max = b->parts_max; S.sbounds = b->sbounds.p;
       v3::slice_bounds_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S);
-      NRT_CUDA_TRY(cudaGetLastError());
-    }
-    if (b->n_stream > 0) {
-      // the window/stream kernel reads per-granule posting bounds of every (query, term clause) and per-query score tables
-      const int64_t total = (int64_t)nq * v2::kT * (b->n_gran + 1);
-      if ((rc = b->gbounds.alloc((size_t)total))) return rc;
-      v2::BoundsLaunch B;
-      B.ix = ix->view(); B.clauses = b->clauses.p; B.queries = b->queries.p; B.nq = nq; B.n_gran = b->n_gran;
-      B.gbounds = b->gbounds.p;
-      v2::granule_bounds_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(B);
-      NRT_CUDA_TRY(cudaGetLastError());
-      if ((rc = b->qtables.alloc((size_t)nq * v2::kQTabFloats))) return rc;
-      v2::QTabLaunch Q;
-      Q.ix = B.ix; Q.clauses = B.clauses; Q.queries = B.queries; Q.field_min_norm = ix->field_min_norm.p; Q.nq = nq;
-      Q.qtables = b->qtables.p;
-      if (nq > 0) v2::query_tables_kernel<<<(unsigned)nq, 256, 0, st>>>(Q);
       NRT_CUDA_TRY(cudaGetLastError());
     }
   }
@@ -1123,11 +1086,8 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
   int rc_dbg = 0;
   NRT_CUDA_TRY(cudaSetDevice(b->ix->ctx->device));
-  static const bool keep_theta = getenv("NRTGPU_EXPERIMENT_KEEP_THETA") != nullptr;   // timing experiment only: a run starts with the previous run's thresholds
-  if (!keep_theta || !b->ran) {
-    NRT_CUDA_TRY(cudaMemsetAsync(b->theta.p, 0, b->theta.bytes(), st));
-    NRT_CUDA_TRY(cudaMemsetAsync(b->total_hits.p, 0, b->total_hits.bytes(), st));
-  }
+  NRT_CUDA_TRY(cudaMemsetAsync(b->theta.p, 0, b->theta.bytes(), st));
+  NRT_CUDA_TRY(cudaMemsetAsync(b->total_hits.p, 0, b->total_hits.bytes(), st));
   NRT_CUDA_TRY(cudaMemsetAsync(b->slice_cnt.p, 0, b->slice_cnt.bytes(), st));
   NRT_CUDA_TRY(cudaMemsetAsync(b->pruned.p, 0, b->pruned.bytes(), st));
   NRT_CUDA_TRY(cudaMemsetAsync(b->terminated.p, 0, b->terminated.bytes(), st));
@@ -1225,46 +1185,12 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         }
         NRT_CUDA_TRY(cudaGetLastError());
       }
-      if (b->n_stream > 0) {
-        v2::StreamLaunch S;
-        S.ix = L.ix; S.clauses = L.clauses; S.queries = L.queries;
-        S.gbounds = b->gbounds.p; S.n_gran = b->n_gran; S.qtables = b->qtables.p; S.n_slices = L.n_slices; S.top_k = L.top_k;
-        S.slice_docs = b->slice_docs;
-        S.threshold = b->threshold; S.pruned = b->pruned.p;
-        S.mode_stats = nullptr;
-        if (debug && !b->use_probe) {
-          if (!b->mode_stats.p && (rc_dbg = b->mode_stats.alloc(13))) return rc_dbg;
-          NRT_CUDA_TRY(cudaMemsetAsync(b->mode_stats.p, 0, 13 * sizeof(unsigned long long), st));
-          S.mode_stats = b->mode_stats.p;
-        }
-        S.theta = L.theta; S.total_hits = L.total_hits; S.slice_keys = L.slice_keys; S.slice_cnt = L.slice_cnt;
-        const int first = n_probe;   // stream items follow the probe items in the work list
-        const int n_simple = b->use_probe ? 0 : b->n_work_simple;
-        if (n_simple > 0) {
-          S.work_query = L.work_query + first; S.work_slice = L.work_slice + first; S.n_work = n_simple;
-          v2::posting_stream_kernel<true><<<n_simple, v2::kThreads, sizeof(v2::StreamSmem), st>>>(S);
-        }
-        if (b->n_stream > n_simple) {
-          S.work_query = L.work_query + first + n_simple; S.work_slice = L.work_slice + first + n_simple;
-          S.n_work = b->n_stream - n_simple;
-          v2::posting_stream_kernel<false><<<S.n_work, v2::kThreads, sizeof(v2::StreamSmem), st>>>(S);
-        }
-        NRT_CUDA_TRY(cudaGetLastError());
-      }
     } else
-      bool_window_kernel<uint64_t><<<b->n_work, kThreads, sizeof(BoolSmem<uint64_t>), st>>>(L);
+      bool_window_kernel<<<b->n_work, kThreads, sizeof(BoolSmem), st>>>(L);
     NRT_CUDA_TRY(cudaGetLastError());
   }
   NRT_CUDA_TRY(cudaEventRecord(ev[1], st));
-  if (debug && b->mode_stats.p && !b->use_probe) {
-    unsigned long long h[13];
-    NRT_CUDA_TRY(cudaMemcpyAsync(h, b->mode_stats.p, sizeof(h), cudaMemcpyDeviceToHost, st));
-    NRT_CUDA_TRY(cudaStreamSynchronize(st));
-    fprintf(stderr, "[nrtgpu modes] window: %llu items %.0f cyc/item %llu driver postings | window+maxscore: %llu items %.0f %llu | sparse: %llu items %.0f %llu\n",
-            h[1], h[1] ? (double)h[0] / h[1] : 0.0, h[6], h[3], h[3] ? (double)h[2] / h[3] : 0.0, h[7], h[5], h[5] ? (double)h[4] / h[5] : 0.0, h[8]);
-    if (h[5]) fprintf(stderr, "[nrtgpu modes] sparse items: set-up %.0f cyc, sweep %.0f, flush+output %.0f, %.2f runs/item\n", (double)h[9] / h[5], (double)h[10] / h[5], (double)h[11] / h[5], (double)h[12] / h[5]);
-  }
-  if (debug && b->probe_stats.p && b->use_probe) {
+  if (debug && b->probe_stats.p && !b->wide_slots) {
     unsigned long long h[32];
     NRT_CUDA_TRY(cudaMemcpyAsync(h, b->probe_stats.p, sizeof(h), cudaMemcpyDeviceToHost, st));
     NRT_CUDA_TRY(cudaStreamSynchronize(st));
@@ -1283,8 +1209,8 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   M.out_docs = b->o_docs(); M.out_scores = b->o_scores(); M.out_counts = b->o_counts();
   M.total_hits = b->total_hits.p; M.pruned = b->pruned.p; M.terminated = b->terminated.p; M.terminate_after = b->ta_scalar;
   M.out_total = b->bound_total; M.out_flags = b->bound_flags;
-  M.theta = b->use_probe ? b->theta.p : nullptr;
-  M.known_hits = (b->use_probe && !b->ix->live_bits.p) ? b->known_hits.p : nullptr;
+  M.theta = !b->wide_slots ? b->theta.p : nullptr;
+  M.known_hits = (!b->wide_slots && !b->ix->live_bits.p) ? b->known_hits.p : nullptr;
   merge_slices_kernel<<<b->nq, kMergeThreads, 0, st>>>(M);
   NRT_CUDA_TRY(cudaGetLastError());
   if (b->order) {   // FieldDoc values of every field; score-first orders map ranks back to docs
@@ -1492,11 +1418,7 @@ int nrtgpu_batch_stats(const nrtgpu_batch* b, int64_t* alg_postings, int32_t* la
   if (launches_per_run) {
     int n = 1;   // slice merge
     if (b->wide_slots) n += b->n_work > 0 ? 1 : 0;
-    else {
-      n += (b->n_probe_simple > 0 ? 1 : 0) + (b->n_probe_generic > 0 ? 1 : 0);
-      const int n_simple = b->use_probe ? 0 : b->n_work_simple;
-      n += (n_simple > 0 ? 1 : 0) + (b->n_stream > n_simple ? 1 : 0);
-    }
+    else n += (b->n_probe_simple > 0 ? 1 : 0) + (b->n_probe_generic > 0 ? 1 : 0);
     *launches_per_run = n;
   }
   if (work_items) *work_items = b->n_work;

@@ -29,18 +29,37 @@
 //     required list is dropped after the probes, before any norm / doc-value gather).
 // Results are bit-identical to the exhaustive oracle (tests/test_gpu_parity.py, tests/test_gpu_probe.py).
 #pragma once
-#include "stream_kernel.cuh"
+#include "bool_kernel.cuh"
 #include "sort_kernel.cuh"
 #include "collect_kernel.cuh"
 
 namespace nrtgpu {
 namespace v3 {
 
-using v2::bulk_g2s;
-using v2::mbar_arrive_expect_tx;
-using v2::mbar_init;
-using v2::mbar_try_wait;
-using v2::smem_u32;
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+  return ok != 0;
+}
+// 1-D TMA bulk copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP)
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+
+// bit s set: byte s (term slot s) of a tf word is non-zero
+__device__ __forceinline__ uint32_t presence4(uint32_t s) {
+  return ((s & 0xffu) ? 1u : 0u) | ((s & 0xff00u) ? 2u : 0u) | ((s & 0xff0000u) ? 4u : 0u) | ((s & 0xff000000u) ? 8u : 0u);
+}
 
 // profiling builds only (-DNRT_PROBE_KNOCK): parts of the kernel can be disabled at run time through ProbeLaunch::knock
 #ifdef NRT_PROBE_KNOCK
@@ -56,10 +75,14 @@ constexpr int kT = 4;
 constexpr int kCtasA = 3, kStageA = 8192;
 constexpr int kCtasB = 4, kStageB = 6656;
 constexpr int kThreads = 256;
-constexpr int kLogGran = v2::kLogGran;       // 1024-doc granules: the granularity of the index-time skip data (gran_tab)
+constexpr int kLogGran = 10;                 // 1024-doc granules: the granularity of the index-time skip data (gran_tab)
 constexpr int kGran = 1 << kLogGran;
 constexpr int kMaxSliceGran = 512;           // a slice spans at most 512K docs (its granule offsets live in shared memory)
 constexpr int kAlign = 16;                   // staged segments start on 16-posting boundaries (TMA: 16-byte aligned tf bytes)
+// padding postings behind the last list of the index image: a staged segment also ends on a kAlign-posting boundary of
+// the global arrays (seg_n), so the segment of the last list can read up to kAlign - 1 postings past its end. 1024 is
+// far more than that; the value keeps the image layout and nrtgpu_index_device_bytes unchanged.
+constexpr int kPostingPad = 1024;
 constexpr int kLongReserve = kT * (kGran + 2 * kAlign);   // one granule of every long list always fits
 #ifndef NRT_PROBE_R
 #define NRT_PROBE_R 2
@@ -68,7 +91,7 @@ constexpr int kR = NRT_PROBE_R;              // driver postings per thread per r
 constexpr int kCand = 1024;                  // candidate buffer entries
 constexpr int kMaxTopK = kCand / 2;
 constexpr int kUbt = 6 * 6 * 6 * 6;
-constexpr int kWarmGran = v2::kWarmGran;
+constexpr int kWarmGran = 32;                // granules (32K docs) of the warm-up work item of a query
 constexpr uint32_t kPiece = 8192;            // bytes per bulk copy
 constexpr uint32_t kTfInexact = 0xFEu;       // tf byte of a plane probe whose 2-bit code saturated (tf >= 3): the exact byte is
                                              // fetched from the byte plane when the doc is scored (rare); >= 5 for the bound table
@@ -174,11 +197,11 @@ __device__ __forceinline__ uint32_t seg_n(uint32_t a, uint32_t b, uint32_t pbm) 
 }
 
 // Universal clause evaluation of one doc given the tf word of its term slots (Lucene BooleanScorerSupplier semantics,
-// as v2::evaluate_doc_generic: conjunction / disjunction sums in double, ReqOptSumScorer float add when msm == 0).
+// as the window kernel's evaluate_doc: conjunction / disjunction sums in double, ReqOptSumScorer float add when msm == 0).
 template <typename SM>
 __device__ __noinline__ bool evaluate_doc(const ProbeLaunch& L, const SM& sm, int32_t doc, uint32_t word, float* out_score) {
   const DevQuery& q = sm.q;
-  const uint32_t m = v2::presence4(word);
+  const uint32_t m = presence4(word);
   if ((m & q.req_term_mask) != q.req_term_mask) return false;
   if (m & q.not_term_mask) return false;
   if (L.ix.live_bits && !((L.ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
@@ -912,7 +935,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
                   const uint32_t sat = __vcmpeq4(codes, 0x03030303u);
                   v |= (codes & ~sat) | (sat & (kTfInexact * 0x01010101u));
                 }
-                const uint32_t pres = v2::presence4(v);
+                const uint32_t pres = presence4(v);
                 const bool surv = doc[j] >= 0 && (v & candbelow) == 0u && (pres & q_req) == q_req && (pres & q_not) == 0u;
                 const unsigned bal = __ballot_sync(0xffffffffu, surv);
                 if (surv) wq[qn + __popc(bal & ((1u << lane) - 1u))] = make_uint2((uint32_t)doc[j], v);
