@@ -25,51 +25,9 @@
 
 namespace nrtgpu {
 
-constexpr int kMaxClauses = 16;     // clauses per flat BooleanQuery on the GPU path
-constexpr int kMaxTermSlots = 8;    // term clauses per query: one tf byte each in the window kernel's 64-bit words
-constexpr int kWindowDocs = 16384;  // W
-constexpr int kSliceWindows = 64;   // windows per work item  => 1,048,576 docs per slice
+// (DevClause, DevQuery, the clause / slot / top_k limits and the window size: batch_plan.h)
 constexpr int kCandCap = 4096;      // candidate buffer (keys) per CTA, power of two
 constexpr int kThreads = 512;
-constexpr int kMaxTopK = 1024;
-
-struct DevClause {
-  int64_t post_base;  // offset of the term's postings in post_docs / post_f8
-  int32_t n_post;
-  int32_t occur;
-  int32_t kind;
-  int32_t slot;       // byte index inside the window word (term clauses), -1 otherwise
-  int32_t field;      // text field (norms + cache) for term clauses
-  int32_t col;        // doc-value column for range clauses
-  float weight;       // boost*idf (term) or constant score = boost (range / match-all)
-  int32_t scoring;    // 1 if the clause contributes to the score (MUST / SHOULD)
-  float ub;           // term clauses: largest score of any posting of the list (index-time max of tf*cache[norm])
-  int32_t plane;      // term clauses: dense tf plane of the term (DevIndexView::dense_tf), -1 if the term has none
-  int32_t gran_row;   // term clauses: row of the index-time granule offset table (DevIndexView::gran_tab), -1 if none
-  int32_t pad_;
-  int64_t lo, hi;
-};
-
-struct DevQuery {
-  int32_t clause_begin, n_clauses;
-  int32_t n_term;          // number of term clauses (= slots used)
-  int32_t n_req;           // MUST + FILTER clauses (all kinds)
-  int32_t need_should;     // minimum matching SHOULD clauses
-  int32_t msm;             // minimumNumberShouldMatch as given
-  uint32_t req_term_mask;  // bit s set: term slot s is MUST/FILTER
-  uint32_t not_term_mask;  // bit s set: term slot s is MUST_NOT
-  uint32_t driver_mask;    // bit s set: term slot s drives pass 2
-  int32_t dense_driver;    // 1: iterate every doc of the window instead of driver postings
-  int32_t has_non_driver;  // 1: some term slot is not a driver (pass 3 needed)
-  int32_t has_nonterm;     // 1: range / match-all clauses present
-  int32_t empty;           // 1: can match nothing
-  int32_t has_after;
-  uint32_t must_term_mask;    // bit s set: term slot s is MUST (scores into the required sum)
-  uint32_t should_term_mask;  // bit s set: term slot s is SHOULD
-  int32_t nonterm_scoring;    // 1: a range / match-all clause is MUST or SHOULD (contributes a constant score)
-  int32_t single_field;       // >= 0: every term clause reads this text field's norms; -1: mixed
-  uint64_t after_key;
-};
 
 struct DevIndexView {
   int32_t n_docs;
@@ -278,8 +236,8 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) 
       int c = i >> 8;
       if (sm.cl[c].kind == NRTGPU_TERM) sm.cache[sm.cl[c].slot][i & 255] = L.ix.caches[sm.cl[c].field * 256 + (i & 255)];
     }
-    const int32_t slice_base = slice * (kSliceWindows * kWindowDocs);
-    int32_t slice_end = slice_base + kSliceWindows * kWindowDocs;
+    const int32_t slice_base = slice * kWideSliceDocs;
+    int32_t slice_end = slice_base + kWideSliceDocs;
     if (slice_end > L.ix.n_docs || slice_end < 0) slice_end = L.ix.n_docs;
     const int nwin = (slice_end - slice_base + kWindowDocs - 1) / kWindowDocs;
     // posting bounds of every term clause at every window boundary (lower_bound over the full list)

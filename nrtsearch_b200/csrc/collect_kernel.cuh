@@ -144,7 +144,6 @@ struct AggSpecDev {
   unsigned int* counts;        // terms: [nq][n_buckets]
   unsigned long long* dvals;   // min / max: ordered-double bits [nq]; sum: double bits [nq] (atomicAdd(double))
 };
-constexpr int kMaxAggs = 8;
 struct AggLaunch {
   AggSpecDev a[kMaxAggs];
   int32_t n_aggs;
@@ -195,7 +194,6 @@ struct AggTermsLaunch {
   int32_t* out_total_buckets; // [nq] non-empty buckets
   long long* out_other;       // [nq] docs counted in buckets not returned
 };
-constexpr int kAggChunk = 2048;
 __global__ void __launch_bounds__(256) agg_terms_topk_kernel(AggTermsLaunch T) {
   __shared__ uint64_t keys[2 * kAggChunk];
   __shared__ unsigned long long sh_sum;

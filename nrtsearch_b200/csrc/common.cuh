@@ -3,12 +3,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string>
+#include "batch_plan.h"
 
 namespace nrtgpu {
 
-// ---- error plumbing (thread-local message, returned through nrtgpu_last_error) ----
-void set_error(const std::string& msg);
-#define NRT_CUDA_TRY(expr)                                                                   \
+#define NRT_CUDA_TRY(expr)                                                                  \
   do {                                                                                       \
     cudaError_t _e = (expr);                                                                 \
     if (_e != cudaSuccess) {                                                                 \
@@ -16,31 +15,6 @@ void set_error(const std::string& msg);
       return (_e == cudaErrorMemoryAllocation) ? NRTGPU_ERR_OOM : NRTGPU_ERR_CUDA;           \
     }                                                                                        \
   } while (0)
-
-// ---- total order on hits: (score desc, doc asc)  <=>  key desc ----
-// reference: src/main/java/org/apache/lucene/search/LazyQueueTopScoreDocCollector.java:129-143
-// key = ordered(score) << 32 | ~doc ; all keys of real hits are > 0, so 0 is the "empty" sentinel.
-__host__ __device__ __forceinline__ uint32_t float_to_ordered(float f) {
-#ifdef __CUDA_ARCH__
-  uint32_t b = __float_as_uint(f);
-#else
-  union { float f; uint32_t u; } c; c.f = f; uint32_t b = c.u;
-#endif
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__host__ __device__ __forceinline__ float ordered_to_float(uint32_t u) {
-  uint32_t b = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
-#ifdef __CUDA_ARCH__
-  return __uint_as_float(b);
-#else
-  union { float f; uint32_t u; } c; c.u = b; return c.f;
-#endif
-}
-__host__ __device__ __forceinline__ uint64_t make_key(float score, int32_t doc) {
-  return ((uint64_t)float_to_ordered(score) << 32) | (uint32_t)(~(uint32_t)doc);
-}
-__host__ __device__ __forceinline__ float key_score(uint64_t k) { return ordered_to_float((uint32_t)(k >> 32)); }
-__host__ __device__ __forceinline__ int32_t key_doc(uint64_t k) { return (int32_t)(~(uint32_t)k); }
 
 #ifdef __CUDACC__
 // BM25 term score exactly as Lucene's BM25Scorer.score (float ops, round-to-nearest, never fused):

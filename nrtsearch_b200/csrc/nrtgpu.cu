@@ -21,16 +21,15 @@
 #include <cstring>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <vector>
 
 namespace nrtgpu {
 static thread_local std::string g_last_error;
 void set_error(const std::string& msg) { g_last_error = msg; }
 }  // namespace nrtgpu
+#include "batch_plan.inc"
 using namespace nrtgpu;
-
-#define NRT_FAIL(code, msg) do { set_error(msg); return (code); } while (0)
-
 
 // index-time impacts: max over a term's postings of x = tf * cache[norm] (what Lucene keeps as competitive (freq, norm)
 // pairs in its skip data); the BM25 score is monotone in x, so score(weight, max x) bounds the whole list.
@@ -99,30 +98,6 @@ __global__ void gran_table_kernel(GranTabLaunch G) {
 
 namespace {
 
-// ---- SmallFloat.byte4ToInt (Lucene) : norm byte -> field length, for the BM25 length table ----
-int64_t int4_to_long(int i) {
-  int64_t bits = i & 0x07;
-  int shift = (i >> 3) - 1;
-  return shift == -1 ? bits : ((bits | 0x08) << shift);
-}
-int32_t byte4_to_int(uint8_t b) {
-  const int kFree = 24;  // 255 - longToInt4(Integer.MAX_VALUE)
-  return b < kFree ? (int32_t)b : (int32_t)(kFree + int4_to_long((int)b - kFree));
-}
-// BM25Similarity.scorer(): cache[i] = 1f / (k1 * ((1 - b) + b * LENGTH_TABLE[i] / avgdl)), float ops
-void bm25_cache(float k1, float b, float avgdl, float* cache) {
-  for (int i = 0; i < 256; ++i) {
-    volatile float t = b * (float)byte4_to_int((uint8_t)i);
-    t = t / avgdl;
-    t = (1.0f - b) + t;
-    t = k1 * t;
-    cache[i] = 1.0f / t;
-  }
-}
-float bm25_idf(int64_t df, int64_t doc_count) {
-  return (float)std::log(1.0 + ((double)doc_count - (double)df + 0.5) / ((double)df + 0.5));
-}
-
 template <typename T>
 struct DevBuf {
   T* p = nullptr;
@@ -155,15 +130,10 @@ struct DevBuf {
 
 struct nrtgpu_ctx {
   int device = 0;
-  int sm_count = 0;
   std::mutex hyb_mu;             // O(k) hybrid stages share one pooled device scratch (no cudaMalloc per call)
   DevBuf<int32_t> hyb_scratch;
-  int64_t item_postings = 32768; // NRTGPU_ITEM_POSTINGS: floor of the postings a (query, slice) may hold before it is split into 2..16 parts
-  int64_t item_share_full = 32;  // NRTGPU_ITEM_SHARE_FULL: the same for launches that visit every posting (ScoreMode.COMPLETE, generic clause evaluation)
-  int64_t item_share = 12;       // NRTGPU_ITEM_SHARE: ... and it is split when it exceeds 1/share of the postings per resident CTA
-  int64_t warm_min_docs = 8ll * v3::kWarmGran * v3::kGran;   // NRTGPU_WARM_MIN_DOCS: shards below this size run without warm-up items
-  int slice_gran = 512;          // NRTGPU_SLICE_GRAN: granules (1024 docs) per slice of the probe kernel, <= v3::kMaxSliceGran
-  int probe_cfg = 0;             // NRTGPU_PROBE_CFG: 0 auto, 1 always A (3 CTAs / SM), 2 always B (4 CTAs / SM)
+  PlanKnobs plan;                // the work planner's knobs, with the device's SM count
+  int probe_cfg = 0;            // NRTGPU_PROBE_CFG: 0 auto, 1 always A (3 CTAs / SM), 2 always B (4 CTAs / SM)
   bool debug_modes = false;     // NRTGPU_DEBUG_MODES=1: per-launch kernel statistics on stderr (adds a stream synchronisation)
 };
 
@@ -250,6 +220,14 @@ struct nrtgpu_index {
     v.gran_tab = gran_tab.p; v.n_gran = gran_n;
     return v;
   }
+  PlanDict dict() const {   // what batch compilation and planning read
+    PlanDict d;
+    d.n_docs = n_docs; d.doc_base = doc_base; d.n_terms = n_terms; d.n_columns = n_columns;
+    d.term_off = term_off.data(); d.term_field = term_field.data(); d.term_df = term_df.data(); d.term_max_x = term_max_x.data();
+    d.term_plane = term_plane.data(); d.term_gran = term_gran.data(); d.field_doc_count = field_doc_count.data();
+    d.col_multi = col_multi.data(); d.col_n_distinct = col_n_distinct.data(); d.has_deletes = live_bits.p != nullptr;
+    return d;
+  }
 };
 
 // a Sort of several fields ranked over one image (sort_kernel.cuh, sort_order_build)
@@ -263,20 +241,14 @@ struct nrtgpu_sort_order {
   DevBuf<uint32_t> rank;                // doc -> position + 1
 };
 
-struct nrtgpu_batch;
-static void free_batch(nrtgpu_batch* b);
 struct nrtgpu_batch {
   nrtgpu_index* ix = nullptr;
-  int32_t nq = 0, top_k = 0, n_slices = 0, n_work = 0;
-  int32_t n_lists = 0;         // per-query candidate lists the kernels fill: n_slices * parts_max (+1: the warm-up items' list)
-  // work list layout of a probe batch: [probe simple | probe generic]
-  int32_t n_probe_simple = 0, n_probe_generic = 0;
+  int32_t nq = 0, top_k = 0;
+  CompiledBatch cb;            // host copies the async uploads read, kept until the next compilation
+  WorkPlan plan;               // (search batches only)
   DevBuf<uint32_t> sbounds;            // probe kernel: [nq][4][n_slices * parts_max + 2] part-boundary posting offsets
   DevBuf<unsigned int> work_counter;   // probe kernel: queue heads [2]
   DevBuf<unsigned long long> probe_stats;
-  bool wide_slots = false;     // more than 4 term clauses or top_k > 512: bool_window_kernel runs the whole batch
-  bool exhaustive = true;
-  int64_t alg_postings = 0;
   DevBuf<DevClause> clauses;
   DevBuf<DevQuery> queries;
   DevBuf<int32_t> work_query, work_slice;
@@ -292,8 +264,7 @@ struct nrtgpu_batch {
   DevBuf<int64_t> out_sort_values;
   std::vector<int32_t> h_after_docs;
   const nrtgpu_sort_order* order = nullptr;   // nrtgpu_search_sorted_fields: the Sort's order (sort_kind COLUMN or kSortScoreRank)
-  // additional collectors (aggregations)
-  std::vector<nrtgpu_aggregation> aggs;
+  // additional collectors (aggregations, cb.aggs)
   DevBuf<unsigned int> agg_counts[kMaxAggs];
   DevBuf<unsigned long long> agg_dvals[kMaxAggs];
   DevBuf<AggLaunch> agg_launch;
@@ -305,13 +276,7 @@ struct nrtgpu_batch {
   long long deadline_ns = 0;       // budget from the first work item on (0: none)
   int64_t ta_scalar = 0;           // terminateAfter (0: none)
   int64_t terminate_after_max_recall = 0;
-  std::vector<DevClause> h_dc; std::vector<DevQuery> h_dq; std::vector<int32_t> h_wq, h_ws;   // host copies the async uploads read
-  int32_t slice_docs = 0;
-  DevBuf<unsigned long long> known_hits;        // probe kernel: docs known to match per query (0: unknown)
-  std::vector<unsigned long long> h_known;
-  int32_t parts_max = 1;       // probe kernel: parts a (query, slice) work item may be split into (power of two)
-  int64_t threshold = INT32_MAX;
-  int32_t n_gran = 0;
+  DevBuf<unsigned long long> known_hits;        // probe kernel: plan.known_hits
   DevBuf<uint64_t> theta;
   DevBuf<unsigned long long> total_hits;
   DevBuf<uint64_t> slice_keys;
@@ -329,10 +294,9 @@ struct nrtgpu_batch {
   int32_t* o_docs() { return bound_docs ? bound_docs : out_docs.p; }
   float* o_scores() { return bound_scores ? bound_scores : out_scores.p; }
   int32_t* o_counts() { return bound_counts ? bound_counts : out_counts.p; }
+  void unbind() { bound_docs = nullptr; bound_scores = nullptr; bound_counts = nullptr; bound_total = nullptr; bound_flags = nullptr; }
   ~nrtgpu_batch() { for (auto& r : ev) for (auto& e : r) if (e) cudaEventDestroy(e); }
 };
-
-static void free_batch(nrtgpu_batch* b) { delete b; }
 
 // index-time impacts: max over a term's postings of tf * cache[norm]; depends on the index-wide avgdl through cache[]
 static int compute_term_max_x(nrtgpu_index* ix) {
@@ -359,14 +323,8 @@ static int upload_live_docs(nrtgpu_index* ix, const uint8_t* live_docs) {
   for (int32_t i = 0; i < ix->n_docs; ++i) if (live_docs[i]) bits[(size_t)i >> 5] |= 1u << (i & 31);
   return ix->live_bits.upload(bits.data(), bits.size());
 }
-extern "C" {
-static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggregation_result* out);
-static int batch_set_limits(nrtgpu_batch* b, const nrtgpu_search_limits* lim, cudaStream_t st);
-static int batch_fetch_impl(nrtgpu_batch* b, void* stream_, int32_t* out_docs, float* out_scores, int32_t* out_counts,
-                            int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout, uint8_t* out_terminated_early);
-}
 nrtgpu_index::~nrtgpu_index() {
-  for (auto* b : ws_free) free_batch(b);
+  for (auto* b : ws_free) delete b;
   for (auto e : knn_ev) if (e) cudaEventDestroy(e);
 }
 
@@ -389,14 +347,14 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   if (prop.major != 9 || prop.minor != 0) NRT_FAIL(NRTGPU_ERR_CUDA, "nrtgpu_init: device is not sm_90 (kernels are built for sm_90a only)");
   std::unique_ptr<nrtgpu_ctx> c(new nrtgpu_ctx);   // released to the caller only when every attribute call succeeded
   c->device = device_id;
-  c->sm_count = prop.multiProcessorCount;
+  c->plan.sm_count = prop.multiProcessorCount;
   c->debug_modes = getenv("NRTGPU_DEBUG_MODES") != nullptr;
   { const char* e = getenv("NRTGPU_PROBE_CFG"); c->probe_cfg = e ? atoi(e) : 0; }
-  { const char* e = getenv("NRTGPU_WARM_MIN_DOCS"); if (e && atoll(e) > 0) c->warm_min_docs = atoll(e); }
-  { const char* e = getenv("NRTGPU_SLICE_GRAN"); if (e && atoi(e) >= 64) c->slice_gran = std::min(atoi(e), (int)v3::kMaxSliceGran); }
-  { const char* e = getenv("NRTGPU_ITEM_POSTINGS"); if (e && atoll(e) > 0) c->item_postings = atoll(e); }
-  { const char* e = getenv("NRTGPU_ITEM_SHARE"); if (e && atoll(e) > 0) c->item_share = atoll(e); }
-  { const char* e = getenv("NRTGPU_ITEM_SHARE_FULL"); if (e && atoll(e) > 0) c->item_share_full = atoll(e); }
+  { const char* e = getenv("NRTGPU_WARM_MIN_DOCS"); if (e && atoll(e) > 0) c->plan.warm_min_docs = atoll(e); }
+  { const char* e = getenv("NRTGPU_SLICE_GRAN"); if (e && atoi(e) >= 64) c->plan.slice_gran = std::min(atoi(e), (int)v3::kMaxSliceGran); }
+  { const char* e = getenv("NRTGPU_ITEM_POSTINGS"); if (e && atoll(e) > 0) c->plan.item_postings = atoll(e); }
+  { const char* e = getenv("NRTGPU_ITEM_SHARE"); if (e && atoll(e) > 0) c->plan.item_share = atoll(e); }
+  { const char* e = getenv("NRTGPU_ITEM_SHARE_FULL"); if (e && atoll(e) > 0) c->plan.item_share_full = atoll(e); }
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
 #define NRT_PROBE_ATTR(S, D) \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasA, v3::kStageA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageA>))); \
@@ -471,21 +429,10 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
     if ((rc = ix->exc_pos.upload(epos.data(), epos.size()))) return rc;
     if ((rc = ix->exc_freq.upload(efreq.data(), efreq.size()))) return rc;
   }
-  // dense tf planes: a term present in >= 1/64 of the docs also gets a direct-address byte per doc (like the bit-set
-  // blocks Lucene's postings format keeps for dense blocks). A list that only needs LOOKUPS in a window (a
-  // non-essential MAXSCORE list) is then one TMA copy of the window's bytes instead of a scatter of its postings.
-  ix->term_plane.assign((size_t)d->n_terms, -1);
-  if (d->n_docs >= 4096) {
+  // dense tf planes (plan_planes)
+  {
     std::vector<int32_t> dense_terms;
-    for (int32_t t = 0; t < d->n_terms; ++t)
-      if ((d->term_off[t + 1] - d->term_off[t]) * 64 >= (int64_t)d->n_docs) dense_terms.push_back(t);
-    const int64_t stride = (((int64_t)d->n_docs + 15) / 16) * 16 + 16;
-    const size_t max_planes = std::min<size_t>(1024, (size_t)((8ll << 30) / stride));
-    if (dense_terms.size() > max_planes) {   // keep the densest
-      std::sort(dense_terms.begin(), dense_terms.end(), [&](int32_t a, int32_t b) {
-        return d->term_off[a + 1] - d->term_off[a] > d->term_off[b + 1] - d->term_off[b]; });
-      dense_terms.resize(max_planes);
-    }
+    const int64_t stride = plan_planes(d->n_docs, d->n_terms, d->term_off, ix->term_plane, dense_terms);
     if (!dense_terms.empty()) {
       ix->dense_stride = stride; ix->n_planes = (int32_t)dense_terms.size();
       if ((rc = ix->dense_tf.alloc((size_t)stride * dense_terms.size()))) return rc;
@@ -493,7 +440,6 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
       for (size_t k = 0; k < dense_terms.size(); ++k) {
         const int32_t t = dense_terms[k];
         const int64_t off = d->term_off[t], n = d->term_off[t + 1] - off;
-        ix->term_plane[(size_t)t] = (int32_t)k;
         plane_fill_kernel<<<(unsigned)((n + 255) / 256), 256>>>(ix->post_docs.p + off, ix->post_f8.p + off, n,
                                                                  ix->dense_tf.p + (size_t)k * stride);
       }
@@ -504,17 +450,10 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
       NRT_CUDA_TRY(cudaGetLastError());
     }
   }
-  // skip data: posting offsets at every 1024-doc granule boundary for the lists long enough to make the per-batch
-  // lower_bound searches expensive (>= 4096 postings); a batch then copies the row instead of searching
-  ix->term_gran.assign((size_t)d->n_terms, -1);
+  // skip data (plan_gran_rows)
   {
-    const int32_t n_gran = std::max<int32_t>(1, (int32_t)(((int64_t)d->n_docs + v3::kGran - 1) / v3::kGran));
     std::vector<int64_t> row_off; std::vector<int32_t> row_n;
-    const size_t max_rows = (size_t)((2ll << 30) / ((int64_t)(n_gran + 1) * 4));
-    for (int32_t t = 0; t < d->n_terms && row_off.size() < max_rows; ++t) {
-      const int64_t n = d->term_off[t + 1] - d->term_off[t];
-      if (n >= 4096) { ix->term_gran[(size_t)t] = (int32_t)row_off.size(); row_off.push_back(d->term_off[t]); row_n.push_back((int32_t)n); }
-    }
+    const int32_t n_gran = plan_gran_rows(d->n_docs, d->n_terms, d->term_off, ix->term_gran, row_off, row_n);
     ix->gran_n = n_gran;
     if (!row_off.empty()) {
       DevBuf<int64_t> d_ro; DevBuf<int32_t> d_rn;
@@ -712,306 +651,53 @@ int nrtgpu_index_update_stats(nrtgpu_index* ix, const int64_t* term_df, const in
   return compute_term_max_x(ix);   // the impacts are functions of the length cache
 }
 
-// ---- batch compilation: flat BooleanQuery -> DevQuery/DevClause, driver selection, work list ----
-// compile + upload a batch into `b` (buffers are reused when large enough); asynchronous on `st`
-static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
-                       const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold,
-                       int32_t flags, cudaStream_t st, const nrtgpu_sort* sort = nullptr, const nrtgpu_aggregation* aggs = nullptr,
-                       int32_t n_aggs = 0, const nrtgpu_sort_order* sort_order = nullptr, const int64_t* order_after = nullptr) {
-  if (!ix || !queries || (n_clauses > 0 && !clauses)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: NULL argument");
-  b->aggs.clear();
+// ---- batch compilation (batch_plan.inc) + uploads ----
+// compile the request and upload its clauses and queries into `b` (buffers are reused when large enough); asynchronous
+// on `st`. What the compile-only entry points need (nrtgpu_score_docs, nrtgpu_rescore_query, nrtgpu_search_knn_filtered).
+static int batch_compile(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r, cudaStream_t st) {
+  if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: NULL argument");
+  int rc;
+  if ((rc = compile_batch(ix->dict(), r, &b->cb))) return rc;
+  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
+  b->ix = ix; b->nq = r.nq; b->top_k = r.top_k;
+  if ((rc = b->clauses.upload_async(b->cb.clauses.data(), b->cb.clauses.size(), st))) return rc;
+  return b->queries.upload_async(b->cb.queries.data(), b->cb.queries.size(), st);
+}
+
+// a search batch: compile, plan the work list, upload, set up sorted searchAfter, allocate the results and launch
+// slice_bounds_kernel
+static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r, cudaStream_t st) {
+  int rc;
+  if ((rc = batch_compile(b, ix, r, st))) return rc;
+  const nrtgpu_sort* sort = r.sort;
+  const nrtgpu_sort_order* sort_order = r.sort_order;
+  const int32_t nq = r.nq, top_k = r.top_k;
   b->order = sort_order;
-  if (n_aggs > 0) {
-    if (!aggs || n_aggs > kMaxAggs) NRT_FAIL(NRTGPU_ERR_INVALID, "at most 8 aggregations per search");
-    for (int i = 0; i < n_aggs; ++i) {
-      const nrtgpu_aggregation& a = aggs[i];
-      if (a.kind < NRTGPU_AGG_TERMS || a.kind > NRTGPU_AGG_SUM) NRT_FAIL(NRTGPU_ERR_INVALID, "bad aggregation kind");
-      if (!ix || a.column < 0 || a.column >= ix->n_columns) NRT_FAIL(NRTGPU_ERR_INVALID, "aggregation column out of range");
-      if (a.value_type < 0 || a.value_type > 2) NRT_FAIL(NRTGPU_ERR_INVALID, "bad aggregation value_type");
-      if (ix->col_multi[(size_t)a.column]) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "aggregation on a multi-valued column");
-      if (a.kind == NRTGPU_AGG_TERMS) {
-        if (a.size <= 0 || a.size > kAggChunk) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "terms aggregation: size must be in [1, 2048]");
-        const int64_t cells = (int64_t)nq * ix->col_n_distinct[(size_t)a.column];
-        if (cells * 4 > (2ll << 30)) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "terms aggregation: batch x distinct values exceeds the 2 GB count table");
-      }
-      b->aggs.push_back(a);
-    }
-    total_hits_threshold = INT32_MAX;   // RelevanceCollector.java:55-62: additional collectors force exact collection
-  }
-  const bool sorted = (sort && sort->kind != NRTGPU_SORT_RELEVANCE) || sort_order;
+  b->ran = false; b->runs_recorded = 0;
   if (sort_order) {   // fields-only order: the COLUMN key with the rank as its code; [score, ...]: kSortScoreRank
     b->sort_kind = sort_order->score_first ? kSortScoreRank : NRTGPU_SORT_COLUMN; b->sort_column = 0;
     b->sort_reverse = sort_order->score_first ? sort_order->score_reverse : 0; b->sort_missing_value = 0;
   } else {
+    const bool sorted = b->cb.sorted;
     b->sort_kind = sorted ? sort->kind : 0; b->sort_column = sorted ? sort->column : 0; b->sort_reverse = sorted ? (sort->reverse != 0) : 0;
     b->sort_missing_value = sorted ? sort->missing_value : 0;
   }
-  if (sorted) {
-    if (!sort_order && sort->kind != NRTGPU_SORT_COLUMN && sort->kind != NRTGPU_SORT_DOCID) NRT_FAIL(NRTGPU_ERR_INVALID, "bad sort kind");
-    if (!sort_order && sort->kind == NRTGPU_SORT_COLUMN && (sort->column < 0 || sort->column >= ix->n_columns))
-      NRT_FAIL(NRTGPU_ERR_INVALID, "sort column out of range (field does not support sorting: no doc values)");
-    if (!sort_order && sort->kind == NRTGPU_SORT_COLUMN && ix->col_multi[(size_t)sort->column]) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "sort on a multi-valued column");
-    total_hits_threshold = INT32_MAX;   // every match is visited: exact totalHits
-  }
-  if (nq <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: nq must be > 0");
-  // LazyQueueTopScoreDocCollectorManager.java:93-96: numHits must be > 0
-  if (top_k <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "numHits must be > 0; please use TotalHitCountCollectorManager if you just need the total hit count");
-  if (top_k > kMaxTopK) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nrtgpu_batch_prepare: top_k > 1024 is not on the GPU path");
-  if (total_hits_threshold < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "totalHitsThreshold must be >= 0");
-  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
-  b->ix = ix; b->nq = nq; b->top_k = top_k;
-  b->alg_postings = 0; b->ran = false; b->runs_recorded = 0;
-  // LazyQueueTopScoreDocCollectorManager.java:102: totalHitsThreshold = max(totalHitsThreshold, numHits);
-  // Integer.MAX_VALUE <=> ScoreMode.COMPLETE (LazyQueueTopScoreDocCollector.java:68-70): exact counts, no list skipping
-  b->threshold = (total_hits_threshold == INT32_MAX || (flags & NRTGPU_FLAG_NO_PRUNING))
-                     ? (int64_t)INT32_MAX : (int64_t)std::max(total_hits_threshold, top_k);
-  b->exhaustive = b->threshold == (int64_t)INT32_MAX;
-  // slice size depends on the kernel: decided after the clauses are known (wide queries / large top_k -> bool_window_kernel)
-  int64_t slice_docs = (int64_t)kSliceWindows * kWindowDocs;
-  std::vector<DevClause> dc;
-  std::vector<DevQuery> dq((size_t)nq);
-  dc.reserve((size_t)n_clauses);
-  int max_terms = 0;
-  for (int qi = 0; qi < nq; ++qi) {
-    const nrtgpu_query& q = queries[qi];
-    if (q.clause_begin < 0 || q.clause_end < q.clause_begin || q.clause_end > n_clauses)
-      NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: clause range out of bounds");
-    if (q.min_should_match < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "minimumNumberShouldMatch must be >= 0");
-    int ncl = q.clause_end - q.clause_begin;
-    if (ncl > kMaxClauses) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nrtgpu_batch_prepare: more than 16 clauses in one BooleanQuery");
-    DevQuery& o = dq[(size_t)qi];
-    std::memset(&o, 0, sizeof(o));
-    o.clause_begin = (int32_t)dc.size(); o.n_clauses = ncl; o.msm = q.min_should_match;
-    int n_term = 0, n_req = 0, n_should = 0, n_req_term = 0, n_req_nonterm = 0, n_should_nonterm = 0;
-    int best_req_slot = -1; int32_t best_req_n = INT32_MAX;
-    uint32_t should_term_mask = 0;
-    int field0 = -2;   // -2: no term yet, -1: mixed
-    for (int ci = q.clause_begin; ci < q.clause_end; ++ci) {
-      const nrtgpu_clause& c = clauses[ci];
-      if (c.occur < NRTGPU_SHOULD || c.occur > NRTGPU_MUST_NOT) NRT_FAIL(NRTGPU_ERR_INVALID, "bad occur");
-      // QueryNodeMapper.java:127-133: the reference rejects boost < 0 with exactly this message and treats the proto default 0 as
-      // "no boost"; the adaptor folds that rule before it fills the clause, so 0 here is a weight of 0, not an error
-      if (c.boost < 0.0f) NRT_FAIL(NRTGPU_ERR_INVALID, "Boost must be a positive number");
-      DevClause x; std::memset(&x, 0, sizeof(x));
-      x.occur = c.occur; x.kind = c.kind; x.slot = -1; x.plane = -1; x.gran_row = -1; x.lo = c.lo; x.hi = c.hi;
-      x.scoring = (c.occur == NRTGPU_MUST || c.occur == NRTGPU_SHOULD) ? 1 : 0;
-      bool required = (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER);
-      if (c.kind == NRTGPU_TERM) {
-        if (c.id < 0 || c.id >= ix->n_terms) NRT_FAIL(NRTGPU_ERR_INVALID, "term id out of range");
-        if (n_term >= kMaxTermSlots) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nrtgpu_batch_prepare: more than 8 term clauses in one BooleanQuery");
-        int f = ix->term_field[c.id];
-        x.post_base = ix->term_off[c.id];
-        x.n_post = (int32_t)(ix->term_off[c.id + 1] - ix->term_off[c.id]);
-        x.slot = n_term; x.field = f; x.plane = ix->term_plane[c.id]; x.gran_row = ix->term_gran[c.id];
-        int64_t df = ix->term_df[c.id];
-        // BM25Scorer: weight = boost * idf
-        x.weight = c.boost * bm25_idf(df > 0 ? df : 1, ix->field_doc_count[f]);
-        {
-          volatile float t1 = 1.0f + ix->term_max_x[c.id];
-          volatile float t2 = x.weight / t1;
-          x.ub = x.weight - t2;
-        }
-        if (required) { o.req_term_mask |= 1u << n_term; ++n_req_term; if (x.n_post < best_req_n) { best_req_n = x.n_post; best_req_slot = n_term; } }
-        if (c.occur == NRTGPU_MUST_NOT) o.not_term_mask |= 1u << n_term;
-        if (c.occur == NRTGPU_SHOULD) should_term_mask |= 1u << n_term;
-        if (c.occur == NRTGPU_MUST) o.must_term_mask |= 1u << n_term;
-        if (x.scoring) field0 = (field0 == -2 || field0 == f) ? f : -1;
-        b->alg_postings += x.n_post;
-        ++n_term;
-      } else if (c.kind == NRTGPU_RANGE_I64) {
-        if (c.id < 0 || c.id >= ix->n_columns) NRT_FAIL(NRTGPU_ERR_INVALID, "column id out of range");
-        x.col = c.id; x.weight = c.boost;  // constant-score query: score = boost
-        o.has_nonterm = 1;
-        if (x.scoring) o.nonterm_scoring = 1;
-        if (required) ++n_req_nonterm;
-        if (c.occur == NRTGPU_SHOULD) ++n_should_nonterm;
-      } else if (c.kind == NRTGPU_MATCH_ALL) {
-        x.weight = c.boost;
-        o.has_nonterm = 1;
-        if (x.scoring) o.nonterm_scoring = 1;
-        if (required) ++n_req_nonterm;
-        if (c.occur == NRTGPU_SHOULD) ++n_should_nonterm;
-      } else NRT_FAIL(NRTGPU_ERR_INVALID, "bad clause kind");
-      if (required) ++n_req;
-      if (c.occur == NRTGPU_SHOULD) ++n_should;
-      dc.push_back(x);
-    }
-    o.n_term = n_term; o.n_req = n_req;
-    o.should_term_mask = should_term_mask;
-    o.single_field = field0 == -2 ? 0 : field0;
-    o.need_should = q.min_should_match > 0 ? q.min_should_match : (n_req == 0 ? 1 : 0);
-    max_terms = std::max(max_terms, n_term);
-    if (q.min_should_match > n_should || (n_req == 0 && n_should == 0)) o.empty = 1;
-    // driver selection
-    if (n_req_term > 0) o.driver_mask = 1u << best_req_slot;           // rarest required posting list leads
-    else if (n_req_nonterm > 0 || n_should_nonterm > 0) o.dense_driver = 1;  // no posting list can lead
-    else o.driver_mask = should_term_mask;                             // pure disjunction: every SHOULD list drives
-    uint32_t all_terms = n_term >= 32 ? 0xffffffffu : ((1u << n_term) - 1u);
-    o.has_non_driver = (!o.dense_driver && (all_terms & ~o.driver_mask)) ? 1 : 0;
-    if (q.has_after && sorted) o.has_after = 1;   // after_key is patched on the device (sort_after_kernel)
-    else if (q.has_after) {
-      o.has_after = 1;
-      int64_t local = (int64_t)q.after_doc - ix->doc_base;
-      uint32_t ord = float_to_ordered(q.after_score);
-      if (local < 0) o.after_key = ((uint64_t)ord + 1ull) << 32;             // every doc here follows afterDoc
-      else if (local >= ix->n_docs) o.after_key = make_key(q.after_score, INT32_MAX);  // every doc here precedes it
-      else o.after_key = make_key(q.after_score, (int32_t)local);
-    }
-  }
-  b->wide_slots = max_terms > 4 || top_k > v3::kMaxTopK;
-  if (n_aggs > 0 && b->wide_slots) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "aggregations: more than 4 term clauses or top_k > 512 is not on the GPU path");
-  if (sorted && b->wide_slots) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "sorted search: more than 4 term clauses or top_k > 512 is not on the GPU path");
-  if (!b->wide_slots) {
-    // slices of equal size, a multiple of the 1024-doc granule, at most 512K docs: a 1.25M-doc shard is 3 x 417K, not 2.38 -> 3 x 512K
-    // (probe kernel: slices of up to slice_gran granules -- NRTGPU_SLICE_GRAN, default and maximum 512: the MAXSCORE roles of an
-    //  item are fixed when it starts, so larger slices prune with staler thresholds -- measured slower -- and smaller ones pay
-    //  the per-item set-up more often)
-    const int64_t max_slice_docs = (int64_t)ix->ctx->slice_gran * v3::kGran;
-    const int64_t n_sl = std::max<int64_t>(1, ((int64_t)ix->n_docs + max_slice_docs - 1) / max_slice_docs);
-    slice_docs = (((int64_t)ix->n_docs + n_sl - 1) / n_sl + v3::kGran - 1) / v3::kGran * v3::kGran;
-    if (slice_docs < v3::kGran) slice_docs = v3::kGran;
-  }
-  b->slice_docs = (int32_t)slice_docs;
-  b->n_slices = (int32_t)std::max<int64_t>(1, ((int64_t)ix->n_docs + slice_docs - 1) / slice_docs);
-  // work list, slice-major so that concurrently resident CTAs share postings of the same doc range in L2;
-  // inside a slice, longer queries first
-  std::vector<int32_t> order;
-  std::vector<int64_t> cost((size_t)nq, 0);
-  for (int qi = 0; qi < nq; ++qi) {
-    if (dq[qi].empty) continue;
-    order.push_back(qi);
-    for (int c = 0; c < dq[qi].n_clauses; ++c) cost[qi] += dc[(size_t)dq[qi].clause_begin + c].n_post;
-    if (dq[qi].dense_driver) cost[qi] += ix->n_docs;
-  }
-  std::stable_sort(order.begin(), order.end(), [&](int a, int c) { return cost[a] > cost[c]; });
-  if (!b->wide_slots) {
-    // probe kernel: inside a slice, queries that share their densest tf plane are adjacent in the queue, so the plane's
-    // bytes of the slice are gathered by CTAs that run together and stay in L2 between them (longer queries first inside
-    // a cluster, clusters of the densest -- most shared -- planes first)
-    std::vector<int64_t> ckey((size_t)nq, INT64_MAX);
-    for (int qi : order) {
-      int64_t best_n = -1;
-      for (int c = 0; c < dq[qi].n_clauses; ++c) {
-        const DevClause& x = dc[(size_t)dq[qi].clause_begin + c];
-        if (x.kind == NRTGPU_TERM && x.plane >= 0 && x.n_post > best_n) { best_n = x.n_post; ckey[(size_t)qi] = ((int64_t)(INT32_MAX - x.n_post) << 32) | (uint32_t)x.plane; }
-      }
-    }
-    std::stable_sort(order.begin(), order.end(), [&](int a, int c) { return ckey[(size_t)a] < ckey[(size_t)c]; });
-  }
-  // pure disjunctions of scoring term clauses over one text field run in their own probe kernel instantiation
-  // (tf-pattern bound, deferred scoring, MAXSCORE): their work items come first. A wide batch (one launch) orders its
-  // work items the same way, but only on a shard without deletes.
-  auto is_simple = [&](int qi) {
-    const DevQuery& o = dq[(size_t)qi];
-    return !sorted && n_aggs == 0 && o.single_field >= 0 && !o.has_nonterm && !o.nonterm_scoring && (!b->wide_slots || ix->live_bits.p == nullptr) && o.n_req == 0 &&
-           o.not_term_mask == 0 && o.msm <= 1 && !o.dense_driver;
-  };
-  std::vector<int32_t>& wq = b->h_wq; std::vector<int32_t>& ws = b->h_ws;
-  wq.clear(); ws.clear();
-  // warm-up items (large shards): a query first sweeps the leading kWarmGran granules of slice 0 as a work item of its
-  // own, ahead of everything else, so that its other work items start with a threshold and a hit count (MAXSCORE can
-  // prune from the first slice on). Both score modes, every query whose lists are expected to hold 2 * top_k hits in
-  // those granules.
-  const bool warm_ok = !b->wide_slots && (int64_t)ix->n_docs >= (int64_t)ix->ctx->warm_min_docs;
-  std::vector<uint8_t> has_warm((size_t)nq, 0);
-  // probe kernel, pure disjunctions on a shard without deletes: the longest list is a lower bound of the matching docs
-  // (pruning may start as soon as that exceeds totalHitsThreshold), and the warm-up SWEEPS the first 32K postings of the
-  // highest-bound (rarest) list over the whole shard instead of the first 32K docs (flags 4)
-  b->h_known.assign((size_t)nq, 0ull);
-  if (!b->wide_slots && !ix->live_bits.p && !sorted && n_aggs == 0)
-    for (int qi : order) {
-      if (!is_simple(qi)) continue;
-      int64_t mx = 0;
-      for (int c = 0; c < dq[qi].n_clauses; ++c) mx = std::max<int64_t>(mx, dc[(size_t)dq[qi].clause_begin + c].n_post);
-      b->h_known[(size_t)qi] = (unsigned long long)mx;
-    }
-  if (warm_ok) {
-    for (int qi : order) {
-      if (!is_simple(qi)) continue;
-      // (not with searchAfter: a doc whose LOWER-BOUND key passes the after filter may in truth lie on an earlier page, and
-      //  would be counted towards the k keys that justify the threshold)
-      if (!dq[qi].has_after) {
-        int best = -1; float best_ub = -1.0f;
-        for (int c = 0; c < dq[qi].n_clauses; ++c) {
-          const DevClause& x = dc[(size_t)dq[qi].clause_begin + c];
-          if (x.kind == NRTGPU_TERM && x.ub > best_ub) { best_ub = x.ub; best = c; }
-        }
-        if (best >= 0 && dc[(size_t)dq[qi].clause_begin + best].n_post >= 2 * (int64_t)top_k) {
-          wq.push_back(qi); ws.push_back(0 | (dc[(size_t)dq[qi].clause_begin + best].slot << 16) | (4 << 24));
-          continue;   // (has_warm stays 0: the query's slice-0 items cover the whole slice)
-        }
-      }
-      if (cost[qi] * (int64_t)(v3::kWarmGran * v3::kGran) >= 2ll * top_k * (int64_t)ix->n_docs) has_warm[(size_t)qi] = 1;
-      if (has_warm[(size_t)qi]) { wq.push_back(qi); ws.push_back(0 | (1 << 24)); }
-    }
-  }
-  // heavy (query, slice) pairs are split into 2..16 parts of equal granule ranges, so that no single work item is a
-  // large share of the launch (the longest item bounds the kernel time from below: what limits small shards)
-  const int gran_per_slice = (int)(slice_docs / v3::kGran);
-  const int n_gran_h = std::max<int>(1, (int)(((int64_t)ix->n_docs + v3::kGran - 1) / v3::kGran));
-  std::vector<uint8_t> lparts((size_t)nq, 0);
-  int lp_max = 0;
-  if (!b->wide_slots) {
-    int64_t total_cost = 0;
-    for (int qi : order) total_cost += cost[qi];
-    const int64_t per_cta = total_cost / ((int64_t)v3::kCtasA * ix->ctx->sm_count);
-    const int64_t item_max_top = std::max<int64_t>(ix->ctx->item_postings, per_cta / ix->ctx->item_share);
-    const int64_t item_max_full = std::max<int64_t>(ix->ctx->item_postings, per_cta / ix->ctx->item_share_full);
-    for (int qi : order) {
-      // pruned sweeps (TOP_SCORES pure disjunctions) skip most of a heavy item's postings; launches that visit every
-      // posting are split finer (their longest item is the tail of the launch)
-      const int64_t item_max = (is_simple(qi) && b->threshold < (int64_t)INT32_MAX) ? item_max_top : item_max_full;
-      const int64_t per_slice = cost[qi] / std::max(1, (int)b->n_slices);
-      int lp = 0;
-      while (lp < 4 && (per_slice >> lp) > item_max && (gran_per_slice >> (lp + 1)) >= 8) ++lp;
-      lparts[(size_t)qi] = (uint8_t)lp;
-      lp_max = std::max(lp_max, lp);
-    }
-  }
-  b->parts_max = 1 << lp_max;
-  b->n_lists = b->n_slices * b->parts_max + (warm_ok ? 1 : 0);
-  auto push_items = [&](int qi, int s) {   // the parts of (query, slice) that hold at least one granule
-    const int lp = lparts[(size_t)qi], P = 1 << lp;
-    const int g_count = std::min(gran_per_slice, n_gran_h - s * gran_per_slice);
-    const int fine = (gran_per_slice + b->parts_max - 1) / b->parts_max, kfine = b->parts_max >> lp;   // as the kernel decodes them
-    const bool behind_warm = s == 0 && has_warm[(size_t)qi];
-    for (int p = 0; p < P; ++p) {
-      int lo = std::min(g_count, p * kfine * fine), hi = (p + 1) * kfine >= b->parts_max ? g_count : std::min(g_count, (p + 1) * kfine * fine);
-      if (behind_warm) lo = std::max(lo, std::min(g_count, (int)v3::kWarmGran));
-      if (P > 1 && lo >= hi) continue;
-      wq.push_back(qi); ws.push_back(s | (p << 16) | (lp << 20) | (behind_warm ? (2 << 24) : 0));
-    }
-  };
-  // simple queries first (with the warm-up items ahead of them), then the generic ones; the generic probe instantiation
-  // also sweeps whole doc ranges when no posting list can lead (match-all / range-led queries)
-  int32_t n_simple_items = 0;
-  for (const bool simple : {true, false}) {
-    for (int s = 0; s < b->n_slices; ++s)
-      for (int qi : order) if (is_simple(qi) == simple) push_items(qi, s);
-    if (simple) n_simple_items = (int32_t)wq.size();
-  }
-  b->n_work = (int32_t)wq.size();
-  b->n_probe_simple = b->wide_slots ? 0 : n_simple_items;
-  b->n_probe_generic = b->wide_slots ? 0 : b->n_work - n_simple_items;
-  b->h_dc.swap(dc); b->h_dq.swap(dq);   // kept alive until the next compilation: the uploads below are asynchronous
-  int rc;
-  if ((rc = b->clauses.upload_async(b->h_dc.data(), b->h_dc.size(), st))) return rc;
-  if ((rc = b->queries.upload_async(b->h_dq.data(), b->h_dq.size(), st))) return rc;
-  if ((rc = b->work_query.upload_async(wq.data(), wq.size(), st))) return rc;
-  if ((rc = b->work_slice.upload_async(ws.data(), ws.size(), st))) return rc;
-  if ((rc = b->known_hits.upload_async(b->h_known.data(), b->h_known.size(), st))) return rc;
-  if (sorted) {
+  WorkPlan& p = b->plan;
+  plan_work(ix->dict(), ix->ctx->plan, b->cb, &p);
+  if ((rc = b->work_query.upload_async(p.work_query.data(), p.work_query.size(), st))) return rc;
+  if ((rc = b->work_slice.upload_async(p.work_item.data(), p.work_item.size(), st))) return rc;
+  if ((rc = b->known_hits.upload_async(p.known_hits.data(), p.known_hits.size(), st))) return rc;
+  if (b->cb.sorted) {
     bool any_after = false;
     b->h_after_docs.assign((size_t)nq, 0);
-    for (int qi = 0; qi < nq; ++qi) if (queries[qi].has_after) { any_after = true; b->h_after_docs[(size_t)qi] = queries[qi].after_doc; }
+    for (int qi = 0; qi < nq; ++qi) if (r.queries[qi].has_after) { any_after = true; b->h_after_docs[(size_t)qi] = r.queries[qi].after_doc; }
     if (sort_order) {
-      if (any_after && !order_after) NRT_FAIL(NRTGPU_ERR_INVALID, "sorted searchAfter needs after_values");
       // (the COLUMN key reads a missing code; ranks are never 0, so it is never used)
       if ((rc = b->sort_missing_code.alloc(1))) return rc;
       NRT_CUDA_TRY(cudaMemsetAsync(b->sort_missing_code.p, 0, sizeof(uint32_t), st));
       if ((rc = b->after_docs.upload_async(b->h_after_docs.data(), (size_t)nq, st))) return rc;
       const size_t nv = (size_t)nq * sort_order->n_fields;
-      if (order_after) { if ((rc = b->after_values.upload_async(order_after, nv, st))) return rc; }
+      if (r.order_after) { if ((rc = b->after_values.upload_async(r.order_after, nv, st))) return rc; }
       else if ((rc = b->after_values.alloc(nv))) return rc;
       SortFieldsAfterLaunch A{};
       A.queries = b->queries.p; A.nq = nq; A.after_docs = b->after_docs.p; A.after_values = b->after_values.p;
@@ -1023,7 +709,6 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
       NRT_CUDA_TRY(cudaGetLastError());
       if ((rc = b->out_sort_values.alloc(nv * top_k))) return rc;
     } else {
-      if (any_after && sort->kind == NRTGPU_SORT_COLUMN && !sort->after_values) NRT_FAIL(NRTGPU_ERR_INVALID, "sorted searchAfter needs after_values");
       if ((rc = b->sort_missing_code.alloc(1))) return rc;
       if ((rc = b->after_docs.upload_async(b->h_after_docs.data(), (size_t)nq, st))) return rc;
       if (sort->after_values) { if ((rc = b->after_values.upload_async(sort->after_values, (size_t)nq, st))) return rc; }
@@ -1042,28 +727,24 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const nrtgpu_clause* c
   }
   if ((rc = b->theta.alloc((size_t)nq))) return rc;
   if ((rc = b->total_hits.alloc((size_t)nq))) return rc;
-  if ((rc = b->slice_keys.alloc((size_t)nq * b->n_lists * top_k))) return rc;
-  if ((rc = b->slice_cnt.alloc((size_t)nq * b->n_lists))) return rc;
+  if ((rc = b->slice_keys.alloc((size_t)nq * p.n_lists * top_k))) return rc;
+  if ((rc = b->slice_cnt.alloc((size_t)nq * p.n_lists))) return rc;
   if ((rc = b->out_docs.alloc((size_t)nq * top_k))) return rc;
   if ((rc = b->out_scores.alloc((size_t)nq * top_k))) return rc;
   if ((rc = b->out_counts.alloc((size_t)nq))) return rc;
   if ((rc = b->pruned.alloc((size_t)nq))) return rc;
   if ((rc = b->terminated.alloc((size_t)nq))) return rc;
-  if (!b->wide_slots) {
-    b->n_gran = (int32_t)(((int64_t)ix->n_docs + v3::kGran - 1) / v3::kGran);
-    if (b->n_gran < 1) b->n_gran = 1;
-    if (b->n_probe_simple + b->n_probe_generic > 0) {
-      // probe kernel: posting offsets of every (query, term slot) at the slice boundaries only (skip data for the long
-      // lists, one lower_bound for the short ones); the granule offsets inside a slice are read from gran_tab by the kernel
-      const int64_t total = (int64_t)nq * v3::kT * ((int64_t)b->n_slices * b->parts_max + 2);
-      if ((rc = b->sbounds.alloc((size_t)total))) return rc;
-      if ((rc = b->work_counter.alloc(2))) return rc;
-      v3::SliceBoundsLaunch S;
-      S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_slices = b->n_slices;
-      S.slice_gran = b->slice_docs / v3::kGran; S.n_gran = b->n_gran; S.parts_max = b->parts_max; S.sbounds = b->sbounds.p;
-      v3::slice_bounds_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S);
-      NRT_CUDA_TRY(cudaGetLastError());
-    }
+  if (p.n_probe_simple + p.n_probe_generic > 0) {
+    // probe kernel: posting offsets of every (query, term slot) at the part boundaries only (skip data for the long lists,
+    // one lower_bound for the short ones); the granule offsets inside a slice are read from gran_tab by the kernel
+    const int64_t total = (int64_t)nq * v3::kT * ((int64_t)p.n_slices * p.parts_max + 2);
+    if ((rc = b->sbounds.alloc((size_t)total))) return rc;
+    if ((rc = b->work_counter.alloc(2))) return rc;
+    v3::SliceBoundsLaunch S;
+    S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_slices = p.n_slices;
+    S.slice_gran = p.slice_docs / v3::kGran; S.n_gran = p.n_gran; S.parts_max = p.parts_max; S.sbounds = b->sbounds.p;
+    v3::slice_bounds_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S);
+    NRT_CUDA_TRY(cudaGetLastError());
   }
   if (!b->ev[0][0]) for (auto& r : b->ev) for (auto& e : r) NRT_CUDA_TRY(cudaEventCreate(&e));
   return NRTGPU_OK;
@@ -1074,7 +755,7 @@ int nrtgpu_batch_prepare(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
                          int32_t total_hits_threshold, int32_t flags, nrtgpu_batch** out) {
   if (!out) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: NULL argument");
   std::unique_ptr<nrtgpu_batch> b(new nrtgpu_batch);
-  int rc = batch_build(b.get(), ix, clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags, (cudaStream_t)0);
+  int rc = batch_build(b.get(), ix, BatchRequest{clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags}, (cudaStream_t)0);
   if (rc) return rc;
   NRT_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)0));
   *out = b.release();
@@ -1099,17 +780,17 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   const bool debug = b->ix->ctx->debug_modes;
   cudaEvent_t* ev = b->ev[b->runs_recorded % nrtgpu_batch::kEvRing];
   NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
-  if (b->n_work > 0) {
+  if (b->plan.n_work() > 0) {
     BoolLaunch L;
     L.ix = b->ix->view();
     L.clauses = b->clauses.p; L.queries = b->queries.p;
     L.work_query = b->work_query.p; L.work_slice = b->work_slice.p;
-    L.n_work = b->n_work; L.n_slices = b->n_lists; L.top_k = b->top_k;
+    L.n_work = b->plan.n_work(); L.n_slices = b->plan.n_lists; L.top_k = b->top_k;
     L.theta = b->theta.p; L.total_hits = b->total_hits.p;
     L.slice_keys = b->slice_keys.p; L.slice_cnt = b->slice_cnt.p;
     L.deadline_ns = b->limits_active ? b->deadline_ns : 0; L.clock0 = b->clock0.p; L.timed_out = b->timed_out.p;
-    if (!b->wide_slots) {
-      const int n_probe = b->n_probe_simple + b->n_probe_generic;
+    if (!b->cb.wide) {
+      const int n_probe = b->plan.n_probe_simple + b->plan.n_probe_generic;
       if (n_probe > 0) {
         v3::ProbeLaunch P;
         P.ix = L.ix; P.clauses = L.clauses; P.queries = L.queries; P.sbounds = b->sbounds.p;
@@ -1120,8 +801,8 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
 #else
         P.knock = 0;
 #endif
-        P.n_lists = b->n_lists; P.parts_max = b->parts_max; P.n_slices = b->n_slices; P.top_k = b->top_k; P.slice_docs = b->slice_docs; P.n_gran = b->n_gran;
-        P.threshold = b->threshold; P.pruned = b->pruned.p; P.theta = L.theta; P.total_hits = L.total_hits;
+        P.n_lists = b->plan.n_lists; P.parts_max = b->plan.parts_max; P.n_slices = b->plan.n_slices; P.top_k = b->top_k; P.slice_docs = b->plan.slice_docs; P.n_gran = b->plan.n_gran;
+        P.threshold = b->cb.threshold; P.pruned = b->pruned.p; P.theta = L.theta; P.total_hits = L.total_hits;
         P.slice_keys = L.slice_keys; P.slice_cnt = L.slice_cnt;
         P.deadline_ns = L.deadline_ns; P.clock0 = L.clock0; P.timed_out = L.timed_out;
         P.terminate_after = b->ta_scalar; P.terminated = b->terminated.p;
@@ -1129,11 +810,11 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         P.sort_codes = b->order ? b->order->rank.p : b->sort_kind == NRTGPU_SORT_COLUMN ? b->ix->col_code[(size_t)b->sort_column]->p : nullptr;
         P.sort_missing_code = b->sort_missing_code.p;
         P.aggs = nullptr;
-        if (!b->aggs.empty()) {
+        if (!b->cb.aggs.empty()) {
           AggLaunch A; std::memset(&A, 0, sizeof(A));
-          A.n_aggs = (int32_t)b->aggs.size();
+          A.n_aggs = (int32_t)b->cb.aggs.size();
           for (int i = 0; i < A.n_aggs; ++i) {
-            const nrtgpu_aggregation& a = b->aggs[(size_t)i];
+            const nrtgpu_aggregation& a = b->cb.aggs[(size_t)i];
             A.a[i].kind = a.kind; A.a[i].column = a.column; A.a[i].value_type = a.value_type;
             if (a.kind == NRTGPU_AGG_TERMS) {
               const int32_t nb = b->ix->col_n_distinct[(size_t)a.column];
@@ -1163,41 +844,41 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         auto launch = [&](auto simple_tag, bool cfg_b, int n_items) {
           constexpr bool S = decltype(simple_tag)::value;
           if (cfg_b) {
-            const int grid = std::min(v3::kCtasB * b->ix->ctx->sm_count, n_items);
+            const int grid = std::min(v3::kCtasB * b->ix->ctx->plan.sm_count, n_items);
             if (debug) v3::posting_probe_kernel<S, true, v3::kCtasB, v3::kStageB><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
             else v3::posting_probe_kernel<S, false, v3::kCtasB, v3::kStageB><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
           } else {
-            const int grid = std::min(v3::kCtasA * b->ix->ctx->sm_count, n_items);
+            const int grid = std::min(v3::kCtasA * b->ix->ctx->plan.sm_count, n_items);
             if (debug) v3::posting_probe_kernel<S, true, v3::kCtasA, v3::kStageA><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageA>), st>>>(P);
             else v3::posting_probe_kernel<S, false, v3::kCtasA, v3::kStageA><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageA>), st>>>(P);
           }
         };
-        if (b->n_probe_simple > 0) {
-          P.work_query = L.work_query; P.work_slice = L.work_slice; P.n_work = b->n_probe_simple; P.work_counter = b->work_counter.p;
+        if (b->plan.n_probe_simple > 0) {
+          P.work_query = L.work_query; P.work_slice = L.work_slice; P.n_work = b->plan.n_probe_simple; P.work_counter = b->work_counter.p;
           P.stats = debug ? b->probe_stats.p : nullptr;
-          launch(std::true_type{}, cfg_b_simple, b->n_probe_simple);
+          launch(std::true_type{}, cfg_b_simple, b->plan.n_probe_simple);
         }
-        if (b->n_probe_generic > 0) {
-          P.work_query = L.work_query + b->n_probe_simple; P.work_slice = L.work_slice + b->n_probe_simple;
-          P.n_work = b->n_probe_generic; P.work_counter = b->work_counter.p + 1;
+        if (b->plan.n_probe_generic > 0) {
+          P.work_query = L.work_query + b->plan.n_probe_simple; P.work_slice = L.work_slice + b->plan.n_probe_simple;
+          P.n_work = b->plan.n_probe_generic; P.work_counter = b->work_counter.p + 1;
           P.stats = debug ? b->probe_stats.p + 16 : nullptr;
-          launch(std::false_type{}, cfg_b_generic, b->n_probe_generic);
+          launch(std::false_type{}, cfg_b_generic, b->plan.n_probe_generic);
         }
         NRT_CUDA_TRY(cudaGetLastError());
       }
     } else
-      bool_window_kernel<<<b->n_work, kThreads, sizeof(BoolSmem), st>>>(L);
+      bool_window_kernel<<<b->plan.n_work(), kThreads, sizeof(BoolSmem), st>>>(L);
     NRT_CUDA_TRY(cudaGetLastError());
   }
   NRT_CUDA_TRY(cudaEventRecord(ev[1], st));
-  if (debug && b->probe_stats.p && !b->wide_slots) {
+  if (debug && b->probe_stats.p && !b->cb.wide) {
     unsigned long long h[32];
     NRT_CUDA_TRY(cudaMemcpyAsync(h, b->probe_stats.p, sizeof(h), cudaMemcpyDeviceToHost, st));
     NRT_CUDA_TRY(cudaStreamSynchronize(st));
     for (int k = 0; k < 2; ++k) {
       const unsigned long long* x = h + 16 * k;
       if (x[0]) fprintf(stderr, "[nrtgpu probe %s] longest item %llu cyc; CTA busy: mean %.0f max %llu cyc; warm-up items %llu, %.0f cyc each; per item: flush %.0f cyc (sort %.0f), TMA wait %.0f cyc\n", k == 0 ? "simple" : "generic",
-                        x[8], (double)x[9] / std::min<double>((double)x[0], (double)(v3::kCtasA * b->ix->ctx->sm_count)), x[10], x[11], x[11] ? (double)x[12] / x[11] : 0.0, (double)x[13] / x[0], (double)x[15] / x[0], (double)x[14] / x[0]);
+                        x[8], (double)x[9] / std::min<double>((double)x[0], (double)(v3::kCtasA * b->ix->ctx->plan.sm_count)), x[10], x[11], x[11] ? (double)x[12] / x[11] : 0.0, (double)x[13] / x[0], (double)x[15] / x[0], (double)x[14] / x[0]);
       if (x[0]) fprintf(stderr, "[nrtgpu probe %s] %llu items, %.0f cyc/item (set-up %.0f), %.2f runs/item (%.2f staged), %.1f rounds/item, %llu driver postings (%.0f/item), %.2f flushes/item\n",
                         k == 0 ? "simple" : "generic", x[0], (double)x[1] / x[0], (double)x[6] / x[0], (double)x[2] / x[0], (double)x[5] / x[0],
                         (double)x[7] / x[0], x[3], (double)x[3] / x[0], (double)x[4] / x[0]);
@@ -1205,12 +886,12 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   }
   MergeLaunch M;
   M.slice_keys = b->slice_keys.p; M.slice_cnt = b->slice_cnt.p;
-  M.n_lists = b->n_lists; M.top_k = b->top_k; M.nq = b->nq; M.doc_base = b->ix->doc_base;
+  M.n_lists = b->plan.n_lists; M.top_k = b->top_k; M.nq = b->nq; M.doc_base = b->ix->doc_base;
   M.out_docs = b->o_docs(); M.out_scores = b->o_scores(); M.out_counts = b->o_counts();
   M.total_hits = b->total_hits.p; M.pruned = b->pruned.p; M.terminated = b->terminated.p; M.terminate_after = b->ta_scalar;
   M.out_total = b->bound_total; M.out_flags = b->bound_flags;
-  M.theta = !b->wide_slots ? b->theta.p : nullptr;
-  M.known_hits = (!b->wide_slots && !b->ix->live_bits.p) ? b->known_hits.p : nullptr;
+  M.theta = !b->cb.wide ? b->theta.p : nullptr;
+  M.known_hits = (!b->cb.wide && !b->ix->live_bits.p) ? b->known_hits.p : nullptr;
   merge_slices_kernel<<<b->nq, kMergeThreads, 0, st>>>(M);
   NRT_CUDA_TRY(cudaGetLastError());
   if (b->order) {   // FieldDoc values of every field; score-first orders map ranks back to docs
@@ -1265,8 +946,8 @@ static int batch_fetch_impl(nrtgpu_batch* b, void* stream_, int32_t* out_docs, f
     if (out_relation) out_relation[i] = (pr[(size_t)i] || term || to) ? 1 : 0;
     if (out_terminated_early) out_terminated_early[i] = term ? 1 : 0;
     if (out_hit_timeout) out_hit_timeout[i] = to ? 1 : 0;
-    if (out_total_hits && pr[(size_t)i] && !term && !to && !b->ix->live_bits.p && (size_t)i < b->h_known.size() && (int64_t)b->h_known[(size_t)i] > out_total_hits[i])
-      out_total_hits[i] = (int64_t)b->h_known[(size_t)i];   // pruned search: the count is a lower bound; so is the longest list
+    if (out_total_hits && pr[(size_t)i] && !term && !to && !b->ix->live_bits.p && (size_t)i < b->plan.known_hits.size() && (int64_t)b->plan.known_hits[(size_t)i] > out_total_hits[i])
+      out_total_hits[i] = (int64_t)b->plan.known_hits[(size_t)i];   // pruned search: the count is a lower bound; so is the longest list
     if (term && out_total_hits && b->terminate_after_max_recall > 0 && out_total_hits[i] > b->terminate_after_max_recall)
       out_total_hits[i] = b->terminate_after_max_recall;
   }
@@ -1289,8 +970,8 @@ int nrtgpu_batch_fetch_ex(nrtgpu_batch* b, void* stream_, int32_t* out_docs, flo
 // aggregation results of the last run -> caller buffers
 static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggregation_result* out) {
   const int nq = b->nq;
-  for (size_t i = 0; i < b->aggs.size(); ++i) {
-    const nrtgpu_aggregation& a = b->aggs[i];
+  for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
+    const nrtgpu_aggregation& a = b->cb.aggs[i];
     const nrtgpu_aggregation_result& r = out[i];
     if (a.kind == NRTGPU_AGG_TERMS) {
       int rc;
@@ -1377,7 +1058,7 @@ int64_t nrtgpu_packed_words(int32_t nq, int32_t top_k) {
 
 int nrtgpu_batch_bind_packed(nrtgpu_batch* b, int32_t* d_record) {
   if (!b) NRT_FAIL(NRTGPU_ERR_INVALID, "NULL batch");
-  if (!d_record) { b->bound_docs = nullptr; b->bound_scores = nullptr; b->bound_counts = nullptr; b->bound_total = nullptr; b->bound_flags = nullptr; return NRTGPU_OK; }
+  if (!d_record) { b->unbind(); return NRTGPU_OK; }
   if (((uintptr_t)d_record & 7u) != 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_bind_packed: record must be 8-byte aligned");
   const int64_t n = (int64_t)b->nq * b->top_k;
   b->bound_docs = d_record; b->bound_scores = (float*)(d_record + n); b->bound_counts = d_record + 2 * n;
@@ -1414,14 +1095,14 @@ int nrtgpu_batch_reset_timing(nrtgpu_batch* b) {
 
 int nrtgpu_batch_stats(const nrtgpu_batch* b, int64_t* alg_postings, int32_t* launches_per_run, int64_t* work_items) {
   if (!b) NRT_FAIL(NRTGPU_ERR_INVALID, "NULL batch");
-  if (alg_postings) *alg_postings = b->alg_postings;
+  if (alg_postings) *alg_postings = b->cb.alg_postings;
   if (launches_per_run) {
     int n = 1;   // slice merge
-    if (b->wide_slots) n += b->n_work > 0 ? 1 : 0;
-    else n += (b->n_probe_simple > 0 ? 1 : 0) + (b->n_probe_generic > 0 ? 1 : 0);
+    if (b->cb.wide) n += b->plan.n_work() > 0 ? 1 : 0;
+    else n += (b->plan.n_probe_simple > 0 ? 1 : 0) + (b->plan.n_probe_generic > 0 ? 1 : 0);
     *launches_per_run = n;
   }
-  if (work_items) *work_items = b->n_work;
+  if (work_items) *work_items = b->plan.n_work();
   return NRTGPU_OK;
 }
 
@@ -1443,46 +1124,48 @@ int nrtgpu_batch_free(nrtgpu_batch* b) {
   return NRTGPU_OK;
 }
 
-// one-shot search: compile + upload the batch into a pooled workspace, run; results either copied to HOST buffers
-// (d_record == NULL) or left in a packed DEVICE record (the multi-GPU path: the caller all-gathers it on `stream`)
-static int search_bool_impl(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
-                            const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags,
-                            const nrtgpu_search_limits* limits, void* stream, int32_t* d_record, int32_t* out_docs, float* out_scores,
-                            int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
-                            uint8_t* out_terminated_early, const nrtgpu_sort* sort = nullptr, int64_t* out_sort_values = nullptr,
-                            const nrtgpu_aggregation* aggs = nullptr, int32_t n_aggs = 0, const nrtgpu_aggregation_result* agg_out = nullptr,
-                            const nrtgpu_sort_order* order = nullptr, const int64_t* order_after = nullptr) {
-  if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool: NULL index");
-  // take a cached workspace (device buffers survive between calls: no cudaMalloc on the request path)
+// a pooled batch workspace of the index (device buffers survive between calls: no cudaMalloc on the request path), checked
+// out for one call; returned with its bound outputs cleared
+struct WorkspaceLease {
+  nrtgpu_index* ix;
   nrtgpu_batch* b = nullptr;
-  {
-    std::lock_guard<std::mutex> g(ix->ws_mu);
-    if (!ix->ws_free.empty()) { b = ix->ws_free.back(); ix->ws_free.pop_back(); }
+  explicit WorkspaceLease(nrtgpu_index* ix_) : ix(ix_) {
+    { std::lock_guard<std::mutex> g(ix->ws_mu); if (!ix->ws_free.empty()) { b = ix->ws_free.back(); ix->ws_free.pop_back(); } }
+    if (!b) b = new nrtgpu_batch;
   }
-  if (!b) b = new nrtgpu_batch;
-  b->bound_docs = nullptr; b->bound_scores = nullptr; b->bound_counts = nullptr; b->bound_total = nullptr; b->bound_flags = nullptr;
-  int rc = batch_build(b, ix, clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags, (cudaStream_t)stream, sort, aggs, n_aggs,
-                       order, order_after);
+  ~WorkspaceLease() { b->unbind(); std::lock_guard<std::mutex> g(ix->ws_mu); ix->ws_free.push_back(b); }
+  WorkspaceLease(const WorkspaceLease&) = delete;
+  WorkspaceLease& operator=(const WorkspaceLease&) = delete;
+};
+
+// where a one-shot search leaves its results: a packed DEVICE record (the multi-GPU path: the caller all-gathers it on
+// the stream), or else the HOST buffers (any may be NULL)
+struct SearchOut {
+  int32_t* d_record = nullptr;
+  int32_t* docs = nullptr; float* scores = nullptr; int32_t* counts = nullptr; int64_t* total_hits = nullptr;
+  uint8_t* relation = nullptr; uint8_t* hit_timeout = nullptr; uint8_t* terminated_early = nullptr;
+  int64_t* sort_values = nullptr;
+  const nrtgpu_aggregation_result* aggs = nullptr;
+};
+
+// one-shot search: compile + upload the batch into a pooled workspace, run, deliver the results
+static int search_bool_impl(nrtgpu_index* ix, const BatchRequest& r, const nrtgpu_search_limits* limits, void* stream, const SearchOut& out) {
+  if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool: NULL index");
+  WorkspaceLease ws(ix);
+  nrtgpu_batch* b = ws.b;
+  int rc = batch_build(b, ix, r, (cudaStream_t)stream);
   if (!rc) rc = batch_set_limits(b, limits, (cudaStream_t)stream);
-  if (!rc && d_record) rc = nrtgpu_batch_bind_packed(b, d_record);
+  if (!rc && out.d_record) rc = nrtgpu_batch_bind_packed(b, out.d_record);
   if (!rc) rc = nrtgpu_batch_run(b, stream);
-  if (!rc) {
-    if (d_record) { cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream); if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); rc = NRTGPU_ERR_CUDA; } }
-    else {
-      if (out_sort_values && b->sort_kind != NRTGPU_SORT_RELEVANCE) {
-        const size_t nv = (size_t)nq * top_k * (order ? order->n_fields : 1);
-        cudaError_t e = cudaMemcpyAsync(out_sort_values, b->out_sort_values.p, nv * sizeof(int64_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
-        if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); rc = NRTGPU_ERR_CUDA; }
-      }
-      if (!rc) rc = batch_fetch_impl(b, stream, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
-      if (!rc && n_aggs > 0 && agg_out) rc = batch_fetch_aggs(b, (cudaStream_t)stream, agg_out);
-    }
+  if (rc) return rc;
+  if (out.d_record) { cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream); if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; } return NRTGPU_OK; }
+  if (out.sort_values && b->sort_kind != NRTGPU_SORT_RELEVANCE) {
+    const size_t nv = (size_t)r.nq * r.top_k * (r.sort_order ? r.sort_order->n_fields : 1);
+    cudaError_t e = cudaMemcpyAsync(out.sort_values, b->out_sort_values.p, nv * sizeof(int64_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
+    if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; }
   }
-  b->bound_docs = nullptr; b->bound_scores = nullptr; b->bound_counts = nullptr; b->bound_total = nullptr; b->bound_flags = nullptr;
-  {
-    std::lock_guard<std::mutex> g(ix->ws_mu);
-    ix->ws_free.push_back(b);
-  }
+  rc = batch_fetch_impl(b, stream, out.docs, out.scores, out.counts, out.total_hits, out.relation, out.hit_timeout, out.terminated_early);
+  if (!rc && !b->cb.aggs.empty() && out.aggs) rc = batch_fetch_aggs(b, (cudaStream_t)stream, out.aggs);
   return rc;
 }
 
@@ -1491,8 +1174,8 @@ int nrtgpu_search_bool(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n
                        int32_t total_hits_threshold, int32_t flags, void* stream, int32_t* out_docs,
                        float* out_scores, int32_t* out_counts, int64_t* out_total_hits,
                        uint8_t* out_relation) {
-  return search_bool_impl(ix, clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags, nullptr, stream, nullptr,
-                          out_docs, out_scores, out_counts, out_total_hits, out_relation, nullptr, nullptr);
+  SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
+  return search_bool_impl(ix, BatchRequest{clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags}, nullptr, stream, o);
 }
 
 int nrtgpu_search_bool_ex(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -1500,8 +1183,9 @@ int nrtgpu_search_bool_ex(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_
                           const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs, float* out_scores,
                           int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
                           uint8_t* out_terminated_early) {
-  return search_bool_impl(ix, clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags, limits, stream, nullptr,
-                          out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
+  SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
+  o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early;
+  return search_bool_impl(ix, BatchRequest{clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags}, limits, stream, o);
 }
 
 int nrtgpu_search_sorted(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -1511,9 +1195,11 @@ int nrtgpu_search_sorted(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
                          int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
                          uint8_t* out_terminated_early) {
   if (!sort) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_sorted: NULL sort");
-  return search_bool_impl(ix, clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags, limits, stream, nullptr,
-                          out_docs, nullptr, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early,
-                          sort, out_sort_values);
+  BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
+  r.sort = sort;
+  SearchOut o; o.docs = out_docs; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
+  o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early; o.sort_values = out_sort_values;
+  return search_bool_impl(ix, r, limits, stream, o);
 }
 
 int nrtgpu_sort_order_create(nrtgpu_index* ix, const nrtgpu_sort_field* fields, int32_t n_fields, void* stream, nrtgpu_sort_order** out) {
@@ -1576,9 +1262,11 @@ int nrtgpu_search_sorted_fields(nrtgpu_index* ix, const nrtgpu_sort_order* order
                                 uint8_t* out_terminated_early) {
   if (!ix || !order) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_sorted_fields: NULL argument");
   if (order->ix != ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_sorted_fields: the sort order was made on another index");
-  return search_bool_impl(ix, clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags, limits, stream, nullptr,
-                          out_docs, nullptr, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early,
-                          nullptr, out_sort_values, nullptr, 0, nullptr, order, after_values);
+  BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
+  r.sort_order = order; r.order_after = after_values;
+  SearchOut o; o.docs = out_docs; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
+  o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early; o.sort_values = out_sort_values;
+  return search_bool_impl(ix, r, limits, stream, o);
 }
 
 int nrtgpu_search_bool_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -1587,8 +1275,15 @@ int nrtgpu_search_bool_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int3
                             void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
                             int64_t* out_total_hits) {
   if (n_aggs <= 0 || !aggs || !results) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool_aggs: no aggregations");
-  return search_bool_impl(ix, clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags, nullptr, stream, nullptr, out_docs, out_scores,
-                          out_counts, out_total_hits, nullptr, nullptr, nullptr, nullptr, nullptr, aggs, n_aggs, results);
+  BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
+  r.aggs = aggs; r.n_aggs = n_aggs;
+  SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.aggs = results;
+  return search_bool_impl(ix, r, nullptr, stream, o);
+}
+
+// the request of the compile-only entry points: exhaustive, one hit per query (they never run the batch)
+static BatchRequest compile_only_request(const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_query* queries, int32_t nq) {
+  return BatchRequest{clauses, n_clauses, queries, nq, 1, INT32_MAX, 0};
 }
 
 int nrtgpu_score_docs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -1596,27 +1291,24 @@ int nrtgpu_score_docs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_
                       const int32_t* counts, void* stream, uint8_t* out_matches, float* out_scores) {
   if (!ix || !docs || !out_matches || !out_scores || n_hits <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_score_docs: bad argument");
   cudaStream_t st = (cudaStream_t)stream;
-  nrtgpu_batch* b = nullptr;
-  { std::lock_guard<std::mutex> g(ix->ws_mu); if (!ix->ws_free.empty()) { b = ix->ws_free.back(); ix->ws_free.pop_back(); } }
-  if (!b) b = new nrtgpu_batch;
-  int rc = batch_build(b, ix, clauses, n_clauses, queries, nq, 1, INT32_MAX, 0, st);
+  WorkspaceLease ws(ix);
+  nrtgpu_batch* b = ws.b;
+  int rc = batch_compile(b, ix, compile_only_request(clauses, n_clauses, queries, nq), st);
   const size_t n = (size_t)nq * n_hits;
   if (!rc) rc = b->sd_docs.upload_async(docs, n, st);
   if (!rc && counts) rc = b->sd_counts.upload_async(counts, (size_t)nq, st);
   if (!rc) rc = b->sd_match.alloc(n);
   if (!rc) rc = b->sd_scores.alloc(n);
-  if (!rc) {
-    ScoreDocsLaunch S; S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_hits = n_hits;
-    S.docs = b->sd_docs.p; S.counts = counts ? b->sd_counts.p : nullptr; S.out_matches = b->sd_match.p; S.out_scores = b->sd_scores.p;
-    score_docs_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(S);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_matches, b->sd_match.p, n, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_scores, b->sd_scores.p, n * sizeof(float), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); rc = NRTGPU_ERR_CUDA; }
-  }
-  { std::lock_guard<std::mutex> g(ix->ws_mu); ix->ws_free.push_back(b); }
-  return rc;
+  if (rc) return rc;
+  ScoreDocsLaunch S; S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_hits = n_hits;
+  S.docs = b->sd_docs.p; S.counts = counts ? b->sd_counts.p : nullptr; S.out_matches = b->sd_match.p; S.out_scores = b->sd_scores.p;
+  score_docs_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(S);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_matches, b->sd_match.p, n, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_scores, b->sd_scores.p, n * sizeof(float), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; }
+  return NRTGPU_OK;
 }
 
 int nrtgpu_rescore_query(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -1626,10 +1318,9 @@ int nrtgpu_rescore_query(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
   if (!ix || !docs || !scores || n_hits <= 0 || window <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_rescore_query: bad argument");
   if (n_hits > kHybCap) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nrtgpu_rescore_query: more than 4096 hits per query");
   cudaStream_t st = (cudaStream_t)stream;
-  nrtgpu_batch* b = nullptr;
-  { std::lock_guard<std::mutex> g(ix->ws_mu); if (!ix->ws_free.empty()) { b = ix->ws_free.back(); ix->ws_free.pop_back(); } }
-  if (!b) b = new nrtgpu_batch;
-  int rc = batch_build(b, ix, clauses, n_clauses, queries, nq, 1, INT32_MAX, 0, st);
+  WorkspaceLease ws(ix);
+  nrtgpu_batch* b = ws.b;
+  int rc = batch_compile(b, ix, compile_only_request(clauses, n_clauses, queries, nq), st);
   const size_t n = (size_t)nq * n_hits;
   // Lucene QueryRescorer.rescore(searcher, hits, topN = windowSize): EVERY first-pass hit is combined and the list
   // re-sorted (score desc, doc asc); then the first topN are kept
@@ -1643,23 +1334,21 @@ int nrtgpu_rescore_query(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
   if (!rc) rc = b->sd_counts.upload_async(wc.data(), (size_t)nq, st);
   if (!rc) rc = b->sd_match.alloc(n);
   if (!rc) rc = b->sd_scores.alloc(n);
-  if (!rc) {
-    ScoreDocsLaunch S; S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_hits = n_hits;
-    S.docs = b->sd_docs.p; S.counts = b->sd_counts.p; S.out_matches = b->sd_match.p; S.out_scores = b->sd_scores.p;
-    score_docs_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(S);
-    RescoreLaunch P;
-    P.nq = nq; P.n_hits = n_hits; P.counts = b->sd_counts.p; P.docs = b->sd_docs.p; P.scores = b->sd_first.p;
-    P.second_matches = b->sd_match.p; P.second_scores = b->sd_scores.p; P.query_weight = query_weight; P.rescore_weight = rescore_weight;
-    rescore_combine_kernel<<<nq, kHybThreads, 0, st>>>(P);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(docs, b->sd_docs.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(scores, b->sd_first.p, n * sizeof(float), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); rc = NRTGPU_ERR_CUDA; }
-    if (!rc && out_counts) for (int q = 0; q < nq; ++q) out_counts[q] = std::min(wc[(size_t)q], window);
-  }
-  { std::lock_guard<std::mutex> g(ix->ws_mu); ix->ws_free.push_back(b); }
-  return rc;
+  if (rc) return rc;
+  ScoreDocsLaunch S; S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_hits = n_hits;
+  S.docs = b->sd_docs.p; S.counts = b->sd_counts.p; S.out_matches = b->sd_match.p; S.out_scores = b->sd_scores.p;
+  score_docs_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(S);
+  RescoreLaunch P;
+  P.nq = nq; P.n_hits = n_hits; P.counts = b->sd_counts.p; P.docs = b->sd_docs.p; P.scores = b->sd_first.p;
+  P.second_matches = b->sd_match.p; P.second_scores = b->sd_scores.p; P.query_weight = query_weight; P.rescore_weight = rescore_weight;
+  rescore_combine_kernel<<<nq, kHybThreads, 0, st>>>(P);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpyAsync(docs, b->sd_docs.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(scores, b->sd_first.p, n * sizeof(float), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; }
+  if (out_counts) for (int q = 0; q < nq; ++q) out_counts[q] = std::min(wc[(size_t)q], window);
+  return NRTGPU_OK;
 }
 
 int nrtgpu_fetch_columns(nrtgpu_index* ix, const int32_t* col_ids, int32_t n_cols, const int32_t* docs, int32_t n,
@@ -1688,8 +1377,8 @@ int nrtgpu_search_bool_packed(nrtgpu_index* ix, const nrtgpu_clause* clauses, in
                               const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags,
                               const nrtgpu_search_limits* limits, void* stream, int32_t* d_record) {
   if (!d_record) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool_packed: NULL record");
-  return search_bool_impl(ix, clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags, limits, stream, d_record,
-                          nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+  SearchOut o; o.d_record = d_record;
+  return search_bool_impl(ix, BatchRequest{clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags}, limits, stream, o);
 }
 
 int nrtgpu_merge_topk_device(nrtgpu_ctx* ctx, int32_t n_lists, int32_t nq, int32_t top_k,
@@ -1751,17 +1440,17 @@ static int knn_filtered_host(nrtgpu_index* ix, const nrtgpu_batch* b, const floa
   if (n_rows > 0) {
     // ---- group the rows so that the bitmaps of a group's distinct terms fit kKnnFilterTermBytes; a term clause points
     //      at its term's bitmap inside its group (terms without postings at none)
-    const int n_cl = (int)b->h_dc.size();
+    const int n_cl = (int)b->cb.clauses.size();
     std::vector<int32_t> clause_term((size_t)std::max(n_cl, 1), -1);
     std::vector<int64_t> term_base, term_pre(1, 0);
     std::vector<int> grp_row{0}, grp_term{0};   // group g: rows [grp_row[g], grp_row[g + 1]), terms [grp_term[g], grp_term[g + 1])
     std::unordered_map<int64_t, int> group_terms;   // post_base -> term index in the current group
     const size_t term_bytes = (size_t)words * 4;
     for (int r = 0; r < n_rows; ++r) {
-      const DevQuery& q = b->h_dq[(size_t)row_filter[(size_t)r]];
+      const DevQuery& q = b->cb.queries[(size_t)row_filter[(size_t)r]];
       int fresh = 0;
       for (int i = 0; i < q.n_clauses; ++i) {
-        const DevClause& c = b->h_dc[(size_t)q.clause_begin + i];
+        const DevClause& c = b->cb.clauses[(size_t)q.clause_begin + i];
         if (c.kind == NRTGPU_TERM && c.n_post > 0 && !group_terms.count(c.post_base)) ++fresh;
       }
       const int rows_in = r - grp_row.back();
@@ -1770,7 +1459,7 @@ static int knn_filtered_host(nrtgpu_index* ix, const nrtgpu_batch* b, const floa
       }
       for (int i = 0; i < q.n_clauses; ++i) {
         const int ci = q.clause_begin + i;
-        const DevClause& c = b->h_dc[(size_t)ci];
+        const DevClause& c = b->cb.clauses[(size_t)ci];
         if (c.kind != NRTGPU_TERM || c.n_post == 0) continue;
         auto it = group_terms.find(c.post_base);
         if (it == group_terms.end()) {
@@ -1924,12 +1613,12 @@ int nrtgpu_search_knn_filtered(nrtgpu_index* ix, const float* queries, int32_t n
   }
   NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
+  std::optional<WorkspaceLease> ws;
   nrtgpu_batch* b = nullptr;
   int rc = NRTGPU_OK;
   if (n_filters > 0) {   // the filters compile as a batch of flat BooleanQuerys (clause checks, UNSUPPORTED shapes)
-    { std::lock_guard<std::mutex> g(ix->ws_mu); if (!ix->ws_free.empty()) { b = ix->ws_free.back(); ix->ws_free.pop_back(); } }
-    if (!b) b = new nrtgpu_batch;
-    rc = batch_build(b, ix, filter_clauses, n_filter_clauses, filters, n_filters, 1, INT32_MAX, 0, st);
+    b = ws.emplace(ix).b;
+    rc = batch_compile(b, ix, compile_only_request(filter_clauses, n_filter_clauses, filters, n_filters), st);
   }
   if (!rc) {
     std::lock_guard<std::mutex> g(ix->knn_mu);
@@ -1966,7 +1655,6 @@ int nrtgpu_search_knn_filtered(nrtgpu_index* ix, const float* queries, int32_t n
       }
     }
   }
-  if (b) { std::lock_guard<std::mutex> g(ix->ws_mu); ix->ws_free.push_back(b); }
   return rc;
 }
 

@@ -67,18 +67,15 @@ __device__ __forceinline__ uint32_t presence4(uint32_t s) {
 #else
 #define NRT_KNOCK(bit) false
 #endif
-constexpr int kT = 4;
+// (kT, kCtasA, the granule, kMaxSliceGran, kWarmGran, kProbeMaxTopK and the work-item word: batch_plan.h)
 // Two launch configurations of the same kernel: 3 CTAs / SM with an 8192-posting stage (80 registers; best for the
 // MAXSCORE-pruned sweeps of TOP_SCORES, whose sparse leading lists want the larger stage) and 4 CTAs / SM with a
 // 6656-posting stage (64 registers; best where every posting is visited: ScoreMode.COMPLETE and the generic clause
 // evaluation, both latency bound on their gathers: 32 resident warps hide more of it than 24).
-constexpr int kCtasA = 3, kStageA = 8192;
+constexpr int kStageA = 8192;
 constexpr int kCtasB = 4, kStageB = 6656;
 constexpr int kThreads = 256;
-constexpr int kLogGran = 10;                 // 1024-doc granules: the granularity of the index-time skip data (gran_tab)
-constexpr int kGran = 1 << kLogGran;
-constexpr int kMaxSliceGran = 512;           // a slice spans at most 512K docs (its granule offsets live in shared memory)
-constexpr int kAlign = 16;                   // staged segments start on 16-posting boundaries (TMA: 16-byte aligned tf bytes)
+constexpr int kAlign = 16;                  // staged segments start on 16-posting boundaries (TMA: 16-byte aligned tf bytes)
 // padding postings behind the last list of the index image: a staged segment also ends on a kAlign-posting boundary of
 // the global arrays (seg_n), so the segment of the last list can read up to kAlign - 1 postings past its end. 1024 is
 // far more than that; the value keeps the image layout and nrtgpu_index_device_bytes unchanged.
@@ -89,9 +86,8 @@ constexpr int kLongReserve = kT * (kGran + 2 * kAlign);   // one granule of ever
 #endif
 constexpr int kR = NRT_PROBE_R;              // driver postings per thread per round (their gathers are in flight together)
 constexpr int kCand = 1024;                  // candidate buffer entries
-constexpr int kMaxTopK = kCand / 2;
+static_assert(kProbeMaxTopK == kCand / 2, "the probe kernel keeps top_k <= half its candidate buffer");
 constexpr int kUbt = 6 * 6 * 6 * 6;
-constexpr int kWarmGran = 32;                // granules (32K docs) of the warm-up work item of a query
 constexpr uint32_t kPiece = 8192;            // bytes per bulk copy
 constexpr uint32_t kTfInexact = 0xFEu;       // tf byte of a plane probe whose 2-bit code saturated (tf >= 3): the exact byte is
                                              // fetched from the byte plane when the doc is scored (rare); >= 5 for the bound table
@@ -103,7 +99,7 @@ struct ProbeLaunch {
   const DevClause* clauses;
   const DevQuery* queries;
   const int32_t* work_query;
-  const int32_t* work_slice;     // slice | part << 16 | log2(parts) << 20 | flags << 24 (4: sweep warm-up item, see the kernel; 1: warm-up item = first kWarmGran granules of slice 0, 2: slice-0 item behind them)
+  const int32_t* work_slice;     // work-item word (batch_plan.h item_encode)
   const uint32_t* sbounds;       // [nq][kT][n_slices * parts_max + 2]: postings of the slot's list below every part boundary, the shard end, the warm-up boundary
   const uint8_t* field_min_norm;
   unsigned int* work_counter;    // queue head
@@ -434,16 +430,15 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     if (sm.skip) continue;
     const long long t_start = kStats ? clock64() : 0ll;
     const int qi = L.work_query[wi];
-    const int slice_raw = L.work_slice[wi];
-    const int slice = slice_raw & 0xffff;
-    const int wflags = slice_raw >> 24;
-    // Sweep warm-up item (flags 4): the first 32K postings of the query's highest-bound list, over the WHOLE shard, probing
-    // only the lists with tf planes (the other lists count as absent: scores are lower bounds). Nothing is output; the
-    // k-th best lower-bound key minus one becomes the query's threshold before any other item of the query runs --
+    const int32_t item = L.work_slice[wi];
+    const int slice = item_slice(item);
+    const int wflags = item_flags(item);
+    // Sweep warm-up item (kItemSweep): the first 32K postings of the query's highest-bound list, over the WHOLE shard,
+    // probing only the lists with tf planes (the other lists count as absent: scores are lower bounds). Nothing is output;
+    // the k-th best lower-bound key minus one becomes the query's threshold before any other item of the query runs --
     // the docs that hold the query's rarest term are where its top-k is, a far better sample than the first 32K docs.
-    const bool sweep_warm = (wflags & 4) != 0;
-    const int warm_slot = (slice_raw >> 16) & 0xf;
-    const int part = sweep_warm ? 0 : ((slice_raw >> 16) & 0xf), lparts = (slice_raw >> 20) & 0xf;   // part `part` of 2^lparts of the slice
+    const bool sweep_warm = (wflags & kItemSweep) != 0;
+    const int warm_slot = item_sweep_slot(item);
     const int ncl = L.queries[qi].n_clauses, cbeg = L.queries[qi].clause_begin, n_term = L.queries[qi].n_term;
     if (tid == 0) {
       sm.q = L.queries[qi];
@@ -461,16 +456,8 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     const int g_first = slice * gran_per_slice;
     const int g_count = min(gran_per_slice, L.n_gran - g_first);
     // granule range of the item inside its slice, and the entries of the boundary table that hold its posting bounds
-    const int kfine = L.parts_max >> lparts;   // finest parts per part of this item
-    int g_lo = min(g_count, part * kfine * fine);
-    int g_hi = ((part + 1) * kfine >= L.parts_max) ? g_count : min(g_count, (part + 1) * kfine * fine);
-    const int e_lo = slice * L.parts_max + part * kfine;
-    int e_hi = slice * L.parts_max + (part + 1) * kfine;   // (part + 1) * kfine == parts_max: entry 0 of the next slice / the end entry
-    const int e_warm = L.n_slices * L.parts_max + 1;
-    if (wflags & 2) g_lo = max(g_lo, min(g_count, kWarmGran));
-    if (wflags & 1) { g_hi = min(g_count, kWarmGran); e_hi = e_warm; }
-    const int e_lo2 = sweep_warm ? 0 : e_lo;                              // whole-shard bounds of every list; one dummy run of one granule
-    if (sweep_warm) { g_lo = 0; g_hi = 1; e_hi = L.n_slices * L.parts_max; }
+    const ItemSpan span = item_span(item, g_count, fine, L.parts_max, L.n_slices);
+    const int g_lo = span.g_lo, g_hi = span.g_hi;
     __syncthreads();   // B1: query + clauses resident
     // terminateAfter (TerminateAfterWrapper.java:150-162): a query that has collected enough hits stops collecting
     if (L.terminate_after > 0 && (long long)sm.hits0 >= L.terminate_after) {
@@ -482,9 +469,9 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       const DevClause& c = sm.cl[tid];
       const int s = c.slot;
       const uint32_t* sb = L.sbounds + ((size_t)qi * kT + s) * sb_stride;
-      uint32_t a = sb[e_lo2];
-      uint32_t b = sb[e_hi];
-      if (wflags & 2) a = max(a, sb[e_warm]);
+      uint32_t a = sb[span.e_lo];
+      uint32_t b = sb[span.e_hi];
+      if (wflags & kItemBehindWarm) a = max(a, sb[boundary_warm_entry(L.n_slices, L.parts_max)]);
       if (sweep_warm && s == warm_slot) b = min(b, a + 32768u);
       sm.s_ia[s] = a; sm.s_ib[s] = max(a, b);
       sm.s_gdocs[s] = L.ix.post_docs + c.post_base;
@@ -971,7 +958,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       if (kStats) ++dbg_flush;
     }
     const int keep = sweep_warm ? 0 : min(sm.cand_count, L.top_k);
-    const int out_list = (wflags & 5) ? L.n_lists - 1 : slice * L.parts_max + part * kfine;
+    const int out_list = item_out_list(item, L.parts_max, L.n_lists);
     uint64_t* out = L.slice_keys + ((size_t)qi * L.n_lists + out_list) * L.top_k;
     for (int i = tid; i < keep; i += kThreads) out[i] = sm.cand[i];
     if (tid == 0) L.slice_cnt[(size_t)qi * L.n_lists + out_list] = keep;
@@ -988,7 +975,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       atomicAdd(&L.stats[7], (unsigned long long)dbg_rounds);
       const unsigned long long cyc = (unsigned long long)(clock64() - t_start);
       atomicMax(&L.stats[8], cyc);
-      if (wflags & 5) { atomicAdd(&L.stats[11], 1ull); atomicAdd(&L.stats[12], cyc); }
+      if (wflags & (kItemWarmDocs | kItemSweep)) { atomicAdd(&L.stats[11], 1ull); atomicAdd(&L.stats[12], cyc); }
       atomicAdd(&L.stats[13], (unsigned long long)dbg_tflush); atomicAdd(&L.stats[14], (unsigned long long)dbg_twait);
     }
   }
@@ -1015,12 +1002,7 @@ __global__ void slice_bounds_kernel(SliceBoundsLaunch B) {
   if (i >= (int64_t)B.nq * kT * per_slot) return;
   const int q = (int)(i / (kT * per_slot)), s = (int)((i / per_slot) % kT), e = (int)(i % per_slot);
   const DevQuery dq = B.queries[q];
-  const int fine = (B.slice_gran + B.parts_max - 1) / B.parts_max;
-  int64_t gran;
-  if (e < n_b) gran = (int64_t)(e / B.parts_max) * B.slice_gran + min(B.slice_gran, (e % B.parts_max) * fine);
-  else if (e == n_b) gran = B.n_gran;
-  else gran = min(kWarmGran, B.slice_gran);
-  if (gran > B.n_gran) gran = B.n_gran;
+  const int64_t gran = boundary_gran(e, B.n_slices, B.parts_max, B.slice_gran, B.n_gran);
   uint32_t out = 0;
   for (int c = 0; c < dq.n_clauses; ++c) {
     const DevClause cl = B.clauses[dq.clause_begin + c];

@@ -1,6 +1,6 @@
 """Wide batches: the window engine (bool_window_kernel, bool_kernel.cuh) against the exhaustive oracle.
 
-batch_build (nrtgpu.cu) picks the engine for a WHOLE batch: one query with more than 4 term clauses, or any top_k above
+compile_batch (csrc/batch_plan.inc) picks the engine for a WHOLE batch: one query with more than 4 term clauses, or any top_k above
 512, sends every query of the batch through bool_window_kernel -- 1,048,576-doc slices of 64 windows of 16,384 docs, a
 4096-key candidate buffer compacted mid-window, exact_freq_slow for tf >= 255, a dense-driver sweep for match-all and
 range-led queries -- then merge_slices_kernel, and merge_pairs_kernel across leaves, at up to top_k 1024.
@@ -31,7 +31,7 @@ N_MIX = 600_000             # > PROBE_SLICE: probe and window batches differ in 
 # ---------------------------------------------------------------- helpers
 
 def n_nonempty(queries):
-    """Queries batch_build gives work items: not (msm > #SHOULD, or no MUST / FILTER / SHOULD clause at all)."""
+    """Queries plan_work gives work items: not (msm > #SHOULD, or no MUST / FILTER / SHOULD clause at all)."""
     carr, _, qarr, nq = compile_queries(queries)
     n = 0
     for i in range(nq):
@@ -232,7 +232,7 @@ def test_clause_mix_5_to_8_terms(mix):
 
 
 def test_16_clauses_run_17_and_9_terms_refused(mix):
-    """The clause limits of batch_build: 8 term + 8 range clauses is the widest query the GPU path runs (and it runs
+    """The clause limits of compile_batch: 8 term + 8 range clauses is the widest query the GPU path runs (and it runs
     wide, equal to the oracle); a 17th clause or a 9th term clause is UNSUPPORTED."""
     sh, oix, gix, extra = mix
     q16 = BooleanQuery()
