@@ -835,8 +835,8 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
           P.aggs = b->agg_launch.p;
         }
         if (debug) {
-          if (!b->probe_stats.p && (rc_dbg = b->probe_stats.alloc(32))) return rc_dbg;
-          NRT_CUDA_TRY(cudaMemsetAsync(b->probe_stats.p, 0, 32 * sizeof(unsigned long long), st));
+          if (!b->probe_stats.p && (rc_dbg = b->probe_stats.alloc(2 * v3::kProbeStats))) return rc_dbg;
+          NRT_CUDA_TRY(cudaMemsetAsync(b->probe_stats.p, 0, 2 * v3::kProbeStats * sizeof(unsigned long long), st));
         }
         // configuration A (3 CTAs / SM) for the pruned sweeps of TOP_SCORES, B (4 CTAs / SM) where every posting is visited
         const bool cfg_b_simple = ix_ctx_probe_cfg(b->ix->ctx, P.threshold >= (int64_t)INT32_MAX);
@@ -861,7 +861,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         if (b->plan.n_probe_generic > 0) {
           P.work_query = L.work_query + b->plan.n_probe_simple; P.work_slice = L.work_slice + b->plan.n_probe_simple;
           P.n_work = b->plan.n_probe_generic; P.work_counter = b->work_counter.p + 1;
-          P.stats = debug ? b->probe_stats.p + 16 : nullptr;
+          P.stats = debug ? b->probe_stats.p + v3::kProbeStats : nullptr;
           launch(std::false_type{}, cfg_b_generic, b->plan.n_probe_generic);
         }
         NRT_CUDA_TRY(cudaGetLastError());
@@ -872,16 +872,16 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   }
   NRT_CUDA_TRY(cudaEventRecord(ev[1], st));
   if (debug && b->probe_stats.p && !b->cb.wide) {
-    unsigned long long h[32];
+    unsigned long long h[2 * v3::kProbeStats];
     NRT_CUDA_TRY(cudaMemcpyAsync(h, b->probe_stats.p, sizeof(h), cudaMemcpyDeviceToHost, st));
     NRT_CUDA_TRY(cudaStreamSynchronize(st));
     for (int k = 0; k < 2; ++k) {
-      const unsigned long long* x = h + 16 * k;
+      const unsigned long long* x = h + v3::kProbeStats * k;
       if (x[0]) fprintf(stderr, "[nrtgpu probe %s] longest item %llu cyc; CTA busy: mean %.0f max %llu cyc; warm-up items %llu, %.0f cyc each; per item: flush %.0f cyc (sort %.0f), TMA wait %.0f cyc\n", k == 0 ? "simple" : "generic",
                         x[8], (double)x[9] / std::min<double>((double)x[0], (double)(v3::kCtasA * b->ix->ctx->plan.sm_count)), x[10], x[11], x[11] ? (double)x[12] / x[11] : 0.0, (double)x[13] / x[0], (double)x[15] / x[0], (double)x[14] / x[0]);
-      if (x[0]) fprintf(stderr, "[nrtgpu probe %s] %llu items, %.0f cyc/item (set-up %.0f), %.2f runs/item (%.2f staged), %.1f rounds/item, %llu driver postings (%.0f/item), %.2f flushes/item\n",
+      if (x[0]) fprintf(stderr, "[nrtgpu probe %s] %llu items, %.0f cyc/item (set-up %.0f), %.2f runs/item (%.2f staged), %.1f rounds/item, %llu driver postings (%.0f/item), %.0f queued/item, %.0f keys admitted/item, %.2f flushes/item\n",
                         k == 0 ? "simple" : "generic", x[0], (double)x[1] / x[0], (double)x[6] / x[0], (double)x[2] / x[0], (double)x[5] / x[0],
-                        (double)x[7] / x[0], x[3], (double)x[3] / x[0], (double)x[4] / x[0]);
+                        (double)x[7] / x[0], x[3], (double)x[3] / x[0], (double)x[16] / x[0], (double)x[17] / x[0], (double)x[4] / x[0]);
     }
   }
   MergeLaunch M;

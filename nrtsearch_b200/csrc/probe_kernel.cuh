@@ -17,8 +17,8 @@
 //     a granule-narrowed binary search of the list's slice segment staged in shared memory by 1-D TMA bulk copies
 //     (cp.async.bulk + mbarrier complete_tx). No window array, no scatter, no per-window barriers: one barrier per
 //     round of kR * 256 postings, whose gathers are all in flight together;
-//   * pure disjunctions: rank-safe tf-pattern bound test before a doc is appended, UNSCORED, to the candidate
-//     buffer; the exact Lucene floats (BM25Scorer expression, double clause sums) are computed at the buffer flush;
+//   * pure disjunctions: rank-safe tf-pattern bound test, then the exact Lucene floats (BM25Scorer expression, double
+//     clause sums) a full warp at a time; only a key that beats the query's threshold enters the candidate buffer;
 //     MAXSCORE partition from index-time list bounds and the query's running threshold theta (one global 64-bit word
 //     per query, atomicMax: the device analogue of LazyMaxScoreAccumulator.java:21-70);
 //   * exact totalHits without sweeping the densest list: hits = |L1| + sum over the other lists of the postings whose
@@ -87,10 +87,13 @@ constexpr int kLongReserve = kT * (kGran + 2 * kAlign);   // one granule of ever
 constexpr int kR = NRT_PROBE_R;              // driver postings per thread per round (their gathers are in flight together)
 constexpr int kCand = 1024;                  // candidate buffer entries
 static_assert(kProbeMaxTopK == kCand / 2, "the probe kernel keeps top_k <= half its candidate buffer");
-constexpr int kUbt = 6 * 6 * 6 * 6;
+constexpr int kUbt = 4 * 4 * 4 * 4;          // tf-pattern bounds: min(tf, 3) per slot
+constexpr int kWq = 32 * kR;                 // per-warp queue entries: the rounds drain it below 32 after their first push; once
+                                             // the buffer is full, the kR - 1 pushes left in the round are not drained
+constexpr int kProbeStats = 24;              // stats words per instantiation (ProbeLaunch::stats)
 constexpr uint32_t kPiece = 8192;            // bytes per bulk copy
 constexpr uint32_t kTfInexact = 0xFEu;       // tf byte of a plane probe whose 2-bit code saturated (tf >= 3): the exact byte is
-                                             // fetched from the byte plane when the doc is scored (rare); >= 5 for the bound table
+                                             // fetched from the byte plane when the doc is scored (rare); >= 3 for the bound table
 
 enum { kAbsent = 0, kLong = 1, kShort = 2, kPlane = 3, kGlobal = 4 };
 
@@ -103,7 +106,9 @@ struct ProbeLaunch {
   const uint32_t* sbounds;       // [nq][kT][n_slices * parts_max + 2]: postings of the slot's list below every part boundary, the shard end, the warm-up boundary
   const uint8_t* field_min_norm;
   unsigned int* work_counter;    // queue head
-  unsigned long long* stats;     // optional [8]: items, item cycles, runs, driver postings, flushes, staged postings, set-up cycles, rounds
+  unsigned long long* stats;     // optional [kProbeStats]: items, item cycles, runs, driver postings, flushes, staged runs, set-up
+                                 // cycles, rounds, longest item, CTA busy (sum, max), warm-up items and cycles, flush, TMA wait and
+                                 // sort cycles, queued entries, admitted keys
   int32_t n_work, n_lists, n_slices, top_k;
   int32_t parts_max;             // result lists / boundary entries per slice (a heavy (query, slice) is split into up to this many items)
   int32_t slice_docs;            // multiple of kGran, <= kMaxSliceGran * kGran
@@ -143,8 +148,9 @@ struct alignas(128) ProbeSmemT {
   uint8_t sf8[kStageT];
   uint32_t gb[kT][kMaxSliceGran + 4];   // granule offsets of the slice for lists with skip data (relative to the list's first posting)
   uint64_t cand[kCand];
+  uint2 wq[kThreads / 32][kWq];    // per-warp queues of (doc, tf word) awaiting their score / clause evaluation
   float ubt[kUbt];
-  float uval[kT][4];
+  float uval[kT][2];
   DevClause cl[kMaxClauses];
   DevQuery q;
   uint64_t stage_bar;
@@ -175,7 +181,6 @@ struct alignas(128) ProbeSmemT {
   int wi;
   int skip;                        // the claimed item is not processed (abort flag set)
   int cand_count;
-  int n_keys;
   unsigned long long hits0;
   unsigned long long hits_known;   // max(hits0, docs known to match)
   int theta_dec;                   // 1: the item publishes (k-th key - 1) as threshold (sweep warm-up: its candidates are not output)
@@ -285,73 +290,13 @@ __device__ __forceinline__ float score_disjunction(const ProbeLaunch& L, const S
   return (float)sum;
 }
 
-// Candidate buffer flush (all threads). Entries [0, n_keys) are keys kept by the previous flush; the rest are keys
-// (generic) or unscored (tf word << 32 | doc) pairs (pure disjunctions) which are scored here, one per thread, so the norm
-// loads of the whole buffer overlap. Keeps the best top_k, publishes the k-th key as the query's threshold.
-template <bool kSimple, typename SM>
-__device__ __noinline__ void flush_candidates(const ProbeLaunch& L, SM& sm, const uint8_t* norms0, int n_term,
-                                                 bool has_after, uint64_t after_key, int top_k, uint64_t* g_theta) {
+// Candidate buffer flush (all threads; the buffer holds keys only): keeps the best top_k, publishes the k-th key (minus
+// theta_dec) as the query's threshold.
+template <typename SM>
+__device__ __noinline__ void flush_candidates(const ProbeLaunch& L, SM& sm, int top_k, uint64_t* g_theta) {
   __syncthreads();
   int n = sm.cand_count;
   if (n > kCand) n = kCand;
-  if (kSimple) {
-    const unsigned long long theta = sm.theta;
-    const int n_keys = sm.n_keys;
-    constexpr int kPer = kCand / kThreads;
-    uint64_t mine[kPer];
-    // every gather of the thread's candidates is issued before the first score is computed: the norm byte, and the
-    // exact tf byte of every slot whose 2-bit plane code saturated
-    uint32_t nbv[kPer], wv[kPer];
-#pragma unroll
-    for (int j = 0; j < kPer; ++j) {
-      const int i = n_keys + (int)threadIdx.x + j * kThreads;
-      mine[j] = (i < n) ? sm.cand[i] : 0ull;
-      const int32_t doc = (int32_t)(uint32_t)mine[j];
-      nbv[j] = (mine[j] && norms0) ? (uint32_t)__ldg(norms0 + doc) : 1u;
-      uint32_t w = (uint32_t)(mine[j] >> 32);
-#pragma unroll
-      for (int s2 = 0; s2 < kT; ++s2)
-        if (((w >> (8 * s2)) & 0xffu) == kTfInexact && sm.s_plane[s2])
-          w = (w & ~(0xffu << (8 * s2))) | ((uint32_t)__ldg(sm.s_plane[s2] + doc) << (8 * s2));
-      wv[j] = w;
-    }
-#pragma unroll
-    for (int j = 0; j < kPer; ++j) {
-      uint64_t key = 0ull;
-      if (mine[j]) {
-        const int32_t doc = (int32_t)(uint32_t)mine[j];
-        double sum = 0.0;   // BM25Scorer.score per slot (float), DisjunctionSumScorer / MaxScoreBulkScorer sum in double, slot order
-#pragma unroll
-        for (int s2 = 0; s2 < kT; ++s2) {
-          const uint32_t b = (wv[j] >> (8 * s2)) & 0xffu;
-          if (s2 >= n_term || b == 0u) continue;
-          const float f = (b == 255u) ? exact_freq_slow<uint32_t>(L.ix, sm.cl[sm.s_clause[s2]], doc) : (float)b;
-          sum += (double)bm25_score(sm.s_weight[s2], f, __ldg(&L.ix.caches[sm.s_field[s2] * 256 + nbv[j]]));
-        }
-        key = make_key((float)sum, doc);
-        if (!(key > theta) || (has_after && !(key < after_key))) key = 0ull;   // a real key is never 0
-      }
-      mine[j] = key;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) sm.cand_count = n_keys;
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < kPer; ++j)
-      if (mine[j]) sm.cand[atomicAdd(&sm.cand_count, 1)] = mine[j];
-    __syncthreads();
-    n = sm.cand_count;
-    if (n < top_k) {   // fewer than top_k keys in all: nothing to drop, no k-th key to publish (the slice merge sorts)
-      __syncthreads();   // every thread has read cand_count before anybody appends again
-      if (threadIdx.x == 0) {
-        sm.n_keys = n;
-        const unsigned long long g = *(volatile unsigned long long*)g_theta;
-        if (g > sm.theta) sm.theta = g;
-      }
-      __syncthreads();
-      return;
-    }
-  }
   const int m = next_pow2(n < 2 ? 2 : n);
   const long long ts = L.stats ? clock64() : 0ll;
   for (int i = n + threadIdx.x; i < m; i += kThreads) sm.cand[i] = 0ull;
@@ -361,7 +306,6 @@ __device__ __noinline__ void flush_candidates(const ProbeLaunch& L, SM& sm, cons
   if (threadIdx.x == 0) {
     const int keep = n < top_k ? n : top_k;
     sm.cand_count = keep;
-    sm.n_keys = keep;
     if (keep == top_k) {
       const unsigned long long kth = sm.cand[top_k - 1] - (unsigned long long)sm.theta_dec;
       const unsigned long long old = atomicMax((unsigned long long*)g_theta, kth);
@@ -443,7 +387,6 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     if (tid == 0) {
       sm.q = L.queries[qi];
       sm.cand_count = 0;
-      sm.n_keys = 0;
       sm.theta = *(volatile unsigned long long*)&L.theta[qi];
       sm.hits0 = *(volatile unsigned long long*)&L.total_hits[qi];
       { const unsigned long long kn = L.known_hits ? L.known_hits[qi] : 0ull; sm.hits_known = kn > sm.hits0 ? kn : sm.hits0; }
@@ -490,8 +433,8 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       const uint32_t* row = L.ix.gran_tab + (size_t)c.gran_row * (size_t)(L.n_gran + 1) + g_first;
       for (int g = g_lo + tid; g <= g_hi; g += kThreads) sm.gb[c.slot][g] = __ldg(row + g);
     }
-    if (kSimple && tid >= 64 && tid < 64 + 4 * kT) {   // per-slot score bounds at tf = 1..4 (shortest field length present)
-      const int s = (tid - 64) >> 2, c = ((tid - 64) & 3) + 1;
+    if (kSimple && tid >= 64 && tid < 64 + 2 * kT) {   // per-slot score bounds at tf = 1, 2 (shortest field length present)
+      const int s = (tid - 64) >> 1, c = ((tid - 64) & 1) + 1;
       float u = 0.0f;
       for (int i = 0; i < ncl; ++i)
         if (sm.cl[i].kind == NRTGPU_TERM && sm.cl[i].slot == s) {
@@ -502,16 +445,16 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     }
     __syncthreads();   // B2: descriptors, granule offsets, bound values
     if (kSimple) {
-      // ubt[sum min(tf_s, 5) * 6^s]: the double clause sum with every term at the shortest field length present
-      // (tf >= 5 bounded by the clause weight, the limit tf -> inf) -- an upper bound of the doc's score
-      const int n_ubt = n_term >= 4 ? kUbt : (n_term == 3 ? 216 : (n_term == 2 ? 36 : 6));   // patterns of the slots that exist
+      // ubt[sum min(tf_s, 3) * 4^s]: the double clause sum with every term at the shortest field length present
+      // (tf >= 3 bounded by the clause weight, the limit tf -> inf) -- an upper bound of the doc's score
+      const int n_ubt = 1 << (2 * min(n_term, kT));   // patterns of the slots that exist
       for (int i = tid; i < n_ubt; i += kThreads) {
-        const int c[kT] = {i % 6, (i / 6) % 6, (i / 36) % 6, i / 216};
+        const int c[kT] = {i & 3, (i >> 2) & 3, (i >> 4) & 3, i >> 6};
         double sum = 0.0;
 #pragma unroll
         for (int t = 0; t < kT; ++t) {
           float u = 0.0f;
-          if (sm.s_kind[t] != kAbsent && c[t] > 0) u = (c[t] <= 4) ? sm.uval[t][c[t] - 1] : sm.s_weight[t];
+          if (sm.s_kind[t] != kAbsent && c[t] > 0) u = (c[t] <= 2) ? sm.uval[t][c[t] - 1] : sm.s_weight[t];
           sum += (double)u;
         }
         sm.ubt[i] = (float)sum;
@@ -599,14 +542,10 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     __syncthreads();   // B3: roles, staging plan
 
     const int32_t slice_base = slice * L.slice_docs;
-    const bool has_after = sm.q.has_after != 0;
-    const uint64_t after_key = sm.q.after_key;
-    const uint8_t* norms0 = (kSimple && sm.q.single_field >= 0) ? L.ix.norms[sm.q.single_field] : nullptr;
     const uint32_t drv_mask = sm.drv_mask, ess_mask = sm.ess_mask;
     const uint32_t plane_mask = sm.plane_mask, long_mask = sm.long_mask, short_mask = sm.short_mask, global_mask = sm.global_mask;
-    const uint8_t* pl0 = sm.s_plane2[0]; const uint8_t* pl1 = sm.s_plane2[1]; const uint8_t* pl2 = sm.s_plane2[2]; const uint8_t* pl3 = sm.s_plane2[3];
     unsigned int my_hits = 0;
-    unsigned long long dbg_post = 0; unsigned int dbg_runs = 0, dbg_rounds = 0, dbg_flush = 0, dbg_staged = 0;
+    unsigned long long dbg_post = 0; unsigned int dbg_runs = 0, dbg_rounds = 0, dbg_flush = 0, dbg_staged = 0, dbg_queued = 0, dbg_admit = 0;
     long long dbg_tflush = 0, dbg_twait = 0;
     const long long t_setup = kStats ? clock64() : 0ll;
 
@@ -746,57 +685,64 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       // where its postings live, who owns a doc) is loop invariant.
       int ct = 0;           // driver slot this thread is working on
       uint32_t cb = 0;      // first posting (of the slot's run segment) of the thread's next round
-      uint64_t park[kR];
-      uint32_t pmask = 0;   // parked candidates of this thread
-      // generic queries: per-warp queue of (doc, tf word) pairs awaiting clause evaluation (lives in the bound table's
-      // shared memory, which only pure disjunctions use); qn is warp-uniform
-      uint2* const wq = reinterpret_cast<uint2*>(sm.ubt) + (tid >> 5) * 64;
-      static_assert(kUbt * sizeof(float) >= (kThreads / 32) * 64 * sizeof(uint2), "warp queues do not fit the bound table");
+      uint64_t park = 0ull;   // this thread's key that did not fit the buffer
+      bool parked = false;
+      // Per-warp queue of the (doc, tf word) pairs that passed the cheap tests of the round: most driver postings fail
+      // them, so scoring (pure disjunctions) or the clause evaluation (generic queries) would run with a handful of lanes.
+      // The queue is drained 32 entries at a time; qn is warp-uniform.
+      uint2* const wq = sm.wq[tid >> 5];
       int qn = 0;
       const uint32_t q_req = sm.q.req_term_mask, q_not = sm.q.not_term_mask;
-      auto drain = [&](int n_take) -> bool {   // evaluates the last n_take (<= 32) queued pairs; true: a lane had to park its hit
+      auto drain = [&](int n_take) -> bool {   // evaluates the last n_take (<= 32) queued pairs; true: a lane had to park its key
         __syncwarp();
-        bool parked = false;
+        bool fail = false;
         const bool have = lane < n_take;
         const uint2 e = have ? wq[qn - n_take + lane] : make_uint2(0u, 0u);
         qn -= n_take;
-        float score;
-        if (have && evaluate_doc(L, sm, (int32_t)e.x, e.y, &score)) {
-          const int32_t d = (int32_t)e.x;
-          ++my_hits;
-          if (L.aggs) agg_collect(*L.aggs, L.ix, qi, d);   // additional collectors see every matching doc
-          uint64_t entry;
-          if (L.sort_kind == NRTGPU_SORT_RELEVANCE || L.sort_kind == kSortScoreRank) {
-            entry = make_key(score, d);
-            // [score, ...] order: ties by the order's rank, which takes the doc's place; ordered(-s) == ~ordered(s) for reverse
-            if (L.sort_kind == kSortScoreRank) entry = make_key(L.sort_reverse ? -score : score, (int32_t)__ldg(L.sort_codes + d));
-          } else {   // TopFieldCollector: the key is the doc's sort value (order-preserving code), ties by doc id
-            uint32_t code = 0;
-            if (L.sort_kind == NRTGPU_SORT_COLUMN) { code = __ldg(L.sort_codes + d); if (code == 0u) code = sort_missing; }
-            entry = ((uint64_t)sort_hi(L.sort_kind, L.sort_reverse, code, d) << 32) | (uint32_t)(~(uint32_t)d);
+        const int32_t d = (int32_t)e.x;
+        uint64_t entry = 0ull;   // a real key is never 0: 0 fails the threshold test below
+        if (kSimple) {
+          if (have) {   // (the query's norms and after key are read here: registers are scarce across the rounds)
+            const uint8_t* norms0 = sm.q.single_field >= 0 ? L.ix.norms[sm.q.single_field] : nullptr;
+            entry = make_key(score_disjunction(L, sm, norms0, n_term, d, e.y), d);
           }
-          const unsigned long long th = sm.theta;
-          if (entry > th && !(has_after && !(entry < after_key)) && !NRT_KNOCK(4)) {
-            const int p = atomicAdd(&sm.cand_count, 1);
-            if (p < kCand) sm.cand[p] = entry;
-            else { park[0] = entry; pmask |= 1u; parked = true; }
+        } else {
+          float score;
+          if (have && evaluate_doc(L, sm, d, e.y, &score)) {
+            ++my_hits;
+            if (L.aggs) agg_collect(*L.aggs, L.ix, qi, d);   // additional collectors see every matching doc
+            if (L.sort_kind == NRTGPU_SORT_RELEVANCE || L.sort_kind == kSortScoreRank) {
+              entry = make_key(score, d);
+              // [score, ...] order: ties by the order's rank, which takes the doc's place; ordered(-s) == ~ordered(s) for reverse
+              if (L.sort_kind == kSortScoreRank) entry = make_key(L.sort_reverse ? -score : score, (int32_t)__ldg(L.sort_codes + d));
+            } else {   // TopFieldCollector: the key is the doc's sort value (order-preserving code), ties by doc id
+              uint32_t code = 0;
+              if (L.sort_kind == NRTGPU_SORT_COLUMN) { code = __ldg(L.sort_codes + d); if (code == 0u) code = sort_missing; }
+              entry = ((uint64_t)sort_hi(L.sort_kind, L.sort_reverse, code, d) << 32) | (uint32_t)(~(uint32_t)d);
+            }
           }
         }
+        // sm.theta never decreases within an item, so a key dropped here would not survive a flush either
+        const unsigned long long th = sm.theta;
+        if (entry > th && !(sm.q.has_after && !(entry < sm.q.after_key)) && !NRT_KNOCK(4)) {
+          if (kStats) ++dbg_admit;
+          const int p = atomicAdd(&sm.cand_count, 1);
+          if (p < kCand) sm.cand[p] = entry;
+          else { park = entry; parked = true; fail = true; }
+        }
         __syncwarp();
-        return parked;
+        return fail;
       };
       for (;;) {
         bool full = false;
-#pragma unroll
-        for (int j = 0; j < kR; ++j)
-          if ((pmask >> j) & 1u) {
-            const int p = atomicAdd(&sm.cand_count, 1);
-            if (p < kCand) { sm.cand[p] = park[j]; pmask &= ~(1u << j); } else full = true;
-          }
-        if (!kSimple) {   // the warp moves together (its queue operations are collective); a queue left >= 32 by a full buffer is
-          full = __any_sync(0xffffffffu, full);   // brought below 32 before the sweep pushes again (capacity 64)
-          while (!full && qn >= 32) full = __any_sync(0xffffffffu, drain(32));
+        if (parked) {
+          const int p = atomicAdd(&sm.cand_count, 1);
+          if (p < kCand) { sm.cand[p] = park; parked = false; } else full = true;
         }
+        // the warp moves together (its queue operations are collective); a queue left >= 32 by a full buffer is brought
+        // below 32 before the sweep pushes again
+        full = __any_sync(0xffffffffu, full);
+        while (!full && qn >= 32) full = __any_sync(0xffffffffu, drain(32));
         const int ct_end = NRT_KNOCK(8) ? 0 : (dense ? n_term + 1 : n_term);   // dense: one more "list" = every doc of the run
         while (!full && ct < ct_end) {
           const bool t_dense = ct == n_term;
@@ -841,10 +787,10 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
             for (int j = 0; j < kR; ++j) {
               const uint32_t d4 = (uint32_t)max(doc[j], 0) >> 2;
               pbyte[j][0] = 0u; pbyte[j][1] = 0u; pbyte[j][2] = 0u; pbyte[j][3] = 0u;
-              if (need_plane & 1u) pbyte[j][0] = (uint32_t)__ldg(pl0 + d4);
-              if (need_plane & 2u) pbyte[j][1] = (uint32_t)__ldg(pl1 + d4);
-              if (need_plane & 4u) pbyte[j][2] = (uint32_t)__ldg(pl2 + d4);
-              if (need_plane & 8u) pbyte[j][3] = (uint32_t)__ldg(pl3 + d4);
+              if (need_plane & 1u) pbyte[j][0] = (uint32_t)__ldg(sm.s_plane2[0] + d4);
+              if (need_plane & 2u) pbyte[j][1] = (uint32_t)__ldg(sm.s_plane2[1] + d4);
+              if (need_plane & 4u) pbyte[j][2] = (uint32_t)__ldg(sm.s_plane2[2] + d4);
+              if (need_plane & 8u) pbyte[j][3] = (uint32_t)__ldg(sm.s_plane2[3] + d4);
             }
             // next round's postings
             {
@@ -879,68 +825,55 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
                 }
               }
             }
-            // ownership, hit count, bound test, append (pure disjunctions; the generic path follows)
+            // ownership, hit count and the cheap tests of every posting of the round, then the survivors are queued (the
+            // gathered bytes are dead before the first drain)
+            uint32_t surv_mask = 0;
 #pragma unroll
-            for (int j = 0; kSimple && j < kR; ++j) {
-              if (doc[j] < 0) continue;
+            for (int j = 0; j < kR; ++j) {
               uint32_t v = word[j];
               if (need_plane) {
                 // the four gathered bytes side by side; the doc's 2-bit code of every plane with one shift and one mask
                 // (bits shifted in from the neighbouring byte fall outside the mask); code 3 = "three or more" becomes
                 // kTfInexact (resolved when the doc is scored)
                 const uint32_t raw = pbyte[j][0] | (pbyte[j][1] << 8) | (pbyte[j][2] << 16) | (pbyte[j][3] << 24);
-                const uint32_t codes = (raw >> (((uint32_t)doc[j] & 3u) * 2u)) & 0x03030303u;
+                const uint32_t codes = (raw >> (((uint32_t)max(doc[j], 0) & 3u) * 2u)) & 0x03030303u;
                 const uint32_t sat = __vcmpeq4(codes, 0x03030303u);   // 0xff where the code saturated
                 v |= (codes & ~sat) | (sat & (kTfInexact * 0x01010101u));
               }
-              uint64_t entry;
+              bool surv = false;
               if (kSimple) {
-                if (live && !((live[doc[j] >> 5] >> (doc[j] & 31)) & 1u)) continue;   // deleted docs are neither counted nor collected
-                if ((v & cntbefore) == 0u) ++my_hits;
-                if (!t_ess || (v & candbelow) != 0u) continue;   // counted only / emitted by a lower list
-                if (sm.ubt[__dp4a(__vminu4(v, 0x05050505u), 0xD8240601u, 0u)] < theta_s) continue;   // cannot reach the top-k
-                entry = ((uint64_t)v << 32) | (uint32_t)doc[j];   // scored at the next flush
-              } else {
-                continue;   // (generic queries: the survivors of the round are queued below and evaluated a full warp at a time)
-              }
-              if (NRT_KNOCK(4)) continue;
-              const int p = atomicAdd(&sm.cand_count, 1);
-              if (p < kCand) sm.cand[p] = entry;
-              else { park[j] = entry; pmask |= 1u << j; full = true; }
-            }
-            if (!kSimple) {
-              // Generic queries: most driver postings fail the other required lists, so the clause evaluation (norm and
-              // doc-value gathers, BM25) would run with a handful of lanes. The survivors of the cheap tests -- not owned by
-              // a lower list, every required term present, no excluded term -- go to a per-warp queue and are evaluated
-              // 32 at a time.
-#pragma unroll
-              for (int j = 0; j < kR; ++j) {
-                uint32_t v = word[j];
-                if (need_plane) {
-                  const uint32_t raw = pbyte[j][0] | (pbyte[j][1] << 8) | (pbyte[j][2] << 16) | (pbyte[j][3] << 24);
-                  const uint32_t codes = (raw >> (((uint32_t)max(doc[j], 0) & 3u) * 2u)) & 0x03030303u;
-                  const uint32_t sat = __vcmpeq4(codes, 0x03030303u);
-                  v |= (codes & ~sat) | (sat & (kTfInexact * 0x01010101u));
+                // deleted docs are neither counted nor collected; a doc owned by a lower list is counted there; a doc whose
+                // tf-pattern bound is below the threshold cannot reach the top-k
+                if (doc[j] >= 0 && !(live && !((live[doc[j] >> 5] >> (doc[j] & 31)) & 1u))) {
+                  if ((v & cntbefore) == 0u) ++my_hits;
+                  surv = t_ess && (v & candbelow) == 0u && !(sm.ubt[__dp4a(__vminu4(v, 0x03030303u), 0x40100401u, 0u)] < theta_s);
                 }
+              } else {   // not owned by a lower list, every required term present, no excluded term
                 const uint32_t pres = presence4(v);
-                const bool surv = doc[j] >= 0 && (v & candbelow) == 0u && (pres & q_req) == q_req && (pres & q_not) == 0u;
-                const unsigned bal = __ballot_sync(0xffffffffu, surv);
-                if (surv) wq[qn + __popc(bal & ((1u << lane) - 1u))] = make_uint2((uint32_t)doc[j], v);
-                qn += __popc(bal);
-                while (!full && qn >= 32) full = __any_sync(0xffffffffu, drain(32));   // (a parked hit stops the warp: park[0] is free whenever drain runs)
+                surv = doc[j] >= 0 && (v & candbelow) == 0u && (pres & q_req) == q_req && (pres & q_not) == 0u;
               }
+              word[j] = v;
+              surv_mask |= surv ? 1u << j : 0u;
+            }
+#pragma unroll
+            for (int j = 0; j < kR; ++j) {
+              const bool surv = (surv_mask >> j) & 1u;
+              const unsigned bal = __ballot_sync(0xffffffffu, surv);
+              if (surv) wq[qn + __popc(bal & ((1u << lane) - 1u))] = make_uint2((uint32_t)doc[j], word[j]);
+              qn += __popc(bal);
+              if (kStats && lane == 0) dbg_queued += __popc(bal);
+              while (!full && qn >= 32) full = __any_sync(0xffffffffu, drain(32));   // (a parked key stops the warp: park is free whenever drain runs)
             }
             cb += kR * kThreads;
             if (kStats && tid == 0) ++dbg_rounds;
           }
         }
-        if (!kSimple) {   // the rest of the warp's queue (a partial warp), unless the buffer is full: then after the flush
-          while (!full && qn > 0) full = __any_sync(0xffffffffu, drain(min(qn, 32)));
-        }
+        // the rest of the warp's queue (a partial warp), unless the buffer is full: then after the flush
+        while (!full && qn > 0) full = __any_sync(0xffffffffu, drain(min(qn, 32)));
         __syncthreads();
         if (sm.cand_count <= kCand) break;   // nobody is parked (the count passes kCand only through a failed append)
         const long long tf = kStats ? clock64() : 0ll;
-        flush_candidates<kSimple>(L, sm, norms0, n_term, has_after, after_key, L.top_k, &L.theta[qi]);
+        flush_candidates(L, sm, L.top_k, &L.theta[qi]);
         if (kStats) dbg_tflush += clock64() - tf;
         if (kStats) ++dbg_flush;
       }
@@ -951,9 +884,9 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
 
     // ---------------- finish the work item (the slice merge sorts, so only a full buffer needs ordering here)
     __syncthreads();
-    if (kSimple ? sm.cand_count > sm.n_keys : sm.cand_count > L.top_k) {
+    if (sm.cand_count > L.top_k) {
       const long long tf = kStats ? clock64() : 0ll;
-      flush_candidates<kSimple>(L, sm, norms0, n_term, has_after, after_key, L.top_k, &L.theta[qi]);
+      flush_candidates(L, sm, L.top_k, &L.theta[qi]);
       if (kStats) dbg_tflush += clock64() - tf;
       if (kStats) ++dbg_flush;
     }
@@ -964,6 +897,10 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     if (tid == 0) L.slice_cnt[(size_t)qi * L.n_lists + out_list] = keep;
     for (int o = 16; o > 0; o >>= 1) my_hits += __shfl_xor_sync(0xffffffffu, my_hits, o);
     if (lane == 0 && my_hits && !sweep_warm) atomicAdd(&L.total_hits[qi], (unsigned long long)my_hits);
+    if (kStats) {
+      for (int o = 16; o > 0; o >>= 1) dbg_admit += __shfl_xor_sync(0xffffffffu, dbg_admit, o);
+      if (lane == 0) { atomicAdd(&L.stats[16], (unsigned long long)dbg_queued); atomicAdd(&L.stats[17], (unsigned long long)dbg_admit); }
+    }
     if (kStats && tid == 0) {
       atomicAdd(&L.stats[0], 1ull);
       atomicAdd(&L.stats[1], (unsigned long long)(clock64() - t_start));
