@@ -256,11 +256,18 @@ int nrtgpu_search_sorted_fields(nrtgpu_index* ix, const nrtgpu_sort_order* order
  *                     (order_desc) or smallest counts, totalBuckets, totalOtherCounts
  *                     ({Int,Long,Float,Double}TermsCollectorManager + TermsCollectorManager.fillBucketResultByCount);
  *   NRTGPU_AGG_MIN / _MAX / _SUM   over the column's values as doubles (Min/Max/SumCollectorManager with the value
- *                     source doc['field'].value; no matching doc => Double.MAX_VALUE / -Double.MAX_VALUE / 0.0).
+ *                     source doc['field'].value). MAX keeps `value > maxValue` started from -Double.MAX_VALUE, MIN
+ *                     `value < minValue` from Double.MAX_VALUE: NaN never wins, nor does -inf for MAX or +inf for MIN
+ *                     (a max over {-inf} is -Double.MAX_VALUE). A query with no match, or a batch with no work (every
+ *                     query without clauses or with minimumNumberShouldMatch above its SHOULD count), gives
+ *                     Double.MAX_VALUE / -Double.MAX_VALUE / 0.0, and a terms aggregation no buckets.
  * value_type says how the column's sortable long maps back to the number: 0 int / long, 1 float, 2 double.
  * Docs without a value contribute nothing. Bucket ties at the cut are unordered in the reference (hash-map order); here
- * the smaller value wins. Float / double sums are accumulated in a different order than the reference's single
- * thread: equal within 1e-12 relative; int / long sums below 2^53, min, max and every count are exact. */
+ * the smaller value wins. Min, max (up to the sign of a zero, which depends on collection order in the reference too)
+ * and every count are exact. Sums are accumulated in a different order than the reference's single thread: for n finite
+ * values the two differ by at most n * 2^-53 * sum|v| (an absolute bound: cancelling values lose the relative one), so
+ * int / long sums with sum|v| < 2^53 are exact, and whether partial sums near Double.MAX_VALUE overflow depends on the
+ * order in both; with a NaN, or both infinities, the sum is NaN, else with an infinity that infinity. */
 enum { NRTGPU_AGG_TERMS = 1, NRTGPU_AGG_MIN = 2, NRTGPU_AGG_MAX = 3, NRTGPU_AGG_SUM = 4 };
 typedef struct {
   int32_t kind, column, value_type;

@@ -5,6 +5,7 @@
 //              .../search/collectors/additional/{Int,Long,Float,Double}TermsCollectorManager.java, Max/Min/SumCollectorManager.java,
 //              fan-out at .../search/SearchCollectorManager.java:192-198.
 #pragma once
+#include <cfloat>
 #include "bool_kernel.cuh"
 #include "../../include/nrtgpu.h"
 
@@ -177,8 +178,10 @@ __device__ __forceinline__ void agg_collect(const AggLaunch& A, const DevIndexVi
     } else {
       const int64_t raw = ix.col32[s.column] ? (int64_t)ix.col32[s.column][doc] : ix.col64[s.column][doc];
       const double v = agg_value(raw, s.value_type);
-      if (s.kind == NRTGPU_AGG_MAX) atomicMax(&s.dvals[q], double_to_ordered(v));
-      else if (s.kind == NRTGPU_AGG_MIN) atomicMin(&s.dvals[q], double_to_ordered(v));
+      // Max/MinCollectorManager keep `value > maxValue` (`value < minValue`) started from -/+Double.MAX_VALUE: NaN and the
+      // infinity on the unset side never win
+      if (s.kind == NRTGPU_AGG_MAX) { if (v > -DBL_MAX) atomicMax(&s.dvals[q], double_to_ordered(v)); }
+      else if (s.kind == NRTGPU_AGG_MIN) { if (v < DBL_MAX) atomicMin(&s.dvals[q], double_to_ordered(v)); }
       else atomicAdd(reinterpret_cast<double*>(&s.dvals[q]), v);
     }
   }

@@ -777,6 +777,19 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
     NRT_CUDA_TRY(cudaMemsetAsync(b->clock0.p, 0, sizeof(unsigned long long), st));
     NRT_CUDA_TRY(cudaMemsetAsync(b->timed_out.p, 0, b->timed_out.bytes(), st));
   }
+  // aggregation outputs start unset on every run, work items or not: batch_fetch_aggs reads those of THIS run.
+  // min starts at +inf / max at -inf in ordered-double space, sum at 0.0 (the "unset" values are applied at fetch)
+  for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
+    const nrtgpu_aggregation& a = b->cb.aggs[i];
+    if (a.kind == NRTGPU_AGG_TERMS) {
+      const int32_t nb = b->ix->col_n_distinct[(size_t)a.column];
+      if ((rc_dbg = b->agg_counts[i].alloc((size_t)b->nq * (size_t)std::max(nb, 1)))) return rc_dbg;
+      NRT_CUDA_TRY(cudaMemsetAsync(b->agg_counts[i].p, 0, b->agg_counts[i].bytes(), st));
+    } else {
+      if ((rc_dbg = b->agg_dvals[i].alloc((size_t)b->nq))) return rc_dbg;
+      NRT_CUDA_TRY(cudaMemsetAsync(b->agg_dvals[i].p, a.kind == NRTGPU_AGG_MIN ? 0xff : 0x00, b->agg_dvals[i].bytes(), st));
+    }
+  }
   const bool debug = b->ix->ctx->debug_modes;
   cudaEvent_t* ev = b->ev[b->runs_recorded % nrtgpu_batch::kEvRing];
   NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
@@ -817,16 +830,9 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
             const nrtgpu_aggregation& a = b->cb.aggs[(size_t)i];
             A.a[i].kind = a.kind; A.a[i].column = a.column; A.a[i].value_type = a.value_type;
             if (a.kind == NRTGPU_AGG_TERMS) {
-              const int32_t nb = b->ix->col_n_distinct[(size_t)a.column];
-              A.a[i].n_buckets = nb;
-              if ((rc_dbg = b->agg_counts[i].alloc((size_t)b->nq * (size_t)std::max(nb, 1)))) return rc_dbg;
-              NRT_CUDA_TRY(cudaMemsetAsync(b->agg_counts[i].p, 0, b->agg_counts[i].bytes(), st));
+              A.a[i].n_buckets = b->ix->col_n_distinct[(size_t)a.column];
               A.a[i].counts = b->agg_counts[i].p; A.codes[i] = b->ix->col_code[(size_t)a.column]->p;
             } else {
-              if ((rc_dbg = b->agg_dvals[i].alloc((size_t)b->nq))) return rc_dbg;
-              // min starts at +inf / max at -inf in ordered-double space, sum at 0.0 (the "unset" values are applied at fetch)
-              const int fill = a.kind == NRTGPU_AGG_MIN ? 0xff : 0x00;
-              NRT_CUDA_TRY(cudaMemsetAsync(b->agg_dvals[i].p, fill, b->agg_dvals[i].bytes(), st));
               A.a[i].dvals = b->agg_dvals[i].p;
             }
           }
