@@ -20,38 +20,13 @@
 // LazyMaxScoreAccumulator (src/main/java/org/apache/lucene/search/LazyMaxScoreAccumulator.java:21-70),
 // used here only to drop hits that provably cannot enter the top-k (results stay exact).
 #pragma once
-#include "common.cuh"
-#include "../../include/nrtgpu.h"
+#include "query_eval.cuh"
 
 namespace nrtgpu {
 
 // (DevClause, DevQuery, the clause / slot / top_k limits and the window size: batch_plan.h)
 constexpr int kCandCap = 4096;      // candidate buffer (keys) per CTA, power of two
 constexpr int kThreads = 512;
-
-struct DevIndexView {
-  int32_t n_docs;
-  int32_t doc_base;
-  const int32_t* post_docs;
-  const uint8_t* post_f8;        // min(freq, 255)
-  const int64_t* exc_pos;        // sorted global posting indices with freq >= 255
-  const int32_t* exc_freq;
-  int32_t n_exc;
-  const uint8_t* const* norms;   // [n_fields] device pointers (NULL = omitNorms)
-  const float* caches;           // [n_fields][256]
-  const int64_t* const* col64;   // [n_columns] (NULL if stored as int32)
-  const int32_t* const* col32;   // [n_columns] (NULL if stored as int64)
-  const uint8_t* const* col_has; // [n_columns] (NULL = all)
-  const int64_t* const* colmv_off;  // [n_columns] multi-valued columns (SORTED_NUMERIC): doc d holds colmv_val[c][off[d] .. off[d + 1]),
-  const int64_t* const* colmv_val;  //              ascending; NULL entry = single-valued column
-  const uint32_t* live_bits;     // bitmap or NULL
-  const uint32_t* gran_tab;      // [n_rows][n_gran + 1] postings of the term below each 1024-doc granule boundary (skip data)
-  int32_t n_gran;
-  const uint8_t* dense_tf;       // [n_planes][dense_stride] min(freq, 255) per doc for the densest terms (0 = absent)
-  int64_t dense_stride;
-  const uint8_t* dense_tf2;      // [n_planes][dense_stride / 4] min(freq, 3) in 2 bits per doc: the planes the probe kernel gathers
-                                 // (a quarter of the L2 / DRAM footprint of the byte planes; 3 = "three or more")
-};
 
 struct BoolLaunch {
   DevIndexView ix;
@@ -73,22 +48,6 @@ struct BoolLaunch {
   int32_t* timed_out;          // [nq]
 };
 
-// numeric range clause on one doc (IndexOrDocValuesQuery's doc-values side, reference IntFieldDef.java:124-158 inclusive
-// bounds): single-valued column = the value is in [lo, hi]; multi-valued (SortedNumericDocValuesRangeQuery) = ANY value is
-__device__ __forceinline__ bool range_matches(const DevIndexView& ix, int col, int32_t doc, int64_t lo, int64_t hi) {
-  const int64_t* off = ix.colmv_off ? ix.colmv_off[col] : nullptr;
-  if (off) {
-    const int64_t* v = ix.colmv_val[col];
-    int64_t a = off[doc], b = off[doc + 1];
-    while (a < b) { const int64_t m = (a + b) >> 1; if (v[m] < lo) a = m + 1; else b = m; }   // values of a doc are sorted
-    return a < off[doc + 1] && v[a] <= hi;
-  }
-  const uint8_t* has = ix.col_has[col];
-  if (has && !has[doc]) return false;
-  const int64_t x = ix.col32[col] ? (int64_t)__ldg(ix.col32[col] + doc) : __ldg(ix.col64[col] + doc);
-  return x >= lo && x <= hi;
-}
-
 struct BoolSmem {
   uint64_t slots[kWindowDocs];   // one tf byte per term slot
   uint64_t cand[kCandCap];
@@ -109,106 +68,24 @@ __device__ __forceinline__ uint32_t presence_mask(uint64_t s) {
   return m;
 }
 
-// exact tf of posting (clause c, doc) when the byte saturated: find the posting, then the exception list.
-// Word is the tf word of the calling engine: uint64_t for the window kernel, uint32_t for the probe and collect kernels.
-// It only gives each engine its own out-of-line copy: one copy shared with the probe kernels costs the window kernel a
-// spilled register (8 more stack bytes, 4 bytes of spill stores and loads in ptxas -v).
-template <typename Word>
-__device__ __noinline__ float exact_freq_slow(const DevIndexView& ix, const DevClause& c, int32_t doc) {
-  const int32_t* docs = ix.post_docs + c.post_base;
-  int lo = 0, hi = c.n_post;
-  while (lo < hi) { int m = (lo + hi) >> 1; if (docs[m] < doc) lo = m + 1; else hi = m; }
-  int64_t gp = c.post_base + lo;
-  int a = 0, b = ix.n_exc;
-  while (a < b) { int m = (a + b) >> 1; if (ix.exc_pos[m] < gp) a = m + 1; else b = m; }
-  if (a < ix.n_exc && ix.exc_pos[a] == gp) return (float)ix.exc_freq[a];
-  return 255.0f;
-}
-
-// Evaluate the boolean constraints + score for one candidate doc. Returns false if the doc does not match.
-// Score combination follows Lucene's BooleanScorerSupplier: conjunction / disjunction sums are double,
-// required+optional is ReqOptSumScorer's float add (msm == 0) or ConjunctionScorer's double add (msm > 0).
+// the clauses of sm.q on one candidate doc; slot holds the doc's tf byte of every term slot
 __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolSmem& sm, int32_t doc,
                                              uint64_t slot, float* out_score) {
-  const DevQuery& q = sm.q;
-  uint32_t m = presence_mask(slot);
-  if ((m & q.req_term_mask) != q.req_term_mask) return false;
-  if (m & q.not_term_mask) return false;
-  if (ix.live_bits && !((ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
-  double must_sum = 0.0, should_sum = 0.0;
-  int n_req = 0, n_should = 0;
-  for (int i = 0; i < q.n_clauses; ++i) {
-    const DevClause& c = sm.cl[i];
-    bool present;
-    float s = 0.0f;
-    if (c.kind == NRTGPU_TERM) {
-      uint32_t b = (uint32_t)((slot >> (8 * c.slot)) & 0xff);
-      present = b != 0;
-      if (present && c.scoring) {
-        float f = (b == 255u) ? exact_freq_slow<uint64_t>(ix, c, doc) : (float)b;
-        const uint8_t* nrm = ix.norms[c.field];
-        uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
-        s = bm25_score(c.weight, f, sm.cache[c.slot][nb]);
-      }
-    } else if (c.kind == NRTGPU_RANGE_I64) {
-      present = range_matches(ix, c.col, doc, c.lo, c.hi);
-      s = c.weight;
-    } else {
-      present = true;
-      s = c.weight;
+  auto term = [&](const DevClause& c, float* s) {
+    const uint32_t b = (uint32_t)((slot >> (8 * c.slot)) & 0xff);
+    if (b == 0) return false;
+    if (c.scoring) {
+      const float f = (b == 255u) ? exact_freq_slow(ix, c, doc) : (float)b;
+      const uint8_t* nrm = ix.norms[c.field];
+      const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
+      *s = bm25_score(c.weight, f, sm.cache[c.slot][nb]);
     }
-    if (!present) {
-      if (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER) return false;
-      continue;
-    }
-    switch (c.occur) {
-      case NRTGPU_MUST: must_sum += (double)s; ++n_req; break;
-      case NRTGPU_FILTER: ++n_req; break;
-      case NRTGPU_SHOULD: should_sum += (double)s; ++n_should; break;
-      default: return false;  // MUST_NOT present
-    }
-  }
-  if (n_should < q.need_should) return false;
-  float score;
-  if (q.n_req == 0) score = (float)should_sum;
-  else {
-    float req = (float)must_sum;
-    if (n_should == 0) score = req;
-    else {
-      float opt = (float)should_sum;
-      score = (q.msm > 0) ? (float)((double)req + (double)opt) : __fadd_rn(req, opt);
-    }
-  }
-  *out_score = score;
-  return true;
+    return true;
+  };
+  return eval_clauses(ix, sm.q, sm.cl, doc, presence_mask(slot), term, out_score);
 }
 
-// sort the candidate buffer, keep the best top_k, raise theta (local + global)
-__device__ __forceinline__ void compact_candidates(BoolSmem& sm, int top_k, uint64_t* g_theta) {
-  __syncthreads();
-  int n = sm.cand_count;
-  if (n > kCandCap) n = kCandCap;  // cannot happen (capacity invariant); defensive
-  int m = next_pow2(n < 2 ? 2 : n);
-  for (int i = n + threadIdx.x; i < m; i += blockDim.x) sm.cand[i] = 0ull;
-  __syncthreads();
-  block_bitonic_sort_desc(sm.cand, m);
-  if (threadIdx.x == 0) {
-    int keep = n < top_k ? n : top_k;
-    sm.cand_count = keep;
-    if (keep == top_k) {
-      unsigned long long kth = sm.cand[top_k - 1];
-      unsigned long long old = atomicMax((unsigned long long*)g_theta, kth);
-      unsigned long long t = old > kth ? old : kth;
-      if (t > sm.theta) sm.theta = t;
-    } else {
-      unsigned long long g = *(volatile unsigned long long*)g_theta;
-      if (g > sm.theta) sm.theta = g;
-    }
-  }
-  __syncthreads();
-}
-
-__global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) {
+__global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_constant__ BoolLaunch L) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   BoolSmem& sm = *reinterpret_cast<BoolSmem*>(smem_raw);
   const int tid = threadIdx.x;
@@ -304,7 +181,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) 
         if (cand_ub > kCandCap - kThreads) {
           __syncthreads();
           int n = sm.cand_count;
-          if (n > kCandCap - kThreads) { compact_candidates(sm, L.top_k, &L.theta[qi]); n = sm.cand_count; }
+          if (n > kCandCap - kThreads) { flush_top_k(sm.cand, sm.cand_count, kCandCap, L.top_k, 0ull, &L.theta[qi], sm.theta); n = sm.cand_count; }
           cand_ub = n;
         }
       };
@@ -364,7 +241,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(BoolLaunch L) 
       }
     }
     // ---------------- finish the work item
-    compact_candidates(sm, L.top_k, &L.theta[qi]);
+    flush_top_k(sm.cand, sm.cand_count, kCandCap, L.top_k, 0ull, &L.theta[qi], sm.theta);
     const int keep = sm.cand_count;
     uint64_t* out = L.slice_keys + ((size_t)qi * L.n_slices + slice) * L.top_k;
     for (int i = tid; i < keep; i += kThreads) out[i] = sm.cand[i];

@@ -6,7 +6,7 @@
 //              fan-out at .../search/SearchCollectorManager.java:192-198.
 #pragma once
 #include <cfloat>
-#include "bool_kernel.cuh"
+#include "query_eval.cuh"
 #include "../../include/nrtgpu.h"
 
 namespace nrtgpu {
@@ -17,7 +17,7 @@ __device__ __forceinline__ float term_freq_of(const DevIndexView& ix, const DevC
     const uint32_t b = ix.dense_tf[(size_t)c.plane * (size_t)ix.dense_stride + doc];
     *present = b != 0;
     if (b != 255u) return (float)b;
-    return exact_freq_slow<uint32_t>(ix, c, doc);
+    return exact_freq_slow(ix, c, doc);
   }
   const int32_t* docs = ix.post_docs + c.post_base;
   int lo = 0, hi = c.n_post;
@@ -26,59 +26,24 @@ __device__ __forceinline__ float term_freq_of(const DevIndexView& ix, const DevC
   if (!*present) return 0.0f;
   const uint32_t b = ix.post_f8[c.post_base + lo];
   if (b != 255u) return (float)b;
-  return exact_freq_slow<uint32_t>(ix, c, doc);
+  return exact_freq_slow(ix, c, doc);
 }
 
-// One flat BooleanQuery on one doc: Lucene BooleanScorerSupplier semantics (conjunction / disjunction sums in double,
-// ReqOptSumScorer float add when minShouldMatch == 0), identical to the top-k kernels' clause evaluation.
+// query q on one doc of the leaf; term presence is found clause by clause, so no presence mask is known up front
 __device__ __forceinline__ bool eval_query_on_doc(const DevIndexView& ix, const DevQuery& q, const DevClause* __restrict__ cl,
                                                   int32_t doc, float* out_score) {
   if (q.empty) return false;
-  if (ix.live_bits && !((ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
-  double must_sum = 0.0, should_sum = 0.0;
-  int n_should = 0;
-  for (int i = 0; i < q.n_clauses; ++i) {
-    const DevClause& c = cl[i];
+  auto term = [&](const DevClause& c, float* s) {
     bool present;
-    float s = 0.0f;
-    if (c.kind == NRTGPU_TERM) {
-      const float f = term_freq_of(ix, c, doc, &present);
-      if (present && c.scoring) {
-        const uint8_t* nrm = ix.norms[c.field];
-        const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
-        s = bm25_score(c.weight, f, ix.caches[c.field * 256 + nb]);
-      }
-    } else if (c.kind == NRTGPU_RANGE_I64) {
-      present = range_matches(ix, c.col, doc, c.lo, c.hi);
-      s = c.weight;
-    } else {
-      present = true;
-      s = c.weight;
+    const float f = term_freq_of(ix, c, doc, &present);
+    if (present && c.scoring) {
+      const uint8_t* nrm = ix.norms[c.field];
+      const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
+      *s = bm25_score(c.weight, f, ix.caches[c.field * 256 + nb]);
     }
-    if (!present) {
-      if (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER) return false;
-      continue;
-    }
-    switch (c.occur) {
-      case NRTGPU_MUST: must_sum += (double)s; break;
-      case NRTGPU_FILTER: break;
-      case NRTGPU_SHOULD: should_sum += (double)s; ++n_should; break;
-      default: return false;   // MUST_NOT present
-    }
-  }
-  if (n_should < q.need_should) return false;
-  float score;
-  if (q.n_req == 0) score = (float)should_sum;
-  else {
-    const float req = (float)must_sum;
-    if (n_should == 0) score = req;
-    else {
-      const float opt = (float)should_sum;
-      score = (q.msm > 0) ? (float)((double)req + (double)opt) : __fadd_rn(req, opt);
-    }
-  }
-  *out_score = score;
-  return true;
+    return present;
+  };
+  return eval_clauses(ix, q, cl, doc, q.req_term_mask, term, out_score);
 }
 
 // QueryRescorer second pass: query q on its own first-pass hits
@@ -91,7 +56,7 @@ struct ScoreDocsLaunch {
   uint8_t* out_matches; float* out_scores;
 };
 
-__global__ void score_docs_kernel(ScoreDocsLaunch L) {
+__global__ void score_docs_kernel(const __grid_constant__ ScoreDocsLaunch L) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L.nq * L.n_hits) return;
   const int q = i / L.n_hits, r = i % L.n_hits;

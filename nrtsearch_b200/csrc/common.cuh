@@ -48,6 +48,34 @@ __device__ __forceinline__ int next_pow2(int x) {
   return p;
 }
 
+// Candidate buffer flush of a posting kernel (all threads of the CTA): sorts the count keys of cand (cap entries, a power
+// of two), keeps the best top_k and, once it holds top_k, publishes the k-th key minus dec as the query's threshold
+// g_theta (atomicMax). The CTA's copy theta is raised to the published threshold.
+__device__ __forceinline__ void flush_top_k(uint64_t* cand, int& count, int cap, int top_k, unsigned long long dec,
+                                            uint64_t* g_theta, unsigned long long& theta) {
+  __syncthreads();
+  int n = count;
+  if (n > cap) n = cap;
+  const int m = next_pow2(n < 2 ? 2 : n);
+  for (int i = n + threadIdx.x; i < m; i += blockDim.x) cand[i] = 0ull;
+  __syncthreads();
+  block_bitonic_sort_desc(cand, m);
+  if (threadIdx.x == 0) {
+    const int keep = n < top_k ? n : top_k;
+    count = keep;
+    if (keep == top_k) {
+      const unsigned long long kth = cand[top_k - 1] - dec;
+      const unsigned long long old = atomicMax((unsigned long long*)g_theta, kth);
+      const unsigned long long t = old > kth ? old : kth;
+      if (t > theta) theta = t;
+    } else {
+      const unsigned long long g = *(volatile unsigned long long*)g_theta;
+      if (g > theta) theta = g;
+    }
+  }
+  __syncthreads();
+}
+
 // Deadline of a run (SearchCutoffWrapper): the first work item of the run stamps *clock0 with %globaltimer; an item
 // that starts more than deadline_ns later is late. deadline_ns < 0: the request's budget was spent before the launch.
 // Called by one thread per work item, only when a deadline is set (deadline_ns != 0).

@@ -4,13 +4,13 @@
 //   * a term clause reads the bitmap of its term, built once per call by scattering the term's postings (cost ~ df);
 //   * a range clause runs range_matches with one lane per doc, a warp ballot forms the word;
 //   * match-all is ~0;
-//   * the words combine as eval_query_on_doc matches: AND of MUST / FILTER, minus the OR of MUST_NOT, and at least
+//   * the words combine as eval_clauses (query_eval.cuh) matches: AND of MUST / FILTER, minus the OR of MUST_NOT, and at least
 //     need_should SHOULD clauses per bit (a bit-sliced counter); an empty query gives 0.
 // The kNN stages then AND bit d of the query's row into their filter test (knn_gemm_tc.cuh, knn_kernel.cuh), and the
 // queries whose row is small are scored exactly over the row's ordinals only (knn_filter_ords_kernel + the gather mode of
 // knn_exact_chunk_kernel).
 #pragma once
-#include "knn_kernel.cuh"
+#include "query_eval.cuh"
 
 namespace nrtgpu {
 

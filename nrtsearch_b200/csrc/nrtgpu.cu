@@ -883,7 +883,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
     NRT_CUDA_TRY(cudaStreamSynchronize(st));
     for (int k = 0; k < 2; ++k) {
       const unsigned long long* x = h + v3::kProbeStats * k;
-      if (x[0]) fprintf(stderr, "[nrtgpu probe %s] longest item %llu cyc; CTA busy: mean %.0f max %llu cyc; warm-up items %llu, %.0f cyc each; per item: flush %.0f cyc (sort %.0f), TMA wait %.0f cyc\n", k == 0 ? "simple" : "generic",
+      if (x[0]) fprintf(stderr, "[nrtgpu probe %s] longest item %llu cyc; CTA busy: mean %.0f max %llu cyc; warm-up items %llu, %.0f cyc each; per item: flush %.0f cyc (%.0f in flush_top_k), TMA wait %.0f cyc\n", k == 0 ? "simple" : "generic",
                         x[8], (double)x[9] / std::min<double>((double)x[0], (double)(v3::kCtasA * b->ix->ctx->plan.sm_count)), x[10], x[11], x[11] ? (double)x[12] / x[11] : 0.0, (double)x[13] / x[0], (double)x[15] / x[0], (double)x[14] / x[0]);
       if (x[0]) fprintf(stderr, "[nrtgpu probe %s] %llu items, %.0f cyc/item (set-up %.0f), %.2f runs/item (%.2f staged), %.1f rounds/item, %llu driver postings (%.0f/item), %.0f queued/item, %.0f keys admitted/item, %.2f flushes/item\n",
                         k == 0 ? "simple" : "generic", x[0], (double)x[1] / x[0], (double)x[6] / x[0], (double)x[2] / x[0], (double)x[5] / x[0],

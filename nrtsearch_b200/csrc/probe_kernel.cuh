@@ -29,7 +29,7 @@
 //     required list is dropped after the probes, before any norm / doc-value gather).
 // Results are bit-identical to the exhaustive oracle (tests/test_gpu_parity.py, tests/test_gpu_probe.py).
 #pragma once
-#include "bool_kernel.cuh"
+#include "query_eval.cuh"
 #include "sort_kernel.cuh"
 #include "collect_kernel.cuh"
 
@@ -108,7 +108,7 @@ struct ProbeLaunch {
   unsigned int* work_counter;    // queue head
   unsigned long long* stats;     // optional [kProbeStats]: items, item cycles, runs, driver postings, flushes, staged runs, set-up
                                  // cycles, rounds, longest item, CTA busy (sum, max), warm-up items and cycles, flush, TMA wait and
-                                 // sort cycles, queued entries, admitted keys
+                                 // flush_top_k cycles, queued entries, admitted keys
   int32_t n_work, n_lists, n_slices, top_k;
   int32_t parts_max;             // result lists / boundary entries per slice (a heavy (query, slice) is split into up to this many items)
   int32_t slice_docs;            // multiple of kGran, <= kMaxSliceGran * kGran
@@ -197,78 +197,29 @@ __device__ __forceinline__ uint32_t seg_n(uint32_t a, uint32_t b, uint32_t pbm) 
   return b > a ? ((b + pbm + kAlign - 1) & ~(uint32_t)(kAlign - 1)) - ((a + pbm) & ~(uint32_t)(kAlign - 1)) : 0u;
 }
 
-// Universal clause evaluation of one doc given the tf word of its term slots (Lucene BooleanScorerSupplier semantics,
-// as the window kernel's evaluate_doc: conjunction / disjunction sums in double, ReqOptSumScorer float add when msm == 0).
+// the clauses of sm.q on one queued doc; word holds the doc's tf byte of every term slot (kTfInexact: a saturated 2-bit
+// code, the exact byte is read from the byte plane). The norm byte is reused while consecutive scored
+// term clauses read one field.
 template <typename SM>
 __device__ __noinline__ bool evaluate_doc(const ProbeLaunch& L, const SM& sm, int32_t doc, uint32_t word, float* out_score) {
-  const DevQuery& q = sm.q;
-  const uint32_t m = presence4(word);
-  if ((m & q.req_term_mask) != q.req_term_mask) return false;
-  if (m & q.not_term_mask) return false;
-  if (L.ix.live_bits && !((L.ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
-  // doc-value clauses first: a doc that fails a required range (or hits an excluded one) is dropped before any norm is
-  // gathered or score computed (what ConjunctionDISI does by advancing the cheapest iterators first)
-  uint32_t range_present = 0;
-  if (q.has_nonterm)
-    for (int i = 0; i < q.n_clauses; ++i) {
-      const DevClause& c = sm.cl[i];
-      if (c.kind != NRTGPU_RANGE_I64) continue;
-      const bool p = range_matches(L.ix, c.col, doc, c.lo, c.hi);
-      if (p) { if (c.occur == NRTGPU_MUST_NOT) return false; range_present |= 1u << i; }
-      else if (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER) return false;
-    }
-  double must_sum = 0.0, should_sum = 0.0;
-  int n_should = 0;
   int cur_field = -1;
   uint32_t nb = 1u;
-  for (int i = 0; i < q.n_clauses; ++i) {
-    const DevClause& c = sm.cl[i];
-    bool present;
-    float s = 0.0f;
-    if (c.kind == NRTGPU_TERM) {
-      uint32_t b = (word >> (8 * c.slot)) & 0xffu;
-      present = b != 0;
-      if (present && c.scoring) {
-        if (b == kTfInexact && sm.s_plane[c.slot]) b = (uint32_t)__ldg(sm.s_plane[c.slot] + doc);   // saturated 2-bit code
-        if (c.field != cur_field) {
-          cur_field = c.field;
-          const uint8_t* nrm = L.ix.norms[c.field];
-          nb = nrm ? (uint32_t)__ldg(nrm + doc) : 1u;
-        }
-        const float f = (b == 255u) ? exact_freq_slow<uint32_t>(L.ix, c, doc) : (float)b;
-        s = bm25_score(c.weight, f, __ldg(&L.ix.caches[c.field * 256 + nb]));
+  auto term = [&](const DevClause& c, float* s) {
+    uint32_t b = (word >> (8 * c.slot)) & 0xffu;
+    if (b == 0) return false;
+    if (c.scoring) {
+      if (b == kTfInexact && sm.s_plane[c.slot]) b = (uint32_t)__ldg(sm.s_plane[c.slot] + doc);
+      if (c.field != cur_field) {
+        cur_field = c.field;
+        const uint8_t* nrm = L.ix.norms[c.field];
+        nb = nrm ? (uint32_t)__ldg(nrm + doc) : 1u;
       }
-    } else if (c.kind == NRTGPU_RANGE_I64) {
-      present = (range_present >> i) & 1u;
-      s = c.weight;
-    } else {
-      present = true;
-      s = c.weight;
+      const float f = (b == 255u) ? exact_freq_slow(L.ix, c, doc) : (float)b;
+      *s = bm25_score(c.weight, f, __ldg(&L.ix.caches[c.field * 256 + nb]));
     }
-    if (!present) {
-      if (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER) return false;
-      continue;
-    }
-    switch (c.occur) {
-      case NRTGPU_MUST: must_sum += (double)s; break;
-      case NRTGPU_FILTER: break;
-      case NRTGPU_SHOULD: should_sum += (double)s; ++n_should; break;
-      default: return false;
-    }
-  }
-  if (n_should < q.need_should) return false;
-  float score;
-  if (q.n_req == 0) score = (float)should_sum;
-  else {
-    const float req = (float)must_sum;
-    if (n_should == 0) score = req;
-    else {
-      const float opt = (float)should_sum;
-      score = (q.msm > 0) ? (float)((double)req + (double)opt) : __fadd_rn(req, opt);
-    }
-  }
-  *out_score = score;
-  return true;
+    return true;
+  };
+  return eval_clauses(L.ix, sm.q, sm.cl, doc, presence4(word), term, out_score);
 }
 
 // exact score of a doc of a pure single-field disjunction: double sum, in slot (= clause) order, of Lucene's BM25 float
@@ -284,7 +235,7 @@ __device__ __forceinline__ float score_disjunction(const ProbeLaunch& L, const S
     uint32_t b = (word >> (8 * s)) & 0xffu;
     if (b == 0) continue;
     if (b == kTfInexact && sm.s_plane[s]) b = (uint32_t)__ldg(sm.s_plane[s] + doc);   // saturated 2-bit code: the exact byte
-    const float f = (b == 255u) ? exact_freq_slow<uint32_t>(L.ix, sm.cl[sm.s_clause[s]], doc) : (float)b;
+    const float f = (b == 255u) ? exact_freq_slow(L.ix, sm.cl[sm.s_clause[s]], doc) : (float)b;
     sum += (double)bm25_score(sm.s_weight[s], f, __ldg(&L.ix.caches[sm.s_field[s] * 256 + nb]));
   }
   return (float)sum;
@@ -294,29 +245,9 @@ __device__ __forceinline__ float score_disjunction(const ProbeLaunch& L, const S
 // theta_dec) as the query's threshold.
 template <typename SM>
 __device__ __noinline__ void flush_candidates(const ProbeLaunch& L, SM& sm, int top_k, uint64_t* g_theta) {
-  __syncthreads();
-  int n = sm.cand_count;
-  if (n > kCand) n = kCand;
-  const int m = next_pow2(n < 2 ? 2 : n);
   const long long ts = L.stats ? clock64() : 0ll;
-  for (int i = n + threadIdx.x; i < m; i += kThreads) sm.cand[i] = 0ull;
-  __syncthreads();
-  block_bitonic_sort_desc(sm.cand, m);
+  flush_top_k(sm.cand, sm.cand_count, kCand, top_k, (unsigned long long)sm.theta_dec, g_theta, sm.theta);
   if (L.stats && threadIdx.x == 0) atomicAdd(&L.stats[15], (unsigned long long)(clock64() - ts));
-  if (threadIdx.x == 0) {
-    const int keep = n < top_k ? n : top_k;
-    sm.cand_count = keep;
-    if (keep == top_k) {
-      const unsigned long long kth = sm.cand[top_k - 1] - (unsigned long long)sm.theta_dec;
-      const unsigned long long old = atomicMax((unsigned long long*)g_theta, kth);
-      const unsigned long long t = old > kth ? old : kth;
-      if (t > sm.theta) sm.theta = t;
-    } else {
-      const unsigned long long g = *(volatile unsigned long long*)g_theta;
-      if (g > sm.theta) sm.theta = g;
-    }
-  }
-  __syncthreads();
 }
 
 // binary search of doc in the sorted smem range [l, h); returns the tf byte (0 = absent)

@@ -1,0 +1,129 @@
+// One flat BooleanQuery on one doc: the device view of the index that every query kernel reads, the doc-value range test,
+// the exact tf of a saturated posting, and the clause rule shared by the window engine (bool_kernel.cuh), the generic
+// probe kernel (probe_kernel.cuh) and the second pass (collect_kernel.cuh). The engines differ only in how they find a
+// term's tf and norm; each passes that in.
+#pragma once
+#include "common.cuh"
+#include "../../include/nrtgpu.h"
+
+namespace nrtgpu {
+
+struct DevIndexView {
+  int32_t n_docs;
+  int32_t doc_base;
+  const int32_t* post_docs;
+  const uint8_t* post_f8;        // min(freq, 255)
+  const int64_t* exc_pos;        // sorted global posting indices with freq >= 255
+  const int32_t* exc_freq;
+  int32_t n_exc;
+  const uint8_t* const* norms;   // [n_fields] device pointers (NULL = omitNorms)
+  const float* caches;           // [n_fields][256]
+  const int64_t* const* col64;   // [n_columns] (NULL if stored as int32)
+  const int32_t* const* col32;   // [n_columns] (NULL if stored as int64)
+  const uint8_t* const* col_has; // [n_columns] (NULL = all)
+  const int64_t* const* colmv_off;  // [n_columns] multi-valued columns (SORTED_NUMERIC): doc d holds colmv_val[c][off[d] .. off[d + 1]),
+  const int64_t* const* colmv_val;  //              ascending; NULL entry = single-valued column
+  const uint32_t* live_bits;     // bitmap or NULL
+  const uint32_t* gran_tab;      // [n_rows][n_gran + 1] postings of the term below each 1024-doc granule boundary (skip data)
+  int32_t n_gran;
+  const uint8_t* dense_tf;       // [n_planes][dense_stride] min(freq, 255) per doc for the densest terms (0 = absent)
+  int64_t dense_stride;
+  const uint8_t* dense_tf2;      // [n_planes][dense_stride / 4] min(freq, 3) in 2 bits per doc: the planes the probe kernel gathers
+                                 // (a quarter of the L2 / DRAM footprint of the byte planes; 3 = "three or more")
+};
+
+// numeric range clause on one doc (IndexOrDocValuesQuery's doc-values side, reference IntFieldDef.java:124-158 inclusive
+// bounds): single-valued column = the value is in [lo, hi]; multi-valued (SortedNumericDocValuesRangeQuery) = ANY value is
+__device__ __forceinline__ bool range_matches(const DevIndexView& ix, int col, int32_t doc, int64_t lo, int64_t hi) {
+  const int64_t* off = ix.colmv_off ? ix.colmv_off[col] : nullptr;
+  if (off) {
+    const int64_t* v = ix.colmv_val[col];
+    int64_t a = off[doc], b = off[doc + 1];
+    while (a < b) { const int64_t m = (a + b) >> 1; if (v[m] < lo) a = m + 1; else b = m; }   // values of a doc are sorted
+    return a < off[doc + 1] && v[a] <= hi;
+  }
+  const uint8_t* has = ix.col_has[col];
+  if (has && !has[doc]) return false;
+  const int64_t x = ix.col32[col] ? (int64_t)__ldg(ix.col32[col] + doc) : __ldg(ix.col64[col] + doc);
+  return x >= lo && x <= hi;
+}
+
+// exact tf of posting (clause c, doc) when the byte saturated: find the posting, then the exception list
+__device__ __noinline__ float exact_freq_slow(const DevIndexView& ix, const DevClause& c, int32_t doc) {
+  const int32_t* docs = ix.post_docs + c.post_base;
+  int lo = 0, hi = c.n_post;
+  while (lo < hi) { int m = (lo + hi) >> 1; if (docs[m] < doc) lo = m + 1; else hi = m; }
+  int64_t gp = c.post_base + lo;
+  int a = 0, b = ix.n_exc;
+  while (a < b) { int m = (a + b) >> 1; if (ix.exc_pos[m] < gp) a = m + 1; else b = m; }
+  if (a < ix.n_exc && ix.exc_pos[a] == gp) return (float)ix.exc_freq[a];
+  return 255.0f;
+}
+
+// Matches and scores doc against the n_clauses clauses cl of q with Lucene's BooleanScorerSupplier rule: an absent MUST /
+// FILTER clause or a present MUST_NOT clause rejects the doc, at least need_should SHOULD clauses must match, each clause
+// scores a float, the MUST and SHOULD sums are doubles added in clause order, and required + optional is
+// ReqOptSumScorer's float add (msm == 0) or ConjunctionScorer's double add (msm > 0).
+//   term_mask: bit s set iff term slot s is present, for an engine that knows it before scoring (a doc missing a required
+//              slot or holding an excluded one is rejected at once); an engine that does not passes q.req_term_mask.
+//   term(c, &s): whether term clause c is present in doc; if it is and c.scoring, sets s to its BM25 float.
+// Doc-value clauses are evaluated before any term is scored: a doc that fails a required range (or holds an excluded one)
+// costs no norm gather, as ConjunctionDISI advances the cheapest iterators first. Ranges have no side effects and the sums
+// stay in clause order, so the order changes no result.
+template <class TermScore>
+__device__ __forceinline__ bool eval_clauses(const DevIndexView& ix, const DevQuery& q, const DevClause* cl,
+                                             int32_t doc, uint32_t term_mask, TermScore term, float* out_score) {
+  if ((term_mask & q.req_term_mask) != q.req_term_mask) return false;
+  if (term_mask & q.not_term_mask) return false;
+  if (ix.live_bits && !((ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
+  uint32_t range_present = 0;
+  if (q.has_nonterm)
+    for (int i = 0; i < q.n_clauses; ++i) {
+      const DevClause& c = cl[i];
+      if (c.kind != NRTGPU_RANGE_I64) continue;
+      const bool p = range_matches(ix, c.col, doc, c.lo, c.hi);
+      if (p) { if (c.occur == NRTGPU_MUST_NOT) return false; range_present |= 1u << i; }
+      else if (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER) return false;
+    }
+  double must_sum = 0.0, should_sum = 0.0;
+  int n_should = 0;
+  for (int i = 0; i < q.n_clauses; ++i) {
+    const DevClause& c = cl[i];
+    bool present;
+    float s = 0.0f;
+    if (c.kind == NRTGPU_TERM) {
+      present = term(c, &s);
+    } else if (c.kind == NRTGPU_RANGE_I64) {
+      present = (range_present >> i) & 1u;
+      s = c.weight;
+    } else {
+      present = true;
+      s = c.weight;
+    }
+    if (!present) {
+      if (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER) return false;
+      continue;
+    }
+    switch (c.occur) {
+      case NRTGPU_MUST: must_sum += (double)s; break;
+      case NRTGPU_FILTER: break;
+      case NRTGPU_SHOULD: should_sum += (double)s; ++n_should; break;
+      default: return false;   // MUST_NOT present
+    }
+  }
+  if (n_should < q.need_should) return false;
+  float score;
+  if (q.n_req == 0) score = (float)should_sum;
+  else {
+    const float req = (float)must_sum;
+    if (n_should == 0) score = req;
+    else {
+      const float opt = (float)should_sum;
+      score = (q.msm > 0) ? (float)((double)req + (double)opt) : __fadd_rn(req, opt);
+    }
+  }
+  *out_score = score;
+  return true;
+}
+
+}  // namespace nrtgpu

@@ -17,7 +17,7 @@
 #include <thrust/sequence.h>
 #include <thrust/sort.h>
 #include <thrust/system/cuda/execution_policy.h>
-#include "bool_kernel.cuh"
+#include "common.cuh"
 
 namespace nrtgpu {
 
