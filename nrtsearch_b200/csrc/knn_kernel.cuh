@@ -395,12 +395,19 @@ __global__ void fill_f32_kernel(float* p, int n, float v) {
   if (i < n) p[i] = v;
 }
 
+// Scratch slots of a kNN call: knn_search_host's, then the per-query filters' (nrtgpu.cu). knn_exact_host runs after the
+// candidate stage and reuses two: its slice keys take the unfused score matrix's slot, its counts and pages the chunk buffer's.
+enum class KnnSlot : int {
+  Theta, ChunkCand, ChunkCandCnt, Overflow, Q, Scores, Cand, CandCnt, OutDocs, OutScores, OutCounts, Boosts, Filter, Qbf16,
+  Unsafe, ExactSel, Qrow, Rows, TermBits, Terms, RowMeta, GatherQ, GatherBoosts, Ords, OrdBegin, GatherRows, GatherQrow,
+  Count, ExactKeys = Scores, ExactCnt = ChunkCand
+};
+
 // device scratch of one kNN call: slots grow on demand and are kept between calls (no cudaMalloc / cudaFree, which
 // synchronise the device, on the request path). The index owns one and serialises the calls that use it.
 struct KnnScratch {
-  static constexpr int kSlots = 32;   // 0-16: knn_search_host, 17-27: per-query filters (knn_filter_kernel.cuh)
-  void* p[kSlots] = {};
-  size_t cap[kSlots] = {};
+  void* p[(int)KnnSlot::Count] = {};
+  size_t cap[(int)KnnSlot::Count] = {};
   ~KnnScratch() { for (auto q : p) if (q) cudaFree(q); }
   int get(int i, size_t bytes, void** out) {
     if (bytes > cap[i]) {
@@ -412,23 +419,76 @@ struct KnnScratch {
     return 0;
   }
 };
-#define NRT_KNN_GET(slot, ptr, bytes) do { int rc_ = sc->get((slot), (bytes), (void**)&(ptr)); if (rc_) return rc_; } while (0)
+#define NRT_KNN_GET(slot, ptr, bytes) do { int rc_ = sc.get((int)(slot), (bytes), (void**)&(ptr)); if (rc_) return rc_; } while (0)
+
+// what the kNN stages read of an index image (nrtgpu_index::knn_corpus)
+struct KnnCorpus {
+  const float* vec; const float* norm2; const int32_t* vec_docs;   // [n][dims] vectors, their |v|^2, ordinal -> doc or NULL
+  int n, dims, sim, doc_base, n_docs;                              // sim | kKnnByteFlag for byte vectors
+  const uint32_t* live_bits; float dmax;                           // liveDocs bitmap or NULL; largest |v|
+  // tensor-core candidate stage: bf16 copy of the vectors, its TMA tensor map, per-vector (a, b); NULL: fp32 SIMT stage
+  const __nv_bfloat16* bf16 = nullptr; const CUtensorMap* tmap = nullptr; const float2* ab = nullptr;
+};
+
+// a batch of queries, in host memory
+struct KnnRequest {
+  const float* queries; int nq, k;   // [nq][dims]
+  const float* boosts; const uint8_t* filter;   // [nq] or NULL; [n_docs] bytes (0 = excluded) or NULL
+  // query q keeps doc d iff bit d of row qrow[q] of d_rows (device, [rows][words]) is set; qrow NULL or qrow[q] < 0: no row
+  const uint32_t* d_rows; const int32_t* qrow; int words;
+};
+
+struct KnnPages { int32_t* docs; float* scores; int32_t* counts; };   // host [nq][k], [nq][k], [nq]
+
+// page i of src -> page sel[i] of dst, for i < n
+inline void knn_scatter(const KnnPages& src, int n, const int32_t* sel, const KnnPages& dst, int k) {
+  for (int i = 0; i < n; ++i) {
+    std::memcpy(dst.docs + (size_t)sel[i] * k, src.docs + (size_t)i * k, (size_t)k * 4);
+    std::memcpy(dst.scores + (size_t)sel[i] * k, src.scores + (size_t)i * k, (size_t)k * 4);
+    dst.counts[sel[i]] = src.counts[i];
+  }
+}
+
+// Runs fn(request, pages) on the queries sel[] of req, their vectors, boosts and rows packed into a request of their own,
+// and writes its pages to rows sel[i] of out. A selection 0, 1, ..., n - 1 runs on req's own arrays and out, uncopied.
+template <class Fn>
+int knn_run_subset(const KnnRequest& req, int dims, const std::vector<int32_t>& sel, const KnnPages& out, Fn&& fn) {
+  const int n = (int)sel.size(), k = req.k;
+  KnnRequest r = req; r.nq = n;
+  bool prefix = true;
+  for (int i = 0; i < n; ++i) prefix &= sel[(size_t)i] == i;
+  if (prefix) return fn(r, out);
+  std::vector<float> qv((size_t)n * dims), bv((size_t)n), sv((size_t)n * k);
+  std::vector<int32_t> rv((size_t)n), dv((size_t)n * k), cv((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    const int q = sel[(size_t)i];
+    std::memcpy(qv.data() + (size_t)i * dims, req.queries + (size_t)q * dims, (size_t)dims * 4);
+    if (req.boosts) bv[(size_t)i] = req.boosts[q];
+    if (req.qrow) rv[(size_t)i] = req.qrow[q];
+  }
+  r.queries = qv.data(); r.boosts = req.boosts ? bv.data() : nullptr; r.qrow = req.qrow ? rv.data() : nullptr;
+  const KnnPages packed{dv.data(), sv.data(), cv.data()};
+  const int rc = fn(r, packed);
+  if (!rc) knn_scatter(packed, n, sel.data(), out, k);
+  return rc;
+}
 
 // Exact evaluation of the queries sel[] (rows of X.Q) with the oracle's arithmetic over n_chunks chunks of kKnnExactChunk
 // vectors each (X.ords set: of their filter row's ordinal list); merge_slices_kernel merges the chunks' lists and the
-// pages overwrite rows sel[i] of the host outputs. X carries everything but qsel, n_chunks, keys and cnt.
-inline int knn_exact_host(KnnScratch* sc, cudaStream_t st, KnnExactLaunch X, int n_chunks, int doc_base,
-                          const std::vector<int32_t>& sel, int32_t* out_docs, float* out_scores, int32_t* out_counts) {
+// pages overwrite rows sel[i] of out. X carries the queries, k and the filters.
+inline int knn_exact_host(const KnnCorpus& corpus, KnnScratch& sc, cudaStream_t st, KnnExactLaunch X, int n_chunks,
+                          const std::vector<int32_t>& sel, const KnnPages& out) {
   const int n_sel = (int)sel.size(), k = X.k;
+  X.D = corpus.vec; X.n = corpus.n; X.dims = corpus.dims; X.sim = corpus.sim; X.live_bits = corpus.live_bits; X.vec_docs = corpus.vec_docs;
   int32_t *dSel = nullptr, *dCnt = nullptr, *dXD = nullptr, *dXC = nullptr; uint64_t* dKeys = nullptr; float* dXS = nullptr;
-  NRT_KNN_GET(15, dSel, (size_t)n_sel * sizeof(int32_t));
+  NRT_KNN_GET(KnnSlot::ExactSel, dSel, (size_t)n_sel * sizeof(int32_t));
   NRT_CUDA_TRY(cudaMemcpyAsync(dSel, sel.data(), (size_t)n_sel * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   // the slice lists can be large (n_sel * n_chunks * k keys): process the selected queries in groups that fit 256 MB
   // (and the 65535 rows of a grid's y dimension)
   const size_t per_q = (size_t)n_chunks * k * sizeof(uint64_t);
   const int group = (int)std::max<size_t>(1, std::min<size_t>({(size_t)n_sel, ((size_t)256 << 20) / per_q, (size_t)65535}));
-  NRT_KNN_GET(5, dKeys, (size_t)group * per_q);   // slot 5 (the unfused score matrix) is free by now
-  NRT_KNN_GET(1, dCnt, (size_t)group * n_chunks * sizeof(int32_t) + (size_t)group * k * 8 + (size_t)group * 4);
+  NRT_KNN_GET(KnnSlot::ExactKeys, dKeys, (size_t)group * per_q);
+  NRT_KNN_GET(KnnSlot::ExactCnt, dCnt, (size_t)group * n_chunks * sizeof(int32_t) + (size_t)group * k * 8 + (size_t)group * 4);
   dXD = dCnt + (size_t)group * n_chunks; dXS = (float*)(dXD + (size_t)group * k); dXC = (int32_t*)(dXS + (size_t)group * k);
   std::vector<int32_t> hd((size_t)group * k), hc((size_t)group); std::vector<float> hs((size_t)group * k);
   for (int g0 = 0; g0 < n_sel; g0 += group) {
@@ -436,7 +496,7 @@ inline int knn_exact_host(KnnScratch* sc, cudaStream_t st, KnnExactLaunch X, int
     X.qsel = dSel + g0; X.n_chunks = n_chunks; X.keys = dKeys; X.cnt = dCnt;
     knn_exact_chunk_kernel<<<dim3((unsigned)n_chunks, (unsigned)gn), 256, 0, st>>>(X);
     NRT_CUDA_TRY(cudaGetLastError());
-    MergeLaunch M; M.slice_keys = dKeys; M.slice_cnt = dCnt; M.n_lists = n_chunks; M.top_k = k; M.nq = gn; M.doc_base = doc_base;
+    MergeLaunch M; M.slice_keys = dKeys; M.slice_cnt = dCnt; M.n_lists = n_chunks; M.top_k = k; M.nq = gn; M.doc_base = corpus.doc_base;
     M.out_docs = dXD; M.out_scores = dXS; M.out_counts = dXC;
     M.total_hits = nullptr; M.pruned = nullptr; M.terminated = nullptr; M.terminate_after = 0; M.out_total = nullptr; M.out_flags = nullptr;
     merge_slices_kernel<<<gn, kMergeThreads, 0, st>>>(M);
@@ -445,78 +505,60 @@ inline int knn_exact_host(KnnScratch* sc, cudaStream_t st, KnnExactLaunch X, int
     NRT_CUDA_TRY(cudaMemcpyAsync(hs.data(), dXS, (size_t)gn * k * 4, cudaMemcpyDeviceToHost, st));
     NRT_CUDA_TRY(cudaMemcpyAsync(hc.data(), dXC, (size_t)gn * 4, cudaMemcpyDeviceToHost, st));
     NRT_CUDA_TRY(cudaStreamSynchronize(st));
-    for (int i = 0; i < gn; ++i) {
-      const int q = sel[(size_t)(g0 + i)];
-      std::memcpy(out_docs + (size_t)q * k, hd.data() + (size_t)i * k, (size_t)k * 4);
-      std::memcpy(out_scores + (size_t)q * k, hs.data() + (size_t)i * k, (size_t)k * 4);
-      out_counts[q] = hc[(size_t)i];
-    }
+    knn_scatter(KnnPages{hd.data(), hs.data(), hc.data()}, gn, sel.data() + g0, out, k);
   }
   return NRTGPU_OK;
 }
 
-// d_vec_bf16 / tm_corpus: bf16 copy of the corpus and its TMA tensor map (NULL => SIMT fp32 candidate stage).
-// stage_ms (optional): [0] = candidate GEMM kernels, [1] = select kernels, [2] = exact re-score (CUDA events on st).
-// d_qfilter / h_qrow (optional): per-query filter rows on the device, query q keeps doc d iff bit d of row h_qrow[q] is set
-// (h_qrow[q] < 0: no filter; ANDed with h_filter and the live docs).
-inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32_t* d_vec_docs, int n, int dims, int sim,
-                           int doc_base, int n_docs, const float* h_queries, int nq, int k, const float* h_boosts,
-                           const uint8_t* h_filter, cudaStream_t st, int32_t* out_docs, float* out_scores,
-                           int32_t* out_counts, const __nv_bfloat16* d_vec_bf16 = nullptr,
-                           const CUtensorMap* tm_corpus = nullptr, float* stage_ms = nullptr, const float2* d_ab = nullptr,
-                           KnnScratch* sc = nullptr, const uint32_t* d_live_bits = nullptr, float dmax = 0.0f,
-                           int32_t* n_uncertified = nullptr, const uint32_t* d_qfilter = nullptr,
-                           const int32_t* h_qrow = nullptr, int qwords = 0) {
-  KnnScratch local_scratch;   // only when the caller brings none (freed on return)
-  if (!sc) sc = &local_scratch;
-  const bool use_tc = d_vec_bf16 != nullptr && tm_corpus != nullptr && d_ab != nullptr;
+// The top-k pages of req over the corpus. stage_ms (optional): [0] = candidate GEMM kernels, [1] = select kernels, [2] =
+// exact re-score (CUDA events on st). n_uncertified (optional): the queries that took the exact fallback.
+inline int knn_search_host(const KnnCorpus& corpus, const KnnRequest& req, KnnScratch& sc, cudaStream_t st,
+                           const KnnPages& out, float* stage_ms, int32_t* n_uncertified) {
+  const int n = corpus.n, dims = corpus.dims, sim = corpus.sim, nq = req.nq, k = req.k;
+  const bool use_tc = corpus.bf16 != nullptr && corpus.tmap != nullptr && corpus.ab != nullptr;
   int kprime = use_tc ? (4 * k < 128 ? 128 : 4 * k) : (2 * k < 64 ? 64 : 2 * k);
   if (kprime > kKnnCandCap - kKnnSelThreads) kprime = kKnnCandCap - kKnnSelThreads;
   bool fused = use_tc && kprime <= 1024;           // best-k' (<= 1024) + chunk survivors (<= 3072) fit one 4096-key sort
   const int cc_cap = kKnnCandCap - 1024;
-  float *dQ = nullptr, *dS = nullptr, *dB = nullptr, *dOS = nullptr; uint8_t* dF = nullptr;
-  uint64_t* dC = nullptr; int32_t *dCn = nullptr, *dOD = nullptr, *dOC = nullptr;
+  float *dQ = nullptr, *dS = nullptr, *dB = nullptr, *dOS = nullptr, *dTheta = nullptr; uint8_t* dF = nullptr;
+  uint64_t *dC = nullptr, *dCC = nullptr; __nv_bfloat16* dQb = nullptr;
+  int32_t *dCn = nullptr, *dOD = nullptr, *dOC = nullptr, *dQrow = nullptr, *dUnsafe = nullptr, *dCCn = nullptr, *dOvf = nullptr;
   const int chunk_max = use_tc ? 65536 : kKnnChunk;
-  float* dTheta = nullptr; uint64_t* dCC = nullptr; int *dCCn = nullptr, *dOvf = nullptr;
   if (fused) {
-    NRT_KNN_GET(0, dTheta, (size_t)nq * sizeof(float));
-    NRT_KNN_GET(1, dCC, (size_t)nq * cc_cap * sizeof(uint64_t));
-    NRT_KNN_GET(2, dCCn, (size_t)nq * sizeof(int));
-    NRT_KNN_GET(3, dOvf, sizeof(int));
+    NRT_KNN_GET(KnnSlot::Theta, dTheta, (size_t)nq * sizeof(float));
+    NRT_KNN_GET(KnnSlot::ChunkCand, dCC, (size_t)nq * cc_cap * sizeof(uint64_t));
+    NRT_KNN_GET(KnnSlot::ChunkCandCnt, dCCn, (size_t)nq * sizeof(int));
+    NRT_KNN_GET(KnnSlot::Overflow, dOvf, sizeof(int));
     NRT_CUDA_TRY(cudaMemsetAsync(dCCn, 0, (size_t)nq * sizeof(int), st));
     NRT_CUDA_TRY(cudaMemsetAsync(dOvf, 0, sizeof(int), st));
     fill_f32_kernel<<<(nq + 255) / 256, 256, 0, st>>>(dTheta, nq, -INFINITY);
   }
   int chunk = n < chunk_max ? n : chunk_max;
   chunk = (chunk + 3) & ~3;   // keep score rows 16-byte aligned
-  NRT_KNN_GET(4, dQ, (size_t)nq * dims * sizeof(float));
+  NRT_KNN_GET(KnnSlot::Q, dQ, (size_t)nq * dims * sizeof(float));
   // fused mode: the first kKnnWarmChunk vectors go through the UNFUSED path (scores stored, knn_select_kernel) to seed
   // every query's threshold; with an empty threshold the fused epilogue would have to keep every value it sees
   const int warm = fused ? (n < kKnnWarmChunk ? ((n + 3) & ~3) : kKnnWarmChunk) : 0;
-  if (!fused) NRT_KNN_GET(5, dS, (size_t)nq * chunk * sizeof(float));
-  else NRT_KNN_GET(5, dS, (size_t)nq * warm * sizeof(float));
-  NRT_KNN_GET(6, dC, (size_t)nq * kprime * sizeof(uint64_t));
-  NRT_KNN_GET(7, dCn, (size_t)nq * sizeof(int32_t));
-  NRT_KNN_GET(8, dOD, (size_t)nq * k * sizeof(int32_t));
-  NRT_KNN_GET(9, dOS, (size_t)nq * k * sizeof(float));
-  NRT_KNN_GET(10, dOC, (size_t)nq * sizeof(int32_t));
-  if (h_boosts) { NRT_KNN_GET(11, dB, (size_t)nq * sizeof(float));
-                  NRT_CUDA_TRY(cudaMemcpyAsync(dB, h_boosts, (size_t)nq * sizeof(float), cudaMemcpyHostToDevice, st)); }
-  if (h_filter) { NRT_KNN_GET(12, dF, (size_t)n_docs);
-                  NRT_CUDA_TRY(cudaMemcpyAsync(dF, h_filter, (size_t)n_docs, cudaMemcpyHostToDevice, st)); }
-  int32_t* dQrow = nullptr;
-  if (h_qrow) { NRT_KNN_GET(16, dQrow, (size_t)nq * sizeof(int32_t));
-                NRT_CUDA_TRY(cudaMemcpyAsync(dQrow, h_qrow, (size_t)nq * sizeof(int32_t), cudaMemcpyHostToDevice, st)); }
-  NRT_CUDA_TRY(cudaMemcpyAsync(dQ, h_queries, (size_t)nq * dims * sizeof(float), cudaMemcpyHostToDevice, st));
+  NRT_KNN_GET(KnnSlot::Scores, dS, (size_t)nq * (fused ? warm : chunk) * sizeof(float));
+  NRT_KNN_GET(KnnSlot::Cand, dC, (size_t)nq * kprime * sizeof(uint64_t));
+  NRT_KNN_GET(KnnSlot::CandCnt, dCn, (size_t)nq * sizeof(int32_t));
+  NRT_KNN_GET(KnnSlot::OutDocs, dOD, (size_t)nq * k * sizeof(int32_t));
+  NRT_KNN_GET(KnnSlot::OutScores, dOS, (size_t)nq * k * sizeof(float));
+  NRT_KNN_GET(KnnSlot::OutCounts, dOC, (size_t)nq * sizeof(int32_t));
+  if (req.boosts) { NRT_KNN_GET(KnnSlot::Boosts, dB, (size_t)nq * sizeof(float));
+                    NRT_CUDA_TRY(cudaMemcpyAsync(dB, req.boosts, (size_t)nq * sizeof(float), cudaMemcpyHostToDevice, st)); }
+  if (req.filter) { NRT_KNN_GET(KnnSlot::Filter, dF, (size_t)corpus.n_docs);
+                    NRT_CUDA_TRY(cudaMemcpyAsync(dF, req.filter, (size_t)corpus.n_docs, cudaMemcpyHostToDevice, st)); }
+  if (req.qrow) { NRT_KNN_GET(KnnSlot::Qrow, dQrow, (size_t)nq * sizeof(int32_t));
+                  NRT_CUDA_TRY(cudaMemcpyAsync(dQrow, req.qrow, (size_t)nq * sizeof(int32_t), cudaMemcpyHostToDevice, st)); }
+  NRT_CUDA_TRY(cudaMemcpyAsync(dQ, req.queries, (size_t)nq * dims * sizeof(float), cudaMemcpyHostToDevice, st));
   NRT_CUDA_TRY(cudaMemsetAsync(dCn, 0, (size_t)nq * sizeof(int32_t), st));
-  __nv_bfloat16* dQb = nullptr;
   CUtensorMap tmQ;
   if (use_tc) {
-    NRT_KNN_GET(13, dQb, (size_t)nq * dims * sizeof(__nv_bfloat16));
+    NRT_KNN_GET(KnnSlot::Qbf16, dQb, (size_t)nq * dims * sizeof(__nv_bfloat16));
     tc::f32_to_bf16_kernel<<<256, 256, 0, st>>>(dQ, dQb, (size_t)nq * dims);
     NRT_CUDA_TRY(cudaGetLastError());
-    int rc = tc::make_tensor_map_bf16(&tmQ, dQb, (uint64_t)nq, (uint64_t)dims, tc::BM);
-    if (rc) return rc;
+    if (int rc = tc::make_tensor_map_bf16(&tmQ, dQb, (uint64_t)nq, (uint64_t)dims, tc::BM)) return rc;
   }
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   float gemm_ms = 0.f, select_ms = 0.f;
@@ -530,16 +572,16 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
     const bool warm_chunk = fused && n_done == 0;
     if (stage_ms) NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
     if (use_tc) {
-      tc::GemmParams G; G.M = nq; G.N = nc; G.K = dims; G.n_base = base; G.dnorm2 = d_norm2 + base; G.ab = d_ab + base; G.sim = sim & 0xff;
+      tc::GemmParams G; G.M = nq; G.N = nc; G.K = dims; G.n_base = base; G.dnorm2 = corpus.norm2 + base; G.ab = corpus.ab + base; G.sim = sim & 0xff;
       G.S = (fused && !warm_chunk) ? nullptr : dS; G.ldS = fused ? warm : chunk;
-      G.theta = dTheta; G.cc = dCC; G.cc_cnt = dCCn; G.cc_cap = cc_cap; G.filter = dF; G.vec_docs = d_vec_docs; G.live_bits = d_live_bits;
-      G.qfilter = d_qfilter; G.qrow = dQrow; G.qwords = qwords;
+      G.theta = dTheta; G.cc = dCC; G.cc_cnt = dCCn; G.cc_cap = cc_cap; G.filter = dF; G.vec_docs = corpus.vec_docs; G.live_bits = corpus.live_bits;
+      G.qfilter = req.d_rows; G.qrow = dQrow; G.qwords = req.words;
       const int tiles = ((nq + tc::BM - 1) / tc::BM) * ((nc + tc::BN - 1) / tc::BN);
-      if (dQrow) tc::knn_gemm_bf16_rows_kernel<<<tiles, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *tm_corpus, G);
-      else tc::knn_gemm_bf16_kernel<<<tiles, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *tm_corpus, G);
+      if (dQrow) tc::knn_gemm_bf16_rows_kernel<<<tiles, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *corpus.tmap, G);
+      else tc::knn_gemm_bf16_kernel<<<tiles, tc::kGemmThreads, tc::kGemmSmem, st>>>(tmQ, *corpus.tmap, G);
     } else {
       dim3 grid((nc + kKnnTile - 1) / kKnnTile, (nq + kKnnTile - 1) / kKnnTile);
-      knn_dot_tile_kernel<<<grid, 256, 0, st>>>(dQ, d_vec + (size_t)base * dims, d_norm2 + base, nq, nc, dims, sim & 0xff, dS, chunk);
+      knn_dot_tile_kernel<<<grid, 256, 0, st>>>(dQ, corpus.vec + (size_t)base * dims, corpus.norm2 + base, nq, nc, dims, sim & 0xff, dS, chunk);
     }
     NRT_CUDA_TRY(cudaGetLastError());
     if (stage_ms) NRT_CUDA_TRY(cudaEventRecord(ev[1], st));
@@ -548,9 +590,9 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
       Mg.theta = dTheta; Mg.overflow = dOvf;
       knn_merge_chunk_kernel<<<nq, kKnnSelThreads, 0, st>>>(Mg);
     } else {
-      KnnSelectLaunch S; S.S = dS; S.ldS = fused ? warm : chunk; S.n_chunk = nc; S.theta_out = fused ? dTheta : nullptr; S.chunk_base = base; S.filter = dF; S.live_bits = d_live_bits; S.vec_docs = d_vec_docs;
-      S.kprime = kprime; S.nq = nq; S.cand = dC; S.cand_cnt = dCn;
-      S.qfilter = d_qfilter; S.qrow = dQrow; S.qwords = qwords;
+      KnnSelectLaunch S; S.S = dS; S.ldS = fused ? warm : chunk; S.n_chunk = nc; S.theta_out = fused ? dTheta : nullptr; S.chunk_base = base; S.filter = dF;
+      S.live_bits = corpus.live_bits; S.vec_docs = corpus.vec_docs; S.kprime = kprime; S.nq = nq; S.cand = dC; S.cand_cnt = dCn;
+      S.qfilter = req.d_rows; S.qrow = dQrow; S.qwords = req.words;
       knn_select_kernel<<<nq, kKnnSelThreads, 0, st>>>(S);
     }
     NRT_CUDA_TRY(cudaGetLastError());
@@ -562,23 +604,21 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
       gemm_ms += a; select_ms += b;
     }
   }
-  if (fused) {   // a chunk produced more survivors than the buffer holds (adversarial order): redo without fusion
+  if (fused) {   // a chunk produced more survivors than the buffer holds (adversarial order): redo with the SIMT stage
     int ovf = 0;
     NRT_CUDA_TRY(cudaMemcpyAsync(&ovf, dOvf, sizeof(int), cudaMemcpyDeviceToHost, st));
     NRT_CUDA_TRY(cudaStreamSynchronize(st));
     if (ovf) {
       if (stage_ms) for (auto& e : ev) cudaEventDestroy(e);
-      return knn_search_host(d_vec, d_norm2, d_vec_docs, n, dims, sim, doc_base, n_docs, h_queries, nq, k, h_boosts, h_filter, st,
-                             out_docs, out_scores, out_counts, nullptr, nullptr, stage_ms, nullptr, sc, d_live_bits, dmax, n_uncertified,
-                             d_qfilter, h_qrow, qwords);
+      KnnCorpus simt = corpus; simt.bf16 = nullptr; simt.tmap = nullptr; simt.ab = nullptr;
+      return knn_search_host(simt, req, sc, st, out, stage_ms, n_uncertified);
     }
   }
   if (stage_ms) NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
-  KnnRescoreLaunch R; R.Q = dQ; R.D = d_vec; R.dims = dims; R.sim = sim; R.cand = dC; R.cand_cnt = dCn; R.kprime = kprime;
-  R.vec_docs = d_vec_docs; R.doc_base = doc_base; R.boosts = dB; R.k = k; R.out_docs = dOD; R.out_scores = dOS; R.out_counts = dOC;
-  int32_t* dUnsafe = nullptr;
-  NRT_KNN_GET(14, dUnsafe, (size_t)nq * sizeof(int32_t));
-  R.unsafe = dUnsafe; R.dmax = dmax;
+  KnnRescoreLaunch R; R.Q = dQ; R.D = corpus.vec; R.dims = dims; R.sim = sim; R.cand = dC; R.cand_cnt = dCn; R.kprime = kprime;
+  R.vec_docs = corpus.vec_docs; R.doc_base = corpus.doc_base; R.boosts = dB; R.k = k; R.out_docs = dOD; R.out_scores = dOS; R.out_counts = dOC;
+  NRT_KNN_GET(KnnSlot::Unsafe, dUnsafe, (size_t)nq * sizeof(int32_t));
+  R.unsafe = dUnsafe; R.dmax = corpus.dmax;
   // bf16 operands: 2^-7 |q||d|; fp32 FMA chain (and byte vectors, whose elements and products are exact in bf16 / fp32): dims * 2^-23
   R.eps_rel = (use_tc && !(sim & kKnnByteFlag)) ? 0.0078125f : (float)dims * 1.1920929e-7f;
   knn_rescore_kernel<<<nq, 256, 0, st>>>(R);
@@ -590,9 +630,9 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
     stage_ms[0] = gemm_ms; stage_ms[1] = select_ms; stage_ms[2] = c;
     for (auto& e : ev) cudaEventDestroy(e);
   }
-  NRT_CUDA_TRY(cudaMemcpyAsync(out_docs, dOD, (size_t)nq * k * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  NRT_CUDA_TRY(cudaMemcpyAsync(out_scores, dOS, (size_t)nq * k * sizeof(float), cudaMemcpyDeviceToHost, st));
-  NRT_CUDA_TRY(cudaMemcpyAsync(out_counts, dOC, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(out.docs, dOD, (size_t)nq * k * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(out.scores, dOS, (size_t)nq * k * sizeof(float), cudaMemcpyDeviceToHost, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(out.counts, dOC, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   std::vector<int32_t> unsafe((size_t)nq);
   NRT_CUDA_TRY(cudaMemcpyAsync(unsafe.data(), dUnsafe, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   NRT_CUDA_TRY(cudaStreamSynchronize(st));
@@ -602,10 +642,8 @@ inline int knn_search_host(const float* d_vec, const float* d_norm2, const int32
   for (int q = 0; q < nq; ++q) if (unsafe[(size_t)q]) sel.push_back(q);
   if (n_uncertified) *n_uncertified = (int32_t)sel.size();
   if (!sel.empty()) {
-    KnnExactLaunch X; X.Q = dQ; X.D = d_vec; X.n = n; X.dims = dims; X.sim = sim; X.boosts = dB; X.filter = dF;
-    X.live_bits = d_live_bits; X.vec_docs = d_vec_docs; X.k = k;
-    X.qfilter = d_qfilter; X.qrow = dQrow; X.qwords = qwords;
-    return knn_exact_host(sc, st, X, (n + kKnnExactChunk - 1) / kKnnExactChunk, doc_base, sel, out_docs, out_scores, out_counts);
+    KnnExactLaunch X; X.Q = dQ; X.boosts = dB; X.filter = dF; X.k = k; X.qfilter = req.d_rows; X.qrow = dQrow; X.qwords = req.words;
+    return knn_exact_host(corpus, sc, st, X, (n + kKnnExactChunk - 1) / kKnnExactChunk, sel, out);
   }
   return NRTGPU_OK;
 }

@@ -228,6 +228,11 @@ struct nrtgpu_index {
     d.col_multi = col_multi.data(); d.col_n_distinct = col_n_distinct.data(); d.has_deletes = live_bits.p != nullptr;
     return d;
   }
+  KnnCorpus knn_corpus() const {   // what the kNN stages read; NRTGPU_KNN_SIMT, read on every call, forces the fp32 SIMT stage
+    const bool t = vec_tc && getenv("NRTGPU_KNN_SIMT") == nullptr;
+    return {vectors.p, vec_norm2.p, vec_docs.p, vec_count, vec_dims, vec_sim | (vec_is_byte ? kKnnByteFlag : 0), doc_base, n_docs,
+            live_bits.p, vec_dmax, t ? vec_bf16.p : nullptr, t ? &vec_tmap : nullptr, t ? vec_ab.p : nullptr};
+  }
 };
 
 // a Sort of several fields ranked over one image (sort_kernel.cuh, sort_order_build)
@@ -1402,19 +1407,21 @@ int nrtgpu_merge_topk_device(nrtgpu_ctx* ctx, int32_t n_lists, int32_t nq, int32
   return NRTGPU_OK;
 }
 
+// nrtgpu_search_knn and nrtgpu_search_knn_timed once their arguments are checked
+static int knn_search_checked(nrtgpu_index* ix, const KnnRequest& req, void* stream, const KnnPages& out, float* stage_ms) {
+  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
+  std::lock_guard<std::mutex> g(ix->knn_mu);
+  return knn_search_host(ix->knn_corpus(), req, ix->knn_scratch, (cudaStream_t)stream, out, stage_ms, &ix->knn_last_uncertified);
+}
+
 int nrtgpu_search_knn(nrtgpu_index* ix, const float* queries, int32_t nq, int32_t k, const float* boosts,
                       const uint8_t* filter, void* stream, int32_t* out_docs, float* out_scores,
                       int32_t* out_counts) {
   if (!ix || !queries || !out_docs || !out_scores || !out_counts) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn: NULL argument");
   if (ix->vec_dims <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn: index has no vector field");
   if (k <= 0 || k > kMaxTopK) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn: k out of range");
-  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
-  const bool tcp = ix->vec_tc && !(getenv("NRTGPU_KNN_SIMT") != nullptr);
-  std::lock_guard<std::mutex> g(ix->knn_mu);
-  return knn_search_host(ix->vectors.p, ix->vec_norm2.p, ix->vec_docs.p, ix->vec_count, ix->vec_dims, ix->vec_sim | (ix->vec_is_byte ? kKnnByteFlag : 0),
-                         ix->doc_base, ix->n_docs, queries, nq, k, boosts, filter, (cudaStream_t)stream, out_docs,
-                         out_scores, out_counts, tcp ? ix->vec_bf16.p : nullptr, tcp ? &ix->vec_tmap : nullptr, nullptr, ix->vec_ab.p,
-                         &ix->knn_scratch, ix->live_bits.p, ix->vec_dmax, &ix->knn_last_uncertified);
+  return knn_search_checked(ix, KnnRequest{queries, nq, k, boosts, filter, nullptr, nullptr, 0}, stream,
+                            KnnPages{out_docs, out_scores, out_counts}, nullptr);
 }
 
 int nrtgpu_search_knn_timed(nrtgpu_index* ix, const float* queries, int32_t nq, int32_t k, void* stream, int32_t* out_docs,
@@ -1422,179 +1429,157 @@ int nrtgpu_search_knn_timed(nrtgpu_index* ix, const float* queries, int32_t nq, 
   if (!ix || !queries || !out_docs || !out_scores || !out_counts || !stage_ms) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_timed: NULL argument");
   if (ix->vec_dims <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_timed: index has no vector field");
   if (k <= 0 || k > kMaxTopK / 4) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_timed: k out of range");
-  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
-  const bool tcp = ix->vec_tc && !(getenv("NRTGPU_KNN_SIMT") != nullptr);
-  std::lock_guard<std::mutex> g(ix->knn_mu);
-  return knn_search_host(ix->vectors.p, ix->vec_norm2.p, ix->vec_docs.p, ix->vec_count, ix->vec_dims, ix->vec_sim | (ix->vec_is_byte ? kKnnByteFlag : 0),
-                         ix->doc_base, ix->n_docs, queries, nq, k, nullptr, nullptr, (cudaStream_t)stream, out_docs,
-                         out_scores, out_counts, tcp ? ix->vec_bf16.p : nullptr, tcp ? &ix->vec_tmap : nullptr, stage_ms, ix->vec_ab.p,
-                         &ix->knn_scratch, ix->live_bits.p, ix->vec_dmax, &ix->knn_last_uncertified);
+  return knn_search_checked(ix, KnnRequest{queries, nq, k, nullptr, nullptr, nullptr, nullptr, 0}, stream,
+                            KnnPages{out_docs, out_scores, out_counts}, stage_ms);
 }
 
 int32_t nrtgpu_knn_last_uncertified(const nrtgpu_index* ix) { return ix ? ix->knn_last_uncertified : 0; }
 
-// Filtered kNN of one group of queries once the filters are compiled into b (NULL: no query has a filter); qrow[q] = filter
-// row of query q or -1, row_filter[r] = the filter behind row r. Adds to the index's filter statistics. Caller holds ix->knn_mu.
-static int knn_filtered_host(nrtgpu_index* ix, const nrtgpu_batch* b, const float* queries, int32_t nq, int32_t k, const float* boosts,
-                             const std::vector<int32_t>& qrow, const std::vector<int32_t>& row_filter, cudaStream_t st,
-                             int32_t* out_docs, float* out_scores, int32_t* out_counts) {
-  KnnScratch* sc = &ix->knn_scratch;
-  const int n_rows = (int)row_filter.size(), words = (ix->n_docs + 31) / 32, n_vec = ix->vec_count, dims = ix->vec_dims;
-  const int sim = ix->vec_sim | (ix->vec_is_byte ? kKnnByteFlag : 0);
-  std::vector<int32_t> cnt((size_t)n_rows, 0);
-  uint32_t* dRows = nullptr; int32_t* dMeta = nullptr;
-  if (n_rows > 0) {
-    // ---- group the rows so that the bitmaps of a group's distinct terms fit kKnnFilterTermBytes; a term clause points
-    //      at its term's bitmap inside its group (terms without postings at none)
-    const int n_cl = (int)b->cb.clauses.size();
-    std::vector<int32_t> clause_term((size_t)std::max(n_cl, 1), -1);
-    std::vector<int64_t> term_base, term_pre(1, 0);
-    std::vector<int> grp_row{0}, grp_term{0};   // group g: rows [grp_row[g], grp_row[g + 1]), terms [grp_term[g], grp_term[g + 1])
-    std::unordered_map<int64_t, int> group_terms;   // post_base -> term index in the current group
-    const size_t term_bytes = (size_t)words * 4;
-    for (int r = 0; r < n_rows; ++r) {
-      const DevQuery& q = b->cb.queries[(size_t)row_filter[(size_t)r]];
-      int fresh = 0;
-      for (int i = 0; i < q.n_clauses; ++i) {
-        const DevClause& c = b->cb.clauses[(size_t)q.clause_begin + i];
-        if (c.kind == NRTGPU_TERM && c.n_post > 0 && !group_terms.count(c.post_base)) ++fresh;
-      }
-      const int rows_in = r - grp_row.back();
-      if (rows_in > 0 && (rows_in == 65535 || (group_terms.size() + fresh) * term_bytes > kKnnFilterTermBytes)) {
-        grp_row.push_back(r); grp_term.push_back((int)term_base.size()); group_terms.clear();
-      }
-      for (int i = 0; i < q.n_clauses; ++i) {
-        const int ci = q.clause_begin + i;
-        const DevClause& c = b->cb.clauses[(size_t)ci];
-        if (c.kind != NRTGPU_TERM || c.n_post == 0) continue;
-        auto it = group_terms.find(c.post_base);
-        if (it == group_terms.end()) {
-          it = group_terms.emplace(c.post_base, (int)group_terms.size()).first;
-          term_base.push_back(c.post_base); term_pre.push_back(term_pre.back() + c.n_post);
-        }
-        clause_term[(size_t)ci] = it->second;
-      }
+struct KnnFilterRows { const uint32_t* bits = nullptr; int32_t* ord_cnt = nullptr; std::vector<int32_t> cnt; };
+
+// The rows of the filters row_filter[] of b (that fit kKnnFilterRowBytes): bit d of row r of bits (device [n_rows][words])
+// is set iff live doc d matches filter row_filter[r], cnt[r] counts them, ord_cnt (device [n_rows], zeroed) is the gather
+// path's. Adds the device time to the filter statistics.
+static int knn_filter_rows(nrtgpu_index* ix, const nrtgpu_batch* b, const std::vector<int32_t>& row_filter, cudaStream_t st,
+                           KnnFilterRows& out) {
+  KnnScratch& sc = ix->knn_scratch;
+  const int n_rows = (int)row_filter.size(), words = (ix->n_docs + 31) / 32;
+  // ---- group the rows so that the bitmaps of a group's distinct terms fit kKnnFilterTermBytes; a term clause points
+  //      at its term's bitmap inside its group (terms without postings at none)
+  const int n_cl = (int)b->cb.clauses.size();
+  std::vector<int32_t> clause_term((size_t)std::max(n_cl, 1), -1);
+  std::vector<int64_t> term_base, term_pre(1, 0);
+  std::vector<int> grp_row{0}, grp_term{0};   // group g: rows [grp_row[g], grp_row[g + 1]), terms [grp_term[g], grp_term[g + 1])
+  std::unordered_map<int64_t, int> group_terms;   // post_base -> term index in the current group
+  const size_t term_bytes = (size_t)words * 4;
+  for (int r = 0; r < n_rows; ++r) {
+    const DevQuery& q = b->cb.queries[(size_t)row_filter[(size_t)r]];
+    int fresh = 0;
+    for (int i = 0; i < q.n_clauses; ++i) {
+      const DevClause& c = b->cb.clauses[(size_t)q.clause_begin + i];
+      if (c.kind == NRTGPU_TERM && c.n_post > 0 && !group_terms.count(c.post_base)) ++fresh;
     }
-    grp_row.push_back(n_rows); grp_term.push_back((int)term_base.size());
-    const int n_terms = (int)term_base.size();
-    int64_t* dTerm = nullptr;
-    NRT_KNN_GET(17, dRows, (size_t)n_rows * words * 4);
-    NRT_KNN_GET(19, dTerm, (size_t)(2 * n_terms + 1) * 8);
-    NRT_KNN_GET(20, dMeta, (size_t)(3 * n_rows + n_cl + 1) * 4);   // row_filter | row_cnt | ord_cnt | clause_term
-    int32_t *dRowFilter = dMeta, *dRowCnt = dMeta + n_rows, *dClauseTerm = dMeta + 3 * n_rows;
-    if (n_terms) NRT_CUDA_TRY(cudaMemcpyAsync(dTerm, term_base.data(), (size_t)n_terms * 8, cudaMemcpyHostToDevice, st));
-    NRT_CUDA_TRY(cudaMemcpyAsync(dTerm + n_terms, term_pre.data(), (size_t)(n_terms + 1) * 8, cudaMemcpyHostToDevice, st));
-    NRT_CUDA_TRY(cudaMemcpyAsync(dRowFilter, row_filter.data(), (size_t)n_rows * 4, cudaMemcpyHostToDevice, st));
-    NRT_CUDA_TRY(cudaMemsetAsync(dRowCnt, 0, (size_t)2 * n_rows * 4, st));
-    NRT_CUDA_TRY(cudaMemcpyAsync(dClauseTerm, clause_term.data(), clause_term.size() * 4, cudaMemcpyHostToDevice, st));
-    if (!ix->knn_ev[0]) for (auto& e : ix->knn_ev) NRT_CUDA_TRY(cudaEventCreate(&e));
-    NRT_CUDA_TRY(cudaEventRecord(ix->knn_ev[0], st));
-    // ---- per group: term bitmaps, then the rows
-    size_t group_bytes = 0;
-    for (size_t g = 0; g + 1 < grp_row.size(); ++g) group_bytes = std::max(group_bytes, (size_t)(grp_term[g + 1] - grp_term[g]) * term_bytes);
-    uint32_t* dTbits = nullptr;
-    NRT_KNN_GET(18, dTbits, std::max<size_t>(group_bytes, 4));
-    for (size_t g = 0; g + 1 < grp_row.size(); ++g) {
-      const int t0 = grp_term[g], nt = grp_term[g + 1] - t0;
-      if (nt > 0) {
-        NRT_CUDA_TRY(cudaMemsetAsync(dTbits, 0, (size_t)nt * term_bytes, st));
-        KnnTermScatterLaunch S; S.post_docs = ix->post_docs.p; S.term_base = dTerm + t0; S.term_pre = dTerm + n_terms + t0;
-        S.n_terms = nt; S.words = words; S.tbits = dTbits;
-        const int64_t posts = term_pre[(size_t)t0 + nt] - term_pre[(size_t)t0];
-        knn_term_scatter_kernel<<<(unsigned)std::min<int64_t>((posts + 255) / 256, 8 * 1024), 256, 0, st>>>(S);
-        NRT_CUDA_TRY(cudaGetLastError());
-      }
-      KnnFilterRowsLaunch R; R.ix = ix->view(); R.clauses = b->clauses.p; R.filters = b->queries.p; R.row_filter = dRowFilter;
-      R.clause_term = dClauseTerm; R.tbits = dTbits; R.row0 = grp_row[g]; R.words = words; R.rows = dRows; R.row_cnt = dRowCnt;
-      knn_filter_rows_kernel<<<dim3((unsigned)((words + 255) / 256), (unsigned)(grp_row[g + 1] - grp_row[g])), 256, 0, st>>>(R);
+    const int rows_in = r - grp_row.back();
+    if (rows_in > 0 && (rows_in == 65535 || (group_terms.size() + fresh) * term_bytes > kKnnFilterTermBytes)) {
+      grp_row.push_back(r); grp_term.push_back((int)term_base.size()); group_terms.clear();
+    }
+    for (int i = 0; i < q.n_clauses; ++i) {
+      const int ci = q.clause_begin + i;
+      const DevClause& c = b->cb.clauses[(size_t)ci];
+      if (c.kind != NRTGPU_TERM || c.n_post == 0) continue;
+      const auto [it, added] = group_terms.emplace(c.post_base, (int)group_terms.size());
+      if (added) { term_base.push_back(c.post_base); term_pre.push_back(term_pre.back() + c.n_post); }
+      clause_term[(size_t)ci] = it->second;
+    }
+  }
+  grp_row.push_back(n_rows); grp_term.push_back((int)term_base.size());
+  const int n_terms = (int)term_base.size();
+  uint32_t* dRows = nullptr; int64_t* dTerm = nullptr; int32_t* dMeta = nullptr;
+  NRT_KNN_GET(KnnSlot::Rows, dRows, (size_t)n_rows * words * 4);
+  NRT_KNN_GET(KnnSlot::Terms, dTerm, (size_t)(2 * n_terms + 1) * 8);
+  NRT_KNN_GET(KnnSlot::RowMeta, dMeta, (size_t)(3 * n_rows + n_cl + 1) * 4);   // row_filter | row_cnt | ord_cnt | clause_term
+  int32_t *dRowFilter = dMeta, *dRowCnt = dMeta + n_rows, *dClauseTerm = dMeta + 3 * n_rows;
+  if (n_terms) NRT_CUDA_TRY(cudaMemcpyAsync(dTerm, term_base.data(), (size_t)n_terms * 8, cudaMemcpyHostToDevice, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(dTerm + n_terms, term_pre.data(), (size_t)(n_terms + 1) * 8, cudaMemcpyHostToDevice, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(dRowFilter, row_filter.data(), (size_t)n_rows * 4, cudaMemcpyHostToDevice, st));
+  NRT_CUDA_TRY(cudaMemsetAsync(dRowCnt, 0, (size_t)2 * n_rows * 4, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(dClauseTerm, clause_term.data(), clause_term.size() * 4, cudaMemcpyHostToDevice, st));
+  if (!ix->knn_ev[0]) for (auto& e : ix->knn_ev) NRT_CUDA_TRY(cudaEventCreate(&e));
+  NRT_CUDA_TRY(cudaEventRecord(ix->knn_ev[0], st));
+  // ---- per group: term bitmaps, then the rows
+  size_t group_bytes = 0;
+  for (size_t g = 0; g + 1 < grp_row.size(); ++g) group_bytes = std::max(group_bytes, (size_t)(grp_term[g + 1] - grp_term[g]) * term_bytes);
+  uint32_t* dTbits = nullptr;
+  NRT_KNN_GET(KnnSlot::TermBits, dTbits, std::max<size_t>(group_bytes, 4));
+  for (size_t g = 0; g + 1 < grp_row.size(); ++g) {
+    const int t0 = grp_term[g], nt = grp_term[g + 1] - t0;
+    if (nt > 0) {
+      NRT_CUDA_TRY(cudaMemsetAsync(dTbits, 0, (size_t)nt * term_bytes, st));
+      KnnTermScatterLaunch S; S.post_docs = ix->post_docs.p; S.term_base = dTerm + t0; S.term_pre = dTerm + n_terms + t0;
+      S.n_terms = nt; S.words = words; S.tbits = dTbits;
+      const int64_t posts = term_pre[(size_t)t0 + nt] - term_pre[(size_t)t0];
+      knn_term_scatter_kernel<<<(unsigned)std::min<int64_t>((posts + 255) / 256, 8 * 1024), 256, 0, st>>>(S);
       NRT_CUDA_TRY(cudaGetLastError());
     }
-    NRT_CUDA_TRY(cudaEventRecord(ix->knn_ev[1], st));
-    NRT_CUDA_TRY(cudaMemcpyAsync(cnt.data(), dRowCnt, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, st));
-    NRT_CUDA_TRY(cudaStreamSynchronize(st));
-    float ms = 0.0f;
-    NRT_CUDA_TRY(cudaEventElapsedTime(&ms, ix->knn_ev[0], ix->knn_ev[1]));
-    ix->knn_last_filter_ms += ms;
+    KnnFilterRowsLaunch R; R.ix = ix->view(); R.clauses = b->clauses.p; R.filters = b->queries.p; R.row_filter = dRowFilter;
+    R.clause_term = dClauseTerm; R.tbits = dTbits; R.row0 = grp_row[g]; R.words = words; R.rows = dRows; R.row_cnt = dRowCnt;
+    knn_filter_rows_kernel<<<dim3((unsigned)((words + 255) / 256), (unsigned)(grp_row[g + 1] - grp_row[g])), 256, 0, st>>>(R);
+    NRT_CUDA_TRY(cudaGetLastError());
   }
-  // ---- partition: a query whose filter matches at most n_vec / kKnnGatherRatio docs is scored over those docs only
-  const bool can_gather = !ix->vec_docs.p || ix->vec_docs_ascending;
-  std::vector<int32_t> gsel, tsel;
-  for (int q = 0; q < nq; ++q) {
-    const int r = qrow[(size_t)q];
-    if (can_gather && r >= 0 && (int64_t)cnt[(size_t)r] * kKnnGatherRatio <= (int64_t)n_vec) gsel.push_back(q); else tsel.push_back(q);
+  NRT_CUDA_TRY(cudaEventRecord(ix->knn_ev[1], st));
+  out.bits = dRows; out.ord_cnt = dMeta + 2 * n_rows; out.cnt.assign((size_t)n_rows, 0);
+  NRT_CUDA_TRY(cudaMemcpyAsync(out.cnt.data(), dRowCnt, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, st));
+  NRT_CUDA_TRY(cudaStreamSynchronize(st));
+  float ms = 0.0f;
+  NRT_CUDA_TRY(cudaEventElapsedTime(&ms, ix->knn_ev[0], ix->knn_ev[1]));
+  ix->knn_last_filter_ms += ms;
+  return NRTGPU_OK;
+}
+
+// Gather path of the queries first .. g.nq - 1 of g: each of their rows' ordinals listed once, then scored exactly.
+static int knn_gather_host(const KnnCorpus& corpus, const KnnRequest& g, int first, const KnnFilterRows& rows, KnnScratch& sc,
+                           cudaStream_t st, const KnnPages& out) {
+  const int nq = g.nq, dims = corpus.dims, n_vec = corpus.n, n_rows = (int)rows.cnt.size();
+  std::vector<int32_t> gsel, grows;
+  std::vector<int64_t> ord_begin((size_t)n_rows, -1);   // -1: no query of the gather path has the row
+  int64_t total = 0; int max_cnt = 0;
+  for (int q = first; q < nq; ++q) {
+    const int r = g.qrow[q];
+    gsel.push_back(q);
+    if (ord_begin[(size_t)r] >= 0) continue;
+    grows.push_back(r);
+    ord_begin[(size_t)r] = total; total += rows.cnt[(size_t)r]; max_cnt = std::max(max_cnt, rows.cnt[(size_t)r]);
+  }
+  int32_t *dOrds = nullptr, *dGrows = nullptr, *dQrow = nullptr; int64_t* dOrdBegin = nullptr; float *dQ = nullptr, *dB = nullptr;
+  NRT_KNN_GET(KnnSlot::GatherQ, dQ, (size_t)nq * dims * 4);
+  NRT_KNN_GET(KnnSlot::Ords, dOrds, (size_t)std::max<int64_t>(total, 1) * 4);
+  NRT_KNN_GET(KnnSlot::OrdBegin, dOrdBegin, (size_t)n_rows * 8);
+  NRT_KNN_GET(KnnSlot::GatherRows, dGrows, grows.size() * 4);
+  NRT_KNN_GET(KnnSlot::GatherQrow, dQrow, (size_t)nq * 4);
+  NRT_CUDA_TRY(cudaMemcpyAsync(dQ, g.queries, (size_t)nq * dims * 4, cudaMemcpyHostToDevice, st));
+  if (g.boosts) { NRT_KNN_GET(KnnSlot::GatherBoosts, dB, (size_t)nq * 4); NRT_CUDA_TRY(cudaMemcpyAsync(dB, g.boosts, (size_t)nq * 4, cudaMemcpyHostToDevice, st)); }
+  NRT_CUDA_TRY(cudaMemcpyAsync(dOrdBegin, ord_begin.data(), (size_t)n_rows * 8, cudaMemcpyHostToDevice, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(dGrows, grows.data(), grows.size() * 4, cudaMemcpyHostToDevice, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(dQrow, g.qrow, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+  KnnFilterOrdsLaunch O; O.rows = rows.bits; O.words = g.words; O.ord_begin = dOrdBegin; O.vec_docs = corpus.vec_docs; O.n_vec = n_vec;
+  O.ords = dOrds; O.ord_cnt = rows.ord_cnt;
+  const int items = corpus.vec_docs ? n_vec : (n_vec + 31) / 32;
+  for (size_t g0 = 0; g0 < grows.size(); g0 += 65535) {
+    O.grows = dGrows + g0;
+    knn_filter_ords_kernel<<<dim3((unsigned)((items + 255) / 256), (unsigned)std::min<size_t>(65535, grows.size() - g0)), 256, 0, st>>>(O);
+    NRT_CUDA_TRY(cudaGetLastError());
+  }
+  KnnExactLaunch X; X.Q = dQ; X.boosts = dB; X.filter = nullptr; X.k = g.k; X.qfilter = rows.bits; X.qrow = dQrow; X.qwords = g.words;
+  X.ords = dOrds; X.ord_begin = dOrdBegin; X.ord_cnt = rows.ord_cnt;
+  return knn_exact_host(corpus, sc, st, X, std::max(1, (max_cnt + kKnnExactChunk - 1) / kKnnExactChunk), gsel, out);
+}
+
+// Filtered kNN of the queries whose row req.qrow[q] is in [r0, r1) (r0 = 0: also those without a filter). A query whose
+// filter matches at most n_vec / kKnnGatherRatio docs is scored over those docs only, every other one by the candidate
+// stage with its row, on a prefix of the batch packed with those first. Caller holds ix->knn_mu.
+static int knn_filtered_group(nrtgpu_index* ix, const nrtgpu_batch* b, const KnnRequest& req,
+                              const std::vector<int32_t>& row_filter, int r0, int r1, cudaStream_t st, const KnnPages& out) {
+  KnnFilterRows rows;
+  if (r1 > r0) if (int rc = knn_filter_rows(ix, b, {row_filter.begin() + r0, row_filter.begin() + r1}, st, rows)) return rc;
+  const KnnCorpus corpus = ix->knn_corpus();
+  const bool can_gather = !corpus.vec_docs || ix->vec_docs_ascending;
+  std::vector<int32_t> lrow((size_t)req.nq, -1), order, gsel;   // lrow: row in this group (-1: none)
+  for (int q = 0; q < req.nq; ++q) {
+    const int r = req.qrow[q], lr = r < 0 ? -1 : r - r0;
+    if (r >= 0 ? r >= r1 || lr < 0 : r0 > 0) continue;
+    lrow[(size_t)q] = lr;
+    (lr >= 0 && can_gather && (int64_t)rows.cnt[(size_t)lr] * kKnnGatherRatio <= (int64_t)corpus.n ? gsel : order).push_back(q);
   }
   ix->knn_last_gather += (int32_t)gsel.size();
-  const bool tcp = ix->vec_tc && !(getenv("NRTGPU_KNN_SIMT") != nullptr);
-  if (!tsel.empty()) {   // candidate GEMM path with the rows; a subset goes through packed copies and is scattered back
-    const bool all = (int)tsel.size() == nq;
-    const int nt = (int)tsel.size();
-    std::vector<float> tq, tb; std::vector<int32_t> tr, td, tc; std::vector<float> ts;
-    int32_t unc = 0;
-    if (!all) {
-      tq.resize((size_t)nt * dims); tr.resize((size_t)nt); td.resize((size_t)nt * k); ts.resize((size_t)nt * k); tc.resize((size_t)nt);
-      if (boosts) tb.resize((size_t)nt);
-      for (int i = 0; i < nt; ++i) {
-        const int q = tsel[(size_t)i];
-        std::memcpy(tq.data() + (size_t)i * dims, queries + (size_t)q * dims, (size_t)dims * 4);
-        tr[(size_t)i] = qrow[(size_t)q];
-        if (boosts) tb[(size_t)i] = boosts[q];
-      }
-    }
-    int rc = knn_search_host(ix->vectors.p, ix->vec_norm2.p, ix->vec_docs.p, n_vec, dims, sim, ix->doc_base, ix->n_docs,
-                             all ? queries : tq.data(), nt, k, (all || !boosts) ? boosts : tb.data(), nullptr, st,
-                             all ? out_docs : td.data(), all ? out_scores : ts.data(), all ? out_counts : tc.data(),
-                             tcp ? ix->vec_bf16.p : nullptr, tcp ? &ix->vec_tmap : nullptr, nullptr, ix->vec_ab.p, sc,
-                             ix->live_bits.p, ix->vec_dmax, &unc, n_rows ? dRows : nullptr,
-                             n_rows ? (all ? qrow.data() : tr.data()) : nullptr, words);
-    if (rc) return rc;
+  const int nt = (int)order.size();
+  order.insert(order.end(), gsel.begin(), gsel.end());
+  KnnRequest greq = req; greq.qrow = r1 > r0 ? lrow.data() : nullptr; greq.d_rows = rows.bits; greq.words = (ix->n_docs + 31) / 32;
+  return knn_run_subset(greq, corpus.dims, order, out, [&](const KnnRequest& g, const KnnPages& o) {
+    KnnRequest t = g; t.nq = nt; int32_t unc = 0;
+    if (int rc = nt > 0 ? knn_search_host(corpus, t, ix->knn_scratch, st, o, nullptr, &unc) : NRTGPU_OK) return rc;
     ix->knn_last_uncertified += unc;
-    if (!all)
-      for (int i = 0; i < nt; ++i) {
-        const int q = tsel[(size_t)i];
-        std::memcpy(out_docs + (size_t)q * k, td.data() + (size_t)i * k, (size_t)k * 4);
-        std::memcpy(out_scores + (size_t)q * k, ts.data() + (size_t)i * k, (size_t)k * 4);
-        out_counts[q] = tc[(size_t)i];
-      }
-  }
-  if (!gsel.empty()) {   // gather path: list each small row's ordinals once, then score them exactly
-    std::vector<int32_t> grows;
-    std::vector<int64_t> ord_begin((size_t)n_rows, 0);
-    std::vector<uint8_t> listed((size_t)n_rows, 0);
-    int64_t total = 0; int max_cnt = 0;
-    for (int q : gsel) {
-      const int r = qrow[(size_t)q];
-      if (listed[(size_t)r]) continue;
-      listed[(size_t)r] = 1; grows.push_back(r);
-      ord_begin[(size_t)r] = total; total += cnt[(size_t)r]; max_cnt = std::max(max_cnt, cnt[(size_t)r]);
-    }
-    int32_t *dOrds = nullptr, *dGrows = nullptr, *dQrow = nullptr; int64_t* dOrdBegin = nullptr; float *dQ = nullptr, *dB = nullptr;
-    NRT_KNN_GET(21, dQ, (size_t)nq * dims * 4);
-    NRT_KNN_GET(23, dOrds, (size_t)std::max<int64_t>(total, 1) * 4);
-    NRT_KNN_GET(24, dOrdBegin, (size_t)n_rows * 8);
-    NRT_KNN_GET(25, dGrows, grows.size() * 4);
-    NRT_KNN_GET(26, dQrow, (size_t)nq * 4);
-    NRT_CUDA_TRY(cudaMemcpyAsync(dQ, queries, (size_t)nq * dims * 4, cudaMemcpyHostToDevice, st));
-    if (boosts) { NRT_KNN_GET(22, dB, (size_t)nq * 4); NRT_CUDA_TRY(cudaMemcpyAsync(dB, boosts, (size_t)nq * 4, cudaMemcpyHostToDevice, st)); }
-    NRT_CUDA_TRY(cudaMemcpyAsync(dOrdBegin, ord_begin.data(), (size_t)n_rows * 8, cudaMemcpyHostToDevice, st));
-    NRT_CUDA_TRY(cudaMemcpyAsync(dGrows, grows.data(), grows.size() * 4, cudaMemcpyHostToDevice, st));
-    NRT_CUDA_TRY(cudaMemcpyAsync(dQrow, qrow.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, st));
-    int32_t* dOrdCnt = dMeta + 2 * n_rows;
-    KnnFilterOrdsLaunch O; O.rows = dRows; O.words = words; O.ord_begin = dOrdBegin; O.vec_docs = ix->vec_docs.p; O.n_vec = n_vec;
-    O.ords = dOrds; O.ord_cnt = dOrdCnt;
-    const int items = ix->vec_docs.p ? n_vec : (n_vec + 31) / 32;
-    for (size_t g0 = 0; g0 < grows.size(); g0 += 65535) {
-      O.grows = dGrows + g0;
-      knn_filter_ords_kernel<<<dim3((unsigned)((items + 255) / 256), (unsigned)std::min<size_t>(65535, grows.size() - g0)), 256, 0, st>>>(O);
-      NRT_CUDA_TRY(cudaGetLastError());
-    }
-    KnnExactLaunch X; X.Q = dQ; X.D = ix->vectors.p; X.n = n_vec; X.dims = dims; X.sim = sim; X.boosts = dB; X.filter = nullptr;
-    X.live_bits = ix->live_bits.p; X.vec_docs = ix->vec_docs.p; X.k = k;
-    X.qfilter = dRows; X.qrow = dQrow; X.qwords = words; X.ords = dOrds; X.ord_begin = dOrdBegin; X.ord_cnt = dOrdCnt;
-    const int n_chunks = std::max(1, (max_cnt + kKnnExactChunk - 1) / kKnnExactChunk);
-    int rc = knn_exact_host(sc, st, X, n_chunks, ix->doc_base, gsel, out_docs, out_scores, out_counts);
-    if (rc) return rc;
-  }
-  return NRTGPU_OK;
+    return g.nq > nt ? knn_gather_host(corpus, g, nt, rows, ix->knn_scratch, st, o) : NRTGPU_OK;
+  });
 }
 
 int nrtgpu_search_knn_filtered(nrtgpu_index* ix, const float* queries, int32_t nq, int32_t k, const float* boosts,
@@ -1632,34 +1617,10 @@ int nrtgpu_search_knn_filtered(nrtgpu_index* ix, const float* queries, int32_t n
     // bounded scratch: the queries run in groups whose distinct rows fit kKnnFilterRowBytes. Rows are numbered in order of
     // first use, so group g owns rows [g * per, (g + 1) * per); a query goes with its row (no filter: group 0).
     const int n_rows = (int)row_filter.size();
-    const int64_t row_bytes = (int64_t)((ix->n_docs + 31) / 32) * 4;
-    const int per = (int)std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t)kKnnFilterRowBytes / row_bytes));
-    if (n_rows <= per) {
-      rc = knn_filtered_host(ix, n_rows ? b : nullptr, queries, nq, k, boosts, qrow, row_filter, st, out_docs, out_scores, out_counts);
-    } else {
-      const int dims = ix->vec_dims;
-      for (int r0 = 0; r0 < n_rows && !rc; r0 += per) {
-        const int r1 = std::min(n_rows, r0 + per);
-        std::vector<int32_t> sel, gq, grow(row_filter.begin() + r0, row_filter.begin() + r1);
-        for (int q = 0; q < nq; ++q) {
-          const int r = qrow[(size_t)q];
-          if ((r >= r0 && r < r1) || (r < 0 && r0 == 0)) { sel.push_back(q); gq.push_back(r < 0 ? -1 : r - r0); }
-        }
-        const size_t n = sel.size();
-        std::vector<float> qv(n * dims), bv(boosts ? n : 0), sv(n * k);
-        std::vector<int32_t> dv(n * k), cv(n);
-        for (size_t i = 0; i < n; ++i) {
-          std::memcpy(qv.data() + i * dims, queries + (size_t)sel[i] * dims, (size_t)dims * 4);
-          if (boosts) bv[i] = boosts[sel[i]];
-        }
-        rc = knn_filtered_host(ix, b, qv.data(), (int32_t)n, k, boosts ? bv.data() : nullptr, gq, grow, st, dv.data(), sv.data(), cv.data());
-        for (size_t i = 0; i < n && !rc; ++i) {
-          std::memcpy(out_docs + (size_t)sel[i] * k, dv.data() + i * k, (size_t)k * 4);
-          std::memcpy(out_scores + (size_t)sel[i] * k, sv.data() + i * k, (size_t)k * 4);
-          out_counts[sel[i]] = cv[i];
-        }
-      }
-    }
+    const int per = (int)std::max<int64_t>(1, std::min<int64_t>(65535, (int64_t)kKnnFilterRowBytes / ((ix->n_docs + 31) / 32 * 4)));
+    const KnnRequest req{queries, nq, k, boosts, nullptr, nullptr, qrow.data(), 0};
+    for (int r0 = 0; !rc && (r0 == 0 || r0 < n_rows); r0 += per)
+      rc = knn_filtered_group(ix, b, req, row_filter, r0, std::min(n_rows, r0 + per), st, KnnPages{out_docs, out_scores, out_counts});
   }
   return rc;
 }
