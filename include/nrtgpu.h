@@ -173,6 +173,43 @@ int nrtgpu_search_bool_ex(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_
                           void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
                           int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
                           uint8_t* out_terminated_early);
+/* Query trees (BooleanQuery and DisjunctionMaxQuery nested in a BooleanQuery, reference QueryNodeMapper.java:257-283 for
+ * bool, :360-395 for a match of several tokens, :429-497 for multi_match BEST_FIELDS). The leaves are the clause kinds
+ * above; a clause of kind NRTGPU_NODE is a nested query whose id indexes nodes[], and each node's clauses are
+ * clauses[clause_begin:clause_end] of the same array. The root of query q is still queries[q] (a BooleanQuery with its
+ * msm and searchAfter); a DisjunctionMaxQuery at the root is a root with one MUST node clause, and scores exactly as the
+ * dismax does.
+ *   BOOL node:   the rule of a flat BooleanQuery, a child node counting as a clause that scores the child's float;
+ *   DISMAX node: matches if any disjunct does, scores (float)((double)max + others * (double)tie_breaker), where others is
+ *                the double sum of the other matching disjuncts (DisjunctionMaxScorer, Lucene 10).
+ * Subtrees under FILTER and MUST_NOT only match. Boosts are folded into the leaves (outermost first, in float): a node
+ * clause has boost 1. Every tree batch runs on the window engine (as a batch with more than 4 term clauses does).
+ *   NRTGPU_ERR_INVALID:     a node id out of range, a node referenced twice or from a cycle, a bad node kind or clause
+ *                           range, a DISMAX clause whose occur is not SHOULD, tie_breaker outside [0, 1], a node clause
+ *                           whose boost is not 1, msm < 0, and every check of nrtgpu_search_bool_ex.
+ *   NRTGPU_ERR_UNSUPPORTED: more than 8 term leaves, 8 nodes or 32 clauses in one tree, more than 4 levels of queries
+ *                           (the root counts as one), top_k > 1024.
+ * With n_nodes == 0 nrtgpu_search_tree is nrtgpu_search_bool_ex (same compile, same engine); the other entry points
+ * reject NRTGPU_NODE clauses as a bad clause kind. */
+enum { NRTGPU_NODE = 3 };
+enum { NRTGPU_NODE_BOOL = 0, NRTGPU_NODE_DISMAX = 1 };
+typedef struct {
+  int32_t kind;                      /* NRTGPU_NODE_BOOL / NRTGPU_NODE_DISMAX */
+  int32_t clause_begin, clause_end;  /* its clauses in the same clauses[] array */
+  int32_t min_should_match;          /* BOOL */
+  float tie_breaker;                 /* DISMAX: tieBreakerMultiplier, in [0, 1] */
+  int32_t reserved;
+} nrtgpu_node;
+int nrtgpu_search_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                       int32_t n_nodes, const nrtgpu_query* queries, int32_t nq, int32_t top_k,
+                       int32_t total_hits_threshold, int32_t flags, const nrtgpu_search_limits* limits, void* stream,
+                       int32_t* out_docs, float* out_scores, int32_t* out_counts, int64_t* out_total_hits,
+                       uint8_t* out_relation, uint8_t* out_hit_timeout, uint8_t* out_terminated_early);
+/* split form of nrtgpu_search_tree: then nrtgpu_batch_run / _fetch / _bind_packed / ... as for nrtgpu_batch_prepare */
+int nrtgpu_batch_prepare_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                              int32_t n_nodes, const nrtgpu_query* queries, int32_t nq, int32_t top_k,
+                              int32_t total_hits_threshold, int32_t flags, nrtgpu_batch** out);
+
 /* same search with HOST query buffers, results left on the DEVICE in one packed record (see nrtgpu_packed_words): the
  * multi-GPU request path (the caller all-gathers the record on `stream`, then nrtgpu_merge_topk_packed). Synchronises. */
 int nrtgpu_search_bool_packed(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -309,7 +346,8 @@ int nrtgpu_rescore_query(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
 int nrtgpu_fetch_columns(nrtgpu_index* ix, const int32_t* col_ids, int32_t n_cols, const int32_t* docs, int32_t n,
                          void* stream, int64_t* out_values, uint8_t* out_has);
 
-/* Split form: compile+upload once, launch many times with everything resident in HBM. */
+/* Split form: compile+upload once, launch many times with everything resident in HBM (query trees:
+ * nrtgpu_batch_prepare_tree). */
 int nrtgpu_batch_prepare(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
                          const nrtgpu_query* queries, int32_t nq, int32_t top_k,
                          int32_t total_hits_threshold, int32_t flags, nrtgpu_batch** out);

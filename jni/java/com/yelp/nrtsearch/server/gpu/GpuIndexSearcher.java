@@ -15,7 +15,9 @@ import org.apache.lucene.search.TotalHits;
  * Reference-side adaptor (not built in the authoring image: no JDK / Lucene jars there). A MyIndexSearcher subclass
  * created at ShardState.ShardSearcherFactory.newSearcher (ShardState.java:506-526). search() pattern-matches the
  * rewritten Query (flat BooleanQuery of TermQuery / IndexOrDocValuesQuery range / MatchAllDocsQuery, optional
- * BoostQuery wrappers) and the RelevanceCollector configuration. A supported request is handed to the NATIVE
+ * BoostQuery wrappers; or a tree of nested BooleanQuery / DisjunctionMaxQuery nodes over those leaves) and the
+ * RelevanceCollector configuration. A compiled request that carries nodes calls nrtgpu_search_tree directly on the
+ * handler thread. Any other supported request is handed to the NATIVE
  * micro-batcher (nrtgpu_batcher_submit): the gRPC handler thread blocks while a worker thread inside libnrtgpu groups
  * the waiting requests into one batched search. Everything else, and NRTGPU_ERR_UNSUPPORTED
  * (UnsupportedOperationException), falls through to super.search(), i.e. Lucene. The image and its batcher are released
@@ -52,6 +54,10 @@ public class GpuIndexSearcher extends MyIndexSearcher {
     if (c.sortFields() != null) {
       T sorted = searchSortedFields(c);
       return sorted != null ? sorted : super.search(query, collectorManager);
+    }
+    if (c.numNodes() > 0) {
+      T tree = searchTree(c);
+      return tree != null ? tree : super.search(query, collectorManager);
     }
     int k = c.topK();
     ByteBuffer docs = direct(4 * k), scores = direct(4 * k), count = direct(4), total = direct(8);
@@ -128,6 +134,35 @@ public class GpuIndexSearcher extends MyIndexSearcher {
         new TotalHits(total.getLong(0), rel), hitDocs, hitValues, hitTimeout.get(0) != 0, terminated.get(0) != 0);
   }
 
+  /**
+   * A query tree (nested BooleanQuery / DisjunctionMaxQuery; the micro-batcher takes flat queries only): one
+   * nrtgpu_search_tree call for this request. null = UNSUPPORTED (past the tree limits): Lucene.
+   */
+  private <T> T searchTree(GpuQueryCompiler.Compiled c) {
+    int k = c.topK();
+    ByteBuffer docs = direct(4 * k), scores = direct(4 * k), count = direct(4), total = direct(8);
+    ByteBuffer relation = direct(1), hitTimeout = direct(1), terminated = direct(1);
+    long t0 = System.nanoTime();
+    try {
+      NrtGpu.searchTree(
+          gpuIndex, c.clauses(), c.numClauses(), c.nodes(), c.numNodes(), c.queries(), 1, k, c.totalHitsThreshold(), 0,
+          c.limits(), docs, scores, count, total, relation, hitTimeout, terminated);
+    } catch (UnsupportedOperationException e) {
+      return null;
+    }
+    double searchMs = (System.nanoTime() - t0) / 1e6;
+    int n = count.getInt(0);
+    ScoreDoc[] hits = new ScoreDoc[n];
+    for (int i = 0; i < n; ++i) {
+      hits[i] = new ScoreDoc(docs.getInt(4 * i), scores.getFloat(4 * i));
+    }
+    TotalHits.Relation rel =
+        relation.get(0) == 0
+            ? TotalHits.Relation.EQUAL_TO
+            : TotalHits.Relation.GREATER_THAN_OR_EQUAL_TO;
+    return c.toResult(new TopDocs(new TotalHits(total.getLong(0), rel), hits), 0.0, searchMs, 1);
+  }
+
   public void close() {
     for (long order : sortOrders.values()) {
       NrtGpu.sortOrderClose(order);
@@ -166,7 +201,7 @@ public class GpuIndexSearcher extends MyIndexSearcher {
         return 0;
       }
 
-      default ByteBuffer queries() { // direct, one nrtgpu_query (has_after / after_doc of the FieldDoc)
+      default ByteBuffer queries() { // direct, one nrtgpu_query (msm of the root; has_after / after_doc, after_score)
         return null;
       }
 
@@ -176,6 +211,15 @@ public class GpuIndexSearcher extends MyIndexSearcher {
 
       default ByteBuffer limits() { // direct nrtgpu_search_limits, or null
         return null;
+      }
+
+      /** Query trees: nrtgpu_node[numNodes()] referenced by the NODE clauses, or null for a flat query. */
+      default ByteBuffer nodes() {
+        return null;
+      }
+
+      default int numNodes() {
+        return 0;
       }
 
       /** TopFieldDocs from raw FieldDoc values (the compiler knows each field's type). */

@@ -49,6 +49,16 @@ public final class NrtGpu {
       ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits, ByteBuffer outRelation,
       ByteBuffer outHitTimeout, ByteBuffer outTerminatedEarly);
 
+  /**
+   * Query trees (nested BooleanQuery / DisjunctionMaxQuery): nodes = nrtgpu_node[nNodes], referenced by clauses of kind 3
+   * (NODE); otherwise as searchBoolEx, which it is with nNodes == 0.
+   */
+  public static native int searchTree(
+      long index, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer queries, int nq,
+      int topK, int totalHitsThreshold, int flags, ByteBuffer limits, ByteBuffer outDocs, ByteBuffer outScores,
+      ByteBuffer outCounts, ByteBuffer outTotalHits, ByteBuffer outRelation, ByteBuffer outHitTimeout,
+      ByteBuffer outTerminatedEarly);
+
   public static native int searchSorted(
       long index, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK, int flags,
       ByteBuffer sort, ByteBuffer limits, ByteBuffer outDocs, ByteBuffer outSortValues,

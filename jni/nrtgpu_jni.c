@@ -93,6 +93,18 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchBoolEx(
                                          (int64_t*)ADDR(env, outTotalHits), (uint8_t*)ADDR(env, outRelation),
                                          (uint8_t*)ADDR(env, outHitTimeout), (uint8_t*)ADDR(env, outTerminatedEarly)));
 }
+/* nodes: a direct ByteBuffer laid out as nrtgpu_node[] (null with nNodes 0: the search of searchBoolEx) */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTree(
+    JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject queries, jint nq,
+    jint topK, jint totalHitsThreshold, jint flags, jobject limits, jobject outDocs, jobject outScores, jobject outCounts,
+    jobject outTotalHits, jobject outRelation, jobject outHitTimeout, jobject outTerminatedEarly) {
+  return fail(env, nrtgpu_search_tree((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                      (const nrtgpu_node*)ADDR(env, nodes), nNodes, (const nrtgpu_query*)ADDR(env, queries), nq,
+                                      topK, totalHitsThreshold, flags, (const nrtgpu_search_limits*)ADDR(env, limits), NULL,
+                                      (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores), (int32_t*)ADDR(env, outCounts),
+                                      (int64_t*)ADDR(env, outTotalHits), (uint8_t*)ADDR(env, outRelation),
+                                      (uint8_t*)ADDR(env, outHitTimeout), (uint8_t*)ADDR(env, outTerminatedEarly)));
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchSorted(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
     jobject sort, jobject limits, jobject outDocs, jobject outSortValues, jobject outCounts, jobject outTotalHits,

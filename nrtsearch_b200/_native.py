@@ -95,6 +95,12 @@ class Query(C.Structure):
                 ("has_after", C.c_int32), ("after_doc", C.c_int32), ("after_score", C.c_float)]
 
 
+class Node(C.Structure):
+    """nrtgpu_node: a nested BooleanQuery (kind 0) or DisjunctionMaxQuery (kind 1) of a query tree."""
+    _fields_ = [("kind", C.c_int32), ("clause_begin", C.c_int32), ("clause_end", C.c_int32), ("min_should_match", C.c_int32),
+                ("tie_breaker", C.c_float), ("reserved", C.c_int32)]
+
+
 # every symbol include/nrtgpu.h declares (tests/test_abi.py checks the header against this list)
 NRTGPU_SYMBOLS = [
     "nrtgpu_last_error", "nrtgpu_version", "nrtgpu_init", "nrtgpu_shutdown", "nrtgpu_index_build",
@@ -104,6 +110,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_blend_rrf", "nrtgpu_blend_scores", "nrtgpu_rescore_combine", "nrtgpu_knn_last_uncertified", "nrtgpu_packed_words", "nrtgpu_search_sorted", "nrtgpu_search_bool_aggs", "nrtgpu_score_docs", "nrtgpu_rescore_query", "nrtgpu_fetch_columns", "nrtgpu_index_set_live_docs", "nrtgpu_index_update_stats", "nrtgpu_searcher_create", "nrtgpu_searcher_search_bool", "nrtgpu_searcher_close", "nrtgpu_batcher_create", "nrtgpu_batcher_submit", "nrtgpu_batcher_stats", "nrtgpu_batcher_close", "nrtgpu_search_bool_ex", "nrtgpu_search_bool_packed", "nrtgpu_batch_set_limits", "nrtgpu_batch_fetch_ex", "nrtgpu_batch_bind_packed", "nrtgpu_merge_topk_packed",
     "nrtgpu_search_knn_filtered", "nrtgpu_knn_filter_stats",
     "nrtgpu_sort_order_create", "nrtgpu_sort_order_device_bytes", "nrtgpu_sort_order_close", "nrtgpu_search_sorted_fields",
+    "nrtgpu_search_tree", "nrtgpu_batch_prepare_tree",
 ]
 
 _gpu = None
@@ -144,6 +151,12 @@ def gpu_lib() -> C.CDLL:
                                                 C.c_void_p, C.c_void_p]
         lib.nrtgpu_search_bool_ex.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32,
                                               C.c_int32, C.c_int32, C.POINTER(SearchLimits), C.c_void_p] + [C.c_void_p] * 7
+        lib.nrtgpu_search_tree.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32, C.POINTER(Query),
+                                           C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(SearchLimits), C.c_void_p] + \
+                                          [C.c_void_p] * 7
+        lib.nrtgpu_batch_prepare_tree.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32,
+                                                  C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                  C.POINTER(C.c_void_p)]
         lib.nrtgpu_search_bool_packed.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32,
                                                   C.c_int32, C.c_int32, C.POINTER(SearchLimits), C.c_void_p, C.c_void_p]
         lib.nrtgpu_search_sorted.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32,

@@ -22,7 +22,7 @@ void set_error(const std::string& msg);
 #define NRT_FAIL(code, msg) do { ::nrtgpu::set_error(msg); return (code); } while (0)
 
 constexpr int kMaxClauses = 16;     // clauses per flat BooleanQuery on the GPU path
-constexpr int kMaxTermSlots = 8;    // term clauses per query: one tf byte each in the window kernel's 64-bit words
+constexpr int kMaxTermSlots = 8;    // term clauses (tree batches: term leaves) per query: one tf byte each in the window kernel's 64-bit words
 constexpr int kWindowDocs = 16384;  // window engine: W
 constexpr int kSliceWindows = 64;   // window engine: windows per work item
 constexpr int kWideSliceDocs = kSliceWindows * kWindowDocs;   // => 1,048,576 docs per slice of the window engine
@@ -43,10 +43,30 @@ struct DevClause {
   float ub;           // term clauses: largest score of any posting of the list (index-time max of tf*cache[norm])
   int32_t plane;      // term clauses: dense tf plane of the term (DevIndexView::dense_tf), -1 if the term has none
   int32_t gran_row;   // term clauses: row of the index-time granule offset table (DevIndexView::gran_tab), -1 if none
-  int32_t pad_;
+  int32_t node;       // tree batches: the child node of an NRTGPU_NODE clause, the node a leaf belongs to; 0 otherwise
   int64_t lo, hi;
 };
 static_assert(sizeof(DevClause) == 72, "DevClause layout");
+
+// Query trees (nrtgpu_search_tree): a tree batch compiles every query into nodes in pre-order, node 0 being the root
+// BooleanQuery, and lays out the clauses node after node, each node's in their given order. A node's clauses are
+// cl[clause_begin, clause_begin + n_clauses) of its query (relative to DevQuery::clause_begin); child nodes follow their
+// parent, so evaluating the nodes in reverse order sees every child before its parent.
+constexpr int kMaxTreeClauses = 32;   // clauses of one tree, nodes and leaves
+constexpr int kMaxTreeNodes = 9;      // the root and up to 8 nested nodes
+constexpr int kMaxTreeDepth = 4;      // levels of queries, the root included
+
+struct DevNode {
+  int32_t kind;           // NRTGPU_NODE_BOOL / NRTGPU_NODE_DISMAX
+  int32_t clause_begin;   // relative to the query's clause_begin
+  int32_t n_clauses;
+  int32_t n_req;          // BOOL: MUST + FILTER clauses
+  int32_t need_should;    // BOOL: minimum matching SHOULD clauses (DISMAX: 1)
+  int32_t msm;            // BOOL: minimumNumberShouldMatch as given
+  float tie_breaker;      // DISMAX
+  int32_t empty;          // 1: can match nothing
+};
+static_assert(sizeof(DevNode) == 32, "DevNode layout");
 
 struct DevQuery {
   int32_t clause_begin, n_clauses;

@@ -19,7 +19,10 @@
 // slices of a query through one global atomicMax word -- the device analogue of the reference's
 // LazyMaxScoreAccumulator (src/main/java/org/apache/lucene/search/LazyMaxScoreAccumulator.java:21-70),
 // used here only to drop hits that provably cannot enter the top-k (results stay exact).
+// Query trees (tree batches, bool_window_kernel<true>) change pass 2 only: the drivers are the term leaves of the root's
+// cover (batch_plan.inc compile_tree), and a doc is evaluated node by node (eval_node) instead of by one clause list.
 #pragma once
+#include <type_traits>
 #include "query_eval.cuh"
 
 namespace nrtgpu {
@@ -46,18 +49,28 @@ struct BoolLaunch {
   long long deadline_ns;       // 0: no deadline; < 0: already expired
   unsigned long long* clock0;
   int32_t* timed_out;          // [nq]
+  // tree batches (batch_plan.h DevNode): the nodes of query q are nodes[node_begin[q], node_begin[q + 1])
+  const DevNode* nodes;
+  const int32_t* node_begin;
 };
 
-struct BoolSmem {
+template <bool kTree>
+struct BoolSmemT {
   uint64_t slots[kWindowDocs];   // one tf byte per term slot
   uint64_t cand[kCandCap];
   uint32_t bounds[kMaxTermSlots][kSliceWindows + 1];
   float cache[kMaxTermSlots][256];
-  DevClause cl[kMaxClauses];
+  DevClause cl[kTree ? kMaxTreeClauses : kMaxClauses];
   DevQuery q;
   int cand_count;
   int skip;   // the work item started after the deadline
   unsigned long long theta;
+};
+using BoolSmem = BoolSmemT<false>;
+// tree batches: the query's nodes next to its clauses
+struct BoolTreeSmem : BoolSmemT<true> {
+  DevNode nodes[kMaxTreeNodes];
+  int n_nodes;
 };
 
 // bit s set: byte s (term slot s) of a window word is non-zero
@@ -85,9 +98,42 @@ __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolS
   return eval_clauses(ix, sm.q, sm.cl, doc, presence_mask(slot), term, out_score);
 }
 
+// the query tree of sm on one candidate doc: the nodes bottom-up (reverse pre-order: children before parents), no recursion
+__device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolTreeSmem& sm, int32_t doc, uint64_t slot,
+                                             float* out_score) {
+  const uint32_t mask = presence_mask(slot);
+  if ((mask & sm.q.req_term_mask) != sm.q.req_term_mask) return false;
+  if (mask & sm.q.not_term_mask) return false;
+  if (ix.live_bits && !((ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
+  auto term = [&](const DevClause& c, float* s) {
+    const uint32_t b = (uint32_t)((slot >> (8 * c.slot)) & 0xff);
+    if (b == 0) return false;
+    if (c.scoring) {
+      const float f = (b == 255u) ? exact_freq_slow(ix, c, doc) : (float)b;
+      const uint8_t* nrm = ix.norms[c.field];
+      const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
+      *s = bm25_score(c.weight, f, sm.cache[c.slot][nb]);
+    }
+    return true;
+  };
+  uint32_t matched = 0;
+  float node_score[kMaxTreeNodes];
+  for (int n = sm.n_nodes - 1; n >= 0; --n) {
+    const DevNode& nd = sm.nodes[n];
+    float s;
+    if (!nd.empty && eval_node(ix, nd, sm.cl, doc, matched, node_score, term, &s)) { matched |= 1u << n; node_score[n] = s; }
+  }
+  if (!(matched & 1u)) return false;
+  *out_score = node_score[0];
+  return true;
+}
+
+// kTree: a tree batch (sm holds the query's nodes, evaluate_doc walks them); otherwise flat BooleanQuerys
+template <bool kTree>
 __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_constant__ BoolLaunch L) {
+  using Smem = typename std::conditional<kTree, BoolTreeSmem, BoolSmem>::type;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  BoolSmem& sm = *reinterpret_cast<BoolSmem*>(smem_raw);
+  Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
   const int tid = threadIdx.x;
   const int lane = tid & 31;
 
@@ -101,11 +147,13 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
       sm.theta = *(volatile unsigned long long*)&L.theta[qi];
       sm.skip = L.deadline_ns && deadline_passed(L.deadline_ns, L.clock0);
       if (sm.skip) L.timed_out[qi] = 1;
+      if constexpr (kTree) sm.n_nodes = L.node_begin[qi + 1] - L.node_begin[qi];
     }
     __syncthreads();
     if (sm.skip) continue;   // (CTA-uniform) slice_cnt stays 0: the slice contributes no keys
     const int ncl = sm.q.n_clauses;
     if (tid < ncl) sm.cl[tid] = L.clauses[sm.q.clause_begin + tid];
+    if constexpr (kTree) if (tid < sm.n_nodes) sm.nodes[tid] = L.nodes[L.node_begin[qi] + tid];
     for (int i = tid; i < kWindowDocs; i += kThreads) sm.slots[i] = 0;
     __syncthreads();
     // per-slot BM25 caches

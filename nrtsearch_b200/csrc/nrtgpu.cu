@@ -256,6 +256,8 @@ struct nrtgpu_batch {
   DevBuf<unsigned long long> probe_stats;
   DevBuf<DevClause> clauses;
   DevBuf<DevQuery> queries;
+  DevBuf<DevNode> nodes;          // tree batches: cb.nodes
+  DevBuf<int32_t> node_begin;     // tree batches: cb.node_begin
   DevBuf<int32_t> work_query, work_slice;
   DevBuf<int32_t> pruned;    // [nq] relation GTE flags
   DevBuf<int32_t> terminated; // [nq] terminateAfter cut the query short
@@ -360,7 +362,8 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   { const char* e = getenv("NRTGPU_ITEM_POSTINGS"); if (e && atoll(e) > 0) c->plan.item_postings = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE"); if (e && atoll(e) > 0) c->plan.item_share = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE_FULL"); if (e && atoll(e) > 0) c->plan.item_share_full = atoll(e); }
-  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
 #define NRT_PROBE_ATTR(S, D) \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasA, v3::kStageA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageA>))); \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasB, v3::kStageB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageB>)));
@@ -666,6 +669,10 @@ static int batch_compile(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& 
   NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
   b->ix = ix; b->nq = r.nq; b->top_k = r.top_k;
   if ((rc = b->clauses.upload_async(b->cb.clauses.data(), b->cb.clauses.size(), st))) return rc;
+  if (b->cb.tree) {
+    if ((rc = b->nodes.upload_async(b->cb.nodes.data(), b->cb.nodes.size(), st))) return rc;
+    if ((rc = b->node_begin.upload_async(b->cb.node_begin.data(), b->cb.node_begin.size(), st))) return rc;
+  }
   return b->queries.upload_async(b->cb.queries.data(), b->cb.queries.size(), st);
 }
 
@@ -767,6 +774,23 @@ int nrtgpu_batch_prepare(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
   return NRTGPU_OK;
 }
 
+static BatchRequest tree_request(const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes, int32_t n_nodes,
+                                 const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags);
+
+int nrtgpu_batch_prepare_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                              int32_t n_nodes, const nrtgpu_query* queries, int32_t nq, int32_t top_k,
+                              int32_t total_hits_threshold, int32_t flags, nrtgpu_batch** out) {
+  if (!out) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: NULL argument");
+  if (n_nodes < 0 || (n_nodes > 0 && !nodes)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_tree: bad nodes");
+  std::unique_ptr<nrtgpu_batch> b(new nrtgpu_batch);
+  int rc = batch_build(b.get(), ix, tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags),
+                       (cudaStream_t)0);
+  if (rc) return rc;
+  NRT_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)0));
+  *out = b.release();
+  return NRTGPU_OK;
+}
+
 int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   if (!b) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_run: NULL batch");
   cudaStream_t st = (cudaStream_t)stream_;
@@ -801,6 +825,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   if (b->plan.n_work() > 0) {
     BoolLaunch L;
     L.ix = b->ix->view();
+    L.nodes = nullptr; L.node_begin = nullptr;
     L.clauses = b->clauses.p; L.queries = b->queries.p;
     L.work_query = b->work_query.p; L.work_slice = b->work_slice.p;
     L.n_work = b->plan.n_work(); L.n_slices = b->plan.n_lists; L.top_k = b->top_k;
@@ -877,8 +902,11 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         }
         NRT_CUDA_TRY(cudaGetLastError());
       }
+    } else if (b->cb.tree) {
+      L.nodes = b->nodes.p; L.node_begin = b->node_begin.p;
+      bool_window_kernel<true><<<b->plan.n_work(), kThreads, sizeof(BoolTreeSmem), st>>>(L);
     } else
-      bool_window_kernel<<<b->plan.n_work(), kThreads, sizeof(BoolSmem), st>>>(L);
+      bool_window_kernel<false><<<b->plan.n_work(), kThreads, sizeof(BoolSmem), st>>>(L);
     NRT_CUDA_TRY(cudaGetLastError());
   }
   NRT_CUDA_TRY(cudaEventRecord(ev[1], st));
@@ -1197,6 +1225,24 @@ int nrtgpu_search_bool_ex(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_
   SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
   o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early;
   return search_bool_impl(ix, BatchRequest{clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags}, limits, stream, o);
+}
+
+// a request of the tree entry points; without nodes it is the flat request of nrtgpu_search_bool_ex
+static BatchRequest tree_request(const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes, int32_t n_nodes,
+                                 const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags) {
+  BatchRequest r{clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags};
+  if (n_nodes > 0) { r.nodes = nodes; r.n_nodes = n_nodes; }
+  return r;
+}
+
+int nrtgpu_search_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes, int32_t n_nodes,
+                       const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags,
+                       const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
+                       int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout, uint8_t* out_terminated_early) {
+  if (n_nodes < 0 || (n_nodes > 0 && !nodes)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_tree: bad nodes");
+  SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
+  o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early;
+  return search_bool_impl(ix, tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags), limits, stream, o);
 }
 
 int nrtgpu_search_sorted(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,

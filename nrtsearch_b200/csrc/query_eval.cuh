@@ -126,4 +126,66 @@ __device__ __forceinline__ bool eval_clauses(const DevIndexView& ix, const DevQu
   return true;
 }
 
+// One node of a query tree (tree batches of the window engine) on one doc, its child nodes already evaluated: node_match
+// bit n is set iff node n matched, node_score[n] is then the float its Scorer returned. The clauses are walked in order.
+//   BOOL:   eval_clauses's rule, a child node counting as a clause that is present when it matched and scores its float;
+//   DISMAX: matches if any disjunct does; DisjunctionMaxScorer's float max and double sum of the others, streamed in clause
+//           order as Lucene 10 streams its disjuncts (a new max moves the old one into the sum), scored
+//           (float)((double)max + others * (double)tie_breaker).
+// term(c, &s) as for eval_clauses. Liveness is the caller's.
+template <class TermScore>
+__device__ __forceinline__ bool eval_node(const DevIndexView& ix, const DevNode& nd, const DevClause* cl, int32_t doc,
+                                          uint32_t node_match, const float* node_score, TermScore term, float* out_score) {
+  double must_sum = 0.0, should_sum = 0.0;
+  float max_s = 0.0f;
+  int n_should = 0;
+  for (int i = 0; i < nd.n_clauses; ++i) {
+    const DevClause& c = cl[nd.clause_begin + i];
+    bool present;
+    float s = 0.0f;
+    if (c.kind == NRTGPU_TERM) {
+      present = term(c, &s);
+    } else if (c.kind == NRTGPU_RANGE_I64) {
+      present = range_matches(ix, c.col, doc, c.lo, c.hi);
+      s = c.weight;
+    } else if (c.kind == NRTGPU_NODE) {
+      present = (node_match >> c.node) & 1u;
+      if (present) s = node_score[c.node];
+    } else {
+      present = true;
+      s = c.weight;
+    }
+    if (!present) {
+      if (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER) return false;
+      continue;
+    }
+    switch (c.occur) {
+      case NRTGPU_MUST: must_sum += (double)s; break;
+      case NRTGPU_FILTER: break;
+      case NRTGPU_SHOULD:
+        if (nd.kind == NRTGPU_NODE_DISMAX) {
+          if (s >= max_s) { should_sum += (double)max_s; max_s = s; }
+          else should_sum += (double)s;
+        } else should_sum += (double)s;
+        ++n_should;
+        break;
+      default: return false;   // MUST_NOT present
+    }
+  }
+  if (n_should < nd.need_should) return false;
+  float score;
+  if (nd.kind == NRTGPU_NODE_DISMAX) score = (float)((double)max_s + should_sum * (double)nd.tie_breaker);
+  else if (nd.n_req == 0) score = (float)should_sum;
+  else {
+    const float req = (float)must_sum;
+    if (n_should == 0) score = req;
+    else {
+      const float opt = (float)should_sum;
+      score = (nd.msm > 0) ? (float)((double)req + (double)opt) : __fadd_rn(req, opt);
+    }
+  }
+  *out_score = score;
+  return true;
+}
+
 }  // namespace nrtgpu

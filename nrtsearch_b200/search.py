@@ -62,6 +62,14 @@ class BoostQuery:
     boost: float
 
 
+@dataclass
+class DisjunctionMaxQuery:
+    """DisjunctionMaxQuery(disjuncts, tieBreakerMultiplier): what multi_match BEST_FIELDS maps to (QueryNodeMapper.java:429-497).
+    A doc matches if any disjunct does and scores max + tie_breaker * (the other matching disjuncts' scores)."""
+    disjuncts: List[object] = field(default_factory=list)
+    tie_breaker: float = 0.0
+
+
 @dataclass(frozen=True)
 class BooleanClause:
     query: object
@@ -298,6 +306,73 @@ def compile_queries(queries: Sequence[object], search_after: Optional[Sequence[O
     return carr, len(flat), qarr, len(qs)
 
 
+def _unboost(q, boost: np.float32):
+    """(the query under any BoostQuerys, the boost folded outermost first in float)"""
+    while isinstance(q, BoostQuery):
+        if q.boost < 0:
+            raise ValueError("Boost must be a positive number")
+        boost = _f32(boost * _f32(q.boost))
+        q = q.query
+    return q, boost
+
+
+def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Optional[ScoreDoc]]] = None):
+    """Query trees -> (Clause[], n_clauses, Node[], n_nodes, Query[], nq) for nrtgpu_search_tree. The root of a query is a
+    BooleanQuery (a bare leaf or DisjunctionMaxQuery becomes its single MUST clause); every BooleanQuery or
+    DisjunctionMaxQuery below it is a node, numbered in pre-order over the batch, whose clauses are one range of the clause
+    array. BoostQuery boosts are folded through the nodes into the leaves, outermost first in float, so node clauses carry
+    boost 1 (BoostQuery.createWeight passes boost * this.boost down)."""
+    flat, nodes, qs = [], [], []
+
+    def parts(q):
+        if isinstance(q, BooleanQuery):
+            return 0, [(c.query, c.occur) for c in q.clauses], q.minimum_number_should_match, 0.0
+        return 1, [(d, Occur.SHOULD) for d in q.disjuncts], 0, float(q.tie_breaker)
+
+    for i, q in enumerate(queries):
+        q, boost = _unboost(q, _f32(1.0))
+        if isinstance(q, BooleanQuery):
+            root = (0, [(c.query, c.occur) for c in q.clauses], q.minimum_number_should_match, 0.0)
+        else:
+            root = (0, [(q, Occur.MUST)], 0, 0.0)
+        order = []   # pre-order: [kind, [(leaf, boost, occur) | (node position, None, occur)], msm, tie]
+
+        def visit(kind, cls, msm, tie, b):
+            pos = len(order)
+            order.append(None)
+            children = []
+            for sub, occ in cls:
+                s, sb = _unboost(sub, b)
+                if isinstance(s, (BooleanQuery, DisjunctionMaxQuery)):
+                    children.append((visit(*parts(s), sb), None, occ))
+                else:
+                    children.append((s, sb, occ))
+            order[pos] = (kind, children, msm, tie)
+            return pos
+
+        visit(*root, boost)
+        base = len(nodes) - 1   # node id of pre-order position p > 0: base + p
+        begin_end = []
+        for kind, children, msm, tie in order:
+            begin = len(flat)
+            for sub, sb, occ in children:
+                if sb is None:
+                    flat.append((int(occ), 3, base + sub, 1.0, 0, 0))
+                else:
+                    _flatten(sub, sb, flat, occ)
+            begin_end.append((begin, len(flat)))
+        for p in range(1, len(order)):
+            kind, _, msm, tie = order[p]
+            nodes.append((kind, begin_end[p][0], begin_end[p][1], msm, tie, 0))
+        after = search_after[i] if search_after is not None else None
+        qs.append((begin_end[0][0], begin_end[0][1], root[2], 1 if after is not None else 0,
+                   after.doc if after is not None else 0, after.score if after is not None else 0.0))
+    carr = (Clause * max(len(flat), 1))(*[Clause(*c) for c in flat])
+    narr = (_native.Node * max(len(nodes), 1))(*[_native.Node(*n) for n in nodes])
+    qarr = (CQuery * max(len(qs), 1))(*[CQuery(*t) for t in qs])
+    return carr, len(flat), narr, len(nodes), qarr, len(qs)
+
+
 def compile_filters(filter_queries: Sequence[Optional[object]], nq: int):
     """Per-query kNN filter queries (KnnQuery.filter; None = no filter) -> (Clause[], n_clauses, Query[], n_filters,
     filter_of int32[nq]) for nrtgpu_search_knn_filtered. Filters that compile to the same flat BooleanQuery, boosts aside
@@ -406,11 +481,16 @@ class BatchResult:
 class PreparedBatch:
     """nrtgpu_batch: compiled batch resident on the device (launch many times, inputs stay in HBM)."""
 
-    def __init__(self, index: GpuIndex, carr, ncl, qarr, nq, top_k, threshold, flags=0):
+    def __init__(self, index: GpuIndex, carr, ncl, qarr, nq, top_k, threshold, flags=0, nodes=None):
+        """nodes: (Node[], n_nodes) of a query-tree batch (nrtgpu_batch_prepare_tree), None for flat queries."""
         self._lib = _native.gpu_lib()
         self.index, self.nq, self.top_k = index, nq, top_k
         h = C.c_void_p()
-        check(self._lib.nrtgpu_batch_prepare(index.handle, carr, ncl, qarr, nq, top_k, threshold, flags, C.byref(h)))
+        if nodes is None:
+            check(self._lib.nrtgpu_batch_prepare(index.handle, carr, ncl, qarr, nq, top_k, threshold, flags, C.byref(h)))
+        else:
+            check(self._lib.nrtgpu_batch_prepare_tree(index.handle, carr, ncl, nodes[0], nodes[1], qarr, nq, top_k, threshold, flags,
+                                                      C.byref(h)))
         self.handle = h
 
     def run(self, stream: int = 0):
@@ -487,6 +567,33 @@ class GpuIndexSearcher:
                                               out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data,
                                               out.relation.ctypes.data, out.hit_timeout.ctypes.data,
                                               out.terminated_early.ctypes.data))
+        return out
+
+    def prepare_tree(self, queries: Sequence[object], collector: RelevanceCollector,
+                     search_after: Optional[Sequence[Optional[ScoreDoc]]] = None, flags: int = 0) -> PreparedBatch:
+        """prepare() for queries that may nest BooleanQuery and DisjunctionMaxQuery (nrtgpu_batch_prepare_tree)."""
+        if search_after is None and collector.search_after is not None:
+            search_after = [collector.search_after] * len(queries)
+        carr, ncl, narr, nn, qarr, nq = compile_tree(queries, search_after)
+        return PreparedBatch(self.index, carr, ncl, qarr, nq, collector.num_hits_to_collect, collector.total_hits_threshold, flags,
+                             nodes=(narr, nn))
+
+    def search_tree(self, queries: Sequence[object], collector: RelevanceCollector,
+                    search_after: Optional[Sequence[Optional[ScoreDoc]]] = None, stream: int = 0) -> BatchResult:
+        """search_batch() for queries that may nest BooleanQuery and DisjunctionMaxQuery (nrtgpu_search_tree): a batch with a
+        nested query runs on the window engine."""
+        if search_after is None and collector.search_after is not None:
+            search_after = [collector.search_after] * len(queries)
+        carr, ncl, narr, nn, qarr, nq = compile_tree(queries, search_after)
+        k = collector.num_hits_to_collect
+        out = BatchResult(np.zeros((nq, max(k, 1)), np.int32), np.zeros((nq, max(k, 1)), np.float32),
+                          np.zeros(nq, np.int32), np.zeros(nq, np.int64), np.zeros(nq, np.uint8),
+                          np.zeros(nq, np.uint8), np.zeros(nq, np.uint8))
+        lim = collector.limits()
+        check(self._lib.nrtgpu_search_tree(self.index.handle, carr, ncl, narr, nn, qarr, nq, k, collector.total_hits_threshold, 0,
+                                           None if lim is None else C.byref(lim), C.c_void_p(stream), out.docs.ctypes.data,
+                                           out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data,
+                                           out.relation.ctypes.data, out.hit_timeout.ctypes.data, out.terminated_early.ctypes.data))
         return out
 
     def knn_query(self, queries: np.ndarray, knn: KnnQuery, sim: int, boosts: Optional[np.ndarray] = None,
