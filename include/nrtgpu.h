@@ -210,6 +210,54 @@ int nrtgpu_batch_prepare_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, in
                               int32_t n_nodes, const nrtgpu_query* queries, int32_t nq, int32_t top_k,
                               int32_t total_hits_threshold, int32_t flags, nrtgpu_batch** out);
 
+/* Term positions of an image (PostingsEnum.nextPosition() with PostingsEnum.POSITIONS): positions[] holds, posting after
+ * posting in the CSR order of the build, the freq positions of that posting, ascending (equal positions are allowed);
+ * n_positions must be the sum of the build's freqs. A second call replaces the positions. They stay valid across
+ * nrtgpu_index_set_live_docs and nrtgpu_index_update_stats, and nrtgpu_index_device_bytes counts them (4 B per position,
+ * 4 B per posting and 8 B per term). NRTGPU_ERR_INVALID: a wrong count, a negative position, positions that descend
+ * within a posting. */
+int nrtgpu_index_add_positions(nrtgpu_index* ix, const int32_t* positions, int64_t n_positions);
+
+/* Phrase leaves of query trees (PhraseQuery / match_phrase, reference QueryNodeMapper.java:285-291, :397-427). A clause of
+ * kind NRTGPU_PHRASE is a leaf whose id indexes phrases[]; its boost is the leaf's folded boost, as for a term leaf. The
+ * phrase's terms are phrase_terms[term_begin:term_end] with their PhraseQuery positions (PhraseQuery.getTerms() /
+ * getPositions()); slop is PhraseQuery.getSlop(). Lucene 10 PhraseWeight semantics:
+ *   weight:  boost * idf, idf = (float) of the double sum of every term's float idf, a repeated term counted each time
+ *            (BM25Similarity.idfExplain over the term statistics); score = BM25(weight, freq, norm of the phrase's field);
+ *   slop 0:  ExactPhraseMatcher. The lead is the term of the smallest position (the first one given on a tie); freq is the
+ *            number of the lead's positions p in the doc (each occurrence counted) at which every other term i has a
+ *            position p - position_lead + position_i. Overlapping occurrences count ("a a" in "a a a" has freq 2);
+ *   slop>0:  SloppyPhraseMatcher without repeats: a queue of (doc position - query position, query position, ordinal) per
+ *            term, the running end and the match-length minimisation; every match of matchLength <= slop adds
+ *            1.0f / (1.0f + matchLength) to freq, in float, in the matcher's order;
+ *   a phrase of no terms matches nothing, one of one term is that term's leaf (Lucene's rewrite). Under FILTER and
+ *   MUST_NOT a phrase only has to match. Phrase terms take term slots: a tree holds at most 8 term leaves and phrase
+ *   terms together. Phrases run on the window engine only.
+ *   NRTGPU_ERR_INVALID:     a phrase id or phrase term id out of range, a term range out of bounds, terms of different
+ *                           fields, negative or descending positions, slop < 0, an image without positions
+ *                           (nrtgpu_index_add_positions: "field was indexed without position data"), every check of
+ *                           nrtgpu_search_tree;
+ *   NRTGPU_ERR_UNSUPPORTED: more than 8 term slots in one tree, a sloppy phrase with a repeated term (Lucene's repeat
+ *                           groups), every limit of nrtgpu_search_tree.
+ * With n_phrases == 0 these are nrtgpu_search_tree / nrtgpu_batch_prepare_tree. A batch holding a phrase is a tree batch
+ * even without nodes (a bare PhraseQuery is a root with one MUST phrase clause). Every other entry point rejects
+ * NRTGPU_PHRASE clauses as a bad clause kind. */
+enum { NRTGPU_PHRASE = 4 };
+typedef struct { int32_t term_begin, term_end; int32_t slop; int32_t reserved; } nrtgpu_phrase;
+typedef struct { int32_t term; int32_t position; } nrtgpu_phrase_term;
+int nrtgpu_search_tree_phrases(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                               int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                               const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                               int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags,
+                               const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs, float* out_scores,
+                               int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
+                               uint8_t* out_terminated_early);
+int nrtgpu_batch_prepare_tree_phrases(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                      const nrtgpu_node* nodes, int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                                      const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms,
+                                      const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold,
+                                      int32_t flags, nrtgpu_batch** out);
+
 /* same search with HOST query buffers, results left on the DEVICE in one packed record (see nrtgpu_packed_words): the
  * multi-GPU request path (the caller all-gathers the record on `stream`, then nrtgpu_merge_topk_packed). Synchronises. */
 int nrtgpu_search_bool_packed(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,

@@ -15,9 +15,10 @@ import org.apache.lucene.search.TotalHits;
  * Reference-side adaptor (not built in the authoring image: no JDK / Lucene jars there). A MyIndexSearcher subclass
  * created at ShardState.ShardSearcherFactory.newSearcher (ShardState.java:506-526). search() pattern-matches the
  * rewritten Query (flat BooleanQuery of TermQuery / IndexOrDocValuesQuery range / MatchAllDocsQuery, optional
- * BoostQuery wrappers; or a tree of nested BooleanQuery / DisjunctionMaxQuery nodes over those leaves) and the
- * RelevanceCollector configuration. A compiled request that carries nodes calls nrtgpu_search_tree directly on the
- * handler thread. Any other supported request is handed to the NATIVE
+ * BoostQuery wrappers; or a tree of nested BooleanQuery / DisjunctionMaxQuery nodes over those leaves and PhraseQuery
+ * leaves) and the RelevanceCollector configuration. A compiled request that carries nodes or phrases calls
+ * nrtgpu_search_tree / nrtgpu_search_tree_phrases directly on the handler thread (MultiPhraseQuery and phrase-prefix
+ * queries are not compiled: Lucene). Any other supported request is handed to the NATIVE
  * micro-batcher (nrtgpu_batcher_submit): the gRPC handler thread blocks while a worker thread inside libnrtgpu groups
  * the waiting requests into one batched search. Everything else, and NRTGPU_ERR_UNSUPPORTED
  * (UnsupportedOperationException), falls through to super.search(), i.e. Lucene. The image and its batcher are released
@@ -55,7 +56,7 @@ public class GpuIndexSearcher extends MyIndexSearcher {
       T sorted = searchSortedFields(c);
       return sorted != null ? sorted : super.search(query, collectorManager);
     }
-    if (c.numNodes() > 0) {
+    if (c.numNodes() > 0 || c.numPhrases() > 0) {
       T tree = searchTree(c);
       return tree != null ? tree : super.search(query, collectorManager);
     }
@@ -135,8 +136,9 @@ public class GpuIndexSearcher extends MyIndexSearcher {
   }
 
   /**
-   * A query tree (nested BooleanQuery / DisjunctionMaxQuery; the micro-batcher takes flat queries only): one
-   * nrtgpu_search_tree call for this request. null = UNSUPPORTED (past the tree limits): Lucene.
+   * A query tree (nested BooleanQuery / DisjunctionMaxQuery, PhraseQuery leaves; the micro-batcher takes flat queries
+   * only): one nrtgpu_search_tree(_phrases) call for this request. null = UNSUPPORTED (past the tree limits, a sloppy
+   * phrase with a repeated term): Lucene.
    */
   private <T> T searchTree(GpuQueryCompiler.Compiled c) {
     int k = c.topK();
@@ -144,9 +146,16 @@ public class GpuIndexSearcher extends MyIndexSearcher {
     ByteBuffer relation = direct(1), hitTimeout = direct(1), terminated = direct(1);
     long t0 = System.nanoTime();
     try {
-      NrtGpu.searchTree(
-          gpuIndex, c.clauses(), c.numClauses(), c.nodes(), c.numNodes(), c.queries(), 1, k, c.totalHitsThreshold(), 0,
-          c.limits(), docs, scores, count, total, relation, hitTimeout, terminated);
+      if (c.numPhrases() > 0) {
+        NrtGpu.searchTreePhrases(
+            gpuIndex, c.clauses(), c.numClauses(), c.nodes(), c.numNodes(), c.phrases(), c.numPhrases(), c.phraseTerms(),
+            c.numPhraseTerms(), c.queries(), 1, k, c.totalHitsThreshold(), 0, c.limits(), docs, scores, count, total,
+            relation, hitTimeout, terminated);
+      } else {
+        NrtGpu.searchTree(
+            gpuIndex, c.clauses(), c.numClauses(), c.nodes(), c.numNodes(), c.queries(), 1, k, c.totalHitsThreshold(), 0,
+            c.limits(), docs, scores, count, total, relation, hitTimeout, terminated);
+      }
     } catch (UnsupportedOperationException e) {
       return null;
     }
@@ -169,6 +178,36 @@ public class GpuIndexSearcher extends MyIndexSearcher {
     }
     NrtGpu.batcherClose(batcher);
     NrtGpu.indexClose(gpuIndex);
+  }
+
+  /**
+   * Appends a Lucene PhraseQuery as one nrtgpu_phrase record (into phrases) and its nrtgpu_phrase_term records (into
+   * phraseTerms, starting at record index firstTerm): PhraseQuery.getTerms() mapped through termId, getPositions() and
+   * getSlop() as they are. Returns the phrase's index for the PHRASE clause's id, or -1 when a term is not in the
+   * dictionary (the compiler then emits a phrase of no terms: it matches nothing, as in Lucene).
+   */
+  public static int appendPhrase(
+      org.apache.lucene.search.PhraseQuery q,
+      java.util.function.ToIntFunction<org.apache.lucene.index.Term> termId,
+      ByteBuffer phrases,
+      int phraseIndex,
+      ByteBuffer phraseTerms,
+      int firstTerm) {
+    org.apache.lucene.index.Term[] terms = q.getTerms();
+    int[] positions = q.getPositions();
+    for (int i = 0; i < terms.length; ++i) {
+      int id = termId.applyAsInt(terms[i]);
+      if (id < 0) {
+        return -1;
+      }
+      phraseTerms.putInt(8 * (firstTerm + i), id).putInt(8 * (firstTerm + i) + 4, positions[i]);
+    }
+    phrases
+        .putInt(16 * phraseIndex, firstTerm)
+        .putInt(16 * phraseIndex + 4, firstTerm + terms.length)
+        .putInt(16 * phraseIndex + 8, q.getSlop())
+        .putInt(16 * phraseIndex + 12, 0);
+    return phraseIndex;
   }
 
   private static ByteBuffer direct(int bytes) {
@@ -219,6 +258,26 @@ public class GpuIndexSearcher extends MyIndexSearcher {
       }
 
       default int numNodes() {
+        return 0;
+      }
+
+      /**
+       * PhraseQuery leaves (clauses of kind 4): nrtgpu_phrase[numPhrases()] and nrtgpu_phrase_term[numPhraseTerms()]
+       * (see appendPhrase), or null for a request without phrases.
+       */
+      default ByteBuffer phrases() {
+        return null;
+      }
+
+      default int numPhrases() {
+        return 0;
+      }
+
+      default ByteBuffer phraseTerms() {
+        return null;
+      }
+
+      default int numPhraseTerms() {
         return 0;
       }
 

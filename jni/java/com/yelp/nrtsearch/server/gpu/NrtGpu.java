@@ -59,6 +59,23 @@ public final class NrtGpu {
       ByteBuffer outCounts, ByteBuffer outTotalHits, ByteBuffer outRelation, ByteBuffer outHitTimeout,
       ByteBuffer outTerminatedEarly);
 
+  /**
+   * Term positions of the image: positions = nPositions int32, posting after posting in the build's CSR order, the freq
+   * positions of each posting ascending (PostingsEnum.nextPosition() with PostingsEnum.POSITIONS).
+   */
+  public static native int addPositions(long index, ByteBuffer positions, long nPositions);
+
+  /**
+   * Query trees with PhraseQuery leaves: phrases = nrtgpu_phrase[nPhrases] referenced by clauses of kind 4 (PHRASE),
+   * phraseTerms = nrtgpu_phrase_term[nPhraseTerms] (term id, PhraseQuery position); otherwise as searchTree, which it is
+   * with nPhrases == 0.
+   */
+  public static native int searchTreePhrases(
+      long index, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer phrases, int nPhrases,
+      ByteBuffer phraseTerms, int nPhraseTerms, ByteBuffer queries, int nq, int topK, int totalHitsThreshold, int flags,
+      ByteBuffer limits, ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits,
+      ByteBuffer outRelation, ByteBuffer outHitTimeout, ByteBuffer outTerminatedEarly);
+
   public static native int searchSorted(
       long index, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK, int flags,
       ByteBuffer sort, ByteBuffer limits, ByteBuffer outDocs, ByteBuffer outSortValues,

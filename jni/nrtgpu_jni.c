@@ -105,6 +105,27 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTree(
                                       (int64_t*)ADDR(env, outTotalHits), (uint8_t*)ADDR(env, outRelation),
                                       (uint8_t*)ADDR(env, outHitTimeout), (uint8_t*)ADDR(env, outTerminatedEarly)));
 }
+/* positions: a direct ByteBuffer of int32 positions, posting after posting (PostingsEnum.nextPosition()) */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_addPositions(JNIEnv* env, jclass c, jlong ix, jobject positions,
+                                                                               jlong nPositions) {
+  return fail(env, nrtgpu_index_add_positions((nrtgpu_index*)(intptr_t)ix, (const int32_t*)ADDR(env, positions), nPositions));
+}
+/* phrases / phraseTerms: direct ByteBuffers laid out as nrtgpu_phrase[] / nrtgpu_phrase_term[] (nPhrases 0: searchTree) */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTreePhrases(
+    JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,
+    jobject phraseTerms, jint nPhraseTerms, jobject queries, jint nq, jint topK, jint totalHitsThreshold, jint flags,
+    jobject limits, jobject outDocs, jobject outScores, jobject outCounts, jobject outTotalHits, jobject outRelation,
+    jobject outHitTimeout, jobject outTerminatedEarly) {
+  return fail(env, nrtgpu_search_tree_phrases((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                              (const nrtgpu_node*)ADDR(env, nodes), nNodes,
+                                              (const nrtgpu_phrase*)ADDR(env, phrases), nPhrases,
+                                              (const nrtgpu_phrase_term*)ADDR(env, phraseTerms), nPhraseTerms,
+                                              (const nrtgpu_query*)ADDR(env, queries), nq, topK, totalHitsThreshold, flags,
+                                              (const nrtgpu_search_limits*)ADDR(env, limits), NULL, (int32_t*)ADDR(env, outDocs),
+                                              (float*)ADDR(env, outScores), (int32_t*)ADDR(env, outCounts),
+                                              (int64_t*)ADDR(env, outTotalHits), (uint8_t*)ADDR(env, outRelation),
+                                              (uint8_t*)ADDR(env, outHitTimeout), (uint8_t*)ADDR(env, outTerminatedEarly)));
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchSorted(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
     jobject sort, jobject limits, jobject outDocs, jobject outSortValues, jobject outCounts, jobject outTotalHits,

@@ -101,6 +101,16 @@ class Node(C.Structure):
                 ("tie_breaker", C.c_float), ("reserved", C.c_int32)]
 
 
+class Phrase(C.Structure):
+    """nrtgpu_phrase: a PhraseQuery leaf of a query tree, its terms phrase_terms[term_begin:term_end]."""
+    _fields_ = [("term_begin", C.c_int32), ("term_end", C.c_int32), ("slop", C.c_int32), ("reserved", C.c_int32)]
+
+
+class PhraseTerm(C.Structure):
+    """nrtgpu_phrase_term: a term of a phrase and its PhraseQuery position."""
+    _fields_ = [("term", C.c_int32), ("position", C.c_int32)]
+
+
 # every symbol include/nrtgpu.h declares (tests/test_abi.py checks the header against this list)
 NRTGPU_SYMBOLS = [
     "nrtgpu_last_error", "nrtgpu_version", "nrtgpu_init", "nrtgpu_shutdown", "nrtgpu_index_build",
@@ -111,6 +121,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_search_knn_filtered", "nrtgpu_knn_filter_stats",
     "nrtgpu_sort_order_create", "nrtgpu_sort_order_device_bytes", "nrtgpu_sort_order_close", "nrtgpu_search_sorted_fields",
     "nrtgpu_search_tree", "nrtgpu_batch_prepare_tree",
+    "nrtgpu_index_add_positions", "nrtgpu_search_tree_phrases", "nrtgpu_batch_prepare_tree_phrases",
 ]
 
 _gpu = None
@@ -157,6 +168,15 @@ def gpu_lib() -> C.CDLL:
         lib.nrtgpu_batch_prepare_tree.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32,
                                                   C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                   C.POINTER(C.c_void_p)]
+        lib.nrtgpu_index_add_positions.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+        lib.nrtgpu_search_tree_phrases.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32,
+                                                   C.POINTER(Phrase), C.c_int32, C.POINTER(PhraseTerm), C.c_int32, C.POINTER(Query),
+                                                   C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(SearchLimits), C.c_void_p] + \
+                                                  [C.c_void_p] * 7
+        lib.nrtgpu_batch_prepare_tree_phrases.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32,
+                                                          C.POINTER(Phrase), C.c_int32, C.POINTER(PhraseTerm), C.c_int32,
+                                                          C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                          C.POINTER(C.c_void_p)]
         lib.nrtgpu_search_bool_packed.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32,
                                                   C.c_int32, C.c_int32, C.POINTER(SearchLimits), C.c_void_p, C.c_void_p]
         lib.nrtgpu_search_sorted.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32,

@@ -44,6 +44,7 @@ struct DevClause {
   int32_t plane;      // term clauses: dense tf plane of the term (DevIndexView::dense_tf), -1 if the term has none
   int32_t gran_row;   // term clauses: row of the index-time granule offset table (DevIndexView::gran_tab), -1 if none
   int32_t node;       // tree batches: the child node of an NRTGPU_NODE clause, the node a leaf belongs to; 0 otherwise
+                      // (col: the term id of a phrase term clause, the record of an NRTGPU_PHRASE clause)
   int64_t lo, hi;
 };
 static_assert(sizeof(DevClause) == 72, "DevClause layout");
@@ -67,6 +68,24 @@ struct DevNode {
   int32_t empty;          // 1: can match nothing
 };
 static_assert(sizeof(DevNode) == 32, "DevNode layout");
+
+// Phrase leaves of tree batches (nrtgpu_search_tree_phrases). Each phrase term is a presence-only term clause of its own
+// slot (scoring 0, col = its term id, which indexes the image's positions), laid out after every node's clauses so that
+// no node walks it; the NRTGPU_PHRASE clause holds the phrase's record index in col (relative to the query's first
+// record, -1: a phrase of no terms, which matches nothing), its field and its weight. A phrase has at least two terms
+// (one term is compiled as that term's leaf), so a tree of 8 term slots holds at most 4 records.
+constexpr int kMaxTreePhrases = kMaxTermSlots / 2;
+struct DevPhrase {
+  int32_t clause0;        // its first term clause, relative to the query's clause_begin; term i is clause0 + i
+  int32_t n_terms;        // 2..8, ordered by query position (stable): term 0 leads the exact matcher
+  int32_t slop;
+  int32_t field;
+  float weight;           // boost * (float) sum of the terms' idf (double sum)
+  int32_t cover_slot;     // the slot of its rarest term
+  int32_t reserved[2];
+  int32_t offset[kMaxTermSlots];   // PhraseQuery positions of the terms
+};
+static_assert(sizeof(DevPhrase) == 64, "DevPhrase layout");
 
 struct DevQuery {
   int32_t clause_begin, n_clauses;

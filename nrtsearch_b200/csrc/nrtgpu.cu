@@ -158,6 +158,11 @@ struct nrtgpu_index {
   DevBuf<uint8_t> post_f8;
   DevBuf<int64_t> exc_pos;
   DevBuf<int32_t> exc_freq;
+  int64_t sum_freq = 0;             // sum of the exact freqs: the positions nrtgpu_index_add_positions expects
+  bool has_positions = false;
+  DevBuf<int32_t> positions;        // term positions, posting after posting (nrtgpu_index_add_positions)
+  DevBuf<uint32_t> pos_off;         // [P] first position of each posting, relative to its term's base
+  DevBuf<int64_t> pos_base;         // [n_terms + 1] first position of each term
   std::vector<std::unique_ptr<DevBuf<uint8_t>>> norms;
   DevBuf<const uint8_t*> norms_ptrs;
   DevBuf<float> caches;
@@ -218,6 +223,7 @@ struct nrtgpu_index {
     v.live_bits = live_bits.p;
     v.dense_tf = dense_tf.p; v.dense_stride = dense_stride; v.dense_tf2 = dense_tf2.p;
     v.gran_tab = gran_tab.p; v.n_gran = gran_n;
+    v.positions = positions.p; v.pos_off = pos_off.p; v.pos_base = pos_base.p;
     return v;
   }
   PlanDict dict() const {   // what batch compilation and planning read
@@ -226,6 +232,7 @@ struct nrtgpu_index {
     d.term_off = term_off.data(); d.term_field = term_field.data(); d.term_df = term_df.data(); d.term_max_x = term_max_x.data();
     d.term_plane = term_plane.data(); d.term_gran = term_gran.data(); d.field_doc_count = field_doc_count.data();
     d.col_multi = col_multi.data(); d.col_n_distinct = col_n_distinct.data(); d.has_deletes = live_bits.p != nullptr;
+    d.has_positions = has_positions;
     return d;
   }
   KnnCorpus knn_corpus() const {   // what the kNN stages read; NRTGPU_KNN_SIMT, read on every call, forces the fp32 SIMT stage
@@ -258,6 +265,8 @@ struct nrtgpu_batch {
   DevBuf<DevQuery> queries;
   DevBuf<DevNode> nodes;          // tree batches: cb.nodes
   DevBuf<int32_t> node_begin;     // tree batches: cb.node_begin
+  DevBuf<DevPhrase> phrases;      // tree batches: cb.phrases
+  DevBuf<int32_t> phrase_begin;   // tree batches: cb.phrase_begin
   DevBuf<int32_t> work_query, work_slice;
   DevBuf<int32_t> pruned;    // [nq] relation GTE flags
   DevBuf<int32_t> terminated; // [nq] terminateAfter cut the query short
@@ -431,6 +440,7 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
     for (int64_t p = 0; p < P; ++p) {
       int32_t f = d->post_freqs[p];
       if (f < 1) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_build: term frequency < 1");
+      ix->sum_freq += f;
       if (f >= 255) { f8[(size_t)p] = 255; epos.push_back(p); efreq.push_back(f); } else f8[(size_t)p] = (uint8_t)f;
     }
     if ((rc = ix->post_f8.upload(f8.data(), (size_t)P + pad))) return rc;
@@ -634,6 +644,48 @@ int nrtgpu_index_close(nrtgpu_index* ix) {
 
 int64_t nrtgpu_index_device_bytes(const nrtgpu_index* ix) { return ix ? ix->device_bytes : 0; }
 
+int nrtgpu_index_add_positions(nrtgpu_index* ix, const int32_t* positions, int64_t n_positions) {
+  if (!ix || (n_positions > 0 && !positions)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_positions: NULL argument");
+  if (n_positions != ix->sum_freq)
+    NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_positions: n_positions must be the sum of the postings' freqs (" +
+                                     std::to_string(ix->sum_freq) + "), not " + std::to_string(n_positions));
+  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
+  NRT_CUDA_TRY(cudaDeviceSynchronize());   // searches in flight on this image finish against the old positions
+  // the exact freq of every posting (the saturated byte and the exception list) gives each posting's position range
+  const int64_t P = ix->n_terms ? ix->term_off[(size_t)ix->n_terms] : 0;
+  std::vector<uint8_t> f8((size_t)P);
+  std::vector<int64_t> epos(ix->exc_pos.n); std::vector<int32_t> efreq(ix->exc_freq.n);
+  if (P) NRT_CUDA_TRY(cudaMemcpy(f8.data(), ix->post_f8.p, (size_t)P, cudaMemcpyDeviceToHost));
+  if (!epos.empty()) NRT_CUDA_TRY(cudaMemcpy(epos.data(), ix->exc_pos.p, epos.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  if (!efreq.empty()) NRT_CUDA_TRY(cudaMemcpy(efreq.data(), ix->exc_freq.p, efreq.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  std::vector<uint32_t> off((size_t)P);
+  std::vector<int64_t> base((size_t)ix->n_terms + 1, 0);
+  int64_t run = 0; size_t e = 0;
+  for (int32_t t = 0; t < ix->n_terms; ++t) {
+    base[(size_t)t] = run;
+    for (int64_t p = ix->term_off[(size_t)t]; p < ix->term_off[(size_t)t + 1]; ++p) {
+      int64_t f = f8[(size_t)p];
+      if (f == 255) { while (e < epos.size() && epos[e] < p) ++e; if (e < epos.size() && epos[e] == p) f = efreq[e]; }
+      if (run - base[(size_t)t] > (int64_t)UINT32_MAX) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nrtgpu_index_add_positions: more than 2^32 positions of one term");
+      off[(size_t)p] = (uint32_t)(run - base[(size_t)t]);
+      for (int64_t i = run; i < run + f; ++i) {
+        if (positions[i] < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_positions: negative position");
+        if (i > run && positions[i] < positions[i - 1]) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_positions: positions descend within a posting");
+      }
+      run += f;
+    }
+  }
+  base[(size_t)ix->n_terms] = run;
+  const int64_t old_bytes = (int64_t)(ix->positions.bytes() + ix->pos_off.bytes() + ix->pos_base.bytes());
+  int rc;
+  if ((rc = ix->positions.upload(positions, (size_t)n_positions))) return rc;
+  if ((rc = ix->pos_off.upload(off.data(), off.size()))) return rc;
+  if ((rc = ix->pos_base.upload(base.data(), base.size()))) return rc;
+  ix->device_bytes += (int64_t)(ix->positions.bytes() + ix->pos_off.bytes() + ix->pos_base.bytes()) - old_bytes;
+  ix->has_positions = true;
+  return NRTGPU_OK;
+}
+
 int nrtgpu_index_set_live_docs(nrtgpu_index* ix, const uint8_t* live_docs) {
   if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_set_live_docs: NULL index");
   NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
@@ -672,6 +724,8 @@ static int batch_compile(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& 
   if (b->cb.tree) {
     if ((rc = b->nodes.upload_async(b->cb.nodes.data(), b->cb.nodes.size(), st))) return rc;
     if ((rc = b->node_begin.upload_async(b->cb.node_begin.data(), b->cb.node_begin.size(), st))) return rc;
+    if ((rc = b->phrases.upload_async(b->cb.phrases.data(), b->cb.phrases.size(), st))) return rc;
+    if ((rc = b->phrase_begin.upload_async(b->cb.phrase_begin.data(), b->cb.phrase_begin.size(), st))) return rc;
   }
   return b->queries.upload_async(b->cb.queries.data(), b->cb.queries.size(), st);
 }
@@ -776,6 +830,8 @@ int nrtgpu_batch_prepare(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
 
 static BatchRequest tree_request(const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes, int32_t n_nodes,
                                  const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags);
+static int phrase_request(BatchRequest* r, const nrtgpu_phrase* phrases, int32_t n_phrases, const nrtgpu_phrase_term* phrase_terms,
+                          int32_t n_phrase_terms);
 
 int nrtgpu_batch_prepare_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
                               int32_t n_nodes, const nrtgpu_query* queries, int32_t nq, int32_t top_k,
@@ -786,6 +842,22 @@ int nrtgpu_batch_prepare_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, in
   int rc = batch_build(b.get(), ix, tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags),
                        (cudaStream_t)0);
   if (rc) return rc;
+  NRT_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)0));
+  *out = b.release();
+  return NRTGPU_OK;
+}
+
+int nrtgpu_batch_prepare_tree_phrases(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                                      int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                                      const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                                      int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags, nrtgpu_batch** out) {
+  if (!out) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_prepare: NULL argument");
+  if (n_nodes < 0 || (n_nodes > 0 && !nodes)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_tree: bad nodes");
+  BatchRequest r = tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags);
+  int rc = phrase_request(&r, phrases, n_phrases, phrase_terms, n_phrase_terms);
+  if (rc) return rc;
+  std::unique_ptr<nrtgpu_batch> b(new nrtgpu_batch);
+  if ((rc = batch_build(b.get(), ix, r, (cudaStream_t)0))) return rc;
   NRT_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)0));
   *out = b.release();
   return NRTGPU_OK;
@@ -825,7 +897,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   if (b->plan.n_work() > 0) {
     BoolLaunch L;
     L.ix = b->ix->view();
-    L.nodes = nullptr; L.node_begin = nullptr;
+    L.nodes = nullptr; L.node_begin = nullptr; L.phrases = nullptr; L.phrase_begin = nullptr;
     L.clauses = b->clauses.p; L.queries = b->queries.p;
     L.work_query = b->work_query.p; L.work_slice = b->work_slice.p;
     L.n_work = b->plan.n_work(); L.n_slices = b->plan.n_lists; L.top_k = b->top_k;
@@ -903,7 +975,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         NRT_CUDA_TRY(cudaGetLastError());
       }
     } else if (b->cb.tree) {
-      L.nodes = b->nodes.p; L.node_begin = b->node_begin.p;
+      L.nodes = b->nodes.p; L.node_begin = b->node_begin.p; L.phrases = b->phrases.p; L.phrase_begin = b->phrase_begin.p;
       bool_window_kernel<true><<<b->plan.n_work(), kThreads, sizeof(BoolTreeSmem), st>>>(L);
     } else
       bool_window_kernel<false><<<b->plan.n_work(), kThreads, sizeof(BoolSmem), st>>>(L);
@@ -1243,6 +1315,31 @@ int nrtgpu_search_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n
   SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
   o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early;
   return search_bool_impl(ix, tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags), limits, stream, o);
+}
+
+// the phrase table of the phrase entry points; without phrases the request stays that of nrtgpu_search_tree
+static int phrase_request(BatchRequest* r, const nrtgpu_phrase* phrases, int32_t n_phrases, const nrtgpu_phrase_term* phrase_terms,
+                          int32_t n_phrase_terms) {
+  if (n_phrases < 0 || n_phrase_terms < 0 || (n_phrases > 0 && !phrases) || (n_phrase_terms > 0 && !phrase_terms))
+    NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_tree_phrases: bad phrases");
+  if (n_phrases > 0) { r->phrases = phrases; r->n_phrases = n_phrases; r->phrase_terms = phrase_terms; r->n_phrase_terms = n_phrase_terms; }
+  return NRTGPU_OK;
+}
+
+int nrtgpu_search_tree_phrases(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                               int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                               const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                               int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags,
+                               const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs, float* out_scores,
+                               int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
+                               uint8_t* out_terminated_early) {
+  if (n_nodes < 0 || (n_nodes > 0 && !nodes)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_tree: bad nodes");
+  BatchRequest r = tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags);
+  int rc = phrase_request(&r, phrases, n_phrases, phrase_terms, n_phrase_terms);
+  if (rc) return rc;
+  SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
+  o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early;
+  return search_bool_impl(ix, r, limits, stream, o);
 }
 
 int nrtgpu_search_sorted(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,

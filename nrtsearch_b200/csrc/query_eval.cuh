@@ -30,6 +30,11 @@ struct DevIndexView {
   int64_t dense_stride;
   const uint8_t* dense_tf2;      // [n_planes][dense_stride / 4] min(freq, 3) in 2 bits per doc: the planes the probe kernel gathers
                                  // (a quarter of the L2 / DRAM footprint of the byte planes; 3 = "three or more")
+  // term positions (nrtgpu_index_add_positions; NULL without): posting p of term t holds positions[pos_base[t] + pos_off[p]
+  // .. end), end = the next posting's start, or pos_base[t + 1] for the term's last posting (its exact freq positions)
+  const int32_t* positions;
+  const uint32_t* pos_off;       // [P]
+  const int64_t* pos_base;       // [n_terms + 1]
 };
 
 // numeric range clause on one doc (IndexOrDocValuesQuery's doc-values side, reference IntFieldDef.java:124-158 inclusive
@@ -132,7 +137,7 @@ __device__ __forceinline__ bool eval_clauses(const DevIndexView& ix, const DevQu
 //   DISMAX: matches if any disjunct does; DisjunctionMaxScorer's float max and double sum of the others, streamed in clause
 //           order as Lucene 10 streams its disjuncts (a new max moves the old one into the sum), scored
 //           (float)((double)max + others * (double)tie_breaker).
-// term(c, &s) as for eval_clauses. Liveness is the caller's.
+// term(c, &s) as for eval_clauses, for term and phrase leaves alike. Liveness is the caller's.
 template <class TermScore>
 __device__ __forceinline__ bool eval_node(const DevIndexView& ix, const DevNode& nd, const DevClause* cl, int32_t doc,
                                           uint32_t node_match, const float* node_score, TermScore term, float* out_score) {
@@ -143,7 +148,7 @@ __device__ __forceinline__ bool eval_node(const DevIndexView& ix, const DevNode&
     const DevClause& c = cl[nd.clause_begin + i];
     bool present;
     float s = 0.0f;
-    if (c.kind == NRTGPU_TERM) {
+    if (c.kind == NRTGPU_TERM || c.kind == NRTGPU_PHRASE) {
       present = term(c, &s);
     } else if (c.kind == NRTGPU_RANGE_I64) {
       present = range_matches(ix, c.col, doc, c.lo, c.hi);

@@ -50,6 +50,9 @@ class HostShard:
     vectors: Optional[np.ndarray] = None      # float32[n_vec, dims]
     vec_similarity: int = SIM_COSINE
     vec_docs: Optional[np.ndarray] = None     # int32[n_vec] ord -> doc
+    # term positions (PostingsEnum.POSITIONS): posting after posting, the post_freqs[p] positions of posting p, ascending;
+    # None = indexed without positions (PhraseQuery is refused)
+    post_positions: Optional[np.ndarray] = None
 
     @property
     def n_terms(self) -> int:
@@ -77,6 +80,13 @@ class HostShard:
         np.cumsum(lens, out=off[1:])
         idx = np.concatenate([np.arange(s, e, dtype=np.int64) for s, e in zip(starts, ends)]) if nt else np.zeros(0, np.int64)
         global_df = self.term_df if self.term_df is not None else np.diff(self.term_off)
+        sub_pos = None
+        if self.post_positions is not None:   # the positions of the kept postings, in their order
+            pstart = np.zeros(len(self.post_freqs) + 1, np.int64)
+            np.cumsum(self.post_freqs, out=pstart[1:])
+            f = self.post_freqs[idx].astype(np.int64)
+            first = np.repeat(pstart[idx] - (np.cumsum(f) - f), f)
+            sub_pos = np.ascontiguousarray(self.post_positions[first + np.arange(int(f.sum()), dtype=np.int64)], np.int32)
         sub_vec = sub_vdocs = None
         if self.vectors is not None:
             vd = self.vec_docs if self.vec_docs is not None else np.arange(len(self.vectors), dtype=np.int32)
@@ -95,7 +105,7 @@ class HostShard:
                             for i in range(len(self.columns))],
             column_has=[None if h is None else np.ascontiguousarray(h[lo:hi]) for h in self.column_has],
             live_docs=None if self.live_docs is None else np.ascontiguousarray(self.live_docs[lo:hi]),
-            vectors=sub_vec, vec_similarity=self.vec_similarity, vec_docs=sub_vdocs)
+            vectors=sub_vec, vec_similarity=self.vec_similarity, vec_docs=sub_vdocs, post_positions=sub_pos)
 
 
 def _ptr(a: Optional[np.ndarray], typ):

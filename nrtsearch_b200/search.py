@@ -70,6 +70,22 @@ class DisjunctionMaxQuery:
     tie_breaker: float = 0.0
 
 
+@dataclass
+class PhraseQuery:
+    """PhraseQuery(slop, terms, positions): what match_phrase maps to (QueryNodeMapper.java:285-291, :397-427). All terms on
+    one text field; positions default to 0, 1, 2, ... as PhraseQuery.Builder.add(term) assigns them. Runs on the window
+    engine as a leaf of a query tree (GpuIndexSearcher.search_tree) over an image with positions."""
+    terms: List[int] = field(default_factory=list)   # the adaptor's dense (field, term) ids
+    positions: Optional[List[int]] = None
+    slop: int = 0
+
+    def term_positions(self) -> List[Tuple[int, int]]:
+        pos = list(range(len(self.terms))) if self.positions is None else list(self.positions)
+        if len(pos) != len(self.terms):
+            raise ValueError("PhraseQuery: one position per term")
+        return [(int(t), int(p)) for t, p in zip(self.terms, pos)]
+
+
 @dataclass(frozen=True)
 class BooleanClause:
     query: object
@@ -316,13 +332,29 @@ def _unboost(q, boost: np.float32):
     return q, boost
 
 
-def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Optional[ScoreDoc]]] = None):
+def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Optional[ScoreDoc]]] = None,
+                 phrase_table: bool = False):
     """Query trees -> (Clause[], n_clauses, Node[], n_nodes, Query[], nq) for nrtgpu_search_tree. The root of a query is a
     BooleanQuery (a bare leaf or DisjunctionMaxQuery becomes its single MUST clause); every BooleanQuery or
     DisjunctionMaxQuery below it is a node, numbered in pre-order over the batch, whose clauses are one range of the clause
     array. BoostQuery boosts are folded through the nodes into the leaves, outermost first in float, so node clauses carry
-    boost 1 (BoostQuery.createWeight passes boost * this.boost down)."""
+    boost 1 (BoostQuery.createWeight passes boost * this.boost down).
+    phrase_table: return (Clause[], n_clauses, Node[], n_nodes, Phrase[], n_phrases, PhraseTerm[], n_phrase_terms, Query[],
+    nq) for nrtgpu_search_tree_phrases instead: a PhraseQuery leaf is a clause of kind 4 whose id indexes the phrase table.
+    Without it a PhraseQuery is refused."""
     flat, nodes, qs = [], [], []
+    phrases, pterms = [], []
+
+    def leaf(sub, sb, occ):
+        if isinstance(sub, PhraseQuery):
+            if not phrase_table:
+                raise NrtGpuUnsupported(3, "PhraseQuery needs compile_tree(..., phrase_table=True)")
+            begin = len(pterms)
+            pterms.extend(sub.term_positions())
+            phrases.append((begin, len(pterms), int(sub.slop), 0))
+            flat.append((int(occ), 4, len(phrases) - 1, float(sb), 0, 0))
+        else:
+            _flatten(sub, sb, flat, occ)
 
     def parts(q):
         if isinstance(q, BooleanQuery):
@@ -359,7 +391,7 @@ def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Opti
                 if sb is None:
                     flat.append((int(occ), 3, base + sub, 1.0, 0, 0))
                 else:
-                    _flatten(sub, sb, flat, occ)
+                    leaf(sub, sb, occ)
             begin_end.append((begin, len(flat)))
         for p in range(1, len(order)):
             kind, _, msm, tie = order[p]
@@ -370,6 +402,10 @@ def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Opti
     carr = (Clause * max(len(flat), 1))(*[Clause(*c) for c in flat])
     narr = (_native.Node * max(len(nodes), 1))(*[_native.Node(*n) for n in nodes])
     qarr = (CQuery * max(len(qs), 1))(*[CQuery(*t) for t in qs])
+    if phrase_table:
+        parr = (_native.Phrase * max(len(phrases), 1))(*[_native.Phrase(*p) for p in phrases])
+        tarr = (_native.PhraseTerm * max(len(pterms), 1))(*[_native.PhraseTerm(*t) for t in pterms])
+        return carr, len(flat), narr, len(nodes), parr, len(phrases), tarr, len(pterms), qarr, len(qs)
     return carr, len(flat), narr, len(nodes), qarr, len(qs)
 
 
@@ -424,6 +460,13 @@ class GpuIndex:
         self.handle = h
         self.n_docs, self.doc_base = shard.n_docs, shard.doc_base
         self._orders = {}
+        if shard.post_positions is not None:
+            self.add_positions(shard.post_positions)
+
+    def add_positions(self, positions: np.ndarray):
+        """Term positions of every posting, posting after posting (HostShard.post_positions): what PhraseQuery needs."""
+        p = np.ascontiguousarray(positions, np.int32)
+        check(self._lib.nrtgpu_index_add_positions(self.handle, p.ctypes.data if len(p) else None, len(p)))
 
     def sort_order(self, fields: Sequence[SortType], stream: int = 0) -> C.c_void_p:
         """The nrtgpu_sort_order of a Sort, built on first use and kept until close(): it depends on the columns only, so
@@ -481,12 +524,16 @@ class BatchResult:
 class PreparedBatch:
     """nrtgpu_batch: compiled batch resident on the device (launch many times, inputs stay in HBM)."""
 
-    def __init__(self, index: GpuIndex, carr, ncl, qarr, nq, top_k, threshold, flags=0, nodes=None):
-        """nodes: (Node[], n_nodes) of a query-tree batch (nrtgpu_batch_prepare_tree), None for flat queries."""
+    def __init__(self, index: GpuIndex, carr, ncl, qarr, nq, top_k, threshold, flags=0, nodes=None, phrases=None):
+        """nodes: (Node[], n_nodes) of a query-tree batch (nrtgpu_batch_prepare_tree), None for flat queries; phrases:
+        (Phrase[], n_phrases, PhraseTerm[], n_phrase_terms) of a tree batch with phrases (nrtgpu_batch_prepare_tree_phrases)."""
         self._lib = _native.gpu_lib()
         self.index, self.nq, self.top_k = index, nq, top_k
         h = C.c_void_p()
-        if nodes is None:
+        if phrases is not None:
+            check(self._lib.nrtgpu_batch_prepare_tree_phrases(index.handle, carr, ncl, nodes[0], nodes[1], *phrases, qarr, nq, top_k,
+                                                              threshold, flags, C.byref(h)))
+        elif nodes is None:
             check(self._lib.nrtgpu_batch_prepare(index.handle, carr, ncl, qarr, nq, top_k, threshold, flags, C.byref(h)))
         else:
             check(self._lib.nrtgpu_batch_prepare_tree(index.handle, carr, ncl, nodes[0], nodes[1], qarr, nq, top_k, threshold, flags,
@@ -574,26 +621,31 @@ class GpuIndexSearcher:
         """prepare() for queries that may nest BooleanQuery and DisjunctionMaxQuery (nrtgpu_batch_prepare_tree)."""
         if search_after is None and collector.search_after is not None:
             search_after = [collector.search_after] * len(queries)
-        carr, ncl, narr, nn, qarr, nq = compile_tree(queries, search_after)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, search_after, phrase_table=True)
         return PreparedBatch(self.index, carr, ncl, qarr, nq, collector.num_hits_to_collect, collector.total_hits_threshold, flags,
-                             nodes=(narr, nn))
+                             nodes=(narr, nn), phrases=(parr, n_ph, tarr, n_pt) if n_ph else None)
 
     def search_tree(self, queries: Sequence[object], collector: RelevanceCollector,
                     search_after: Optional[Sequence[Optional[ScoreDoc]]] = None, stream: int = 0) -> BatchResult:
         """search_batch() for queries that may nest BooleanQuery and DisjunctionMaxQuery (nrtgpu_search_tree): a batch with a
-        nested query runs on the window engine."""
+        nested query or a PhraseQuery runs on the window engine (phrases: nrtgpu_search_tree_phrases)."""
         if search_after is None and collector.search_after is not None:
             search_after = [collector.search_after] * len(queries)
-        carr, ncl, narr, nn, qarr, nq = compile_tree(queries, search_after)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, search_after, phrase_table=True)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, max(k, 1)), np.int32), np.zeros((nq, max(k, 1)), np.float32),
                           np.zeros(nq, np.int32), np.zeros(nq, np.int64), np.zeros(nq, np.uint8),
                           np.zeros(nq, np.uint8), np.zeros(nq, np.uint8))
         lim = collector.limits()
-        check(self._lib.nrtgpu_search_tree(self.index.handle, carr, ncl, narr, nn, qarr, nq, k, collector.total_hits_threshold, 0,
-                                           None if lim is None else C.byref(lim), C.c_void_p(stream), out.docs.ctypes.data,
-                                           out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data,
-                                           out.relation.ctypes.data, out.hit_timeout.ctypes.data, out.terminated_early.ctypes.data))
+        outs = (None if lim is None else C.byref(lim), C.c_void_p(stream), out.docs.ctypes.data, out.scores.ctypes.data,
+                out.counts.ctypes.data, out.total_hits.ctypes.data, out.relation.ctypes.data, out.hit_timeout.ctypes.data,
+                out.terminated_early.ctypes.data)
+        if n_ph:
+            check(self._lib.nrtgpu_search_tree_phrases(self.index.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k,
+                                                       collector.total_hits_threshold, 0, *outs))
+        else:
+            check(self._lib.nrtgpu_search_tree(self.index.handle, carr, ncl, narr, nn, qarr, nq, k, collector.total_hits_threshold, 0,
+                                               *outs))
         return out
 
     def knn_query(self, queries: np.ndarray, knn: KnnQuery, sim: int, boosts: Optional[np.ndarray] = None,
