@@ -388,6 +388,25 @@ int nrtgpu_rescore_query(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
                          const nrtgpu_query* queries, int32_t nq, int32_t n_hits, const int32_t* counts,
                          int32_t window, double query_weight, double rescore_weight, void* stream,
                          int32_t* docs, float* scores, int32_t* out_counts /*[nq] or NULL*/);
+/* The same pair for rescore queries that are query trees or hold phrases (a QueryRescorer whose rescore query is a
+ * match_phrase, a multi_match or a bool of those). They take the tree and phrase arguments of nrtgpu_search_tree_phrases and
+ * keep the semantics of nrtgpu_score_docs / nrtgpu_rescore_query: global doc ids, counts may be NULL in score_docs, a doc
+ * outside the leaf, a deleted doc and an entry past counts[q] get match 0 and score 0. A matching doc's score is the float
+ * the window engine gives the same doc for the same tree (the node rules of nrtgpu_search_tree, the phrase weight and freq
+ * rules of nrtgpu_search_tree_phrases). Every refusal of nrtgpu_search_tree_phrases applies, and every argument check of the
+ * flat pair. With n_nodes == 0 and n_phrases == 0 they are nrtgpu_score_docs / nrtgpu_rescore_query; a batch holding a
+ * nested query or a phrase is evaluated as a tree batch, its flat queries included. */
+int nrtgpu_score_docs_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                           int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                           const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                           int32_t nq, int32_t n_hits, const int32_t* docs, const int32_t* counts /*[nq] or NULL*/,
+                           void* stream, uint8_t* out_matches, float* out_scores);
+int nrtgpu_rescore_query_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                              int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                              const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                              int32_t nq, int32_t n_hits, const int32_t* counts, int32_t window, double query_weight,
+                              double rescore_weight, void* stream, int32_t* docs, float* scores,
+                              int32_t* out_counts /*[nq] or NULL*/);
 
 /* Fetch phase on doc-value columns (SearchHandler.java:397-522, FillDocsTask.fetchFromDocVales / LoadedDocValues): the
  * values of n_cols columns for n hits (global doc ids): out_values / out_has [n_cols*n]. */

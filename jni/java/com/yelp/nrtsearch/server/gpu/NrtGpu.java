@@ -100,6 +100,21 @@ public final class NrtGpu {
       long index, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int nHits,
       ByteBuffer docs, ByteBuffer counts, ByteBuffer outMatches, ByteBuffer outScores);
 
+  /**
+   * QueryRescorer second pass (scoreDocsTree) and whole rescore (rescoreQueryTree, docs / scores rescored in place) for a
+   * rescore query that is a query tree or holds phrases; the tree and phrase buffers are laid out as for searchTreePhrases,
+   * the hit buffers as for scoreDocs.
+   */
+  public static native int scoreDocsTree(
+      long index, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer phrases, int nPhrases,
+      ByteBuffer phraseTerms, int nPhraseTerms, ByteBuffer queries, int nq, int nHits, ByteBuffer docs, ByteBuffer counts,
+      ByteBuffer outMatches, ByteBuffer outScores);
+
+  public static native int rescoreQueryTree(
+      long index, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer phrases, int nPhrases,
+      ByteBuffer phraseTerms, int nPhraseTerms, ByteBuffer queries, int nq, int nHits, ByteBuffer counts, int window,
+      double queryWeight, double rescoreWeight, ByteBuffer docs, ByteBuffer scores, ByteBuffer outCounts);
+
   public static native int fetchColumns(
       long index, ByteBuffer colIds, int nCols, ByteBuffer docs, int n, ByteBuffer outValues,
       ByteBuffer outHas);

@@ -171,6 +171,29 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_scoreDocs(
                                      (const int32_t*)ADDR(env, counts), NULL, (uint8_t*)ADDR(env, outMatches),
                                      (float*)ADDR(env, outScores)));
 }
+/* the second pass of a tree / phrase rescore query: the tree and phrase buffers as searchTreePhrases */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_scoreDocsTree(
+    JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,
+    jobject phraseTerms, jint nPhraseTerms, jobject queries, jint nq, jint nHits, jobject docs, jobject counts,
+    jobject outMatches, jobject outScores) {
+  return fail(env, nrtgpu_score_docs_tree((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                          (const nrtgpu_node*)ADDR(env, nodes), nNodes, (const nrtgpu_phrase*)ADDR(env, phrases),
+                                          nPhrases, (const nrtgpu_phrase_term*)ADDR(env, phraseTerms), nPhraseTerms,
+                                          (const nrtgpu_query*)ADDR(env, queries), nq, nHits, (const int32_t*)ADDR(env, docs),
+                                          (const int32_t*)ADDR(env, counts), NULL, (uint8_t*)ADDR(env, outMatches),
+                                          (float*)ADDR(env, outScores)));
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_rescoreQueryTree(
+    JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,
+    jobject phraseTerms, jint nPhraseTerms, jobject queries, jint nq, jint nHits, jobject counts, jint window,
+    jdouble queryWeight, jdouble rescoreWeight, jobject docs, jobject scores, jobject outCounts) {
+  return fail(env, nrtgpu_rescore_query_tree((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                             (const nrtgpu_node*)ADDR(env, nodes), nNodes, (const nrtgpu_phrase*)ADDR(env, phrases),
+                                             nPhrases, (const nrtgpu_phrase_term*)ADDR(env, phraseTerms), nPhraseTerms,
+                                             (const nrtgpu_query*)ADDR(env, queries), nq, nHits, (const int32_t*)ADDR(env, counts),
+                                             window, queryWeight, rescoreWeight, NULL, (int32_t*)ADDR(env, docs),
+                                             (float*)ADDR(env, scores), (int32_t*)ADDR(env, outCounts)));
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_fetchColumns(
     JNIEnv* env, jclass c, jlong ix, jobject colIds, jint nCols, jobject docs, jint n, jobject outValues, jobject outHas) {
   return fail(env, nrtgpu_fetch_columns((nrtgpu_index*)(intptr_t)ix, (const int32_t*)ADDR(env, colIds), nCols,

@@ -122,6 +122,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_sort_order_create", "nrtgpu_sort_order_device_bytes", "nrtgpu_sort_order_close", "nrtgpu_search_sorted_fields",
     "nrtgpu_search_tree", "nrtgpu_batch_prepare_tree",
     "nrtgpu_index_add_positions", "nrtgpu_search_tree_phrases", "nrtgpu_batch_prepare_tree_phrases",
+    "nrtgpu_score_docs_tree", "nrtgpu_rescore_query_tree",
 ]
 
 _gpu = None
@@ -193,6 +194,13 @@ def gpu_lib() -> C.CDLL:
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.nrtgpu_rescore_query.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32, C.c_void_p,
                                              C.c_int32, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.nrtgpu_score_docs_tree.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32, C.POINTER(Phrase),
+                                               C.c_int32, C.POINTER(PhraseTerm), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.nrtgpu_rescore_query_tree.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32,
+                                                  C.POINTER(Phrase), C.c_int32, C.POINTER(PhraseTerm), C.c_int32, C.POINTER(Query),
+                                                  C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p]
         lib.nrtgpu_fetch_columns.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.nrtgpu_index_set_live_docs.argtypes = [C.c_void_p, C.c_void_p]
         lib.nrtgpu_index_update_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -78,14 +78,6 @@ struct BoolTreeSmem : BoolSmemT<true> {
   int n_phrases;
 };
 
-// bit s set: byte s (term slot s) of a window word is non-zero
-__device__ __forceinline__ uint32_t presence_mask(uint64_t s) {
-  uint32_t m = 0;
-#pragma unroll
-  for (int i = 0; i < kMaxTermSlots; ++i) m |= (((s >> (8 * i)) & 0xff) != 0 ? 1u : 0u) << i;
-  return m;
-}
-
 // the clauses of sm.q on one candidate doc; slot holds the doc's tf byte of every term slot
 __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolSmem& sm, int32_t doc,
                                              uint64_t slot, float* out_score) {
@@ -103,129 +95,19 @@ __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolS
   return eval_clauses(ix, sm.q, sm.cl, doc, presence_mask(slot), term, out_score);
 }
 
-// The freq of phrase ph in doc, which holds every term of it (PhraseScorer: the sum of sloppyWeight over the matches), or
-// with first_only 1 as soon as one match is found (a phrase under FILTER / MUST_NOT only has to match); 0: no match.
-// Each term's posting is found by a lower_bound inside its slot's window bounds (sm.bounds), its positions are the
-// posting's range of the image's positions. Fixed-size per-thread state, no recursion.
-//   slop 0: ExactPhraseMatcher: every position of the lead (term 0, the smallest query position) at which each other term
-//           has the position lead - offset[0] + offset[j] counts 1;
-//   slop>0: SloppyPhraseMatcher without repeats: the PhraseQueue of (position - offset, offset, ordinal) -- a total order, so
-//           a scan for its minimum pops what the heap pops --, the running end and the match-length minimisation; every
-//           match adds 1.0f / (1.0f + matchLength) in float.
-__device__ __noinline__ float phrase_freq(const DevIndexView& ix, const BoolTreeSmem& sm, const DevPhrase& ph, int32_t doc,
-                                          bool first_only) {
-  const int n = ph.n_terms;
+// a phrase term's posting in the window engine: a lower_bound inside its slot's bounds of the doc's window (sm.bounds)
+__device__ __forceinline__ uint32_t phrase_posting(const DevIndexView& ix, const BoolTreeSmem& sm, const DevClause& t, int32_t doc) {
   const int w = (doc & (kWideSliceDocs - 1)) / kWindowDocs;   // the doc's window in its slice
-  int64_t cur[kMaxTermSlots], end[kMaxTermSlots];
-  for (int i = 0; i < n; ++i) {
-    const DevClause& t = sm.cl[ph.clause0 + i];
-    const int32_t* docs = ix.post_docs + t.post_base;
-    uint32_t lo = sm.bounds[t.slot][w], hi = sm.bounds[t.slot][w + 1];
-    while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (__ldg(docs + m) < doc) lo = m + 1; else hi = m; }
-    const int64_t gp = t.post_base + lo, base = __ldg(ix.pos_base + t.col);
-    cur[i] = base + __ldg(ix.pos_off + gp);
-    end[i] = (int64_t)lo + 1 < (int64_t)t.n_post ? base + __ldg(ix.pos_off + gp + 1) : __ldg(ix.pos_base + t.col + 1);
-  }
-  const int32_t* P = ix.positions;
-  float freq = 0.0f;
-  if (ph.slop == 0) {
-    for (int64_t a = cur[0]; a < end[0]; ++a) {
-      const int32_t phrase_pos = __ldg(P + a) - ph.offset[0];
-      bool ok = true;
-      for (int j = 1; j < n && ok; ++j) {
-        const int32_t want = phrase_pos + ph.offset[j];
-        while (cur[j] < end[j] && __ldg(P + cur[j]) < want) ++cur[j];
-        if (cur[j] == end[j]) return freq;   // term j has no position left: no later lead position can match
-        ok = __ldg(P + cur[j]) == want;
-      }
-      if (ok) { freq = __fadd_rn(freq, 1.0f); if (first_only) return freq; }
-    }
-    return freq;
-  }
-  int32_t pos[kMaxTermSlots];
-  int32_t end_pos = INT_MIN;
-  uint32_t inq = 0;
-  for (int i = 0; i < n; ++i) {
-    pos[i] = __ldg(P + cur[i]) - ph.offset[i]; ++cur[i];
-    end_pos = max(end_pos, pos[i]);
-    inq |= 1u << i;
-  }
-  auto top = [&](uint32_t m) {   // the queue's least element: position, then offset, then ordinal
-    int best = -1;
-    for (int i = 0; i < n; ++i) {
-      if (!((m >> i) & 1u)) continue;
-      if (best < 0 || pos[i] < pos[best] || (pos[i] == pos[best] && ph.offset[i] < ph.offset[best])) best = i;
-    }
-    return best;
-  };
-  for (;;) {   // nextMatch
-    int pp = top(inq);
-    inq &= ~(1u << pp);
-    int32_t match_len = end_pos - pos[pp];
-    int32_t next = pos[top(inq)];
-    bool positioned = true, matched = false;
-    for (;;) {
-      if (cur[pp] >= end[pp]) { positioned = false; matched = match_len <= ph.slop; break; }
-      pos[pp] = __ldg(P + cur[pp]) - ph.offset[pp]; ++cur[pp];
-      end_pos = max(end_pos, pos[pp]);
-      if (pos[pp] > next) {   // done minimising the current match length
-        inq |= 1u << pp;
-        if (match_len <= ph.slop) { matched = true; break; }
-        pp = top(inq);
-        inq &= ~(1u << pp);
-        next = pos[top(inq)];
-        match_len = end_pos - pos[pp];
-      } else {
-        match_len = min(match_len, end_pos - pos[pp]);
-      }
-    }
-    if (!matched) return freq;
-    freq = __fadd_rn(freq, __fdiv_rn(1.0f, __fadd_rn(1.0f, (float)match_len)));
-    if (first_only || !positioned) return freq;
-  }
+  const int32_t* docs = ix.post_docs + t.post_base;
+  uint32_t lo = sm.bounds[t.slot][w], hi = sm.bounds[t.slot][w + 1];
+  while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (__ldg(docs + m) < doc) lo = m + 1; else hi = m; }
+  return lo;
 }
 
-// the query tree of sm on one candidate doc: the nodes bottom-up (reverse pre-order: children before parents), no recursion
+// the query tree of sm on one candidate doc
 __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolTreeSmem& sm, int32_t doc, uint64_t slot,
                                              float* out_score) {
-  const uint32_t mask = presence_mask(slot);
-  if ((mask & sm.q.req_term_mask) != sm.q.req_term_mask) return false;
-  if (mask & sm.q.not_term_mask) return false;
-  if (ix.live_bits && !((ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
-  auto term = [&](const DevClause& c, float* s) {
-    if (c.kind == NRTGPU_PHRASE) {
-      if (c.col < 0) return false;   // a phrase of no terms
-      const DevPhrase& ph = sm.phrases[c.col];
-      for (int i = 0; i < ph.n_terms; ++i) if (!((mask >> sm.cl[ph.clause0 + i].slot) & 1u)) return false;
-      const float f = phrase_freq(ix, sm, ph, doc, !c.scoring);
-      if (f == 0.0f) return false;
-      if (c.scoring) {
-        const uint8_t* nrm = ix.norms[ph.field];
-        const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
-        *s = bm25_score(c.weight, f, sm.cache[sm.cl[ph.clause0].slot][nb]);
-      }
-      return true;
-    }
-    const uint32_t b = (uint32_t)((slot >> (8 * c.slot)) & 0xff);
-    if (b == 0) return false;
-    if (c.scoring) {
-      const float f = (b == 255u) ? exact_freq_slow(ix, c, doc) : (float)b;
-      const uint8_t* nrm = ix.norms[c.field];
-      const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
-      *s = bm25_score(c.weight, f, sm.cache[c.slot][nb]);
-    }
-    return true;
-  };
-  uint32_t matched = 0;
-  float node_score[kMaxTreeNodes];
-  for (int n = sm.n_nodes - 1; n >= 0; --n) {
-    const DevNode& nd = sm.nodes[n];
-    float s;
-    if (!nd.empty && eval_node(ix, nd, sm.cl, doc, matched, node_score, term, &s)) { matched |= 1u << n; node_score[n] = s; }
-  }
-  if (!(matched & 1u)) return false;
-  *out_score = node_score[0];
-  return true;
+  return eval_tree(ix, sm, doc, slot, out_score);
 }
 
 // kTree: a tree batch (sm holds the query's nodes, evaluate_doc walks them); otherwise flat BooleanQuerys

@@ -72,6 +72,85 @@ __global__ void score_docs_kernel(const __grid_constant__ ScoreDocsLaunch L) {
   L.out_matches[i] = m; L.out_scores[i] = s;
 }
 
+// QueryRescorer second pass of a tree batch (query trees, phrase leaves): one CTA per (query, chunk of kScoreTreeThreads
+// hits), the query's clauses, nodes, phrase records and per-slot BM25 caches staged once per CTA, one hit per thread
+struct ScoreDocsTreeLaunch : ScoreDocsLaunch {
+  const DevNode* nodes; const int32_t* node_begin;        // the nodes of query q: nodes[node_begin[q], node_begin[q + 1])
+  const DevPhrase* phrases; const int32_t* phrase_begin;  // its phrase records: phrases[phrase_begin[q], phrase_begin[q + 1])
+  int32_t n_chunks;                                       // CTAs per query: blockIdx.x = q * n_chunks + chunk
+};
+
+constexpr int kScoreTreeThreads = 256;
+
+struct ScoreTreeSmem {
+  DevClause cl[kMaxTreeClauses];
+  DevNode nodes[kMaxTreeNodes];
+  DevPhrase phrases[kMaxTreePhrases];
+  float cache[kMaxTermSlots][256];
+  uint32_t post[kMaxTermSlots][kScoreTreeThreads];   // the posting (index in its term's list) of each slot present in a thread's doc
+  DevQuery q;
+  int n_nodes;
+};
+
+// a phrase term's posting in the second pass: the one the slot lookup found
+__device__ __forceinline__ uint32_t phrase_posting(const DevIndexView&, const ScoreTreeSmem& sm, const DevClause& t, int32_t) {
+  return sm.post[t.slot][threadIdx.x];
+}
+
+// The tf byte and posting of term clause c in doc: a lower_bound over the term's postings, narrowed by its granule row (the
+// index-time skip data) to the postings of the doc's 1024-doc granule when it has one. 0: the doc holds no posting.
+__device__ __forceinline__ uint32_t slot_lookup(const DevIndexView& ix, const DevClause& c, int32_t doc, uint32_t* post) {
+  const int32_t* docs = ix.post_docs + c.post_base;
+  uint32_t lo = 0, hi = (uint32_t)c.n_post;
+  if (c.gran_row >= 0) {
+    const uint32_t* row = ix.gran_tab + (size_t)c.gran_row * (size_t)(ix.n_gran + 1) + (doc >> v3::kLogGran);
+    lo = __ldg(row); hi = __ldg(row + 1);
+  }
+  const uint32_t end = hi;
+  while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (__ldg(docs + m) < doc) lo = m + 1; else hi = m; }
+  if (lo == end || __ldg(docs + lo) != doc) return 0u;
+  *post = lo;
+  return c.scoring ? (uint32_t)__ldg(ix.post_f8 + c.post_base + lo) : 1u;   // (pass 1 of the window engine stores the same byte)
+}
+
+__global__ void __launch_bounds__(kScoreTreeThreads) score_docs_tree_kernel(const __grid_constant__ ScoreDocsTreeLaunch L) {
+  __shared__ ScoreTreeSmem sm;
+  const int q = blockIdx.x / L.n_chunks, chunk = blockIdx.x % L.n_chunks;
+  const int tid = threadIdx.x;
+  if (tid == 0) { sm.q = L.queries[q]; sm.n_nodes = L.node_begin[q + 1] - L.node_begin[q]; }
+  __syncthreads();
+  const int ncl = sm.q.n_clauses;
+  const int n_phrases = L.phrase_begin[q + 1] - L.phrase_begin[q];
+  if (tid < ncl) sm.cl[tid] = L.clauses[sm.q.clause_begin + tid];
+  if (tid < sm.n_nodes) sm.nodes[tid] = L.nodes[L.node_begin[q] + tid];
+  if (tid < n_phrases) sm.phrases[tid] = L.phrases[L.phrase_begin[q] + tid];
+  __syncthreads();
+  for (int i = tid; i < ncl * 256; i += kScoreTreeThreads) {
+    const int c = i >> 8;
+    if (sm.cl[c].kind == NRTGPU_TERM) sm.cache[sm.cl[c].slot][i & 255] = L.ix.caches[sm.cl[c].field * 256 + (i & 255)];
+  }
+  __syncthreads();
+  const int r = chunk * kScoreTreeThreads + tid;
+  if (r >= L.n_hits) return;
+  const size_t i = (size_t)q * L.n_hits + r;
+  uint8_t m = 0; float s = 0.0f;
+  if (!sm.q.empty && r < (L.counts ? L.counts[q] : L.n_hits)) {
+    const int64_t local = (int64_t)L.docs[i] - L.ix.doc_base;
+    if (local >= 0 && local < L.ix.n_docs) {
+      const int32_t doc = (int32_t)local;
+      uint64_t word = 0;   // the doc's tf byte of every term slot, as the window engine's pass 1 leaves it
+      for (int c = 0; c < ncl; ++c) {
+        const DevClause& cl = sm.cl[c];
+        if (cl.kind != NRTGPU_TERM) continue;
+        word |= (uint64_t)slot_lookup(L.ix, cl, doc, &sm.post[cl.slot][tid]) << (8 * cl.slot);
+      }
+      float sc;
+      if (eval_tree(L.ix, sm, doc, word, &sc)) { m = 1; s = sc; }
+    }
+  }
+  L.out_matches[i] = m; L.out_scores[i] = s;
+}
+
 // fetch phase: doc values of n_cols columns for n docs
 struct FetchLaunch {
   DevIndexView ix;

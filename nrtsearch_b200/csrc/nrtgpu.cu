@@ -1440,58 +1440,73 @@ static BatchRequest compile_only_request(const nrtgpu_clause* clauses, int32_t n
   return BatchRequest{clauses, n_clauses, queries, nq, 1, INT32_MAX, 0};
 }
 
-int nrtgpu_score_docs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
-                      const nrtgpu_query* queries, int32_t nq, int32_t n_hits, const int32_t* docs,
-                      const int32_t* counts, void* stream, uint8_t* out_matches, float* out_scores) {
-  if (!ix || !docs || !out_matches || !out_scores || n_hits <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_score_docs: bad argument");
+// the second pass of a compiled request on the hit lists in b->sd_docs (b->sd_counts when counts is set): the flat
+// score_docs_kernel, or score_docs_tree_kernel for a tree batch
+static int launch_score_docs(nrtgpu_batch* b, nrtgpu_index* ix, int32_t nq, int32_t n_hits, bool counts, cudaStream_t st) {
+  const size_t n = (size_t)nq * n_hits;
+  int rc;
+  if ((rc = b->sd_match.alloc(n)) || (rc = b->sd_scores.alloc(n))) return rc;
+  ScoreDocsLaunch S; S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_hits = n_hits;
+  S.docs = b->sd_docs.p; S.counts = counts ? b->sd_counts.p : nullptr; S.out_matches = b->sd_match.p; S.out_scores = b->sd_scores.p;
+  if (!b->cb.tree) {
+    score_docs_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(S);
+  } else {
+    ScoreDocsTreeLaunch T;
+    static_cast<ScoreDocsLaunch&>(T) = S;
+    T.nodes = b->nodes.p; T.node_begin = b->node_begin.p; T.phrases = b->phrases.p; T.phrase_begin = b->phrase_begin.p;
+    T.n_chunks = (n_hits + kScoreTreeThreads - 1) / kScoreTreeThreads;
+    if ((int64_t)T.n_chunks * nq > INT32_MAX) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "second pass: too many hits in one batch");
+    score_docs_tree_kernel<<<(unsigned)(T.n_chunks * nq), kScoreTreeThreads, 0, st>>>(T);
+  }
+  NRT_CUDA_TRY(cudaGetLastError());
+  return NRTGPU_OK;
+}
+
+// nrtgpu_score_docs / nrtgpu_score_docs_tree (fn names the entry point in messages)
+static int score_docs_impl(const char* fn, nrtgpu_index* ix, const BatchRequest& r, int32_t n_hits, const int32_t* docs,
+                           const int32_t* counts, void* stream, uint8_t* out_matches, float* out_scores) {
+  if (!ix || !docs || !out_matches || !out_scores || n_hits <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, std::string(fn) + ": bad argument");
   cudaStream_t st = (cudaStream_t)stream;
   WorkspaceLease ws(ix);
   nrtgpu_batch* b = ws.b;
-  int rc = batch_compile(b, ix, compile_only_request(clauses, n_clauses, queries, nq), st);
+  const int32_t nq = r.nq;
+  int rc = batch_compile(b, ix, r, st);
   const size_t n = (size_t)nq * n_hits;
   if (!rc) rc = b->sd_docs.upload_async(docs, n, st);
   if (!rc && counts) rc = b->sd_counts.upload_async(counts, (size_t)nq, st);
-  if (!rc) rc = b->sd_match.alloc(n);
-  if (!rc) rc = b->sd_scores.alloc(n);
+  if (!rc) rc = launch_score_docs(b, ix, nq, n_hits, counts != nullptr, st);
   if (rc) return rc;
-  ScoreDocsLaunch S; S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_hits = n_hits;
-  S.docs = b->sd_docs.p; S.counts = counts ? b->sd_counts.p : nullptr; S.out_matches = b->sd_match.p; S.out_scores = b->sd_scores.p;
-  score_docs_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(S);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out_matches, b->sd_match.p, n, cudaMemcpyDeviceToHost, st);
+  cudaError_t e = cudaMemcpyAsync(out_matches, b->sd_match.p, n, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaMemcpyAsync(out_scores, b->sd_scores.p, n * sizeof(float), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; }
   return NRTGPU_OK;
 }
 
-int nrtgpu_rescore_query(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
-                         const nrtgpu_query* queries, int32_t nq, int32_t n_hits, const int32_t* counts,
-                         int32_t window, double query_weight, double rescore_weight, void* stream,
-                         int32_t* docs, float* scores, int32_t* out_counts) {
-  if (!ix || !docs || !scores || n_hits <= 0 || window <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_rescore_query: bad argument");
-  if (n_hits > kHybCap) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nrtgpu_rescore_query: more than 4096 hits per query");
+// nrtgpu_rescore_query / nrtgpu_rescore_query_tree
+static int rescore_query_impl(const char* fn, nrtgpu_index* ix, const BatchRequest& r, int32_t n_hits, const int32_t* counts,
+                              int32_t window, double query_weight, double rescore_weight, void* stream, int32_t* docs,
+                              float* scores, int32_t* out_counts) {
+  if (!ix || !docs || !scores || n_hits <= 0 || window <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, std::string(fn) + ": bad argument");
+  if (n_hits > kHybCap) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, std::string(fn) + ": more than 4096 hits per query");
   cudaStream_t st = (cudaStream_t)stream;
   WorkspaceLease ws(ix);
   nrtgpu_batch* b = ws.b;
-  int rc = batch_compile(b, ix, compile_only_request(clauses, n_clauses, queries, nq), st);
+  const int32_t nq = r.nq;
+  int rc = batch_compile(b, ix, r, st);
   const size_t n = (size_t)nq * n_hits;
   // Lucene QueryRescorer.rescore(searcher, hits, topN = windowSize): EVERY first-pass hit is combined and the list
   // re-sorted (score desc, doc asc); then the first topN are kept
   std::vector<int32_t> wc((size_t)nq);
   for (int q = 0; q < nq; ++q) {
     wc[(size_t)q] = counts ? counts[q] : n_hits;
-    if (wc[(size_t)q] < 0 || wc[(size_t)q] > n_hits) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_rescore_query: counts out of range");
+    if (wc[(size_t)q] < 0 || wc[(size_t)q] > n_hits) NRT_FAIL(NRTGPU_ERR_INVALID, std::string(fn) + ": counts out of range");
   }
   if (!rc) rc = b->sd_docs.upload_async(docs, n, st);
   if (!rc) rc = b->sd_first.upload_async(scores, n, st);
   if (!rc) rc = b->sd_counts.upload_async(wc.data(), (size_t)nq, st);
-  if (!rc) rc = b->sd_match.alloc(n);
-  if (!rc) rc = b->sd_scores.alloc(n);
+  if (!rc) rc = launch_score_docs(b, ix, nq, n_hits, true, st);
   if (rc) return rc;
-  ScoreDocsLaunch S; S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_hits = n_hits;
-  S.docs = b->sd_docs.p; S.counts = b->sd_counts.p; S.out_matches = b->sd_match.p; S.out_scores = b->sd_scores.p;
-  score_docs_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(S);
   RescoreLaunch P;
   P.nq = nq; P.n_hits = n_hits; P.counts = b->sd_counts.p; P.docs = b->sd_docs.p; P.scores = b->sd_first.p;
   P.second_matches = b->sd_match.p; P.second_scores = b->sd_scores.p; P.query_weight = query_weight; P.rescore_weight = rescore_weight;
@@ -1503,6 +1518,52 @@ int nrtgpu_rescore_query(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
   if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; }
   if (out_counts) for (int q = 0; q < nq; ++q) out_counts[q] = std::min(wc[(size_t)q], window);
   return NRTGPU_OK;
+}
+
+int nrtgpu_score_docs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                      const nrtgpu_query* queries, int32_t nq, int32_t n_hits, const int32_t* docs,
+                      const int32_t* counts, void* stream, uint8_t* out_matches, float* out_scores) {
+  return score_docs_impl("nrtgpu_score_docs", ix, compile_only_request(clauses, n_clauses, queries, nq), n_hits, docs, counts, stream,
+                         out_matches, out_scores);
+}
+
+int nrtgpu_rescore_query(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                         const nrtgpu_query* queries, int32_t nq, int32_t n_hits, const int32_t* counts,
+                         int32_t window, double query_weight, double rescore_weight, void* stream,
+                         int32_t* docs, float* scores, int32_t* out_counts) {
+  return rescore_query_impl("nrtgpu_rescore_query", ix, compile_only_request(clauses, n_clauses, queries, nq), n_hits, counts, window,
+                            query_weight, rescore_weight, stream, docs, scores, out_counts);
+}
+
+// the compile-only request of the tree entry points: that of nrtgpu_score_docs with the node and phrase tables
+static int compile_only_tree_request(BatchRequest* r, const nrtgpu_node* nodes, int32_t n_nodes, const nrtgpu_phrase* phrases,
+                                     int32_t n_phrases, const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms) {
+  if (n_nodes < 0 || (n_nodes > 0 && !nodes)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_tree: bad nodes");
+  if (n_nodes > 0) { r->nodes = nodes; r->n_nodes = n_nodes; }
+  return phrase_request(r, phrases, n_phrases, phrase_terms, n_phrase_terms);
+}
+
+int nrtgpu_score_docs_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                           int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                           const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                           int32_t nq, int32_t n_hits, const int32_t* docs, const int32_t* counts, void* stream,
+                           uint8_t* out_matches, float* out_scores) {
+  BatchRequest r = compile_only_request(clauses, n_clauses, queries, nq);
+  int rc = compile_only_tree_request(&r, nodes, n_nodes, phrases, n_phrases, phrase_terms, n_phrase_terms);
+  if (rc) return rc;
+  return score_docs_impl("nrtgpu_score_docs_tree", ix, r, n_hits, docs, counts, stream, out_matches, out_scores);
+}
+
+int nrtgpu_rescore_query_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                              int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                              const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                              int32_t nq, int32_t n_hits, const int32_t* counts, int32_t window, double query_weight,
+                              double rescore_weight, void* stream, int32_t* docs, float* scores, int32_t* out_counts) {
+  BatchRequest r = compile_only_request(clauses, n_clauses, queries, nq);
+  int rc = compile_only_tree_request(&r, nodes, n_nodes, phrases, n_phrases, phrase_terms, n_phrase_terms);
+  if (rc) return rc;
+  return rescore_query_impl("nrtgpu_rescore_query_tree", ix, r, n_hits, counts, window, query_weight, rescore_weight, stream, docs,
+                            scores, out_counts);
 }
 
 int nrtgpu_fetch_columns(nrtgpu_index* ix, const int32_t* col_ids, int32_t n_cols, const int32_t* docs, int32_t n,

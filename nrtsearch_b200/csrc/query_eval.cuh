@@ -1,7 +1,8 @@
-// One flat BooleanQuery on one doc: the device view of the index that every query kernel reads, the doc-value range test,
-// the exact tf of a saturated posting, and the clause rule shared by the window engine (bool_kernel.cuh), the generic
-// probe kernel (probe_kernel.cuh) and the second pass (collect_kernel.cuh). The engines differ only in how they find a
-// term's tf and norm; each passes that in.
+// One query on one doc: the device view of the index that every query kernel reads, the doc-value range test, the exact
+// tf of a saturated posting, the flat clause rule shared by the window engine (bool_kernel.cuh), the generic probe kernel
+// (probe_kernel.cuh) and the second pass (collect_kernel.cuh), and the query-tree walk with its phrase matcher shared by
+// the window engine's tree instantiation and the second pass of tree batches. The engines differ only in how they find a
+// term's tf and norm, and a phrase term's posting; each passes that in.
 #pragma once
 #include "common.cuh"
 #include "../../include/nrtgpu.h"
@@ -131,7 +132,7 @@ __device__ __forceinline__ bool eval_clauses(const DevIndexView& ix, const DevQu
   return true;
 }
 
-// One node of a query tree (tree batches of the window engine) on one doc, its child nodes already evaluated: node_match
+// One node of a query tree (tree batches: the window engine, the second pass) on one doc, its child nodes already evaluated: node_match
 // bit n is set iff node n matched, node_score[n] is then the float its Scorer returned. The clauses are walked in order.
 //   BOOL:   eval_clauses's rule, a child node counting as a clause that is present when it matched and scores its float;
 //   DISMAX: matches if any disjunct does; DisjunctionMaxScorer's float max and double sum of the others, streamed in clause
@@ -190,6 +191,141 @@ __device__ __forceinline__ bool eval_node(const DevIndexView& ix, const DevNode&
     }
   }
   *out_score = score;
+  return true;
+}
+
+// bit s set: byte s (term slot s) of a slot word is non-zero
+__device__ __forceinline__ uint32_t presence_mask(uint64_t s) {
+  uint32_t m = 0;
+#pragma unroll
+  for (int i = 0; i < kMaxTermSlots; ++i) m |= (((s >> (8 * i)) & 0xff) != 0 ? 1u : 0u) << i;
+  return m;
+}
+
+// The freq of phrase ph in doc, which holds every term of it (PhraseScorer: the sum of sloppyWeight over the matches), or
+// with first_only 1 as soon as one match is found (a phrase under FILTER / MUST_NOT only has to match); 0: no match.
+// Term i's posting is phrase_posting(ix, sm, term clause, doc), the engine's (its index in the term's list); its positions are
+// the posting's range of the image's positions. Fixed-size per-thread state, no recursion.
+//   slop 0: ExactPhraseMatcher: every position of the lead (term 0, the smallest query position) at which each other term
+//           has the position lead - offset[0] + offset[j] counts 1;
+//   slop>0: SloppyPhraseMatcher without repeats: the PhraseQueue of (position - offset, offset, ordinal) -- a total order, so
+//           a scan for its minimum pops what the heap pops --, the running end and the match-length minimisation; every
+//           match adds 1.0f / (1.0f + matchLength) in float.
+template <class Smem>
+__device__ __noinline__ float phrase_freq(const DevIndexView& ix, const Smem& sm, const DevPhrase& ph, int32_t doc,
+                                          bool first_only) {
+  const int n = ph.n_terms;
+  int64_t cur[kMaxTermSlots], end[kMaxTermSlots];
+  for (int i = 0; i < n; ++i) {
+    const DevClause& t = sm.cl[ph.clause0 + i];
+    const uint32_t lo = phrase_posting(ix, sm, t, doc);
+    const int64_t gp = t.post_base + lo, base = __ldg(ix.pos_base + t.col);
+    cur[i] = base + __ldg(ix.pos_off + gp);
+    end[i] = (int64_t)lo + 1 < (int64_t)t.n_post ? base + __ldg(ix.pos_off + gp + 1) : __ldg(ix.pos_base + t.col + 1);
+  }
+  const int32_t* P = ix.positions;
+  float freq = 0.0f;
+  if (ph.slop == 0) {
+    for (int64_t a = cur[0]; a < end[0]; ++a) {
+      const int32_t phrase_pos = __ldg(P + a) - ph.offset[0];
+      bool ok = true;
+      for (int j = 1; j < n && ok; ++j) {
+        const int32_t want = phrase_pos + ph.offset[j];
+        while (cur[j] < end[j] && __ldg(P + cur[j]) < want) ++cur[j];
+        if (cur[j] == end[j]) return freq;   // term j has no position left: no later lead position can match
+        ok = __ldg(P + cur[j]) == want;
+      }
+      if (ok) { freq = __fadd_rn(freq, 1.0f); if (first_only) return freq; }
+    }
+    return freq;
+  }
+  int32_t pos[kMaxTermSlots];
+  int32_t end_pos = INT_MIN;
+  uint32_t inq = 0;
+  for (int i = 0; i < n; ++i) {
+    pos[i] = __ldg(P + cur[i]) - ph.offset[i]; ++cur[i];
+    end_pos = max(end_pos, pos[i]);
+    inq |= 1u << i;
+  }
+  auto top = [&](uint32_t m) {   // the queue's least element: position, then offset, then ordinal
+    int best = -1;
+    for (int i = 0; i < n; ++i) {
+      if (!((m >> i) & 1u)) continue;
+      if (best < 0 || pos[i] < pos[best] || (pos[i] == pos[best] && ph.offset[i] < ph.offset[best])) best = i;
+    }
+    return best;
+  };
+  for (;;) {   // nextMatch
+    int pp = top(inq);
+    inq &= ~(1u << pp);
+    int32_t match_len = end_pos - pos[pp];
+    int32_t next = pos[top(inq)];
+    bool positioned = true, matched = false;
+    for (;;) {
+      if (cur[pp] >= end[pp]) { positioned = false; matched = match_len <= ph.slop; break; }
+      pos[pp] = __ldg(P + cur[pp]) - ph.offset[pp]; ++cur[pp];
+      end_pos = max(end_pos, pos[pp]);
+      if (pos[pp] > next) {   // done minimising the current match length
+        inq |= 1u << pp;
+        if (match_len <= ph.slop) { matched = true; break; }
+        pp = top(inq);
+        inq &= ~(1u << pp);
+        next = pos[top(inq)];
+        match_len = end_pos - pos[pp];
+      } else {
+        match_len = min(match_len, end_pos - pos[pp]);
+      }
+    }
+    if (!matched) return freq;
+    freq = __fadd_rn(freq, __fdiv_rn(1.0f, __fadd_rn(1.0f, (float)match_len)));
+    if (first_only || !positioned) return freq;
+  }
+}
+
+// The query tree staged in sm on one doc whose slot word holds the tf byte of every term slot (0: absent; phrase terms and
+// terms that do not score: 1): the root's required and excluded slots, liveness, then the nodes bottom-up (reverse
+// pre-order: children before parents) through eval_node, no recursion. sm holds the query (q), its clauses (cl), nodes
+// (nodes, n_nodes), phrase records (phrases) and the per-slot BM25 caches (cache[slot][norm byte]); phrase_posting(ix, sm, ...)
+// is the engine's.
+template <class Smem>
+__device__ __forceinline__ bool eval_tree(const DevIndexView& ix, const Smem& sm, int32_t doc, uint64_t slot, float* out_score) {
+  const uint32_t mask = presence_mask(slot);
+  if ((mask & sm.q.req_term_mask) != sm.q.req_term_mask) return false;
+  if (mask & sm.q.not_term_mask) return false;
+  if (ix.live_bits && !((ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
+  auto term = [&](const DevClause& c, float* s) {
+    if (c.kind == NRTGPU_PHRASE) {
+      if (c.col < 0) return false;   // a phrase of no terms
+      const DevPhrase& ph = sm.phrases[c.col];
+      for (int i = 0; i < ph.n_terms; ++i) if (!((mask >> sm.cl[ph.clause0 + i].slot) & 1u)) return false;
+      const float f = phrase_freq(ix, sm, ph, doc, !c.scoring);
+      if (f == 0.0f) return false;
+      if (c.scoring) {
+        const uint8_t* nrm = ix.norms[ph.field];
+        const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
+        *s = bm25_score(c.weight, f, sm.cache[sm.cl[ph.clause0].slot][nb]);
+      }
+      return true;
+    }
+    const uint32_t b = (uint32_t)((slot >> (8 * c.slot)) & 0xff);
+    if (b == 0) return false;
+    if (c.scoring) {
+      const float f = (b == 255u) ? exact_freq_slow(ix, c, doc) : (float)b;
+      const uint8_t* nrm = ix.norms[c.field];
+      const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;
+      *s = bm25_score(c.weight, f, sm.cache[c.slot][nb]);
+    }
+    return true;
+  };
+  uint32_t matched = 0;
+  float node_score[kMaxTreeNodes];
+  for (int n = sm.n_nodes - 1; n >= 0; --n) {
+    const DevNode& nd = sm.nodes[n];
+    float s;
+    if (!nd.empty && eval_node(ix, nd, sm.cl, doc, matched, node_score, term, &s)) { matched |= 1u << n; node_score[n] = s; }
+  }
+  if (!(matched & 1u)) return false;
+  *out_score = node_score[0];
   return true;
 }
 

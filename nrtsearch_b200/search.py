@@ -768,6 +768,32 @@ class GpuIndexSearcher:
                                              rescore_weight, C.c_void_p(stream), d.ctypes.data, s.ctypes.data, oc.ctypes.data))
         return d, s, oc
 
+    def score_docs_tree(self, queries: Sequence[object], docs: np.ndarray, counts: Optional[np.ndarray] = None, stream: int = 0):
+        """score_docs() for rescore queries that may nest BooleanQuery and DisjunctionMaxQuery or hold PhraseQuery leaves
+        (nrtgpu_score_docs_tree): the queries search_tree takes."""
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, phrase_table=True)
+        d = np.ascontiguousarray(docs, np.int32)
+        cn = None if counts is None else np.ascontiguousarray(counts, np.int32)
+        m, s = np.zeros(d.shape, np.uint8), np.zeros(d.shape, np.float32)
+        check(self._lib.nrtgpu_score_docs_tree(self.index.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, d.shape[1],
+                                               d.ctypes.data, None if cn is None else cn.ctypes.data, C.c_void_p(stream),
+                                               m.ctypes.data, s.ctypes.data))
+        return m, s
+
+    def rescore_query_tree(self, queries: Sequence[object], docs: np.ndarray, scores: np.ndarray, counts: np.ndarray, window: int,
+                           query_weight: float, rescore_weight: float, stream: int = 0):
+        """rescore_query() for rescore queries that may nest BooleanQuery and DisjunctionMaxQuery or hold PhraseQuery leaves
+        (nrtgpu_rescore_query_tree): returns docs, scores, counts of the rescored lists."""
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, phrase_table=True)
+        d = np.ascontiguousarray(docs, np.int32).copy()
+        s = np.ascontiguousarray(scores, np.float32).copy()
+        cn = np.ascontiguousarray(counts, np.int32)
+        oc = np.zeros(nq, np.int32)
+        check(self._lib.nrtgpu_rescore_query_tree(self.index.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, d.shape[1],
+                                                  cn.ctypes.data, window, query_weight, rescore_weight, C.c_void_p(stream),
+                                                  d.ctypes.data, s.ctypes.data, oc.ctypes.data))
+        return d, s, oc
+
     def fetch_columns(self, columns: Sequence[int], docs: np.ndarray, stream: int = 0):
         """Fetch phase on doc-value columns: values int64 [n_cols, n], has uint8 [n_cols, n] for the hits `docs`."""
         cols = np.ascontiguousarray(columns, np.int32)
