@@ -414,7 +414,8 @@ int nrtgpu_fetch_columns(nrtgpu_index* ix, const int32_t* col_ids, int32_t n_col
                          void* stream, int64_t* out_values, uint8_t* out_has);
 
 /* Split form: compile+upload once, launch many times with everything resident in HBM (query trees:
- * nrtgpu_batch_prepare_tree). */
+ * nrtgpu_batch_prepare_tree). A prepared batch holds the weights and score bounds of the statistics it was compiled with:
+ * it stays valid across nrtgpu_index_set_live_docs; after nrtgpu_index_update_stats prepare it again. */
 int nrtgpu_batch_prepare(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
                          const nrtgpu_query* queries, int32_t nq, int32_t top_k,
                          int32_t total_hits_threshold, int32_t flags, nrtgpu_batch** out);

@@ -148,6 +148,35 @@ constexpr int kMaxSliceGran = 512;           // a slice spans at most 512K docs 
 constexpr int kWarmGran = 32;                // granules (32K docs) of the warm-up work item of a query
 constexpr int kProbeMaxTopK = 512;           // largest top_k of the probe kernel (half its candidate buffer)
 
+// ---- per-query record of the probe kernel ----
+// Everything a work item's set-up needs that depends on (query, index image) only, built on the device once per prepared
+// batch (probe_query_kernel) and copied into shared memory by every item of the query; the item adds its posting bounds,
+// its granule offsets and the roles that follow from the query's threshold. The record points into the index image and
+// holds floats derived from its length caches: it is valid for the statistics the batch was prepared with, like the
+// compiled weight / ub of its clauses.
+struct alignas(16) DevProbeQuery {
+  // per term slot (a slot without a term clause: kind kAbsent, NULL pointers, row -1)
+  const int32_t* gdocs[kT];        // global postings of the list
+  const uint8_t* gf8[kT];
+  const uint8_t* plane[kT];        // byte plane (exact min(tf, 255) per doc) of the list, or NULL
+  const uint8_t* plane2[kT];       // 2-bit plane (min(tf, 3), four docs per byte): what the probes gather
+  float weight[kT];
+  float ub[kT];
+  int32_t kind[kT];                // kPlane / kLong / kShort / kAbsent (an item may turn kShort into kGlobal)
+  int32_t clause[kT];
+  int32_t field[kT];
+  uint32_t pbm[kT];                // post_base mod 16 (alignment of the list inside the global posting arrays)
+  int32_t row[kT];                 // row of the index-time granule offsets, -1: none
+  // MAXSCORE order: the slots ascending by ub (equal bounds in slot order) and the float of the running double sum of
+  // their bounds; the non-essential lists of an item are the longest prefix with pre[a] < theta.score
+  int32_t ord[kT];
+  float pre[kT];
+  DevQuery q;
+  DevClause cl[kMaxClauses];
+  float ubt[256];                  // pure disjunctions: score bound per tf pattern, index sum min(tf_s, 3) * 4^s
+};
+static_assert(sizeof(DevProbeQuery) % 16 == 0, "DevProbeQuery is copied 16 bytes at a time");
+
 // ---- work item of the probe kernel: slice | part << 16 | log2(parts) << 20 | flags << 24 ----
 // A (query, slice) is split into 2^lparts parts of equal granule ranges; part p covers the finest parts
 // [p * kfine, (p + 1) * kfine) of the slice's parts_max, kfine = parts_max >> lparts.

@@ -259,6 +259,7 @@ struct nrtgpu_batch {
   CompiledBatch cb;            // host copies the async uploads read, kept until the next compilation
   WorkPlan plan;               // (search batches only)
   DevBuf<uint32_t> sbounds;            // probe kernel: [nq][4][n_slices * parts_max + 2] part-boundary posting offsets
+  DevBuf<v3::DevProbeQuery> pquery;    // probe kernel: [nq] per-query records (probe_query_kernel)
   DevBuf<unsigned int> work_counter;   // probe kernel: queue heads [2]
   DevBuf<unsigned long long> probe_stats;
   DevBuf<DevClause> clauses;
@@ -811,6 +812,12 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
     S.slice_gran = p.slice_docs / v3::kGran; S.n_gran = p.n_gran; S.parts_max = p.parts_max; S.sbounds = b->sbounds.p;
     v3::slice_bounds_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S);
     NRT_CUDA_TRY(cudaGetLastError());
+    // ... and the state of every query that no work item changes, which each item copies instead of deriving it
+    if ((rc = b->pquery.alloc((size_t)nq))) return rc;
+    v3::ProbeQueryLaunch Q;
+    Q.ix = S.ix; Q.clauses = b->clauses.p; Q.queries = b->queries.p; Q.field_min_norm = ix->field_min_norm.p; Q.out = b->pquery.p;
+    v3::probe_query_kernel<<<(unsigned)nq, v3::kUbt, 0, st>>>(Q);
+    NRT_CUDA_TRY(cudaGetLastError());
   }
   if (!b->ev[0][0]) for (auto& r : b->ev) for (auto& e : r) NRT_CUDA_TRY(cudaEventCreate(&e));
   return NRTGPU_OK;
@@ -908,8 +915,8 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
       const int n_probe = b->plan.n_probe_simple + b->plan.n_probe_generic;
       if (n_probe > 0) {
         v3::ProbeLaunch P;
-        P.ix = L.ix; P.clauses = L.clauses; P.queries = L.queries; P.sbounds = b->sbounds.p;
-        P.field_min_norm = b->ix->field_min_norm.p; P.stats = nullptr;
+        P.ix = L.ix; P.pquery = b->pquery.p; P.sbounds = b->sbounds.p;
+        P.stats = nullptr;
         P.known_hits = b->ix->live_bits.p ? nullptr : b->known_hits.p;   // (deletes installed after the batch was prepared: list lengths no longer bound the hits)
 #ifdef NRT_PROBE_KNOCK
         { const char* e = getenv("NRTGPU_KNOCK"); P.knock = e ? atoi(e) : 0; }   // profiling builds only (tools/knock.py)

@@ -61,6 +61,11 @@ __device__ __forceinline__ uint32_t presence4(uint32_t s) {
   return ((s & 0xffu) ? 1u : 0u) | ((s & 0xff00u) ? 2u : 0u) | ((s & 0xff0000u) ? 4u : 0u) | ((s & 0xff000000u) ? 8u : 0u);
 }
 
+// byte s 0xff where bit s of m is set (the inverse of presence4)
+__device__ __forceinline__ uint32_t expand4(uint32_t m) {
+  return ((m & 1u) ? 0xffu : 0u) | ((m & 2u) ? 0xff00u : 0u) | ((m & 4u) ? 0xff0000u : 0u) | ((m & 8u) ? 0xff000000u : 0u);
+}
+
 // profiling builds only (-DNRT_PROBE_KNOCK): parts of the kernel can be disabled at run time through ProbeLaunch::knock
 #ifdef NRT_PROBE_KNOCK
 #define NRT_KNOCK(bit) ((L.knock & (bit)) != 0)
@@ -88,6 +93,7 @@ constexpr int kR = NRT_PROBE_R;              // driver postings per thread per r
 constexpr int kCand = 1024;                  // candidate buffer entries
 static_assert(kProbeMaxTopK == kCand / 2, "the probe kernel keeps top_k <= half its candidate buffer");
 constexpr int kUbt = 4 * 4 * 4 * 4;          // tf-pattern bounds: min(tf, 3) per slot
+static_assert(sizeof(DevProbeQuery::ubt) == kUbt * sizeof(float), "one bound per tf pattern");
 constexpr int kWq = 32 * kR;                 // per-warp queue entries: the rounds drain it below 32 after their first push; once
                                              // the buffer is full, the kR - 1 pushes left in the round are not drained
 constexpr int kProbeStats = 24;              // stats words per instantiation (ProbeLaunch::stats)
@@ -99,12 +105,10 @@ enum { kAbsent = 0, kLong = 1, kShort = 2, kPlane = 3, kGlobal = 4 };
 
 struct ProbeLaunch {
   DevIndexView ix;
-  const DevClause* clauses;
-  const DevQuery* queries;
+  const DevProbeQuery* pquery;   // [nq] per-query records (probe_query_kernel)
   const int32_t* work_query;
   const int32_t* work_slice;     // work-item word (batch_plan.h item_encode)
   const uint32_t* sbounds;       // [nq][kT][n_slices * parts_max + 2]: postings of the slot's list below every part boundary, the shard end, the warm-up boundary
-  const uint8_t* field_min_norm;
   unsigned int* work_counter;    // queue head
   unsigned long long* stats;     // optional [kProbeStats]: items, item cycles, runs, driver postings, flushes, staged runs, set-up
                                  // cycles, rounds, longest item, CTA busy (sum, max), warm-up items and cycles, flush, TMA wait and
@@ -149,26 +153,12 @@ struct alignas(128) ProbeSmemT {
   uint32_t gb[kT][kMaxSliceGran + 4];   // granule offsets of the slice for lists with skip data (relative to the list's first posting)
   uint64_t cand[kCand];
   uint2 wq[kThreads / 32][kWq];    // per-warp queues of (doc, tf word) awaiting their score / clause evaluation
-  float ubt[kUbt];
-  float uval[kT][2];
-  DevClause cl[kMaxClauses];
-  DevQuery q;
+  DevProbeQuery pq;                // the query's record, copied whole by every item (an item patches kind and row)
   uint64_t stage_bar;
-  // per slot (CTA-uniform, written by thread 0 / threads < kT between barriers)
-  const int32_t* s_gdocs[kT];      // global postings of the list
-  const uint8_t* s_gf8[kT];
-  const uint8_t* s_plane[kT];      // byte plane (exact min(tf, 255) per doc) of the list, or NULL
-  const uint8_t* s_plane2[kT];     // 2-bit plane (min(tf, 3), four docs per byte): what the probes gather
-  float s_weight[kT];
-  float s_ub[kT];
-  int32_t s_kind[kT];
-  int32_t s_clause[kT];
-  int32_t s_field[kT];
+  // per slot, of the item (CTA-uniform, written between the set-up barriers)
   uint32_t s_ia[kT], s_ib[kT];     // item bounds (postings relative to the list's first)
   uint32_t s_ra[kT], s_rb[kT];     // run bounds
   int32_t s_sdelta[kT];            // staged lists: smem index of posting x = x + s_sdelta
-  uint32_t s_pbm[kT];              // post_base mod 16 (alignment of the list inside the global posting arrays)
-  int32_t s_row[kT];               // row of the index-time granule offsets (gb[] holds the slice's part), -1: none
   uint32_t s_need[kT];             // slots a driver posting of this slot probes
   uint32_t s_candbelow[kT];        // word bytes of the lists that own a doc before this slot (candidate emission)
   uint32_t s_cntbefore[kT];        // ... (hit counting)
@@ -197,7 +187,7 @@ __device__ __forceinline__ uint32_t seg_n(uint32_t a, uint32_t b, uint32_t pbm) 
   return b > a ? ((b + pbm + kAlign - 1) & ~(uint32_t)(kAlign - 1)) - ((a + pbm) & ~(uint32_t)(kAlign - 1)) : 0u;
 }
 
-// the clauses of sm.q on one queued doc; word holds the doc's tf byte of every term slot (kTfInexact: a saturated 2-bit
+// the clauses of sm.pq.q on one queued doc; word holds the doc's tf byte of every term slot (kTfInexact: a saturated 2-bit
 // code, the exact byte is read from the byte plane). The norm byte is reused while consecutive scored
 // term clauses read one field.
 template <typename SM>
@@ -208,7 +198,7 @@ __device__ __noinline__ bool evaluate_doc(const ProbeLaunch& L, const SM& sm, in
     uint32_t b = (word >> (8 * c.slot)) & 0xffu;
     if (b == 0) return false;
     if (c.scoring) {
-      if (b == kTfInexact && sm.s_plane[c.slot]) b = (uint32_t)__ldg(sm.s_plane[c.slot] + doc);
+      if (b == kTfInexact && sm.pq.plane[c.slot]) b = (uint32_t)__ldg(sm.pq.plane[c.slot] + doc);
       if (c.field != cur_field) {
         cur_field = c.field;
         const uint8_t* nrm = L.ix.norms[c.field];
@@ -219,7 +209,7 @@ __device__ __noinline__ bool evaluate_doc(const ProbeLaunch& L, const SM& sm, in
     }
     return true;
   };
-  return eval_clauses(L.ix, sm.q, sm.cl, doc, presence4(word), term, out_score);
+  return eval_clauses(L.ix, sm.pq.q, sm.pq.cl, doc, presence4(word), term, out_score);
 }
 
 // exact score of a doc of a pure single-field disjunction: double sum, in slot (= clause) order, of Lucene's BM25 float
@@ -234,9 +224,9 @@ __device__ __forceinline__ float score_disjunction(const ProbeLaunch& L, const S
     if (s >= n_term) break;
     uint32_t b = (word >> (8 * s)) & 0xffu;
     if (b == 0) continue;
-    if (b == kTfInexact && sm.s_plane[s]) b = (uint32_t)__ldg(sm.s_plane[s] + doc);   // saturated 2-bit code: the exact byte
-    const float f = (b == 255u) ? exact_freq_slow(L.ix, sm.cl[sm.s_clause[s]], doc) : (float)b;
-    sum += (double)bm25_score(sm.s_weight[s], f, __ldg(&L.ix.caches[sm.s_field[s] * 256 + nb]));
+    if (b == kTfInexact && sm.pq.plane[s]) b = (uint32_t)__ldg(sm.pq.plane[s] + doc);   // saturated 2-bit code: the exact byte
+    const float f = (b == 255u) ? exact_freq_slow(L.ix, sm.pq.cl[sm.pq.clause[s]], doc) : (float)b;
+    sum += (double)bm25_score(sm.pq.weight[s], f, __ldg(&L.ix.caches[sm.pq.field[s] * 256 + nb]));
   }
   return (float)sum;
 }
@@ -314,163 +304,144 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     // the docs that hold the query's rarest term are where its top-k is, a far better sample than the first 32K docs.
     const bool sweep_warm = (wflags & kItemSweep) != 0;
     const int warm_slot = item_sweep_slot(item);
-    const int ncl = L.queries[qi].n_clauses, cbeg = L.queries[qi].clause_begin, n_term = L.queries[qi].n_term;
-    if (tid == 0) {
-      sm.q = L.queries[qi];
-      sm.cand_count = 0;
-      sm.theta = *(volatile unsigned long long*)&L.theta[qi];
-      sm.hits0 = *(volatile unsigned long long*)&L.total_hits[qi];
-      { const unsigned long long kn = L.known_hits ? L.known_hits[qi] : 0ull; sm.hits_known = kn > sm.hits0 ? kn : sm.hits0; }
-      sm.theta_dec = sweep_warm ? 1 : 0;
-    }
-    if (tid < ncl) sm.cl[tid] = L.clauses[cbeg + tid];
-    if (tid >= 32 && tid < 32 + kT) { const int s = tid - 32; sm.s_kind[s] = kAbsent; sm.s_ia[s] = 0; sm.s_ib[s] = 0; sm.s_ra[s] = 0; sm.s_rb[s] = 0;
-                                      sm.s_plane[s] = nullptr; sm.s_plane2[s] = nullptr; sm.s_gdocs[s] = nullptr; sm.s_gf8[s] = nullptr; sm.s_weight[s] = 0.f; sm.s_ub[s] = 0.f;
-                                      sm.s_clause[s] = 0; sm.s_field[s] = 0; sm.s_sdelta[s] = 0; sm.s_pbm[s] = 0; sm.s_row[s] = -1; }
     const int g_first = slice * gran_per_slice;
     const int g_count = min(gran_per_slice, L.n_gran - g_first);
     // granule range of the item inside its slice, and the entries of the boundary table that hold its posting bounds
     const ItemSpan span = item_span(item, g_count, fine, L.parts_max, L.n_slices);
     const int g_lo = span.g_lo, g_hi = span.g_hi;
-    __syncthreads();   // B1: query + clauses resident
+    // ---- everything that needs only the item word: the query's record (16 bytes per thread; ubt only where it is
+    // read), the item's posting bounds, the query's threshold and hit count, and one step behind the record's rows the
+    // granule offsets of the lists with skip data. Every load is issued before the first value is stored, so that the
+    // set-up costs two dependent round trips and not one per loop iteration.
+    {
+      constexpr int n16 = (int)((kSimple ? sizeof(DevProbeQuery) : offsetof(DevProbeQuery, ubt)) / 16);
+      static_assert(n16 <= kThreads && kThreads == 64 * kT, "one 16-byte piece per thread; 64 threads per slot's granule offsets");
+      constexpr int kGbIter = (kMaxSliceGran + 1 + 63) / 64;
+      const int gs = tid >> 6, gj = g_lo + (tid & 63);   // this thread's slot and first granule of gb[]
+      const int gran_row = sweep_warm ? -1 : __ldg(&L.pquery[qi].row[gs]);
+      uint4 piece = make_uint4(0u, 0u, 0u, 0u);
+      if (tid < n16) piece = __ldg(reinterpret_cast<const uint4*>(L.pquery + qi) + tid);
+      unsigned long long theta = 0ull, hits0 = 0ull, known = 0ull;
+      uint32_t ba = 0, bb = 0, bw = 0;
+      if (tid == 0) {
+        theta = *(volatile unsigned long long*)&L.theta[qi];
+        hits0 = *(volatile unsigned long long*)&L.total_hits[qi];
+        if (L.known_hits) known = L.known_hits[qi];
+      }
+      if (tid >= 32 && tid < 32 + kT) {   // (the boundary entries of a slot without a term clause are 0)
+        const uint32_t* sb = L.sbounds + ((size_t)qi * kT + (tid - 32)) * sb_stride;
+        ba = sb[span.e_lo];
+        bb = sb[span.e_hi];
+        if (wflags & kItemBehindWarm) bw = sb[boundary_warm_entry(L.n_slices, L.parts_max)];
+      }
+      uint32_t gv[kGbIter];
+      const uint32_t* row = L.ix.gran_tab + (size_t)max(gran_row, 0) * (size_t)(L.n_gran + 1) + g_first;
+#pragma unroll
+      for (int k = 0; k < kGbIter; ++k) gv[k] = (gran_row >= 0 && gj + 64 * k <= g_hi) ? __ldg(row + gj + 64 * k) : 0u;
+      if (tid < n16) reinterpret_cast<uint4*>(&sm.pq)[tid] = piece;
+      if (tid == 0) {
+        sm.cand_count = 0;
+        sm.theta = theta; sm.hits0 = hits0; sm.hits_known = known > hits0 ? known : hits0;
+        sm.theta_dec = sweep_warm ? 1 : 0;
+      }
+      if (tid >= 32 && tid < 32 + kT) {
+        const int s = tid - 32;
+        const uint32_t a = max(ba, bw);
+        if (sweep_warm && s == warm_slot) bb = min(bb, a + 32768u);
+        sm.s_ia[s] = a; sm.s_ib[s] = max(a, bb); sm.s_ra[s] = 0; sm.s_rb[s] = 0; sm.s_sdelta[s] = 0;
+      }
+#pragma unroll
+      for (int k = 0; k < kGbIter; ++k) if (gran_row >= 0 && gj + 64 * k <= g_hi) sm.gb[gs][gj + 64 * k] = gv[k];
+    }
+    __syncthreads();   // B1: record, item bounds, threshold, granule offsets
     // terminateAfter (TerminateAfterWrapper.java:150-162): a query that has collected enough hits stops collecting
     if (L.terminate_after > 0 && (long long)sm.hits0 >= L.terminate_after) {
       if (tid == 0) L.terminated[qi] = 1;
       continue;
     }
-    // ---- per-slot descriptors (one thread per clause), granule offsets of the lists with skip data (all threads)
-    if (tid < ncl && sm.cl[tid].kind == NRTGPU_TERM) {
-      const DevClause& c = sm.cl[tid];
-      const int s = c.slot;
-      const uint32_t* sb = L.sbounds + ((size_t)qi * kT + s) * sb_stride;
-      uint32_t a = sb[span.e_lo];
-      uint32_t b = sb[span.e_hi];
-      if (wflags & kItemBehindWarm) a = max(a, sb[boundary_warm_entry(L.n_slices, L.parts_max)]);
-      if (sweep_warm && s == warm_slot) b = min(b, a + 32768u);
-      sm.s_ia[s] = a; sm.s_ib[s] = max(a, b);
-      sm.s_gdocs[s] = L.ix.post_docs + c.post_base;
-      sm.s_gf8[s] = L.ix.post_f8 + c.post_base;
-      const bool has_plane = c.plane >= 0 && L.ix.dense_tf != nullptr && L.ix.dense_tf2 != nullptr;
-      sm.s_plane[s] = has_plane ? L.ix.dense_tf + (size_t)c.plane * (size_t)L.ix.dense_stride : nullptr;
-      sm.s_plane2[s] = has_plane ? L.ix.dense_tf2 + (size_t)c.plane * (size_t)(L.ix.dense_stride >> 2) : nullptr;
-      sm.s_kind[s] = has_plane ? kPlane : (c.gran_row >= 0 ? kLong : kShort);   // kShort may become kGlobal below
-      if (sweep_warm && !has_plane && s != warm_slot) sm.s_kind[s] = kAbsent;   // not probed by the sweep warm-up: counts as absent
-      sm.s_weight[s] = c.weight; sm.s_ub[s] = c.ub; sm.s_clause[s] = tid; sm.s_field[s] = c.field;
-      sm.s_pbm[s] = (uint32_t)(c.post_base & (int64_t)(kAlign - 1)); sm.s_row[s] = sweep_warm ? -1 : c.gran_row;
-    }
-    for (int i = 0; i < ncl; ++i) {
-      const DevClause& c = sm.cl[i];
-      if (c.kind != NRTGPU_TERM || c.gran_row < 0 || sweep_warm) continue;
-      const uint32_t* row = L.ix.gran_tab + (size_t)c.gran_row * (size_t)(L.n_gran + 1) + g_first;
-      for (int g = g_lo + tid; g <= g_hi; g += kThreads) sm.gb[c.slot][g] = __ldg(row + g);
-    }
-    if (kSimple && tid >= 64 && tid < 64 + 2 * kT) {   // per-slot score bounds at tf = 1, 2 (shortest field length present)
-      const int s = (tid - 64) >> 1, c = ((tid - 64) & 1) + 1;
-      float u = 0.0f;
-      for (int i = 0; i < ncl; ++i)
-        if (sm.cl[i].kind == NRTGPU_TERM && sm.cl[i].slot == s) {
-          const uint32_t nbmin = (sm.q.single_field >= 0 && L.field_min_norm) ? (uint32_t)L.field_min_norm[sm.q.single_field] : 0u;
-          u = bm25_score(sm.cl[i].weight, (float)c, __ldg(&L.ix.caches[sm.cl[i].field * 256 + nbmin]));
-        }
-      sm.uval[s][c - 1] = u;
-    }
-    __syncthreads();   // B2: descriptors, granule offsets, bound values
-    if (kSimple) {
-      // ubt[sum min(tf_s, 3) * 4^s]: the double clause sum with every term at the shortest field length present
-      // (tf >= 3 bounded by the clause weight, the limit tf -> inf) -- an upper bound of the doc's score
-      const int n_ubt = 1 << (2 * min(n_term, kT));   // patterns of the slots that exist
-      for (int i = tid; i < n_ubt; i += kThreads) {
-        const int c[kT] = {i & 3, (i >> 2) & 3, (i >> 4) & 3, i >> 6};
-        double sum = 0.0;
-#pragma unroll
-        for (int t = 0; t < kT; ++t) {
-          float u = 0.0f;
-          if (sm.s_kind[t] != kAbsent && c[t] > 0) u = (c[t] <= 2) ? sm.uval[t][c[t] - 1] : sm.s_weight[t];
-          sum += (double)u;
-        }
-        sm.ubt[i] = (float)sum;
-      }
-    }
-    if (tid == 0) {
-      // ---- roles. MAXSCORE split (pure disjunctions): the lists whose list-wide bounds sum (double, ascending) below
-      // theta.score are non-essential: they never lead, docs found only in them cannot enter the top-k.
+    const int n_term = sm.pq.q.n_term;
+    // ---- roles: one thread per slot (each derives the CTA-uniform split for itself), then thread 0 plans the staging
+    if (tid < kT) {
+      const int t = tid;
       const uint32_t all = (n_term >= 32) ? 0xffffffffu : ((1u << n_term) - 1u);
-      uint32_t ne = 0;
       const bool complete = L.threshold >= (int64_t)INT32_MAX;
+      // MAXSCORE split (pure disjunctions): the lists whose list-wide bounds sum (double, ascending) below theta.score
+      // are non-essential: they never lead, docs found only in them cannot enter the top-k.
+      uint32_t ne = 0;
       if (kSimple && !sweep_warm && sm.theta != 0ull && (complete || (int64_t)sm.hits_known > L.threshold)) {
         const float theta_s = key_score(sm.theta);
-        int ord[kT]; int n = 0;
-        for (int s = 0; s < n_term; ++s) ord[n++] = s;
-        for (int a = 1; a < n; ++a) { const int x = ord[a]; int b = a - 1; while (b >= 0 && sm.s_ub[ord[b]] > sm.s_ub[x]) { ord[b + 1] = ord[b]; --b; } ord[b + 1] = x; }
-        double pre = 0.0;
-        for (int a = 0; a < n; ++a) {
-          const double s2 = pre + (double)sm.s_ub[ord[a]];
-          if (!((float)s2 < theta_s)) break;
-          pre = s2; ne |= 1u << ord[a];
+        for (int a = 0; a < n_term; ++a) {
+          if (!(sm.pq.pre[a] < theta_s)) break;
+          ne |= 1u << sm.pq.ord[a];
         }
       }
-      if (ne && !complete) L.pruned[qi] = 1;
-      // short lists are staged whole at the first run; what does not fit the reserve is searched in global memory
-      int st = 0;
-      uint32_t pm = 0, lm = 0, shm = 0, gm = 0;
-      for (int s = 0; s < n_term; ++s) {
-        const int k = sm.s_kind[s];
-        if (k == kPlane) pm |= 1u << s;
-        else if (k == kLong) lm |= 1u << s;
-        else if (k == kShort) {
-          const uint32_t a = sm.s_ia[s], b = sm.s_ib[s];
-          const int need = (int)seg_n(a, b, sm.s_pbm[s]);
-          if (st + need <= kShortMax) { sm.s_sdelta[s] = st - seg_first(a, sm.s_pbm[s]); st += need; shm |= 1u << s; }
-          else { sm.s_kind[s] = kGlobal; gm |= 1u << s; }
-        }
-      }
-      if (sweep_warm) { st = 0; lm = 0; shm = 0; gm = 0; }   // the leading list is read in place, nothing is staged or searched
-      sm.short_total = st;
-      sm.plane_mask = pm; sm.long_mask = lm; sm.short_mask = shm; sm.global_mask = gm;
+      uint32_t pm = 0;
+      for (int s = 0; s < n_term; ++s) if (sm.pq.kind[s] == kPlane) pm |= 1u << s;
       uint32_t drv, ess;
+      int cnt_first = -1;
       if (kSimple && sweep_warm) {
         drv = ess = 1u << warm_slot;
-        for (int t = 0; t < n_term; ++t) { sm.s_candbelow[t] = 0u; sm.s_cntbefore[t] = 0xffffffffu; sm.s_need[t] = pm & ~(1u << t); }   // (cntbefore: nothing is counted)
+        if (t < n_term) { sm.s_candbelow[t] = 0u; sm.s_cntbefore[t] = 0xffffffffu; sm.s_need[t] = pm & ~(1u << t); }   // (cntbefore: nothing is counted)
       } else if (kSimple) {
         ess = all & ~ne;
-        int cnt_first = -1;
         if (complete && ne && !L.ix.live_bits) {   // the densest non-essential list with a plane contributes its posting count unread
           uint32_t best = 0;
           for (int s = 0; s < n_term; ++s)
-            if (((ne >> s) & 1u) && sm.s_kind[s] == kPlane && sm.s_ib[s] - sm.s_ia[s] >= best) { best = sm.s_ib[s] - sm.s_ia[s]; cnt_first = s; }
+            if (((ne & pm) >> s) & 1u) { const uint32_t n = sm.s_ib[s] - sm.s_ia[s]; if (n >= best) { best = n; cnt_first = s; } }
         }
         drv = complete ? (cnt_first >= 0 ? all & ~(1u << cnt_first) : all) : ess;
-        for (int t = 0; t < n_term; ++t) {
-          uint32_t below_ess = 0, before_cnt = 0;
-          for (int s = 0; s < t; ++s) {
-            if ((ess >> s) & 1u) below_ess |= 0xffu << (8 * s);
-            if (s != cnt_first) before_cnt |= 0xffu << (8 * s);
-          }
-          if (cnt_first >= 0 && cnt_first != t) before_cnt |= 0xffu << (8 * cnt_first);
+        if (t < n_term) {
+          const uint32_t lower = (1u << t) - 1u;   // the slots before t
+          const uint32_t first = cnt_first >= 0 ? 1u << cnt_first : 0u;
+          const uint32_t below_ess = expand4(ess & lower);
+          const uint32_t before_cnt = expand4((lower | first) & ~(1u << t));
           sm.s_candbelow[t] = below_ess;
           sm.s_cntbefore[t] = complete ? before_cnt : below_ess;
-          uint32_t need = all & ~(1u << t);
-          if (complete && !((ess >> t) & 1u)) {   // a non-essential list is swept only to count: probe the earlier lists
-            need = 0;
-            for (int s = 0; s < n_term; ++s) if (s != t && (s == cnt_first || s < t)) need |= 1u << s;
-          }
-          sm.s_need[t] = need;
+          // a non-essential list is swept only to count: it probes the earlier lists (and the one counted unread)
+          sm.s_need[t] = (complete && !((ess >> t) & 1u)) ? ((lower | first) & ~(1u << t)) : (all & ~(1u << t));
         }
-        if (complete && cnt_first >= 0 && g_lo < g_hi)
-          atomicAdd(&L.total_hits[qi], (unsigned long long)(sm.s_ib[cnt_first] - sm.s_ia[cnt_first]));
       } else {
-        ess = sm.q.dense_driver ? 0u : (sm.q.driver_mask & all);   // dense: every doc of the slice is visited, all lists are probed
+        ess = sm.pq.q.dense_driver ? 0u : (sm.pq.q.driver_mask & all);   // dense: every doc of the slice is visited, all lists are probed
         drv = ess;
-        for (int t = 0; t < n_term; ++t) {
-          uint32_t below = 0;
-          for (int s = 0; s < t; ++s) if ((drv >> s) & 1u) below |= 0xffu << (8 * s);
+        if (t < n_term) {
+          const uint32_t below = expand4(drv & ((1u << t) - 1u));
           sm.s_candbelow[t] = below; sm.s_cntbefore[t] = below;
           sm.s_need[t] = all & ~(1u << t);
         }
       }
-      sm.drv_mask = drv; sm.ess_mask = ess;
+      // sweep warm-up: a list without a plane is not probed and counts as absent (scores are lower bounds), nothing is
+      // narrowed by granule. The record's ubt still holds: a slot that is not probed has tf code 0 in every table index,
+      // and the pattern sums of such indexes add (double)0 for it whatever its kind.
+      __syncwarp((1u << kT) - 1u);   // every lane has read the record's kinds
+      if (sweep_warm) {
+        if (sm.pq.kind[t] != kPlane && t != warm_slot) sm.pq.kind[t] = kAbsent;
+        sm.pq.row[t] = -1;
+      }
+      __syncwarp((1u << kT) - 1u);
+      if (t == 0) {
+        if (ne && !complete) L.pruned[qi] = 1;
+        // short lists are staged whole at the first run; what does not fit the reserve is searched in global memory
+        int st = 0;
+        uint32_t lm = 0, shm = 0, gm = 0;
+        for (int s = 0; s < n_term; ++s) {
+          const int k = sm.pq.kind[s];
+          if (k == kLong) lm |= 1u << s;
+          else if (k == kShort) {
+            const uint32_t a = sm.s_ia[s], b = sm.s_ib[s];
+            const int need = (int)seg_n(a, b, sm.pq.pbm[s]);
+            if (st + need <= kShortMax) { sm.s_sdelta[s] = st - seg_first(a, sm.pq.pbm[s]); st += need; shm |= 1u << s; }
+            else { sm.pq.kind[s] = kGlobal; gm |= 1u << s; }
+          }
+        }
+        if (sweep_warm) { st = 0; lm = 0; shm = 0; gm = 0; }   // the leading list is read in place, nothing is staged or searched
+        sm.short_total = st;
+        sm.plane_mask = pm; sm.long_mask = lm; sm.short_mask = shm; sm.global_mask = gm;
+        if (cnt_first >= 0 && g_lo < g_hi)
+          atomicAdd(&L.total_hits[qi], (unsigned long long)(sm.s_ib[cnt_first] - sm.s_ia[cnt_first]));
+        sm.drv_mask = drv; sm.ess_mask = ess;
+      }
     }
-    __syncthreads();   // B3: roles, staging plan
+    __syncthreads();   // B2: roles, staging plan
 
     const int32_t slice_base = slice * L.slice_docs;
     const uint32_t drv_mask = sm.drv_mask, ess_mask = sm.ess_mask;
@@ -480,7 +451,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     long long dbg_tflush = 0, dbg_twait = 0;
     const long long t_setup = kStats ? clock64() : 0ll;
 
-    const bool dense = !kSimple && sm.q.dense_driver != 0;
+    const bool dense = !kSimple && sm.pq.q.dense_driver != 0;
     const uint32_t* live = L.ix.live_bits;
     const uint32_t sort_missing = (!kSimple && L.sort_kind == NRTGPU_SORT_COLUMN) ? *L.sort_missing_code : 0u;
     int g0 = g_lo;
@@ -495,7 +466,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
           int tot = 0;
 #pragma unroll
           for (int s = 0; s < kT; ++s)
-            if ((long_mask >> s) & 1u) tot += (int)seg_n(sm.gb[s][g0], sm.gb[s][g1], sm.s_pbm[s]);
+            if ((long_mask >> s) & 1u) tot += (int)seg_n(sm.gb[s][g0], sm.gb[s][g1], sm.pq.pbm[s]);
           return tot <= cap;
         };
         int hi = g_hi, lo = g0 + 1;
@@ -513,9 +484,9 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
         // run bounds of every list: skip data where the list has it, else a search by doc (staged short lists: in shared
         // memory once resident -- their first-run bounds are fixed up below; lists read from global memory: there)
         for (int s = 0; s < n_term; ++s) {
-          const int k = sm.s_kind[s];
+          const int k = sm.pq.kind[s];
           uint32_t a = sm.s_ia[s], b = sm.s_ib[s];
-          if (sm.s_row[s] >= 0) { a = max(a, sm.gb[s][g0]); b = min(b, sm.gb[s][g1]); }
+          if (sm.pq.row[s] >= 0) { a = max(a, sm.gb[s][g0]); b = min(b, sm.gb[s][g1]); }
           else if (!whole && b > a) {
             if (k == kShort) {
               if (!first_run) {
@@ -528,7 +499,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
                 a = na; b = (uint32_t)(l - base);
               }
             } else {   // kPlane without skip data, kGlobal
-              const int32_t* gd = sm.s_gdocs[s];
+              const int32_t* gd = sm.pq.gdocs[s];
               uint32_t l = a, h = b;
               while (l < h) { const uint32_t m = (l + h) >> 1; if (__ldg(gd + m) < d0) l = m + 1; else h = m; }
               const uint32_t na = l;
@@ -544,20 +515,20 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
         uint32_t total = 0;
         if (first_run)
           for (int s = 0; s < n_term; ++s)
-            if ((short_mask >> s) & 1u) total += seg_n(sm.s_ia[s], sm.s_ib[s], sm.s_pbm[s]) * 5u;
+            if ((short_mask >> s) & 1u) total += seg_n(sm.s_ia[s], sm.s_ib[s], sm.pq.pbm[s]) * 5u;
         for (int s = 0; s < n_term; ++s)
-          if ((long_mask >> s) & 1u) total += seg_n(sm.s_ra[s], sm.s_rb[s], sm.s_pbm[s]) * 5u;
+          if ((long_mask >> s) & 1u) total += seg_n(sm.s_ra[s], sm.s_rb[s], sm.pq.pbm[s]) * 5u;
         sm.staged = total != 0u;
         if (total) {
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy reads of the stage precede the async writes
           mbar_arrive_expect_tx(&sm.stage_bar, total);
           auto stage = [&](int s, uint32_t a, uint32_t b, int at) {   // copy the aligned range around [a, b) to sdocs/sf8[at...]
-            const uint32_t pbm = sm.s_pbm[s];
+            const uint32_t pbm = sm.pq.pbm[s];
             const int32_t f = seg_first(a, pbm);
             const uint32_t n = seg_n(a, b, pbm);
             sm.s_sdelta[s] = at - f;
-            const unsigned char* gd = reinterpret_cast<const unsigned char*>(sm.s_gdocs[s] + f);
-            const unsigned char* gf = reinterpret_cast<const unsigned char*>(sm.s_gf8[s] + f);
+            const unsigned char* gd = reinterpret_cast<const unsigned char*>(sm.pq.gdocs[s] + f);
+            const unsigned char* gf = reinterpret_cast<const unsigned char*>(sm.pq.gf8[s] + f);
             unsigned char* dd = reinterpret_cast<unsigned char*>(&sm.sdocs[at]);
             unsigned char* df = reinterpret_cast<unsigned char*>(&sm.sf8[at]);
             for (uint32_t o = 0; o < n * 4u; o += kPiece) bulk_g2s(dd + o, gd + o, min(kPiece, n * 4u - o), &sm.stage_bar);
@@ -567,7 +538,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
           if (first_run)
             for (int s = 0; s < n_term; ++s)
               if (((short_mask >> s) & 1u) && sm.s_ib[s] > sm.s_ia[s])
-                stage(s, sm.s_ia[s], sm.s_ib[s], sm.s_sdelta[s] + seg_first(sm.s_ia[s], sm.s_pbm[s]));
+                stage(s, sm.s_ia[s], sm.s_ib[s], sm.s_sdelta[s] + seg_first(sm.s_ia[s], sm.pq.pbm[s]));
           int st = sm.short_total;
           for (int s = 0; s < n_term; ++s)
             if (((long_mask >> s) & 1u) && sm.s_rb[s] > sm.s_ra[s]) st += stage(s, sm.s_ra[s], sm.s_rb[s], st);
@@ -623,7 +594,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       // The queue is drained 32 entries at a time; qn is warp-uniform.
       uint2* const wq = sm.wq[tid >> 5];
       int qn = 0;
-      const uint32_t q_req = sm.q.req_term_mask, q_not = sm.q.not_term_mask;
+      const uint32_t q_req = sm.pq.q.req_term_mask, q_not = sm.pq.q.not_term_mask;
       auto drain = [&](int n_take) -> bool {   // evaluates the last n_take (<= 32) queued pairs; true: a lane had to park its key
         __syncwarp();
         bool fail = false;
@@ -634,7 +605,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
         uint64_t entry = 0ull;   // a real key is never 0: 0 fails the threshold test below
         if (kSimple) {
           if (have) {   // (the query's norms and after key are read here: registers are scarce across the rounds)
-            const uint8_t* norms0 = sm.q.single_field >= 0 ? L.ix.norms[sm.q.single_field] : nullptr;
+            const uint8_t* norms0 = sm.pq.q.single_field >= 0 ? L.ix.norms[sm.pq.q.single_field] : nullptr;
             entry = make_key(score_disjunction(L, sm, norms0, n_term, d, e.y), d);
           }
         } else {
@@ -655,7 +626,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
         }
         // sm.theta never decreases within an item, so a key dropped here would not survive a flush either
         const unsigned long long th = sm.theta;
-        if (entry > th && !(sm.q.has_after && !(entry < sm.q.after_key)) && !NRT_KNOCK(4)) {
+        if (entry > th && !(sm.pq.q.has_after && !(entry < sm.pq.q.after_key)) && !NRT_KNOCK(4)) {
           if (kStats) ++dbg_admit;
           const int p = atomicAdd(&sm.cand_count, 1);
           if (p < kCand) sm.cand[p] = entry;
@@ -689,8 +660,8 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
           const int32_t dense_d0 = sm.run_d0;
           const int32_t* sdoc_t = sm.sdocs + ((int)sm.s_ra[t] + sm.s_sdelta[t]);   // posting x of the run segment: sdoc_t[x]
           const uint8_t* sf8_t = sm.sf8 + ((int)sm.s_ra[t] + sm.s_sdelta[t]);
-          const int32_t* gdoc_t = sm.s_gdocs[t] + sm.s_ra[t];
-          const uint8_t* gf8_t = sm.s_gf8[t] + sm.s_ra[t];
+          const int32_t* gdoc_t = sm.pq.gdocs[t] + sm.s_ra[t];
+          const uint8_t* gf8_t = sm.pq.gf8[t] + sm.s_ra[t];
           const uint32_t tshift = t_dense ? 0u : 8u * (uint32_t)t;
           // software pipeline: the postings of the NEXT round are fetched before the current round is processed
           // (generic pointers: one load path for staged -- shared memory -- and plane / global -- HBM -- driver lists)
@@ -718,10 +689,10 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
             for (int j = 0; j < kR; ++j) {
               const uint32_t d4 = (uint32_t)max(doc[j], 0) >> 2;
               pbyte[j][0] = 0u; pbyte[j][1] = 0u; pbyte[j][2] = 0u; pbyte[j][3] = 0u;
-              if (need_plane & 1u) pbyte[j][0] = (uint32_t)__ldg(sm.s_plane2[0] + d4);
-              if (need_plane & 2u) pbyte[j][1] = (uint32_t)__ldg(sm.s_plane2[1] + d4);
-              if (need_plane & 4u) pbyte[j][2] = (uint32_t)__ldg(sm.s_plane2[2] + d4);
-              if (need_plane & 8u) pbyte[j][3] = (uint32_t)__ldg(sm.s_plane2[3] + d4);
+              if (need_plane & 1u) pbyte[j][0] = (uint32_t)__ldg(sm.pq.plane2[0] + d4);
+              if (need_plane & 2u) pbyte[j][1] = (uint32_t)__ldg(sm.pq.plane2[1] + d4);
+              if (need_plane & 4u) pbyte[j][2] = (uint32_t)__ldg(sm.pq.plane2[2] + d4);
+              if (need_plane & 8u) pbyte[j][3] = (uint32_t)__ldg(sm.pq.plane2[3] + d4);
             }
             // next round's postings
             {
@@ -750,7 +721,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
                   } else if ((need_short >> u) & 1u) {
                     if (sm.s_rb[u] > sm.s_ra[u]) b = probe_smem(sm, (int)sm.s_ra[u] + sm.s_sdelta[u], (int)sm.s_rb[u] + sm.s_sdelta[u], doc[j]);
                   } else if ((need_glob >> u) & 1u) {
-                    if (sm.s_rb[u] > sm.s_ra[u]) b = probe_global(sm.s_gdocs[u], sm.s_gf8[u], sm.s_ra[u], sm.s_rb[u], doc[j]);
+                    if (sm.s_rb[u] > sm.s_ra[u]) b = probe_global(sm.pq.gdocs[u], sm.pq.gf8[u], sm.s_ra[u], sm.s_rb[u], doc[j]);
                   }
                   word[j] |= b << (8 * u);
                 }
@@ -777,7 +748,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
                 // tf-pattern bound is below the threshold cannot reach the top-k
                 if (doc[j] >= 0 && !(live && !((live[doc[j] >> 5] >> (doc[j] & 31)) & 1u))) {
                   if ((v & cntbefore) == 0u) ++my_hits;
-                  surv = t_ess && (v & candbelow) == 0u && !(sm.ubt[__dp4a(__vminu4(v, 0x03030303u), 0x40100401u, 0u)] < theta_s);
+                  surv = t_ess && (v & candbelow) == 0u && !(sm.pq.ubt[__dp4a(__vminu4(v, 0x03030303u), 0x40100401u, 0u)] < theta_s);
                 }
               } else {   // not owned by a lower list, every required term present, no excluded term
                 const uint32_t pres = presence4(v);
@@ -885,6 +856,79 @@ __global__ void slice_bounds_kernel(SliceBoundsLaunch B) {
     break;
   }
   B.sbounds[i] = out;
+}
+
+// the per-query records of a probe batch (DevProbeQuery, batch_plan.h): one CTA per query, once per prepared batch
+struct ProbeQueryLaunch {
+  DevIndexView ix;
+  const DevClause* clauses;
+  const DevQuery* queries;
+  const uint8_t* field_min_norm;
+  DevProbeQuery* out;   // [nq]
+};
+
+__global__ void __launch_bounds__(kUbt) probe_query_kernel(ProbeQueryLaunch B) {
+  __shared__ DevProbeQuery r;
+  __shared__ float uval[kT][2];   // per-slot score bounds at tf = 1, 2 (shortest field length present)
+  const int qi = blockIdx.x, tid = threadIdx.x;
+  const DevQuery dq = B.queries[qi];
+  const int ncl = dq.n_clauses, n_term = dq.n_term;
+  if (tid == 0) r.q = dq;
+  if (tid < kMaxClauses) r.cl[tid] = tid < ncl ? B.clauses[dq.clause_begin + tid] : DevClause{};
+  if (tid >= 32 && tid < 32 + kT) {
+    const int s = tid - 32;
+    r.kind[s] = kAbsent; r.plane[s] = nullptr; r.plane2[s] = nullptr; r.gdocs[s] = nullptr; r.gf8[s] = nullptr;
+    r.weight[s] = 0.f; r.ub[s] = 0.f; r.clause[s] = 0; r.field[s] = 0; r.pbm[s] = 0; r.row[s] = -1; r.ord[s] = 0; r.pre[s] = 0.f;
+  }
+  __syncthreads();
+  if (tid < ncl && r.cl[tid].kind == NRTGPU_TERM) {   // per-slot descriptors (one thread per clause)
+    const DevClause& c = r.cl[tid];
+    const int s = c.slot;
+    r.gdocs[s] = B.ix.post_docs + c.post_base;
+    r.gf8[s] = B.ix.post_f8 + c.post_base;
+    const bool has_plane = c.plane >= 0 && B.ix.dense_tf != nullptr && B.ix.dense_tf2 != nullptr;
+    r.plane[s] = has_plane ? B.ix.dense_tf + (size_t)c.plane * (size_t)B.ix.dense_stride : nullptr;
+    r.plane2[s] = has_plane ? B.ix.dense_tf2 + (size_t)c.plane * (size_t)(B.ix.dense_stride >> 2) : nullptr;
+    r.kind[s] = has_plane ? kPlane : (c.gran_row >= 0 ? kLong : kShort);
+    r.weight[s] = c.weight; r.ub[s] = c.ub; r.clause[s] = tid; r.field[s] = c.field;
+    r.pbm[s] = (uint32_t)(c.post_base & (int64_t)(kAlign - 1)); r.row[s] = c.gran_row;
+  }
+  if (tid >= 64 && tid < 64 + 2 * kT) {
+    const int s = (tid - 64) >> 1, c = ((tid - 64) & 1) + 1;
+    float u = 0.0f;
+    for (int i = 0; i < ncl; ++i)
+      if (r.cl[i].kind == NRTGPU_TERM && r.cl[i].slot == s) {
+        const uint32_t nbmin = (dq.single_field >= 0 && B.field_min_norm) ? (uint32_t)B.field_min_norm[dq.single_field] : 0u;
+        u = bm25_score(r.cl[i].weight, (float)c, __ldg(&B.ix.caches[r.cl[i].field * 256 + nbmin]));
+      }
+    uval[s][c - 1] = u;
+  }
+  __syncthreads();
+  {
+    // ubt[sum min(tf_s, 3) * 4^s]: the double clause sum with every term at the shortest field length present
+    // (tf >= 3 bounded by the clause weight, the limit tf -> inf) -- an upper bound of the doc's score
+    const int i = tid;
+    const int c[kT] = {i & 3, (i >> 2) & 3, (i >> 4) & 3, i >> 6};
+    double sum = 0.0;
+#pragma unroll
+    for (int t = 0; t < kT; ++t) {
+      float u = 0.0f;
+      if (r.kind[t] != kAbsent && c[t] > 0) u = (c[t] <= 2) ? uval[t][c[t] - 1] : r.weight[t];
+      sum += (double)u;
+    }
+    r.ubt[i] = (float)sum;
+  }
+  if (tid == 0) {   // MAXSCORE order: insertion sort by ub (equal bounds keep slot order), running double sums
+    int ord[kT]; int n = 0;
+    for (int s = 0; s < n_term; ++s) ord[n++] = s;
+    for (int a = 1; a < n; ++a) { const int x = ord[a]; int b = a - 1; while (b >= 0 && r.ub[ord[b]] > r.ub[x]) { ord[b + 1] = ord[b]; --b; } ord[b + 1] = x; }
+    double pre = 0.0;
+    for (int a = 0; a < n; ++a) { pre += (double)r.ub[ord[a]]; r.ord[a] = ord[a]; r.pre[a] = (float)pre; }
+  }
+  __syncthreads();
+  const uint4* src = reinterpret_cast<const uint4*>(&r);
+  uint4* dst = reinterpret_cast<uint4*>(B.out + qi);
+  for (int i = tid; i < (int)(sizeof(DevProbeQuery) / 16); i += kUbt) dst[i] = src[i];
 }
 
 }  // namespace v3
