@@ -375,6 +375,58 @@ int nrtgpu_search_bool_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int3
                             void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
                             int64_t* out_total_hits);
 
+/* Nested collectors of a terms aggregation (search.proto Collector.nestedCollectors, CollectorCreator.java:73-126): each
+ * is computed per bucket over exactly the docs its parent bucket counts (matching, live, with a value in the parent
+ * column). A terms aggregation (aggs[parent]) carries up to 4:
+ *   NRTGPU_AGG_MIN / _MAX / _SUM   over a single-valued column, with the rules of the top-level ones above (started from
+ *                     +/-Double.MAX_VALUE, NaN never wins, the same sum bound); a bucket with no value in the column keeps
+ *                     the unset value (Double.MAX_VALUE / -Double.MAX_VALUE / 0.0);
+ *   NRTGPU_AGG_TOP_HITS  TopScoreDocCollectorManager(top_hits, null, Integer.MAX_VALUE) per bucket
+ *                     (TopHitsCollectorManager.java:126-130): hits by score descending, then global doc ascending; positions
+ *                     [start_hit, top_hits) are returned (:162), totalHits is the bucket's count (EQUAL_TO), and a score is
+ *                     the float the top-level hit list gives that doc. Valid only as a nested kind.
+ * orders_parent: at most one nested MIN / MAX / SUM of a parent orders its buckets instead of the count (BucketOrder by a
+ * nested collector's name, TermsCollectorManager.fillBucketResultByNestedOrder :930-994), in the parent's order_desc
+ * direction by Double.compare; ties, unordered in the reference's heap, go to the smaller bucket value; a bucket without
+ * values takes part with the unset value. totalBuckets and totalOtherCounts keep their meaning.
+ * Results are per returned bucket (the parent's `size` slots; entries past its n_buckets are 0):
+ *   values [nq*size]   MIN / MAX / SUM of the bucket;
+ *   TOP_HITS: hit_docs (global ids) / hit_scores [nq*size*(top_hits-start_hit)], hit_counts [nq*size] hits returned,
+ *   hit_total [nq*size] the bucket's count.
+ * Top hits are collected exactly in a second run of the batch's probe launch, after the buckets are chosen: the keys
+ * (score, doc) of every collected doc of a returned bucket go into a buffer sized by the bucket's count, then one CTA per
+ * bucket selects its best top_hits. The second run writes none of the request's hits, totalHits or aggregation tables.
+ * When the buffers of the batch exceed 512 MB (2^26 keys) the second run goes over groups of queries.
+ * nrtgpu_search_bool_aggs_nested: nrtgpu_search_bool_aggs (every refusal, the same hits and results) plus the nested
+ * collectors; with n_nested == 0 it is nrtgpu_search_bool_aggs.
+ *   NRTGPU_ERR_INVALID: a parent out of range or not a terms aggregation, a bad kind or value_type, a column out of range,
+ *     start_hit outside [0, top_hits), two orders_parent on one parent (or on a TOP_HITS);
+ *   NRTGPU_ERR_UNSUPPORTED: more than 4 nested collectors on a parent, a multi-valued nested column, top_hits > 1024,
+ *     a batch x distinct values table of a nested metric over 2 GB, top-hit outputs over 2^24 entries per collector
+ *     (nq * size * top_hits), a single query whose returned buckets hold more than 2^26 keys. */
+enum { NRTGPU_AGG_TOP_HITS = 5 };
+typedef struct {
+  int32_t parent;         /* index into aggs[] of the terms aggregation */
+  int32_t kind;           /* NRTGPU_AGG_MIN / _MAX / _SUM / _TOP_HITS */
+  int32_t column, value_type;   /* MIN / MAX / SUM */
+  int32_t top_hits, start_hit;  /* TOP_HITS */
+  int32_t orders_parent;  /* MIN / MAX / SUM: 1 = the parent's buckets are ordered by this value */
+  int32_t reserved;
+} nrtgpu_nested_aggregation;
+typedef struct {          /* caller-allocated outputs of one nested collector (unused pointers may be NULL) */
+  double* values;         /* [nq*size] */
+  int32_t* hit_docs;      /* [nq*size*(top_hits-start_hit)] */
+  float* hit_scores;      /* [nq*size*(top_hits-start_hit)] */
+  int32_t* hit_counts;    /* [nq*size] */
+  int64_t* hit_total;     /* [nq*size] */
+} nrtgpu_nested_result;
+int nrtgpu_search_bool_aggs_nested(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                   const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                   const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                                   const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                   const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs,
+                                   float* out_scores, int32_t* out_counts, int64_t* out_total_hits);
+
 /* QueryRescorer second pass (QueryRescore.java:39-57 -> Lucene QueryRescorer.rescore): query q of the batch evaluated on
  * ITS OWN hit list docs[q][0..counts[q]) (global doc ids): out_matches / out_scores [nq*n_hits]. */
 int nrtgpu_score_docs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,

@@ -115,6 +115,16 @@ public final class NrtGpu {
       ByteBuffer phraseTerms, int nPhraseTerms, ByteBuffer queries, int nq, int nHits, ByteBuffer counts, int window,
       double queryWeight, double rescoreWeight, ByteBuffer docs, ByteBuffer scores, ByteBuffer outCounts);
 
+  /**
+   * Additional collectors with nested collectors (nrtgpu_search_bool_aggs_nested): aggs = nAggs nrtgpu_aggregation, nested =
+   * nNested nrtgpu_nested_aggregation; aggOut holds 6 buffers (or null) per aggregation in nrtgpu_aggregation_result field
+   * order, nestedOut 5 per nested collector in nrtgpu_nested_result field order.
+   */
+  public static native int searchBoolAggsNested(
+      long index, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK, int flags, ByteBuffer aggs,
+      int nAggs, ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, ByteBuffer outDocs,
+      ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits);
+
   public static native int fetchColumns(
       long index, ByteBuffer colIds, int nCols, ByteBuffer docs, int n, ByteBuffer outValues,
       ByteBuffer outHas);

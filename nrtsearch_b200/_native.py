@@ -90,6 +90,16 @@ class AggregationResult(C.Structure):
                 ("total_buckets", C.c_void_p), ("other_counts", C.c_void_p)]
 
 
+class NestedAggregation(C.Structure):
+    _fields_ = [("parent", C.c_int32), ("kind", C.c_int32), ("column", C.c_int32), ("value_type", C.c_int32),
+                ("top_hits", C.c_int32), ("start_hit", C.c_int32), ("orders_parent", C.c_int32), ("reserved", C.c_int32)]
+
+
+class NestedResult(C.Structure):
+    _fields_ = [("values", C.c_void_p), ("hit_docs", C.c_void_p), ("hit_scores", C.c_void_p), ("hit_counts", C.c_void_p),
+                ("hit_total", C.c_void_p)]
+
+
 class Query(C.Structure):
     _fields_ = [("clause_begin", C.c_int32), ("clause_end", C.c_int32), ("min_should_match", C.c_int32),
                 ("has_after", C.c_int32), ("after_doc", C.c_int32), ("after_score", C.c_float)]
@@ -123,6 +133,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_search_tree", "nrtgpu_batch_prepare_tree",
     "nrtgpu_index_add_positions", "nrtgpu_search_tree_phrases", "nrtgpu_batch_prepare_tree_phrases",
     "nrtgpu_score_docs_tree", "nrtgpu_rescore_query_tree",
+    "nrtgpu_search_bool_aggs_nested",
 ]
 
 _gpu = None
@@ -190,6 +201,10 @@ def gpu_lib() -> C.CDLL:
                                                     C.c_int32, C.c_int32, C.c_void_p, C.POINTER(SearchLimits), C.c_void_p] + [C.c_void_p] * 7
         lib.nrtgpu_search_bool_aggs.argtypes =[C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32,
                                                 C.POINTER(Aggregation), C.c_int32, C.POINTER(AggregationResult), C.c_void_p] + [C.c_void_p] * 4
+        lib.nrtgpu_search_bool_aggs_nested.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32,
+                                                       C.c_int32, C.POINTER(Aggregation), C.c_int32, C.POINTER(AggregationResult),
+                                                       C.POINTER(NestedAggregation), C.c_int32, C.POINTER(NestedResult),
+                                                       C.c_void_p] + [C.c_void_p] * 4
         lib.nrtgpu_score_docs.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.nrtgpu_rescore_query.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32, C.c_void_p,

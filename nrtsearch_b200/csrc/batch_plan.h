@@ -29,6 +29,10 @@ constexpr int kWideSliceDocs = kSliceWindows * kWindowDocs;   // => 1,048,576 do
 constexpr int kMaxTopK = 1024;
 constexpr int kMaxAggs = 8;         // aggregations per search
 constexpr int kAggChunk = 2048;     // largest size of a terms aggregation (agg_terms_topk_kernel)
+constexpr int kMaxNested = 4;       // nested collectors per terms aggregation
+constexpr int kMaxNestedTopHits = 1024;               // top_hits of a nested top-hits collector (nested_top_hits_kernel)
+constexpr int64_t kMaxNestedHitOutputs = 1ll << 24;   // nq * size * top_hits of one nested top-hits collector
+constexpr int64_t kNestedHitBudget = 1ll << 26;       // keys (8 B) of one pass-2 group of a batch's nested top hits
 
 struct DevClause {
   int64_t post_base;  // offset of the term's postings in post_docs / post_f8

@@ -189,10 +189,24 @@ struct AggSpecDev {
   unsigned int* counts;        // terms: [nq][n_buckets]
   unsigned long long* dvals;   // min / max: ordered-double bits [nq]; sum: double bits [nq] (atomicAdd(double))
 };
+// a nested collector of a terms aggregation, at the parent's (query, bucket) cell
+struct AggNestedDev {
+  int32_t kind;                 // NRTGPU_AGG_MIN / _MAX / _SUM (pass 1) or NRTGPU_AGG_TOP_HITS (pass 2)
+  int32_t column, value_type;   // MIN / MAX / SUM
+  int32_t size;                 // TOP_HITS: the parent's size (slots per query)
+  int32_t q_lo, q_hi;           // TOP_HITS: the queries of this pass-2 group
+  unsigned long long* dvals;    // MIN / MAX / SUM: [nq][n_buckets] words as AggSpecDev::dvals
+  const int32_t* slot_of;       // TOP_HITS: [nq][n_buckets] returned slot of the bucket, -1: not returned
+  const long long* hit_off;     // TOP_HITS: [q_hi - q_lo][size] first key of the (query, slot)
+  unsigned int* hit_fill;       // TOP_HITS: [q_hi - q_lo][size] keys written
+  uint64_t* hit_keys;           // TOP_HITS: make_key(score, doc) of the collected docs
+};
 struct AggLaunch {
   AggSpecDev a[kMaxAggs];
   int32_t n_aggs;
   const uint32_t* codes[kMaxAggs];   // terms: sort codes of the column (bucket = code / 2 - 1)
+  int32_t nested_begin[kMaxAggs + 1];   // terms: nested[nested_begin[i], nested_begin[i + 1]) are aggregation i's
+  AggNestedDev nested[kMaxAggs * kMaxNested];
 };
 
 __device__ __forceinline__ unsigned long long double_to_ordered(double d) {
@@ -210,25 +224,65 @@ __host__ __device__ __forceinline__ double ordered_to_double(unsigned long long 
   return d;
 }
 
-// called by the posting kernels for every matching doc of query q
-__device__ __forceinline__ void agg_collect(const AggLaunch& A, const DevIndexView& ix, int q, int32_t doc) {
+// a min / max / sum collector's word takes the doc's value in `column`, if it has one
+__device__ __forceinline__ void agg_metric_collect(int kind, int column, int value_type, unsigned long long* w,
+                                                   const DevIndexView& ix, int32_t doc) {
+  const uint8_t* has = ix.col_has[column];
+  if (has && !has[doc]) return;   // LoadedDocValues.size() == 0: nothing to collect for this doc
+  const int64_t raw = ix.col32[column] ? (int64_t)ix.col32[column][doc] : ix.col64[column][doc];
+  const double v = agg_value(raw, value_type);
+  // Max/MinCollectorManager keep `value > maxValue` (`value < minValue`) started from -/+Double.MAX_VALUE: NaN and the
+  // infinity on the unset side never win
+  if (kind == NRTGPU_AGG_MAX) { if (v > -DBL_MAX) atomicMax(w, double_to_ordered(v)); }
+  else if (kind == NRTGPU_AGG_MIN) { if (v < DBL_MAX) atomicMin(w, double_to_ordered(v)); }
+  else atomicAdd(reinterpret_cast<double*>(w), v);
+}
+
+// the nested collectors of a terms aggregation for a doc counted in bucket cell (q * n_buckets + bucket)
+__device__ __noinline__ void agg_nested_collect(const AggLaunch& A, int i, const DevIndexView& ix, int q, size_t cell,
+                                                int32_t doc, float score) {
+  for (int j = A.nested_begin[i]; j < A.nested_begin[i + 1]; ++j) {
+    const AggNestedDev& n = A.nested[j];
+    if (n.kind != NRTGPU_AGG_TOP_HITS) { agg_metric_collect(n.kind, n.column, n.value_type, n.dvals + cell, ix, doc); continue; }
+    if (q < n.q_lo || q >= n.q_hi) continue;
+    const int slot = n.slot_of[cell];
+    if (slot < 0) continue;
+    const size_t s = (size_t)(q - n.q_lo) * n.size + slot;
+    n.hit_keys[n.hit_off[s] + atomicAdd(&n.hit_fill[s], 1u)] = make_key(score, doc);   // sized by the bucket's count
+  }
+}
+
+// called by the posting kernels for every matching doc of query q (score: its score under a relevance sort)
+__device__ __forceinline__ void agg_collect(const AggLaunch& A, const DevIndexView& ix, int q, int32_t doc, float score) {
   for (int i = 0; i < A.n_aggs; ++i) {
     const AggSpecDev& s = A.a[i];
-    const uint8_t* has = ix.col_has[s.column];
-    if (has && !has[doc]) continue;   // LoadedDocValues.size() == 0: nothing to collect for this doc
     if (s.kind == NRTGPU_AGG_TERMS) {
+      const uint8_t* has = ix.col_has[s.column];
+      if (has && !has[doc]) continue;
       const uint32_t code = A.codes[i][doc];
-      if (code) atomicAdd(&s.counts[(size_t)q * s.n_buckets + (code >> 1) - 1], 1u);
+      if (!code) continue;
+      const size_t cell = (size_t)q * s.n_buckets + (code >> 1) - 1;
+      if (s.counts) atomicAdd(&s.counts[cell], 1u);   // (NULL in the top-hits run)
+      if (A.nested_begin[i + 1] > A.nested_begin[i]) agg_nested_collect(A, i, ix, q, cell, doc, score);
     } else {
-      const int64_t raw = ix.col32[s.column] ? (int64_t)ix.col32[s.column][doc] : ix.col64[s.column][doc];
-      const double v = agg_value(raw, s.value_type);
-      // Max/MinCollectorManager keep `value > maxValue` (`value < minValue`) started from -/+Double.MAX_VALUE: NaN and the
-      // infinity on the unset side never win
-      if (s.kind == NRTGPU_AGG_MAX) { if (v > -DBL_MAX) atomicMax(&s.dvals[q], double_to_ordered(v)); }
-      else if (s.kind == NRTGPU_AGG_MIN) { if (v < DBL_MAX) atomicMin(&s.dvals[q], double_to_ordered(v)); }
-      else atomicAdd(reinterpret_cast<double*>(&s.dvals[q]), v);
+      agg_metric_collect(s.kind, s.column, s.value_type, &s.dvals[q], ix, doc);
     }
   }
+}
+
+// the double a min / max / sum word stands for, the collectors' unset value where no doc had a value
+__host__ __device__ __forceinline__ double agg_word_value(int kind, unsigned long long w) {
+  if (kind == NRTGPU_AGG_SUM) {
+    double v;
+#ifdef __CUDA_ARCH__
+    v = __longlong_as_double((long long)w);
+#else
+    memcpy(&v, &w, sizeof(v));
+#endif
+    return v;
+  }
+  if (kind == NRTGPU_AGG_MAX) return w == 0ull ? -DBL_MAX : ordered_to_double(w);   // MaxCollectorManager.UNSET_VALUE
+  return w == ~0ull ? DBL_MAX : ordered_to_double(w);                                // MinCollectorManager.UNSET_VALUE
 }
 
 // terms aggregation result of one query: the `size` buckets with the largest (or smallest) counts
@@ -240,6 +294,7 @@ struct AggTermsLaunch {
   int32_t* out_n;             // [nq] buckets returned
   int32_t* out_total_buckets; // [nq] non-empty buckets
   long long* out_other;       // [nq] docs counted in buckets not returned
+  int32_t* out_bucket;        // optional [nq][size] bucket of each returned slot, -1 past out_n (nested collectors)
 };
 __global__ void __launch_bounds__(256) agg_terms_topk_kernel(AggTermsLaunch T) {
   __shared__ uint64_t keys[2 * kAggChunk];
@@ -286,11 +341,161 @@ __global__ void __launch_bounds__(256) agg_terms_topk_kernel(AggTermsLaunch T) {
       key = (int64_t)(T.distinct[bkt] ^ 0x8000000000000000ull);
     }
     T.out_keys[(size_t)q * T.size + i] = key; T.out_counts[(size_t)q * T.size + i] = cnt;
+    if (T.out_bucket) T.out_bucket[(size_t)q * T.size + i] = i < n_out ? (int32_t)~(uint32_t)keys[i] : -1;
   }
   if (tid == 0) {
     for (int i = 0; i < n_out; ++i) { const uint32_t hi = (uint32_t)(keys[i] >> 32); shown += T.order_desc ? hi : ~hi; }
     T.out_n[q] = n_out; T.out_total_buckets[q] = sh_nonzero; T.out_other[q] = (long long)(sh_sum - shown);
   }
+}
+
+// In-place bitonic sort of n (power of two) (key, tag) pairs in shared memory by the whole CTA, descending by key, then tag.
+__device__ __forceinline__ void block_bitonic_sort_pairs_desc(uint64_t* a, uint32_t* t, int n) {
+  for (int k = 2; k <= n; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = threadIdx.x; i < (n >> 1); i += blockDim.x) {
+        const int lo = ((i & ~(j - 1)) << 1) | (i & (j - 1)), hi = lo | j;
+        const bool desc = (lo & k) == 0;
+        const uint64_t x = a[lo], y = a[hi];
+        const uint32_t tx = t[lo], ty = t[hi];
+        if ((x < y || (x == y && tx < ty)) == desc) { a[lo] = y; a[hi] = x; t[lo] = ty; t[hi] = tx; }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// terms aggregation ordered by a nested min / max / sum (TermsCollectorManager.fillBucketResultByNestedOrder :930-994): the
+// `size` non-empty buckets whose value is largest (order_desc) or smallest by Double.compare, ties to the smaller bucket
+// value. Outputs as agg_terms_topk_kernel. Dynamic shared memory: kAggByValueSmem.
+constexpr int kAggByValueSmem = 2 * kAggChunk * (int)(sizeof(uint64_t) + sizeof(uint32_t));
+__global__ void __launch_bounds__(256) agg_terms_by_value_kernel(AggTermsLaunch T, const unsigned long long* words, int kind) {
+  extern __shared__ uint64_t dyn_keys[];
+  uint64_t* keys = dyn_keys;                                    // the value's Double.compare order (flipped for ASC)
+  uint32_t* tags = reinterpret_cast<uint32_t*>(dyn_keys + 2 * kAggChunk);   // ~bucket; 0: no bucket
+  __shared__ unsigned long long sh_sum;
+  __shared__ int sh_nonzero;
+  const int q = blockIdx.x, tid = threadIdx.x;
+  if (tid == 0) { sh_sum = 0ull; sh_nonzero = 0; }
+  __syncthreads();
+  const unsigned int* row = T.counts + (size_t)q * T.n_buckets;
+  const unsigned long long* wrow = words + (size_t)q * T.n_buckets;
+  int have = 0;
+  unsigned long long my_sum = 0; int my_nz = 0;
+  for (int base = 0; base < T.n_buckets; base += kAggChunk) {
+    for (int i = tid; i < kAggChunk; i += 256) {
+      const int bkt = base + i;
+      uint64_t k = 0ull; uint32_t g = 0u;
+      if (bkt < T.n_buckets) {
+        const unsigned int c = row[bkt];
+        if (c) {   // the reference's counts map holds the buckets with a doc
+          ++my_nz; my_sum += c;
+          double v = agg_word_value(kind, wrow[bkt]);
+          if (v != v) v = __longlong_as_double(0x7ff8000000000000ll);   // Double.compare: every NaN above +inf
+          const uint64_t o = double_to_ordered(v);
+          k = T.order_desc ? o : ~o;
+          g = ~(uint32_t)bkt;
+        }
+      }
+      keys[have + i] = k; tags[have + i] = g;
+    }
+    const int n = have + kAggChunk;
+    const int m = next_pow2(n);
+    for (int i = n + tid; i < m; i += 256) { keys[i] = 0ull; tags[i] = 0u; }
+    __syncthreads();
+    block_bitonic_sort_pairs_desc(keys, tags, m);
+    have = min(T.size, kAggChunk);
+    __syncthreads();
+  }
+  atomicAdd(&sh_sum, my_sum); atomicAdd(&sh_nonzero, my_nz);
+  __syncthreads();
+  int n_out = 0;
+  for (int i = 0; i < have; ++i) if (tags[i]) ++n_out; else break;
+  for (int i = tid; i < T.size; i += 256) {
+    int64_t key = 0; int32_t cnt = 0, bkt = -1;
+    if (i < n_out) {
+      bkt = (int32_t)~tags[i];
+      cnt = (int32_t)row[bkt];
+      key = (int64_t)(T.distinct[bkt] ^ 0x8000000000000000ull);
+    }
+    T.out_keys[(size_t)q * T.size + i] = key; T.out_counts[(size_t)q * T.size + i] = cnt;
+    if (T.out_bucket) T.out_bucket[(size_t)q * T.size + i] = bkt;
+  }
+  if (tid == 0) {
+    unsigned long long shown = 0;
+    for (int i = 0; i < n_out; ++i) shown += row[~tags[i]];
+    T.out_n[q] = n_out; T.out_total_buckets[q] = sh_nonzero; T.out_other[q] = (long long)(sh_sum - shown);
+  }
+}
+
+// per returned slot of a terms aggregation: the slot map of its buckets (top hits) and its nested min / max / sum values
+struct AggNestedOutLaunch {
+  const int32_t* bucket;      // [nq][size] (out_bucket of the selection)
+  int32_t nq, size, n_buckets;
+  int32_t* slot_of;           // optional [nq][n_buckets], preset to -1
+  int32_t n_vals;
+  int32_t kind[kMaxNested];
+  const unsigned long long* words[kMaxNested];   // [nq][n_buckets]
+  double* values[kMaxNested];                    // [nq][size]; 0 past the returned buckets
+};
+__global__ void agg_nested_out_kernel(AggNestedOutLaunch O) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= O.nq * O.size) return;
+  const int32_t b = O.bucket[i];
+  const size_t cell = (size_t)(i / O.size) * O.n_buckets + b;
+  if (O.slot_of && b >= 0) O.slot_of[cell] = i % O.size;
+  for (int j = 0; j < O.n_vals; ++j) O.values[j][i] = b >= 0 ? agg_word_value(O.kind[j], O.words[j][cell]) : 0.0;
+}
+
+// nested top hits of the returned buckets of one pass-2 group: one CTA per (query, slot) keeps the best top_hits keys of
+// its segment (a chunk is sorted only when one of its keys beats the current top_hits-th) and writes [start_hit, top_hits)
+struct NestedHitsLaunch {
+  const uint64_t* hit_keys;
+  const long long* hit_off;     // [group * size + 1]
+  const unsigned int* hit_fill; // [group * size]
+  int32_t q_lo, size, top_hits, start_hit, doc_base;
+  int32_t* out_docs; float* out_scores;   // [nq][size][top_hits - start_hit]
+  int32_t* out_counts;                    // [nq][size]
+};
+__global__ void __launch_bounds__(256) nested_top_hits_kernel(NestedHitsLaunch H) {
+  __shared__ uint64_t keys[2 * kAggChunk];   // the best (<= 1024) and a chunk's admitted keys
+  __shared__ int sh_new;
+  const int g = blockIdx.x, tid = threadIdx.x;
+  const long long off = H.hit_off[g];
+  const int n = (int)min((long long)H.hit_fill[g], H.hit_off[g + 1] - off);
+  const uint64_t* src = H.hit_keys + off;
+  int have = 0;
+  uint64_t kth = 0ull;
+  for (int base = 0; base < n; base += kAggChunk) {
+    if (tid == 0) sh_new = 0;
+    __syncthreads();
+    for (int i = tid; i < kAggChunk; i += 256) {
+      const int x = base + i;
+      if (x < n) {
+        const uint64_t k = src[x];
+        if (have < H.top_hits || k > kth) keys[have + atomicAdd(&sh_new, 1)] = k;   // (keys are distinct: doc ids)
+      }
+    }
+    __syncthreads();
+    const int added = sh_new;
+    __syncthreads();
+    if (added == 0) continue;
+    const int tot = have + added, m = next_pow2(tot < 2 ? 2 : tot);
+    for (int i = tot + tid; i < m; i += 256) keys[i] = 0ull;
+    __syncthreads();
+    block_bitonic_sort_desc(keys, m);
+    have = min(tot, H.top_hits);
+    kth = keys[have - 1];
+  }
+  const int w = H.top_hits - H.start_hit;
+  const size_t qs = (size_t)(H.q_lo + g / H.size) * H.size + g % H.size;
+  for (int i = tid; i < w; i += 256) {
+    const int p = H.start_hit + i;
+    int32_t doc = 0; float score = 0.0f;
+    if (p < have) { doc = key_doc(keys[p]) + H.doc_base; score = key_score(keys[p]); }
+    H.out_docs[qs * w + i] = doc; H.out_scores[qs * w + i] = score;
+  }
+  if (tid == 0) H.out_counts[qs] = max(0, have - H.start_hit);
 }
 
 }  // namespace nrtgpu

@@ -286,6 +286,14 @@ struct nrtgpu_batch {
   DevBuf<unsigned long long> agg_dvals[kMaxAggs];
   DevBuf<AggLaunch> agg_launch;
   DevBuf<int64_t> agg_keys; DevBuf<int32_t> agg_cnts, agg_n, agg_tot; DevBuf<long long> agg_other;
+  // nested collectors (cb.nested): [nq][n_buckets] words of the min / max / sum ones (pass 1), the selection's returned
+  // buckets and slot map, and the top-hits run's key buffers (pass 2)
+  DevBuf<unsigned long long> nest_words[kMaxAggs * kMaxNested];
+  DevBuf<int32_t> agg_bucket, nest_slot; DevBuf<double> nest_vals;
+  DevBuf<uint64_t> nest_keys; DevBuf<long long> nest_off; DevBuf<unsigned int> nest_fill;
+  DevBuf<int32_t> nest_docs, nest_hcounts; DevBuf<float> nest_scores;
+  DevBuf<AggLaunch> nest_launch;
+  DevBuf<unsigned long long> p2_total; DevBuf<int32_t> p2_flags;   // the top-hits run's totalHits / pruned / terminated
   // second pass of QueryRescorer (nrtgpu_score_docs / nrtgpu_rescore_query)
   DevBuf<int32_t> sd_docs, sd_counts; DevBuf<uint8_t> sd_match; DevBuf<float> sd_scores, sd_first;
   bool limits_active = false, disallow_partial = false;
@@ -870,6 +878,61 @@ int nrtgpu_batch_prepare_tree_phrases(nrtgpu_index* ix, const nrtgpu_clause* cla
   return NRTGPU_OK;
 }
 
+// the probe kernel's parameters for the batch's own outputs (no collectors, no stats; the work items are set at launch)
+static v3::ProbeLaunch probe_params(nrtgpu_batch* b) {
+  v3::ProbeLaunch P;
+  P.ix = b->ix->view(); P.pquery = b->pquery.p; P.sbounds = b->sbounds.p;
+  P.stats = nullptr;
+  P.known_hits = b->ix->live_bits.p ? nullptr : b->known_hits.p;   // (deletes installed after the batch was prepared: list lengths no longer bound the hits)
+#ifdef NRT_PROBE_KNOCK
+  { const char* e = getenv("NRTGPU_KNOCK"); P.knock = e ? atoi(e) : 0; }   // profiling builds only (tools/knock.py)
+#else
+  P.knock = 0;
+#endif
+  P.n_lists = b->plan.n_lists; P.parts_max = b->plan.parts_max; P.n_slices = b->plan.n_slices; P.top_k = b->top_k; P.slice_docs = b->plan.slice_docs; P.n_gran = b->plan.n_gran;
+  P.threshold = b->cb.threshold; P.pruned = b->pruned.p; P.theta = b->theta.p; P.total_hits = b->total_hits.p;
+  P.slice_keys = b->slice_keys.p; P.slice_cnt = b->slice_cnt.p;
+  P.deadline_ns = b->limits_active ? b->deadline_ns : 0; P.clock0 = b->clock0.p; P.timed_out = b->timed_out.p;
+  P.terminate_after = b->ta_scalar; P.terminated = b->terminated.p;
+  P.sort_kind = b->sort_kind; P.sort_reverse = b->sort_reverse;
+  P.sort_codes = b->order ? b->order->rank.p : b->sort_kind == NRTGPU_SORT_COLUMN ? b->ix->col_code[(size_t)b->sort_column]->p : nullptr;
+  P.sort_missing_code = b->sort_missing_code.p;
+  P.aggs = nullptr;
+  return P;
+}
+
+// the probe kernel over the batch's work items: the simple ones, then the generic ones (queue heads work_counter[0], [1])
+static int probe_launch(nrtgpu_batch* b, v3::ProbeLaunch P, bool debug, cudaStream_t st) {
+  // configuration A (3 CTAs / SM) for the pruned sweeps of TOP_SCORES, B (4 CTAs / SM) where every posting is visited
+  const bool cfg_b_simple = ix_ctx_probe_cfg(b->ix->ctx, P.threshold >= (int64_t)INT32_MAX);
+  const bool cfg_b_generic = ix_ctx_probe_cfg(b->ix->ctx, true);
+  auto launch = [&](auto simple_tag, bool cfg_b, int n_items) {
+    constexpr bool S = decltype(simple_tag)::value;
+    if (cfg_b) {
+      const int grid = std::min(v3::kCtasB * b->ix->ctx->plan.sm_count, n_items);
+      if (debug) v3::posting_probe_kernel<S, true, v3::kCtasB, v3::kStageB><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
+      else v3::posting_probe_kernel<S, false, v3::kCtasB, v3::kStageB><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
+    } else {
+      const int grid = std::min(v3::kCtasA * b->ix->ctx->plan.sm_count, n_items);
+      if (debug) v3::posting_probe_kernel<S, true, v3::kCtasA, v3::kStageA><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageA>), st>>>(P);
+      else v3::posting_probe_kernel<S, false, v3::kCtasA, v3::kStageA><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageA>), st>>>(P);
+    }
+  };
+  if (b->plan.n_probe_simple > 0) {
+    P.work_query = b->work_query.p; P.work_slice = b->work_slice.p; P.n_work = b->plan.n_probe_simple; P.work_counter = b->work_counter.p;
+    P.stats = debug ? b->probe_stats.p : nullptr;
+    launch(std::true_type{}, cfg_b_simple, b->plan.n_probe_simple);
+  }
+  if (b->plan.n_probe_generic > 0) {
+    P.work_query = b->work_query.p + b->plan.n_probe_simple; P.work_slice = b->work_slice.p + b->plan.n_probe_simple;
+    P.n_work = b->plan.n_probe_generic; P.work_counter = b->work_counter.p + 1;
+    P.stats = debug ? b->probe_stats.p + v3::kProbeStats : nullptr;
+    launch(std::false_type{}, cfg_b_generic, b->plan.n_probe_generic);
+  }
+  NRT_CUDA_TRY(cudaGetLastError());
+  return NRTGPU_OK;
+}
+
 int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   if (!b) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_run: NULL batch");
   cudaStream_t st = (cudaStream_t)stream_;
@@ -898,6 +961,13 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
       NRT_CUDA_TRY(cudaMemsetAsync(b->agg_dvals[i].p, a.kind == NRTGPU_AGG_MIN ? 0xff : 0x00, b->agg_dvals[i].bytes(), st));
     }
   }
+  for (size_t j = 0; j < b->cb.nested.size(); ++j) {   // nested min / max / sum: one word per (query, parent bucket), as above
+    const nrtgpu_nested_aggregation& n = b->cb.nested[j];
+    if (n.kind == NRTGPU_AGG_TOP_HITS) continue;
+    const int32_t nb = b->ix->col_n_distinct[(size_t)b->cb.aggs[(size_t)n.parent].column];
+    if ((rc_dbg = b->nest_words[j].alloc((size_t)b->nq * (size_t)std::max(nb, 1)))) return rc_dbg;
+    NRT_CUDA_TRY(cudaMemsetAsync(b->nest_words[j].p, n.kind == NRTGPU_AGG_MIN ? 0xff : 0x00, b->nest_words[j].bytes(), st));
+  }
   const bool debug = b->ix->ctx->debug_modes;
   cudaEvent_t* ev = b->ev[b->runs_recorded % nrtgpu_batch::kEvRing];
   NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
@@ -914,24 +984,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
     if (!b->cb.wide) {
       const int n_probe = b->plan.n_probe_simple + b->plan.n_probe_generic;
       if (n_probe > 0) {
-        v3::ProbeLaunch P;
-        P.ix = L.ix; P.pquery = b->pquery.p; P.sbounds = b->sbounds.p;
-        P.stats = nullptr;
-        P.known_hits = b->ix->live_bits.p ? nullptr : b->known_hits.p;   // (deletes installed after the batch was prepared: list lengths no longer bound the hits)
-#ifdef NRT_PROBE_KNOCK
-        { const char* e = getenv("NRTGPU_KNOCK"); P.knock = e ? atoi(e) : 0; }   // profiling builds only (tools/knock.py)
-#else
-        P.knock = 0;
-#endif
-        P.n_lists = b->plan.n_lists; P.parts_max = b->plan.parts_max; P.n_slices = b->plan.n_slices; P.top_k = b->top_k; P.slice_docs = b->plan.slice_docs; P.n_gran = b->plan.n_gran;
-        P.threshold = b->cb.threshold; P.pruned = b->pruned.p; P.theta = L.theta; P.total_hits = L.total_hits;
-        P.slice_keys = L.slice_keys; P.slice_cnt = L.slice_cnt;
-        P.deadline_ns = L.deadline_ns; P.clock0 = L.clock0; P.timed_out = L.timed_out;
-        P.terminate_after = b->ta_scalar; P.terminated = b->terminated.p;
-        P.sort_kind = b->sort_kind; P.sort_reverse = b->sort_reverse;
-        P.sort_codes = b->order ? b->order->rank.p : b->sort_kind == NRTGPU_SORT_COLUMN ? b->ix->col_code[(size_t)b->sort_column]->p : nullptr;
-        P.sort_missing_code = b->sort_missing_code.p;
-        P.aggs = nullptr;
+        v3::ProbeLaunch P = probe_params(b);
         if (!b->cb.aggs.empty()) {
           AggLaunch A; std::memset(&A, 0, sizeof(A));
           A.n_aggs = (int32_t)b->cb.aggs.size();
@@ -944,6 +997,13 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
             } else {
               A.a[i].dvals = b->agg_dvals[i].p;
             }
+            A.nested_begin[i + 1] = A.nested_begin[i];   // pass 1: the nested min / max / sum collectors
+            for (size_t j = 0; j < b->cb.nested.size(); ++j) {
+              const nrtgpu_nested_aggregation& n = b->cb.nested[j];
+              if (n.parent != i || n.kind == NRTGPU_AGG_TOP_HITS) continue;
+              AggNestedDev& d = A.nested[A.nested_begin[i + 1]++];
+              d.kind = n.kind; d.column = n.column; d.value_type = n.value_type; d.dvals = b->nest_words[j].p;
+            }
           }
           if ((rc_dbg = b->agg_launch.upload_async(&A, 1, st))) return rc_dbg;
           NRT_CUDA_TRY(cudaStreamSynchronize(st));   // A is a stack object
@@ -953,33 +1013,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
           if (!b->probe_stats.p && (rc_dbg = b->probe_stats.alloc(2 * v3::kProbeStats))) return rc_dbg;
           NRT_CUDA_TRY(cudaMemsetAsync(b->probe_stats.p, 0, 2 * v3::kProbeStats * sizeof(unsigned long long), st));
         }
-        // configuration A (3 CTAs / SM) for the pruned sweeps of TOP_SCORES, B (4 CTAs / SM) where every posting is visited
-        const bool cfg_b_simple = ix_ctx_probe_cfg(b->ix->ctx, P.threshold >= (int64_t)INT32_MAX);
-        const bool cfg_b_generic = ix_ctx_probe_cfg(b->ix->ctx, true);
-        auto launch = [&](auto simple_tag, bool cfg_b, int n_items) {
-          constexpr bool S = decltype(simple_tag)::value;
-          if (cfg_b) {
-            const int grid = std::min(v3::kCtasB * b->ix->ctx->plan.sm_count, n_items);
-            if (debug) v3::posting_probe_kernel<S, true, v3::kCtasB, v3::kStageB><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
-            else v3::posting_probe_kernel<S, false, v3::kCtasB, v3::kStageB><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
-          } else {
-            const int grid = std::min(v3::kCtasA * b->ix->ctx->plan.sm_count, n_items);
-            if (debug) v3::posting_probe_kernel<S, true, v3::kCtasA, v3::kStageA><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageA>), st>>>(P);
-            else v3::posting_probe_kernel<S, false, v3::kCtasA, v3::kStageA><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageA>), st>>>(P);
-          }
-        };
-        if (b->plan.n_probe_simple > 0) {
-          P.work_query = L.work_query; P.work_slice = L.work_slice; P.n_work = b->plan.n_probe_simple; P.work_counter = b->work_counter.p;
-          P.stats = debug ? b->probe_stats.p : nullptr;
-          launch(std::true_type{}, cfg_b_simple, b->plan.n_probe_simple);
-        }
-        if (b->plan.n_probe_generic > 0) {
-          P.work_query = L.work_query + b->plan.n_probe_simple; P.work_slice = L.work_slice + b->plan.n_probe_simple;
-          P.n_work = b->plan.n_probe_generic; P.work_counter = b->work_counter.p + 1;
-          P.stats = debug ? b->probe_stats.p + v3::kProbeStats : nullptr;
-          launch(std::false_type{}, cfg_b_generic, b->plan.n_probe_generic);
-        }
-        NRT_CUDA_TRY(cudaGetLastError());
+        if ((rc_dbg = probe_launch(b, P, debug, st))) return rc_dbg;
       }
     } else if (b->cb.tree) {
       L.nodes = b->nodes.p; L.node_begin = b->node_begin.p; L.phrases = b->phrases.p; L.phrase_begin = b->phrase_begin.p;
@@ -1085,8 +1119,100 @@ int nrtgpu_batch_fetch_ex(nrtgpu_batch* b, void* stream_, int32_t* out_docs, flo
   return batch_fetch_impl(b, stream_, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
 }
 
-// aggregation results of the last run -> caller buffers
-static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggregation_result* out) {
+// Nested top hits of terms aggregation `parent` (pass 2): the batch's probe launch runs again with a collector that only
+// appends make_key(score, doc) of the docs of returned buckets (slot map nest_slot) to per-(query, slot) segments sized by
+// the bucket counts h_cnt [nq*size]; its totalHits / pruned / terminated go to scratch, and theta / slice lists / queue
+// heads are the batch's, already merged. Queries are taken in groups whose keys fit kNestedHitBudget.
+static int batch_nested_top_hits(nrtgpu_batch* b, cudaStream_t st, int parent, const std::vector<int32_t>& h_cnt,
+                                 const nrtgpu_nested_result* nres) {
+  const int nq = b->nq;
+  const nrtgpu_aggregation& a = b->cb.aggs[(size_t)parent];
+  const int size = a.size;
+  std::vector<size_t> th;   // the parent's top-hits collectors (indices into cb.nested)
+  for (size_t j = 0; j < b->cb.nested.size(); ++j)
+    if (b->cb.nested[j].parent == parent && b->cb.nested[j].kind == NRTGPU_AGG_TOP_HITS) th.push_back(j);
+  const int n_th = (int)th.size();
+  std::vector<size_t> out_base((size_t)n_th + 1, 0);
+  for (int k = 0; k < n_th; ++k) {
+    const nrtgpu_nested_aggregation& n = b->cb.nested[th[(size_t)k]];
+    out_base[(size_t)k + 1] = out_base[(size_t)k] + (size_t)nq * size * (size_t)(n.top_hits - n.start_hit);
+  }
+  int rc;
+  if ((rc = b->nest_docs.alloc(out_base.back())) || (rc = b->nest_scores.alloc(out_base.back())) ||
+      (rc = b->nest_hcounts.alloc((size_t)n_th * nq * size)) || (rc = b->p2_total.alloc((size_t)nq)) || (rc = b->p2_flags.alloc(2 * (size_t)nq)))
+    return rc;
+  std::vector<long long> per_q((size_t)nq, 0);
+  for (int q = 0; q < nq; ++q)
+    for (int s = 0; s < size; ++s) per_q[(size_t)q] += (long long)n_th * h_cnt[(size_t)q * size + s];
+  for (int q_lo = 0; q_lo < nq;) {
+    if (per_q[(size_t)q_lo] > kNestedHitBudget)
+      NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nested top hits: the returned buckets of one query hold more than 2^26 hits");
+    long long total = 0;
+    int q_hi = q_lo;
+    while (q_hi < nq && total + per_q[(size_t)q_hi] <= kNestedHitBudget) total += per_q[(size_t)q_hi++];
+    const int gq = q_hi - q_lo, gs = gq * size;
+    std::vector<long long> off((size_t)n_th * (gs + 1));   // per collector: the segments of the group, laid out one after the other
+    long long at = 0;
+    for (int k = 0; k < n_th; ++k)
+      for (int g = 0; g <= gs; ++g) {
+        off[(size_t)k * (gs + 1) + g] = at;
+        if (g < gs) at += h_cnt[(size_t)q_lo * size + g];
+      }
+    if ((rc = b->nest_off.upload_async(off.data(), off.size(), st)) || (rc = b->nest_fill.alloc((size_t)n_th * gs)) ||
+        (rc = b->nest_keys.alloc((size_t)std::max(at, 1ll)))) return rc;
+    NRT_CUDA_TRY(cudaMemsetAsync(b->nest_fill.p, 0, b->nest_fill.bytes(), st));
+    if (at > 0 && b->plan.n_probe_simple + b->plan.n_probe_generic > 0) {
+      AggLaunch A; std::memset(&A, 0, sizeof(A));
+      A.n_aggs = 1;
+      A.a[0].kind = NRTGPU_AGG_TERMS; A.a[0].column = a.column; A.a[0].value_type = a.value_type;
+      A.a[0].n_buckets = b->ix->col_n_distinct[(size_t)a.column];
+      A.codes[0] = b->ix->col_code[(size_t)a.column]->p;   // counts stay NULL: the pass-1 tables are not touched
+      A.nested_begin[1] = n_th;
+      for (int k = 0; k < n_th; ++k) {
+        AggNestedDev& d = A.nested[k];
+        d.kind = NRTGPU_AGG_TOP_HITS; d.size = size; d.q_lo = q_lo; d.q_hi = q_hi; d.slot_of = b->nest_slot.p;
+        d.hit_off = b->nest_off.p + (size_t)k * (gs + 1); d.hit_fill = b->nest_fill.p + (size_t)k * gs; d.hit_keys = b->nest_keys.p;
+      }
+      if ((rc = b->nest_launch.upload_async(&A, 1, st))) return rc;
+      NRT_CUDA_TRY(cudaMemsetAsync(b->theta.p, 0, b->theta.bytes(), st));
+      NRT_CUDA_TRY(cudaMemsetAsync(b->slice_cnt.p, 0, b->slice_cnt.bytes(), st));
+      NRT_CUDA_TRY(cudaMemsetAsync(b->work_counter.p, 0, b->work_counter.bytes(), st));
+      NRT_CUDA_TRY(cudaMemsetAsync(b->p2_total.p, 0, b->p2_total.bytes(), st));
+      NRT_CUDA_TRY(cudaMemsetAsync(b->p2_flags.p, 0, b->p2_flags.bytes(), st));
+      v3::ProbeLaunch P = probe_params(b);
+      P.total_hits = b->p2_total.p; P.pruned = b->p2_flags.p; P.terminated = b->p2_flags.p + nq;
+      P.deadline_ns = 0; P.terminate_after = 0;
+      P.aggs = b->nest_launch.p;
+      if ((rc = probe_launch(b, P, false, st))) return rc;
+    }
+    for (int k = 0; k < n_th; ++k) {
+      const nrtgpu_nested_aggregation& n = b->cb.nested[th[(size_t)k]];
+      NestedHitsLaunch H;
+      H.hit_keys = b->nest_keys.p; H.hit_off = b->nest_off.p + (size_t)k * (gs + 1); H.hit_fill = b->nest_fill.p + (size_t)k * gs;
+      H.q_lo = q_lo; H.size = size; H.top_hits = n.top_hits; H.start_hit = n.start_hit; H.doc_base = b->ix->doc_base;
+      H.out_docs = b->nest_docs.p + out_base[(size_t)k]; H.out_scores = b->nest_scores.p + out_base[(size_t)k];
+      H.out_counts = b->nest_hcounts.p + (size_t)k * nq * size;
+      nested_top_hits_kernel<<<gs, 256, 0, st>>>(H);
+      NRT_CUDA_TRY(cudaGetLastError());
+    }
+    NRT_CUDA_TRY(cudaStreamSynchronize(st));   // A and off are stack objects; the next group reuses the buffers
+    q_lo = q_hi;
+  }
+  for (int k = 0; k < n_th; ++k) {
+    const size_t j = th[(size_t)k];
+    const nrtgpu_nested_result& r = nres[j];
+    const size_t nw = out_base[(size_t)k + 1] - out_base[(size_t)k];
+    if (r.hit_docs) NRT_CUDA_TRY(cudaMemcpyAsync(r.hit_docs, b->nest_docs.p + out_base[(size_t)k], nw * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (r.hit_scores) NRT_CUDA_TRY(cudaMemcpyAsync(r.hit_scores, b->nest_scores.p + out_base[(size_t)k], nw * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (r.hit_counts) NRT_CUDA_TRY(cudaMemcpyAsync(r.hit_counts, b->nest_hcounts.p + (size_t)k * nq * size, (size_t)nq * size * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (r.hit_total) for (size_t x = 0; x < (size_t)nq * size; ++x) r.hit_total[x] = h_cnt[x];   // TopDocs.totalHits: the bucket's count
+  }
+  NRT_CUDA_TRY(cudaStreamSynchronize(st));
+  return NRTGPU_OK;
+}
+
+// aggregation results of the last run -> caller buffers (nres: the results of cb.nested, in request order; NULL: none)
+static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggregation_result* out, const nrtgpu_nested_result* nres) {
   const int nq = b->nq;
   for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
     const nrtgpu_aggregation& a = b->cb.aggs[i];
@@ -1096,29 +1222,68 @@ static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggre
       const size_t n = (size_t)nq * a.size;
       if ((rc = b->agg_keys.alloc(n)) || (rc = b->agg_cnts.alloc(n)) || (rc = b->agg_n.alloc((size_t)nq)) || (rc = b->agg_tot.alloc((size_t)nq)) ||
           (rc = b->agg_other.alloc((size_t)nq))) return rc;
+      int n_nested = 0, order_by = -1;
+      bool top_hits = false;
+      for (size_t j = 0; j < b->cb.nested.size(); ++j)
+        if (b->cb.nested[j].parent == (int32_t)i) {
+          ++n_nested;
+          if (b->cb.nested[j].orders_parent) order_by = (int)j;
+          top_hits |= b->cb.nested[j].kind == NRTGPU_AGG_TOP_HITS;
+        }
       AggTermsLaunch T;
       T.counts = b->agg_counts[i].p; T.n_buckets = b->ix->col_n_distinct[(size_t)a.column]; T.nq = nq; T.size = a.size; T.order_desc = a.order_desc != 0;
       T.distinct = b->ix->col_distinct[(size_t)a.column]->p;
       T.out_keys = b->agg_keys.p; T.out_counts = b->agg_cnts.p; T.out_n = b->agg_n.p; T.out_total_buckets = b->agg_tot.p; T.out_other = b->agg_other.p;
-      agg_terms_topk_kernel<<<nq, 256, 0, st>>>(T);
+      T.out_bucket = nullptr;
+      if (n_nested > 0) {
+        if ((rc = b->agg_bucket.alloc(n))) return rc;
+        T.out_bucket = b->agg_bucket.p;
+      }
+      if (order_by >= 0) {
+        NRT_CUDA_TRY(cudaFuncSetAttribute(agg_terms_by_value_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAggByValueSmem));
+        agg_terms_by_value_kernel<<<nq, 256, kAggByValueSmem, st>>>(T, b->nest_words[(size_t)order_by].p, b->cb.nested[(size_t)order_by].kind);
+      } else {
+        agg_terms_topk_kernel<<<nq, 256, 0, st>>>(T);
+      }
       NRT_CUDA_TRY(cudaGetLastError());
+      std::vector<int32_t> h_cnt;
+      if (n_nested > 0) {   // per returned slot: nested values, the slot map of the top-hits run
+        AggNestedOutLaunch O; std::memset(&O, 0, sizeof(O));
+        O.bucket = b->agg_bucket.p; O.nq = nq; O.size = a.size; O.n_buckets = T.n_buckets;
+        std::vector<size_t> vals;   // the min / max / sum collectors (indices into cb.nested)
+        for (size_t j = 0; j < b->cb.nested.size(); ++j)
+          if (b->cb.nested[j].parent == (int32_t)i && b->cb.nested[j].kind != NRTGPU_AGG_TOP_HITS) vals.push_back(j);
+        if ((rc = b->nest_vals.alloc(std::max<size_t>(vals.size(), 1) * n))) return rc;
+        O.n_vals = (int32_t)vals.size();
+        for (size_t k = 0; k < vals.size(); ++k) {
+          O.kind[k] = b->cb.nested[vals[k]].kind; O.words[k] = b->nest_words[vals[k]].p; O.values[k] = b->nest_vals.p + k * n;
+        }
+        if (top_hits) {
+          const size_t cells = (size_t)nq * (size_t)std::max(T.n_buckets, 1);
+          if ((rc = b->nest_slot.alloc(cells))) return rc;
+          NRT_CUDA_TRY(cudaMemsetAsync(b->nest_slot.p, 0xff, cells * sizeof(int32_t), st));
+          O.slot_of = b->nest_slot.p;
+        }
+        agg_nested_out_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(O);
+        NRT_CUDA_TRY(cudaGetLastError());
+        for (size_t k = 0; k < vals.size(); ++k)
+          if (nres && nres[vals[k]].values)
+            NRT_CUDA_TRY(cudaMemcpyAsync(nres[vals[k]].values, b->nest_vals.p + k * n, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+        h_cnt.resize(n);
+        NRT_CUDA_TRY(cudaMemcpyAsync(h_cnt.data(), b->agg_cnts.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+      }
       if (r.bucket_keys) NRT_CUDA_TRY(cudaMemcpyAsync(r.bucket_keys, b->agg_keys.p, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
       if (r.bucket_counts) NRT_CUDA_TRY(cudaMemcpyAsync(r.bucket_counts, b->agg_cnts.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       if (r.n_buckets) NRT_CUDA_TRY(cudaMemcpyAsync(r.n_buckets, b->agg_n.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       if (r.total_buckets) NRT_CUDA_TRY(cudaMemcpyAsync(r.total_buckets, b->agg_tot.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       if (r.other_counts) NRT_CUDA_TRY(cudaMemcpyAsync(r.other_counts, b->agg_other.p, (size_t)nq * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
       NRT_CUDA_TRY(cudaStreamSynchronize(st));   // the scratch is reused by the next terms aggregation
+      if (top_hits && (rc = batch_nested_top_hits(b, st, (int)i, h_cnt, nres))) return rc;
     } else if (r.values) {
       std::vector<unsigned long long> h((size_t)nq);
       NRT_CUDA_TRY(cudaMemcpyAsync(h.data(), b->agg_dvals[i].p, (size_t)nq * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
       NRT_CUDA_TRY(cudaStreamSynchronize(st));
-      for (int q = 0; q < nq; ++q) {
-        double v;
-        if (a.kind == NRTGPU_AGG_SUM) std::memcpy(&v, &h[(size_t)q], sizeof(v));
-        else if (a.kind == NRTGPU_AGG_MAX) v = h[(size_t)q] == 0ull ? -DBL_MAX : ordered_to_double(h[(size_t)q]);              // MaxCollectorManager.UNSET_VALUE
-        else v = h[(size_t)q] == 0xffffffffffffffffull ? DBL_MAX : ordered_to_double(h[(size_t)q]);                          // MinCollectorManager.UNSET_VALUE
-        r.values[q] = v;
-      }
+      for (int q = 0; q < nq; ++q) r.values[q] = agg_word_value(a.kind, h[(size_t)q]);
     }
   }
   return NRTGPU_OK;
@@ -1264,6 +1429,7 @@ struct SearchOut {
   uint8_t* relation = nullptr; uint8_t* hit_timeout = nullptr; uint8_t* terminated_early = nullptr;
   int64_t* sort_values = nullptr;
   const nrtgpu_aggregation_result* aggs = nullptr;
+  const nrtgpu_nested_result* nested = nullptr;
 };
 
 // one-shot search: compile + upload the batch into a pooled workspace, run, deliver the results
@@ -1283,7 +1449,7 @@ static int search_bool_impl(nrtgpu_index* ix, const BatchRequest& r, const nrtgp
     if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; }
   }
   rc = batch_fetch_impl(b, stream, out.docs, out.scores, out.counts, out.total_hits, out.relation, out.hit_timeout, out.terminated_early);
-  if (!rc && !b->cb.aggs.empty() && out.aggs) rc = batch_fetch_aggs(b, (cudaStream_t)stream, out.aggs);
+  if (!rc && !b->cb.aggs.empty() && out.aggs) rc = batch_fetch_aggs(b, (cudaStream_t)stream, out.aggs, out.nested);
   return rc;
 }
 
@@ -1439,6 +1605,22 @@ int nrtgpu_search_bool_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int3
   BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
   r.aggs = aggs; r.n_aggs = n_aggs;
   SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.aggs = results;
+  return search_bool_impl(ix, r, nullptr, stream, o);
+}
+
+int nrtgpu_search_bool_aggs_nested(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                   const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                   const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                                   const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                   const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs,
+                                   float* out_scores, int32_t* out_counts, int64_t* out_total_hits) {
+  if (n_aggs <= 0 || !aggs || !results) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool_aggs: no aggregations");
+  if (n_nested < 0 || (n_nested > 0 && (!nested || !nested_results))) NRT_FAIL(NRTGPU_ERR_INVALID, "nested aggregations: NULL argument");
+  BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
+  r.aggs = aggs; r.n_aggs = n_aggs;
+  if (n_nested > 0) { r.nested = nested; r.n_nested = n_nested; }
+  SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.aggs = results;
+  o.nested = n_nested > 0 ? nested_results : nullptr;
   return search_bool_impl(ix, r, nullptr, stream, o);
 }
 

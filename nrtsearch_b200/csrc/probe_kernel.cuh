@@ -612,7 +612,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
           float score;
           if (have && evaluate_doc(L, sm, d, e.y, &score)) {
             ++my_hits;
-            if (L.aggs) agg_collect(*L.aggs, L.ix, qi, d);   // additional collectors see every matching doc
+            if (L.aggs) agg_collect(*L.aggs, L.ix, qi, d, score);   // additional collectors see every matching doc
             if (L.sort_kind == NRTGPU_SORT_RELEVANCE || L.sort_kind == kSortScoreRank) {
               entry = make_key(score, d);
               // [score, ...] order: ties by the order's rank, which takes the doc's place; ordered(-s) == ~ordered(s) for reverse

@@ -22,7 +22,8 @@ from typing import List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _native
-from ._native import (Aggregation as CAgg, AggregationResult as CAggResult, Clause, CollectionTimeoutException, NrtGpuError,
+from ._native import (Aggregation as CAgg, AggregationResult as CAggResult, NestedAggregation as CNested,
+                      NestedResult as CNestedResult, Clause, CollectionTimeoutException, NrtGpuError,
                       NrtGpuUnsupported, Query as CQuery, SearchLimits, Sort as CSort, check)
 from .index import HostShard, PinnedDesc
 
@@ -221,11 +222,23 @@ class SortFieldCollector:
 @dataclass(frozen=True)
 class TermsCollector:
     """TermsCollector over a numeric doc-value field ({Int,Long,Float,Double}TermsCollectorManager): `size` buckets ordered
-    by count (BucketOrder COUNT, desc by default)."""
+    by count (BucketOrder COUNT, desc by default). nested: up to 4 (name, MinCollector | MaxCollector | SumCollector |
+    TopHitsCollector) computed per bucket (Collector.nestedCollectors); order_by: the name of a nested min / max / sum
+    that orders the buckets instead of the count (BucketOrder by a nested collector, in the order_desc direction)."""
     column: int
     size: int
     order_desc: bool = True
     field_type: str = "long"
+    nested: tuple = ()
+    order_by: Optional[str] = None
+
+
+@dataclass(frozen=True)
+class TopHitsCollector:
+    """TopHitsCollector as a nested collector of a terms bucket (TopHitsCollectorManager): the bucket's hits by score
+    descending, then doc ascending, positions [start_hit, top_hits)."""
+    top_hits: int
+    start_hit: int = 0
 
 
 @dataclass(frozen=True)
@@ -719,14 +732,16 @@ class GpuIndexSearcher:
     def search_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
                                stream: int = 0):
         """IndexSearcher.search with additional collectors (SearchCollectorManager fan-out): returns (BatchResult, results)
-        where results[i] is a float64 [nq] array (min / max / sum) or a dict of bucket arrays (terms)."""
+        where results[i] is a float64 [nq] array (min / max / sum) or a dict of bucket arrays (terms). A terms collector with
+        nested collectors adds "nested": {name: float64 [nq, size] (min / max / sum) or {"docs", "scores" [nq, size,
+        top_hits - start_hit], "counts", "total_hits" [nq, size]} (top hits)}, per returned bucket."""
         carr, ncl, qarr, nq = compile_queries(queries)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
         aggs = (CAgg * len(additional))()
         res = (CAggResult * len(additional))()
-        outs = []
+        outs, nested, nested_res = [], [], []
         for i, a in enumerate(additional):
             vt = _VALUE_TYPE[a.field_type]
             if isinstance(a, TermsCollector):
@@ -735,16 +750,52 @@ class GpuIndexSearcher:
                      "total_buckets": np.zeros(nq, np.int32), "other_counts": np.zeros(nq, np.int64)}
                 res[i] = CAggResult(None, o["keys"].ctypes.data, o["counts"].ctypes.data, o["n"].ctypes.data,
                                     o["total_buckets"].ctypes.data, o["other_counts"].ctypes.data)
+                if a.nested or a.order_by is not None:
+                    o["nested"] = self._nested_specs(i, a, nq, nested, nested_res)
             else:
                 kind = 2 if isinstance(a, MinCollector) else 3 if isinstance(a, MaxCollector) else 4
                 aggs[i] = CAgg(kind, a.column, vt, 0, 0, 0)
                 o = np.zeros(nq, np.float64)
                 res[i] = CAggResult(o.ctypes.data, None, None, None, None, None)
             outs.append(o)
-        check(self._lib.nrtgpu_search_bool_aggs(self.index.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res, C.c_void_p(stream),
-                                                out.docs.ctypes.data, out.scores.ctypes.data, out.counts.ctypes.data,
-                                                out.total_hits.ctypes.data))
+        hits = (out.docs.ctypes.data, out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data)
+        if nested:
+            narr = (CNested * len(nested))(*nested)
+            nres = (CNestedResult * len(nested))(*nested_res)
+            check(self._lib.nrtgpu_search_bool_aggs_nested(self.index.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
+                                                           narr, len(nested), nres, C.c_void_p(stream), *hits))
+        else:
+            check(self._lib.nrtgpu_search_bool_aggs(self.index.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
+                                                    C.c_void_p(stream), *hits))
         return out, outs
+
+    @staticmethod
+    def _nested_specs(parent: int, a: TermsCollector, nq: int, nested: list, nested_res: list) -> dict:
+        """the nrtgpu_nested_aggregation records and result buffers of terms collector `parent` (appended to nested /
+        nested_res); returns the result dict they fill"""
+        names = [name for name, _ in a.nested]
+        if len(set(names)) != len(names):
+            raise ValueError("nested collector names must be unique")
+        if a.order_by is not None and a.order_by not in names:
+            raise ValueError(f"order_by {a.order_by!r} is not a nested collector")
+        o = {}
+        for name, c in a.nested:
+            if isinstance(c, TopHitsCollector):
+                w = max(c.top_hits - c.start_hit, 0)
+                r = {"docs": np.zeros((nq, a.size, w), np.int32), "scores": np.zeros((nq, a.size, w), np.float32),
+                     "counts": np.zeros((nq, a.size), np.int32), "total_hits": np.zeros((nq, a.size), np.int64)}
+                nested.append(CNested(parent, 5, 0, 0, c.top_hits, c.start_hit, 1 if name == a.order_by else 0, 0))
+                nested_res.append(CNestedResult(None, r["docs"].ctypes.data, r["scores"].ctypes.data, r["counts"].ctypes.data,
+                                                r["total_hits"].ctypes.data))
+            elif isinstance(c, (MinCollector, MaxCollector, SumCollector)):
+                kind = 2 if isinstance(c, MinCollector) else 3 if isinstance(c, MaxCollector) else 4
+                r = np.zeros((nq, a.size), np.float64)
+                nested.append(CNested(parent, kind, c.column, _VALUE_TYPE[c.field_type], 0, 0, 1 if name == a.order_by else 0, 0))
+                nested_res.append(CNestedResult(r.ctypes.data, None, None, None, None))
+            else:
+                raise ValueError(f"nested collector {name!r}: {type(c).__name__} is not on the GPU path")
+            o[name] = r
+        return o
 
     def score_docs(self, queries: Sequence[object], docs: np.ndarray, counts: Optional[np.ndarray] = None, stream: int = 0):
         """Second pass of QueryRescorer: query q on its own hit list -> (matches uint8 [nq, n], scores float32 [nq, n])."""
