@@ -509,7 +509,12 @@ int nrtgpu_batch_free(nrtgpu_batch* b);
  * shard) are never hits, as through IndexSearcher's acceptDocs; `filter` is ANDed on top. Exact BY CONSTRUCTION: the
  * tensor-core candidate stage is followed by an fp64 re-score and a rank-safety certificate (every vector outside the
  * candidate list is proven, with the bf16 error bound 2^-7 |q||d|, to score below the k-th exact score); queries the
- * certificate rejects are re-run by exact evaluation of every vector (nrtgpu_knn_last_uncertified counts them). */
+ * certificate rejects are re-run by exact evaluation of every vector (nrtgpu_knn_last_uncertified counts them).
+ * NRTGPU_ERR_INVALID: nq <= 0, k outside 1..1024, an index without vectors, or a boost that is not a BoostQuery boost:
+ * every boosts[q] must be finite and >= 0 (negative, -0, NaN and infinite boosts are refused, as Lucene's BoostQuery does;
+ * with a negative boost the final order would be the reverse of the candidate order and the certificate would accept the
+ * worst vectors). Boost 0 is legal: every score is 0 and the page holds the first k docs. The same rule holds for
+ * nrtgpu_search_knn_filtered; nrtgpu_search_knn_timed takes no boosts and refuses nq <= 0. */
 int nrtgpu_search_knn(nrtgpu_index* ix, const float* queries, int32_t nq, int32_t k,
                       const float* boosts /*[nq] or NULL*/, const uint8_t* filter /*[n_docs] 0/1 or NULL*/,
                       void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts);
@@ -531,7 +536,7 @@ int32_t nrtgpu_knn_last_uncertified(const nrtgpu_index* ix);
  * filter, so counts[q] < k when fewer match. Matching follows the boolean path: an empty clause range matches nothing, as an
  * empty BooleanQuery does; so does a query of MUST_NOT clauses only.
  * NRTGPU_ERR_INVALID: has_after on a filter, a filter_of entry or clause id out of range, an index without vectors, k outside
- * 1..1024. NRTGPU_ERR_UNSUPPORTED: a filter shape outside the boolean path (more than 16 clauses or 8 term clauses); the
+ * 1..1024, nq <= 0, a boost that is negative, -0, NaN or infinite. NRTGPU_ERR_UNSUPPORTED: a filter shape outside the boolean path (more than 16 clauses or 8 term clauses); the
  * byte filter of nrtgpu_search_knn still serves it.
  * A query whose filter matches at most 1/320 of the vectors is scored exactly over those docs only; the others go through
  * the candidate GEMM with the filter applied. The first path needs one vector per doc in doc order (ascending vec_docs, as

@@ -1800,6 +1800,14 @@ int nrtgpu_merge_topk_device(nrtgpu_ctx* ctx, int32_t n_lists, int32_t nq, int32
   return NRTGPU_OK;
 }
 
+// A kNN boost is a BoostQuery boost: finite and not negative (Lucene's BoostQuery constructor refuses anything else, -0
+// included). The rank-safety certificate depends on it: score * boost must not decrease when the score grows, or the
+// candidate stage keeps the worst vectors and knn_score_upper_bound certifies them.
+static bool knn_boosts_valid(const float* boosts, int32_t nq) {
+  for (int32_t q = 0; boosts && q < nq; ++q) if (!std::isfinite(boosts[q]) || std::signbit(boosts[q])) return false;
+  return true;
+}
+
 // nrtgpu_search_knn and nrtgpu_search_knn_timed once their arguments are checked
 static int knn_search_checked(nrtgpu_index* ix, const KnnRequest& req, void* stream, const KnnPages& out, float* stage_ms) {
   NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
@@ -1812,7 +1820,9 @@ int nrtgpu_search_knn(nrtgpu_index* ix, const float* queries, int32_t nq, int32_
                       int32_t* out_counts) {
   if (!ix || !queries || !out_docs || !out_scores || !out_counts) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn: NULL argument");
   if (ix->vec_dims <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn: index has no vector field");
+  if (nq <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn: nq must be > 0");
   if (k <= 0 || k > kMaxTopK) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn: k out of range");
+  if (!knn_boosts_valid(boosts, nq)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn: a boost must be finite and >= 0");
   return knn_search_checked(ix, KnnRequest{queries, nq, k, boosts, filter, nullptr, nullptr, 0}, stream,
                             KnnPages{out_docs, out_scores, out_counts}, nullptr);
 }
@@ -1821,6 +1831,7 @@ int nrtgpu_search_knn_timed(nrtgpu_index* ix, const float* queries, int32_t nq, 
                             float* out_scores, int32_t* out_counts, float* stage_ms /*[3]: gemm, select, rescore*/) {
   if (!ix || !queries || !out_docs || !out_scores || !out_counts || !stage_ms) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_timed: NULL argument");
   if (ix->vec_dims <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_timed: index has no vector field");
+  if (nq <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_timed: nq must be > 0");
   if (k <= 0 || k > kMaxTopK / 4) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_timed: k out of range");
   return knn_search_checked(ix, KnnRequest{queries, nq, k, nullptr, nullptr, nullptr, nullptr, 0}, stream,
                             KnnPages{out_docs, out_scores, out_counts}, stage_ms);
@@ -1984,6 +1995,7 @@ int nrtgpu_search_knn_filtered(nrtgpu_index* ix, const float* queries, int32_t n
   if (nq <= 0 || n_filters < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_filtered: nq must be > 0 and n_filters >= 0");
   if (ix->vec_dims <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_filtered: index has no vector field");
   if (k <= 0 || k > kMaxTopK) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_filtered: k out of range");
+  if (!knn_boosts_valid(boosts, nq)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_filtered: a boost must be finite and >= 0");
   for (int f = 0; f < n_filters; ++f)
     if (filters[f].has_after) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_knn_filtered: a filter query has no searchAfter");
   // rows: the filters some query uses, in order of first use

@@ -868,6 +868,9 @@ class GpuIndexSearcher:
         scores = np.zeros((nq, k), np.float32)
         counts = np.zeros(nq, np.int32)
         b = None if boosts is None else np.ascontiguousarray(boosts, dtype=np.float32)
+        # a kNN boost is a BoostQuery boost (KnnUtils.java:62-64); the rank-safety certificate needs score * boost monotone
+        if b is not None and not (np.isfinite(b) & ~np.signbit(b)).all():
+            raise ValueError("Boost must be a positive number")
         if filter_queries is not None:
             if filter_docs is not None:
                 raise ValueError("pass filter_docs or filter_queries, not both")
