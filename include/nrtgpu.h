@@ -275,7 +275,11 @@ int nrtgpu_search_bool_packed(nrtgpu_index* ix, const nrtgpu_clause* clauses, in
  *   missing_value: what a doc WITHOUT a value sorts as (Integer/Long.MIN|MAX_VALUE, -+Infinity in the sortable domain:
  *                  the reference picks MAX when missingLast, irrespective of `reverse`);
  *   after_values:  per query, the sort value of the last hit of the previous page (FieldDoc.fields[0]); used with
- *                  nrtgpu_query.has_after / after_doc (LastHitInfo, SortParser.parseLastHitInfo :131-160).
+ *                  nrtgpu_query.has_after / after_doc (LastHitInfo, SortParser.parseLastHitInfo :131-160). A hit
+ *                  qualifies iff its value sorts strictly after the after value, or ties with it and has a greater
+ *                  global doc id than after_doc; the value need not be held by any doc of this leaf. A doc without a
+ *                  value sorts as missing_value whether or not any doc holds that value: it ties with an after value
+ *                  equal to missing_value, and is compared by value with any other after value.
  * Results: docs in sort order, out_sort_values = the FieldDoc value of every hit (missing docs carry missing_value),
  * scores are NaN (TopFieldCollector does not track scores), totalHits exact (relation EQUAL_TO). */
 enum { NRTGPU_SORT_RELEVANCE = 0, NRTGPU_SORT_COLUMN = 1, NRTGPU_SORT_DOCID = 2 };

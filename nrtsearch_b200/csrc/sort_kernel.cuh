@@ -71,7 +71,10 @@ __device__ __forceinline__ uint32_t sort_hi(int kind, int reverse, uint32_t code
   return reverse ? code : ~code;
 }
 
-// patches DevQuery::after_key of every query with searchAfter: a hit qualifies iff key < after_key
+// patches DevQuery::after_key of every query with searchAfter: a hit qualifies iff key < after_key. An odd code is held by
+// no doc, but the docs without a value carry the code of missing_value, which may be that same odd code: an after value
+// equal to missing_value ties with them (the doc part decides, as for a held value); any other after value in the same
+// gap between held values precedes all of them or follows all of them, by the order of the two values.
 __global__ void sort_after_kernel(SortAfterLaunch S) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q == 0 && S.kind == NRTGPU_SORT_COLUMN) *S.missing_code = sort_code_of(S.distinct, S.n_distinct, S.missing_value);
@@ -81,10 +84,17 @@ __global__ void sort_after_kernel(SortAfterLaunch S) {
   if (S.kind == NRTGPU_SORT_DOCID && S.reverse) {
     key = local < 0 ? 0ull : (local >= S.n_docs ? 0xffffffffffffffffull : ((uint64_t)((uint32_t)local + 1u) << 32));
   } else {
-    uint32_t code = 0; bool exact = true;
-    if (S.kind == NRTGPU_SORT_COLUMN) { code = sort_code_of(S.distinct, S.n_distinct, S.after_values[q]); exact = (code & 1u) == 0u; }
+    uint32_t code = 0; bool exact = true, missing_follow = false;
+    if (S.kind == NRTGPU_SORT_COLUMN) {
+      const int64_t v = S.after_values[q];
+      code = sort_code_of(S.distinct, S.n_distinct, v);
+      exact = (code & 1u) == 0u || v == S.missing_value;
+      missing_follow = !exact && code == sort_code_of(S.distinct, S.n_distinct, S.missing_value) &&
+                       (S.reverse ? S.missing_value < v : S.missing_value > v);
+    }
     const uint32_t hi = sort_hi(S.kind, S.reverse, code, 0);
-    if (!exact) key = (uint64_t)hi << 32;                                   // no doc holds the value: the doc part is moot
+    if (missing_follow) key = ((uint64_t)hi + 1ull) << 32;                  // every doc with this code lacks a value and follows
+    else if (!exact) key = (uint64_t)hi << 32;                              // no doc with this code follows: the doc part is moot
     else if (local < 0) key = ((uint64_t)hi + 1ull) << 32;                  // every tied doc here follows afterDoc
     else if (local >= S.n_docs) key = (uint64_t)hi << 32;                   // every tied doc here precedes it
     else key = ((uint64_t)hi << 32) | (uint32_t)(~(uint32_t)local);
