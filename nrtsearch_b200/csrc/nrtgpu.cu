@@ -1034,6 +1034,10 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
       if (x[0]) fprintf(stderr, "[nrtgpu probe %s] %llu items, %.0f cyc/item (set-up %.0f), %.2f runs/item (%.2f staged), %.1f rounds/item, %llu driver postings (%.0f/item), %.0f queued/item, %.0f keys admitted/item, %.2f flushes/item\n",
                         k == 0 ? "simple" : "generic", x[0], (double)x[1] / x[0], (double)x[6] / x[0], (double)x[2] / x[0], (double)x[5] / x[0],
                         (double)x[7] / x[0], x[3], (double)x[3] / x[0], (double)x[16] / x[0], (double)x[17] / x[0], (double)x[4] / x[0]);
+      if (k == 0 && x[0]) fprintf(stderr, "[nrtgpu probe simple] roles: %llu items start without a threshold (%.1f%% of item cycles; slice 0 %llu, slice 1 %llu); "
+                                  "%llu items end with stale roles (%.1f%% of item cycles, %.0f cyc each, %llu driver postings, %llu in lists that turned non-essential; slice 0 %llu, slice 1 %llu)\n",
+                                  x[18], 100.0 * (double)x[19] / (double)x[1], x[20], x[21], x[22], 100.0 * (double)x[23] / (double)x[1],
+                                  x[22] ? (double)x[23] / x[22] : 0.0, x[24], x[25], x[26], x[27]);
     }
   }
   MergeLaunch M;

@@ -96,7 +96,7 @@ constexpr int kUbt = 4 * 4 * 4 * 4;          // tf-pattern bounds: min(tf, 3) pe
 static_assert(sizeof(DevProbeQuery::ubt) == kUbt * sizeof(float), "one bound per tf pattern");
 constexpr int kWq = 32 * kR;                 // per-warp queue entries: the rounds drain it below 32 after their first push; once
                                              // the buffer is full, the kR - 1 pushes left in the round are not drained
-constexpr int kProbeStats = 24;              // stats words per instantiation (ProbeLaunch::stats)
+constexpr int kProbeStats = 28;              // stats words per instantiation (ProbeLaunch::stats)
 constexpr uint32_t kPiece = 8192;            // bytes per bulk copy
 constexpr uint32_t kTfInexact = 0xFEu;       // tf byte of a plane probe whose 2-bit code saturated (tf >= 3): the exact byte is
                                              // fetched from the byte plane when the doc is scored (rare); >= 3 for the bound table
@@ -112,7 +112,9 @@ struct ProbeLaunch {
   unsigned int* work_counter;    // queue head
   unsigned long long* stats;     // optional [kProbeStats]: items, item cycles, runs, driver postings, flushes, staged runs, set-up
                                  // cycles, rounds, longest item, CTA busy (sum, max), warm-up items and cycles, flush, TMA wait and
-                                 // flush_top_k cycles, queued entries, admitted keys
+                                 // flush_top_k cycles, queued entries, admitted keys; pure-disjunction items that started with no
+                                 // threshold (count, cycles, in slice 0 / 1) and whose MAXSCORE roles went stale (count, cycles,
+                                 // driver postings, postings of the lists that turned non-essential, in slice 0 / 1)
   int32_t n_work, n_lists, n_slices, top_k;
   int32_t parts_max;             // result lists / boundary entries per slice (a heavy (query, slice) is split into up to this many items)
   int32_t slice_docs;            // multiple of kGran, <= kMaxSliceGran * kGran
@@ -175,6 +177,7 @@ struct alignas(128) ProbeSmemT {
   unsigned long long hits_known;   // max(hits0, docs known to match)
   int theta_dec;                   // 1: the item publishes (k-th key - 1) as threshold (sweep warm-up: its candidates are not output)
   unsigned long long theta;
+  int dbg_theta0;                  // profiling instantiation: the item started without a threshold
 };
 static_assert(sizeof(ProbeSmemT<kStageA>) <= 232448 / kCtasA - 1024 && sizeof(ProbeSmemT<kStageB>) <= 232448 / kCtasB - 1024, "ProbeSmem exceeds the per-CTA shared memory budget");
 
@@ -257,6 +260,45 @@ __device__ __noinline__ uint32_t probe_global(const int32_t* docs, const uint8_t
     if (__ldg(docs + mid) < doc) l = mid + 1; else h = mid;
   }
   return (l < end && __ldg(docs + l) == doc) ? (uint32_t)__ldg(f8 + l) : 0u;
+}
+
+// MAXSCORE split of a pure disjunction: the slots whose list-wide bounds sum (double, ascending) below theta.score are
+// non-essential -- they never lead, docs found only in them cannot enter the top-k. Pruning needs a threshold and, in
+// TOP_SCORES, more hits known than totalHitsThreshold (hits_known by reference: read only once theta is set).
+__device__ __forceinline__ uint32_t maxscore_nonessential(const DevProbeQuery& pq, int n_term, unsigned long long theta, bool complete,
+                                                          const unsigned long long& hits_known, int64_t threshold) {
+  uint32_t ne = 0;
+  if (theta != 0ull && (complete || (int64_t)hits_known > threshold)) {
+    const float theta_s = key_score(theta);
+    for (int a = 0; a < n_term; ++a) {
+      if (!(pq.pre[a] < theta_s)) break;
+      ne |= 1u << pq.ord[a];
+    }
+  }
+  return ne;
+}
+
+// Profiling instantiation, end of a pure-disjunction item (thread 0): the MAXSCORE roles it swept with, against the split
+// the query's threshold and hit count give now. A strict superset of non-essential lists marks an item that led with
+// lists a later split would not have led with; their postings bound what refreshing the roles inside the item could save.
+template <typename SM>
+__device__ __noinline__ void count_role_stats(const ProbeLaunch& L, const SM& sm, int qi, int slice, uint32_t ess_mask,
+                                              unsigned long long cyc, unsigned long long driver_postings) {
+  const int n_term = sm.pq.q.n_term;
+  const uint32_t all = (1u << n_term) - 1u;
+  const bool complete = L.threshold >= (int64_t)INT32_MAX;
+  const unsigned long long theta = *(volatile unsigned long long*)&L.theta[qi];
+  const unsigned long long hits = *(volatile unsigned long long*)&L.total_hits[qi];
+  const unsigned long long hits_known = hits > sm.hits_known ? hits : sm.hits_known;
+  const uint32_t ne0 = all & ~ess_mask;
+  const uint32_t ne1 = maxscore_nonessential(sm.pq, n_term, theta > sm.theta ? theta : sm.theta, complete, hits_known, L.threshold);
+  if (sm.dbg_theta0) atomicAdd(&L.stats[19], cyc);
+  if ((ne1 & ne0) == ne0 && ne1 != ne0) {
+    unsigned long long turned = 0;   // postings of the item's lists that turned non-essential
+    for (int s = 0; s < n_term; ++s) if (((ne1 & ~ne0) >> s) & 1u) turned += sm.s_ib[s] - sm.s_ia[s];
+    atomicAdd(&L.stats[22], 1ull); atomicAdd(&L.stats[23], cyc); atomicAdd(&L.stats[24], driver_postings); atomicAdd(&L.stats[25], turned);
+    if (slice <= 1) atomicAdd(&L.stats[26 + slice], 1ull);
+  }
 }
 
 // kStats: the profiling instantiation (NRTGPU_DEBUG_MODES=1) keeps cycle counters; the production one has none of their registers
@@ -365,16 +407,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       const int t = tid;
       const uint32_t all = (n_term >= 32) ? 0xffffffffu : ((1u << n_term) - 1u);
       const bool complete = L.threshold >= (int64_t)INT32_MAX;
-      // MAXSCORE split (pure disjunctions): the lists whose list-wide bounds sum (double, ascending) below theta.score
-      // are non-essential: they never lead, docs found only in them cannot enter the top-k.
-      uint32_t ne = 0;
-      if (kSimple && !sweep_warm && sm.theta != 0ull && (complete || (int64_t)sm.hits_known > L.threshold)) {
-        const float theta_s = key_score(sm.theta);
-        for (int a = 0; a < n_term; ++a) {
-          if (!(sm.pq.pre[a] < theta_s)) break;
-          ne |= 1u << sm.pq.ord[a];
-        }
-      }
+      const uint32_t ne = (kSimple && !sweep_warm) ? maxscore_nonessential(sm.pq, n_term, sm.theta, complete, sm.hits_known, L.threshold) : 0u;
       uint32_t pm = 0;
       for (int s = 0; s < n_term; ++s) if (sm.pq.kind[s] == kPlane) pm |= 1u << s;
       uint32_t drv, ess;
@@ -439,6 +472,10 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
         if (cnt_first >= 0 && g_lo < g_hi)
           atomicAdd(&L.total_hits[qi], (unsigned long long)(sm.s_ib[cnt_first] - sm.s_ia[cnt_first]));
         sm.drv_mask = drv; sm.ess_mask = ess;
+        if (kStats) {
+          sm.dbg_theta0 = kSimple && !sweep_warm && sm.theta == 0ull;
+          if (sm.dbg_theta0) { atomicAdd(&L.stats[18], 1ull); if (slice <= 1) atomicAdd(&L.stats[20 + slice], 1ull); }
+        }
       }
     }
     __syncthreads();   // B2: roles, staging plan
@@ -804,18 +841,19 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       if (lane == 0) { atomicAdd(&L.stats[16], (unsigned long long)dbg_queued); atomicAdd(&L.stats[17], (unsigned long long)dbg_admit); }
     }
     if (kStats && tid == 0) {
+      const unsigned long long cyc = (unsigned long long)(clock64() - t_start);
       atomicAdd(&L.stats[0], 1ull);
-      atomicAdd(&L.stats[1], (unsigned long long)(clock64() - t_start));
+      atomicAdd(&L.stats[1], cyc);
       atomicAdd(&L.stats[2], (unsigned long long)dbg_runs);
       atomicAdd(&L.stats[3], dbg_post);
       atomicAdd(&L.stats[4], (unsigned long long)dbg_flush);
       atomicAdd(&L.stats[5], (unsigned long long)dbg_staged);
       atomicAdd(&L.stats[6], (unsigned long long)(t_setup - t_start));
       atomicAdd(&L.stats[7], (unsigned long long)dbg_rounds);
-      const unsigned long long cyc = (unsigned long long)(clock64() - t_start);
       atomicMax(&L.stats[8], cyc);
       if (wflags & (kItemWarmDocs | kItemSweep)) { atomicAdd(&L.stats[11], 1ull); atomicAdd(&L.stats[12], cyc); }
       atomicAdd(&L.stats[13], (unsigned long long)dbg_tflush); atomicAdd(&L.stats[14], (unsigned long long)dbg_twait);
+      if (kSimple && !sweep_warm) count_role_stats(L, sm, qi, item_slice(item), ess_mask, cyc, dbg_post);
     }
   }
   if (kStats && tid == 0) {

@@ -3,6 +3,9 @@
 configs[1] and configs[2]): N runs of the TOP_SCORES batch, N of the ScoreMode.COMPLETE batch, N of the conjunctive
 batch -- nothing else launches a posting_probe kernel, so `ncu -k regex:posting_probe -s <skip> -c <count>` picks
 launches by position. Without ncu it prints the CUDA-event kernel time of each leg (stage 0 of nrtgpu_batch_stage_ms).
+With NRTGPU_DEBUG_MODES=1 the profiling instantiation writes its counters to stderr after every run: per item cycles,
+runs, rounds, driver postings, flushes, and (pure disjunctions) the items that started without a threshold and those
+whose MAXSCORE roles went stale.
 
   python tools/prof_probe.py [--runs 2] [--docs 10000000] [--legs top,complete,conj]
 """
