@@ -339,6 +339,30 @@ int nrtgpu_search_sorted_fields(nrtgpu_index* ix, const nrtgpu_sort_order* order
                                 int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
                                 uint8_t* out_terminated_early);
 
+/* Packed sorted result record: what TopFieldDocs.merge needs of one leaf or shard, in ONE device buffer (the sorted
+ * counterpart of the score record of nrtgpu_packed_words). int32 words:
+ *   docs [nq*top_k] (global ids) | counts [nq] | flags [nq] (bit 0: relation GTE, bit 1: terminated early, bit 2: hit
+ *   timeout) | pad to 8 bytes | totalHits [nq] int64 | values [nq*top_k*n_fields] int64
+ * values are out_sort_values of nrtgpu_search_sorted_fields (FieldDoc.fields of every hit); docs and values past counts[q]
+ * are 0 in a merged record. nrtgpu_sorted_packed_words = record size in words (0 for nq or top_k <= 0, n_fields outside
+ * 1..8); records must be 8-byte aligned.
+ *   nrtgpu_search_sorted_fields_packed: nrtgpu_search_sorted_fields (the same refusals and results) with the results left
+ *     in the caller-owned DEVICE record d_record; synchronises `stream`. With disallow_partial_results a timeout is
+ *     NRTGPU_ERR_TIMEOUT, as on the host path.
+ *   nrtgpu_merge_sorted_packed: TopFieldDocs.merge of n_lists records [n_lists][words] of the same Sort into d_out_record,
+ *     on `stream` (asynchronous). fields = the Sort's nrtgpu_sort_field records; only kind and reverse are read. Hits
+ *     compare field by field: COLUMN and DOCID by the value as a sortable long, ascending unless reverse; SCORE by the float
+ *     of its bits, higher first unless reverse; the fields after the first DOCID are ignored; then the global doc id
+ *     ascending. totalHits are summed and the flags ORed. NRTGPU_ERR_INVALID: n_lists < 1, n_fields outside 1..8, a bad
+ *     kind, nq <= 0, top_k outside 1..1024, an unaligned record. */
+int64_t nrtgpu_sorted_packed_words(int32_t nq, int32_t top_k, int32_t n_fields);
+int nrtgpu_search_sorted_fields_packed(nrtgpu_index* ix, const nrtgpu_sort_order* order, const nrtgpu_clause* clauses,
+                                       int32_t n_clauses, const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                       const int64_t* after_values, const nrtgpu_search_limits* limits, void* stream,
+                                       int32_t* d_record);
+int nrtgpu_merge_sorted_packed(nrtgpu_ctx* ctx, const nrtgpu_sort_field* fields, int32_t n_fields, int32_t n_lists, int32_t nq,
+                               int32_t top_k, const int32_t* d_records, int32_t* d_out_record, void* stream);
+
 /* Aggregating "additional collectors" over ALL docs matching each query (ScoreMode.COMPLETE: RelevanceCollector.java:55-62
  * forces totalHitsThreshold = MAX when additional collectors exist; fan-out SearchCollectorManager.java:192-198):
  *   NRTGPU_AGG_TERMS  counts per distinct value of a numeric doc-value column, the `size` buckets with the largest
@@ -605,6 +629,42 @@ int nrtgpu_searcher_search_bool(nrtgpu_searcher* s, const nrtgpu_clause* clauses
                                 void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
                                 int64_t* out_total_hits, uint8_t* out_relation);
 int nrtgpu_searcher_close(nrtgpu_searcher* s);
+/* The other top-k searches over the leaves: every leaf runs the request into a device record (the leaves' searches are
+ * sequential), the records are merged on the device, the merged page is copied to the host outputs (any may be NULL).
+ * Every refusal of the single-image entry point applies: the first failing leaf's code is returned and no output is
+ * written. Limits are handed to every leaf unchanged, as by nrtgpu_searcher_search_bool; a leaf's hit_timeout /
+ * terminated_early / relation GTE make the merged query's.
+ *   nrtgpu_searcher_search_sorted_fields: nrtgpu_search_sorted_fields over the leaves (TopFieldDocs.merge,
+ *     nrtgpu_merge_sorted_packed). orders[n_orders]: one nrtgpu_sort_order per leaf, in leaf order, all of the same Sort (the
+ *     same kinds and directions, and for a column field the same column, selector and missing value). after_values /
+ *     after_doc are reader-wide and go to every leaf unchanged. A one-field Sort is a one-field order here.
+ *     NRTGPU_ERR_INVALID: n_orders != the number of leaves, an order made on another index than its leaf, orders of
+ *     different Sorts.
+ *   nrtgpu_searcher_search_tree_phrases: nrtgpu_search_tree_phrases over the leaves (n_nodes / n_phrases may be 0);
+ *     TopDocs.merge of the leaves' pages by nrtgpu_merge_topk_packed.
+ *   nrtgpu_searcher_search_knn / _filtered: the single-image kNN searches over the leaves (per-leaf exact top-k, then
+ *     TopDocs.merge by score desc, doc asc). filter: one byte per global doc id (leaf l reads filter[doc_base ..
+ *     doc_base + n_docs)). A leaf without vectors contributes no hits; NRTGPU_ERR_INVALID when no leaf has vectors. */
+int nrtgpu_searcher_search_sorted_fields(nrtgpu_searcher* s, const nrtgpu_sort_order* const* orders, int32_t n_orders,
+                                         const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_query* queries, int32_t nq,
+                                         int32_t top_k, int32_t flags, const int64_t* after_values,
+                                         const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs,
+                                         int64_t* out_sort_values, int32_t* out_counts, int64_t* out_total_hits,
+                                         uint8_t* out_relation, uint8_t* out_hit_timeout, uint8_t* out_terminated_early);
+int nrtgpu_searcher_search_tree_phrases(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                                        int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                                        const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                                        int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags,
+                                        const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs, float* out_scores,
+                                        int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation,
+                                        uint8_t* out_hit_timeout, uint8_t* out_terminated_early);
+int nrtgpu_searcher_search_knn(nrtgpu_searcher* s, const float* queries, int32_t nq, int32_t k, const float* boosts /*[nq] or NULL*/,
+                               const uint8_t* filter /*one byte per global doc or NULL*/, void* stream, int32_t* out_docs,
+                               float* out_scores, int32_t* out_counts);
+int nrtgpu_searcher_search_knn_filtered(nrtgpu_searcher* s, const float* queries, int32_t nq, int32_t k, const float* boosts,
+                                        const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses, const nrtgpu_query* filters,
+                                        int32_t n_filters, const int32_t* filter_of, void* stream, int32_t* out_docs,
+                                        float* out_scores, int32_t* out_counts);
 
 /* Request micro-batcher: the reference's search API is ONE query per RPC (clientlib/src/main/proto/yelp/nrtsearch/
  * luceneserver.proto:164), each on its own SERVER-pool thread (GrpcServerExecutorSupplier.java:68-75). Handler threads call

@@ -134,6 +134,43 @@ public final class NrtGpu {
   public static native int indexUpdateStats(
       long index, ByteBuffer termDf, ByteBuffer fieldDocCount, ByteBuffer fieldSumTtf);
 
+  /** Size in int32 words of a packed sorted record (include/nrtgpu.h nrtgpu_sorted_packed_words). */
+  public static native long sortedPackedWords(int nq, int topK, int nFields);
+
+  /** searchSortedFields with the results left in the DEVICE record at address dRecord. */
+  public static native int searchSortedFieldsPacked(
+      long index, long order, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK,
+      int flags, ByteBuffer afterValues, ByteBuffer limits, long dRecord);
+
+  /** TopFieldDocs.merge of nLists DEVICE sorted records at dRecords into dOutRecord; fields = the Sort's nrtgpu_sort_field. */
+  public static native int mergeSortedPacked(
+      long ctx, ByteBuffer fields, int nFields, int nLists, int nq, int topK, long dRecords, long dOutRecord);
+
+  /** Sorted search over the leaves of a searcher: orders = one sort order handle (int64) per leaf, all of one Sort. */
+  public static native int searcherSearchSortedFields(
+      long searcher, ByteBuffer orders, int nOrders, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq,
+      int topK, int flags, ByteBuffer afterValues, ByteBuffer limits, ByteBuffer outDocs, ByteBuffer outSortValues,
+      ByteBuffer outCounts, ByteBuffer outTotalHits, ByteBuffer outRelation, ByteBuffer outHitTimeout,
+      ByteBuffer outTerminatedEarly);
+
+  /** searchTreePhrases over the leaves of a searcher. */
+  public static native int searcherSearchTreePhrases(
+      long searcher, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer phrases, int nPhrases,
+      ByteBuffer phraseTerms, int nPhraseTerms, ByteBuffer queries, int nq, int topK, int totalHitsThreshold, int flags,
+      ByteBuffer limits, ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits,
+      ByteBuffer outRelation, ByteBuffer outHitTimeout, ByteBuffer outTerminatedEarly);
+
+  /** searchKnn over the leaves of a searcher; filter = one byte per global doc id (or null). */
+  public static native int searcherSearchKnn(
+      long searcher, ByteBuffer queries, int nq, int k, ByteBuffer boosts, ByteBuffer filter,
+      ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts);
+
+  /** searchKnnFiltered over the leaves of a searcher. */
+  public static native int searcherSearchKnnFiltered(
+      long searcher, ByteBuffer queries, int nq, int k, ByteBuffer boosts, ByteBuffer filterClauses,
+      int nFilterClauses, ByteBuffer filters, int nFilters, ByteBuffer filterOf, ByteBuffer outDocs,
+      ByteBuffer outScores, ByteBuffer outCounts);
+
   public static native long batcherCreate(long index, int maxBatch, int maxWaitUs);
 
   /** Blocks until the batch this request rode in is back; diag = nrtgpu_diagnostics (24 bytes) or null. */

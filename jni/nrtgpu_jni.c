@@ -243,6 +243,72 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_indexUpdateStat
   return fail(env, nrtgpu_index_update_stats((nrtgpu_index*)(intptr_t)ix, (const int64_t*)ADDR(env, termDf),
                                              (const int64_t*)ADDR(env, fieldDocCount), (const int64_t*)ADDR(env, fieldSumTtf)));
 }
+/* packed sorted records (nrtgpu_sorted_packed_words): dRecord / dRecords / dOutRecord are DEVICE addresses (the buffers a
+ * multi-GPU step all-gathers), fields a direct ByteBuffer of nFields nrtgpu_sort_field */
+JNIEXPORT jlong JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_sortedPackedWords(JNIEnv* env, jclass c, jint nq, jint topK, jint nFields) {
+  return (jlong)nrtgpu_sorted_packed_words(nq, topK, nFields);
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchSortedFieldsPacked(
+    JNIEnv* env, jclass c, jlong ix, jlong order, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
+    jobject afterValues, jobject limits, jlong dRecord) {
+  return fail(env, nrtgpu_search_sorted_fields_packed((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_sort_order*)(intptr_t)order,
+                                                      (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                                      (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                                      (const int64_t*)ADDR(env, afterValues),
+                                                      (const nrtgpu_search_limits*)ADDR(env, limits), NULL, (int32_t*)(intptr_t)dRecord));
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_mergeSortedPacked(
+    JNIEnv* env, jclass c, jlong ctx, jobject fields, jint nFields, jint nLists, jint nq, jint topK, jlong dRecords, jlong dOutRecord) {
+  return fail(env, nrtgpu_merge_sorted_packed((nrtgpu_ctx*)(intptr_t)ctx, (const nrtgpu_sort_field*)ADDR(env, fields), nFields, nLists,
+                                              nq, topK, (const int32_t*)(intptr_t)dRecords, (int32_t*)(intptr_t)dOutRecord, NULL));
+}
+/* searchers over the leaves of one reader version: orders = a direct ByteBuffer of nOrders sort order handles (int64 each) */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchSortedFields(
+    JNIEnv* env, jclass c, jlong s, jobject orders, jint nOrders, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK,
+    jint flags, jobject afterValues, jobject limits, jobject outDocs, jobject outSortValues, jobject outCounts, jobject outTotalHits,
+    jobject outRelation, jobject outHitTimeout, jobject outTerminatedEarly) {
+  return fail(env, nrtgpu_searcher_search_sorted_fields((nrtgpu_searcher*)(intptr_t)s, (const nrtgpu_sort_order* const*)ADDR(env, orders),
+                                                        nOrders, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                                        (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                                        (const int64_t*)ADDR(env, afterValues),
+                                                        (const nrtgpu_search_limits*)ADDR(env, limits), NULL, (int32_t*)ADDR(env, outDocs),
+                                                        (int64_t*)ADDR(env, outSortValues), (int32_t*)ADDR(env, outCounts),
+                                                        (int64_t*)ADDR(env, outTotalHits), (uint8_t*)ADDR(env, outRelation),
+                                                        (uint8_t*)ADDR(env, outHitTimeout), (uint8_t*)ADDR(env, outTerminatedEarly)));
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchTreePhrases(
+    JNIEnv* env, jclass c, jlong s, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,
+    jobject phraseTerms, jint nPhraseTerms, jobject queries, jint nq, jint topK, jint totalHitsThreshold, jint flags,
+    jobject limits, jobject outDocs, jobject outScores, jobject outCounts, jobject outTotalHits, jobject outRelation,
+    jobject outHitTimeout, jobject outTerminatedEarly) {
+  return fail(env, nrtgpu_searcher_search_tree_phrases((nrtgpu_searcher*)(intptr_t)s, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                                       (const nrtgpu_node*)ADDR(env, nodes), nNodes,
+                                                       (const nrtgpu_phrase*)ADDR(env, phrases), nPhrases,
+                                                       (const nrtgpu_phrase_term*)ADDR(env, phraseTerms), nPhraseTerms,
+                                                       (const nrtgpu_query*)ADDR(env, queries), nq, topK, totalHitsThreshold, flags,
+                                                       (const nrtgpu_search_limits*)ADDR(env, limits), NULL,
+                                                       (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
+                                                       (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits),
+                                                       (uint8_t*)ADDR(env, outRelation), (uint8_t*)ADDR(env, outHitTimeout),
+                                                       (uint8_t*)ADDR(env, outTerminatedEarly)));
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchKnn(
+    JNIEnv* env, jclass c, jlong s, jobject queries, jint nq, jint k, jobject boosts, jobject filter, jobject outDocs,
+    jobject outScores, jobject outCounts) {
+  return fail(env, nrtgpu_searcher_search_knn((nrtgpu_searcher*)(intptr_t)s, (const float*)ADDR(env, queries), nq, k,
+                                              (const float*)ADDR(env, boosts), (const uint8_t*)ADDR(env, filter), NULL,
+                                              (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores), (int32_t*)ADDR(env, outCounts)));
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchKnnFiltered(
+    JNIEnv* env, jclass c, jlong s, jobject queries, jint nq, jint k, jobject boosts, jobject filterClauses,
+    jint nFilterClauses, jobject filters, jint nFilters, jobject filterOf, jobject outDocs, jobject outScores, jobject outCounts) {
+  return fail(env, nrtgpu_searcher_search_knn_filtered((nrtgpu_searcher*)(intptr_t)s, (const float*)ADDR(env, queries), nq, k,
+                                                       (const float*)ADDR(env, boosts), (const nrtgpu_clause*)ADDR(env, filterClauses),
+                                                       nFilterClauses, (const nrtgpu_query*)ADDR(env, filters), nFilters,
+                                                       (const int32_t*)ADDR(env, filterOf), NULL, (int32_t*)ADDR(env, outDocs),
+                                                       (float*)ADDR(env, outScores), (int32_t*)ADDR(env, outCounts)));
+}
+
 /* micro-batcher: one per searcher version; submit blocks the calling gRPC handler thread until its batch is back.
  * diag: 24-byte direct buffer laid out as nrtgpu_diagnostics, or null */
 JNIEXPORT jlong JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_batcherCreate(JNIEnv* env, jclass c, jlong ix, jint maxBatch, jint maxWaitUs) {

@@ -134,6 +134,9 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_index_add_positions", "nrtgpu_search_tree_phrases", "nrtgpu_batch_prepare_tree_phrases",
     "nrtgpu_score_docs_tree", "nrtgpu_rescore_query_tree",
     "nrtgpu_search_bool_aggs_nested",
+    "nrtgpu_sorted_packed_words", "nrtgpu_search_sorted_fields_packed", "nrtgpu_merge_sorted_packed",
+    "nrtgpu_searcher_search_sorted_fields", "nrtgpu_searcher_search_tree_phrases", "nrtgpu_searcher_search_knn",
+    "nrtgpu_searcher_search_knn_filtered",
 ]
 
 _gpu = None
@@ -223,6 +226,25 @@ def gpu_lib() -> C.CDLL:
         lib.nrtgpu_searcher_search_bool.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32,
                                                     C.c_int32, C.POINTER(SearchLimits), C.c_void_p] + [C.c_void_p] * 5
         lib.nrtgpu_searcher_close.argtypes = [C.c_void_p]
+        lib.nrtgpu_sorted_packed_words.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+        lib.nrtgpu_sorted_packed_words.restype = C.c_int64
+        lib.nrtgpu_search_sorted_fields_packed.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Query),
+                                                           C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(SearchLimits),
+                                                           C.c_void_p, C.c_void_p]
+        lib.nrtgpu_merge_sorted_packed.argtypes = [C.c_void_p, C.POINTER(SortField), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.nrtgpu_searcher_search_sorted_fields.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Clause), C.c_int32,
+                                                             C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                                             C.POINTER(SearchLimits), C.c_void_p] + [C.c_void_p] * 7
+        lib.nrtgpu_searcher_search_tree_phrases.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32,
+                                                            C.POINTER(Phrase), C.c_int32, C.POINTER(PhraseTerm), C.c_int32,
+                                                            C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                            C.POINTER(SearchLimits), C.c_void_p] + [C.c_void_p] * 7
+        lib.nrtgpu_searcher_search_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.nrtgpu_searcher_search_knn_filtered.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(Clause),
+                                                            C.c_int32, C.POINTER(Query), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                            C.c_void_p, C.c_void_p]
         lib.nrtgpu_batcher_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
         lib.nrtgpu_batcher_submit.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Diagnostics)]

@@ -249,6 +249,7 @@ struct nrtgpu_sort_order {
   bool score_first = false; int32_t score_reverse = 0;
   int32_t n_rank = 0;                   // fields of the rank: after the leading SCORE, up to the first DOCID inclusive
   SortFieldDev f[kMaxSortFields] = {};  // every field of the Sort (device pointers into the image)
+  nrtgpu_sort_field spec[kMaxSortFields] = {};   // the Sort as given (orders of the leaves of one searcher must agree)
   DevBuf<int32_t> perm;                 // position -> doc
   DevBuf<uint32_t> rank;                // doc -> position + 1
 };
@@ -316,10 +317,14 @@ struct nrtgpu_batch {
   // optional caller-provided device output buffers (e.g. torch tensors feeding the NCCL all-gather)
   int32_t* bound_docs = nullptr; float* bound_scores = nullptr; int32_t* bound_counts = nullptr;
   long long* bound_total = nullptr; int32_t* bound_flags = nullptr;   // packed record (nrtgpu_batch_bind_packed)
+  int64_t* bound_values = nullptr;   // sorted record (batch_bind_sorted): FieldDoc values
   int32_t* o_docs() { return bound_docs ? bound_docs : out_docs.p; }
   float* o_scores() { return bound_scores ? bound_scores : out_scores.p; }
   int32_t* o_counts() { return bound_counts ? bound_counts : out_counts.p; }
-  void unbind() { bound_docs = nullptr; bound_scores = nullptr; bound_counts = nullptr; bound_total = nullptr; bound_flags = nullptr; }
+  int64_t* o_sort_values() { return bound_values ? bound_values : out_sort_values.p; }
+  void unbind() {
+    bound_docs = nullptr; bound_scores = nullptr; bound_counts = nullptr; bound_total = nullptr; bound_flags = nullptr; bound_values = nullptr;
+  }
   ~nrtgpu_batch() { for (auto& r : ev) for (auto& e : r) if (e) cudaEventDestroy(e); }
 };
 
@@ -1056,7 +1061,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
     V.docs = b->o_docs(); V.counts = b->o_counts(); V.nq = b->nq; V.top_k = b->top_k; V.doc_base = b->ix->doc_base;
     V.n_fields = o->n_fields; V.score_first = o->score_first ? 1 : 0; V.score_reverse = o->score_reverse;
     for (int i = 0; i < o->n_fields; ++i) V.f[i] = o->f[i];
-    V.perm = o->perm.p; V.scores = b->o_scores(); V.out_values = b->out_sort_values.p;
+    V.perm = o->perm.p; V.scores = b->o_scores(); V.out_values = b->o_sort_values();
     const int n = b->nq * b->top_k;
     sort_fields_values_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(V);
     NRT_CUDA_TRY(cudaGetLastError());
@@ -1066,7 +1071,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
     const bool col = b->sort_kind == NRTGPU_SORT_COLUMN;
     V.c64 = col ? b->ix->col64[(size_t)b->sort_column]->p : nullptr; V.c32 = col ? b->ix->col32[(size_t)b->sort_column]->p : nullptr;
     V.has = col ? b->ix->col_has[(size_t)b->sort_column]->p : nullptr; V.missing_value = b->sort_missing_value;
-    V.out_values = b->out_sort_values.p; V.out_scores = b->o_scores();
+    V.out_values = b->o_sort_values(); V.out_scores = b->o_scores();
     const int n = b->nq * b->top_k;
     sort_values_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(V);
     NRT_CUDA_TRY(cudaGetLastError());
@@ -1331,7 +1336,7 @@ int nrtgpu_batch_device_results(nrtgpu_batch* b, int32_t** d_docs, float** d_sco
 int nrtgpu_batch_bind_output(nrtgpu_batch* b, int32_t* d_docs, float* d_scores, int32_t* d_counts) {
   if (!b) NRT_FAIL(NRTGPU_ERR_INVALID, "NULL batch");
   b->bound_docs = d_docs; b->bound_scores = d_scores; b->bound_counts = d_counts;
-  b->bound_total = nullptr; b->bound_flags = nullptr;
+  b->bound_total = nullptr; b->bound_flags = nullptr; b->bound_values = nullptr;
   return NRTGPU_OK;
 }
 
@@ -1348,6 +1353,7 @@ int nrtgpu_batch_bind_packed(nrtgpu_batch* b, int32_t* d_record) {
   if (!d_record) { b->unbind(); return NRTGPU_OK; }
   if (((uintptr_t)d_record & 7u) != 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_bind_packed: record must be 8-byte aligned");
   const int64_t n = (int64_t)b->nq * b->top_k;
+  b->bound_values = nullptr;
   b->bound_docs = d_record; b->bound_scores = (float*)(d_record + n); b->bound_counts = d_record + 2 * n;
   b->bound_flags = d_record + 2 * n + b->nq;
   int64_t w = 2 * n + 2ll * b->nq; w = (w + 1) & ~1ll;
@@ -1411,6 +1417,18 @@ int nrtgpu_batch_free(nrtgpu_batch* b) {
   return NRTGPU_OK;
 }
 
+// redirects the results of subsequent runs of a sort-order batch into a sorted record (sorted_record_layout); the scores the
+// score-first key needs stay in the batch's own buffer
+static int batch_bind_sorted(nrtgpu_batch* b, int32_t* d_record, int32_t n_fields) {
+  if (((uintptr_t)d_record & 7u) != 0) NRT_FAIL(NRTGPU_ERR_INVALID, "sorted record must be 8-byte aligned");
+  if (!b->order || n_fields <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "a sorted record needs a sort order");
+  const SortedRecordLayout L = sorted_record_layout(b->nq, b->top_k, n_fields);
+  b->unbind();
+  b->bound_docs = d_record; b->bound_counts = d_record + L.counts; b->bound_flags = d_record + L.flags;
+  b->bound_total = (long long*)(d_record + L.totals); b->bound_values = (int64_t*)(d_record + L.values);
+  return NRTGPU_OK;
+}
+
 // a pooled batch workspace of the index (device buffers survive between calls: no cudaMalloc on the request path), checked
 // out for one call; returned with its bound outputs cleared
 struct WorkspaceLease {
@@ -1426,9 +1444,13 @@ struct WorkspaceLease {
 };
 
 // where a one-shot search leaves its results: a packed DEVICE record (the multi-GPU path: the caller all-gathers it on
-// the stream), or else the HOST buffers (any may be NULL)
+// the stream), a packed sorted DEVICE record (d_sorted_record, searches with a sort order), or else the HOST buffers (any
+// may be NULL). record_limits: a record also carries what batch_fetch_impl derives from the limits on the host (hit_timeout
+// as flags bit 2 and relation GTE, the terminateAfterMaxRecallCount cap, and NRTGPU_ERR_TIMEOUT with disallow_partial_results).
 struct SearchOut {
   int32_t* d_record = nullptr;
+  int32_t* d_sorted_record = nullptr;
+  bool record_limits = false;
   int32_t* docs = nullptr; float* scores = nullptr; int32_t* counts = nullptr; int64_t* total_hits = nullptr;
   uint8_t* relation = nullptr; uint8_t* hit_timeout = nullptr; uint8_t* terminated_early = nullptr;
   int64_t* sort_values = nullptr;
@@ -1444,9 +1466,27 @@ static int search_bool_impl(nrtgpu_index* ix, const BatchRequest& r, const nrtgp
   int rc = batch_build(b, ix, r, (cudaStream_t)stream);
   if (!rc) rc = batch_set_limits(b, limits, (cudaStream_t)stream);
   if (!rc && out.d_record) rc = nrtgpu_batch_bind_packed(b, out.d_record);
+  if (!rc && out.d_sorted_record) rc = batch_bind_sorted(b, out.d_sorted_record, r.sort_order ? r.sort_order->n_fields : 0);
   if (!rc) rc = nrtgpu_batch_run(b, stream);
   if (rc) return rc;
-  if (out.d_record) { cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream); if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; } return NRTGPU_OK; }
+  if (out.d_record || out.d_sorted_record) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (out.record_limits && (b->limits_active || b->terminate_after_max_recall > 0)) {
+      record_limits_kernel<<<(unsigned)((r.nq + 127) / 128), 128, 0, st>>>(r.nq, b->limits_active ? b->timed_out.p : nullptr,
+                                                                          b->terminate_after_max_recall, b->bound_flags, b->bound_total);
+      NRT_CUDA_TRY(cudaGetLastError());
+    }
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; }
+    if (out.record_limits && b->limits_active && b->disallow_partial) {
+      std::vector<int32_t>& to = b->h_flags;
+      to.resize((size_t)r.nq);
+      NRT_CUDA_TRY(cudaMemcpy(to.data(), b->timed_out.p, (size_t)r.nq * sizeof(int32_t), cudaMemcpyDeviceToHost));
+      for (int q = 0; q < r.nq; ++q)
+        if (to[(size_t)q]) NRT_FAIL(NRTGPU_ERR_TIMEOUT, "Search collection exceeded timeout of " + std::to_string(b->timeout_sec) + "s");
+    }
+    return NRTGPU_OK;
+  }
   if (out.sort_values && b->sort_kind != NRTGPU_SORT_RELEVANCE) {
     const size_t nv = (size_t)r.nq * r.top_k * (r.sort_order ? r.sort_order->n_fields : 1);
     cudaError_t e = cudaMemcpyAsync(out.sort_values, b->out_sort_values.p, nv * sizeof(int64_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
@@ -1542,6 +1582,7 @@ int nrtgpu_sort_order_create(nrtgpu_index* ix, const nrtgpu_sort_field* fields, 
   for (int i = 0; i < n_fields; ++i) {
     const nrtgpu_sort_field& s = fields[i];
     SortFieldDev& f = o->f[i];
+    o->spec[i] = s;
     f.kind = s.kind; f.reverse = s.reverse != 0; f.selector = s.selector; f.missing = s.missing_value;
     if (s.kind == NRTGPU_SORT_COLUMN) {
       if (s.column < 0 || s.column >= ix->n_columns) NRT_FAIL(NRTGPU_ERR_INVALID, "sort column out of range (field does not support sorting: no doc values)");
@@ -1598,6 +1639,45 @@ int nrtgpu_search_sorted_fields(nrtgpu_index* ix, const nrtgpu_sort_order* order
   SearchOut o; o.docs = out_docs; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
   o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early; o.sort_values = out_sort_values;
   return search_bool_impl(ix, r, limits, stream, o);
+}
+
+int64_t nrtgpu_sorted_packed_words(int32_t nq, int32_t top_k, int32_t n_fields) {
+  if (nq <= 0 || top_k <= 0 || n_fields < 1 || n_fields > kMaxSortFields) return 0;
+  return sorted_record_layout(nq, top_k, n_fields).words;
+}
+
+int nrtgpu_search_sorted_fields_packed(nrtgpu_index* ix, const nrtgpu_sort_order* order, const nrtgpu_clause* clauses,
+                                       int32_t n_clauses, const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                       const int64_t* after_values, const nrtgpu_search_limits* limits, void* stream,
+                                       int32_t* d_record) {
+  if (!ix || !order || !d_record) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_sorted_fields_packed: NULL argument");
+  if (order->ix != ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_sorted_fields_packed: the sort order was made on another index");
+  BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
+  r.sort_order = order; r.order_after = after_values;
+  SearchOut o; o.d_sorted_record = d_record; o.record_limits = true;
+  return search_bool_impl(ix, r, limits, stream, o);
+}
+
+int nrtgpu_merge_sorted_packed(nrtgpu_ctx* ctx, const nrtgpu_sort_field* fields, int32_t n_fields, int32_t n_lists, int32_t nq,
+                               int32_t top_k, const int32_t* d_records, int32_t* d_out_record, void* stream) {
+  if (!ctx || !fields || !d_records || !d_out_record) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_merge_sorted_packed: NULL argument");
+  if (n_lists < 1 || n_fields < 1 || n_fields > kMaxSortFields || nq <= 0 || top_k <= 0 || top_k > kMaxTopK)
+    NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_merge_sorted_packed: bad argument");
+  if ((((uintptr_t)d_records | (uintptr_t)d_out_record) & 7u) != 0)
+    NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_merge_sorted_packed: records must be 8-byte aligned");
+  SortMergeLaunch S{};
+  S.records = d_records; S.out = d_out_record; S.L = sorted_record_layout(nq, top_k, n_fields);
+  S.n_lists = n_lists; S.nq = nq; S.top_k = top_k; S.n_fields = n_fields; S.n_cmp = n_fields;
+  for (int i = n_fields - 1; i >= 0; --i) {   // the fields after the first DOCID cannot decide anything
+    const int32_t k = fields[i].kind;
+    if (k != NRTGPU_SORT_COLUMN && k != NRTGPU_SORT_DOCID && k != NRTGPU_SORT_SCORE) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_merge_sorted_packed: bad sort field kind");
+    if (k == NRTGPU_SORT_DOCID) S.n_cmp = i + 1;
+    S.kind[i] = k; S.reverse[i] = fields[i].reverse != 0;
+  }
+  NRT_CUDA_TRY(cudaSetDevice(ctx->device));
+  sort_merge_kernel<<<(unsigned)nq, kSortMergeThreads, 0, (cudaStream_t)stream>>>(S);
+  NRT_CUDA_TRY(cudaGetLastError());
+  return NRTGPU_OK;
 }
 
 int nrtgpu_search_bool_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -2137,6 +2217,8 @@ int nrtgpu_rescore_combine(nrtgpu_ctx* ctx, int32_t nq, int32_t n_hits, const in
   return NRTGPU_OK;
 }
 
+}  // extern "C"
+
 // ---- searcher over several leaf images of one shard (NRT: a new reader version adds images for the NEW leaves only)
 struct nrtgpu_searcher {
   nrtgpu_ctx* ctx = nullptr;
@@ -2145,6 +2227,85 @@ struct nrtgpu_searcher {
   DevBuf<int32_t> records, merged;   // [n_leaves][words], [words]
   std::vector<int32_t> host;
 };
+
+// the flags word of a record: relation GTE, terminated early, hit timeout
+static void unpack_record_flags(const int32_t* flags, int32_t nq, uint8_t* out_relation, uint8_t* out_hit_timeout,
+                                uint8_t* out_terminated_early) {
+  for (int q = 0; q < nq; ++q) {
+    if (out_relation) out_relation[q] = (uint8_t)(flags[q] & 1);
+    if (out_terminated_early) out_terminated_early[q] = (uint8_t)((flags[q] >> 1) & 1);
+    if (out_hit_timeout) out_hit_timeout[q] = (uint8_t)((flags[q] >> 2) & 1);
+  }
+}
+
+// Score-ranked search over the leaves: run(l, d_record) leaves leaf l's page in its packed score record
+// (nrtgpu_packed_words), the records are merged on the device (TopDocs.merge: nrtgpu_merge_topk_packed) and the merged
+// page is copied to the host outputs (any may be NULL). The first failing leaf's code is returned and no output is written.
+template <class Fn>
+static int searcher_scored(nrtgpu_searcher* s, const char* fn, int32_t nq, int32_t top_k, void* stream, Fn&& run, int32_t* out_docs,
+                           float* out_scores, int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation,
+                           uint8_t* out_hit_timeout, uint8_t* out_terminated_early) {
+  if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, std::string(fn) + ": NULL searcher");
+  if (nq <= 0 || top_k <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, std::string(fn) + ": nq and top_k must be > 0");
+  NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> g(s->mu);
+  const int64_t words = nrtgpu_packed_words(nq, top_k);
+  const int n_leaves = (int)s->leaves.size();
+  int rc;
+  if ((rc = s->records.alloc((size_t)words * n_leaves)) || (rc = s->merged.alloc((size_t)words))) return rc;
+  for (int l = 0; l < n_leaves; ++l)
+    if ((rc = run(l, s->records.p + (size_t)l * words))) return rc;
+  NRT_CUDA_TRY(cudaMemsetAsync(s->merged.p, 0, (size_t)words * sizeof(int32_t), st));   // slots past a query's count read 0
+  if ((rc = nrtgpu_merge_topk_packed(s->ctx, n_leaves, nq, top_k, s->records.p, s->merged.p, stream))) return rc;
+  s->host.resize((size_t)words);
+  NRT_CUDA_TRY(cudaMemcpyAsync(s->host.data(), s->merged.p, (size_t)words * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  NRT_CUDA_TRY(cudaStreamSynchronize(st));
+  const int64_t n = (int64_t)nq * top_k;
+  int64_t w = 2 * n + 2ll * nq; w = (w + 1) & ~1ll;
+  if (out_docs) std::memcpy(out_docs, s->host.data(), (size_t)n * 4);
+  if (out_scores) std::memcpy(out_scores, s->host.data() + n, (size_t)n * 4);
+  if (out_counts) std::memcpy(out_counts, s->host.data() + 2 * n, (size_t)nq * 4);
+  unpack_record_flags(s->host.data() + 2 * n + nq, nq, out_relation, out_hit_timeout, out_terminated_early);
+  if (out_total_hits) std::memcpy(out_total_hits, s->host.data() + w, (size_t)nq * 8);
+  return NRTGPU_OK;
+}
+
+// a kNN page of one leaf (host pages of the single-image search) uploaded into a packed score record; a leaf without
+// vectors contributes an empty page
+template <class Fn>
+static int knn_leaf_record(nrtgpu_index* ix, int32_t nq, int32_t k, void* stream, int32_t* d_record, Fn&& search) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t n = (size_t)nq * k;
+  NRT_CUDA_TRY(cudaMemsetAsync(d_record, 0, (size_t)nrtgpu_packed_words(nq, k) * sizeof(int32_t), st));
+  if (ix->vec_dims <= 0) return NRTGPU_OK;
+  std::vector<int32_t> docs(n), counts((size_t)nq);
+  std::vector<float> scores(n);
+  if (int rc = search(docs.data(), scores.data(), counts.data())) return rc;
+  NRT_CUDA_TRY(cudaMemcpyAsync(d_record, docs.data(), n * 4, cudaMemcpyHostToDevice, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(d_record + n, scores.data(), n * 4, cudaMemcpyHostToDevice, st));
+  NRT_CUDA_TRY(cudaMemcpyAsync(d_record + 2 * n, counts.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+  NRT_CUDA_TRY(cudaStreamSynchronize(st));   // the staging vectors are freed on return
+  return NRTGPU_OK;
+}
+
+static bool searcher_has_vectors(const nrtgpu_searcher* s) {
+  for (const nrtgpu_index* ix : s->leaves) if (ix->vec_dims > 0) return true;
+  return false;
+}
+
+// two sort orders rank by the same Sort: every field's kind and direction, and a column field's column, selector and missing value
+static bool same_sort(const nrtgpu_sort_order* a, const nrtgpu_sort_order* b) {
+  if (a->n_fields != b->n_fields) return false;
+  for (int i = 0; i < a->n_fields; ++i) {
+    const nrtgpu_sort_field &x = a->spec[i], &y = b->spec[i];
+    if (x.kind != y.kind || (x.reverse != 0) != (y.reverse != 0)) return false;
+    if (x.kind == NRTGPU_SORT_COLUMN && (x.column != y.column || x.selector != y.selector || x.missing_value != y.missing_value)) return false;
+  }
+  return true;
+}
+
+extern "C" {
 
 int nrtgpu_searcher_create(nrtgpu_ctx* ctx, nrtgpu_index* const* leaves, int32_t n_leaves, nrtgpu_searcher** out) {
   if (!ctx || !leaves || n_leaves <= 0 || !out) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_create: bad argument");
@@ -2189,6 +2350,96 @@ int nrtgpu_searcher_search_bool(nrtgpu_searcher* s, const nrtgpu_clause* clauses
   if (out_relation) for (int q = 0; q < nq; ++q) out_relation[q] = (uint8_t)(s->host[(size_t)(2 * n + nq + q)] & 1);
   if (out_total_hits) std::memcpy(out_total_hits, s->host.data() + w, (size_t)nq * 8);
   return NRTGPU_OK;
+}
+
+int nrtgpu_searcher_search_sorted_fields(nrtgpu_searcher* s, const nrtgpu_sort_order* const* orders, int32_t n_orders,
+                                         const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_query* queries, int32_t nq,
+                                         int32_t top_k, int32_t flags, const int64_t* after_values,
+                                         const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs,
+                                         int64_t* out_sort_values, int32_t* out_counts, int64_t* out_total_hits,
+                                         uint8_t* out_relation, uint8_t* out_hit_timeout, uint8_t* out_terminated_early) {
+  if (!s || !orders) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_sorted_fields: NULL argument");
+  const int n_leaves = (int)s->leaves.size();
+  if (n_orders != n_leaves) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_sorted_fields: one sort order per leaf is needed");
+  for (int l = 0; l < n_leaves; ++l) {
+    if (!orders[l]) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_sorted_fields: NULL sort order");
+    if (orders[l]->ix != s->leaves[(size_t)l])
+      NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_sorted_fields: the sort order of leaf " + std::to_string(l) + " was made on another index");
+    if (!same_sort(orders[l], orders[0])) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_sorted_fields: the leaves' sort orders are of different Sorts");
+  }
+  if (nq <= 0 || top_k <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_sorted_fields: nq and top_k must be > 0");
+  NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> g(s->mu);
+  const int32_t nf = orders[0]->n_fields;
+  const SortedRecordLayout L = sorted_record_layout(nq, top_k, nf);
+  int rc;
+  if ((rc = s->records.alloc((size_t)L.words * n_leaves)) || (rc = s->merged.alloc((size_t)L.words))) return rc;
+  for (int l = 0; l < n_leaves; ++l)   // every leaf pages after the same reader-wide FieldDoc
+    if ((rc = nrtgpu_search_sorted_fields_packed(s->leaves[(size_t)l], orders[l], clauses, n_clauses, queries, nq, top_k, flags, after_values,
+                                                 limits, stream, s->records.p + (size_t)l * L.words))) return rc;
+  // TopFieldDocs.merge over the leaves
+  if ((rc = nrtgpu_merge_sorted_packed(s->ctx, orders[0]->spec, nf, n_leaves, nq, top_k, s->records.p, s->merged.p, stream))) return rc;
+  s->host.resize((size_t)L.words);
+  NRT_CUDA_TRY(cudaMemcpyAsync(s->host.data(), s->merged.p, (size_t)L.words * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  NRT_CUDA_TRY(cudaStreamSynchronize(st));
+  const int64_t n = (int64_t)nq * top_k;
+  if (out_docs) std::memcpy(out_docs, s->host.data(), (size_t)n * 4);
+  if (out_sort_values) std::memcpy(out_sort_values, s->host.data() + L.values, (size_t)n * nf * 8);
+  if (out_counts) std::memcpy(out_counts, s->host.data() + L.counts, (size_t)nq * 4);
+  unpack_record_flags(s->host.data() + L.flags, nq, out_relation, out_hit_timeout, out_terminated_early);
+  if (out_total_hits) std::memcpy(out_total_hits, s->host.data() + L.totals, (size_t)nq * 8);
+  return NRTGPU_OK;
+}
+
+int nrtgpu_searcher_search_tree_phrases(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                                        int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                                        const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                                        int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags,
+                                        const nrtgpu_search_limits* limits, void* stream, int32_t* out_docs, float* out_scores,
+                                        int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation,
+                                        uint8_t* out_hit_timeout, uint8_t* out_terminated_early) {
+  if (n_nodes < 0 || (n_nodes > 0 && !nodes)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_tree: bad nodes");
+  BatchRequest r = tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags);
+  int rc = phrase_request(&r, phrases, n_phrases, phrase_terms, n_phrase_terms);
+  if (rc) return rc;
+  return searcher_scored(s, "nrtgpu_searcher_search_tree_phrases", nq, top_k, stream, [&](int l, int32_t* d_record) {
+    SearchOut o; o.d_record = d_record; o.record_limits = true;
+    return search_bool_impl(s->leaves[(size_t)l], r, limits, stream, o);
+  }, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
+}
+
+int nrtgpu_searcher_search_knn(nrtgpu_searcher* s, const float* queries, int32_t nq, int32_t k, const float* boosts,
+                               const uint8_t* filter, void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts) {
+  if (!s || !queries || !out_docs || !out_scores || !out_counts) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn: NULL argument");
+  if (!searcher_has_vectors(s)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn: no leaf has a vector field");
+  if (nq <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn: nq must be > 0");
+  if (k <= 0 || k > kMaxTopK) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn: k out of range");
+  if (!knn_boosts_valid(boosts, nq)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn: a boost must be finite and >= 0");
+  return searcher_scored(s, "nrtgpu_searcher_search_knn", nq, k, stream, [&](int l, int32_t* d_record) {
+    nrtgpu_index* ix = s->leaves[(size_t)l];
+    return knn_leaf_record(ix, nq, k, stream, d_record, [&](int32_t* d, float* sc, int32_t* c) {
+      return nrtgpu_search_knn(ix, queries, nq, k, boosts, filter ? filter + ix->doc_base : nullptr, stream, d, sc, c);
+    });
+  }, out_docs, out_scores, out_counts, nullptr, nullptr, nullptr, nullptr);
+}
+
+int nrtgpu_searcher_search_knn_filtered(nrtgpu_searcher* s, const float* queries, int32_t nq, int32_t k, const float* boosts,
+                                        const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses, const nrtgpu_query* filters,
+                                        int32_t n_filters, const int32_t* filter_of, void* stream, int32_t* out_docs,
+                                        float* out_scores, int32_t* out_counts) {
+  if (!s || !queries || !out_docs || !out_scores || !out_counts || !filter_of || (n_filters > 0 && !filters))
+    NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn_filtered: NULL argument");
+  if (!searcher_has_vectors(s)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn_filtered: no leaf has a vector field");
+  if (nq <= 0 || n_filters < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn_filtered: nq must be > 0 and n_filters >= 0");
+  if (k <= 0 || k > kMaxTopK) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn_filtered: k out of range");
+  return searcher_scored(s, "nrtgpu_searcher_search_knn_filtered", nq, k, stream, [&](int l, int32_t* d_record) {
+    nrtgpu_index* ix = s->leaves[(size_t)l];
+    return knn_leaf_record(ix, nq, k, stream, d_record, [&](int32_t* d, float* sc, int32_t* c) {
+      return nrtgpu_search_knn_filtered(ix, queries, nq, k, boosts, filter_clauses, n_filter_clauses, filters, n_filters, filter_of,
+                                        stream, d, sc, c);
+    });
+  }, out_docs, out_scores, out_counts, nullptr, nullptr, nullptr, nullptr);
 }
 
 #include "batcher.inc"

@@ -293,4 +293,129 @@ __global__ void sort_fields_values_kernel(SortFieldsValuesLaunch S) {
     out[j] = S.f[j].kind == NRTGPU_SORT_SCORE ? (int64_t)__float_as_uint(score) : sort_field_value(S.f[j], d, S.doc_base);
 }
 
+// ---- TopFieldDocs.merge of packed sorted records (nrtgpu_merge_sorted_packed; record layout in include/nrtgpu.h) ----
+// Word offsets of the parts of one sorted record: docs [nq*top_k] | counts [nq] | flags [nq] | pad to 8 B | totalHits [nq]
+// int64 | values [nq*top_k*n_fields] int64. Every part that holds int64 starts on an even word.
+struct SortedRecordLayout {
+  int64_t counts, flags, totals, values, words;
+};
+__host__ __device__ inline SortedRecordLayout sorted_record_layout(int32_t nq, int32_t top_k, int32_t n_fields) {
+  SortedRecordLayout L;
+  const int64_t n = (int64_t)nq * top_k;
+  L.counts = n; L.flags = n + nq;
+  L.totals = (n + 2ll * nq + 1) & ~1ll;
+  L.values = L.totals + 2ll * nq;
+  L.words = L.values + 2 * n * n_fields;
+  return L;
+}
+
+constexpr int kSortMergeThreads = 256;
+
+struct SortMergeLaunch {
+  const int32_t* records;        // [n_lists][L.words]
+  int32_t* out;                  // [L.words]
+  SortedRecordLayout L;
+  int32_t n_lists, nq, top_k, n_fields;
+  int32_t n_cmp;                 // fields that decide: up to and including the first DOCID
+  int32_t kind[kMaxSortFields], reverse[kMaxSortFields];
+};
+
+// entries of query q in record r (clamped to [0, top_k])
+__device__ __forceinline__ int sort_record_count(const int32_t* r, int64_t counts, int q, int K) {
+  const int c = r[counts + q];
+  return c < 0 ? 0 : (c > K ? K : c);
+}
+
+// ascending merge key of one FieldDoc value: COLUMN / DOCID by the sortable long, SCORE by its float bits, higher first
+__device__ __forceinline__ uint64_t sort_merge_key(int32_t kind, int32_t reverse, int64_t v) {
+  if (kind == NRTGPU_SORT_SCORE) {
+    const uint32_t o = float_to_ordered(__uint_as_float((uint32_t)v));
+    return (uint64_t)(reverse ? o : ~o);
+  }
+  return sortable_u64(v) ^ (reverse ? ~0ull : 0ull);
+}
+
+// One CTA per query, a merge by rank: entry i of list l lands at position i + (entries of every other list m that sort
+// before it), each counted by a binary search of list m. Entries that tie on every field and the doc are ordered by list
+// (lists m < l first), so the positions are a permutation even then; global doc ids of distinct leaves never tie.
+// An entry stops searching once its position reaches top_k. Slots past the merged count are zeroed.
+__global__ void __launch_bounds__(kSortMergeThreads) sort_merge_kernel(SortMergeLaunch S) {
+  const int q = blockIdx.x;
+  const int tid = threadIdx.x;
+  const SortedRecordLayout L = S.L;
+  const int K = S.top_k, F = S.n_fields;
+  int32_t* out_docs = S.out + (size_t)q * K;
+  int64_t* out_vals = (int64_t*)(S.out + L.values) + (size_t)q * K * F;
+  __shared__ int32_t s_total;
+  if (tid == 0) {
+    long long t = 0; int32_t f = 0, n = 0;
+    for (int m = 0; m < S.n_lists; ++m) {
+      const int32_t* r = S.records + (size_t)m * L.words;
+      t += ((const long long*)(r + L.totals))[q];
+      f |= r[L.flags + q];
+      n += sort_record_count(r, L.counts, q, K);
+    }
+    n = n < K ? n : K;
+    S.out[L.counts + q] = n; S.out[L.flags + q] = f; ((long long*)(S.out + L.totals))[q] = t;
+    s_total = n;
+  }
+  __syncthreads();
+  const int n_out = s_total;
+  for (int i = n_out + tid; i < K; i += kSortMergeThreads) {
+    out_docs[i] = 0;
+    for (int j = 0; j < F; ++j) out_vals[(size_t)i * F + j] = 0;
+  }
+  for (int l = 0; l < S.n_lists; ++l) {
+    const int32_t* rl = S.records + (size_t)l * L.words;
+    const int cl = sort_record_count(rl, L.counts, q, K);
+    const int32_t* docs_l = rl + (size_t)q * K;
+    const int64_t* vals_l = (const int64_t*)(rl + L.values) + (size_t)q * K * F;
+    for (int i = tid; i < cl; i += kSortMergeThreads) {
+      const int32_t doc = docs_l[i];
+      const int64_t* v = vals_l + (size_t)i * F;
+      uint64_t ke[kMaxSortFields];
+#pragma unroll
+      for (int f = 0; f < kMaxSortFields; ++f) ke[f] = f < S.n_cmp ? sort_merge_key(S.kind[f], S.reverse[f], v[f]) : 0ull;
+      int pos = i;
+      for (int m = 0; m < S.n_lists && pos < K; ++m) {
+        if (m == l) continue;
+        const int32_t* rm = S.records + (size_t)m * L.words;
+        const int32_t* docs_m = rm + (size_t)q * K;
+        const int64_t* vals_m = (const int64_t*)(rm + L.values) + (size_t)q * K * F;
+        int lo = 0, hi = sort_record_count(rm, L.counts, q, K);   // first entry of list m that does not sort before (l, i)
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          const int64_t* w = vals_m + (size_t)mid * F;
+          int c = 0;
+#pragma unroll
+          for (int f = 0; f < kMaxSortFields; ++f) {
+            if (f < S.n_cmp && c == 0) {
+              const uint64_t k = sort_merge_key(S.kind[f], S.reverse[f], w[f]);
+              c = k < ke[f] ? -1 : (k > ke[f] ? 1 : 0);
+            }
+          }
+          if (c == 0) { const int32_t d = docs_m[mid]; c = d < doc ? -1 : (d > doc ? 1 : (m < l ? -1 : 1)); }
+          if (c < 0) lo = mid + 1; else hi = mid;
+        }
+        pos += lo;
+      }
+      if (pos < K) {
+        out_docs[pos] = doc;
+        for (int j = 0; j < F; ++j) out_vals[(size_t)pos * F + j] = v[j];
+      }
+    }
+  }
+}
+
+// a leaf's sorted or score record after its run: a timed-out query is partial (hit_timeout, relation GTE), and the
+// totalHits of a query that terminateAfter cut short are capped at terminateAfterMaxRecallCount (as batch_fetch_impl does
+// for host results)
+__global__ void record_limits_kernel(int32_t nq, const int32_t* __restrict__ timed_out, long long max_recall,
+                                     int32_t* __restrict__ flags, long long* __restrict__ totals) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nq) return;
+  if (timed_out && timed_out[q]) flags[q] |= 1 | 4;
+  if (max_recall > 0 && (flags[q] & 2) && totals[q] > max_recall) totals[q] = max_recall;
+}
+
 }  // namespace nrtgpu

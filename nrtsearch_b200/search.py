@@ -913,6 +913,85 @@ class GpuLeafSearcher:
                                                     out.relation.ctypes.data))
         return out
 
+    def search_sorted(self, queries: Sequence[object], collector: SortFieldCollector,
+                      search_after: Optional[Sequence[Optional[FieldDoc]]] = None, stream: int = 0) -> SortedResult:
+        """GpuIndexSearcher.search_sorted over the leaves (nrtgpu_searcher_search_sorted_fields): every leaf searches with its
+        cached order of the Sort (GpuIndex.sort_order), the pages are merged on the device (TopFieldDocs.merge). A one-field
+        Sort runs as a one-field order and returns sort_values [nq, k], as the single-image search does; search_after holds
+        reader-wide FieldDocs."""
+        st = collector.sort
+        fields = [st] if isinstance(st, SortType) else list(st)
+        orders = (C.c_void_p * len(self.leaves))(*[l.sort_order(fields, stream).value for l in self.leaves])
+        nf = len(fields)
+        after_sd = None if search_after is None else [None if a is None else ScoreDoc(a.doc, 0.0) for a in search_after]
+        carr, ncl, qarr, nq = compile_queries(queries, after_sd)
+        k = collector.num_hits_to_collect
+        out = SortedResult(np.zeros((nq, k), np.int32), np.zeros((nq, k, nf), np.int64), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
+                           np.zeros(nq, np.uint8), np.zeros(nq, np.uint8), np.zeros(nq, np.uint8))
+        av = None
+        if search_after is not None:
+            av = np.zeros((nq, nf), np.int64)
+            for i, a in enumerate(search_after):
+                if a is not None:
+                    av[i] = a.values if a.values is not None else (a.value,)
+        lim = None
+        if collector.timeout_sec > 0 or collector.terminate_after > 0:
+            lim = SearchLimits(collector.timeout_sec, 0.0, 0, collector.terminate_after, 0)
+        check(self._lib.nrtgpu_searcher_search_sorted_fields(self.handle, orders, len(self.leaves), carr, ncl, qarr, nq, k, 0,
+                                                             None if av is None else av.ctypes.data,
+                                                             None if lim is None else C.byref(lim), C.c_void_p(stream),
+                                                             out.docs.ctypes.data, out.sort_values.ctypes.data, out.counts.ctypes.data,
+                                                             out.total_hits.ctypes.data, out.relation.ctypes.data,
+                                                             out.hit_timeout.ctypes.data, out.terminated_early.ctypes.data))
+        if isinstance(st, SortType) and st.field != "score":
+            out.sort_values = out.sort_values.reshape(nq, k)
+        return out
+
+    def search_tree(self, queries: Sequence[object], collector: RelevanceCollector,
+                    search_after: Optional[Sequence[Optional[ScoreDoc]]] = None, stream: int = 0) -> BatchResult:
+        """GpuIndexSearcher.search_tree over the leaves (nrtgpu_searcher_search_tree_phrases): query trees and phrases, the
+        leaves' pages merged on the device (TopDocs.merge)."""
+        if search_after is None and collector.search_after is not None:
+            search_after = [collector.search_after] * len(queries)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, search_after, phrase_table=True)
+        k = collector.num_hits_to_collect
+        out = BatchResult(np.zeros((nq, max(k, 1)), np.int32), np.zeros((nq, max(k, 1)), np.float32),
+                          np.zeros(nq, np.int32), np.zeros(nq, np.int64), np.zeros(nq, np.uint8),
+                          np.zeros(nq, np.uint8), np.zeros(nq, np.uint8))
+        lim = collector.limits()
+        check(self._lib.nrtgpu_searcher_search_tree_phrases(self.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k,
+                                                            collector.total_hits_threshold, 0, None if lim is None else C.byref(lim),
+                                                            C.c_void_p(stream), out.docs.ctypes.data, out.scores.ctypes.data,
+                                                            out.counts.ctypes.data, out.total_hits.ctypes.data, out.relation.ctypes.data,
+                                                            out.hit_timeout.ctypes.data, out.terminated_early.ctypes.data))
+        return out
+
+    def knn(self, queries: np.ndarray, k: int, boosts: Optional[np.ndarray] = None,
+            filter_docs: Optional[np.ndarray] = None, stream: int = 0, filter_queries: Optional[Sequence[Optional[object]]] = None):
+        """GpuIndexSearcher.knn over the leaves (nrtgpu_searcher_search_knn / _filtered): every leaf's exact top-k, merged by
+        (score desc, doc asc) on the device. filter_docs: one 0/1 byte per global doc id of the reader."""
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        nq = q.shape[0]
+        docs = np.zeros((nq, k), np.int32)
+        scores = np.zeros((nq, k), np.float32)
+        counts = np.zeros(nq, np.int32)
+        b = None if boosts is None else np.ascontiguousarray(boosts, dtype=np.float32)
+        if b is not None and not (np.isfinite(b) & ~np.signbit(b)).all():
+            raise ValueError("Boost must be a positive number")
+        if filter_queries is not None:
+            if filter_docs is not None:
+                raise ValueError("pass filter_docs or filter_queries, not both")
+            carr, ncl, qarr, nf, filter_of = compile_filters(filter_queries, nq)
+            check(self._lib.nrtgpu_searcher_search_knn_filtered(self.handle, q.ctypes.data, nq, k, None if b is None else b.ctypes.data,
+                                                                carr, ncl, qarr, nf, filter_of.ctypes.data, C.c_void_p(stream),
+                                                                docs.ctypes.data, scores.ctypes.data, counts.ctypes.data))
+            return docs, scores, counts
+        f = None if filter_docs is None else np.ascontiguousarray(filter_docs, dtype=np.uint8)
+        check(self._lib.nrtgpu_searcher_search_knn(self.handle, q.ctypes.data, nq, k, None if b is None else b.ctypes.data,
+                                                   None if f is None else f.ctypes.data, C.c_void_p(stream),
+                                                   docs.ctypes.data, scores.ctypes.data, counts.ctypes.data))
+        return docs, scores, counts
+
     def close(self):
         if self.handle:
             self._lib.nrtgpu_searcher_close(self.handle)

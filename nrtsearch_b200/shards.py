@@ -110,6 +110,62 @@ class PackedGather:
         return unpack_record(r, self.nq, self.k)
 
 
+class SortedPackedGather:
+    """The sorted counterpart of PackedGather: every rank's packed sorted record (docs, counts, flags, totalHits and the
+    FieldDoc values of all queries; include/nrtgpu.h nrtgpu_sorted_packed_words), filled by
+    nrtgpu_search_sorted_fields_packed, is all-gathered once, then nrtgpu_merge_sorted_packed does TopFieldDocs.merge on
+    every rank. fields: the Sort's SortTypes (search.SortType)."""
+
+    def __init__(self, nq: int, k: int, fields, world: int, device):
+        import torch
+        from . import _native
+        self.nq, self.k, self.world = nq, k, world
+        self.fields = list(fields)
+        self.n_fields = len(self.fields)
+        self.words = (int(_native.gpu_lib().nrtgpu_sorted_packed_words(nq, k, self.n_fields)) if device.type == "cuda"
+                      else sorted_packed_words(nq, k, self.n_fields))
+        self.local = torch.zeros(self.words, dtype=torch.int32, device=device)
+        self.all = torch.zeros(world * self.words, dtype=torch.int32, device=device)
+        self.merged = torch.zeros(self.words, dtype=torch.int32, device=device)
+
+    def gather(self, group=None):
+        import torch.distributed as dist
+        if self.world == 1:
+            self.all.copy_(self.local)
+        else:
+            dist.all_gather_into_tensor(self.all, self.local, group=group)
+
+    def merge_on_device(self, ctx, stream: int):
+        import ctypes
+        from . import _native
+        cf = [f.c_field() for f in self.fields]
+        arr = (_native.SortField * len(cf))(*cf)
+        _native.check(_native.gpu_lib().nrtgpu_merge_sorted_packed(
+            ctx.handle, arr, self.n_fields, self.world, self.nq, self.k, self.all.data_ptr(), self.merged.data_ptr(),
+            ctypes.c_void_p(stream)))
+
+    def unpack(self, record=None):
+        """Host view of a record: docs [nq,k], values [nq,k,n_fields], counts [nq], flags [nq], total_hits [nq]."""
+        r = (self.merged if record is None else record).cpu().numpy()
+        return unpack_sorted_record(r, self.nq, self.k, self.n_fields)
+
+
+def sorted_packed_words(nq: int, k: int, n_fields: int) -> int:
+    w = (nq * k + 2 * nq + 1) & ~1
+    return w + 2 * nq + 2 * nq * k * n_fields
+
+
+def unpack_sorted_record(r: np.ndarray, nq: int, k: int, n_fields: int):
+    n = nq * k
+    w = (n + 2 * nq + 1) & ~1
+    docs = r[:n].reshape(nq, k)
+    counts = r[n:n + nq]
+    flags = r[n + nq:n + 2 * nq]
+    total = r[w:w + 2 * nq].view(np.int64)
+    values = r[w + 2 * nq:w + 2 * nq + 2 * n * n_fields].view(np.int64).reshape(nq, k, n_fields)
+    return docs, values, counts, flags, total
+
+
 def packed_words(nq: int, k: int) -> int:
     w = nq * k * 2 + 2 * nq
     w = (w + 1) & ~1
