@@ -665,6 +665,26 @@ int nrtgpu_searcher_search_knn_filtered(nrtgpu_searcher* s, const float* queries
                                         const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses, const nrtgpu_query* filters,
                                         int32_t n_filters, const int32_t* filter_of, void* stream, int32_t* out_docs,
                                         float* out_scores, int32_t* out_counts);
+/* nrtgpu_searcher_search_bool_aggs_nested: nrtgpu_search_bool_aggs_nested over the leaves (n_nested may be 0). Terms buckets
+ * are counted by value across the leaves, as TermsCollectorManager.reduce merges its per-slice maps: each leaf numbers a
+ * column's values in its own dictionary, so the first aggregation on a column builds the searcher's reader-wide dictionary
+ * of it (the union of the leaves' distinct values, and per leaf its doc codes renumbered to it: 4 B per doc, except in a
+ * leaf whose dictionary is the union or that holds no value), kept until nrtgpu_searcher_close. Every leaf counts into one
+ * set of tables of nq x U buckets (U: the union's size), and buckets, totalBuckets, otherCounts and the nested values are
+ * selected once from them. Nested top hits are chosen per reader-wide bucket over every leaf's hits, ties by global doc; the
+ * scores are the leaves' own, the shard's when the leaves carry the index-wide statistics. The page is TopDocs.merge of the
+ * leaves' pages (nrtgpu_merge_topk_packed); totalHits is exact and summed over the leaves.
+ *   Every refusal of nrtgpu_search_bool_aggs_nested applies with the same code and message, on every leaf: query trees and
+ *   wide batches are NRTGPU_ERR_UNSUPPORTED, so is a column multi-valued in any leaf; a column index some leaf lacks is
+ *   NRTGPU_ERR_INVALID. The 2 GB limits of the count and nested-word tables apply at the reader-wide U: a batch whose leaves
+ *   each fit but whose union does not is refused before any batch is built or table allocated. On a refusal no output is
+ *   written. NULL searcher: NRTGPU_ERR_INVALID. */
+int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                            const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                            const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                                            const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                            const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs,
+                                            float* out_scores, int32_t* out_counts, int64_t* out_total_hits);
 
 /* Request micro-batcher: the reference's search API is ONE query per RPC (clientlib/src/main/proto/yelp/nrtsearch/
  * luceneserver.proto:164), each on its own SERVER-pool thread (GrpcServerExecutorSupplier.java:68-75). Handler threads call

@@ -171,6 +171,15 @@ public final class NrtGpu {
       int nFilterClauses, ByteBuffer filters, int nFilters, ByteBuffer filterOf, ByteBuffer outDocs,
       ByteBuffer outScores, ByteBuffer outCounts);
 
+  /**
+   * searchBoolAggsNested over the leaves of a searcher (nNested may be 0): terms buckets counted by value across the
+   * leaves, nested top hits chosen per reader-wide bucket; the same buffers as searchBoolAggsNested.
+   */
+  public static native int searcherSearchBoolAggsNested(
+      long searcher, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK, int flags, ByteBuffer aggs,
+      int nAggs, ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, ByteBuffer outDocs,
+      ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits);
+
   public static native long batcherCreate(long index, int maxBatch, int maxWaitUs);
 
   /** Blocks until the batch this request rode in is back; diag = nrtgpu_diagnostics (24 bytes) or null. */

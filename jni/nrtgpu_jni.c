@@ -197,34 +197,41 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_rescoreQueryTre
 }
 /* additional collectors with nested collectors. aggs / nested: direct ByteBuffers of nrtgpu_aggregation[nAggs] /
  * nrtgpu_nested_aggregation[nNested]; aggOut: 6 direct buffers (or null) per aggregation in nrtgpu_aggregation_result field
- * order, nestedOut: 5 per nested collector in nrtgpu_nested_result field order. */
+ * order, nestedOut: 5 per nested collector in nrtgpu_nested_result field order. agg_results unpacks aggOut / nestedOut into
+ * the result records (freed by the caller, also when it fails). */
+static int agg_results(JNIEnv* env, jobjectArray aggOut, jint nAggs, jobjectArray nestedOut, jint nNested,
+                       nrtgpu_aggregation_result** out_ar, nrtgpu_nested_result** out_nr) {
+  nrtgpu_aggregation_result* ar = *out_ar = (nrtgpu_aggregation_result*)calloc(nAggs > 0 ? (size_t)nAggs : 1, sizeof(*ar));
+  nrtgpu_nested_result* nr = *out_nr = (nrtgpu_nested_result*)calloc(nNested > 0 ? (size_t)nNested : 1, sizeof(*nr));
+  if (!ar || !nr) return NRTGPU_ERR_OOM;
+  for (jint i = 0; i < nAggs; ++i) {
+    void* p[6];
+    for (int f = 0; f < 6; ++f) p[f] = ADDR(env, (*env)->GetObjectArrayElement(env, aggOut, 6 * i + f));
+    ar[i].values = (double*)p[0]; ar[i].bucket_keys = (int64_t*)p[1]; ar[i].bucket_counts = (int32_t*)p[2];
+    ar[i].n_buckets = (int32_t*)p[3]; ar[i].total_buckets = (int32_t*)p[4]; ar[i].other_counts = (int64_t*)p[5];
+  }
+  for (jint i = 0; i < nNested; ++i) {
+    void* p[5];
+    for (int f = 0; f < 5; ++f) p[f] = ADDR(env, (*env)->GetObjectArrayElement(env, nestedOut, 5 * i + f));
+    nr[i].values = (double*)p[0]; nr[i].hit_docs = (int32_t*)p[1]; nr[i].hit_scores = (float*)p[2];
+    nr[i].hit_counts = (int32_t*)p[3]; nr[i].hit_total = (int64_t*)p[4];
+  }
+  return NRTGPU_OK;
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchBoolAggsNested(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
     jobject aggs, jint nAggs, jobjectArray aggOut, jobject nested, jint nNested, jobjectArray nestedOut, jobject outDocs,
     jobject outScores, jobject outCounts, jobject outTotalHits) {
-  nrtgpu_aggregation_result* ar = (nrtgpu_aggregation_result*)calloc(nAggs > 0 ? (size_t)nAggs : 1, sizeof(*ar));
-  nrtgpu_nested_result* nr = (nrtgpu_nested_result*)calloc(nNested > 0 ? (size_t)nNested : 1, sizeof(*nr));
-  int rc = NRTGPU_ERR_OOM;
-  if (ar && nr) {
-    for (jint i = 0; i < nAggs; ++i) {
-      void* p[6];
-      for (int f = 0; f < 6; ++f) p[f] = ADDR(env, (*env)->GetObjectArrayElement(env, aggOut, 6 * i + f));
-      ar[i].values = (double*)p[0]; ar[i].bucket_keys = (int64_t*)p[1]; ar[i].bucket_counts = (int32_t*)p[2];
-      ar[i].n_buckets = (int32_t*)p[3]; ar[i].total_buckets = (int32_t*)p[4]; ar[i].other_counts = (int64_t*)p[5];
-    }
-    for (jint i = 0; i < nNested; ++i) {
-      void* p[5];
-      for (int f = 0; f < 5; ++f) p[f] = ADDR(env, (*env)->GetObjectArrayElement(env, nestedOut, 5 * i + f));
-      nr[i].values = (double*)p[0]; nr[i].hit_docs = (int32_t*)p[1]; nr[i].hit_scores = (float*)p[2];
-      nr[i].hit_counts = (int32_t*)p[3]; nr[i].hit_total = (int64_t*)p[4];
-    }
+  nrtgpu_aggregation_result* ar = NULL;
+  nrtgpu_nested_result* nr = NULL;
+  int rc = agg_results(env, aggOut, nAggs, nestedOut, nNested, &ar, &nr);
+  if (!rc)
     rc = nrtgpu_search_bool_aggs_nested((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
                                         (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
                                         (const nrtgpu_aggregation*)ADDR(env, aggs), nAggs, ar,
                                         (const nrtgpu_nested_aggregation*)ADDR(env, nested), nNested, nr, NULL,
                                         (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
                                         (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
-  }
   free(ar);
   free(nr);
   return fail(env, rc);
@@ -307,6 +314,24 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchK
                                                        nFilterClauses, (const nrtgpu_query*)ADDR(env, filters), nFilters,
                                                        (const int32_t*)ADDR(env, filterOf), NULL, (int32_t*)ADDR(env, outDocs),
                                                        (float*)ADDR(env, outScores), (int32_t*)ADDR(env, outCounts)));
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchBoolAggsNested(
+    JNIEnv* env, jclass c, jlong s, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
+    jobject aggs, jint nAggs, jobjectArray aggOut, jobject nested, jint nNested, jobjectArray nestedOut, jobject outDocs,
+    jobject outScores, jobject outCounts, jobject outTotalHits) {
+  nrtgpu_aggregation_result* ar = NULL;
+  nrtgpu_nested_result* nr = NULL;
+  int rc = agg_results(env, aggOut, nAggs, nestedOut, nNested, &ar, &nr);
+  if (!rc)
+    rc = nrtgpu_searcher_search_bool_aggs_nested((nrtgpu_searcher*)(intptr_t)s, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                                 (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                                 (const nrtgpu_aggregation*)ADDR(env, aggs), nAggs, ar,
+                                                 (const nrtgpu_nested_aggregation*)ADDR(env, nested), nNested, nr, NULL,
+                                                 (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
+                                                 (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
+  free(ar);
+  free(nr);
+  return fail(env, rc);
 }
 
 /* micro-batcher: one per searcher version; submit blocks the calling gRPC handler thread until its batch is back.

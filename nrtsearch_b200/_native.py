@@ -136,7 +136,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_search_bool_aggs_nested",
     "nrtgpu_sorted_packed_words", "nrtgpu_search_sorted_fields_packed", "nrtgpu_merge_sorted_packed",
     "nrtgpu_searcher_search_sorted_fields", "nrtgpu_searcher_search_tree_phrases", "nrtgpu_searcher_search_knn",
-    "nrtgpu_searcher_search_knn_filtered",
+    "nrtgpu_searcher_search_knn_filtered", "nrtgpu_searcher_search_bool_aggs_nested",
 ]
 
 _gpu = None
@@ -245,6 +245,7 @@ def gpu_lib() -> C.CDLL:
         lib.nrtgpu_searcher_search_knn_filtered.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(Clause),
                                                             C.c_int32, C.POINTER(Query), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                             C.c_void_p, C.c_void_p]
+        lib.nrtgpu_searcher_search_bool_aggs_nested.argtypes = lib.nrtgpu_search_bool_aggs_nested.argtypes
         lib.nrtgpu_batcher_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
         lib.nrtgpu_batcher_submit.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Diagnostics)]

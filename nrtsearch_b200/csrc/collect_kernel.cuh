@@ -195,11 +195,12 @@ struct AggNestedDev {
   int32_t column, value_type;   // MIN / MAX / SUM
   int32_t size;                 // TOP_HITS: the parent's size (slots per query)
   int32_t q_lo, q_hi;           // TOP_HITS: the queries of this pass-2 group
+  int32_t doc_base;             // TOP_HITS: the image's first global doc (keys of several leaves share the segments)
   unsigned long long* dvals;    // MIN / MAX / SUM: [nq][n_buckets] words as AggSpecDev::dvals
   const int32_t* slot_of;       // TOP_HITS: [nq][n_buckets] returned slot of the bucket, -1: not returned
   const long long* hit_off;     // TOP_HITS: [q_hi - q_lo][size] first key of the (query, slot)
   unsigned int* hit_fill;       // TOP_HITS: [q_hi - q_lo][size] keys written
-  uint64_t* hit_keys;           // TOP_HITS: make_key(score, doc) of the collected docs
+  uint64_t* hit_keys;           // TOP_HITS: make_key(score, global doc) of the collected docs
 };
 struct AggLaunch {
   AggSpecDev a[kMaxAggs];
@@ -248,7 +249,7 @@ __device__ __noinline__ void agg_nested_collect(const AggLaunch& A, int i, const
     const int slot = n.slot_of[cell];
     if (slot < 0) continue;
     const size_t s = (size_t)(q - n.q_lo) * n.size + slot;
-    n.hit_keys[n.hit_off[s] + atomicAdd(&n.hit_fill[s], 1u)] = make_key(score, doc);   // sized by the bucket's count
+    n.hit_keys[n.hit_off[s] + atomicAdd(&n.hit_fill[s], 1u)] = make_key(score, doc + n.doc_base);   // sized by the bucket's count
   }
 }
 
@@ -268,6 +269,27 @@ __device__ __forceinline__ void agg_collect(const AggLaunch& A, const DevIndexVi
       agg_metric_collect(s.kind, s.column, s.value_type, &s.dvals[q], ix, doc);
     }
   }
+}
+
+// ---- reader-wide value dictionary of a searcher over several leaves: every leaf numbers a column's values in its own
+// dictionary (col_distinct, col_code), so a leaf's codes are renumbered to the sorted union of the leaves' dictionaries,
+// whose bucket g is code 2g + 2 in every leaf. Union order is value order, so the selection's tie rules hold unchanged.
+// the reader-wide bucket of each bucket of a leaf: the position of its value in the union (where it is present)
+__global__ void dict_map_kernel(const uint64_t* __restrict__ leaf, int32_t n_leaf, const uint64_t* __restrict__ uni, int32_t n_uni,
+                                uint32_t* __restrict__ map) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_leaf) return;
+  const uint64_t v = leaf[i];
+  int lo = 0, hi = n_uni;
+  while (lo < hi) { const int m = (lo + hi) >> 1; if (uni[m] < v) lo = m + 1; else hi = m; }
+  map[i] = (uint32_t)lo;
+}
+// a leaf's codes through that map: 2b + 2 -> 2 map[b] + 2; 0 (no value) stays 0
+__global__ void dict_remap_kernel(const uint32_t* __restrict__ codes, int32_t n, const uint32_t* __restrict__ map, uint32_t* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t c = codes[i];
+  out[i] = c ? 2u * map[(c >> 1) - 1] + 2u : 0u;
 }
 
 // the double a min / max / sum word stands for, the collectors' unset value where no doc had a value

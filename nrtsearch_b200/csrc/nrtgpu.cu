@@ -9,10 +9,13 @@
 #include "knn_filter_kernel.cuh"
 #include "hybrid_kernel.cuh"
 
+#include <thrust/unique.h>
+
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
 #include <deque>
+#include <map>
 #include <thread>
 #include <unordered_map>
 #include <cfloat>
@@ -254,6 +257,20 @@ struct nrtgpu_sort_order {
   DevBuf<uint32_t> rank;                // doc -> position + 1
 };
 
+// Where the additional collectors of a run count (cb.aggs, cb.nested): per aggregation its count table [nq][n_buckets]
+// (terms) or metric words [nq] (min / max / sum), the bucket codes of its column and the distinct values they number; per
+// nested min / max / sum collector its words [nq][n_buckets of the parent]. A single image fills it from the batch's own
+// buffers and the image's columns on every run; a searcher points the batches of all its leaves at one set of reader-wide
+// tables, each with that leaf's codes (agg_shared).
+struct AggTables {
+  unsigned int* counts[kMaxAggs];
+  unsigned long long* dvals[kMaxAggs];
+  const uint32_t* codes[kMaxAggs];
+  int32_t n_buckets[kMaxAggs];
+  const uint64_t* distinct[kMaxAggs];
+  unsigned long long* nest_words[kMaxAggs * kMaxNested];
+};
+
 struct nrtgpu_batch {
   nrtgpu_index* ix = nullptr;
   int32_t nq = 0, top_k = 0;
@@ -286,6 +303,8 @@ struct nrtgpu_batch {
   DevBuf<unsigned int> agg_counts[kMaxAggs];
   DevBuf<unsigned long long> agg_dvals[kMaxAggs];
   DevBuf<AggLaunch> agg_launch;
+  AggTables agg_tab = {};      // the tables of the current run (agg_shared: set by the searcher, not reset by the run)
+  bool agg_shared = false;
   DevBuf<int64_t> agg_keys; DevBuf<int32_t> agg_cnts, agg_n, agg_tot; DevBuf<long long> agg_other;
   // nested collectors (cb.nested): [nq][n_buckets] words of the min / max / sum ones (pass 1), the selection's returned
   // buckets and slot map, and the top-hits run's key buffers (pass 2)
@@ -754,6 +773,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
   const int32_t nq = r.nq, top_k = r.top_k;
   b->order = sort_order;
   b->ran = false; b->runs_recorded = 0;
+  b->agg_shared = false;
   if (sort_order) {   // fields-only order: the COLUMN key with the rank as its code; [score, ...]: kSortScoreRank
     b->sort_kind = sort_order->score_first ? kSortScoreRank : NRTGPU_SORT_COLUMN; b->sort_column = 0;
     b->sort_reverse = sort_order->score_first ? sort_order->score_reverse : 0; b->sort_missing_value = 0;
@@ -938,6 +958,43 @@ static int probe_launch(nrtgpu_batch* b, v3::ProbeLaunch P, bool debug, cudaStre
   return NRTGPU_OK;
 }
 
+// a column's bucket codes and sorted distinct values in an image (NULL in an image without docs: it has no such arrays)
+static const uint32_t* ix_col_code(const nrtgpu_index* ix, int32_t c) {
+  return (size_t)c < ix->col_code.size() ? ix->col_code[(size_t)c]->p : nullptr;
+}
+static const uint64_t* ix_col_distinct(const nrtgpu_index* ix, int32_t c) {
+  return (size_t)c < ix->col_distinct.size() ? ix->col_distinct[(size_t)c]->p : nullptr;
+}
+
+// Allocates the tables of the batch's collectors in its own buffers, n_buckets[i] buckets for terms aggregation i, and
+// resets them on `st`: counts to 0, min words to +inf and max words to -inf in ordered-double space, sums to 0.0 (the
+// "unset" values are applied at fetch). Fills every field of *t but the codes and distinct values, which are the caller's.
+static int batch_agg_tables(nrtgpu_batch* b, const int32_t* n_buckets, cudaStream_t st, AggTables* t) {
+  int rc;
+  for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
+    const nrtgpu_aggregation& a = b->cb.aggs[i];
+    if (a.kind == NRTGPU_AGG_TERMS) {
+      t->n_buckets[i] = n_buckets[i];
+      if ((rc = b->agg_counts[i].alloc((size_t)b->nq * (size_t)std::max(n_buckets[i], 1)))) return rc;
+      NRT_CUDA_TRY(cudaMemsetAsync(b->agg_counts[i].p, 0, b->agg_counts[i].bytes(), st));
+      t->counts[i] = b->agg_counts[i].p;
+    } else {
+      if ((rc = b->agg_dvals[i].alloc((size_t)b->nq))) return rc;
+      NRT_CUDA_TRY(cudaMemsetAsync(b->agg_dvals[i].p, a.kind == NRTGPU_AGG_MIN ? 0xff : 0x00, b->agg_dvals[i].bytes(), st));
+      t->dvals[i] = b->agg_dvals[i].p;
+    }
+  }
+  for (size_t j = 0; j < b->cb.nested.size(); ++j) {   // nested min / max / sum: one word per (query, parent bucket), as above
+    const nrtgpu_nested_aggregation& n = b->cb.nested[j];
+    if (n.kind == NRTGPU_AGG_TOP_HITS) continue;
+    const int32_t nb = n_buckets[n.parent];
+    if ((rc = b->nest_words[j].alloc((size_t)b->nq * (size_t)std::max(nb, 1)))) return rc;
+    NRT_CUDA_TRY(cudaMemsetAsync(b->nest_words[j].p, n.kind == NRTGPU_AGG_MIN ? 0xff : 0x00, b->nest_words[j].bytes(), st));
+    t->nest_words[j] = b->nest_words[j].p;
+  }
+  return NRTGPU_OK;
+}
+
 int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   if (!b) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_batch_run: NULL batch");
   cudaStream_t st = (cudaStream_t)stream_;
@@ -953,25 +1010,19 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
     NRT_CUDA_TRY(cudaMemsetAsync(b->clock0.p, 0, sizeof(unsigned long long), st));
     NRT_CUDA_TRY(cudaMemsetAsync(b->timed_out.p, 0, b->timed_out.bytes(), st));
   }
-  // aggregation outputs start unset on every run, work items or not: batch_fetch_aggs reads those of THIS run.
-  // min starts at +inf / max at -inf in ordered-double space, sum at 0.0 (the "unset" values are applied at fetch)
-  for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
-    const nrtgpu_aggregation& a = b->cb.aggs[i];
-    if (a.kind == NRTGPU_AGG_TERMS) {
-      const int32_t nb = b->ix->col_n_distinct[(size_t)a.column];
-      if ((rc_dbg = b->agg_counts[i].alloc((size_t)b->nq * (size_t)std::max(nb, 1)))) return rc_dbg;
-      NRT_CUDA_TRY(cudaMemsetAsync(b->agg_counts[i].p, 0, b->agg_counts[i].bytes(), st));
-    } else {
-      if ((rc_dbg = b->agg_dvals[i].alloc((size_t)b->nq))) return rc_dbg;
-      NRT_CUDA_TRY(cudaMemsetAsync(b->agg_dvals[i].p, a.kind == NRTGPU_AGG_MIN ? 0xff : 0x00, b->agg_dvals[i].bytes(), st));
+  // aggregation outputs start unset on every run, work items or not: batch_fetch_aggs reads those of THIS run (a searcher
+  // resets its shared tables once per call, before the first leaf runs)
+  if (!b->agg_shared && !b->cb.aggs.empty()) {
+    AggTables& t = b->agg_tab;
+    t = AggTables{};
+    int32_t nb[kMaxAggs] = {};
+    for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
+      const int32_t c = b->cb.aggs[i].column;
+      if (b->cb.aggs[i].kind != NRTGPU_AGG_TERMS) continue;
+      nb[i] = b->ix->col_n_distinct[(size_t)c];
+      t.codes[i] = ix_col_code(b->ix, c); t.distinct[i] = ix_col_distinct(b->ix, c);
     }
-  }
-  for (size_t j = 0; j < b->cb.nested.size(); ++j) {   // nested min / max / sum: one word per (query, parent bucket), as above
-    const nrtgpu_nested_aggregation& n = b->cb.nested[j];
-    if (n.kind == NRTGPU_AGG_TOP_HITS) continue;
-    const int32_t nb = b->ix->col_n_distinct[(size_t)b->cb.aggs[(size_t)n.parent].column];
-    if ((rc_dbg = b->nest_words[j].alloc((size_t)b->nq * (size_t)std::max(nb, 1)))) return rc_dbg;
-    NRT_CUDA_TRY(cudaMemsetAsync(b->nest_words[j].p, n.kind == NRTGPU_AGG_MIN ? 0xff : 0x00, b->nest_words[j].bytes(), st));
+    if ((rc_dbg = batch_agg_tables(b, nb, st, &t))) return rc_dbg;
   }
   const bool debug = b->ix->ctx->debug_modes;
   cudaEvent_t* ev = b->ev[b->runs_recorded % nrtgpu_batch::kEvRing];
@@ -991,23 +1042,24 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
       if (n_probe > 0) {
         v3::ProbeLaunch P = probe_params(b);
         if (!b->cb.aggs.empty()) {
+          const AggTables& t = b->agg_tab;
           AggLaunch A; std::memset(&A, 0, sizeof(A));
           A.n_aggs = (int32_t)b->cb.aggs.size();
           for (int i = 0; i < A.n_aggs; ++i) {
             const nrtgpu_aggregation& a = b->cb.aggs[(size_t)i];
             A.a[i].kind = a.kind; A.a[i].column = a.column; A.a[i].value_type = a.value_type;
             if (a.kind == NRTGPU_AGG_TERMS) {
-              A.a[i].n_buckets = b->ix->col_n_distinct[(size_t)a.column];
-              A.a[i].counts = b->agg_counts[i].p; A.codes[i] = b->ix->col_code[(size_t)a.column]->p;
+              A.a[i].n_buckets = t.n_buckets[i];
+              A.a[i].counts = t.counts[i]; A.codes[i] = t.codes[i];
             } else {
-              A.a[i].dvals = b->agg_dvals[i].p;
+              A.a[i].dvals = t.dvals[i];
             }
             A.nested_begin[i + 1] = A.nested_begin[i];   // pass 1: the nested min / max / sum collectors
             for (size_t j = 0; j < b->cb.nested.size(); ++j) {
               const nrtgpu_nested_aggregation& n = b->cb.nested[j];
               if (n.parent != i || n.kind == NRTGPU_AGG_TOP_HITS) continue;
               AggNestedDev& d = A.nested[A.nested_begin[i + 1]++];
-              d.kind = n.kind; d.column = n.column; d.value_type = n.value_type; d.dvals = b->nest_words[j].p;
+              d.kind = n.kind; d.column = n.column; d.value_type = n.value_type; d.dvals = t.nest_words[j];
             }
           }
           if ((rc_dbg = b->agg_launch.upload_async(&A, 1, st))) return rc_dbg;
@@ -1128,12 +1180,15 @@ int nrtgpu_batch_fetch_ex(nrtgpu_batch* b, void* stream_, int32_t* out_docs, flo
   return batch_fetch_impl(b, stream_, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
 }
 
-// Nested top hits of terms aggregation `parent` (pass 2): the batch's probe launch runs again with a collector that only
-// appends make_key(score, doc) of the docs of returned buckets (slot map nest_slot) to per-(query, slot) segments sized by
-// the bucket counts h_cnt [nq*size]; its totalHits / pruned / terminated go to scratch, and theta / slice lists / queue
-// heads are the batch's, already merged. Queries are taken in groups whose keys fit kNestedHitBudget.
-static int batch_nested_top_hits(nrtgpu_batch* b, cudaStream_t st, int parent, const std::vector<int32_t>& h_cnt,
+// Nested top hits of terms aggregation `parent` (pass 2) over the batches bs[0 .. n_b) that counted into one set of tables
+// (a single image: one batch; a searcher: one per leaf). Each batch's probe launch runs again with a collector that only
+// appends make_key(score, global doc) of the docs of returned buckets (slot map nest_slot) to per-(query, slot) segments
+// sized by the bucket counts h_cnt [nq*size]; its totalHits / pruned / terminated go to scratch, and theta / slice lists /
+// queue heads are its own, already merged. Queries are taken in groups whose keys fit kNestedHitBudget; each group runs
+// every batch's launch into the same segments, then selects once. Scratch and results are bs[0]'s.
+static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t st, int parent, const std::vector<int32_t>& h_cnt,
                                  const nrtgpu_nested_result* nres) {
+  nrtgpu_batch* b = bs[0];
   const int nq = b->nq;
   const nrtgpu_aggregation& a = b->cb.aggs[(size_t)parent];
   const int size = a.size;
@@ -1170,35 +1225,40 @@ static int batch_nested_top_hits(nrtgpu_batch* b, cudaStream_t st, int parent, c
     if ((rc = b->nest_off.upload_async(off.data(), off.size(), st)) || (rc = b->nest_fill.alloc((size_t)n_th * gs)) ||
         (rc = b->nest_keys.alloc((size_t)std::max(at, 1ll)))) return rc;
     NRT_CUDA_TRY(cudaMemsetAsync(b->nest_fill.p, 0, b->nest_fill.bytes(), st));
-    if (at > 0 && b->plan.n_probe_simple + b->plan.n_probe_generic > 0) {
-      AggLaunch A; std::memset(&A, 0, sizeof(A));
+    std::vector<AggLaunch> launches((size_t)n_b);   // uploaded asynchronously: kept until the group's synchronize
+    for (int l = 0; l < n_b && at > 0; ++l) {
+      nrtgpu_batch* x = bs[l];
+      if (x->plan.n_probe_simple + x->plan.n_probe_generic == 0) continue;
+      AggLaunch& A = launches[(size_t)l];
+      std::memset(&A, 0, sizeof(A));
       A.n_aggs = 1;
       A.a[0].kind = NRTGPU_AGG_TERMS; A.a[0].column = a.column; A.a[0].value_type = a.value_type;
-      A.a[0].n_buckets = b->ix->col_n_distinct[(size_t)a.column];
-      A.codes[0] = b->ix->col_code[(size_t)a.column]->p;   // counts stay NULL: the pass-1 tables are not touched
+      A.a[0].n_buckets = x->agg_tab.n_buckets[parent];
+      A.codes[0] = x->agg_tab.codes[parent];   // counts stay NULL: the pass-1 tables are not touched
       A.nested_begin[1] = n_th;
       for (int k = 0; k < n_th; ++k) {
         AggNestedDev& d = A.nested[k];
         d.kind = NRTGPU_AGG_TOP_HITS; d.size = size; d.q_lo = q_lo; d.q_hi = q_hi; d.slot_of = b->nest_slot.p;
         d.hit_off = b->nest_off.p + (size_t)k * (gs + 1); d.hit_fill = b->nest_fill.p + (size_t)k * gs; d.hit_keys = b->nest_keys.p;
+        d.doc_base = x->ix->doc_base;
       }
-      if ((rc = b->nest_launch.upload_async(&A, 1, st))) return rc;
-      NRT_CUDA_TRY(cudaMemsetAsync(b->theta.p, 0, b->theta.bytes(), st));
-      NRT_CUDA_TRY(cudaMemsetAsync(b->slice_cnt.p, 0, b->slice_cnt.bytes(), st));
-      NRT_CUDA_TRY(cudaMemsetAsync(b->work_counter.p, 0, b->work_counter.bytes(), st));
+      if ((rc = x->nest_launch.upload_async(&A, 1, st))) return rc;
+      NRT_CUDA_TRY(cudaMemsetAsync(x->theta.p, 0, x->theta.bytes(), st));
+      NRT_CUDA_TRY(cudaMemsetAsync(x->slice_cnt.p, 0, x->slice_cnt.bytes(), st));
+      NRT_CUDA_TRY(cudaMemsetAsync(x->work_counter.p, 0, x->work_counter.bytes(), st));
       NRT_CUDA_TRY(cudaMemsetAsync(b->p2_total.p, 0, b->p2_total.bytes(), st));
       NRT_CUDA_TRY(cudaMemsetAsync(b->p2_flags.p, 0, b->p2_flags.bytes(), st));
-      v3::ProbeLaunch P = probe_params(b);
+      v3::ProbeLaunch P = probe_params(x);
       P.total_hits = b->p2_total.p; P.pruned = b->p2_flags.p; P.terminated = b->p2_flags.p + nq;
       P.deadline_ns = 0; P.terminate_after = 0;
-      P.aggs = b->nest_launch.p;
-      if ((rc = probe_launch(b, P, false, st))) return rc;
+      P.aggs = x->nest_launch.p;
+      if ((rc = probe_launch(x, P, false, st))) return rc;
     }
     for (int k = 0; k < n_th; ++k) {
       const nrtgpu_nested_aggregation& n = b->cb.nested[th[(size_t)k]];
       NestedHitsLaunch H;
       H.hit_keys = b->nest_keys.p; H.hit_off = b->nest_off.p + (size_t)k * (gs + 1); H.hit_fill = b->nest_fill.p + (size_t)k * gs;
-      H.q_lo = q_lo; H.size = size; H.top_hits = n.top_hits; H.start_hit = n.start_hit; H.doc_base = b->ix->doc_base;
+      H.q_lo = q_lo; H.size = size; H.top_hits = n.top_hits; H.start_hit = n.start_hit; H.doc_base = 0;   // keys hold global docs
       H.out_docs = b->nest_docs.p + out_base[(size_t)k]; H.out_scores = b->nest_scores.p + out_base[(size_t)k];
       H.out_counts = b->nest_hcounts.p + (size_t)k * nq * size;
       nested_top_hits_kernel<<<gs, 256, 0, st>>>(H);
@@ -1220,8 +1280,12 @@ static int batch_nested_top_hits(nrtgpu_batch* b, cudaStream_t st, int parent, c
   return NRTGPU_OK;
 }
 
-// aggregation results of the last run -> caller buffers (nres: the results of cb.nested, in request order; NULL: none)
-static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggregation_result* out, const nrtgpu_nested_result* nres) {
+// aggregation results of the last run of the batches bs[0 .. n_b), which counted into one set of tables (agg_tab) ->
+// caller buffers (nres: the results of cb.nested, in request order; NULL: none). The selection runs once on those tables.
+static int batch_fetch_aggs(nrtgpu_batch* const* bs, int n_b, cudaStream_t st, const nrtgpu_aggregation_result* out,
+                            const nrtgpu_nested_result* nres) {
+  nrtgpu_batch* b = bs[0];
+  const AggTables& t = b->agg_tab;
   const int nq = b->nq;
   for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
     const nrtgpu_aggregation& a = b->cb.aggs[i];
@@ -1240,8 +1304,8 @@ static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggre
           top_hits |= b->cb.nested[j].kind == NRTGPU_AGG_TOP_HITS;
         }
       AggTermsLaunch T;
-      T.counts = b->agg_counts[i].p; T.n_buckets = b->ix->col_n_distinct[(size_t)a.column]; T.nq = nq; T.size = a.size; T.order_desc = a.order_desc != 0;
-      T.distinct = b->ix->col_distinct[(size_t)a.column]->p;
+      T.counts = t.counts[i]; T.n_buckets = t.n_buckets[i]; T.nq = nq; T.size = a.size; T.order_desc = a.order_desc != 0;
+      T.distinct = t.distinct[i];
       T.out_keys = b->agg_keys.p; T.out_counts = b->agg_cnts.p; T.out_n = b->agg_n.p; T.out_total_buckets = b->agg_tot.p; T.out_other = b->agg_other.p;
       T.out_bucket = nullptr;
       if (n_nested > 0) {
@@ -1250,7 +1314,7 @@ static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggre
       }
       if (order_by >= 0) {
         NRT_CUDA_TRY(cudaFuncSetAttribute(agg_terms_by_value_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAggByValueSmem));
-        agg_terms_by_value_kernel<<<nq, 256, kAggByValueSmem, st>>>(T, b->nest_words[(size_t)order_by].p, b->cb.nested[(size_t)order_by].kind);
+        agg_terms_by_value_kernel<<<nq, 256, kAggByValueSmem, st>>>(T, t.nest_words[(size_t)order_by], b->cb.nested[(size_t)order_by].kind);
       } else {
         agg_terms_topk_kernel<<<nq, 256, 0, st>>>(T);
       }
@@ -1265,7 +1329,7 @@ static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggre
         if ((rc = b->nest_vals.alloc(std::max<size_t>(vals.size(), 1) * n))) return rc;
         O.n_vals = (int32_t)vals.size();
         for (size_t k = 0; k < vals.size(); ++k) {
-          O.kind[k] = b->cb.nested[vals[k]].kind; O.words[k] = b->nest_words[vals[k]].p; O.values[k] = b->nest_vals.p + k * n;
+          O.kind[k] = b->cb.nested[vals[k]].kind; O.words[k] = t.nest_words[vals[k]]; O.values[k] = b->nest_vals.p + k * n;
         }
         if (top_hits) {
           const size_t cells = (size_t)nq * (size_t)std::max(T.n_buckets, 1);
@@ -1287,10 +1351,10 @@ static int batch_fetch_aggs(nrtgpu_batch* b, cudaStream_t st, const nrtgpu_aggre
       if (r.total_buckets) NRT_CUDA_TRY(cudaMemcpyAsync(r.total_buckets, b->agg_tot.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       if (r.other_counts) NRT_CUDA_TRY(cudaMemcpyAsync(r.other_counts, b->agg_other.p, (size_t)nq * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
       NRT_CUDA_TRY(cudaStreamSynchronize(st));   // the scratch is reused by the next terms aggregation
-      if (top_hits && (rc = batch_nested_top_hits(b, st, (int)i, h_cnt, nres))) return rc;
+      if (top_hits && (rc = batch_nested_top_hits(bs, n_b, st, (int)i, h_cnt, nres))) return rc;
     } else if (r.values) {
       std::vector<unsigned long long> h((size_t)nq);
-      NRT_CUDA_TRY(cudaMemcpyAsync(h.data(), b->agg_dvals[i].p, (size_t)nq * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      NRT_CUDA_TRY(cudaMemcpyAsync(h.data(), t.dvals[i], (size_t)nq * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
       NRT_CUDA_TRY(cudaStreamSynchronize(st));
       for (int q = 0; q < nq; ++q) r.values[q] = agg_word_value(a.kind, h[(size_t)q]);
     }
@@ -1493,7 +1557,7 @@ static int search_bool_impl(nrtgpu_index* ix, const BatchRequest& r, const nrtgp
     if (e != cudaSuccess) { set_error(cudaGetErrorString(e)); return NRTGPU_ERR_CUDA; }
   }
   rc = batch_fetch_impl(b, stream, out.docs, out.scores, out.counts, out.total_hits, out.relation, out.hit_timeout, out.terminated_early);
-  if (!rc && !b->cb.aggs.empty() && out.aggs) rc = batch_fetch_aggs(b, (cudaStream_t)stream, out.aggs, out.nested);
+  if (!rc && !b->cb.aggs.empty() && out.aggs) rc = batch_fetch_aggs(&b, 1, (cudaStream_t)stream, out.aggs, out.nested);
   return rc;
 }
 
@@ -2220,13 +2284,70 @@ int nrtgpu_rescore_combine(nrtgpu_ctx* ctx, int32_t nq, int32_t n_hits, const in
 }  // extern "C"
 
 // ---- searcher over several leaf images of one shard (NRT: a new reader version adds images for the NEW leaves only)
+// The reader-wide value dictionary of one column (collect_kernel.cuh, dict_map_kernel): the sorted union of the leaves'
+// distinct values, and per leaf the codes that number its docs' values in it. A leaf whose dictionary is the union, or
+// which holds no value, counts through its own col_code; every other leaf through a renumbered copy (4 B per doc).
+struct ReaderDict {
+  DevBuf<uint64_t> values;   // [n] ascending, the sortable domain of col_distinct
+  int32_t n = 0;
+  std::vector<std::unique_ptr<DevBuf<uint32_t>>> own;   // per leaf: the renumbered codes (unallocated where col_code serves)
+  std::vector<const uint32_t*> codes;                   // per leaf: the codes its docs count through
+};
+
 struct nrtgpu_searcher {
   nrtgpu_ctx* ctx = nullptr;
   std::vector<nrtgpu_index*> leaves;
   std::mutex mu;
   DevBuf<int32_t> records, merged;   // [n_leaves][words], [words]
   std::vector<int32_t> host;
+  // per aggregated column, built by its first aggregation and kept for the searcher's life: leaf columns never change
+  // (set_live_docs and update_stats leave them alone, and a dictionary keeps the values of deleted docs)
+  std::map<int32_t, std::unique_ptr<ReaderDict>> dicts;
 };
+
+static int32_t ix_n_distinct(const nrtgpu_index* ix, int32_t c) {
+  return (size_t)c < ix->col_n_distinct.size() ? ix->col_n_distinct[(size_t)c] : 0;
+}
+
+// the reader-wide dictionary of `column` (built on `st` the first time it is asked for)
+static int searcher_dict(nrtgpu_searcher* s, int32_t column, cudaStream_t st, const ReaderDict** out) {
+  auto it = s->dicts.find(column);
+  if (it != s->dicts.end()) { *out = it->second.get(); return NRTGPU_OK; }
+  std::unique_ptr<ReaderDict> d(new ReaderDict);
+  size_t total = 0;
+  for (const nrtgpu_index* ix : s->leaves) total += (size_t)ix_n_distinct(ix, column);
+  int rc;
+  if ((rc = d->values.alloc(std::max<size_t>(total, 1)))) return rc;
+  size_t at = 0;
+  for (const nrtgpu_index* ix : s->leaves) {   // the leaves' dictionaries one after the other, then sorted and deduplicated
+    const size_t nd = (size_t)ix_n_distinct(ix, column);
+    if (nd) NRT_CUDA_TRY(cudaMemcpyAsync(d->values.p + at, ix_col_distinct(ix, column), nd * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
+    at += nd;
+  }
+  if (total) {
+    thrust::sort(thrust::cuda::par.on(st), d->values.p, d->values.p + total);
+    d->n = (int32_t)(thrust::unique(thrust::cuda::par.on(st), d->values.p, d->values.p + total) - d->values.p);
+  }
+  d->values.n = (size_t)d->n;
+  DevBuf<uint32_t> map;
+  for (const nrtgpu_index* ix : s->leaves) {
+    const int32_t nd = ix_n_distinct(ix, column);
+    d->own.emplace_back(new DevBuf<uint32_t>);
+    if (nd == d->n || nd == 0) { d->codes.push_back(ix_col_code(ix, column)); continue; }   // codes already reader-wide, or all 0
+    DevBuf<uint32_t>& own = *d->own.back();
+    if ((rc = map.alloc((size_t)nd)) || (rc = own.alloc((size_t)ix->n_docs))) return rc;
+    dict_map_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, st>>>(ix_col_distinct(ix, column), nd, d->values.p, d->n, map.p);
+    NRT_CUDA_TRY(cudaGetLastError());
+    dict_remap_kernel<<<(unsigned)((ix->n_docs + 255) / 256), 256, 0, st>>>(ix_col_code(ix, column), ix->n_docs, map.p, own.p);
+    NRT_CUDA_TRY(cudaGetLastError());
+    NRT_CUDA_TRY(cudaStreamSynchronize(st));   // the map is reused by the next leaf
+    d->codes.push_back(own.p);
+  }
+  NRT_CUDA_TRY(cudaStreamSynchronize(st));
+  *out = d.get();
+  s->dicts[column] = std::move(d);
+  return NRTGPU_OK;
+}
 
 // the flags word of a record: relation GTE, terminated early, hit timeout
 static void unpack_record_flags(const int32_t* flags, int32_t nq, uint8_t* out_relation, uint8_t* out_hit_timeout,
@@ -2238,6 +2359,10 @@ static void unpack_record_flags(const int32_t* flags, int32_t nq, uint8_t* out_r
   }
 }
 
+static int searcher_merge_scored(nrtgpu_searcher* s, int32_t nq, int32_t top_k, void* stream, int32_t* out_docs, float* out_scores,
+                                 int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
+                                 uint8_t* out_terminated_early);
+
 // Score-ranked search over the leaves: run(l, d_record) leaves leaf l's page in its packed score record
 // (nrtgpu_packed_words), the records are merged on the device (TopDocs.merge: nrtgpu_merge_topk_packed) and the merged
 // page is copied to the host outputs (any may be NULL). The first failing leaf's code is returned and no output is written.
@@ -2248,7 +2373,6 @@ static int searcher_scored(nrtgpu_searcher* s, const char* fn, int32_t nq, int32
   if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, std::string(fn) + ": NULL searcher");
   if (nq <= 0 || top_k <= 0) NRT_FAIL(NRTGPU_ERR_INVALID, std::string(fn) + ": nq and top_k must be > 0");
   NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> g(s->mu);
   const int64_t words = nrtgpu_packed_words(nq, top_k);
   const int n_leaves = (int)s->leaves.size();
@@ -2256,6 +2380,18 @@ static int searcher_scored(nrtgpu_searcher* s, const char* fn, int32_t nq, int32
   if ((rc = s->records.alloc((size_t)words * n_leaves)) || (rc = s->merged.alloc((size_t)words))) return rc;
   for (int l = 0; l < n_leaves; ++l)
     if ((rc = run(l, s->records.p + (size_t)l * words))) return rc;
+  return searcher_merge_scored(s, nq, top_k, stream, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout,
+                               out_terminated_early);
+}
+
+// the tail of searcher_scored: the leaves' records in s->records merged on the device, the merged page to the host outputs
+static int searcher_merge_scored(nrtgpu_searcher* s, int32_t nq, int32_t top_k, void* stream, int32_t* out_docs, float* out_scores,
+                                 int32_t* out_counts, int64_t* out_total_hits, uint8_t* out_relation, uint8_t* out_hit_timeout,
+                                 uint8_t* out_terminated_early) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t words = nrtgpu_packed_words(nq, top_k);
+  const int n_leaves = (int)s->leaves.size();
+  int rc;
   NRT_CUDA_TRY(cudaMemsetAsync(s->merged.p, 0, (size_t)words * sizeof(int32_t), st));   // slots past a query's count read 0
   if ((rc = nrtgpu_merge_topk_packed(s->ctx, n_leaves, nq, top_k, s->records.p, s->merged.p, stream))) return rc;
   s->host.resize((size_t)words);
@@ -2440,6 +2576,70 @@ int nrtgpu_searcher_search_knn_filtered(nrtgpu_searcher* s, const float* queries
                                         stream, d, sc, c);
     });
   }, out_docs, out_scores, out_counts, nullptr, nullptr, nullptr, nullptr);
+}
+
+// Aggregations over the leaves: every leaf's batch counts into one set of reader-wide tables through its codes renumbered
+// to the column's reader-wide dictionary (searcher_dict); the selection and the nested top hits then run once on them
+int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                            const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                            const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                                            const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                            const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs,
+                                            float* out_scores, int32_t* out_counts, int64_t* out_total_hits) {
+  if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_bool_aggs_nested: NULL searcher");
+  if (n_aggs <= 0 || !aggs || !results) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool_aggs: no aggregations");
+  if (n_nested < 0 || (n_nested > 0 && (!nested || !nested_results))) NRT_FAIL(NRTGPU_ERR_INVALID, "nested aggregations: NULL argument");
+  BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
+  r.aggs = aggs; r.n_aggs = n_aggs;
+  if (n_nested > 0) { r.nested = nested; r.n_nested = n_nested; }
+  NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> g(s->mu);
+  const int n_leaves = (int)s->leaves.size();
+  int rc;
+  {   // every refusal of the single-image call, on every leaf's columns, before any batch is built
+    CompiledBatch cb;
+    for (nrtgpu_index* ix : s->leaves)
+      if ((rc = compile_batch(ix->dict(), r, &cb))) return rc;
+  }
+  // the reader-wide dictionaries, and the table limits of the single-image call at their size
+  const ReaderDict* dict[kMaxAggs] = {};
+  int32_t n_buckets[kMaxAggs] = {};
+  for (int i = 0; i < n_aggs; ++i) {
+    if (aggs[i].kind != NRTGPU_AGG_TERMS) continue;
+    if ((rc = searcher_dict(s, aggs[i].column, st, &dict[i]))) return rc;
+    n_buckets[i] = dict[i]->n;
+    if ((int64_t)nq * n_buckets[i] * 4 > (2ll << 30))
+      NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "terms aggregation: batch x distinct values exceeds the 2 GB count table");
+  }
+  for (int j = 0; j < n_nested; ++j)
+    if (nested[j].kind != NRTGPU_AGG_TOP_HITS && (int64_t)nq * n_buckets[nested[j].parent] * 8 > (2ll << 30))
+      NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nested aggregation: batch x distinct values exceeds the 2 GB table");
+  // one pooled workspace per leaf, held until the nested top hits of every leaf are collected
+  std::vector<std::unique_ptr<WorkspaceLease>> ws;
+  std::vector<nrtgpu_batch*> bs;
+  for (nrtgpu_index* ix : s->leaves) { ws.emplace_back(new WorkspaceLease(ix)); bs.push_back(ws.back()->b); }
+  const int64_t words = nrtgpu_packed_words(nq, top_k);
+  if ((rc = s->records.alloc((size_t)words * n_leaves)) || (rc = s->merged.alloc((size_t)words))) return rc;
+  for (int l = 0; l < n_leaves; ++l) {
+    if ((rc = batch_build(bs[(size_t)l], s->leaves[(size_t)l], r, st)) || (rc = batch_set_limits(bs[(size_t)l], nullptr, st)) ||
+        (rc = nrtgpu_batch_bind_packed(bs[(size_t)l], s->records.p + (size_t)l * words))) return rc;
+  }
+  // the reader-wide tables live in leaf 0's workspace and are reset once; every leaf counts into them with its own codes
+  AggTables t = {};
+  if ((rc = batch_agg_tables(bs[0], n_buckets, st, &t))) return rc;
+  for (int l = 0; l < n_leaves; ++l) {
+    AggTables& x = bs[(size_t)l]->agg_tab;
+    x = t;
+    for (int i = 0; i < n_aggs; ++i)
+      if (dict[i]) { x.codes[i] = dict[i]->codes[(size_t)l]; x.distinct[i] = dict[i]->values.p; }
+    bs[(size_t)l]->agg_shared = true;
+  }
+  for (int l = 0; l < n_leaves; ++l)
+    if ((rc = nrtgpu_batch_run(bs[(size_t)l], stream))) return rc;
+  if ((rc = batch_fetch_aggs(bs.data(), n_leaves, st, results, n_nested > 0 ? nested_results : nullptr))) return rc;
+  // TopDocs.merge of the leaves' pages; totalHits is exact (every match is counted) and summed over the leaves
+  return searcher_merge_scored(s, nq, top_k, stream, out_docs, out_scores, out_counts, out_total_hits, nullptr, nullptr, nullptr);
 }
 
 #include "batcher.inc"

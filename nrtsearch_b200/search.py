@@ -596,6 +596,62 @@ class PreparedBatch:
             self.handle = None
 
 
+def _collector_records(nq: int, additional: Sequence[object]):
+    """The records of a batch's additional collectors (search_with_collectors of either searcher): the nrtgpu_aggregation and
+    _result arrays, the nrtgpu_nested_aggregation and _result arrays of their terms collectors' nested collectors (None
+    without any) and their count, and the result objects the call fills, one per collector."""
+    aggs = (CAgg * len(additional))()
+    res = (CAggResult * len(additional))()
+    outs, nested, nested_res = [], [], []
+    for i, a in enumerate(additional):
+        vt = _VALUE_TYPE[a.field_type]
+        if isinstance(a, TermsCollector):
+            aggs[i] = CAgg(1, a.column, vt, a.size, 1 if a.order_desc else 0, 0)
+            o = {"keys": np.zeros((nq, a.size), np.int64), "counts": np.zeros((nq, a.size), np.int32), "n": np.zeros(nq, np.int32),
+                 "total_buckets": np.zeros(nq, np.int32), "other_counts": np.zeros(nq, np.int64)}
+            res[i] = CAggResult(None, o["keys"].ctypes.data, o["counts"].ctypes.data, o["n"].ctypes.data,
+                                o["total_buckets"].ctypes.data, o["other_counts"].ctypes.data)
+            if a.nested or a.order_by is not None:
+                o["nested"] = _nested_specs(i, a, nq, nested, nested_res)
+        else:
+            kind = 2 if isinstance(a, MinCollector) else 3 if isinstance(a, MaxCollector) else 4
+            aggs[i] = CAgg(kind, a.column, vt, 0, 0, 0)
+            o = np.zeros(nq, np.float64)
+            res[i] = CAggResult(o.ctypes.data, None, None, None, None, None)
+        outs.append(o)
+    narr = (CNested * len(nested))(*nested) if nested else None
+    nres = (CNestedResult * len(nested))(*nested_res) if nested else None
+    return aggs, res, narr, nres, len(nested), outs
+
+
+def _nested_specs(parent: int, a: TermsCollector, nq: int, nested: list, nested_res: list) -> dict:
+    """the nrtgpu_nested_aggregation records and result buffers of terms collector `parent` (appended to nested /
+    nested_res); returns the result dict they fill"""
+    names = [name for name, _ in a.nested]
+    if len(set(names)) != len(names):
+        raise ValueError("nested collector names must be unique")
+    if a.order_by is not None and a.order_by not in names:
+        raise ValueError(f"order_by {a.order_by!r} is not a nested collector")
+    o = {}
+    for name, c in a.nested:
+        if isinstance(c, TopHitsCollector):
+            w = max(c.top_hits - c.start_hit, 0)
+            r = {"docs": np.zeros((nq, a.size, w), np.int32), "scores": np.zeros((nq, a.size, w), np.float32),
+                 "counts": np.zeros((nq, a.size), np.int32), "total_hits": np.zeros((nq, a.size), np.int64)}
+            nested.append(CNested(parent, 5, 0, 0, c.top_hits, c.start_hit, 1 if name == a.order_by else 0, 0))
+            nested_res.append(CNestedResult(None, r["docs"].ctypes.data, r["scores"].ctypes.data, r["counts"].ctypes.data,
+                                            r["total_hits"].ctypes.data))
+        elif isinstance(c, (MinCollector, MaxCollector, SumCollector)):
+            kind = 2 if isinstance(c, MinCollector) else 3 if isinstance(c, MaxCollector) else 4
+            r = np.zeros((nq, a.size), np.float64)
+            nested.append(CNested(parent, kind, c.column, _VALUE_TYPE[c.field_type], 0, 0, 1 if name == a.order_by else 0, 0))
+            nested_res.append(CNestedResult(r.ctypes.data, None, None, None, None))
+        else:
+            raise ValueError(f"nested collector {name!r}: {type(c).__name__} is not on the GPU path")
+        o[name] = r
+    return o
+
+
 class GpuIndexSearcher:
     """Batched stand-in for MyIndexSearcher.search(Query, CollectorManager)."""
 
@@ -739,63 +795,15 @@ class GpuIndexSearcher:
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
-        aggs = (CAgg * len(additional))()
-        res = (CAggResult * len(additional))()
-        outs, nested, nested_res = [], [], []
-        for i, a in enumerate(additional):
-            vt = _VALUE_TYPE[a.field_type]
-            if isinstance(a, TermsCollector):
-                aggs[i] = CAgg(1, a.column, vt, a.size, 1 if a.order_desc else 0, 0)
-                o = {"keys": np.zeros((nq, a.size), np.int64), "counts": np.zeros((nq, a.size), np.int32), "n": np.zeros(nq, np.int32),
-                     "total_buckets": np.zeros(nq, np.int32), "other_counts": np.zeros(nq, np.int64)}
-                res[i] = CAggResult(None, o["keys"].ctypes.data, o["counts"].ctypes.data, o["n"].ctypes.data,
-                                    o["total_buckets"].ctypes.data, o["other_counts"].ctypes.data)
-                if a.nested or a.order_by is not None:
-                    o["nested"] = self._nested_specs(i, a, nq, nested, nested_res)
-            else:
-                kind = 2 if isinstance(a, MinCollector) else 3 if isinstance(a, MaxCollector) else 4
-                aggs[i] = CAgg(kind, a.column, vt, 0, 0, 0)
-                o = np.zeros(nq, np.float64)
-                res[i] = CAggResult(o.ctypes.data, None, None, None, None, None)
-            outs.append(o)
+        aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         hits = (out.docs.ctypes.data, out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data)
-        if nested:
-            narr = (CNested * len(nested))(*nested)
-            nres = (CNestedResult * len(nested))(*nested_res)
+        if n_nested:
             check(self._lib.nrtgpu_search_bool_aggs_nested(self.index.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
-                                                           narr, len(nested), nres, C.c_void_p(stream), *hits))
+                                                           narr, n_nested, nres, C.c_void_p(stream), *hits))
         else:
             check(self._lib.nrtgpu_search_bool_aggs(self.index.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
                                                     C.c_void_p(stream), *hits))
         return out, outs
-
-    @staticmethod
-    def _nested_specs(parent: int, a: TermsCollector, nq: int, nested: list, nested_res: list) -> dict:
-        """the nrtgpu_nested_aggregation records and result buffers of terms collector `parent` (appended to nested /
-        nested_res); returns the result dict they fill"""
-        names = [name for name, _ in a.nested]
-        if len(set(names)) != len(names):
-            raise ValueError("nested collector names must be unique")
-        if a.order_by is not None and a.order_by not in names:
-            raise ValueError(f"order_by {a.order_by!r} is not a nested collector")
-        o = {}
-        for name, c in a.nested:
-            if isinstance(c, TopHitsCollector):
-                w = max(c.top_hits - c.start_hit, 0)
-                r = {"docs": np.zeros((nq, a.size, w), np.int32), "scores": np.zeros((nq, a.size, w), np.float32),
-                     "counts": np.zeros((nq, a.size), np.int32), "total_hits": np.zeros((nq, a.size), np.int64)}
-                nested.append(CNested(parent, 5, 0, 0, c.top_hits, c.start_hit, 1 if name == a.order_by else 0, 0))
-                nested_res.append(CNestedResult(None, r["docs"].ctypes.data, r["scores"].ctypes.data, r["counts"].ctypes.data,
-                                                r["total_hits"].ctypes.data))
-            elif isinstance(c, (MinCollector, MaxCollector, SumCollector)):
-                kind = 2 if isinstance(c, MinCollector) else 3 if isinstance(c, MaxCollector) else 4
-                r = np.zeros((nq, a.size), np.float64)
-                nested.append(CNested(parent, kind, c.column, _VALUE_TYPE[c.field_type], 0, 0, 1 if name == a.order_by else 0, 0))
-                nested_res.append(CNestedResult(r.ctypes.data, None, None, None, None))
-            else:
-                raise ValueError(f"nested collector {name!r}: {type(c).__name__} is not on the GPU path")
-            o[name] = r
-        return o
 
     def score_docs(self, queries: Sequence[object], docs: np.ndarray, counts: Optional[np.ndarray] = None, stream: int = 0):
         """Second pass of QueryRescorer: query q on its own hit list -> (matches uint8 [nq, n], scores float32 [nq, n])."""
@@ -991,6 +999,23 @@ class GpuLeafSearcher:
                                                    None if f is None else f.ctypes.data, C.c_void_p(stream),
                                                    docs.ctypes.data, scores.ctypes.data, counts.ctypes.data))
         return docs, scores, counts
+
+    def search_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
+                               stream: int = 0):
+        """GpuIndexSearcher.search_with_collectors over the leaves (nrtgpu_searcher_search_bool_aggs_nested): every leaf counts
+        into reader-wide tables, buckets by value (the searcher's reader-wide dictionary of each terms column, built by the
+        column's first aggregation), and the buckets, nested values and nested top hits are selected once from them; the
+        leaves' pages are merged on the device (TopDocs.merge). Returns what the single-image method returns."""
+        carr, ncl, qarr, nq = compile_queries(queries)
+        k = collector.num_hits_to_collect
+        out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
+                          np.zeros(nq, np.uint8))
+        aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
+        check(self._lib.nrtgpu_searcher_search_bool_aggs_nested(self.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
+                                                                narr, n_nested, nres, C.c_void_p(stream), out.docs.ctypes.data,
+                                                                out.scores.ctypes.data, out.counts.ctypes.data,
+                                                                out.total_hits.ctypes.data))
+        return out, outs
 
     def close(self):
         if self.handle:
