@@ -517,7 +517,10 @@ int nrtgpu_batch_bind_output(nrtgpu_batch* b, int32_t* d_docs, float* d_scores, 
  *   early) | pad to 8 bytes | totalHits [nq] int64.      nrtgpu_packed_words = record size in words.
  * nrtgpu_batch_bind_packed redirects the results of subsequent runs into a caller-owned DEVICE record (NULL restores
  * the internal buffers); nrtgpu_merge_topk_packed is TopDocs.merge over n_lists gathered records (totalHits summed,
- * relation GTE if any shard's is: LazyQueueTopScoreDocCollectorManager.java:137-144) into one record, on the device. */
+ * relation GTE if any shard's is: LazyQueueTopScoreDocCollectorManager.java:137-144) into one record, on the device.
+ * Every score-ranked page of top_k slots (this record, the bound or internal outputs of a batch, nrtgpu_merge_topk_device,
+ * nrtgpu_searcher_search_bool, nrtgpu_blend_rrf / _scores) holds its count hits first; the slots past the count hold
+ * doc 0 and score 0.0, whatever an earlier request left in the buffer (a sorted page keeps NaN scores there). */
 int64_t nrtgpu_packed_words(int32_t nq, int32_t top_k);
 int nrtgpu_batch_bind_packed(nrtgpu_batch* b, int32_t* d_record);
 int nrtgpu_merge_topk_packed(nrtgpu_ctx* ctx, int32_t n_lists, int32_t nq, int32_t top_k, const int32_t* d_records,

@@ -388,10 +388,10 @@ __global__ void __launch_bounds__(kMergeThreads) merge_slices_kernel(MergeLaunch
   if (dirty) sort_and_cut();
   if (M.n_lists <= 0) have = 0;
   __syncthreads();
-  for (int i = tid; i < have; i += kMergeThreads) {
-    uint64_t k = keys[i];
-    M.out_docs[(size_t)q * M.top_k + i] = key_doc(k) + M.doc_base;
-    M.out_scores[(size_t)q * M.top_k + i] = key_score(k);
+  for (int i = tid; i < M.top_k; i += kMergeThreads) {   // slots past the count: doc 0, score 0.0 (include/nrtgpu.h)
+    const uint64_t k = keys[i < have ? i : 0];
+    M.out_docs[(size_t)q * M.top_k + i] = i < have ? key_doc(k) + M.doc_base : 0;
+    M.out_scores[(size_t)q * M.top_k + i] = i < have ? key_score(k) : 0.0f;
   }
   if (tid == 0) {
     M.out_counts[q] = have;
@@ -442,10 +442,10 @@ __global__ void __launch_bounds__(kMergeThreads) merge_pairs_kernel(MergePairsLa
     have = fill < M.top_k ? fill : M.top_k;
   }
   __syncthreads();
-  for (int i = tid; i < have; i += kMergeThreads) {
-    uint64_t k = keys[i];
-    M.out_docs[(size_t)q * M.top_k + i] = key_doc(k);
-    M.out_scores[(size_t)q * M.top_k + i] = key_score(k);
+  for (int i = tid; i < M.top_k; i += kMergeThreads) {   // slots past the count: doc 0, score 0.0 (include/nrtgpu.h)
+    const uint64_t k = keys[i < have ? i : 0];
+    M.out_docs[(size_t)q * M.top_k + i] = i < have ? key_doc(k) : 0;
+    M.out_scores[(size_t)q * M.top_k + i] = i < have ? key_score(k) : 0.0f;
   }
   if (tid == 0) {
     M.out_counts[q] = have;

@@ -83,9 +83,10 @@ __global__ void __launch_bounds__(kHybThreads) rrf_blend_kernel(RrfLaunch P) {
   block_bitonic_sort_desc(keys, m);
   const int total = n_heads;
   const int keep = total < P.top_out ? total : P.top_out;
-  for (int i = tid; i < keep; i += kHybThreads) {
-    P.out_docs[(size_t)q * P.top_out + i] = key_doc(keys[i]);
-    P.out_scores[(size_t)q * P.top_out + i] = key_score(keys[i]);
+  for (int i = tid; i < P.top_out; i += kHybThreads) {   // slots past the count: doc 0, score 0.0 (include/nrtgpu.h)
+    const uint64_t k = keys[i < keep ? i : 0];
+    P.out_docs[(size_t)q * P.top_out + i] = i < keep ? key_doc(k) : 0;
+    P.out_scores[(size_t)q * P.top_out + i] = i < keep ? key_score(k) : 0.0f;
   }
   if (tid == 0) { P.out_counts[q] = keep; P.out_total[q] = total; }
 }

@@ -2392,7 +2392,6 @@ static int searcher_merge_scored(nrtgpu_searcher* s, int32_t nq, int32_t top_k, 
   const int64_t words = nrtgpu_packed_words(nq, top_k);
   const int n_leaves = (int)s->leaves.size();
   int rc;
-  NRT_CUDA_TRY(cudaMemsetAsync(s->merged.p, 0, (size_t)words * sizeof(int32_t), st));   // slots past a query's count read 0
   if ((rc = nrtgpu_merge_topk_packed(s->ctx, n_leaves, nq, top_k, s->records.p, s->merged.p, stream))) return rc;
   s->host.resize((size_t)words);
   NRT_CUDA_TRY(cudaMemcpyAsync(s->host.data(), s->merged.p, (size_t)words * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
