@@ -386,7 +386,8 @@ typedef struct {
   int32_t kind, column, value_type;
   int32_t size;        /* terms: buckets returned (<= 2048) */
   int32_t order_desc;  /* terms: 1 = largest counts first (BucketOrder DESC by count, the default) */
-  int32_t reserved;
+  int32_t filter_agg;  /* terms / filter: 1 + the index of the FILTER aggregation this one is nested under; 0: top level
+                          (nrtgpu_search_bool_aggs_filtered) */
 } nrtgpu_aggregation;
 typedef struct {       /* caller-allocated outputs of one aggregation (unused pointers may be NULL) */
   double* values;          /* [nq]        min / max / sum */
@@ -434,7 +435,7 @@ int nrtgpu_search_bool_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int3
  *     (nq * size * top_hits), a single query whose returned buckets hold more than 2^26 keys. */
 enum { NRTGPU_AGG_TOP_HITS = 5 };
 typedef struct {
-  int32_t parent;         /* index into aggs[] of the terms aggregation */
+  int32_t parent;         /* index into aggs[] of the terms (or filter) aggregation */
   int32_t kind;           /* NRTGPU_AGG_MIN / _MAX / _SUM / _TOP_HITS */
   int32_t column, value_type;   /* MIN / MAX / SUM */
   int32_t top_hits, start_hit;  /* TOP_HITS */
@@ -454,6 +455,55 @@ int nrtgpu_search_bool_aggs_nested(nrtgpu_index* ix, const nrtgpu_clause* clause
                                    const nrtgpu_nested_aggregation* nested, int32_t n_nested,
                                    const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs,
                                    float* out_scores, int32_t* out_counts, int64_t* out_total_hits);
+
+/* Filter collectors (search.proto Collector.filter, FilterCollectorManager.java): of the docs a query collects, those that
+ * pass the filter are counted (docCount) and handed to the collectors nested under it.
+ *   NRTGPU_AGG_FILTER  a top-level aggregation; its result is bucket_counts[nq], the query's docCount (the other result
+ *                      pointers are unused). It needs a collector under it: a TERMS or FILTER aggregation whose filter_agg
+ *                      names it, or a nested MIN / MAX / SUM / TOP_HITS whose parent it is; else NRTGPU_ERR_INVALID
+ *                      'Filter collector "aggs[i]" must have nested collectors'.
+ *   filter_agg         (nrtgpu_aggregation) 1 + the index of an EARLIER FILTER aggregation: a TERMS aggregation then counts,
+ *                      and a FILTER aggregation passes, only the docs that pass that filter (a filter under a filter: both
+ *                      must pass). Only TERMS and FILTER aggregations may set it; a MIN / MAX / SUM under a filter is a
+ *                      nested collector of it. A terms aggregation under a filter keeps every terms rule above.
+ *   nested collectors  parent may name a FILTER aggregation: MIN / MAX / SUM / TOP_HITS over the docs that pass, at most 4,
+ *                      orders_parent refused. Results use the terms layout with size 1: values [nq], hit_docs / hit_scores
+ *                      [nq*(top_hits-start_hit)], hit_counts [nq], hit_total [nq] = docCount.
+ * The filter of a FILTER aggregation is agg_filters[i] (an array parallel to aggs, read for FILTER aggregations only):
+ *   NRTGPU_AGG_FILTER_QUERY      filter_queries[query], a flat BooleanQuery in the clause format of nrtgpu_search_bool over
+ *                      filter_clauses (QueryFilter: only matching counts, boosts and scores are ignored). The kNN filters'
+ *                      rules apply: has_after is NRTGPU_ERR_INVALID, more than 16 clauses or 8 term clauses
+ *                      NRTGPU_ERR_UNSUPPORTED, an empty clause range or MUST_NOT clauses only match nothing.
+ *   NRTGPU_AGG_FILTER_VALUE_SET  values[n_values] in the sortable-long domain of `column` (SetQueryFilter over a
+ *                      TermInSetQuery): a doc passes when one of its values (a single-valued or multi-valued column) is in
+ *                      the set, by bit equality in that domain, so -0.0 != 0.0 and NaN == NaN as in Java's boxed equals.
+ *                      Any order, duplicates allowed; n_values == 0 passes nothing. A set of another term type than the
+ *                      field's never matches in the reference: the caller passes an empty set.
+ * Every query of the batch takes the same filters. Deleted docs never pass.
+ * nrtgpu_search_bool_aggs_filtered: nrtgpu_search_bool_aggs_nested (every refusal, the same hits and results) plus filter
+ * collectors; nrtgpu_search_bool_aggs and _aggs_nested are this call without filter records.
+ *   NRTGPU_ERR_INVALID: a FILTER aggregation without agg_filters, a bad record kind, a query or column out of range,
+ *     n_values < 0 or values NULL with n_values > 0, a filter_agg that is not an earlier FILTER aggregation or set on a MIN /
+ *     MAX / SUM, orders_parent under a FILTER parent, a FILTER aggregation nothing is nested under.
+ *   The 8-aggregation cap counts the FILTER aggregations. Query trees and wide batches stay NRTGPU_ERR_UNSUPPORTED. A refused
+ *   call writes no output. */
+enum { NRTGPU_AGG_FILTER = 6 };
+enum { NRTGPU_AGG_FILTER_QUERY = 1, NRTGPU_AGG_FILTER_VALUE_SET = 2 };
+typedef struct {
+  int32_t kind;           /* NRTGPU_AGG_FILTER_QUERY / _VALUE_SET */
+  int32_t query;          /* QUERY: index into filter_queries */
+  int32_t column;         /* VALUE_SET */
+  int32_t n_values;       /* VALUE_SET */
+  const int64_t* values;  /* VALUE_SET: [n_values] */
+} nrtgpu_agg_filter;
+int nrtgpu_search_bool_aggs_filtered(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                     const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                     const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                                     const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                     const nrtgpu_nested_result* nested_results, const nrtgpu_agg_filter* agg_filters,
+                                     const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses,
+                                     const nrtgpu_query* filter_queries, int32_t n_filter_queries, void* stream,
+                                     int32_t* out_docs, float* out_scores, int32_t* out_counts, int64_t* out_total_hits);
 
 /* QueryRescorer second pass (QueryRescore.java:39-57 -> Lucene QueryRescorer.rescore): query q of the batch evaluated on
  * ITS OWN hit list docs[q][0..counts[q]) (global doc ids): out_matches / out_scores [nq*n_hits]. */
@@ -688,6 +738,20 @@ int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_cla
                                             const nrtgpu_nested_aggregation* nested, int32_t n_nested,
                                             const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs,
                                             float* out_scores, int32_t* out_counts, int64_t* out_total_hits);
+/* nrtgpu_searcher_search_bool_aggs_filtered: nrtgpu_search_bool_aggs_filtered over the leaves, with the rules above. Each leaf
+ * evaluates the filters on its own image; every leaf counts into the one set of tables, so docCount and the values nested
+ * under a filter are reader-wide, a terms aggregation under a filter uses the reader-wide dictionary, and top hits under a
+ * filter are chosen over every leaf, ties by global doc. nrtgpu_searcher_search_bool_aggs_nested is this call without
+ * filter records. */
+int nrtgpu_searcher_search_bool_aggs_filtered(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                              const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                              const nrtgpu_aggregation* aggs, int32_t n_aggs,
+                                              const nrtgpu_aggregation_result* results, const nrtgpu_nested_aggregation* nested,
+                                              int32_t n_nested, const nrtgpu_nested_result* nested_results,
+                                              const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses,
+                                              int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
+                                              int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores,
+                                              int32_t* out_counts, int64_t* out_total_hits);
 
 /* Request micro-batcher: the reference's search API is ONE query per RPC (clientlib/src/main/proto/yelp/nrtsearch/
  * luceneserver.proto:164), each on its own SERVER-pool thread (GrpcServerExecutorSupplier.java:68-75). Handler threads call

@@ -180,6 +180,25 @@ public final class NrtGpu {
       int nAggs, ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, ByteBuffer outDocs,
       ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits);
 
+  /**
+   * Additional collectors with filter collectors (nrtgpu_search_bool_aggs_filtered): the buffers of searchBoolAggsNested, plus
+   * aggFilters = nAggs nrtgpu_agg_filter (their values fields are ignored), filterValues = one int64 buffer (or null) per
+   * aggregation holding a VALUE_SET filter's set, and the filter queries (filterClauses / filterQueries, the clause format
+   * of searchBool). A FILTER aggregation's docCount comes back in its bucket_counts buffer.
+   */
+  public static native int searchBoolAggsFiltered(
+      long index, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK, int flags, ByteBuffer aggs,
+      int nAggs, ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, ByteBuffer aggFilters,
+      ByteBuffer[] filterValues, ByteBuffer filterClauses, int nFilterClauses, ByteBuffer filterQueries, int nFilterQueries,
+      ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits);
+
+  /** searchBoolAggsFiltered over the leaves of a searcher: docCount and everything under a filter are reader-wide. */
+  public static native int searcherSearchBoolAggsFiltered(
+      long searcher, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK, int flags, ByteBuffer aggs,
+      int nAggs, ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, ByteBuffer aggFilters,
+      ByteBuffer[] filterValues, ByteBuffer filterClauses, int nFilterClauses, ByteBuffer filterQueries, int nFilterQueries,
+      ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits);
+
   public static native long batcherCreate(long index, int maxBatch, int maxWaitUs);
 
   /** Blocks until the batch this request rode in is back; diag = nrtgpu_diagnostics (24 bytes) or null. */

@@ -8,6 +8,7 @@
 #include <jni.h>
 #include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 #include "nrtgpu.h"
 
 #define ADDR(env, buf) ((buf) ? (*(env))->GetDirectBufferAddress((env), (buf)) : NULL)
@@ -236,6 +237,44 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchBoolAggsN
   free(nr);
   return fail(env, rc);
 }
+/* filter collectors: aggFilters = a direct ByteBuffer of nrtgpu_agg_filter[nAggs] (the values fields are ignored), filterValues
+ * one direct buffer of int64 (or null) per aggregation, the value set of a VALUE_SET filter. agg_filter_records copies the
+ * records with their values pointers set (freed by the caller, also when it fails); a null aggFilters gives NULL. */
+static int agg_filter_records(JNIEnv* env, jobject aggFilters, jobjectArray filterValues, jint nAggs, nrtgpu_agg_filter** out) {
+  *out = NULL;
+  const void* src = ADDR(env, aggFilters);
+  if (!src || nAggs <= 0) return NRTGPU_OK;
+  nrtgpu_agg_filter* f = *out = (nrtgpu_agg_filter*)calloc((size_t)nAggs, sizeof(*f));
+  if (!f) return NRTGPU_ERR_OOM;
+  memcpy(f, src, (size_t)nAggs * sizeof(*f));
+  for (jint i = 0; i < nAggs; ++i)
+    f[i].values = filterValues ? (const int64_t*)ADDR(env, (*env)->GetObjectArrayElement(env, filterValues, i)) : NULL;
+  return NRTGPU_OK;
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchBoolAggsFiltered(
+    JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
+    jobject aggs, jint nAggs, jobjectArray aggOut, jobject nested, jint nNested, jobjectArray nestedOut, jobject aggFilters,
+    jobjectArray filterValues, jobject filterClauses, jint nFilterClauses, jobject filterQueries, jint nFilterQueries,
+    jobject outDocs, jobject outScores, jobject outCounts, jobject outTotalHits) {
+  nrtgpu_aggregation_result* ar = NULL;
+  nrtgpu_nested_result* nr = NULL;
+  nrtgpu_agg_filter* af = NULL;
+  int rc = agg_results(env, aggOut, nAggs, nestedOut, nNested, &ar, &nr);
+  if (!rc) rc = agg_filter_records(env, aggFilters, filterValues, nAggs, &af);
+  if (!rc)
+    rc = nrtgpu_search_bool_aggs_filtered((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                          (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                          (const nrtgpu_aggregation*)ADDR(env, aggs), nAggs, ar,
+                                          (const nrtgpu_nested_aggregation*)ADDR(env, nested), nNested, nr, af,
+                                          (const nrtgpu_clause*)ADDR(env, filterClauses), nFilterClauses,
+                                          (const nrtgpu_query*)ADDR(env, filterQueries), nFilterQueries, NULL,
+                                          (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
+                                          (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
+  free(ar);
+  free(nr);
+  free(af);
+  return fail(env, rc);
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_fetchColumns(
     JNIEnv* env, jclass c, jlong ix, jobject colIds, jint nCols, jobject docs, jint n, jobject outValues, jobject outHas) {
   return fail(env, nrtgpu_fetch_columns((nrtgpu_index*)(intptr_t)ix, (const int32_t*)ADDR(env, colIds), nCols,
@@ -331,6 +370,31 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchB
                                                  (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
   free(ar);
   free(nr);
+  return fail(env, rc);
+}
+
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchBoolAggsFiltered(
+    JNIEnv* env, jclass c, jlong s, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
+    jobject aggs, jint nAggs, jobjectArray aggOut, jobject nested, jint nNested, jobjectArray nestedOut, jobject aggFilters,
+    jobjectArray filterValues, jobject filterClauses, jint nFilterClauses, jobject filterQueries, jint nFilterQueries,
+    jobject outDocs, jobject outScores, jobject outCounts, jobject outTotalHits) {
+  nrtgpu_aggregation_result* ar = NULL;
+  nrtgpu_nested_result* nr = NULL;
+  nrtgpu_agg_filter* af = NULL;
+  int rc = agg_results(env, aggOut, nAggs, nestedOut, nNested, &ar, &nr);
+  if (!rc) rc = agg_filter_records(env, aggFilters, filterValues, nAggs, &af);
+  if (!rc)
+    rc = nrtgpu_searcher_search_bool_aggs_filtered((nrtgpu_searcher*)(intptr_t)s, (const nrtgpu_clause*)ADDR(env, clauses),
+                                                   nClauses, (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                                   (const nrtgpu_aggregation*)ADDR(env, aggs), nAggs, ar,
+                                                   (const nrtgpu_nested_aggregation*)ADDR(env, nested), nNested, nr, af,
+                                                   (const nrtgpu_clause*)ADDR(env, filterClauses), nFilterClauses,
+                                                   (const nrtgpu_query*)ADDR(env, filterQueries), nFilterQueries, NULL,
+                                                   (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
+                                                   (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
+  free(ar);
+  free(nr);
+  free(af);
   return fail(env, rc);
 }
 

@@ -82,7 +82,13 @@ class Diagnostics(C.Structure):
 
 class Aggregation(C.Structure):
     _fields_ = [("kind", C.c_int32), ("column", C.c_int32), ("value_type", C.c_int32), ("size", C.c_int32),
-                ("order_desc", C.c_int32), ("reserved", C.c_int32)]
+                ("order_desc", C.c_int32), ("filter_agg", C.c_int32)]
+
+
+class AggFilter(C.Structure):
+    """nrtgpu_agg_filter: the filter of a FILTER aggregation, a filter query (kind 1) or a value set (kind 2)."""
+    _fields_ = [("kind", C.c_int32), ("query", C.c_int32), ("column", C.c_int32), ("n_values", C.c_int32),
+                ("values", C.c_void_p)]
 
 
 class AggregationResult(C.Structure):
@@ -137,6 +143,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_sorted_packed_words", "nrtgpu_search_sorted_fields_packed", "nrtgpu_merge_sorted_packed",
     "nrtgpu_searcher_search_sorted_fields", "nrtgpu_searcher_search_tree_phrases", "nrtgpu_searcher_search_knn",
     "nrtgpu_searcher_search_knn_filtered", "nrtgpu_searcher_search_bool_aggs_nested",
+    "nrtgpu_search_bool_aggs_filtered", "nrtgpu_searcher_search_bool_aggs_filtered",
 ]
 
 _gpu = None
@@ -246,6 +253,9 @@ def gpu_lib() -> C.CDLL:
                                                             C.c_int32, C.POINTER(Query), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                             C.c_void_p, C.c_void_p]
         lib.nrtgpu_searcher_search_bool_aggs_nested.argtypes = lib.nrtgpu_search_bool_aggs_nested.argtypes
+        lib.nrtgpu_search_bool_aggs_filtered.argtypes = lib.nrtgpu_search_bool_aggs_nested.argtypes[:13] + \
+            [C.POINTER(AggFilter), C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_void_p] + [C.c_void_p] * 4
+        lib.nrtgpu_searcher_search_bool_aggs_filtered.argtypes = lib.nrtgpu_search_bool_aggs_filtered.argtypes
         lib.nrtgpu_batcher_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
         lib.nrtgpu_batcher_submit.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Diagnostics)]

@@ -104,6 +104,62 @@ __global__ void __launch_bounds__(256) knn_filter_rows_kernel(KnnFilterRowsLaunc
   if (lane == 0 && n) atomicAdd(L.row_cnt + row, n);
 }
 
+// The row of a filter collector's value set (FilterCollectorManager.SetQueryFilter over a TermInSetQuery): bit d is set iff
+// live doc d has a value of `column` in set[0 .. n_set), sorted and distinct in the column's sortable-long domain, so a
+// match is bit equality (-0.0 != 0.0, NaN == NaN, as Java's boxed equals). One lane per doc and a warp ballot per word, as
+// the range branch above; a multi-valued doc passes when any of its values is in the set.
+struct AggValueSetLaunch {
+  DevIndexView ix;
+  int32_t column, n_set, words;
+  const int64_t* set;
+  uint32_t* row;   // [words]
+};
+
+__device__ __forceinline__ bool in_sorted_set(const int64_t* __restrict__ set, int n, int64_t v) {
+  int lo = 0, hi = n;
+  while (lo < hi) { const int m = (lo + hi) >> 1; if (__ldg(set + m) < v) lo = m + 1; else hi = m; }
+  return lo < n && __ldg(set + lo) == v;
+}
+
+__global__ void __launch_bounds__(256) agg_value_set_kernel(AggValueSetLaunch L) {
+  const int64_t doc = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  bool m = false;
+  if (doc < L.ix.n_docs && L.n_set > 0) {
+    const int32_t d = (int32_t)doc;
+    const int64_t* off = L.ix.colmv_off ? L.ix.colmv_off[L.column] : nullptr;
+    if (off) {
+      const int64_t* v = L.ix.colmv_val[L.column];
+      for (int64_t j = off[d]; j < off[d + 1] && !m; ++j) m = in_sorted_set(L.set, L.n_set, v[j]);
+    } else {
+      const uint8_t* has = L.ix.col_has[L.column];
+      if (!has || has[d])
+        m = in_sorted_set(L.set, L.n_set, L.ix.col32[L.column] ? (int64_t)__ldg(L.ix.col32[L.column] + d) : __ldg(L.ix.col64[L.column] + d));
+    }
+  }
+  uint32_t word = __ballot_sync(0xffffffffu, m);
+  const int64_t w = doc >> 5;
+  if ((threadIdx.x & 31) == 0 && w < L.words) {
+    if (L.ix.live_bits) word &= L.ix.live_bits[w];
+    L.row[w] = word;
+  }
+}
+
+// a filter nested under a filter: its row ANDs its parent's
+__global__ void row_and_kernel(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src, int words) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < words) dst[i] &= src[i];
+}
+
+// The codes a filter collector's aggregation counts through in agg_collect, which sees it as a terms aggregation: a filter
+// is one bucket (code 2) where its row passes, and a terms aggregation under a filter keeps its column's codes (src) there;
+// 0 (no bucket) elsewhere
+__global__ void agg_row_codes_kernel(const uint32_t* __restrict__ row, const uint32_t* __restrict__ src, int32_t n_docs,
+                                     uint32_t* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_docs) return;
+  out[i] = ((row[i >> 5] >> (i & 31)) & 1u) ? (src ? src[i] : 2u) : 0u;
+}
+
 struct KnnFilterOrdsLaunch {
   const uint32_t* rows; int words;
   const int32_t* grows;         // rows to compact: grows[blockIdx.y]

@@ -314,6 +314,16 @@ struct nrtgpu_batch {
   DevBuf<int32_t> nest_docs, nest_hcounts; DevBuf<float> nest_scores;
   DevBuf<AggLaunch> nest_launch;
   DevBuf<unsigned long long> p2_total; DevBuf<int32_t> p2_flags;   // the top-hits run's totalHits / pruned / terminated
+  // filter collectors (cb.agg_filters): one row per FILTER aggregation on this image (agg_rows), built by batch_filter_rows
+  // from the compiled filter queries (agg_fq) and the sorted value sets (agg_set), with the term bitmaps in agg_scratch (not
+  // the index's kNN scratch, which a concurrent kNN call owns); agg_gate[i]: the row that gates aggregation i, NULL: none
+  std::unique_ptr<nrtgpu_batch> agg_fq;
+  KnnScratch agg_scratch;
+  DevBuf<uint32_t> agg_rows; DevBuf<int64_t> agg_set;
+  const uint32_t* agg_gate[kMaxAggs] = {};
+  // the codes aggregation i counts through in the current run: its column's (agg_tab.codes), or, under a row, agg_row_codes_kernel's
+  DevBuf<uint32_t> agg_fcodes[kMaxAggs];
+  const uint32_t* agg_codes[kMaxAggs] = {};
   // second pass of QueryRescorer (nrtgpu_score_docs / nrtgpu_rescore_query)
   DevBuf<int32_t> sd_docs, sd_counts; DevBuf<uint8_t> sd_match; DevBuf<float> sd_scores, sd_first;
   bool limits_active = false, disallow_partial = false;
@@ -551,7 +561,9 @@ int nrtgpu_index_build(nrtgpu_ctx* ctx, const nrtgpu_shard_desc* d, nrtgpu_index
   {
     std::vector<const int64_t*> p64((size_t)d->n_columns, nullptr);
     std::vector<const int32_t*> p32((size_t)d->n_columns, nullptr);
-    std::vector<const uint8_t*> ph((size_t)d->n_columns, nullptr);
+    // (one more entry than columns, always NULL: the column a filter collector's aggregation names, a column without a has
+    // array, so agg_collect counts it through its codes alone)
+    std::vector<const uint8_t*> ph((size_t)d->n_columns + 1, nullptr);
     std::vector<const int64_t*> pmo((size_t)d->n_columns, nullptr), pmv((size_t)d->n_columns, nullptr);
     ix->col_multi.assign((size_t)d->n_columns, 0);
     for (int c = 0; c < d->n_columns; ++c) {
@@ -763,8 +775,10 @@ static int batch_compile(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& 
   return b->queries.upload_async(b->cb.queries.data(), b->cb.queries.size(), st);
 }
 
-// a search batch: compile, plan the work list, upload, set up sorted searchAfter, allocate the results and launch
-// slice_bounds_kernel
+static int batch_filter_rows(nrtgpu_batch* b, const BatchRequest& r, cudaStream_t st);
+
+// a search batch: compile, plan the work list, upload, set up sorted searchAfter, allocate the results, launch
+// slice_bounds_kernel and build the rows of the filter collectors
 static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r, cudaStream_t st) {
   int rc;
   if ((rc = batch_compile(b, ix, r, st))) return rc;
@@ -853,7 +867,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
     NRT_CUDA_TRY(cudaGetLastError());
   }
   if (!b->ev[0][0]) for (auto& r : b->ev) for (auto& e : r) NRT_CUDA_TRY(cudaEventCreate(&e));
-  return NRTGPU_OK;
+  return batch_filter_rows(b, r, st);
 }
 
 int nrtgpu_batch_prepare(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -966,14 +980,15 @@ static const uint64_t* ix_col_distinct(const nrtgpu_index* ix, int32_t c) {
   return (size_t)c < ix->col_distinct.size() ? ix->col_distinct[(size_t)c]->p : nullptr;
 }
 
-// Allocates the tables of the batch's collectors in its own buffers, n_buckets[i] buckets for terms aggregation i, and
+// Allocates the tables of the batch's collectors in its own buffers, n_buckets[i] buckets for terms aggregation i (1 for a
+// filter aggregation), and
 // resets them on `st`: counts to 0, min words to +inf and max words to -inf in ordered-double space, sums to 0.0 (the
 // "unset" values are applied at fetch). Fills every field of *t but the codes and distinct values, which are the caller's.
 static int batch_agg_tables(nrtgpu_batch* b, const int32_t* n_buckets, cudaStream_t st, AggTables* t) {
   int rc;
   for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
     const nrtgpu_aggregation& a = b->cb.aggs[i];
-    if (a.kind == NRTGPU_AGG_TERMS) {
+    if (a.kind == NRTGPU_AGG_TERMS || a.kind == NRTGPU_AGG_FILTER) {
       t->n_buckets[i] = n_buckets[i];
       if ((rc = b->agg_counts[i].alloc((size_t)b->nq * (size_t)std::max(n_buckets[i], 1)))) return rc;
       NRT_CUDA_TRY(cudaMemsetAsync(b->agg_counts[i].p, 0, b->agg_counts[i].bytes(), st));
@@ -991,6 +1006,25 @@ static int batch_agg_tables(nrtgpu_batch* b, const int32_t* n_buckets, cudaStrea
     if ((rc = b->nest_words[j].alloc((size_t)b->nq * (size_t)std::max(nb, 1)))) return rc;
     NRT_CUDA_TRY(cudaMemsetAsync(b->nest_words[j].p, n.kind == NRTGPU_AGG_MIN ? 0xff : 0x00, b->nest_words[j].bytes(), st));
     t->nest_words[j] = b->nest_words[j].p;
+  }
+  return NRTGPU_OK;
+}
+
+// The codes every aggregation of the run counts through (agg_codes): its column's codes in agg_tab, or, for an aggregation
+// a row gates (batch_filter_rows), agg_row_codes_kernel's: a filter collector is a one-bucket terms aggregation to the
+// probe kernel, and a terms aggregation under a filter counts its column's codes where the filter's row passes. So the
+// probe kernel's collector is the one it was before filter collectors, and the launches without them run the same code.
+static int batch_agg_codes(nrtgpu_batch* b, cudaStream_t st) {
+  for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
+    b->agg_codes[i] = b->agg_tab.codes[i];
+    const uint32_t* row = b->agg_gate[i];
+    if (!row) continue;
+    const int32_t n = b->ix->n_docs;
+    if (int rc = b->agg_fcodes[i].alloc((size_t)n)) return rc;
+    agg_row_codes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(row, b->cb.aggs[i].kind == NRTGPU_AGG_FILTER ? nullptr : b->agg_tab.codes[i],
+                                                                    n, b->agg_fcodes[i].p);
+    NRT_CUDA_TRY(cudaGetLastError());
+    b->agg_codes[i] = b->agg_fcodes[i].p;
   }
   return NRTGPU_OK;
 }
@@ -1018,6 +1052,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
     int32_t nb[kMaxAggs] = {};
     for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
       const int32_t c = b->cb.aggs[i].column;
+      nb[i] = 1;   // (a filter's one bucket)
       if (b->cb.aggs[i].kind != NRTGPU_AGG_TERMS) continue;
       nb[i] = b->ix->col_n_distinct[(size_t)c];
       t.codes[i] = ix_col_code(b->ix, c); t.distinct[i] = ix_col_distinct(b->ix, c);
@@ -1043,14 +1078,18 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         v3::ProbeLaunch P = probe_params(b);
         if (!b->cb.aggs.empty()) {
           const AggTables& t = b->agg_tab;
+          if ((rc_dbg = batch_agg_codes(b, st))) return rc_dbg;
           AggLaunch A; std::memset(&A, 0, sizeof(A));
           A.n_aggs = (int32_t)b->cb.aggs.size();
           for (int i = 0; i < A.n_aggs; ++i) {
             const nrtgpu_aggregation& a = b->cb.aggs[(size_t)i];
             A.a[i].kind = a.kind; A.a[i].column = a.column; A.a[i].value_type = a.value_type;
-            if (a.kind == NRTGPU_AGG_TERMS) {
+            if (a.kind == NRTGPU_AGG_FILTER) {   // a one-bucket terms aggregation over the image's column without a has array
+              A.a[i].kind = NRTGPU_AGG_TERMS; A.a[i].column = b->ix->n_columns;
+            }
+            if (a.kind == NRTGPU_AGG_TERMS || a.kind == NRTGPU_AGG_FILTER) {
               A.a[i].n_buckets = t.n_buckets[i];
-              A.a[i].counts = t.counts[i]; A.codes[i] = t.codes[i];
+              A.a[i].counts = t.counts[i]; A.codes[i] = b->agg_codes[i];
             } else {
               A.a[i].dvals = t.dvals[i];
             }
@@ -1180,7 +1219,7 @@ int nrtgpu_batch_fetch_ex(nrtgpu_batch* b, void* stream_, int32_t* out_docs, flo
   return batch_fetch_impl(b, stream_, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
 }
 
-// Nested top hits of terms aggregation `parent` (pass 2) over the batches bs[0 .. n_b) that counted into one set of tables
+// Nested top hits of terms or filter aggregation `parent` (pass 2) over the batches bs[0 .. n_b) that counted into one set of tables
 // (a single image: one batch; a searcher: one per leaf). Each batch's probe launch runs again with a collector that only
 // appends make_key(score, global doc) of the docs of returned buckets (slot map nest_slot) to per-(query, slot) segments
 // sized by the bucket counts h_cnt [nq*size]; its totalHits / pruned / terminated go to scratch, and theta / slice lists /
@@ -1232,9 +1271,10 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
       AggLaunch& A = launches[(size_t)l];
       std::memset(&A, 0, sizeof(A));
       A.n_aggs = 1;
-      A.a[0].kind = NRTGPU_AGG_TERMS; A.a[0].column = a.column; A.a[0].value_type = a.value_type;
+      A.a[0].kind = NRTGPU_AGG_TERMS; A.a[0].column = a.kind == NRTGPU_AGG_FILTER ? x->ix->n_columns : a.column;
+      A.a[0].value_type = a.value_type;
       A.a[0].n_buckets = x->agg_tab.n_buckets[parent];
-      A.codes[0] = x->agg_tab.codes[parent];   // counts stay NULL: the pass-1 tables are not touched
+      A.codes[0] = x->agg_codes[parent];   // the codes pass 1 counted through; counts stay NULL: the pass-1 tables are not touched
       A.nested_begin[1] = n_th;
       for (int k = 0; k < n_th; ++k) {
         AggNestedDev& d = A.nested[k];
@@ -1290,7 +1330,8 @@ static int batch_fetch_aggs(nrtgpu_batch* const* bs, int n_b, cudaStream_t st, c
   for (size_t i = 0; i < b->cb.aggs.size(); ++i) {
     const nrtgpu_aggregation& a = b->cb.aggs[i];
     const nrtgpu_aggregation_result& r = out[i];
-    if (a.kind == NRTGPU_AGG_TERMS) {
+    if (a.kind == NRTGPU_AGG_TERMS || a.kind == NRTGPU_AGG_FILTER) {
+      const bool filter = a.kind == NRTGPU_AGG_FILTER;   // one bucket per query (size 1): its count is the docCount
       int rc;
       const size_t n = (size_t)nq * a.size;
       if ((rc = b->agg_keys.alloc(n)) || (rc = b->agg_cnts.alloc(n)) || (rc = b->agg_n.alloc((size_t)nq)) || (rc = b->agg_tot.alloc((size_t)nq)) ||
@@ -1312,7 +1353,10 @@ static int batch_fetch_aggs(nrtgpu_batch* const* bs, int n_b, cudaStream_t st, c
         if ((rc = b->agg_bucket.alloc(n))) return rc;
         T.out_bucket = b->agg_bucket.p;
       }
-      if (order_by >= 0) {
+      if (filter) {
+        NRT_CUDA_TRY(cudaMemcpyAsync(b->agg_cnts.p, t.counts[i], n * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+        if (T.out_bucket) NRT_CUDA_TRY(cudaMemsetAsync(T.out_bucket, 0, n * sizeof(int32_t), st));
+      } else if (order_by >= 0) {
         NRT_CUDA_TRY(cudaFuncSetAttribute(agg_terms_by_value_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAggByValueSmem));
         agg_terms_by_value_kernel<<<nq, 256, kAggByValueSmem, st>>>(T, t.nest_words[(size_t)order_by], b->cb.nested[(size_t)order_by].kind);
       } else {
@@ -1345,11 +1389,13 @@ static int batch_fetch_aggs(nrtgpu_batch* const* bs, int n_b, cudaStream_t st, c
         h_cnt.resize(n);
         NRT_CUDA_TRY(cudaMemcpyAsync(h_cnt.data(), b->agg_cnts.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       }
-      if (r.bucket_keys) NRT_CUDA_TRY(cudaMemcpyAsync(r.bucket_keys, b->agg_keys.p, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
       if (r.bucket_counts) NRT_CUDA_TRY(cudaMemcpyAsync(r.bucket_counts, b->agg_cnts.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-      if (r.n_buckets) NRT_CUDA_TRY(cudaMemcpyAsync(r.n_buckets, b->agg_n.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-      if (r.total_buckets) NRT_CUDA_TRY(cudaMemcpyAsync(r.total_buckets, b->agg_tot.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-      if (r.other_counts) NRT_CUDA_TRY(cudaMemcpyAsync(r.other_counts, b->agg_other.p, (size_t)nq * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+      if (!filter) {   // (a filter's docCount is its only result)
+        if (r.bucket_keys) NRT_CUDA_TRY(cudaMemcpyAsync(r.bucket_keys, b->agg_keys.p, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        if (r.n_buckets) NRT_CUDA_TRY(cudaMemcpyAsync(r.n_buckets, b->agg_n.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        if (r.total_buckets) NRT_CUDA_TRY(cudaMemcpyAsync(r.total_buckets, b->agg_tot.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        if (r.other_counts) NRT_CUDA_TRY(cudaMemcpyAsync(r.other_counts, b->agg_other.p, (size_t)nq * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+      }
       NRT_CUDA_TRY(cudaStreamSynchronize(st));   // the scratch is reused by the next terms aggregation
       if (top_hits && (rc = batch_nested_top_hits(bs, n_b, st, (int)i, h_cnt, nres))) return rc;
     } else if (r.values) {
@@ -1749,11 +1795,8 @@ int nrtgpu_search_bool_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int3
                             const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
                             void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
                             int64_t* out_total_hits) {
-  if (n_aggs <= 0 || !aggs || !results) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool_aggs: no aggregations");
-  BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
-  r.aggs = aggs; r.n_aggs = n_aggs;
-  SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.aggs = results;
-  return search_bool_impl(ix, r, nullptr, stream, o);
+  return nrtgpu_search_bool_aggs_filtered(ix, clauses, n_clauses, queries, nq, top_k, flags, aggs, n_aggs, results, nullptr, 0, nullptr,
+                                          nullptr, nullptr, 0, nullptr, 0, stream, out_docs, out_scores, out_counts, out_total_hits);
 }
 
 int nrtgpu_search_bool_aggs_nested(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -1762,11 +1805,40 @@ int nrtgpu_search_bool_aggs_nested(nrtgpu_index* ix, const nrtgpu_clause* clause
                                    const nrtgpu_nested_aggregation* nested, int32_t n_nested,
                                    const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs,
                                    float* out_scores, int32_t* out_counts, int64_t* out_total_hits) {
+  return nrtgpu_search_bool_aggs_filtered(ix, clauses, n_clauses, queries, nq, top_k, flags, aggs, n_aggs, results, nested, n_nested,
+                                          nested_results, nullptr, nullptr, 0, nullptr, 0, stream, out_docs, out_scores, out_counts,
+                                          out_total_hits);
+}
+
+// the request of the additional-collector entry points (single image and searcher): exhaustive, with the collectors
+static int aggs_request(BatchRequest* r, const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                        const nrtgpu_nested_aggregation* nested, int32_t n_nested, const nrtgpu_nested_result* nested_results,
+                        const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses,
+                        const nrtgpu_query* filter_queries, int32_t n_filter_queries) {
   if (n_aggs <= 0 || !aggs || !results) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool_aggs: no aggregations");
   if (n_nested < 0 || (n_nested > 0 && (!nested || !nested_results))) NRT_FAIL(NRTGPU_ERR_INVALID, "nested aggregations: NULL argument");
+  if (n_filter_clauses < 0 || n_filter_queries < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "filter aggregation: negative filter query count");
+  r->total_hits_threshold = INT32_MAX;
+  r->aggs = aggs; r->n_aggs = n_aggs;
+  if (n_nested > 0) { r->nested = nested; r->n_nested = n_nested; }
+  r->agg_filters = agg_filters;
+  r->filter_clauses = filter_clauses; r->n_filter_clauses = n_filter_clauses;
+  r->filter_queries = filter_queries; r->n_filter_queries = n_filter_queries;
+  return NRTGPU_OK;
+}
+
+int nrtgpu_search_bool_aggs_filtered(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                     const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                     const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                                     const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                     const nrtgpu_nested_result* nested_results, const nrtgpu_agg_filter* agg_filters,
+                                     const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses,
+                                     const nrtgpu_query* filter_queries, int32_t n_filter_queries, void* stream,
+                                     int32_t* out_docs, float* out_scores, int32_t* out_counts, int64_t* out_total_hits) {
   BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
-  r.aggs = aggs; r.n_aggs = n_aggs;
-  if (n_nested > 0) { r.nested = nested; r.n_nested = n_nested; }
+  int rc = aggs_request(&r, aggs, n_aggs, results, nested, n_nested, nested_results, agg_filters, filter_clauses, n_filter_clauses,
+                        filter_queries, n_filter_queries);
+  if (rc) return rc;
   SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.aggs = results;
   o.nested = n_nested > 0 ? nested_results : nullptr;
   return search_bool_impl(ix, r, nullptr, stream, o);
@@ -1989,12 +2061,12 @@ int32_t nrtgpu_knn_last_uncertified(const nrtgpu_index* ix) { return ix ? ix->kn
 
 struct KnnFilterRows { const uint32_t* bits = nullptr; int32_t* ord_cnt = nullptr; std::vector<int32_t> cnt; };
 
-// The rows of the filters row_filter[] of b (that fit kKnnFilterRowBytes): bit d of row r of bits (device [n_rows][words])
-// is set iff live doc d matches filter row_filter[r], cnt[r] counts them, ord_cnt (device [n_rows], zeroed) is the gather
-// path's. Adds the device time to the filter statistics.
-static int knn_filter_rows(nrtgpu_index* ix, const nrtgpu_batch* b, const std::vector<int32_t>& row_filter, cudaStream_t st,
-                           KnnFilterRows& out) {
-  KnnScratch& sc = ix->knn_scratch;
+// The rows of the filters row_filter[] of b (the compiled filter queries): bit d of row r of `rows` (the caller's device
+// buffer, [n_rows][words]) is set iff live doc d matches filter row_filter[r]; cnt[r] counts them, ord_cnt (device [n_rows],
+// zeroed) is the kNN gather path's. The term bitmaps and row metadata live in the caller's scratch sc. Asynchronous on st:
+// the caller synchronises it before it reads cnt.
+static int filter_rows(nrtgpu_index* ix, const nrtgpu_batch* b, const std::vector<int32_t>& row_filter, KnnScratch& sc,
+                       uint32_t* dRows, cudaStream_t st, KnnFilterRows& out) {
   const int n_rows = (int)row_filter.size(), words = (ix->n_docs + 31) / 32;
   // ---- group the rows so that the bitmaps of a group's distinct terms fit kKnnFilterTermBytes; a term clause points
   //      at its term's bitmap inside its group (terms without postings at none)
@@ -2026,8 +2098,7 @@ static int knn_filter_rows(nrtgpu_index* ix, const nrtgpu_batch* b, const std::v
   }
   grp_row.push_back(n_rows); grp_term.push_back((int)term_base.size());
   const int n_terms = (int)term_base.size();
-  uint32_t* dRows = nullptr; int64_t* dTerm = nullptr; int32_t* dMeta = nullptr;
-  NRT_KNN_GET(KnnSlot::Rows, dRows, (size_t)n_rows * words * 4);
+  int64_t* dTerm = nullptr; int32_t* dMeta = nullptr;
   NRT_KNN_GET(KnnSlot::Terms, dTerm, (size_t)(2 * n_terms + 1) * 8);
   NRT_KNN_GET(KnnSlot::RowMeta, dMeta, (size_t)(3 * n_rows + n_cl + 1) * 4);   // row_filter | row_cnt | ord_cnt | clause_term
   int32_t *dRowFilter = dMeta, *dRowCnt = dMeta + n_rows, *dClauseTerm = dMeta + 3 * n_rows;
@@ -2036,8 +2107,6 @@ static int knn_filter_rows(nrtgpu_index* ix, const nrtgpu_batch* b, const std::v
   NRT_CUDA_TRY(cudaMemcpyAsync(dRowFilter, row_filter.data(), (size_t)n_rows * 4, cudaMemcpyHostToDevice, st));
   NRT_CUDA_TRY(cudaMemsetAsync(dRowCnt, 0, (size_t)2 * n_rows * 4, st));
   NRT_CUDA_TRY(cudaMemcpyAsync(dClauseTerm, clause_term.data(), clause_term.size() * 4, cudaMemcpyHostToDevice, st));
-  if (!ix->knn_ev[0]) for (auto& e : ix->knn_ev) NRT_CUDA_TRY(cudaEventCreate(&e));
-  NRT_CUDA_TRY(cudaEventRecord(ix->knn_ev[0], st));
   // ---- per group: term bitmaps, then the rows
   size_t group_bytes = 0;
   for (size_t g = 0; g + 1 < grp_row.size(); ++g) group_bytes = std::max(group_bytes, (size_t)(grp_term[g + 1] - grp_term[g]) * term_bytes);
@@ -2058,13 +2127,87 @@ static int knn_filter_rows(nrtgpu_index* ix, const nrtgpu_batch* b, const std::v
     knn_filter_rows_kernel<<<dim3((unsigned)((words + 255) / 256), (unsigned)(grp_row[g + 1] - grp_row[g])), 256, 0, st>>>(R);
     NRT_CUDA_TRY(cudaGetLastError());
   }
-  NRT_CUDA_TRY(cudaEventRecord(ix->knn_ev[1], st));
   out.bits = dRows; out.ord_cnt = dMeta + 2 * n_rows; out.cnt.assign((size_t)n_rows, 0);
   NRT_CUDA_TRY(cudaMemcpyAsync(out.cnt.data(), dRowCnt, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, st));
+  return NRTGPU_OK;
+}
+
+// The rows of a kNN call's filters (filter_rows in the index's kNN scratch); adds their device time to the filter statistics.
+static int knn_filter_rows(nrtgpu_index* ix, const nrtgpu_batch* b, const std::vector<int32_t>& row_filter, cudaStream_t st,
+                           KnnFilterRows& out) {
+  KnnScratch& sc = ix->knn_scratch;
+  uint32_t* dRows = nullptr;
+  NRT_KNN_GET(KnnSlot::Rows, dRows, row_filter.size() * (size_t)((ix->n_docs + 31) / 32) * 4);
+  if (!ix->knn_ev[0]) for (auto& e : ix->knn_ev) NRT_CUDA_TRY(cudaEventCreate(&e));
+  NRT_CUDA_TRY(cudaEventRecord(ix->knn_ev[0], st));
+  if (int rc = filter_rows(ix, b, row_filter, sc, dRows, st, out)) return rc;
+  NRT_CUDA_TRY(cudaEventRecord(ix->knn_ev[1], st));
   NRT_CUDA_TRY(cudaStreamSynchronize(st));
   float ms = 0.0f;
   NRT_CUDA_TRY(cudaEventElapsedTime(&ms, ix->knn_ev[0], ix->knn_ev[1]));
   ix->knn_last_filter_ms += ms;
+  return NRTGPU_OK;
+}
+
+// The rows of the batch's FILTER aggregations on its image (batch_build; nothing without them): the k-th FILTER aggregation
+// owns row k of agg_rows, the filter queries' rows first (filter_rows on the filters compiled into agg_fq, as the kNN
+// filters are), then the value sets' (agg_value_set_kernel, each set sorted and de-duplicated here). A filter under a filter
+// then ANDs its parent's row into its own, in request order, so one row gates each aggregation: agg_gate[i] is aggregation
+// i's own row for a FILTER aggregation, its filter_agg's row for a TERMS one (batch_agg_codes turns them into codes).
+static int batch_filter_rows(nrtgpu_batch* b, const BatchRequest& r, cudaStream_t st) {
+  std::fill(b->agg_gate, b->agg_gate + kMaxAggs, nullptr);
+  const CompiledBatch& cb = b->cb;
+  nrtgpu_index* ix = b->ix;
+  std::vector<int32_t> row_filter, sets, row_of(cb.aggs.size(), -1);
+  for (size_t i = 0; i < cb.aggs.size(); ++i)
+    if (cb.aggs[i].kind == NRTGPU_AGG_FILTER) {
+      if (cb.agg_filters[i].kind == NRTGPU_AGG_FILTER_QUERY) { row_of[i] = (int32_t)row_filter.size(); row_filter.push_back(cb.agg_filters[i].query); }
+      else sets.push_back((int32_t)i);
+    }
+  const int n_rows = (int)(row_filter.size() + sets.size()), words = (ix->n_docs + 31) / 32;
+  if (n_rows == 0) return NRTGPU_OK;
+  int rc;
+  if (cb.agg_filter_queries) {   // compiled here, before any run, so that a refused filter writes no output
+    if (!b->agg_fq) b->agg_fq.reset(new nrtgpu_batch);
+    if ((rc = batch_compile(b->agg_fq.get(), ix, compile_only_request(r.filter_clauses, r.n_filter_clauses, r.filter_queries,
+                                                                      r.n_filter_queries), st))) return rc;
+  }
+  if (words == 0) return NRTGPU_OK;   // an image without docs: nothing is collected
+  if ((rc = b->agg_rows.alloc((size_t)n_rows * words))) return rc;
+  KnnFilterRows qrows;
+  if (!row_filter.empty() && (rc = filter_rows(ix, b->agg_fq.get(), row_filter, b->agg_scratch, b->agg_rows.p, st, qrows))) return rc;
+  std::vector<int64_t> vals;   // the sets, sorted and distinct, one after the other
+  std::vector<size_t> set_at;
+  for (int32_t i : sets) {
+    const nrtgpu_agg_filter& f = cb.agg_filters[(size_t)i];
+    set_at.push_back(vals.size());
+    const size_t at = vals.size();
+    vals.insert(vals.end(), f.values, f.values + f.n_values);
+    std::sort(vals.begin() + (std::ptrdiff_t)at, vals.end());
+    vals.erase(std::unique(vals.begin() + (std::ptrdiff_t)at, vals.end()), vals.end());
+  }
+  set_at.push_back(vals.size());
+  if ((rc = b->agg_set.upload_async(vals.data(), vals.size(), st))) return rc;
+  for (size_t k = 0; k < sets.size(); ++k) {
+    const int32_t i = sets[k];
+    row_of[(size_t)i] = (int32_t)(row_filter.size() + k);
+    AggValueSetLaunch L;
+    L.ix = ix->view(); L.column = cb.agg_filters[(size_t)i].column; L.n_set = (int32_t)(set_at[k + 1] - set_at[k]); L.words = words;
+    L.set = b->agg_set.p + set_at[k]; L.row = b->agg_rows.p + (size_t)row_of[(size_t)i] * words;
+    agg_value_set_kernel<<<(unsigned)(((int64_t)words * 32 + 255) / 256), 256, 0, st>>>(L);
+    NRT_CUDA_TRY(cudaGetLastError());
+  }
+  for (size_t i = 0; i < cb.aggs.size(); ++i) {
+    const nrtgpu_aggregation& a = cb.aggs[i];
+    uint32_t* own = row_of[i] >= 0 ? b->agg_rows.p + (size_t)row_of[i] * words : nullptr;
+    const uint32_t* parent = a.filter_agg > 0 ? b->agg_gate[a.filter_agg - 1] : nullptr;
+    if (own && parent) {
+      row_and_kernel<<<(unsigned)((words + 255) / 256), 256, 0, st>>>(own, parent, words);
+      NRT_CUDA_TRY(cudaGetLastError());
+    }
+    b->agg_gate[i] = own ? own : parent;
+  }
+  NRT_CUDA_TRY(cudaStreamSynchronize(st));   // (the host sets and counts are read by the async copies)
   return NRTGPU_OK;
 }
 
@@ -2577,8 +2720,6 @@ int nrtgpu_searcher_search_knn_filtered(nrtgpu_searcher* s, const float* queries
   }, out_docs, out_scores, out_counts, nullptr, nullptr, nullptr, nullptr);
 }
 
-// Aggregations over the leaves: every leaf's batch counts into one set of reader-wide tables through its codes renumbered
-// to the column's reader-wide dictionary (searcher_dict); the selection and the nested top hits then run once on them
 int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
                                             const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
                                             const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
@@ -2586,16 +2727,32 @@ int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_cla
                                             const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs,
                                             float* out_scores, int32_t* out_counts, int64_t* out_total_hits) {
   if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_bool_aggs_nested: NULL searcher");
-  if (n_aggs <= 0 || !aggs || !results) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool_aggs: no aggregations");
-  if (n_nested < 0 || (n_nested > 0 && (!nested || !nested_results))) NRT_FAIL(NRTGPU_ERR_INVALID, "nested aggregations: NULL argument");
+  return nrtgpu_searcher_search_bool_aggs_filtered(s, clauses, n_clauses, queries, nq, top_k, flags, aggs, n_aggs, results, nested,
+                                                   n_nested, nested_results, nullptr, nullptr, 0, nullptr, 0, stream, out_docs,
+                                                   out_scores, out_counts, out_total_hits);
+}
+
+// Aggregations over the leaves: every leaf's batch counts into one set of reader-wide tables through its codes renumbered
+// to the column's reader-wide dictionary (searcher_dict) and tests its own image's filter rows; the selection and the
+// nested top hits then run once on them
+int nrtgpu_searcher_search_bool_aggs_filtered(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                              const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                              const nrtgpu_aggregation* aggs, int32_t n_aggs,
+                                              const nrtgpu_aggregation_result* results, const nrtgpu_nested_aggregation* nested,
+                                              int32_t n_nested, const nrtgpu_nested_result* nested_results,
+                                              const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses,
+                                              int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
+                                              int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores,
+                                              int32_t* out_counts, int64_t* out_total_hits) {
+  if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_bool_aggs_filtered: NULL searcher");
   BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
-  r.aggs = aggs; r.n_aggs = n_aggs;
-  if (n_nested > 0) { r.nested = nested; r.n_nested = n_nested; }
+  int rc = aggs_request(&r, aggs, n_aggs, results, nested, n_nested, nested_results, agg_filters, filter_clauses, n_filter_clauses,
+                        filter_queries, n_filter_queries);
+  if (rc) return rc;
   NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> g(s->mu);
   const int n_leaves = (int)s->leaves.size();
-  int rc;
   {   // every refusal of the single-image call, on every leaf's columns, before any batch is built
     CompiledBatch cb;
     for (nrtgpu_index* ix : s->leaves)
@@ -2605,6 +2762,7 @@ int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_cla
   const ReaderDict* dict[kMaxAggs] = {};
   int32_t n_buckets[kMaxAggs] = {};
   for (int i = 0; i < n_aggs; ++i) {
+    n_buckets[i] = 1;   // (a filter's one bucket)
     if (aggs[i].kind != NRTGPU_AGG_TERMS) continue;
     if ((rc = searcher_dict(s, aggs[i].column, st, &dict[i]))) return rc;
     n_buckets[i] = dict[i]->n;

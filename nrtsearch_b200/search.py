@@ -22,7 +22,7 @@ from typing import List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _native
-from ._native import (Aggregation as CAgg, AggregationResult as CAggResult, NestedAggregation as CNested,
+from ._native import (AggFilter as CAggFilter, Aggregation as CAgg, AggregationResult as CAggResult, NestedAggregation as CNested,
                       NestedResult as CNestedResult, Clause, CollectionTimeoutException, NrtGpuError,
                       NrtGpuUnsupported, Query as CQuery, SearchLimits, Sort as CSort, check)
 from .index import HostShard, PinnedDesc
@@ -257,6 +257,37 @@ class MaxCollector:
 class SumCollector:
     column: int
     field_type: str = "long"
+
+
+@dataclass(frozen=True)
+class ValueSetFilter:
+    """The set filter of a FilterCollector (FilterCollectorManager.SetQueryFilter over a TermInSetQuery): a doc passes when one
+    of its values of `column` (single- or multi-valued) is in `values`, numbers of the field's type compared as Java's boxed
+    equals does, by their bits (-0.0 != 0.0, NaN == NaN). A set of another term type than the field's never matches in the
+    reference: the adaptor passes an empty set for it."""
+    column: int
+    values: tuple
+    field_type: str = "long"
+
+    def sortable(self) -> np.ndarray:
+        """the values in the column's sortable-long domain"""
+        if self.field_type == "float":
+            return np.array([float_to_sortable_int(v) for v in self.values], np.int64)
+        if self.field_type == "double":
+            return np.array([double_to_sortable_long(v) for v in self.values], np.int64)
+        return np.array([int(v) for v in self.values], np.int64)
+
+
+@dataclass(frozen=True)
+class FilterCollector:
+    """FilterCollector (FilterCollectorManager): of the docs a query collects, those that pass `filter` are counted (the
+    docCount) and handed to the nested collectors. filter: a flat query (BooleanQuery / TermQuery / RangeQuery /
+    MatchAllDocsQuery; only matching counts) or a ValueSetFilter. nested: (name, TermsCollector | MinCollector | MaxCollector |
+    SumCollector | TopHitsCollector | FilterCollector) pairs, at least one. Its result is {"doc_count": int32 [nq], name:
+    the nested collector's result}: a terms or filter collector's own result, float64 [nq] (min / max / sum), or {"docs",
+    "scores" [nq, top_hits - start_hit], "counts", "total_hits" [nq]} (top hits)."""
+    filter: object
+    nested: tuple = ()
 
 
 _VALUE_TYPE = {"int": 0, "long": 0, "float": 1, "double": 2}
@@ -624,6 +655,84 @@ def _collector_records(nq: int, additional: Sequence[object]):
     return aggs, res, narr, nres, len(nested), outs
 
 
+class _FilteredRecords:
+    """The records of a batch whose additional collectors hold filter collectors (nrtgpu_search_bool_aggs_filtered): every
+    terms, min / max / sum and filter collector becomes an nrtgpu_aggregation, a terms or filter collector under a filter
+    names it by filter_agg (parents before children), a min / max / sum / top hits under a filter is a nested collector of
+    it, and each filter gets its nrtgpu_agg_filter record (filter queries compiled by compile_queries). outs: the result
+    objects the call fills, one per top-level collector; args: the records in the entry point's order."""
+
+    def __init__(self, nq: int, additional: Sequence[object]):
+        self.nq = nq
+        self.aggs, self.res, self.filters, self.nested, self.nested_res = [], [], [], [], []
+        self.filter_queries, self.keep = [], []
+        self.outs = [self._add(a, 0) for a in additional]
+        n = len(self.aggs)
+        aggs, res = (CAgg * n)(*self.aggs), (CAggResult * n)(*self.res)
+        filt = (CAggFilter * n)(*self.filters)
+        narr = (CNested * len(self.nested))(*self.nested) if self.nested else None
+        nres = (CNestedResult * len(self.nested))(*self.nested_res) if self.nested else None
+        fcarr, fncl, fqarr, fnq = compile_queries(self.filter_queries) if self.filter_queries else (None, 0, None, 0)
+        self.args = (aggs, n, res, narr, len(self.nested), nres, filt, fcarr, fncl, fqarr, fnq)
+
+    def _add(self, a, filter_agg: int):
+        nq, i = self.nq, len(self.aggs)
+        self.filters.append(CAggFilter())
+        if isinstance(a, TermsCollector):
+            self.aggs.append(CAgg(1, a.column, _VALUE_TYPE[a.field_type], a.size, 1 if a.order_desc else 0, filter_agg))
+            o = {"keys": np.zeros((nq, a.size), np.int64), "counts": np.zeros((nq, a.size), np.int32), "n": np.zeros(nq, np.int32),
+                 "total_buckets": np.zeros(nq, np.int32), "other_counts": np.zeros(nq, np.int64)}
+            self.res.append(CAggResult(None, o["keys"].ctypes.data, o["counts"].ctypes.data, o["n"].ctypes.data,
+                                       o["total_buckets"].ctypes.data, o["other_counts"].ctypes.data))
+            if a.nested or a.order_by is not None:
+                o["nested"] = _nested_specs(i, a, nq, self.nested, self.nested_res)
+            return o
+        if isinstance(a, FilterCollector):
+            self.aggs.append(CAgg(6, 0, 0, 0, 0, filter_agg))
+            o = {"doc_count": np.zeros(nq, np.int32)}
+            self.res.append(CAggResult(None, None, o["doc_count"].ctypes.data, None, None, None))
+            f = a.filter
+            if isinstance(f, ValueSetFilter):
+                vals = np.ascontiguousarray(f.sortable(), np.int64)
+                self.keep.append(vals)
+                self.filters[i] = CAggFilter(2, 0, f.column, len(vals), vals.ctypes.data if len(vals) else None)
+            else:
+                self.filters[i] = CAggFilter(1, len(self.filter_queries), 0, 0, None)
+                self.filter_queries.append(f)
+            names = [name for name, _ in a.nested]
+            if len(set(names)) != len(names) or "doc_count" in names:
+                raise ValueError("nested collector names must be unique and not 'doc_count'")
+            for name, c in a.nested:
+                if isinstance(c, (TermsCollector, FilterCollector)):
+                    o[name] = self._add(c, i + 1)
+                elif isinstance(c, TopHitsCollector):
+                    w = max(c.top_hits - c.start_hit, 0)
+                    r = {"docs": np.zeros((nq, w), np.int32), "scores": np.zeros((nq, w), np.float32),
+                         "counts": np.zeros(nq, np.int32), "total_hits": np.zeros(nq, np.int64)}
+                    self.nested.append(CNested(i, 5, 0, 0, c.top_hits, c.start_hit, 0, 0))
+                    self.nested_res.append(CNestedResult(None, r["docs"].ctypes.data, r["scores"].ctypes.data,
+                                                         r["counts"].ctypes.data, r["total_hits"].ctypes.data))
+                    o[name] = r
+                elif isinstance(c, (MinCollector, MaxCollector, SumCollector)):
+                    kind = 2 if isinstance(c, MinCollector) else 3 if isinstance(c, MaxCollector) else 4
+                    r = np.zeros(nq, np.float64)
+                    self.nested.append(CNested(i, kind, c.column, _VALUE_TYPE[c.field_type], 0, 0, 0, 0))
+                    self.nested_res.append(CNestedResult(r.ctypes.data, None, None, None, None))
+                    o[name] = r
+                else:
+                    raise ValueError(f"nested collector {name!r}: {type(c).__name__} is not on the GPU path")
+            return o
+        kind = 2 if isinstance(a, MinCollector) else 3 if isinstance(a, MaxCollector) else 4
+        self.aggs.append(CAgg(kind, a.column, _VALUE_TYPE[a.field_type], 0, 0, 0))
+        o = np.zeros(nq, np.float64)
+        self.res.append(CAggResult(o.ctypes.data, None, None, None, None, None))
+        return o
+
+
+def _has_filter(additional: Sequence[object]) -> bool:
+    return any(isinstance(a, FilterCollector) for a in additional)
+
+
 def _nested_specs(parent: int, a: TermsCollector, nq: int, nested: list, nested_res: list) -> dict:
     """the nrtgpu_nested_aggregation records and result buffers of terms collector `parent` (appended to nested /
     nested_res); returns the result dict they fill"""
@@ -790,13 +899,19 @@ class GpuIndexSearcher:
         """IndexSearcher.search with additional collectors (SearchCollectorManager fan-out): returns (BatchResult, results)
         where results[i] is a float64 [nq] array (min / max / sum) or a dict of bucket arrays (terms). A terms collector with
         nested collectors adds "nested": {name: float64 [nq, size] (min / max / sum) or {"docs", "scores" [nq, size,
-        top_hits - start_hit], "counts", "total_hits" [nq, size]} (top hits)}, per returned bucket."""
+        top_hits - start_hit], "counts", "total_hits" [nq, size]} (top hits)}, per returned bucket. A FilterCollector's result
+        is the dict its docstring describes (nrtgpu_search_bool_aggs_filtered)."""
         carr, ncl, qarr, nq = compile_queries(queries)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
-        aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         hits = (out.docs.ctypes.data, out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data)
+        if _has_filter(additional):   # filter collectors: the flattened records of _FilteredRecords
+            fr = _FilteredRecords(nq, additional)
+            check(self._lib.nrtgpu_search_bool_aggs_filtered(self.index.handle, carr, ncl, qarr, nq, k, 0, *fr.args,
+                                                             C.c_void_p(stream), *hits))
+            return out, fr.outs
+        aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         if n_nested:
             check(self._lib.nrtgpu_search_bool_aggs_nested(self.index.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
                                                            narr, n_nested, nres, C.c_void_p(stream), *hits))
@@ -1010,6 +1125,12 @@ class GpuLeafSearcher:
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
+        if _has_filter(additional):
+            fr = _FilteredRecords(nq, additional)
+            check(self._lib.nrtgpu_searcher_search_bool_aggs_filtered(self.handle, carr, ncl, qarr, nq, k, 0, *fr.args,
+                                                                      C.c_void_p(stream), out.docs.ctypes.data, out.scores.ctypes.data,
+                                                                      out.counts.ctypes.data, out.total_hits.ctypes.data))
+            return out, fr.outs
         aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         check(self._lib.nrtgpu_searcher_search_bool_aggs_nested(self.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
                                                                 narr, n_nested, nres, C.c_void_p(stream), out.docs.ctypes.data,
