@@ -505,6 +505,43 @@ int nrtgpu_search_bool_aggs_filtered(nrtgpu_index* ix, const nrtgpu_clause* clau
                                      const nrtgpu_query* filter_queries, int32_t n_filter_queries, void* stream,
                                      int32_t* out_docs, float* out_scores, int32_t* out_counts, int64_t* out_total_hits);
 
+/* Sorted top hits (TopHitsCollector with a querySort: TopHitsCollectorManager.java:126-130 uses
+ * TopFieldCollectorManager(sort, top_hits, null, Integer.MAX_VALUE) instead of the score collector). nested_sorts is an
+ * array parallel to `nested` (NULL: every top hits by score); entry j, read for a TOP_HITS record only:
+ *   orders   NULL: by score, exactly as nrtgpu_search_bool_aggs_filtered. Else the Sort's nrtgpu_sort_order: orders[0] on
+ *            the single image; one per leaf, in leaf order, for a searcher (as nrtgpu_searcher_search_sorted_fields takes
+ *            them). The bucket's docs are ordered by the Sort with the rules of nrtgpu_search_sorted_fields: a column
+ *            ascending unless reverse, missing_value for a doc without a value, the MIN / MAX selector on a multi-valued
+ *            column; DOCID the global doc id; a leading SCORE the float the top-level hit list gives that doc. Ties go to
+ *            the smaller global doc. Positions [start_hit, top_hits) are returned, hit_total is the bucket's count.
+ *            hit_scores are NaN (the reduce sets Hit.score = Double.NaN); a leading SCORE's value is in `values`.
+ *   values   NULL, or [nq*size*(top_hits-start_hit)*n_fields] (size 1 under a FILTER parent): FieldDoc.fields of every
+ *            returned hit, in the encoding of out_sort_values of nrtgpu_search_sorted_fields; 0 past hit_counts.
+ * A top-level TopHitsCollector ("the page by relevance, plus the 5 newest matches") is the nested top hits of a FILTER
+ * aggregation whose filter query is match-all: every doc the query collects passes, so hit_total is the query's totalHits.
+ * On a searcher each leaf selects its own top_hits of a bucket by its order, and the leaves' lists are merged as
+ * TopFieldDocs.merge does (nrtgpu_merge_sorted_packed); the lists of one pass-2 group of queries take
+ * (n_leaves + 1) * nq_group * size * (top_hits * (1 + 2 * n_fields) + 4) * 4 bytes per sorted collector, and the groups
+ * are cut so that this stays under 512 MB unless one query needs more by itself.
+ * nrtgpu_search_bool_aggs_filtered is this call without nested_sorts.
+ *   NRTGPU_ERR_INVALID, beside every refusal of nrtgpu_search_bool_aggs_filtered: orders on a record that is not TOP_HITS,
+ *     a NULL order, an order made on another index (or, for a searcher, another leaf), leaf orders of different Sorts.
+ *     orders_parent on a TOP_HITS stays 'top hits cannot order the buckets'. The 8-field limit and the SCORE-first rule are
+ *     nrtgpu_sort_order_create's. A refused call writes no output. */
+typedef struct {
+  const nrtgpu_sort_order* const* orders;   /* NULL: by score; else [1] (single image) or [n_leaves] (searcher) */
+  int64_t* values;                          /* [nq*size*(top_hits-start_hit)*n_fields] or NULL */
+} nrtgpu_nested_sort;
+int nrtgpu_search_bool_aggs_sorted_hits(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                        const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                        const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                                        const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                        const nrtgpu_nested_result* nested_results, const nrtgpu_nested_sort* nested_sorts,
+                                        const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses,
+                                        int32_t n_filter_clauses, const nrtgpu_query* filter_queries, int32_t n_filter_queries,
+                                        void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
+                                        int64_t* out_total_hits);
+
 /* QueryRescorer second pass (QueryRescore.java:39-57 -> Lucene QueryRescorer.rescore): query q of the batch evaluated on
  * ITS OWN hit list docs[q][0..counts[q]) (global doc ids): out_matches / out_scores [nq*n_hits]. */
 int nrtgpu_score_docs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
@@ -752,6 +789,20 @@ int nrtgpu_searcher_search_bool_aggs_filtered(nrtgpu_searcher* s, const nrtgpu_c
                                               int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
                                               int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores,
                                               int32_t* out_counts, int64_t* out_total_hits);
+/* nrtgpu_searcher_search_bool_aggs_sorted_hits: nrtgpu_search_bool_aggs_sorted_hits over the leaves (one order per leaf in
+ * nested_sorts[j].orders); sorted top hits are selected per leaf and merged as TopFieldDocs.merge does, ties by global doc;
+ * top hits by score are chosen over every leaf at once as before. nrtgpu_searcher_search_bool_aggs_filtered is this call
+ * without nested_sorts. */
+int nrtgpu_searcher_search_bool_aggs_sorted_hits(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                                 const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                                 const nrtgpu_aggregation* aggs, int32_t n_aggs,
+                                                 const nrtgpu_aggregation_result* results,
+                                                 const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                                 const nrtgpu_nested_result* nested_results, const nrtgpu_nested_sort* nested_sorts,
+                                                 const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses,
+                                                 int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
+                                                 int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores,
+                                                 int32_t* out_counts, int64_t* out_total_hits);
 
 /* Request micro-batcher: the reference's search API is ONE query per RPC (clientlib/src/main/proto/yelp/nrtsearch/
  * luceneserver.proto:164), each on its own SERVER-pool thread (GrpcServerExecutorSupplier.java:68-75). Handler threads call

@@ -199,6 +199,27 @@ public final class NrtGpu {
       ByteBuffer[] filterValues, ByteBuffer filterClauses, int nFilterClauses, ByteBuffer filterQueries, int nFilterQueries,
       ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits);
 
+  /**
+   * searchBoolAggsFiltered plus sorted top hits (TopHitsCollector.querySort; include/nrtgpu.h
+   * nrtgpu_search_bool_aggs_sorted_hits): sortOrders[j] the sort-order handles of nested collector j (one, from
+   * sortOrderCreate on this index; null: by score), sortValues[j] a direct buffer for its FieldDoc values (or null). A
+   * top-level TopHitsCollector is the nested top hits of a FILTER aggregation with a match-all filter query.
+   */
+  public static native int searchBoolAggsSortedHits(
+      long index, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK, int flags, ByteBuffer aggs,
+      int nAggs, ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, long[][] sortOrders,
+      ByteBuffer[] sortValues, ByteBuffer aggFilters, ByteBuffer[] filterValues, ByteBuffer filterClauses, int nFilterClauses,
+      ByteBuffer filterQueries, int nFilterQueries, ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts,
+      ByteBuffer outTotalHits);
+
+  /** searchBoolAggsSortedHits over the leaves of a searcher: sortOrders[j] holds one order per leaf, in leaf order. */
+  public static native int searcherSearchBoolAggsSortedHits(
+      long searcher, ByteBuffer clauses, int nClauses, ByteBuffer queries, int nq, int topK, int flags, ByteBuffer aggs,
+      int nAggs, ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, long[][] sortOrders,
+      ByteBuffer[] sortValues, ByteBuffer aggFilters, ByteBuffer[] filterValues, ByteBuffer filterClauses, int nFilterClauses,
+      ByteBuffer filterQueries, int nFilterQueries, ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts,
+      ByteBuffer outTotalHits);
+
   public static native long batcherCreate(long index, int maxBatch, int maxWaitUs);
 
   /** Blocks until the batch this request rode in is back; diag = nrtgpu_diagnostics (24 bytes) or null. */

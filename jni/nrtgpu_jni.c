@@ -275,6 +275,58 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchBoolAggsF
   free(af);
   return fail(env, rc);
 }
+/* the nrtgpu_nested_sort records of nested collector j: sortOrders[j] a long[] of sort-order handles (one per image; null:
+ * by score), sortValues[j] a direct buffer for the FieldDoc values (or null). *orders holds the handle arrays (freed by
+ * the caller with free_nested_sorts). */
+static int nested_sort_records(JNIEnv* env, jobjectArray sortOrders, jobjectArray sortValues, jint nNested, nrtgpu_nested_sort** out,
+                               const nrtgpu_sort_order*** orders) {
+  *out = NULL; *orders = NULL;
+  if (!sortOrders || nNested <= 0) return NRTGPU_OK;
+  nrtgpu_nested_sort* s = *out = (nrtgpu_nested_sort*)calloc((size_t)nNested, sizeof(*s));
+  const nrtgpu_sort_order** o = *orders = (const nrtgpu_sort_order**)calloc((size_t)nNested * 64, sizeof(*o));
+  if (!s || !o) return NRTGPU_ERR_OOM;
+  for (jint j = 0; j < nNested; ++j) {
+    jlongArray h = (jlongArray)(*env)->GetObjectArrayElement(env, sortOrders, j);
+    if (!h) continue;
+    const jsize n = (*env)->GetArrayLength(env, h);
+    if (n > 64) return NRTGPU_ERR_INVALID;
+    jlong* v = (*env)->GetLongArrayElements(env, h, NULL);
+    for (jsize l = 0; l < n; ++l) o[(size_t)j * 64 + l] = (const nrtgpu_sort_order*)(intptr_t)v[l];
+    (*env)->ReleaseLongArrayElements(env, h, v, JNI_ABORT);
+    s[j].orders = o + (size_t)j * 64;
+    s[j].values = sortValues ? (int64_t*)ADDR(env, (*env)->GetObjectArrayElement(env, sortValues, j)) : NULL;
+  }
+  return NRTGPU_OK;
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchBoolAggsSortedHits(
+    JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
+    jobject aggs, jint nAggs, jobjectArray aggOut, jobject nested, jint nNested, jobjectArray nestedOut, jobjectArray sortOrders,
+    jobjectArray sortValues, jobject aggFilters, jobjectArray filterValues, jobject filterClauses, jint nFilterClauses,
+    jobject filterQueries, jint nFilterQueries, jobject outDocs, jobject outScores, jobject outCounts, jobject outTotalHits) {
+  nrtgpu_aggregation_result* ar = NULL;
+  nrtgpu_nested_result* nr = NULL;
+  nrtgpu_agg_filter* af = NULL;
+  nrtgpu_nested_sort* ns = NULL;
+  const nrtgpu_sort_order** so = NULL;
+  int rc = agg_results(env, aggOut, nAggs, nestedOut, nNested, &ar, &nr);
+  if (!rc) rc = agg_filter_records(env, aggFilters, filterValues, nAggs, &af);
+  if (!rc) rc = nested_sort_records(env, sortOrders, sortValues, nNested, &ns, &so);
+  if (!rc)
+    rc = nrtgpu_search_bool_aggs_sorted_hits((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                             (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                             (const nrtgpu_aggregation*)ADDR(env, aggs), nAggs, ar,
+                                             (const nrtgpu_nested_aggregation*)ADDR(env, nested), nNested, nr, ns, af,
+                                             (const nrtgpu_clause*)ADDR(env, filterClauses), nFilterClauses,
+                                             (const nrtgpu_query*)ADDR(env, filterQueries), nFilterQueries, NULL,
+                                             (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
+                                             (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
+  free(ar);
+  free(nr);
+  free(af);
+  free(ns);
+  free((void*)so);
+  return fail(env, rc);
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_fetchColumns(
     JNIEnv* env, jclass c, jlong ix, jobject colIds, jint nCols, jobject docs, jint n, jobject outValues, jobject outHas) {
   return fail(env, nrtgpu_fetch_columns((nrtgpu_index*)(intptr_t)ix, (const int32_t*)ADDR(env, colIds), nCols,
@@ -395,6 +447,35 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchB
   free(ar);
   free(nr);
   free(af);
+  return fail(env, rc);
+}
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchBoolAggsSortedHits(
+    JNIEnv* env, jclass c, jlong s, jobject clauses, jint nClauses, jobject queries, jint nq, jint topK, jint flags,
+    jobject aggs, jint nAggs, jobjectArray aggOut, jobject nested, jint nNested, jobjectArray nestedOut, jobjectArray sortOrders,
+    jobjectArray sortValues, jobject aggFilters, jobjectArray filterValues, jobject filterClauses, jint nFilterClauses,
+    jobject filterQueries, jint nFilterQueries, jobject outDocs, jobject outScores, jobject outCounts, jobject outTotalHits) {
+  nrtgpu_aggregation_result* ar = NULL;
+  nrtgpu_nested_result* nr = NULL;
+  nrtgpu_agg_filter* af = NULL;
+  nrtgpu_nested_sort* ns = NULL;
+  const nrtgpu_sort_order** so = NULL;
+  int rc = agg_results(env, aggOut, nAggs, nestedOut, nNested, &ar, &nr);
+  if (!rc) rc = agg_filter_records(env, aggFilters, filterValues, nAggs, &af);
+  if (!rc) rc = nested_sort_records(env, sortOrders, sortValues, nNested, &ns, &so);
+  if (!rc)
+    rc = nrtgpu_searcher_search_bool_aggs_sorted_hits((nrtgpu_searcher*)(intptr_t)s, (const nrtgpu_clause*)ADDR(env, clauses),
+                                                      nClauses, (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                                      (const nrtgpu_aggregation*)ADDR(env, aggs), nAggs, ar,
+                                                      (const nrtgpu_nested_aggregation*)ADDR(env, nested), nNested, nr, ns, af,
+                                                      (const nrtgpu_clause*)ADDR(env, filterClauses), nFilterClauses,
+                                                      (const nrtgpu_query*)ADDR(env, filterQueries), nFilterQueries, NULL,
+                                                      (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
+                                                      (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
+  free(ar);
+  free(nr);
+  free(af);
+  free(ns);
+  free((void*)so);
   return fail(env, rc);
 }
 

@@ -101,6 +101,12 @@ class NestedAggregation(C.Structure):
                 ("top_hits", C.c_int32), ("start_hit", C.c_int32), ("orders_parent", C.c_int32), ("reserved", C.c_int32)]
 
 
+class NestedSort(C.Structure):
+    """nrtgpu_nested_sort: the Sort of a nested top hits, one nrtgpu_sort_order per image (orders NULL: by score), and its
+    FieldDoc values output."""
+    _fields_ = [("orders", C.c_void_p), ("values", C.c_void_p)]
+
+
 class NestedResult(C.Structure):
     _fields_ = [("values", C.c_void_p), ("hit_docs", C.c_void_p), ("hit_scores", C.c_void_p), ("hit_counts", C.c_void_p),
                 ("hit_total", C.c_void_p)]
@@ -144,6 +150,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_searcher_search_sorted_fields", "nrtgpu_searcher_search_tree_phrases", "nrtgpu_searcher_search_knn",
     "nrtgpu_searcher_search_knn_filtered", "nrtgpu_searcher_search_bool_aggs_nested",
     "nrtgpu_search_bool_aggs_filtered", "nrtgpu_searcher_search_bool_aggs_filtered",
+    "nrtgpu_search_bool_aggs_sorted_hits", "nrtgpu_searcher_search_bool_aggs_sorted_hits",
 ]
 
 _gpu = None
@@ -256,6 +263,9 @@ def gpu_lib() -> C.CDLL:
         lib.nrtgpu_search_bool_aggs_filtered.argtypes = lib.nrtgpu_search_bool_aggs_nested.argtypes[:13] + \
             [C.POINTER(AggFilter), C.POINTER(Clause), C.c_int32, C.POINTER(Query), C.c_int32, C.c_void_p] + [C.c_void_p] * 4
         lib.nrtgpu_searcher_search_bool_aggs_filtered.argtypes = lib.nrtgpu_search_bool_aggs_filtered.argtypes
+        lib.nrtgpu_search_bool_aggs_sorted_hits.argtypes = lib.nrtgpu_search_bool_aggs_filtered.argtypes[:13] + \
+            [C.POINTER(NestedSort)] + lib.nrtgpu_search_bool_aggs_filtered.argtypes[13:]
+        lib.nrtgpu_searcher_search_bool_aggs_sorted_hits.argtypes = lib.nrtgpu_search_bool_aggs_sorted_hits.argtypes
         lib.nrtgpu_batcher_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
         lib.nrtgpu_batcher_submit.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Diagnostics)]

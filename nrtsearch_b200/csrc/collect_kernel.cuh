@@ -200,7 +200,10 @@ struct AggNestedDev {
   const int32_t* slot_of;       // TOP_HITS: [nq][n_buckets] returned slot of the bucket, -1: not returned
   const long long* hit_off;     // TOP_HITS: [q_hi - q_lo][size] first key of the (query, slot)
   unsigned int* hit_fill;       // TOP_HITS: [q_hi - q_lo][size] keys written
-  uint64_t* hit_keys;           // TOP_HITS: make_key(score, global doc) of the collected docs
+  uint64_t* hit_keys;           // TOP_HITS: make_key(score, global doc) of the collected docs, or their Sort keys (rank)
+  const uint32_t* rank;         // TOP_HITS by a Sort: the order's rank of each doc of the image (NULL: by score)
+  int32_t score_key;            // TOP_HITS: the key's high word is the ordered score (by score, or a Sort led by SCORE) ...
+  int32_t score_reverse;        // ... negated (a reversed leading SCORE: lower scores first)
 };
 struct AggLaunch {
   AggSpecDev a[kMaxAggs];
@@ -249,7 +252,11 @@ __device__ __noinline__ void agg_nested_collect(const AggLaunch& A, int i, const
     const int slot = n.slot_of[cell];
     if (slot < 0) continue;
     const size_t s = (size_t)(q - n.q_lo) * n.size + slot;
-    n.hit_keys[n.hit_off[s] + atomicAdd(&n.hit_fill[s], 1u)] = make_key(score, doc + n.doc_base);   // sized by the bucket's count
+    // by score make_key(score, global doc); by a Sort a key whose descending order is the Sort's: ~rank (unique, 1-based, it
+    // holds the doc tie-break), under a leading SCORE the ordered score above it, flipped for reverse (kSortScoreRank's key)
+    const uint32_t lo = n.rank ? n.rank[doc] : (uint32_t)(doc + n.doc_base);
+    const uint32_t hi = n.score_key ? float_to_ordered(n.score_reverse ? -score : score) : 0u;
+    n.hit_keys[n.hit_off[s] + atomicAdd(&n.hit_fill[s], 1u)] = ((uint64_t)hi << 32) | (uint32_t)~lo;   // sized by the bucket's count
   }
 }
 

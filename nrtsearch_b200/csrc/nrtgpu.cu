@@ -312,6 +312,9 @@ struct nrtgpu_batch {
   DevBuf<int32_t> agg_bucket, nest_slot; DevBuf<double> nest_vals;
   DevBuf<uint64_t> nest_keys; DevBuf<long long> nest_off; DevBuf<unsigned int> nest_fill;
   DevBuf<int32_t> nest_docs, nest_hcounts; DevBuf<float> nest_scores;
+  // sorted top hits: FieldDoc values of the results; over several leaves the group's packed sorted records (leaves', then
+  // merged) and the key scores of a leaf's selection
+  DevBuf<int64_t> nest_svals, nest_rec; DevBuf<float> nest_rscores;
   DevBuf<AggLaunch> nest_launch;
   DevBuf<unsigned long long> p2_total; DevBuf<int32_t> p2_flags;   // the top-hits run's totalHits / pruned / terminated
   // filter collectors (cb.agg_filters): one row per FILTER aggregation on this image (agg_rows), built by batch_filter_rows
@@ -1219,12 +1222,33 @@ int nrtgpu_batch_fetch_ex(nrtgpu_batch* b, void* stream_, int32_t* out_docs, flo
   return batch_fetch_impl(b, stream_, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
 }
 
+// The FieldDoc values of sorted nested top hits under order o (sort_fields_values_kernel): n lists of top_k docs that hold
+// rank + doc_base become global docs, their scores (key score words) NaN, and values [n][top_k][n_fields] are written; 0
+// past counts
+static int sorted_hit_values(const nrtgpu_sort_order* o, int32_t doc_base, int32_t* docs, const int32_t* counts, float* scores, int n,
+                             int top_k, int64_t* values, cudaStream_t st) {
+  SortFieldsValuesLaunch V{};
+  V.docs = docs; V.counts = counts; V.nq = n; V.top_k = top_k; V.doc_base = doc_base; V.n_fields = o->n_fields;
+  V.score_first = o->score_first ? 1 : 0; V.score_reverse = o->score_reverse; V.ranks = 1;
+  for (int i = 0; i < o->n_fields; ++i) V.f[i] = o->f[i];
+  V.perm = o->perm.p; V.scores = scores; V.out_values = values;
+  const int64_t m = (int64_t)n * top_k;
+  if (m <= 0) return NRTGPU_OK;
+  sort_fields_values_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(V);
+  NRT_CUDA_TRY(cudaGetLastError());
+  return NRTGPU_OK;
+}
+
 // Nested top hits of terms or filter aggregation `parent` (pass 2) over the batches bs[0 .. n_b) that counted into one set of tables
 // (a single image: one batch; a searcher: one per leaf). Each batch's probe launch runs again with a collector that only
-// appends make_key(score, global doc) of the docs of returned buckets (slot map nest_slot) to per-(query, slot) segments
-// sized by the bucket counts h_cnt [nq*size]; its totalHits / pruned / terminated go to scratch, and theta / slice lists /
-// queue heads are its own, already merged. Queries are taken in groups whose keys fit kNestedHitBudget; each group runs
-// every batch's launch into the same segments, then selects once. Scratch and results are bs[0]'s.
+// appends the key of each doc of a returned bucket (slot map nest_slot) to per-(query, slot) segments sized by the bucket
+// counts h_cnt [nq*size]: make_key(score, global doc), or for a sorted collector its Sort key over that leaf's order
+// (agg_nested_collect); its totalHits / pruned / terminated go to scratch, and theta / slice lists / queue heads are its
+// own, already merged. Queries are taken in groups whose keys fit kNestedHitBudget; each group runs every batch's launch
+// into the same segments, then selects once. Sorted keys of distinct leaves do not compare, so over several leaves a sorted
+// collector's segments are reset before each leaf's launch, the leaf selects its own top_hits into a packed sorted record
+// (one list per (query, slot)), and the leaves' records are merged as TopFieldDocs.merge does before start_hit is applied.
+// Scratch and results are bs[0]'s.
 static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t st, int parent, const std::vector<int32_t>& h_cnt,
                                  const nrtgpu_nested_result* nres) {
   nrtgpu_batch* b = bs[0];
@@ -1235,24 +1259,41 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
   for (size_t j = 0; j < b->cb.nested.size(); ++j)
     if (b->cb.nested[j].parent == parent && b->cb.nested[j].kind == NRTGPU_AGG_TOP_HITS) th.push_back(j);
   const int n_th = (int)th.size();
-  std::vector<size_t> out_base((size_t)n_th + 1, 0);
+  // the order of collector k on batch l (NULL: by score)
+  auto order_of = [&](int k, int l) -> const nrtgpu_sort_order* {
+    const nrtgpu_nested_sort& so = b->cb.nested_sorts[th[(size_t)k]];
+    return so.orders ? so.orders[l] : nullptr;
+  };
+  const bool merge = n_b > 1;   // several leaves: sorted collectors select per leaf, then merge
+  std::vector<size_t> out_base((size_t)n_th + 1, 0), val_base((size_t)n_th + 1, 0);
+  std::vector<long long> rec_q((size_t)n_th, 0);   // merge: bytes of a sorted collector's records per query of a group
   for (int k = 0; k < n_th; ++k) {
     const nrtgpu_nested_aggregation& n = b->cb.nested[th[(size_t)k]];
-    out_base[(size_t)k + 1] = out_base[(size_t)k] + (size_t)nq * size * (size_t)(n.top_hits - n.start_hit);
+    const size_t nw = (size_t)nq * size * (size_t)(n.top_hits - n.start_hit);
+    const nrtgpu_sort_order* o = order_of(k, 0);
+    out_base[(size_t)k + 1] = out_base[(size_t)k] + nw;
+    val_base[(size_t)k + 1] = val_base[(size_t)k] + (o ? nw * (size_t)o->n_fields : 0);
+    if (o && merge) rec_q[(size_t)k] = (long long)(n_b + 1) * size * ((long long)n.top_hits * (1 + 2 * o->n_fields) + 4) * 4;
   }
   int rc;
   if ((rc = b->nest_docs.alloc(out_base.back())) || (rc = b->nest_scores.alloc(out_base.back())) ||
+      (rc = b->nest_svals.alloc(std::max<size_t>(val_base.back(), 1))) ||
       (rc = b->nest_hcounts.alloc((size_t)n_th * nq * size)) || (rc = b->p2_total.alloc((size_t)nq)) || (rc = b->p2_flags.alloc(2 * (size_t)nq)))
     return rc;
   std::vector<long long> per_q((size_t)nq, 0);
   for (int q = 0; q < nq; ++q)
     for (int s = 0; s < size; ++s) per_q[(size_t)q] += (long long)n_th * h_cnt[(size_t)q * size + s];
+  long long rec_per_q = 0;
+  for (long long x : rec_q) rec_per_q += x;
   for (int q_lo = 0; q_lo < nq;) {
     if (per_q[(size_t)q_lo] > kNestedHitBudget)
       NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "nested top hits: the returned buckets of one query hold more than 2^26 hits");
     long long total = 0;
     int q_hi = q_lo;
-    while (q_hi < nq && total + per_q[(size_t)q_hi] <= kNestedHitBudget) total += per_q[(size_t)q_hi++];
+    // (the sorted records of a group stay under 512 MB too, unless one query needs more by itself)
+    while (q_hi < nq && total + per_q[(size_t)q_hi] <= kNestedHitBudget &&
+           (q_hi == q_lo || (q_hi - q_lo + 1) * rec_per_q <= kNestedHitBudget * 8))
+      total += per_q[(size_t)q_hi++];
     const int gq = q_hi - q_lo, gs = gq * size;
     std::vector<long long> off((size_t)n_th * (gs + 1));   // per collector: the segments of the group, laid out one after the other
     long long at = 0;
@@ -1264,41 +1305,95 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
     if ((rc = b->nest_off.upload_async(off.data(), off.size(), st)) || (rc = b->nest_fill.alloc((size_t)n_th * gs)) ||
         (rc = b->nest_keys.alloc((size_t)std::max(at, 1ll)))) return rc;
     NRT_CUDA_TRY(cudaMemsetAsync(b->nest_fill.p, 0, b->nest_fill.bytes(), st));
+    // merge: per sorted collector, n_b leaf records then the merged one (int32 words; every record starts 8-byte aligned)
+    std::vector<SortedRecordLayout> rl((size_t)n_th);
+    std::vector<size_t> rec_at((size_t)n_th + 1, 0);
+    int k_max = 1;
+    for (int k = 0; k < n_th; ++k) {
+      const nrtgpu_sort_order* o = order_of(k, 0);
+      rec_at[(size_t)k + 1] = rec_at[(size_t)k];
+      if (!o || !merge) continue;
+      const int K = b->cb.nested[th[(size_t)k]].top_hits;
+      rl[(size_t)k] = sorted_record_layout(gs, K, o->n_fields);
+      rec_at[(size_t)k + 1] += (size_t)(n_b + 1) * (size_t)rl[(size_t)k].words;
+      k_max = std::max(k_max, K);
+    }
+    if (rec_at.back() > 0) {
+      if ((rc = b->nest_rec.alloc(rec_at.back() / 2)) || (rc = b->nest_rscores.alloc((size_t)gs * k_max))) return rc;
+      NRT_CUDA_TRY(cudaMemsetAsync(b->nest_rec.p, 0, rec_at.back() * 4, st));
+    }
+    int32_t* rec = reinterpret_cast<int32_t*>(b->nest_rec.p);
     std::vector<AggLaunch> launches((size_t)n_b);   // uploaded asynchronously: kept until the group's synchronize
     for (int l = 0; l < n_b && at > 0; ++l) {
       nrtgpu_batch* x = bs[l];
-      if (x->plan.n_probe_simple + x->plan.n_probe_generic == 0) continue;
-      AggLaunch& A = launches[(size_t)l];
-      std::memset(&A, 0, sizeof(A));
-      A.n_aggs = 1;
-      A.a[0].kind = NRTGPU_AGG_TERMS; A.a[0].column = a.kind == NRTGPU_AGG_FILTER ? x->ix->n_columns : a.column;
-      A.a[0].value_type = a.value_type;
-      A.a[0].n_buckets = x->agg_tab.n_buckets[parent];
-      A.codes[0] = x->agg_codes[parent];   // the codes pass 1 counted through; counts stay NULL: the pass-1 tables are not touched
-      A.nested_begin[1] = n_th;
-      for (int k = 0; k < n_th; ++k) {
-        AggNestedDev& d = A.nested[k];
-        d.kind = NRTGPU_AGG_TOP_HITS; d.size = size; d.q_lo = q_lo; d.q_hi = q_hi; d.slot_of = b->nest_slot.p;
-        d.hit_off = b->nest_off.p + (size_t)k * (gs + 1); d.hit_fill = b->nest_fill.p + (size_t)k * gs; d.hit_keys = b->nest_keys.p;
-        d.doc_base = x->ix->doc_base;
+      if (merge)   // this leaf's sorted keys start from empty segments
+        for (int k = 0; k < n_th; ++k)
+          if (order_of(k, l)) NRT_CUDA_TRY(cudaMemsetAsync(b->nest_fill.p + (size_t)k * gs, 0, (size_t)gs * sizeof(unsigned int), st));
+      if (x->plan.n_probe_simple + x->plan.n_probe_generic > 0) {
+        AggLaunch& A = launches[(size_t)l];
+        std::memset(&A, 0, sizeof(A));
+        A.n_aggs = 1;
+        A.a[0].kind = NRTGPU_AGG_TERMS; A.a[0].column = a.kind == NRTGPU_AGG_FILTER ? x->ix->n_columns : a.column;
+        A.a[0].value_type = a.value_type;
+        A.a[0].n_buckets = x->agg_tab.n_buckets[parent];
+        A.codes[0] = x->agg_codes[parent];   // the codes pass 1 counted through; counts stay NULL: the pass-1 tables are not touched
+        A.nested_begin[1] = n_th;
+        for (int k = 0; k < n_th; ++k) {
+          AggNestedDev& d = A.nested[k];
+          d.kind = NRTGPU_AGG_TOP_HITS; d.size = size; d.q_lo = q_lo; d.q_hi = q_hi; d.slot_of = b->nest_slot.p;
+          d.hit_off = b->nest_off.p + (size_t)k * (gs + 1); d.hit_fill = b->nest_fill.p + (size_t)k * gs; d.hit_keys = b->nest_keys.p;
+          d.doc_base = x->ix->doc_base; d.score_key = 1;
+          if (const nrtgpu_sort_order* o = order_of(k, l)) { d.rank = o->rank.p; d.score_key = o->score_first; d.score_reverse = o->score_reverse; }
+        }
+        if ((rc = x->nest_launch.upload_async(&A, 1, st))) return rc;
+        NRT_CUDA_TRY(cudaMemsetAsync(x->theta.p, 0, x->theta.bytes(), st));
+        NRT_CUDA_TRY(cudaMemsetAsync(x->slice_cnt.p, 0, x->slice_cnt.bytes(), st));
+        NRT_CUDA_TRY(cudaMemsetAsync(x->work_counter.p, 0, x->work_counter.bytes(), st));
+        NRT_CUDA_TRY(cudaMemsetAsync(b->p2_total.p, 0, b->p2_total.bytes(), st));
+        NRT_CUDA_TRY(cudaMemsetAsync(b->p2_flags.p, 0, b->p2_flags.bytes(), st));
+        v3::ProbeLaunch P = probe_params(x);
+        P.total_hits = b->p2_total.p; P.pruned = b->p2_flags.p; P.terminated = b->p2_flags.p + nq;
+        P.deadline_ns = 0; P.terminate_after = 0;
+        P.aggs = x->nest_launch.p;
+        if ((rc = probe_launch(x, P, false, st))) return rc;
       }
-      if ((rc = x->nest_launch.upload_async(&A, 1, st))) return rc;
-      NRT_CUDA_TRY(cudaMemsetAsync(x->theta.p, 0, x->theta.bytes(), st));
-      NRT_CUDA_TRY(cudaMemsetAsync(x->slice_cnt.p, 0, x->slice_cnt.bytes(), st));
-      NRT_CUDA_TRY(cudaMemsetAsync(x->work_counter.p, 0, x->work_counter.bytes(), st));
-      NRT_CUDA_TRY(cudaMemsetAsync(b->p2_total.p, 0, b->p2_total.bytes(), st));
-      NRT_CUDA_TRY(cudaMemsetAsync(b->p2_flags.p, 0, b->p2_flags.bytes(), st));
-      v3::ProbeLaunch P = probe_params(x);
-      P.total_hits = b->p2_total.p; P.pruned = b->p2_flags.p; P.terminated = b->p2_flags.p + nq;
-      P.deadline_ns = 0; P.terminate_after = 0;
-      P.aggs = x->nest_launch.p;
-      if ((rc = probe_launch(x, P, false, st))) return rc;
+      for (int k = 0; k < n_th && merge; ++k) {   // this leaf's best top_hits of each list, by its order, into its record
+        const nrtgpu_sort_order* o = order_of(k, l);
+        if (!o) continue;
+        const SortedRecordLayout& L = rl[(size_t)k];
+        int32_t* r = rec + rec_at[(size_t)k] + (size_t)l * L.words;
+        NestedHitsLaunch H;
+        H.hit_keys = b->nest_keys.p; H.hit_off = b->nest_off.p + (size_t)k * (gs + 1); H.hit_fill = b->nest_fill.p + (size_t)k * gs;
+        H.q_lo = 0; H.size = size; H.top_hits = b->cb.nested[th[(size_t)k]].top_hits; H.start_hit = 0; H.doc_base = x->ix->doc_base;
+        H.out_docs = r; H.out_scores = b->nest_rscores.p; H.out_counts = r + L.counts;
+        nested_top_hits_kernel<<<gs, 256, 0, st>>>(H);
+        NRT_CUDA_TRY(cudaGetLastError());
+        if ((rc = sorted_hit_values(o, x->ix->doc_base, r, r + L.counts, b->nest_rscores.p, gs, H.top_hits,
+                                    reinterpret_cast<int64_t*>(r + L.values), st))) return rc;
+      }
     }
     for (int k = 0; k < n_th; ++k) {
       const nrtgpu_nested_aggregation& n = b->cb.nested[th[(size_t)k]];
+      const nrtgpu_sort_order* o = order_of(k, 0);
+      if (o && merge) {   // TopFieldDocs.merge of the leaves' lists, then positions [start_hit, top_hits)
+        const SortedRecordLayout& L = rl[(size_t)k];
+        int32_t* r = rec + rec_at[(size_t)k];
+        if ((rc = nrtgpu_merge_sorted_packed(b->ix->ctx, o->spec, o->n_fields, n_b, gs, n.top_hits, r, r + (size_t)n_b * L.words, st)))
+          return rc;
+        SortedHitsOutLaunch S;
+        S.record = r + (size_t)n_b * L.words; S.L = L; S.n = gs; S.top_k = n.top_hits; S.n_fields = o->n_fields;
+        S.start_hit = n.start_hit; S.w = n.top_hits - n.start_hit; S.q_lo = q_lo; S.size = size;
+        S.out_docs = b->nest_docs.p + out_base[(size_t)k]; S.out_scores = b->nest_scores.p + out_base[(size_t)k];
+        S.out_counts = b->nest_hcounts.p + (size_t)k * nq * size; S.out_values = b->nest_svals.p + val_base[(size_t)k];
+        const int m = gs * S.w;
+        sorted_hits_out_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(S);
+        NRT_CUDA_TRY(cudaGetLastError());
+        continue;
+      }
       NestedHitsLaunch H;
       H.hit_keys = b->nest_keys.p; H.hit_off = b->nest_off.p + (size_t)k * (gs + 1); H.hit_fill = b->nest_fill.p + (size_t)k * gs;
-      H.q_lo = q_lo; H.size = size; H.top_hits = n.top_hits; H.start_hit = n.start_hit; H.doc_base = 0;   // keys hold global docs
+      H.q_lo = q_lo; H.size = size; H.top_hits = n.top_hits; H.start_hit = n.start_hit;
+      H.doc_base = o ? b->ix->doc_base : 0;   // score keys hold global docs; Sort keys the image's ranks
       H.out_docs = b->nest_docs.p + out_base[(size_t)k]; H.out_scores = b->nest_scores.p + out_base[(size_t)k];
       H.out_counts = b->nest_hcounts.p + (size_t)k * nq * size;
       nested_top_hits_kernel<<<gs, 256, 0, st>>>(H);
@@ -1311,9 +1406,17 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
     const size_t j = th[(size_t)k];
     const nrtgpu_nested_result& r = nres[j];
     const size_t nw = out_base[(size_t)k + 1] - out_base[(size_t)k];
+    const nrtgpu_sort_order* o = order_of(k, 0);
+    if (o && !merge && (rc = sorted_hit_values(o, b->ix->doc_base, b->nest_docs.p + out_base[(size_t)k], b->nest_hcounts.p + (size_t)k * nq * size,
+                                               b->nest_scores.p + out_base[(size_t)k], nq * size,
+                                               b->cb.nested[j].top_hits - b->cb.nested[j].start_hit, b->nest_svals.p + val_base[(size_t)k], st)))
+      return rc;
     if (r.hit_docs) NRT_CUDA_TRY(cudaMemcpyAsync(r.hit_docs, b->nest_docs.p + out_base[(size_t)k], nw * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     if (r.hit_scores) NRT_CUDA_TRY(cudaMemcpyAsync(r.hit_scores, b->nest_scores.p + out_base[(size_t)k], nw * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (r.hit_counts) NRT_CUDA_TRY(cudaMemcpyAsync(r.hit_counts, b->nest_hcounts.p + (size_t)k * nq * size, (size_t)nq * size * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (o && b->cb.nested_sorts[j].values)
+      NRT_CUDA_TRY(cudaMemcpyAsync(b->cb.nested_sorts[j].values, b->nest_svals.p + val_base[(size_t)k],
+                                   (val_base[(size_t)k + 1] - val_base[(size_t)k]) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     if (r.hit_total) for (size_t x = 0; x < (size_t)nq * size; ++x) r.hit_total[x] = h_cnt[x];   // TopDocs.totalHits: the bucket's count
   }
   NRT_CUDA_TRY(cudaStreamSynchronize(st));
@@ -1813,17 +1916,38 @@ int nrtgpu_search_bool_aggs_nested(nrtgpu_index* ix, const nrtgpu_clause* clause
 // the request of the additional-collector entry points (single image and searcher): exhaustive, with the collectors
 static int aggs_request(BatchRequest* r, const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
                         const nrtgpu_nested_aggregation* nested, int32_t n_nested, const nrtgpu_nested_result* nested_results,
-                        const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses,
-                        const nrtgpu_query* filter_queries, int32_t n_filter_queries) {
+                        const nrtgpu_nested_sort* nested_sorts, const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses,
+                        int32_t n_filter_clauses, const nrtgpu_query* filter_queries, int32_t n_filter_queries) {
   if (n_aggs <= 0 || !aggs || !results) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_bool_aggs: no aggregations");
   if (n_nested < 0 || (n_nested > 0 && (!nested || !nested_results))) NRT_FAIL(NRTGPU_ERR_INVALID, "nested aggregations: NULL argument");
   if (n_filter_clauses < 0 || n_filter_queries < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "filter aggregation: negative filter query count");
   r->total_hits_threshold = INT32_MAX;
   r->aggs = aggs; r->n_aggs = n_aggs;
-  if (n_nested > 0) { r->nested = nested; r->n_nested = n_nested; }
+  if (n_nested > 0) { r->nested = nested; r->n_nested = n_nested; r->nested_sorts = nested_sorts; }
   r->agg_filters = agg_filters;
   r->filter_clauses = filter_clauses; r->n_filter_clauses = n_filter_clauses;
   r->filter_queries = filter_queries; r->n_filter_queries = n_filter_queries;
+  return NRTGPU_OK;
+}
+
+static bool same_sort(const nrtgpu_sort_order* a, const nrtgpu_sort_order* b);
+
+// the orders of the sorted top hits of a request (nested_sorts) on the images leaves[0 .. n_leaves): one per leaf, made on
+// it, all of one Sort. An order on another kind of record is the compiler's refusal.
+static int check_nested_sorts(const char* fn, const BatchRequest& r, nrtgpu_index* const* leaves, int n_leaves) {
+  if (!r.nested_sorts) return NRTGPU_OK;
+  const std::string f(fn);
+  for (int j = 0; j < r.n_nested; ++j) {
+    const nrtgpu_sort_order* const* orders = r.nested_sorts[j].orders;
+    if (!orders || r.nested[j].kind != NRTGPU_AGG_TOP_HITS) continue;
+    for (int l = 0; l < n_leaves; ++l) {
+      if (!orders[l]) NRT_FAIL(NRTGPU_ERR_INVALID, f + ": NULL sort order");
+      if (orders[l]->ix != leaves[l])
+        NRT_FAIL(NRTGPU_ERR_INVALID, f + (n_leaves == 1 ? ": the sort order was made on another index"
+                                                         : ": the sort order of leaf " + std::to_string(l) + " was made on another index"));
+      if (!same_sort(orders[l], orders[0])) NRT_FAIL(NRTGPU_ERR_INVALID, f + ": the leaves' sort orders are of different Sorts");
+    }
+  }
   return NRTGPU_OK;
 }
 
@@ -1835,10 +1959,24 @@ int nrtgpu_search_bool_aggs_filtered(nrtgpu_index* ix, const nrtgpu_clause* clau
                                      const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses,
                                      const nrtgpu_query* filter_queries, int32_t n_filter_queries, void* stream,
                                      int32_t* out_docs, float* out_scores, int32_t* out_counts, int64_t* out_total_hits) {
+  return nrtgpu_search_bool_aggs_sorted_hits(ix, clauses, n_clauses, queries, nq, top_k, flags, aggs, n_aggs, results, nested, n_nested,
+                                             nested_results, nullptr, agg_filters, filter_clauses, n_filter_clauses, filter_queries,
+                                             n_filter_queries, stream, out_docs, out_scores, out_counts, out_total_hits);
+}
+
+int nrtgpu_search_bool_aggs_sorted_hits(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                        const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                        const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                                        const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                        const nrtgpu_nested_result* nested_results, const nrtgpu_nested_sort* nested_sorts,
+                                        const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses,
+                                        int32_t n_filter_clauses, const nrtgpu_query* filter_queries, int32_t n_filter_queries,
+                                        void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
+                                        int64_t* out_total_hits) {
   BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
-  int rc = aggs_request(&r, aggs, n_aggs, results, nested, n_nested, nested_results, agg_filters, filter_clauses, n_filter_clauses,
-                        filter_queries, n_filter_queries);
-  if (rc) return rc;
+  int rc = aggs_request(&r, aggs, n_aggs, results, nested, n_nested, nested_results, nested_sorts, agg_filters, filter_clauses,
+                        n_filter_clauses, filter_queries, n_filter_queries);
+  if (rc || (rc = check_nested_sorts("nrtgpu_search_bool_aggs_sorted_hits", r, &ix, 1))) return rc;
   SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.aggs = results;
   o.nested = n_nested > 0 ? nested_results : nullptr;
   return search_bool_impl(ix, r, nullptr, stream, o);
@@ -2732,9 +2870,6 @@ int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_cla
                                                    out_scores, out_counts, out_total_hits);
 }
 
-// Aggregations over the leaves: every leaf's batch counts into one set of reader-wide tables through its codes renumbered
-// to the column's reader-wide dictionary (searcher_dict) and tests its own image's filter rows; the selection and the
-// nested top hits then run once on them
 int nrtgpu_searcher_search_bool_aggs_filtered(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
                                               const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
                                               const nrtgpu_aggregation* aggs, int32_t n_aggs,
@@ -2745,10 +2880,31 @@ int nrtgpu_searcher_search_bool_aggs_filtered(nrtgpu_searcher* s, const nrtgpu_c
                                               int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores,
                                               int32_t* out_counts, int64_t* out_total_hits) {
   if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_bool_aggs_filtered: NULL searcher");
+  return nrtgpu_searcher_search_bool_aggs_sorted_hits(s, clauses, n_clauses, queries, nq, top_k, flags, aggs, n_aggs, results, nested,
+                                                      n_nested, nested_results, nullptr, agg_filters, filter_clauses, n_filter_clauses,
+                                                      filter_queries, n_filter_queries, stream, out_docs, out_scores, out_counts,
+                                                      out_total_hits);
+}
+
+// Aggregations over the leaves: every leaf's batch counts into one set of reader-wide tables through its codes renumbered
+// to the column's reader-wide dictionary (searcher_dict) and tests its own image's filter rows; the selection and the
+// nested top hits then run once on them (sorted top hits: per leaf, then merged; batch_nested_top_hits)
+int nrtgpu_searcher_search_bool_aggs_sorted_hits(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
+                                                 const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                                                 const nrtgpu_aggregation* aggs, int32_t n_aggs,
+                                                 const nrtgpu_aggregation_result* results,
+                                                 const nrtgpu_nested_aggregation* nested, int32_t n_nested,
+                                                 const nrtgpu_nested_result* nested_results, const nrtgpu_nested_sort* nested_sorts,
+                                                 const nrtgpu_agg_filter* agg_filters, const nrtgpu_clause* filter_clauses,
+                                                 int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
+                                                 int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores,
+                                                 int32_t* out_counts, int64_t* out_total_hits) {
+  if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_bool_aggs_sorted_hits: NULL searcher");
   BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
-  int rc = aggs_request(&r, aggs, n_aggs, results, nested, n_nested, nested_results, agg_filters, filter_clauses, n_filter_clauses,
-                        filter_queries, n_filter_queries);
-  if (rc) return rc;
+  int rc = aggs_request(&r, aggs, n_aggs, results, nested, n_nested, nested_results, nested_sorts, agg_filters, filter_clauses,
+                        n_filter_clauses, filter_queries, n_filter_queries);
+  if (rc || (rc = check_nested_sorts("nrtgpu_searcher_search_bool_aggs_sorted_hits", r, s->leaves.data(), (int)s->leaves.size())))
+    return rc;
   NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> g(s->mu);

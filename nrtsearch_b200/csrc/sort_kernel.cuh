@@ -266,10 +266,10 @@ __global__ void sort_fields_after_kernel(SortFieldsAfterLaunch S) {
   S.queries[q].after_key = key;
 }
 
-// FieldDoc.fields of the final hits ([nq][top_k][n_fields]); score-first orders: the merged "doc" is a rank, mapped back
-// to the doc through perm, and the score is recovered from the key's score word
+// FieldDoc.fields of the final hits ([nq][top_k][n_fields]); score-first orders (and sorted nested top hits, `ranks`): the
+// "doc" is a rank + doc_base, mapped back to the doc through perm; the score is recovered from the key's score word
 struct SortFieldsValuesLaunch {
-  int32_t* docs; const int32_t* counts; int32_t nq, top_k, doc_base, n_fields, score_first, score_reverse;
+  int32_t* docs; const int32_t* counts; int32_t nq, top_k, doc_base, n_fields, score_first, score_reverse, ranks;
   SortFieldDev f[kMaxSortFields];   // every field of the sort (a SCORE entry takes the hit's score)
   const int32_t* perm;
   float* scores; int64_t* out_values;
@@ -284,11 +284,11 @@ __global__ void sort_fields_values_kernel(SortFieldsValuesLaunch S) {
   if (r >= S.counts[q]) { for (int j = 0; j < S.n_fields; ++j) out[j] = 0; return; }
   int32_t d = S.docs[i] - S.doc_base;
   float score = 0.0f;
-  if (S.score_first) {
+  if (S.score_first || S.ranks) {
     d = S.perm[d - 1];
     S.docs[i] = d + S.doc_base;
-    score = S.score_reverse ? ordered_to_float(~float_to_ordered(key_score)) : key_score;
   }
+  if (S.score_first) score = S.score_reverse ? ordered_to_float(~float_to_ordered(key_score)) : key_score;
   for (int j = 0; j < S.n_fields; ++j)
     out[j] = S.f[j].kind == NRTGPU_SORT_SCORE ? (int64_t)__float_as_uint(score) : sort_field_value(S.f[j], d, S.doc_base);
 }
@@ -405,6 +405,28 @@ __global__ void __launch_bounds__(kSortMergeThreads) sort_merge_kernel(SortMerge
       }
     }
   }
+}
+
+// positions [start_hit, start_hit + w) of each list of a merged sorted record ([n][top_k], the leaves' sorted nested top
+// hits of one pass-2 group, list g = (query q_lo + g / size, slot g % size)) -> the caller's layout [nq][size][w]: docs,
+// FieldDoc values, NaN scores (TopHitsCollectorManager.reduce: Hit.score = Double.NaN) and the counts past start_hit
+struct SortedHitsOutLaunch {
+  const int32_t* record; SortedRecordLayout L;
+  int32_t n, top_k, n_fields, start_hit, w, q_lo, size;
+  int32_t* out_docs; float* out_scores; int32_t* out_counts; int64_t* out_values;
+};
+__global__ void sorted_hits_out_kernel(SortedHitsOutLaunch S) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= S.n * S.w) return;
+  const int g = i / S.w, r = i % S.w, p = S.start_hit + r;
+  const int cnt = S.record[S.L.counts + g];
+  const size_t qs = (size_t)(S.q_lo + g / S.size) * S.size + g % S.size;
+  const bool hit = p < cnt;
+  S.out_docs[qs * S.w + r] = hit ? S.record[(size_t)g * S.top_k + p] : 0;
+  S.out_scores[qs * S.w + r] = __int_as_float(0x7fc00000);
+  const int64_t* v = (const int64_t*)(S.record + S.L.values) + ((size_t)g * S.top_k + p) * S.n_fields;
+  for (int j = 0; j < S.n_fields; ++j) S.out_values[(qs * S.w + r) * S.n_fields + j] = hit ? v[j] : 0;
+  if (r == 0) S.out_counts[qs] = max(0, cnt - S.start_hit);
 }
 
 // a leaf's sorted or score record after its run: a timed-out query is partial (hit_timeout, relation GTE), and the

@@ -23,6 +23,7 @@ import numpy as np
 
 from . import _native
 from ._native import (AggFilter as CAggFilter, Aggregation as CAgg, AggregationResult as CAggResult, NestedAggregation as CNested,
+                      NestedSort as CNestedSort,
                       NestedResult as CNestedResult, Clause, CollectionTimeoutException, NrtGpuError,
                       NrtGpuUnsupported, Query as CQuery, SearchLimits, Sort as CSort, check)
 from .index import HostShard, PinnedDesc
@@ -235,10 +236,18 @@ class TermsCollector:
 
 @dataclass(frozen=True)
 class TopHitsCollector:
-    """TopHitsCollector as a nested collector of a terms bucket (TopHitsCollectorManager): the bucket's hits by score
-    descending, then doc ascending, positions [start_hit, top_hits)."""
+    """TopHitsCollector (TopHitsCollectorManager): a bucket's hits by score descending, then doc ascending, positions
+    [start_hit, top_hits). sort (querySort): a SortType or a sequence of up to 8, as SortFieldCollector.sort; the hits are
+    then in that Sort's order, ties by doc, their scores NaN, and the result gains "sort_values" (FieldDoc.fields of every
+    hit). Nested in a terms or filter collector it works per bucket; in `additional` (top level) it sees every doc the
+    query collects: its result is {"docs", "scores" [nq, top_hits - start_hit], "counts", "total_hits" [nq] (the query's
+    exact totalHits)[, "sort_values" [nq, top_hits - start_hit, n_fields]]}."""
     top_hits: int
     start_hit: int = 0
+    sort: object = None
+
+    def sort_fields(self) -> List[SortType]:
+        return [self.sort] if isinstance(self.sort, SortType) else list(self.sort)
 
 
 @dataclass(frozen=True)
@@ -285,7 +294,8 @@ class FilterCollector:
     MatchAllDocsQuery; only matching counts) or a ValueSetFilter. nested: (name, TermsCollector | MinCollector | MaxCollector |
     SumCollector | TopHitsCollector | FilterCollector) pairs, at least one. Its result is {"doc_count": int32 [nq], name:
     the nested collector's result}: a terms or filter collector's own result, float64 [nq] (min / max / sum), or {"docs",
-    "scores" [nq, top_hits - start_hit], "counts", "total_hits" [nq]} (top hits)."""
+    "scores" [nq, top_hits - start_hit], "counts", "total_hits" [nq][, "sort_values" [nq, top_hits - start_hit, n_fields]]}
+    (top hits)."""
     filter: object
     nested: tuple = ()
 
@@ -656,15 +666,19 @@ def _collector_records(nq: int, additional: Sequence[object]):
 
 
 class _FilteredRecords:
-    """The records of a batch whose additional collectors hold filter collectors (nrtgpu_search_bool_aggs_filtered): every
-    terms, min / max / sum and filter collector becomes an nrtgpu_aggregation, a terms or filter collector under a filter
-    names it by filter_agg (parents before children), a min / max / sum / top hits under a filter is a nested collector of
-    it, and each filter gets its nrtgpu_agg_filter record (filter queries compiled by compile_queries). outs: the result
-    objects the call fills, one per top-level collector; args: the records in the entry point's order."""
+    """The records of a batch whose additional collectors hold filter collectors or top hits that need more than a terms
+    bucket by score (nrtgpu_search_bool_aggs_sorted_hits): every terms, min / max / sum and filter collector becomes an
+    nrtgpu_aggregation, a terms or filter collector under a filter names it by filter_agg (parents before children), a min /
+    max / sum / top hits under a filter is a nested collector of it, and each filter gets its nrtgpu_agg_filter record
+    (filter queries compiled by compile_queries). A top-level TopHitsCollector is the nested top hits of an implicit
+    FilterCollector(MatchAllDocsQuery()): one filter row and 4 B of codes per doc on the device. A sorted top hits gets its
+    nrtgpu_nested_sort, the orders of its Sort from orders_of(fields) (one per image). outs: the result objects the call
+    fills, one per top-level collector; args: the records in the order of nrtgpu_search_bool_aggs_filtered, sorted_args in
+    that of nrtgpu_search_bool_aggs_sorted_hits."""
 
-    def __init__(self, nq: int, additional: Sequence[object]):
-        self.nq = nq
-        self.aggs, self.res, self.filters, self.nested, self.nested_res = [], [], [], [], []
+    def __init__(self, nq: int, additional: Sequence[object], orders_of=None):
+        self.nq, self.orders_of = nq, orders_of
+        self.aggs, self.res, self.filters, self.nested, self.nested_res, self.sorts = [], [], [], [], [], []
         self.filter_queries, self.keep = [], []
         self.outs = [self._add(a, 0) for a in additional]
         n = len(self.aggs)
@@ -672,8 +686,13 @@ class _FilteredRecords:
         filt = (CAggFilter * n)(*self.filters)
         narr = (CNested * len(self.nested))(*self.nested) if self.nested else None
         nres = (CNestedResult * len(self.nested))(*self.nested_res) if self.nested else None
+        nsort = (CNestedSort * len(self.nested))(*self.sorts) if any(x.orders for x in self.sorts) else None
         fcarr, fncl, fqarr, fnq = compile_queries(self.filter_queries) if self.filter_queries else (None, 0, None, 0)
         self.args = (aggs, n, res, narr, len(self.nested), nres, filt, fcarr, fncl, fqarr, fnq)
+        self.sorted_args = self.args[:6] + (nsort,) + self.args[6:]
+
+    def _top_hits(self, c: "TopHitsCollector", parent: int, shape: tuple, orders_parent: int = 0) -> dict:
+        return _top_hits_spec(c, parent, shape, self.nested, self.nested_res, orders_parent, self.sorts, self.orders_of, self.keep)
 
     def _add(self, a, filter_agg: int):
         nq, i = self.nq, len(self.aggs)
@@ -685,8 +704,14 @@ class _FilteredRecords:
             self.res.append(CAggResult(None, o["keys"].ctypes.data, o["counts"].ctypes.data, o["n"].ctypes.data,
                                        o["total_buckets"].ctypes.data, o["other_counts"].ctypes.data))
             if a.nested or a.order_by is not None:
-                o["nested"] = _nested_specs(i, a, nq, self.nested, self.nested_res)
+                o["nested"] = _nested_specs(i, a, nq, self.nested, self.nested_res, self.sorts, self.orders_of, self.keep)
             return o
+        if isinstance(a, TopHitsCollector):   # top level: the nested top hits of FilterCollector(MatchAllDocsQuery())
+            self.aggs.append(CAgg(6, 0, 0, 0, 0, 0))
+            self.res.append(CAggResult(None, None, None, None, None, None))
+            self.filters[i] = CAggFilter(1, len(self.filter_queries), 0, 0, None)
+            self.filter_queries.append(MatchAllDocsQuery())
+            return self._top_hits(a, i, (nq,))
         if isinstance(a, FilterCollector):
             self.aggs.append(CAgg(6, 0, 0, 0, 0, filter_agg))
             o = {"doc_count": np.zeros(nq, np.int32)}
@@ -706,18 +731,13 @@ class _FilteredRecords:
                 if isinstance(c, (TermsCollector, FilterCollector)):
                     o[name] = self._add(c, i + 1)
                 elif isinstance(c, TopHitsCollector):
-                    w = max(c.top_hits - c.start_hit, 0)
-                    r = {"docs": np.zeros((nq, w), np.int32), "scores": np.zeros((nq, w), np.float32),
-                         "counts": np.zeros(nq, np.int32), "total_hits": np.zeros(nq, np.int64)}
-                    self.nested.append(CNested(i, 5, 0, 0, c.top_hits, c.start_hit, 0, 0))
-                    self.nested_res.append(CNestedResult(None, r["docs"].ctypes.data, r["scores"].ctypes.data,
-                                                         r["counts"].ctypes.data, r["total_hits"].ctypes.data))
-                    o[name] = r
+                    o[name] = self._top_hits(c, i, (nq,))
                 elif isinstance(c, (MinCollector, MaxCollector, SumCollector)):
                     kind = 2 if isinstance(c, MinCollector) else 3 if isinstance(c, MaxCollector) else 4
                     r = np.zeros(nq, np.float64)
                     self.nested.append(CNested(i, kind, c.column, _VALUE_TYPE[c.field_type], 0, 0, 0, 0))
                     self.nested_res.append(CNestedResult(r.ctypes.data, None, None, None, None))
+                    self.sorts.append(CNestedSort())
                     o[name] = r
                 else:
                     raise ValueError(f"nested collector {name!r}: {type(c).__name__} is not on the GPU path")
@@ -730,12 +750,42 @@ class _FilteredRecords:
 
 
 def _has_filter(additional: Sequence[object]) -> bool:
-    return any(isinstance(a, FilterCollector) for a in additional)
+    """whether the request takes the filtered records (_FilteredRecords): a filter collector, a top-level top hits, or a
+    top hits with a Sort anywhere"""
+    def sorted_hits(c) -> bool:
+        if isinstance(c, TopHitsCollector):
+            return c.sort is not None
+        return isinstance(c, (TermsCollector, FilterCollector)) and any(sorted_hits(x) for _, x in c.nested)
+    return any(isinstance(a, (FilterCollector, TopHitsCollector)) or sorted_hits(a) for a in additional)
 
 
-def _nested_specs(parent: int, a: TermsCollector, nq: int, nested: list, nested_res: list) -> dict:
+def _top_hits_spec(c: TopHitsCollector, parent: int, shape: tuple, nested: list, nested_res: list, orders_parent: int = 0,
+                   sorts: Optional[list] = None, orders_of=None, keep: Optional[list] = None) -> dict:
+    """the nrtgpu_nested_aggregation record and result buffers of top hits collector c under aggregation `parent` (appended
+    to nested / nested_res; its nrtgpu_nested_sort to sorts, when the call takes them); shape: the result's leading
+    dimensions ([nq, size] under a terms collector, [nq] else); returns the result dict they fill"""
+    w = max(c.top_hits - c.start_hit, 0)
+    r = {"docs": np.zeros(shape + (w,), np.int32), "scores": np.zeros(shape + (w,), np.float32),
+         "counts": np.zeros(shape, np.int32), "total_hits": np.zeros(shape, np.int64)}
+    nested.append(CNested(parent, 5, 0, 0, c.top_hits, c.start_hit, orders_parent, 0))
+    nested_res.append(CNestedResult(None, r["docs"].ctypes.data, r["scores"].ctypes.data, r["counts"].ctypes.data,
+                                    r["total_hits"].ctypes.data))
+    ns = CNestedSort()
+    if c.sort is not None:
+        fields = c.sort_fields()
+        orders = orders_of(fields)
+        keep.append(orders)
+        r["sort_values"] = np.zeros(shape + (w, len(fields)), np.int64)
+        ns = CNestedSort(C.cast(orders, C.c_void_p), r["sort_values"].ctypes.data)
+    if sorts is not None:
+        sorts.append(ns)
+    return r
+
+
+def _nested_specs(parent: int, a: TermsCollector, nq: int, nested: list, nested_res: list, sorts: Optional[list] = None,
+                  orders_of=None, keep: Optional[list] = None) -> dict:
     """the nrtgpu_nested_aggregation records and result buffers of terms collector `parent` (appended to nested /
-    nested_res); returns the result dict they fill"""
+    nested_res, and their nrtgpu_nested_sort to sorts when the call takes them); returns the result dict they fill"""
     names = [name for name, _ in a.nested]
     if len(set(names)) != len(names):
         raise ValueError("nested collector names must be unique")
@@ -744,17 +794,14 @@ def _nested_specs(parent: int, a: TermsCollector, nq: int, nested: list, nested_
     o = {}
     for name, c in a.nested:
         if isinstance(c, TopHitsCollector):
-            w = max(c.top_hits - c.start_hit, 0)
-            r = {"docs": np.zeros((nq, a.size, w), np.int32), "scores": np.zeros((nq, a.size, w), np.float32),
-                 "counts": np.zeros((nq, a.size), np.int32), "total_hits": np.zeros((nq, a.size), np.int64)}
-            nested.append(CNested(parent, 5, 0, 0, c.top_hits, c.start_hit, 1 if name == a.order_by else 0, 0))
-            nested_res.append(CNestedResult(None, r["docs"].ctypes.data, r["scores"].ctypes.data, r["counts"].ctypes.data,
-                                            r["total_hits"].ctypes.data))
+            r = _top_hits_spec(c, parent, (nq, a.size), nested, nested_res, 1 if name == a.order_by else 0, sorts, orders_of, keep)
         elif isinstance(c, (MinCollector, MaxCollector, SumCollector)):
             kind = 2 if isinstance(c, MinCollector) else 3 if isinstance(c, MaxCollector) else 4
             r = np.zeros((nq, a.size), np.float64)
             nested.append(CNested(parent, kind, c.column, _VALUE_TYPE[c.field_type], 0, 0, 1 if name == a.order_by else 0, 0))
             nested_res.append(CNestedResult(r.ctypes.data, None, None, None, None))
+            if sorts is not None:
+                sorts.append(CNestedSort())
         else:
             raise ValueError(f"nested collector {name!r}: {type(c).__name__} is not on the GPU path")
         o[name] = r
@@ -899,17 +946,18 @@ class GpuIndexSearcher:
         """IndexSearcher.search with additional collectors (SearchCollectorManager fan-out): returns (BatchResult, results)
         where results[i] is a float64 [nq] array (min / max / sum) or a dict of bucket arrays (terms). A terms collector with
         nested collectors adds "nested": {name: float64 [nq, size] (min / max / sum) or {"docs", "scores" [nq, size,
-        top_hits - start_hit], "counts", "total_hits" [nq, size]} (top hits)}, per returned bucket. A FilterCollector's result
-        is the dict its docstring describes (nrtgpu_search_bool_aggs_filtered)."""
+        top_hits - start_hit], "counts", "total_hits" [nq, size][, "sort_values" [nq, size, top_hits - start_hit, n_fields]]}
+        (top hits)}, per returned bucket. A FilterCollector's and a top-level TopHitsCollector's results are the dicts their
+        docstrings describe (nrtgpu_search_bool_aggs_sorted_hits)."""
         carr, ncl, qarr, nq = compile_queries(queries)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
         hits = (out.docs.ctypes.data, out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data)
-        if _has_filter(additional):   # filter collectors: the flattened records of _FilteredRecords
-            fr = _FilteredRecords(nq, additional)
-            check(self._lib.nrtgpu_search_bool_aggs_filtered(self.index.handle, carr, ncl, qarr, nq, k, 0, *fr.args,
-                                                             C.c_void_p(stream), *hits))
+        if _has_filter(additional):   # filter collectors, top-level or sorted top hits: the records of _FilteredRecords
+            fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * 1)(self.index.sort_order(fields, stream).value))
+            check(self._lib.nrtgpu_search_bool_aggs_sorted_hits(self.index.handle, carr, ncl, qarr, nq, k, 0, *fr.sorted_args,
+                                                                C.c_void_p(stream), *hits))
             return out, fr.outs
         aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         if n_nested:
@@ -1126,10 +1174,12 @@ class GpuLeafSearcher:
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
         if _has_filter(additional):
-            fr = _FilteredRecords(nq, additional)
-            check(self._lib.nrtgpu_searcher_search_bool_aggs_filtered(self.handle, carr, ncl, qarr, nq, k, 0, *fr.args,
-                                                                      C.c_void_p(stream), out.docs.ctypes.data, out.scores.ctypes.data,
-                                                                      out.counts.ctypes.data, out.total_hits.ctypes.data))
+            fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * len(self.leaves))(
+                *[l.sort_order(fields, stream).value for l in self.leaves]))
+            check(self._lib.nrtgpu_searcher_search_bool_aggs_sorted_hits(self.handle, carr, ncl, qarr, nq, k, 0, *fr.sorted_args,
+                                                                         C.c_void_p(stream), out.docs.ctypes.data,
+                                                                         out.scores.ctypes.data, out.counts.ctypes.data,
+                                                                         out.total_hits.ctypes.data))
             return out, fr.outs
         aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         check(self._lib.nrtgpu_searcher_search_bool_aggs_nested(self.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
