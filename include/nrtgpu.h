@@ -541,6 +541,26 @@ int nrtgpu_search_bool_aggs_sorted_hits(nrtgpu_index* ix, const nrtgpu_clause* c
                                         int32_t n_filter_clauses, const nrtgpu_query* filter_queries, int32_t n_filter_queries,
                                         void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
                                         int64_t* out_total_hits);
+/* nrtgpu_search_tree_aggs: nrtgpu_search_bool_aggs_sorted_hits for the queries of nrtgpu_search_tree_phrases ("deep dish
+ * pizza" as a match_phrase or a multi_match, by category, plus the 3 best per category). The batch takes the tree and phrase
+ * arguments of nrtgpu_search_tree_phrases (n_nodes / n_phrases may be 0; nodes / phrases may then be NULL) and every
+ * collector argument of nrtgpu_search_bool_aggs_sorted_hits, with its meaning and result layout. A batch holding a nested
+ * query or a phrase, or a flat batch of more than 4 term clauses or top_k > 512, runs on the window engine
+ * (bool_window_kernel), which hands every matching doc and its score to the collectors, and runs again for the nested top
+ * hits; any other flat batch runs on the probe kernel exactly as nrtgpu_search_bool_aggs_sorted_hits runs it. The page and
+ * totalHits are those of nrtgpu_search_tree_phrases at totalHitsThreshold = INT32_MAX (totalHits exact).
+ *   Every refusal of nrtgpu_search_tree_phrases and of nrtgpu_search_bool_aggs_sorted_hits applies with its code and message,
+ *   but for "aggregations over a query tree" and "aggregations: more than 4 term clauses or top_k > 512", which this call
+ *   accepts. A refused call writes no output. */
+int nrtgpu_search_tree_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes, int32_t n_nodes,
+                            const nrtgpu_phrase* phrases, int32_t n_phrases, const nrtgpu_phrase_term* phrase_terms,
+                            int32_t n_phrase_terms, const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                            const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                            const nrtgpu_nested_aggregation* nested, int32_t n_nested, const nrtgpu_nested_result* nested_results,
+                            const nrtgpu_nested_sort* nested_sorts, const nrtgpu_agg_filter* agg_filters,
+                            const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
+                            int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
+                            int64_t* out_total_hits);
 
 /* QueryRescorer second pass (QueryRescore.java:39-57 -> Lucene QueryRescorer.rescore): query q of the batch evaluated on
  * ITS OWN hit list docs[q][0..counts[q]) (global doc ids): out_matches / out_scores [nq*n_hits]. */
@@ -803,6 +823,19 @@ int nrtgpu_searcher_search_bool_aggs_sorted_hits(nrtgpu_searcher* s, const nrtgp
                                                  int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
                                                  int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores,
                                                  int32_t* out_counts, int64_t* out_total_hits);
+/* nrtgpu_searcher_search_tree_aggs: nrtgpu_search_tree_aggs over the leaves, with the rules of
+ * nrtgpu_searcher_search_bool_aggs_sorted_hits (reader-wide tables and dictionaries, one order per leaf, sorted top hits
+ * merged as TopFieldDocs.merge does, the page by TopDocs.merge). Every leaf runs the batch on the same engine. */
+int nrtgpu_searcher_search_tree_aggs(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                                     int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                                     const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                                     int32_t nq, int32_t top_k, int32_t flags, const nrtgpu_aggregation* aggs, int32_t n_aggs,
+                                     const nrtgpu_aggregation_result* results, const nrtgpu_nested_aggregation* nested,
+                                     int32_t n_nested, const nrtgpu_nested_result* nested_results,
+                                     const nrtgpu_nested_sort* nested_sorts, const nrtgpu_agg_filter* agg_filters,
+                                     const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses,
+                                     const nrtgpu_query* filter_queries, int32_t n_filter_queries, void* stream, int32_t* out_docs,
+                                     float* out_scores, int32_t* out_counts, int64_t* out_total_hits);
 
 /* Request micro-batcher: the reference's search API is ONE query per RPC (clientlib/src/main/proto/yelp/nrtsearch/
  * luceneserver.proto:164), each on its own SERVER-pool thread (GrpcServerExecutorSupplier.java:68-75). Handler threads call

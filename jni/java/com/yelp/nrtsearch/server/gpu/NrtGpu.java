@@ -220,6 +220,27 @@ public final class NrtGpu {
       ByteBuffer filterQueries, int nFilterQueries, ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts,
       ByteBuffer outTotalHits);
 
+  /**
+   * searchBoolAggsSortedHits for the queries of searchTreePhrases (include/nrtgpu.h nrtgpu_search_tree_aggs): nested
+   * BooleanQuery / DisjunctionMaxQuery, PhraseQuery leaves and flat batches of more than 4 term clauses or topK > 512, their
+   * collectors run by the window engine. The tree and phrase buffers as searchTreePhrases (nNodes / nPhrases may be 0), the
+   * collector arguments as searchBoolAggsSortedHits.
+   */
+  public static native int searchTreeAggs(
+      long index, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer phrases, int nPhrases,
+      ByteBuffer phraseTerms, int nPhraseTerms, ByteBuffer queries, int nq, int topK, int flags, ByteBuffer aggs, int nAggs,
+      ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, long[][] sortOrders, ByteBuffer[] sortValues,
+      ByteBuffer aggFilters, ByteBuffer[] filterValues, ByteBuffer filterClauses, int nFilterClauses, ByteBuffer filterQueries,
+      int nFilterQueries, ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits);
+
+  /** searchTreeAggs over the leaves of a searcher: sortOrders[j] holds one order per leaf, in leaf order. */
+  public static native int searcherSearchTreeAggs(
+      long searcher, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer phrases, int nPhrases,
+      ByteBuffer phraseTerms, int nPhraseTerms, ByteBuffer queries, int nq, int topK, int flags, ByteBuffer aggs, int nAggs,
+      ByteBuffer[] aggOut, ByteBuffer nested, int nNested, ByteBuffer[] nestedOut, long[][] sortOrders, ByteBuffer[] sortValues,
+      ByteBuffer aggFilters, ByteBuffer[] filterValues, ByteBuffer filterClauses, int nFilterClauses, ByteBuffer filterQueries,
+      int nFilterQueries, ByteBuffer outDocs, ByteBuffer outScores, ByteBuffer outCounts, ByteBuffer outTotalHits);
+
   public static native long batcherCreate(long index, int maxBatch, int maxWaitUs);
 
   /** Blocks until the batch this request rode in is back; diag = nrtgpu_diagnostics (24 bytes) or null. */

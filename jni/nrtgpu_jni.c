@@ -327,6 +327,39 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchBoolAggsS
   free((void*)so);
   return fail(env, rc);
 }
+/* searchBoolAggsSortedHits for query trees, phrases and wide batches: the tree and phrase buffers as searchTreePhrases */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTreeAggs(
+    JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,
+    jobject phraseTerms, jint nPhraseTerms, jobject queries, jint nq, jint topK, jint flags, jobject aggs, jint nAggs,
+    jobjectArray aggOut, jobject nested, jint nNested, jobjectArray nestedOut, jobjectArray sortOrders, jobjectArray sortValues,
+    jobject aggFilters, jobjectArray filterValues, jobject filterClauses, jint nFilterClauses, jobject filterQueries,
+    jint nFilterQueries, jobject outDocs, jobject outScores, jobject outCounts, jobject outTotalHits) {
+  nrtgpu_aggregation_result* ar = NULL;
+  nrtgpu_nested_result* nr = NULL;
+  nrtgpu_agg_filter* af = NULL;
+  nrtgpu_nested_sort* ns = NULL;
+  const nrtgpu_sort_order** so = NULL;
+  int rc = agg_results(env, aggOut, nAggs, nestedOut, nNested, &ar, &nr);
+  if (!rc) rc = agg_filter_records(env, aggFilters, filterValues, nAggs, &af);
+  if (!rc) rc = nested_sort_records(env, sortOrders, sortValues, nNested, &ns, &so);
+  if (!rc)
+    rc = nrtgpu_search_tree_aggs((nrtgpu_index*)(intptr_t)ix, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                 (const nrtgpu_node*)ADDR(env, nodes), nNodes, (const nrtgpu_phrase*)ADDR(env, phrases), nPhrases,
+                                 (const nrtgpu_phrase_term*)ADDR(env, phraseTerms), nPhraseTerms,
+                                 (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                 (const nrtgpu_aggregation*)ADDR(env, aggs), nAggs, ar,
+                                 (const nrtgpu_nested_aggregation*)ADDR(env, nested), nNested, nr, ns, af,
+                                 (const nrtgpu_clause*)ADDR(env, filterClauses), nFilterClauses,
+                                 (const nrtgpu_query*)ADDR(env, filterQueries), nFilterQueries, NULL,
+                                 (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
+                                 (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
+  free(ar);
+  free(nr);
+  free(af);
+  free(ns);
+  free((void*)so);
+  return fail(env, rc);
+}
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_fetchColumns(
     JNIEnv* env, jclass c, jlong ix, jobject colIds, jint nCols, jobject docs, jint n, jobject outValues, jobject outHas) {
   return fail(env, nrtgpu_fetch_columns((nrtgpu_index*)(intptr_t)ix, (const int32_t*)ADDR(env, colIds), nCols,
@@ -471,6 +504,39 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchB
                                                       (const nrtgpu_query*)ADDR(env, filterQueries), nFilterQueries, NULL,
                                                       (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
                                                       (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
+  free(ar);
+  free(nr);
+  free(af);
+  free(ns);
+  free((void*)so);
+  return fail(env, rc);
+}
+
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherSearchTreeAggs(
+    JNIEnv* env, jclass c, jlong s, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,
+    jobject phraseTerms, jint nPhraseTerms, jobject queries, jint nq, jint topK, jint flags, jobject aggs, jint nAggs,
+    jobjectArray aggOut, jobject nested, jint nNested, jobjectArray nestedOut, jobjectArray sortOrders, jobjectArray sortValues,
+    jobject aggFilters, jobjectArray filterValues, jobject filterClauses, jint nFilterClauses, jobject filterQueries,
+    jint nFilterQueries, jobject outDocs, jobject outScores, jobject outCounts, jobject outTotalHits) {
+  nrtgpu_aggregation_result* ar = NULL;
+  nrtgpu_nested_result* nr = NULL;
+  nrtgpu_agg_filter* af = NULL;
+  nrtgpu_nested_sort* ns = NULL;
+  const nrtgpu_sort_order** so = NULL;
+  int rc = agg_results(env, aggOut, nAggs, nestedOut, nNested, &ar, &nr);
+  if (!rc) rc = agg_filter_records(env, aggFilters, filterValues, nAggs, &af);
+  if (!rc) rc = nested_sort_records(env, sortOrders, sortValues, nNested, &ns, &so);
+  if (!rc)
+    rc = nrtgpu_searcher_search_tree_aggs((nrtgpu_searcher*)(intptr_t)s, (const nrtgpu_clause*)ADDR(env, clauses), nClauses,
+                                          (const nrtgpu_node*)ADDR(env, nodes), nNodes, (const nrtgpu_phrase*)ADDR(env, phrases),
+                                          nPhrases, (const nrtgpu_phrase_term*)ADDR(env, phraseTerms), nPhraseTerms,
+                                          (const nrtgpu_query*)ADDR(env, queries), nq, topK, flags,
+                                          (const nrtgpu_aggregation*)ADDR(env, aggs), nAggs, ar,
+                                          (const nrtgpu_nested_aggregation*)ADDR(env, nested), nNested, nr, ns, af,
+                                          (const nrtgpu_clause*)ADDR(env, filterClauses), nFilterClauses,
+                                          (const nrtgpu_query*)ADDR(env, filterQueries), nFilterQueries, NULL,
+                                          (int32_t*)ADDR(env, outDocs), (float*)ADDR(env, outScores),
+                                          (int32_t*)ADDR(env, outCounts), (int64_t*)ADDR(env, outTotalHits));
   free(ar);
   free(nr);
   free(af);

@@ -151,6 +151,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_searcher_search_knn_filtered", "nrtgpu_searcher_search_bool_aggs_nested",
     "nrtgpu_search_bool_aggs_filtered", "nrtgpu_searcher_search_bool_aggs_filtered",
     "nrtgpu_search_bool_aggs_sorted_hits", "nrtgpu_searcher_search_bool_aggs_sorted_hits",
+    "nrtgpu_search_tree_aggs", "nrtgpu_searcher_search_tree_aggs",
 ]
 
 _gpu = None
@@ -266,6 +267,11 @@ def gpu_lib() -> C.CDLL:
         lib.nrtgpu_search_bool_aggs_sorted_hits.argtypes = lib.nrtgpu_search_bool_aggs_filtered.argtypes[:13] + \
             [C.POINTER(NestedSort)] + lib.nrtgpu_search_bool_aggs_filtered.argtypes[13:]
         lib.nrtgpu_searcher_search_bool_aggs_sorted_hits.argtypes = lib.nrtgpu_search_bool_aggs_sorted_hits.argtypes
+        # the tree and phrase arguments of nrtgpu_search_tree_phrases, then those of nrtgpu_search_bool_aggs_sorted_hits
+        lib.nrtgpu_search_tree_aggs.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32, C.POINTER(Phrase),
+                                                C.c_int32, C.POINTER(PhraseTerm), C.c_int32] + \
+            lib.nrtgpu_search_bool_aggs_sorted_hits.argtypes[3:]
+        lib.nrtgpu_searcher_search_tree_aggs.argtypes = lib.nrtgpu_search_tree_aggs.argtypes
         lib.nrtgpu_batcher_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
         lib.nrtgpu_batcher_submit.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(Diagnostics)]

@@ -19,11 +19,14 @@
 // slices of a query through one global atomicMax word -- the device analogue of the reference's
 // LazyMaxScoreAccumulator (src/main/java/org/apache/lucene/search/LazyMaxScoreAccumulator.java:21-70),
 // used here only to drop hits that provably cannot enter the top-k (results stay exact).
-// Query trees (tree batches, bool_window_kernel<true>) change pass 2 only: the drivers are the term leaves of the root's
+// Query trees (tree batches, bool_window_kernel<true, *>) change pass 2 only: the drivers are the term leaves of the root's
 // cover (batch_plan.inc compile_tree), and a doc is evaluated node by node (eval_node) instead of by one clause list.
+// Additional collectors (nrtgpu_search_tree_aggs, bool_window_kernel<kTree, true>): every matching doc is also handed to
+// agg_collect with its score, where pass 2 counts it, as the probe kernel's generic instantiation does.
 #pragma once
 #include <type_traits>
 #include "query_eval.cuh"
+#include "collect_kernel.cuh"
 
 namespace nrtgpu {
 
@@ -55,6 +58,8 @@ struct BoolLaunch {
   // tree batches with phrases (batch_plan.h DevPhrase): the records of query q are phrases[phrase_begin[q], phrase_begin[q + 1])
   const DevPhrase* phrases;
   const int32_t* phrase_begin;
+  // additional collectors (the kAggs instantiations; device pointer)
+  const AggLaunch* aggs;
 };
 
 template <bool kTree>
@@ -110,8 +115,9 @@ __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolT
   return eval_tree(ix, sm, doc, slot, out_score);
 }
 
-// kTree: a tree batch (sm holds the query's nodes, evaluate_doc walks them); otherwise flat BooleanQuerys
-template <bool kTree>
+// kTree: a tree batch (sm holds the query's nodes, evaluate_doc walks them); otherwise flat BooleanQuerys.
+// kAggs: every matching doc also goes to the collectors of L.aggs (the other instantiations never read it)
+template <bool kTree, bool kAggs>
 __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_constant__ BoolLaunch L) {
   using Smem = typename std::conditional<kTree, BoolTreeSmem, BoolSmem>::type;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -201,6 +207,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
         uint64_t key = 0;
         if (matched) {
           ++my_hits;
+          if constexpr (kAggs) agg_collect(*L.aggs, L.ix, qi, doc, score);   // additional collectors see every matching doc
           key = make_key(score, doc);
           is_cand = key > sm.theta && (!has_after || key < after_key);
         }

@@ -417,8 +417,10 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   { const char* e = getenv("NRTGPU_ITEM_POSTINGS"); if (e && atoll(e) > 0) c->plan.item_postings = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE"); if (e && atoll(e) > 0) c->plan.item_share = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE_FULL"); if (e && atoll(e) > 0) c->plan.item_share_full = atoll(e); }
-  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
-  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
 #define NRT_PROBE_ATTR(S, D) \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasA, v3::kStageA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageA>))); \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasB, v3::kStageB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageB>)));
@@ -975,6 +977,43 @@ static int probe_launch(nrtgpu_batch* b, v3::ProbeLaunch P, bool debug, cudaStre
   return NRTGPU_OK;
 }
 
+// The batch's engine over its work items: the probe kernel, or bool_window_kernel for wide and tree batches, with the
+// additional collectors `aggs` (device pointer, NULL: none). Pass 1 (p2_total NULL) counts into the batch's own totalHits and
+// flags under its limits. The top-hits run of batch_nested_top_hits counts totalHits into p2_total and the probe kernel's
+// pruned / terminated into p2_flags [2 * nq], without deadline or terminateAfter; the caller has reset the engine's theta,
+// slice counts and queue heads.
+static int batch_engine_launch(nrtgpu_batch* b, const AggLaunch* aggs, unsigned long long* p2_total, int32_t* p2_flags, bool debug,
+                               cudaStream_t st) {
+  const bool p2 = p2_total != nullptr;
+  if (!b->cb.wide) {
+    v3::ProbeLaunch P = probe_params(b);
+    P.aggs = aggs;
+    if (p2) { P.total_hits = p2_total; P.pruned = p2_flags; P.terminated = p2_flags + b->nq; P.deadline_ns = 0; P.terminate_after = 0; }
+    return probe_launch(b, P, debug && !p2, st);
+  }
+  BoolLaunch L;
+  L.ix = b->ix->view();
+  L.nodes = nullptr; L.node_begin = nullptr; L.phrases = nullptr; L.phrase_begin = nullptr;
+  L.clauses = b->clauses.p; L.queries = b->queries.p;
+  L.work_query = b->work_query.p; L.work_slice = b->work_slice.p;
+  L.n_work = b->plan.n_work(); L.n_slices = b->plan.n_lists; L.top_k = b->top_k;
+  L.theta = b->theta.p; L.total_hits = p2 ? p2_total : b->total_hits.p;
+  L.slice_keys = b->slice_keys.p; L.slice_cnt = b->slice_cnt.p;
+  L.deadline_ns = (!p2 && b->limits_active) ? b->deadline_ns : 0; L.clock0 = b->clock0.p; L.timed_out = b->timed_out.p;
+  L.aggs = aggs;
+  const unsigned grid = (unsigned)b->plan.n_work();
+  if (b->cb.tree) {
+    L.nodes = b->nodes.p; L.node_begin = b->node_begin.p; L.phrases = b->phrases.p; L.phrase_begin = b->phrase_begin.p;
+    if (aggs) bool_window_kernel<true, true><<<grid, kThreads, sizeof(BoolTreeSmem), st>>>(L);
+    else bool_window_kernel<true, false><<<grid, kThreads, sizeof(BoolTreeSmem), st>>>(L);
+  } else {
+    if (aggs) bool_window_kernel<false, true><<<grid, kThreads, sizeof(BoolSmem), st>>>(L);
+    else bool_window_kernel<false, false><<<grid, kThreads, sizeof(BoolSmem), st>>>(L);
+  }
+  NRT_CUDA_TRY(cudaGetLastError());
+  return NRTGPU_OK;
+}
+
 // a column's bucket codes and sorted distinct values in an image (NULL in an image without docs: it has no such arrays)
 static const uint32_t* ix_col_code(const nrtgpu_index* ix, int32_t c) {
   return (size_t)c < ix->col_code.size() ? ix->col_code[(size_t)c]->p : nullptr;
@@ -1066,60 +1105,41 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   cudaEvent_t* ev = b->ev[b->runs_recorded % nrtgpu_batch::kEvRing];
   NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
   if (b->plan.n_work() > 0) {
-    BoolLaunch L;
-    L.ix = b->ix->view();
-    L.nodes = nullptr; L.node_begin = nullptr; L.phrases = nullptr; L.phrase_begin = nullptr;
-    L.clauses = b->clauses.p; L.queries = b->queries.p;
-    L.work_query = b->work_query.p; L.work_slice = b->work_slice.p;
-    L.n_work = b->plan.n_work(); L.n_slices = b->plan.n_lists; L.top_k = b->top_k;
-    L.theta = b->theta.p; L.total_hits = b->total_hits.p;
-    L.slice_keys = b->slice_keys.p; L.slice_cnt = b->slice_cnt.p;
-    L.deadline_ns = b->limits_active ? b->deadline_ns : 0; L.clock0 = b->clock0.p; L.timed_out = b->timed_out.p;
-    if (!b->cb.wide) {
-      const int n_probe = b->plan.n_probe_simple + b->plan.n_probe_generic;
-      if (n_probe > 0) {
-        v3::ProbeLaunch P = probe_params(b);
-        if (!b->cb.aggs.empty()) {
-          const AggTables& t = b->agg_tab;
-          if ((rc_dbg = batch_agg_codes(b, st))) return rc_dbg;
-          AggLaunch A; std::memset(&A, 0, sizeof(A));
-          A.n_aggs = (int32_t)b->cb.aggs.size();
-          for (int i = 0; i < A.n_aggs; ++i) {
-            const nrtgpu_aggregation& a = b->cb.aggs[(size_t)i];
-            A.a[i].kind = a.kind; A.a[i].column = a.column; A.a[i].value_type = a.value_type;
-            if (a.kind == NRTGPU_AGG_FILTER) {   // a one-bucket terms aggregation over the image's column without a has array
-              A.a[i].kind = NRTGPU_AGG_TERMS; A.a[i].column = b->ix->n_columns;
-            }
-            if (a.kind == NRTGPU_AGG_TERMS || a.kind == NRTGPU_AGG_FILTER) {
-              A.a[i].n_buckets = t.n_buckets[i];
-              A.a[i].counts = t.counts[i]; A.codes[i] = b->agg_codes[i];
-            } else {
-              A.a[i].dvals = t.dvals[i];
-            }
-            A.nested_begin[i + 1] = A.nested_begin[i];   // pass 1: the nested min / max / sum collectors
-            for (size_t j = 0; j < b->cb.nested.size(); ++j) {
-              const nrtgpu_nested_aggregation& n = b->cb.nested[j];
-              if (n.parent != i || n.kind == NRTGPU_AGG_TOP_HITS) continue;
-              AggNestedDev& d = A.nested[A.nested_begin[i + 1]++];
-              d.kind = n.kind; d.column = n.column; d.value_type = n.value_type; d.dvals = t.nest_words[j];
-            }
-          }
-          if ((rc_dbg = b->agg_launch.upload_async(&A, 1, st))) return rc_dbg;
-          NRT_CUDA_TRY(cudaStreamSynchronize(st));   // A is a stack object
-          P.aggs = b->agg_launch.p;
+    const AggLaunch* aggs = nullptr;
+    if (!b->cb.aggs.empty()) {   // pass 1 of the collectors, on either engine
+      const AggTables& t = b->agg_tab;
+      if ((rc_dbg = batch_agg_codes(b, st))) return rc_dbg;
+      AggLaunch A; std::memset(&A, 0, sizeof(A));
+      A.n_aggs = (int32_t)b->cb.aggs.size();
+      for (int i = 0; i < A.n_aggs; ++i) {
+        const nrtgpu_aggregation& a = b->cb.aggs[(size_t)i];
+        A.a[i].kind = a.kind; A.a[i].column = a.column; A.a[i].value_type = a.value_type;
+        if (a.kind == NRTGPU_AGG_FILTER) {   // a one-bucket terms aggregation over the image's column without a has array
+          A.a[i].kind = NRTGPU_AGG_TERMS; A.a[i].column = b->ix->n_columns;
         }
-        if (debug) {
-          if (!b->probe_stats.p && (rc_dbg = b->probe_stats.alloc(2 * v3::kProbeStats))) return rc_dbg;
-          NRT_CUDA_TRY(cudaMemsetAsync(b->probe_stats.p, 0, 2 * v3::kProbeStats * sizeof(unsigned long long), st));
+        if (a.kind == NRTGPU_AGG_TERMS || a.kind == NRTGPU_AGG_FILTER) {
+          A.a[i].n_buckets = t.n_buckets[i];
+          A.a[i].counts = t.counts[i]; A.codes[i] = b->agg_codes[i];
+        } else {
+          A.a[i].dvals = t.dvals[i];
         }
-        if ((rc_dbg = probe_launch(b, P, debug, st))) return rc_dbg;
+        A.nested_begin[i + 1] = A.nested_begin[i];   // pass 1: the nested min / max / sum collectors
+        for (size_t j = 0; j < b->cb.nested.size(); ++j) {
+          const nrtgpu_nested_aggregation& n = b->cb.nested[j];
+          if (n.parent != i || n.kind == NRTGPU_AGG_TOP_HITS) continue;
+          AggNestedDev& d = A.nested[A.nested_begin[i + 1]++];
+          d.kind = n.kind; d.column = n.column; d.value_type = n.value_type; d.dvals = t.nest_words[j];
+        }
       }
-    } else if (b->cb.tree) {
-      L.nodes = b->nodes.p; L.node_begin = b->node_begin.p; L.phrases = b->phrases.p; L.phrase_begin = b->phrase_begin.p;
-      bool_window_kernel<true><<<b->plan.n_work(), kThreads, sizeof(BoolTreeSmem), st>>>(L);
-    } else
-      bool_window_kernel<false><<<b->plan.n_work(), kThreads, sizeof(BoolSmem), st>>>(L);
-    NRT_CUDA_TRY(cudaGetLastError());
+      if ((rc_dbg = b->agg_launch.upload_async(&A, 1, st))) return rc_dbg;
+      NRT_CUDA_TRY(cudaStreamSynchronize(st));   // A is a stack object
+      aggs = b->agg_launch.p;
+    }
+    if (debug && !b->cb.wide) {
+      if (!b->probe_stats.p && (rc_dbg = b->probe_stats.alloc(2 * v3::kProbeStats))) return rc_dbg;
+      NRT_CUDA_TRY(cudaMemsetAsync(b->probe_stats.p, 0, 2 * v3::kProbeStats * sizeof(unsigned long long), st));
+    }
+    if ((rc_dbg = batch_engine_launch(b, aggs, nullptr, nullptr, debug, st))) return rc_dbg;
   }
   NRT_CUDA_TRY(cudaEventRecord(ev[1], st));
   if (debug && b->probe_stats.p && !b->cb.wide) {
@@ -1240,7 +1260,8 @@ static int sorted_hit_values(const nrtgpu_sort_order* o, int32_t doc_base, int32
 }
 
 // Nested top hits of terms or filter aggregation `parent` (pass 2) over the batches bs[0 .. n_b) that counted into one set of tables
-// (a single image: one batch; a searcher: one per leaf). Each batch's probe launch runs again with a collector that only
+// (a single image: one batch; a searcher: one per leaf). Each batch's engine runs again (batch_engine_launch: the probe
+// kernel, or the window engine for tree and wide batches) with a collector that only
 // appends the key of each doc of a returned bucket (slot map nest_slot) to per-(query, slot) segments sized by the bucket
 // counts h_cnt [nq*size]: make_key(score, global doc), or for a sorted collector its Sort key over that leaf's order
 // (agg_nested_collect); its totalHits / pruned / terminated go to scratch, and theta / slice lists / queue heads are its
@@ -1329,7 +1350,7 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
       if (merge)   // this leaf's sorted keys start from empty segments
         for (int k = 0; k < n_th; ++k)
           if (order_of(k, l)) NRT_CUDA_TRY(cudaMemsetAsync(b->nest_fill.p + (size_t)k * gs, 0, (size_t)gs * sizeof(unsigned int), st));
-      if (x->plan.n_probe_simple + x->plan.n_probe_generic > 0) {
+      if (x->plan.n_work() > 0) {
         AggLaunch& A = launches[(size_t)l];
         std::memset(&A, 0, sizeof(A));
         A.n_aggs = 1;
@@ -1348,14 +1369,10 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
         if ((rc = x->nest_launch.upload_async(&A, 1, st))) return rc;
         NRT_CUDA_TRY(cudaMemsetAsync(x->theta.p, 0, x->theta.bytes(), st));
         NRT_CUDA_TRY(cudaMemsetAsync(x->slice_cnt.p, 0, x->slice_cnt.bytes(), st));
-        NRT_CUDA_TRY(cudaMemsetAsync(x->work_counter.p, 0, x->work_counter.bytes(), st));
+        if (x->work_counter.p) NRT_CUDA_TRY(cudaMemsetAsync(x->work_counter.p, 0, x->work_counter.bytes(), st));   // (probe batches)
         NRT_CUDA_TRY(cudaMemsetAsync(b->p2_total.p, 0, b->p2_total.bytes(), st));
         NRT_CUDA_TRY(cudaMemsetAsync(b->p2_flags.p, 0, b->p2_flags.bytes(), st));
-        v3::ProbeLaunch P = probe_params(x);
-        P.total_hits = b->p2_total.p; P.pruned = b->p2_flags.p; P.terminated = b->p2_flags.p + nq;
-        P.deadline_ns = 0; P.terminate_after = 0;
-        P.aggs = x->nest_launch.p;
-        if ((rc = probe_launch(x, P, false, st))) return rc;
+        if ((rc = batch_engine_launch(x, x->nest_launch.p, b->p2_total.p, b->p2_flags.p, false, st))) return rc;
       }
       for (int k = 0; k < n_th && merge; ++k) {   // this leaf's best top_hits of each list, by its order, into its record
         const nrtgpu_sort_order* o = order_of(k, l);
@@ -1977,6 +1994,44 @@ int nrtgpu_search_bool_aggs_sorted_hits(nrtgpu_index* ix, const nrtgpu_clause* c
   int rc = aggs_request(&r, aggs, n_aggs, results, nested, n_nested, nested_results, nested_sorts, agg_filters, filter_clauses,
                         n_filter_clauses, filter_queries, n_filter_queries);
   if (rc || (rc = check_nested_sorts("nrtgpu_search_bool_aggs_sorted_hits", r, &ix, 1))) return rc;
+  SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.aggs = results;
+  o.nested = n_nested > 0 ? nested_results : nullptr;
+  return search_bool_impl(ix, r, nullptr, stream, o);
+}
+
+// the request of the tree entry points with collectors: a tree (or flat) batch with the phrase table and the collectors of
+// nrtgpu_search_bool_aggs_sorted_hits, collected by whichever engine runs the batch
+static int tree_aggs_request(BatchRequest* r, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes, int32_t n_nodes,
+                             const nrtgpu_phrase* phrases, int32_t n_phrases, const nrtgpu_phrase_term* phrase_terms,
+                             int32_t n_phrase_terms, const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                             const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                             const nrtgpu_nested_aggregation* nested, int32_t n_nested, const nrtgpu_nested_result* nested_results,
+                             const nrtgpu_nested_sort* nested_sorts, const nrtgpu_agg_filter* agg_filters,
+                             const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
+                             int32_t n_filter_queries) {
+  if (n_nodes < 0 || (n_nodes > 0 && !nodes)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_search_tree: bad nodes");
+  *r = tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, INT32_MAX, flags);
+  int rc = phrase_request(r, phrases, n_phrases, phrase_terms, n_phrase_terms);
+  if (rc || (rc = aggs_request(r, aggs, n_aggs, results, nested, n_nested, nested_results, nested_sorts, agg_filters, filter_clauses,
+                               n_filter_clauses, filter_queries, n_filter_queries))) return rc;
+  r->window_collectors = true;
+  return NRTGPU_OK;
+}
+
+int nrtgpu_search_tree_aggs(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes, int32_t n_nodes,
+                            const nrtgpu_phrase* phrases, int32_t n_phrases, const nrtgpu_phrase_term* phrase_terms,
+                            int32_t n_phrase_terms, const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
+                            const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,
+                            const nrtgpu_nested_aggregation* nested, int32_t n_nested, const nrtgpu_nested_result* nested_results,
+                            const nrtgpu_nested_sort* nested_sorts, const nrtgpu_agg_filter* agg_filters,
+                            const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses, const nrtgpu_query* filter_queries,
+                            int32_t n_filter_queries, void* stream, int32_t* out_docs, float* out_scores, int32_t* out_counts,
+                            int64_t* out_total_hits) {
+  BatchRequest r;
+  int rc = tree_aggs_request(&r, clauses, n_clauses, nodes, n_nodes, phrases, n_phrases, phrase_terms, n_phrase_terms, queries, nq, top_k,
+                             flags, aggs, n_aggs, results, nested, n_nested, nested_results, nested_sorts, agg_filters, filter_clauses,
+                             n_filter_clauses, filter_queries, n_filter_queries);
+  if (rc || (rc = check_nested_sorts("nrtgpu_search_tree_aggs", r, &ix, 1))) return rc;
   SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.aggs = results;
   o.nested = n_nested > 0 ? nested_results : nullptr;
   return search_bool_impl(ix, r, nullptr, stream, o);
@@ -2705,6 +2760,10 @@ static int knn_leaf_record(nrtgpu_index* ix, int32_t nq, int32_t k, void* stream
   return NRTGPU_OK;
 }
 
+static int searcher_aggs(nrtgpu_searcher* s, const char* fn, const BatchRequest& r, const nrtgpu_aggregation_result* results,
+                         const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs, float* out_scores,
+                         int32_t* out_counts, int64_t* out_total_hits);
+
 static bool searcher_has_vectors(const nrtgpu_searcher* s) {
   for (const nrtgpu_index* ix : s->leaves) if (ix->vec_dims > 0) return true;
   return false;
@@ -2886,9 +2945,7 @@ int nrtgpu_searcher_search_bool_aggs_filtered(nrtgpu_searcher* s, const nrtgpu_c
                                                       out_total_hits);
 }
 
-// Aggregations over the leaves: every leaf's batch counts into one set of reader-wide tables through its codes renumbered
-// to the column's reader-wide dictionary (searcher_dict) and tests its own image's filter rows; the selection and the
-// nested top hits then run once on them (sorted top hits: per leaf, then merged; batch_nested_top_hits)
+// Aggregations over the leaves (searcher_aggs)
 int nrtgpu_searcher_search_bool_aggs_sorted_hits(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
                                                  const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
                                                  const nrtgpu_aggregation* aggs, int32_t n_aggs,
@@ -2903,8 +2960,47 @@ int nrtgpu_searcher_search_bool_aggs_sorted_hits(nrtgpu_searcher* s, const nrtgp
   BatchRequest r{clauses, n_clauses, queries, nq, top_k, INT32_MAX, flags};
   int rc = aggs_request(&r, aggs, n_aggs, results, nested, n_nested, nested_results, nested_sorts, agg_filters, filter_clauses,
                         n_filter_clauses, filter_queries, n_filter_queries);
-  if (rc || (rc = check_nested_sorts("nrtgpu_searcher_search_bool_aggs_sorted_hits", r, s->leaves.data(), (int)s->leaves.size())))
-    return rc;
+  if (rc) return rc;
+  return searcher_aggs(s, "nrtgpu_searcher_search_bool_aggs_sorted_hits", r, results, nested_results, stream, out_docs, out_scores,
+                       out_counts, out_total_hits);
+}
+
+int nrtgpu_searcher_search_tree_aggs(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
+                                     int32_t n_nodes, const nrtgpu_phrase* phrases, int32_t n_phrases,
+                                     const nrtgpu_phrase_term* phrase_terms, int32_t n_phrase_terms, const nrtgpu_query* queries,
+                                     int32_t nq, int32_t top_k, int32_t flags, const nrtgpu_aggregation* aggs, int32_t n_aggs,
+                                     const nrtgpu_aggregation_result* results, const nrtgpu_nested_aggregation* nested,
+                                     int32_t n_nested, const nrtgpu_nested_result* nested_results,
+                                     const nrtgpu_nested_sort* nested_sorts, const nrtgpu_agg_filter* agg_filters,
+                                     const nrtgpu_clause* filter_clauses, int32_t n_filter_clauses,
+                                     const nrtgpu_query* filter_queries, int32_t n_filter_queries, void* stream, int32_t* out_docs,
+                                     float* out_scores, int32_t* out_counts, int64_t* out_total_hits) {
+  if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_tree_aggs: NULL searcher");
+  BatchRequest r;
+  int rc = tree_aggs_request(&r, clauses, n_clauses, nodes, n_nodes, phrases, n_phrases, phrase_terms, n_phrase_terms, queries, nq, top_k,
+                             flags, aggs, n_aggs, results, nested, n_nested, nested_results, nested_sorts, agg_filters, filter_clauses,
+                             n_filter_clauses, filter_queries, n_filter_queries);
+  if (rc) return rc;
+  return searcher_aggs(s, "nrtgpu_searcher_search_tree_aggs", r, results, nested_results, stream, out_docs, out_scores, out_counts,
+                       out_total_hits);
+}
+
+#include "batcher.inc"
+
+}  // extern "C"
+
+// The collector searches over the leaves (request r from aggs_request; fn names the entry point in refusals): every leaf's
+// batch counts into one set of reader-wide tables through its codes renumbered to the column's reader-wide dictionary
+// (searcher_dict) and tests its own image's filter rows; the selection and the nested top hits then run once on them
+// (sorted top hits: per leaf, then merged; batch_nested_top_hits)
+static int searcher_aggs(nrtgpu_searcher* s, const char* fn, const BatchRequest& r, const nrtgpu_aggregation_result* results,
+                         const nrtgpu_nested_result* nested_results, void* stream, int32_t* out_docs, float* out_scores,
+                         int32_t* out_counts, int64_t* out_total_hits) {
+  const nrtgpu_aggregation* aggs = r.aggs;
+  const nrtgpu_nested_aggregation* nested = r.nested;
+  const int32_t nq = r.nq, top_k = r.top_k, n_aggs = r.n_aggs, n_nested = r.n_nested;
+  int rc;
+  if ((rc = check_nested_sorts(fn, r, s->leaves.data(), (int)s->leaves.size()))) return rc;
   NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> g(s->mu);
@@ -2954,7 +3050,3 @@ int nrtgpu_searcher_search_bool_aggs_sorted_hits(nrtgpu_searcher* s, const nrtgp
   // TopDocs.merge of the leaves' pages; totalHits is exact (every match is counted) and summed over the leaves
   return searcher_merge_scored(s, nq, top_k, stream, out_docs, out_scores, out_counts, out_total_hits, nullptr, nullptr, nullptr);
 }
-
-#include "batcher.inc"
-
-}  // extern "C"

@@ -968,6 +968,21 @@ class GpuIndexSearcher:
                                                     C.c_void_p(stream), *hits))
         return out, outs
 
+    def search_tree_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
+                                    stream: int = 0):
+        """search_with_collectors() for the queries of search_tree(): nested BooleanQuery and DisjunctionMaxQuery, PhraseQuery
+        leaves, and flat batches of any width (nrtgpu_search_tree_aggs). The same collectors, the same (BatchResult, results)
+        return; a batch with a nested query or a phrase, or a wide one, is collected by the window engine."""
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, phrase_table=True)
+        k = collector.num_hits_to_collect
+        out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
+                          np.zeros(nq, np.uint8))
+        fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * 1)(self.index.sort_order(fields, stream).value))
+        check(self._lib.nrtgpu_search_tree_aggs(self.index.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k, 0,
+                                                *fr.sorted_args, C.c_void_p(stream), out.docs.ctypes.data, out.scores.ctypes.data,
+                                                out.counts.ctypes.data, out.total_hits.ctypes.data))
+        return out, fr.outs
+
     def score_docs(self, queries: Sequence[object], docs: np.ndarray, counts: Optional[np.ndarray] = None, stream: int = 0):
         """Second pass of QueryRescorer: query q on its own hit list -> (matches uint8 [nq, n], scores float32 [nq, n])."""
         carr, ncl, qarr, nq = compile_queries(queries)
@@ -1187,6 +1202,21 @@ class GpuLeafSearcher:
                                                                 out.scores.ctypes.data, out.counts.ctypes.data,
                                                                 out.total_hits.ctypes.data))
         return out, outs
+
+    def search_tree_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
+                                    stream: int = 0):
+        """GpuIndexSearcher.search_tree_with_collectors over the leaves (nrtgpu_searcher_search_tree_aggs), with the reader-wide
+        tables and merges of search_with_collectors. Returns what the single-image method returns."""
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, phrase_table=True)
+        k = collector.num_hits_to_collect
+        out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
+                          np.zeros(nq, np.uint8))
+        fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * len(self.leaves))(
+            *[l.sort_order(fields, stream).value for l in self.leaves]))
+        check(self._lib.nrtgpu_searcher_search_tree_aggs(self.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k, 0,
+                                                         *fr.sorted_args, C.c_void_p(stream), out.docs.ctypes.data,
+                                                         out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data))
+        return out, fr.outs
 
     def close(self):
         if self.handle:
