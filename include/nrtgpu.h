@@ -218,6 +218,35 @@ int nrtgpu_batch_prepare_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, in
  * within a posting. */
 int nrtgpu_index_add_positions(nrtgpu_index* ix, const int32_t* positions, int64_t n_positions);
 
+/* Keyword columns of an image (string doc values of atom / text-with-docValues fields: SortedDocValues and
+ * SortedSetDocValues of the leaf). Column k of the call is keyword column k of the image; terms aggregations name it with
+ * value_type NRTGPU_AGG_VALUE_KEYWORD. Per column:
+ *   term_bytes / term_offsets [n_terms + 1]  the leaf's term dictionary, term i = term_bytes[term_offsets[i], term_offsets[i + 1]),
+ *            strictly ascending in unsigned-byte order (BytesRef.compareTo); ordinal i is term i;
+ *   multi_valued 0 (SORTED)      ords [n_docs]: the doc's ordinal, -1: no value;
+ *   multi_valued 1 (SORTED_SET)  doc_offsets [n_docs + 1] (doc_offsets[0] == 0, non-decreasing) and ords [doc_offsets[n_docs]]:
+ *            the doc's ordinals strictly ascending (SortedSetDocValues has each term of a doc once).
+ * On the device an ordinal i is the bucket code 2i + 2 (0: no value): 4 B per doc (SORTED), or 4 B per value plus the
+ * int64 doc offsets (SORTED_SET). The dictionary stays on the host (bucket keys, reader-wide dictionaries).
+ * nrtgpu_index_device_bytes counts the device arrays. The columns stay valid across nrtgpu_index_set_live_docs and
+ * nrtgpu_index_update_stats.
+ *   NRTGPU_ERR_INVALID (the image is left unchanged): n < 0, a NULL array, a bad multi_valued, n_terms < 0, term offsets that
+ *     do not start at 0 or descend, terms that are not strictly ascending (unsorted or duplicate), an ordinal outside
+ *     [0, n_terms) (SORTED: -1 allowed), doc offsets that do not start at 0 or descend, ordinals of a doc that do not strictly
+ *     ascend, and a second call on the image. */
+typedef struct {
+  int32_t n_terms;
+  int32_t multi_valued;          /* 0: SORTED, 1: SORTED_SET */
+  const uint8_t* term_bytes;
+  const int64_t* term_offsets;   /* [n_terms + 1] */
+  const int32_t* ords;           /* SORTED: [n_docs]; SORTED_SET: [doc_offsets[n_docs]] */
+  const int64_t* doc_offsets;    /* SORTED_SET: [n_docs + 1]; SORTED: unused */
+} nrtgpu_keyword_column;
+int nrtgpu_index_add_keyword_columns(nrtgpu_index* ix, const nrtgpu_keyword_column* cols, int32_t n);
+/* The bytes of term `ord` of keyword column `column` of an image: its length in *len, and its first min(len, cap) bytes
+ * in out (out may be NULL when cap is 0). NRTGPU_ERR_INVALID: a column or ordinal out of range, len NULL. */
+int nrtgpu_index_keyword_term(const nrtgpu_index* ix, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len);
+
 /* Phrase leaves of query trees (PhraseQuery / match_phrase, reference QueryNodeMapper.java:285-291, :397-427). A clause of
  * kind NRTGPU_PHRASE is a leaf whose id indexes phrases[]; its boost is the leaf's folded boost, as for a term leaf. The
  * phrase's terms are phrase_terms[term_begin:term_end] with their PhraseQuery positions (PhraseQuery.getTerms() /
@@ -375,6 +404,15 @@ int nrtgpu_merge_sorted_packed(nrtgpu_ctx* ctx, const nrtgpu_sort_field* fields,
  *                     query without clauses or with minimumNumberShouldMatch above its SHOULD count), gives
  *                     Double.MAX_VALUE / -Double.MAX_VALUE / 0.0, and a terms aggregation no buckets.
  * value_type says how the column's sortable long maps back to the number: 0 int / long, 1 float, 2 double.
+ * Keyword terms (OrdinalTermsCollectorManager, TermsCollectorManager.java:154-170): a TERMS aggregation with value_type
+ *   NRTGPU_AGG_VALUE_KEYWORD (3) counts keyword column `column` (nrtgpu_index_add_keyword_columns) per term. A doc of a
+ *   SORTED_SET column counts once in the bucket of each of its terms (and is handed to the nested collectors once per
+ *   term). bucket_keys are ordinals: the image's own, or on a searcher reader-wide ordinals into the byte-order union of
+ *   the leaves' dictionaries (nrtgpu_index_keyword_term / nrtgpu_searcher_keyword_term give the bytes). Every other rule
+ *   reads "value" as "term": size, order_desc, totalBuckets, totalOtherCounts, ties to the smaller term in byte order,
+ *   the 2 GB nq x terms table (on a searcher with the union's term count), filters, nested collectors and the window
+ *   engine, with no limit on a doc's terms. NRTGPU_ERR_INVALID: a keyword column out of range; MIN / MAX / SUM with value_type 3 keep "bad aggregation value_type" (a keyword has no
+ *   number).
  * Docs without a value contribute nothing. Bucket ties at the cut are unordered in the reference (hash-map order); here
  * the smaller value wins. Min, max (up to the sign of a zero, which depends on collection order in the reference too)
  * and every count are exact. Sums are accumulated in a different order than the reference's single thread: for n finite
@@ -382,6 +420,7 @@ int nrtgpu_merge_sorted_packed(nrtgpu_ctx* ctx, const nrtgpu_sort_field* fields,
  * int / long sums with sum|v| < 2^53 are exact, and whether partial sums near Double.MAX_VALUE overflow depends on the
  * order in both; with a NaN, or both infinities, the sum is NaN, else with an infinity that infinity. */
 enum { NRTGPU_AGG_TERMS = 1, NRTGPU_AGG_MIN = 2, NRTGPU_AGG_MAX = 3, NRTGPU_AGG_SUM = 4 };
+enum { NRTGPU_AGG_VALUE_KEYWORD = 3 };   /* value_type of a terms aggregation over a keyword column */
 typedef struct {
   int32_t kind, column, value_type;
   int32_t size;        /* terms: buckets returned (<= 2048) */
@@ -391,7 +430,7 @@ typedef struct {
 } nrtgpu_aggregation;
 typedef struct {       /* caller-allocated outputs of one aggregation (unused pointers may be NULL) */
   double* values;          /* [nq]        min / max / sum */
-  int64_t* bucket_keys;    /* [nq*size]   terms: column values (sortable-long domain) */
+  int64_t* bucket_keys;    /* [nq*size]   terms: column values (sortable-long domain); keyword terms: ordinals */
   int32_t* bucket_counts;  /* [nq*size] */
   int32_t* n_buckets;      /* [nq]        buckets filled */
   int32_t* total_buckets;  /* [nq]        BucketResult.totalBuckets */
@@ -788,7 +827,17 @@ int nrtgpu_searcher_search_knn_filtered(nrtgpu_searcher* s, const float* queries
  *   wide batches are NRTGPU_ERR_UNSUPPORTED, so is a column multi-valued in any leaf; a column index some leaf lacks is
  *   NRTGPU_ERR_INVALID. The 2 GB limits of the count and nested-word tables apply at the reader-wide U: a batch whose leaves
  *   each fit but whose union does not is refused before any batch is built or table allocated. On a refusal no output is
- *   written. NULL searcher: NRTGPU_ERR_INVALID. */
+ *   written. NULL searcher: NRTGPU_ERR_INVALID.
+ * Keyword terms over the leaves: the reader-wide dictionary of a keyword column is the byte-order union of the leaves' term
+ * dictionaries, built on the host by its first aggregation (or nrtgpu_searcher_keyword_term) and kept until close; each
+ * leaf's ordinals are mapped to it (its codes renumbered: 4 B per doc for SORTED, per value for SORTED_SET, except in a
+ * leaf whose dictionary is the union). bucket_keys are ordinals of the union. A keyword column index some leaf lacks is
+ * NRTGPU_ERR_INVALID. */
+/* The bytes of reader-wide term `ord` of keyword column `column` (as nrtgpu_index_keyword_term); builds the column's
+ * reader-wide dictionary if no call has yet, on the default stream. *n_terms (may be NULL) receives the union's size.
+ * NRTGPU_ERR_INVALID: a column some leaf lacks, an ordinal out of range (ord -1 only asks for n_terms), len NULL. */
+int nrtgpu_searcher_keyword_term(nrtgpu_searcher* s, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len,
+                                 int32_t* n_terms);
 int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
                                             const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
                                             const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,

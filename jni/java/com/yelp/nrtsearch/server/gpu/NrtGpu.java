@@ -66,6 +66,21 @@ public final class NrtGpu {
   public static native int addPositions(long index, ByteBuffer positions, long nPositions);
 
   /**
+   * Keyword columns of an image, read per leaf from SortedDocValues / SortedSetDocValues when the image is built: column k
+   * has nTerms[k] terms (termBytes, termOffsets int64[nTerms + 1], ascending in BytesRef order) and ords int32 per doc
+   * (SORTED, -1: no value) or int32 per value with docOffsets int64[maxDoc + 1] (SORTED_SET, multiValued[k] = 1). Once per
+   * image. A TermsCollector on the field is then an nrtgpu_aggregation with value_type 3 naming column k.
+   */
+  public static native int addKeywordColumns(long index, int[] nTerms, int[] multiValued, ByteBuffer[] termBytes,
+      ByteBuffer[] termOffsets, ByteBuffer[] ords, ByteBuffer[] docOffsets);
+
+  /** The bytes of term ord of keyword column `column` into out (at most cap); returns its length (bucket keys -> BytesRef). */
+  public static native int keywordTerm(long index, int column, int ord, ByteBuffer out, int cap);
+
+  /** keywordTerm for a searcher's reader-wide ordinals; ord -1 returns the number of reader-wide terms. */
+  public static native int searcherKeywordTerm(long searcher, int column, int ord, ByteBuffer out, int cap);
+
+  /**
    * Query trees with PhraseQuery leaves: phrases = nrtgpu_phrase[nPhrases] referenced by clauses of kind 4 (PHRASE),
    * phraseTerms = nrtgpu_phrase_term[nPhraseTerms] (term id, PhraseQuery position); otherwise as searchTree, which it is
    * with nPhrases == 0.

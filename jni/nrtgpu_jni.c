@@ -112,6 +112,59 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_addPositions(JN
                                                                                jlong nPositions) {
   return fail(env, nrtgpu_index_add_positions((nrtgpu_index*)(intptr_t)ix, (const int32_t*)ADDR(env, positions), nPositions));
 }
+/* keyword columns (SortedDocValues / SortedSetDocValues of the leaf), column k from element k of each array: termBytes,
+ * termOffsets (int64[nTerms + 1]), ords (int32) and docOffsets (int64[maxDoc + 1], SORTED_SET; null for SORTED) are direct
+ * ByteBuffers */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_addKeywordColumns(JNIEnv* env, jclass c, jlong ix, jintArray nTerms,
+                                                                                   jintArray multiValued, jobjectArray termBytes,
+                                                                                   jobjectArray termOffsets, jobjectArray ords,
+                                                                                   jobjectArray docOffsets) {
+  const jsize n = nTerms ? (*env)->GetArrayLength(env, nTerms) : 0;
+  if (n > 0 && (!multiValued || !termBytes || !termOffsets || !ords || !docOffsets || (*env)->GetArrayLength(env, multiValued) != n ||
+                (*env)->GetArrayLength(env, termBytes) != n || (*env)->GetArrayLength(env, termOffsets) != n ||
+                (*env)->GetArrayLength(env, ords) != n || (*env)->GetArrayLength(env, docOffsets) != n)) {
+    (*env)->ThrowNew(env, (*env)->FindClass(env, "java/lang/IllegalArgumentException"),
+                     "addKeywordColumns: the six arrays must have one element per column");
+    return NRTGPU_ERR_INVALID;
+  }
+  nrtgpu_keyword_column* cols = (nrtgpu_keyword_column*)calloc(n > 0 ? (size_t)n : 1, sizeof(nrtgpu_keyword_column));
+  if (!cols) return fail(env, NRTGPU_ERR_OOM);
+  jint* nt = n ? (*env)->GetIntArrayElements(env, nTerms, NULL) : NULL;
+  jint* mv = n ? (*env)->GetIntArrayElements(env, multiValued, NULL) : NULL;
+  for (jsize k = 0; k < n; ++k) {
+    cols[k].n_terms = nt[k]; cols[k].multi_valued = mv[k];
+    jobject tb = (*env)->GetObjectArrayElement(env, termBytes, k), to = (*env)->GetObjectArrayElement(env, termOffsets, k);
+    jobject od = (*env)->GetObjectArrayElement(env, ords, k), dof = (*env)->GetObjectArrayElement(env, docOffsets, k);
+    cols[k].term_bytes = (const uint8_t*)ADDR(env, tb);
+    cols[k].term_offsets = (const int64_t*)ADDR(env, to);
+    cols[k].ords = (const int32_t*)ADDR(env, od);
+    cols[k].doc_offsets = (const int64_t*)ADDR(env, dof);
+    /* the direct buffers stay reachable from the caller's arrays: their addresses outlive these local references */
+    if (tb) (*env)->DeleteLocalRef(env, tb);
+    if (to) (*env)->DeleteLocalRef(env, to);
+    if (od) (*env)->DeleteLocalRef(env, od);
+    if (dof) (*env)->DeleteLocalRef(env, dof);
+  }
+  if (n) { (*env)->ReleaseIntArrayElements(env, nTerms, nt, JNI_ABORT); (*env)->ReleaseIntArrayElements(env, multiValued, mv, JNI_ABORT); }
+  const int rc = nrtgpu_index_add_keyword_columns((nrtgpu_index*)(intptr_t)ix, cols, n);
+  free(cols);
+  return fail(env, rc);
+}
+/* the bytes of a keyword term into out (at most cap of them); returns the term's length */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_keywordTerm(JNIEnv* env, jclass c, jlong ix, jint column, jint ord,
+                                                                             jobject out, jint cap) {
+  int32_t len = 0;
+  if (fail(env, nrtgpu_index_keyword_term((const nrtgpu_index*)(intptr_t)ix, column, ord, (uint8_t*)ADDR(env, out), cap, &len))) return -1;
+  return len;
+}
+/* a reader-wide keyword term of a searcher (ord -1: the term count of the union is returned) */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherKeywordTerm(JNIEnv* env, jclass c, jlong s, jint column,
+                                                                                     jint ord, jobject out, jint cap) {
+  int32_t len = 0, n_terms = 0;
+  if (fail(env, nrtgpu_searcher_keyword_term((nrtgpu_searcher*)(intptr_t)s, column, ord, (uint8_t*)ADDR(env, out), cap, &len, &n_terms)))
+    return -1;
+  return ord == -1 ? n_terms : len;
+}
 /* phrases / phraseTerms: direct ByteBuffers laid out as nrtgpu_phrase[] / nrtgpu_phrase_term[] (nPhrases 0: searchTree) */
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTreePhrases(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,

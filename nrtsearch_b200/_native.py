@@ -112,6 +112,13 @@ class NestedResult(C.Structure):
                 ("hit_total", C.c_void_p)]
 
 
+class KeywordColumn(C.Structure):
+    """nrtgpu_keyword_column: a keyword column's term dictionary and its per-doc ordinals (SORTED) or CSR of ordinals
+    (SORTED_SET)."""
+    _fields_ = [("n_terms", C.c_int32), ("multi_valued", C.c_int32), ("term_bytes", C.c_void_p), ("term_offsets", C.c_void_p),
+                ("ords", C.c_void_p), ("doc_offsets", C.c_void_p)]
+
+
 class Query(C.Structure):
     _fields_ = [("clause_begin", C.c_int32), ("clause_end", C.c_int32), ("min_should_match", C.c_int32),
                 ("has_after", C.c_int32), ("after_doc", C.c_int32), ("after_score", C.c_float)]
@@ -152,6 +159,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_search_bool_aggs_filtered", "nrtgpu_searcher_search_bool_aggs_filtered",
     "nrtgpu_search_bool_aggs_sorted_hits", "nrtgpu_searcher_search_bool_aggs_sorted_hits",
     "nrtgpu_search_tree_aggs", "nrtgpu_searcher_search_tree_aggs",
+    "nrtgpu_index_add_keyword_columns", "nrtgpu_index_keyword_term", "nrtgpu_searcher_keyword_term",
 ]
 
 _gpu = None
@@ -199,6 +207,10 @@ def gpu_lib() -> C.CDLL:
                                                   C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                   C.POINTER(C.c_void_p)]
         lib.nrtgpu_index_add_positions.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+        lib.nrtgpu_index_add_keyword_columns.argtypes = [C.c_void_p, C.POINTER(KeywordColumn), C.c_int32]
+        lib.nrtgpu_index_keyword_term.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]
+        lib.nrtgpu_searcher_keyword_term.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32),
+                                                     C.POINTER(C.c_int32)]
         lib.nrtgpu_search_tree_phrases.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32,
                                                    C.POINTER(Phrase), C.c_int32, C.POINTER(PhraseTerm), C.c_int32, C.POINTER(Query),
                                                    C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(SearchLimits), C.c_void_p] + \

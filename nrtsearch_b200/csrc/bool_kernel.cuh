@@ -116,8 +116,9 @@ __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolT
 }
 
 // kTree: a tree batch (sm holds the query's nodes, evaluate_doc walks them); otherwise flat BooleanQuerys.
-// kAggs: every matching doc also goes to the collectors of L.aggs (the other instantiations never read it)
-template <bool kTree, bool kAggs>
+// kAggs: every matching doc also goes to the collectors of L.aggs (the other instantiations never read it); kMulti: they
+// count a SORTED_SET keyword column (agg_collect<true>)
+template <bool kTree, bool kAggs, bool kMulti = false>
 __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_constant__ BoolLaunch L) {
   using Smem = typename std::conditional<kTree, BoolTreeSmem, BoolSmem>::type;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -207,7 +208,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
         uint64_t key = 0;
         if (matched) {
           ++my_hits;
-          if constexpr (kAggs) agg_collect(*L.aggs, L.ix, qi, doc, score);   // additional collectors see every matching doc
+          if constexpr (kAggs) agg_collect<kMulti>(*L.aggs, L.ix, qi, doc, score);   // additional collectors see every matching doc
           key = make_key(score, doc);
           is_cand = key > sm.theta && (!has_after || key < after_key);
         }

@@ -211,6 +211,9 @@ struct AggLaunch {
   const uint32_t* codes[kMaxAggs];   // terms: sort codes of the column (bucket = code / 2 - 1)
   int32_t nested_begin[kMaxAggs + 1];   // terms: nested[nested_begin[i], nested_begin[i + 1]) are aggregation i's
   AggNestedDev nested[kMaxAggs * kMaxNested];
+  // terms over a SORTED_SET keyword column (read by the kMulti instantiations only; last, so that the other members keep
+  // their offsets): doc d's value codes are codes[i][offsets[i][d], offsets[i][d + 1]); NULL: one code per doc
+  const int64_t* offsets[kMaxAggs];
 };
 
 __device__ __forceinline__ unsigned long long double_to_ordered(double d) {
@@ -260,13 +263,35 @@ __device__ __noinline__ void agg_nested_collect(const AggLaunch& A, int i, const
   }
 }
 
-// called by the posting kernels for every matching doc of query q (score: its score under a relevance sort)
+// terms aggregation i over a SORTED_SET keyword column for a matching doc: the doc counts once in the bucket of each of its
+// terms and is handed to the nested collectors once per term (OrdinalTermsCollectorManager: nestedLeafCollectors.collect(
+// globalOrd, doc) per ord). A doc's terms are distinct, so no bucket sees a doc twice.
+__device__ __forceinline__ void agg_collect_values(const AggLaunch& A, int i, const DevIndexView& ix, int q, int32_t doc, float score) {
+  const AggSpecDev& s = A.a[i];
+  const bool nested = A.nested_begin[i + 1] > A.nested_begin[i];
+  const uint32_t* codes = A.codes[i];
+  for (int64_t v = A.offsets[i][doc], e = A.offsets[i][doc + 1]; v < e; ++v) {
+    const uint32_t code = codes[v];
+    if (!code) continue;   // (a value whose doc a filter's row gates out)
+    const size_t cell = (size_t)q * s.n_buckets + (code >> 1) - 1;
+    if (s.counts) atomicAdd(&s.counts[cell], 1u);   // (NULL in the top-hits run)
+    if (nested) agg_nested_collect(A, i, ix, q, cell, doc, score);
+  }
+}
+
+// called by the posting kernels for every matching doc of query q (score: its score under a relevance sort). kMulti: the
+// launch carries a SORTED_SET keyword terms aggregation (A.offsets); only the kMulti kernel instantiations read A.offsets,
+// so the others run the code they ran before keyword columns.
+template <bool kMulti = false>
 __device__ __forceinline__ void agg_collect(const AggLaunch& A, const DevIndexView& ix, int q, int32_t doc, float score) {
   for (int i = 0; i < A.n_aggs; ++i) {
     const AggSpecDev& s = A.a[i];
     if (s.kind == NRTGPU_AGG_TERMS) {
       const uint8_t* has = ix.col_has[s.column];
       if (has && !has[doc]) continue;
+      if constexpr (kMulti) {
+        if (A.offsets[i]) { agg_collect_values(A, i, ix, q, doc, score); continue; }
+      }
       const uint32_t code = A.codes[i][doc];
       if (!code) continue;
       const size_t cell = (size_t)q * s.n_buckets + (code >> 1) - 1;
@@ -292,8 +317,8 @@ __global__ void dict_map_kernel(const uint64_t* __restrict__ leaf, int32_t n_lea
   map[i] = (uint32_t)lo;
 }
 // a leaf's codes through that map: 2b + 2 -> 2 map[b] + 2; 0 (no value) stays 0
-__global__ void dict_remap_kernel(const uint32_t* __restrict__ codes, int32_t n, const uint32_t* __restrict__ map, uint32_t* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void dict_remap_kernel(const uint32_t* __restrict__ codes, int64_t n, const uint32_t* __restrict__ map, uint32_t* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t c = codes[i];
   out[i] = c ? 2u * map[(c >> 1) - 1] + 2u : 0u;
@@ -318,7 +343,7 @@ __host__ __device__ __forceinline__ double agg_word_value(int kind, unsigned lon
 // (TermsCollectorManager.fillBucketResultByCount :430-480), bucket keys as column values
 struct AggTermsLaunch {
   const unsigned int* counts; int32_t n_buckets, nq, size, order_desc;
-  const uint64_t* distinct;   // sorted distinct values (sortable u64) of the column
+  const uint64_t* distinct;   // sorted distinct values (sortable u64) of the column; NULL: keys are the buckets (keyword ordinals)
   int64_t* out_keys; int32_t* out_counts;   // [nq][size]
   int32_t* out_n;             // [nq] buckets returned
   int32_t* out_total_buckets; // [nq] non-empty buckets
@@ -367,7 +392,7 @@ __global__ void __launch_bounds__(256) agg_terms_topk_kernel(AggTermsLaunch T) {
     if (i < n_out) {
       const uint32_t hi = (uint32_t)(keys[i] >> 32), bkt = ~(uint32_t)keys[i];
       cnt = (int32_t)(T.order_desc ? hi : ~hi);
-      key = (int64_t)(T.distinct[bkt] ^ 0x8000000000000000ull);
+      key = T.distinct ? (int64_t)(T.distinct[bkt] ^ 0x8000000000000000ull) : (int64_t)bkt;
     }
     T.out_keys[(size_t)q * T.size + i] = key; T.out_counts[(size_t)q * T.size + i] = cnt;
     if (T.out_bucket) T.out_bucket[(size_t)q * T.size + i] = i < n_out ? (int32_t)~(uint32_t)keys[i] : -1;
@@ -445,7 +470,7 @@ __global__ void __launch_bounds__(256) agg_terms_by_value_kernel(AggTermsLaunch 
     if (i < n_out) {
       bkt = (int32_t)~tags[i];
       cnt = (int32_t)row[bkt];
-      key = (int64_t)(T.distinct[bkt] ^ 0x8000000000000000ull);
+      key = T.distinct ? (int64_t)(T.distinct[bkt] ^ 0x8000000000000000ull) : (int64_t)bkt;
     }
     T.out_keys[(size_t)q * T.size + i] = key; T.out_counts[(size_t)q * T.size + i] = cnt;
     if (T.out_bucket) T.out_bucket[(size_t)q * T.size + i] = bkt;

@@ -160,6 +160,16 @@ __global__ void agg_row_codes_kernel(const uint32_t* __restrict__ row, const uin
   out[i] = ((row[i >> 5] >> (i & 31)) & 1u) ? (src ? src[i] : 2u) : 0u;
 }
 
+// agg_row_codes_kernel for a terms aggregation over a SORTED_SET keyword column: each value of a doc keeps its code (src,
+// value-indexed through the doc offsets off) where the doc's row passes, 0 elsewhere
+__global__ void agg_row_value_codes_kernel(const uint32_t* __restrict__ row, const uint32_t* __restrict__ src,
+                                           const int64_t* __restrict__ off, int32_t n_docs, uint32_t* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_docs) return;
+  const bool pass = (row[i >> 5] >> (i & 31)) & 1u;
+  for (int64_t v = off[i]; v < off[i + 1]; ++v) out[v] = pass ? src[v] : 0u;
+}
+
 struct KnnFilterOrdsLaunch {
   const uint32_t* rows; int words;
   const int32_t* grows;         // rows to compact: grows[blockIdx.y]

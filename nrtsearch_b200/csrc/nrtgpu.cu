@@ -131,6 +131,19 @@ struct DevBuf {
 
 }  // namespace
 
+// A keyword column of an image (nrtgpu_index_add_keyword_columns): its term dictionary on the host, and on the device the
+// bucket code 2i + 2 of ordinal i (0: no value) per doc (SORTED) or per value with the doc offsets (SORTED_SET, counted by
+// the kMulti kernel instantiations: agg_collect_values)
+struct KeywordColumn {
+  int32_t n_terms = 0;
+  bool multi = false;
+  int64_t n_values = 0;               // length of codes
+  std::vector<uint8_t> bytes;         // the dictionary: term t is bytes[off[t], off[t + 1])
+  std::vector<int64_t> off;
+  DevBuf<uint32_t> codes;             // [n_values]
+  DevBuf<int64_t> doc_off;            // SORTED_SET: [n_docs + 1]
+};
+
 struct nrtgpu_ctx {
   int device = 0;
   std::mutex hyb_mu;             // O(k) hybrid stages share one pooled device scratch (no cudaMalloc per call)
@@ -188,6 +201,9 @@ struct nrtgpu_index {
   std::vector<std::unique_ptr<DevBuf<int64_t>>> colmv_off;   // multi-valued columns: per-doc offsets (values sit in col64)
   DevBuf<const int64_t*> colmv_off_ptrs, colmv_val_ptrs;
   std::vector<uint8_t> col_multi;                            // [n_columns] 1 = multi-valued
+  std::vector<std::unique_ptr<KeywordColumn>> kw;            // keyword columns (nrtgpu_index_add_keyword_columns)
+  std::vector<int32_t> kw_n_terms;
+  bool kw_added = false;
   DevBuf<uint32_t> live_bits;
   // vectors
   int32_t vec_dims = 0, vec_sim = 0, vec_count = 0;
@@ -236,6 +252,7 @@ struct nrtgpu_index {
     d.term_plane = term_plane.data(); d.term_gran = term_gran.data(); d.field_doc_count = field_doc_count.data();
     d.col_multi = col_multi.data(); d.col_n_distinct = col_n_distinct.data(); d.has_deletes = live_bits.p != nullptr;
     d.has_positions = has_positions;
+    d.n_keyword = (int32_t)kw.size(); d.kw_n_terms = kw_n_terms.data();
     return d;
   }
   KnnCorpus knn_corpus() const {   // what the kNN stages read; NRTGPU_KNN_SIMT, read on every call, forces the fp32 SIMT stage
@@ -266,8 +283,9 @@ struct AggTables {
   unsigned int* counts[kMaxAggs];
   unsigned long long* dvals[kMaxAggs];
   const uint32_t* codes[kMaxAggs];
+  const int64_t* offsets[kMaxAggs];   // SORTED_SET keyword terms: the doc offsets of codes (NULL: one code per doc)
   int32_t n_buckets[kMaxAggs];
-  const uint64_t* distinct[kMaxAggs];
+  const uint64_t* distinct[kMaxAggs];  // NULL for keyword terms: bucket keys are ordinals
   unsigned long long* nest_words[kMaxAggs * kMaxNested];
 };
 
@@ -421,6 +439,12 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<false, false, v3::kCtasA, v3::kStageA, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)sizeof(v3::ProbeSmemT<v3::kStageA>)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<false, false, v3::kCtasB, v3::kStageB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)sizeof(v3::ProbeSmemT<v3::kStageB>)));
 #define NRT_PROBE_ATTR(S, D) \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasA, v3::kStageA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageA>))); \
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<S, D, v3::kCtasB, v3::kStageB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(v3::ProbeSmemT<v3::kStageB>)));
@@ -736,6 +760,54 @@ int nrtgpu_index_add_positions(nrtgpu_index* ix, const int32_t* positions, int64
   return NRTGPU_OK;
 }
 
+int nrtgpu_index_add_keyword_columns(nrtgpu_index* ix, const nrtgpu_keyword_column* cols, int32_t n) {
+  if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_keyword_columns: NULL index");
+  if (ix->kw_added) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_keyword_columns: the image already has its keyword columns");
+  int rc;
+  if ((rc = check_keyword_columns(ix->n_docs, cols, n))) return rc;
+  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
+  std::vector<std::unique_ptr<KeywordColumn>> kw;
+  int64_t bytes = 0;
+  for (int32_t k = 0; k < n; ++k) {   // built aside: a failure leaves the image as it was
+    const nrtgpu_keyword_column& c = cols[k];
+    std::unique_ptr<KeywordColumn> x(new KeywordColumn);
+    x->n_terms = c.n_terms; x->multi = c.multi_valued != 0;
+    x->n_values = x->multi ? c.doc_offsets[ix->n_docs] : ix->n_docs;
+    x->off.assign(c.term_offsets, c.term_offsets + c.n_terms + 1);
+    if (c.term_offsets[c.n_terms] > 0) x->bytes.assign(c.term_bytes, c.term_bytes + c.term_offsets[c.n_terms]);
+    std::vector<uint32_t> code((size_t)x->n_values);
+    for (int64_t v = 0; v < x->n_values; ++v) code[(size_t)v] = c.ords[v] < 0 ? 0u : 2u * (uint32_t)c.ords[v] + 2u;
+    if ((rc = x->codes.alloc(std::max<size_t>(code.size(), 1)))) return rc;   // (one word at least: a column without values)
+    if (!code.empty()) NRT_CUDA_TRY(cudaMemcpy(x->codes.p, code.data(), code.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    x->codes.n = code.size();
+    if (x->multi && (rc = x->doc_off.upload(c.doc_offsets, (size_t)ix->n_docs + 1))) return rc;
+    bytes += (int64_t)(x->codes.bytes() + x->doc_off.bytes());
+    kw.push_back(std::move(x));
+  }
+  ix->kw = std::move(kw);
+  for (auto& x : ix->kw) ix->kw_n_terms.push_back(x->n_terms);
+  ix->kw_added = true;
+  ix->device_bytes += bytes;
+  return NRTGPU_OK;
+}
+
+// the bytes of term `ord` of a host dictionary (bytes, off) into out (min(len, cap) of them), its length into *len
+static void copy_term(const std::vector<uint8_t>& bytes, const std::vector<int64_t>& off, int32_t ord, uint8_t* out, int32_t cap,
+                      int32_t* len) {
+  const int64_t a = off[(size_t)ord], l = off[(size_t)ord + 1] - a;
+  *len = (int32_t)l;
+  if (out && cap > 0 && l > 0) std::memcpy(out, bytes.data() + a, (size_t)std::min<int64_t>(l, cap));
+}
+
+int nrtgpu_index_keyword_term(const nrtgpu_index* ix, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len) {
+  if (!ix || !len) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_term: NULL argument");
+  if (column < 0 || (size_t)column >= ix->kw.size()) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_term: keyword column out of range");
+  const KeywordColumn& c = *ix->kw[(size_t)column];
+  if (ord < 0 || ord >= c.n_terms) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_term: ordinal out of range");
+  copy_term(c.bytes, c.off, ord, out, cap, len);
+  return NRTGPU_OK;
+}
+
 int nrtgpu_index_set_live_docs(nrtgpu_index* ix, const uint8_t* live_docs) {
   if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_set_live_docs: NULL index");
   NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
@@ -946,13 +1018,20 @@ static v3::ProbeLaunch probe_params(nrtgpu_batch* b) {
 }
 
 // the probe kernel over the batch's work items: the simple ones, then the generic ones (queue heads work_counter[0], [1])
-static int probe_launch(nrtgpu_batch* b, v3::ProbeLaunch P, bool debug, cudaStream_t st) {
+// multi: the collectors count a SORTED_SET keyword column, so the generic items run the kMulti instantiation (without the
+// profiling counters)
+static int probe_launch(nrtgpu_batch* b, v3::ProbeLaunch P, bool debug, bool multi, cudaStream_t st) {
   // configuration A (3 CTAs / SM) for the pruned sweeps of TOP_SCORES, B (4 CTAs / SM) where every posting is visited
   const bool cfg_b_simple = ix_ctx_probe_cfg(b->ix->ctx, P.threshold >= (int64_t)INT32_MAX);
   const bool cfg_b_generic = ix_ctx_probe_cfg(b->ix->ctx, true);
   auto launch = [&](auto simple_tag, bool cfg_b, int n_items) {
     constexpr bool S = decltype(simple_tag)::value;
-    if (cfg_b) {
+    if (!S && multi) {
+      const int ctas = cfg_b ? v3::kCtasB : v3::kCtasA;
+      const int grid = std::min(ctas * b->ix->ctx->plan.sm_count, n_items);
+      if (cfg_b) v3::posting_probe_kernel<false, false, v3::kCtasB, v3::kStageB, true><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
+      else v3::posting_probe_kernel<false, false, v3::kCtasA, v3::kStageA, true><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageA>), st>>>(P);
+    } else if (cfg_b) {
       const int grid = std::min(v3::kCtasB * b->ix->ctx->plan.sm_count, n_items);
       if (debug) v3::posting_probe_kernel<S, true, v3::kCtasB, v3::kStageB><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
       else v3::posting_probe_kernel<S, false, v3::kCtasB, v3::kStageB><<<grid, v3::kThreads, sizeof(v3::ProbeSmemT<v3::kStageB>), st>>>(P);
@@ -981,15 +1060,15 @@ static int probe_launch(nrtgpu_batch* b, v3::ProbeLaunch P, bool debug, cudaStre
 // additional collectors `aggs` (device pointer, NULL: none). Pass 1 (p2_total NULL) counts into the batch's own totalHits and
 // flags under its limits. The top-hits run of batch_nested_top_hits counts totalHits into p2_total and the probe kernel's
 // pruned / terminated into p2_flags [2 * nq], without deadline or terminateAfter; the caller has reset the engine's theta,
-// slice counts and queue heads.
-static int batch_engine_launch(nrtgpu_batch* b, const AggLaunch* aggs, unsigned long long* p2_total, int32_t* p2_flags, bool debug,
-                               cudaStream_t st) {
+// slice counts and queue heads. multi: a collector counts a SORTED_SET keyword column (the kMulti instantiations).
+static int batch_engine_launch(nrtgpu_batch* b, const AggLaunch* aggs, bool multi, unsigned long long* p2_total, int32_t* p2_flags,
+                               bool debug, cudaStream_t st) {
   const bool p2 = p2_total != nullptr;
   if (!b->cb.wide) {
     v3::ProbeLaunch P = probe_params(b);
     P.aggs = aggs;
     if (p2) { P.total_hits = p2_total; P.pruned = p2_flags; P.terminated = p2_flags + b->nq; P.deadline_ns = 0; P.terminate_after = 0; }
-    return probe_launch(b, P, debug && !p2, st);
+    return probe_launch(b, P, debug && !p2, multi, st);
   }
   BoolLaunch L;
   L.ix = b->ix->view();
@@ -1004,10 +1083,12 @@ static int batch_engine_launch(nrtgpu_batch* b, const AggLaunch* aggs, unsigned 
   const unsigned grid = (unsigned)b->plan.n_work();
   if (b->cb.tree) {
     L.nodes = b->nodes.p; L.node_begin = b->node_begin.p; L.phrases = b->phrases.p; L.phrase_begin = b->phrase_begin.p;
-    if (aggs) bool_window_kernel<true, true><<<grid, kThreads, sizeof(BoolTreeSmem), st>>>(L);
+    if (multi) bool_window_kernel<true, true, true><<<grid, kThreads, sizeof(BoolTreeSmem), st>>>(L);
+    else if (aggs) bool_window_kernel<true, true><<<grid, kThreads, sizeof(BoolTreeSmem), st>>>(L);
     else bool_window_kernel<true, false><<<grid, kThreads, sizeof(BoolTreeSmem), st>>>(L);
   } else {
-    if (aggs) bool_window_kernel<false, true><<<grid, kThreads, sizeof(BoolSmem), st>>>(L);
+    if (multi) bool_window_kernel<false, true, true><<<grid, kThreads, sizeof(BoolSmem), st>>>(L);
+    else if (aggs) bool_window_kernel<false, true><<<grid, kThreads, sizeof(BoolSmem), st>>>(L);
     else bool_window_kernel<false, false><<<grid, kThreads, sizeof(BoolSmem), st>>>(L);
   }
   NRT_CUDA_TRY(cudaGetLastError());
@@ -1062,9 +1143,14 @@ static int batch_agg_codes(nrtgpu_batch* b, cudaStream_t st) {
     const uint32_t* row = b->agg_gate[i];
     if (!row) continue;
     const int32_t n = b->ix->n_docs;
-    if (int rc = b->agg_fcodes[i].alloc((size_t)n)) return rc;
-    agg_row_codes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(row, b->cb.aggs[i].kind == NRTGPU_AGG_FILTER ? nullptr : b->agg_tab.codes[i],
-                                                                    n, b->agg_fcodes[i].p);
+    if (const int64_t* off = b->agg_tab.offsets[i]) {   // SORTED_SET keyword terms: every value of a passing doc
+      if (int rc = b->agg_fcodes[i].alloc((size_t)std::max<int64_t>(b->ix->kw[(size_t)b->cb.aggs[i].column]->n_values, 1))) return rc;
+      agg_row_value_codes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(row, b->agg_tab.codes[i], off, n, b->agg_fcodes[i].p);
+    } else {
+      if (int rc = b->agg_fcodes[i].alloc((size_t)n)) return rc;
+      agg_row_codes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(row, b->cb.aggs[i].kind == NRTGPU_AGG_FILTER ? nullptr : b->agg_tab.codes[i],
+                                                                      n, b->agg_fcodes[i].p);
+    }
     NRT_CUDA_TRY(cudaGetLastError());
     b->agg_codes[i] = b->agg_fcodes[i].p;
   }
@@ -1096,6 +1182,11 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
       const int32_t c = b->cb.aggs[i].column;
       nb[i] = 1;   // (a filter's one bucket)
       if (b->cb.aggs[i].kind != NRTGPU_AGG_TERMS) continue;
+      if (agg_keyword(b->cb.aggs[i])) {   // ordinals of the image's dictionary
+        const KeywordColumn& k = *b->ix->kw[(size_t)c];
+        nb[i] = k.n_terms; t.codes[i] = k.codes.p; t.offsets[i] = k.doc_off.p;
+        continue;
+      }
       nb[i] = b->ix->col_n_distinct[(size_t)c];
       t.codes[i] = ix_col_code(b->ix, c); t.distinct[i] = ix_col_distinct(b->ix, c);
     }
@@ -1106,6 +1197,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
   NRT_CUDA_TRY(cudaEventRecord(ev[0], st));
   if (b->plan.n_work() > 0) {
     const AggLaunch* aggs = nullptr;
+    bool multi = false;   // a SORTED_SET keyword terms aggregation
     if (!b->cb.aggs.empty()) {   // pass 1 of the collectors, on either engine
       const AggTables& t = b->agg_tab;
       if ((rc_dbg = batch_agg_codes(b, st))) return rc_dbg;
@@ -1117,6 +1209,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
         if (a.kind == NRTGPU_AGG_FILTER) {   // a one-bucket terms aggregation over the image's column without a has array
           A.a[i].kind = NRTGPU_AGG_TERMS; A.a[i].column = b->ix->n_columns;
         }
+        if (agg_keyword(a)) { A.a[i].column = b->ix->n_columns; A.offsets[i] = t.offsets[i]; }   // (codes alone say which docs have a term)
         if (a.kind == NRTGPU_AGG_TERMS || a.kind == NRTGPU_AGG_FILTER) {
           A.a[i].n_buckets = t.n_buckets[i];
           A.a[i].counts = t.counts[i]; A.codes[i] = b->agg_codes[i];
@@ -1130,6 +1223,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
           AggNestedDev& d = A.nested[A.nested_begin[i + 1]++];
           d.kind = n.kind; d.column = n.column; d.value_type = n.value_type; d.dvals = t.nest_words[j];
         }
+        multi |= A.offsets[i] != nullptr;
       }
       if ((rc_dbg = b->agg_launch.upload_async(&A, 1, st))) return rc_dbg;
       NRT_CUDA_TRY(cudaStreamSynchronize(st));   // A is a stack object
@@ -1139,7 +1233,7 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
       if (!b->probe_stats.p && (rc_dbg = b->probe_stats.alloc(2 * v3::kProbeStats))) return rc_dbg;
       NRT_CUDA_TRY(cudaMemsetAsync(b->probe_stats.p, 0, 2 * v3::kProbeStats * sizeof(unsigned long long), st));
     }
-    if ((rc_dbg = batch_engine_launch(b, aggs, nullptr, nullptr, debug, st))) return rc_dbg;
+    if ((rc_dbg = batch_engine_launch(b, aggs, multi, nullptr, nullptr, debug, st))) return rc_dbg;
   }
   NRT_CUDA_TRY(cudaEventRecord(ev[1], st));
   if (debug && b->probe_stats.p && !b->cb.wide) {
@@ -1354,10 +1448,11 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
         AggLaunch& A = launches[(size_t)l];
         std::memset(&A, 0, sizeof(A));
         A.n_aggs = 1;
-        A.a[0].kind = NRTGPU_AGG_TERMS; A.a[0].column = a.kind == NRTGPU_AGG_FILTER ? x->ix->n_columns : a.column;
+        A.a[0].kind = NRTGPU_AGG_TERMS; A.a[0].column = a.kind == NRTGPU_AGG_FILTER || agg_keyword(a) ? x->ix->n_columns : a.column;
         A.a[0].value_type = a.value_type;
         A.a[0].n_buckets = x->agg_tab.n_buckets[parent];
         A.codes[0] = x->agg_codes[parent];   // the codes pass 1 counted through; counts stay NULL: the pass-1 tables are not touched
+        A.offsets[0] = x->agg_tab.offsets[parent];
         A.nested_begin[1] = n_th;
         for (int k = 0; k < n_th; ++k) {
           AggNestedDev& d = A.nested[k];
@@ -1372,7 +1467,7 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
         if (x->work_counter.p) NRT_CUDA_TRY(cudaMemsetAsync(x->work_counter.p, 0, x->work_counter.bytes(), st));   // (probe batches)
         NRT_CUDA_TRY(cudaMemsetAsync(b->p2_total.p, 0, b->p2_total.bytes(), st));
         NRT_CUDA_TRY(cudaMemsetAsync(b->p2_flags.p, 0, b->p2_flags.bytes(), st));
-        if ((rc = batch_engine_launch(x, x->nest_launch.p, b->p2_total.p, b->p2_flags.p, false, st))) return rc;
+        if ((rc = batch_engine_launch(x, x->nest_launch.p, A.offsets[0] != nullptr, b->p2_total.p, b->p2_flags.p, false, st))) return rc;
       }
       for (int k = 0; k < n_th && merge; ++k) {   // this leaf's best top_hits of each list, by its order, into its record
         const nrtgpu_sort_order* o = order_of(k, l);
@@ -2623,9 +2718,12 @@ int nrtgpu_rescore_combine(nrtgpu_ctx* ctx, int32_t nq, int32_t n_hits, const in
 // The reader-wide value dictionary of one column (collect_kernel.cuh, dict_map_kernel): the sorted union of the leaves'
 // distinct values, and per leaf the codes that number its docs' values in it. A leaf whose dictionary is the union, or
 // which holds no value, counts through its own col_code; every other leaf through a renumbered copy (4 B per doc).
+// A keyword column's reader-wide dictionary is the byte-order union of the leaves' term dictionaries, built on the host
+// (bytes / off); values stays empty, and a leaf's codes (per doc or per value) are renumbered through its ordinal map.
 struct ReaderDict {
   DevBuf<uint64_t> values;   // [n] ascending, the sortable domain of col_distinct
   int32_t n = 0;
+  std::vector<uint8_t> bytes; std::vector<int64_t> off;   // keyword columns: term g of the union is bytes[off[g], off[g + 1])
   std::vector<std::unique_ptr<DevBuf<uint32_t>>> own;   // per leaf: the renumbered codes (unallocated where col_code serves)
   std::vector<const uint32_t*> codes;                   // per leaf: the codes its docs count through
 };
@@ -2639,7 +2737,55 @@ struct nrtgpu_searcher {
   // per aggregated column, built by its first aggregation and kept for the searcher's life: leaf columns never change
   // (set_live_docs and update_stats leave them alone, and a dictionary keeps the values of deleted docs)
   std::map<int32_t, std::unique_ptr<ReaderDict>> dicts;
+  std::map<int32_t, std::unique_ptr<ReaderDict>> kw_dicts;   // the same per keyword column
 };
+
+// the reader-wide dictionary of keyword column `column` (built on `st` the first time it is asked for); the caller checked
+// that every leaf has the column
+static int searcher_kw_dict(nrtgpu_searcher* s, int32_t column, cudaStream_t st, const ReaderDict** out) {
+  auto it = s->kw_dicts.find(column);
+  if (it != s->kw_dicts.end()) { *out = it->second.get(); return NRTGPU_OK; }
+  std::unique_ptr<ReaderDict> d(new ReaderDict);
+  auto term = [](const KeywordColumn& c, int32_t t) {
+    return std::string(reinterpret_cast<const char*>(c.bytes.data()) + c.off[(size_t)t], (size_t)(c.off[(size_t)t + 1] - c.off[(size_t)t]));
+  };
+  std::vector<std::string> uni;   // std::string compares as unsigned bytes, then length: BytesRef order
+  for (const nrtgpu_index* ix : s->leaves) {
+    const KeywordColumn& c = *ix->kw[(size_t)column];
+    for (int32_t t = 0; t < c.n_terms; ++t) uni.push_back(term(c, t));
+  }
+  std::sort(uni.begin(), uni.end());
+  uni.erase(std::unique(uni.begin(), uni.end()), uni.end());
+  if (uni.size() > (size_t)INT32_MAX / 2) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "keyword terms: more than 2^30 terms over the leaves");
+  d->n = (int32_t)uni.size();
+  d->off.assign(1, 0);
+  for (const std::string& x : uni) { d->bytes.insert(d->bytes.end(), x.begin(), x.end()); d->off.push_back((int64_t)d->bytes.size()); }
+  DevBuf<uint32_t> map;
+  int rc;
+  for (const nrtgpu_index* ix : s->leaves) {
+    const KeywordColumn& c = *ix->kw[(size_t)column];
+    d->own.emplace_back(new DevBuf<uint32_t>);
+    const int64_t n_codes = c.n_values;
+    if (c.n_terms == d->n || c.n_terms == 0 || n_codes == 0) { d->codes.push_back(c.codes.p); continue; }   // already reader-wide, or all 0
+    std::vector<uint32_t> m((size_t)c.n_terms);
+    for (int32_t t = 0; t < c.n_terms; ++t) m[(size_t)t] = (uint32_t)(std::lower_bound(uni.begin(), uni.end(), term(c, t)) - uni.begin());
+    DevBuf<uint32_t>& own = *d->own.back();
+    if ((rc = map.upload_async(m.data(), m.size(), st)) || (rc = own.alloc((size_t)n_codes))) return rc;
+    dict_remap_kernel<<<(unsigned)((n_codes + 255) / 256), 256, 0, st>>>(c.codes.p, n_codes, map.p, own.p);   // (per doc or per value)
+    NRT_CUDA_TRY(cudaGetLastError());
+    NRT_CUDA_TRY(cudaStreamSynchronize(st));   // the map (and m) are reused by the next leaf
+    d->codes.push_back(own.p);
+  }
+  *out = d.get();
+  s->kw_dicts[column] = std::move(d);
+  return NRTGPU_OK;
+}
+
+// whether every leaf of s has keyword column `column`
+static bool searcher_has_kw(const nrtgpu_searcher* s, int32_t column) {
+  for (const nrtgpu_index* ix : s->leaves) if (column < 0 || (size_t)column >= ix->kw.size()) return false;
+  return true;
+}
 
 static int32_t ix_n_distinct(const nrtgpu_index* ix, int32_t c) {
   return (size_t)c < ix->col_n_distinct.size() ? ix->col_n_distinct[(size_t)c] : 0;
@@ -2795,6 +2941,22 @@ int nrtgpu_searcher_create(nrtgpu_ctx* ctx, nrtgpu_index* const* leaves, int32_t
 }
 
 int nrtgpu_searcher_close(nrtgpu_searcher* s) { delete s; return NRTGPU_OK; }
+
+int nrtgpu_searcher_keyword_term(nrtgpu_searcher* s, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len,
+                                 int32_t* n_terms) {
+  if (!s || !len) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_keyword_term: NULL argument");
+  if (!searcher_has_kw(s, column)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_keyword_term: keyword column out of range");
+  NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
+  std::lock_guard<std::mutex> g(s->mu);
+  const ReaderDict* d = nullptr;
+  if (int rc = searcher_kw_dict(s, column, nullptr, &d)) return rc;
+  if (n_terms) *n_terms = d->n;
+  *len = 0;
+  if (ord == -1 && n_terms) return NRTGPU_OK;
+  if (ord < 0 || ord >= d->n) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_keyword_term: ordinal out of range");
+  copy_term(d->bytes, d->off, ord, out, cap, len);
+  return NRTGPU_OK;
+}
 
 int nrtgpu_searcher_search_bool(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
                                 const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold,
@@ -3016,7 +3178,8 @@ static int searcher_aggs(nrtgpu_searcher* s, const char* fn, const BatchRequest&
   for (int i = 0; i < n_aggs; ++i) {
     n_buckets[i] = 1;   // (a filter's one bucket)
     if (aggs[i].kind != NRTGPU_AGG_TERMS) continue;
-    if ((rc = searcher_dict(s, aggs[i].column, st, &dict[i]))) return rc;
+    if ((rc = agg_keyword(aggs[i]) ? searcher_kw_dict(s, aggs[i].column, st, &dict[i]) : searcher_dict(s, aggs[i].column, st, &dict[i])))
+      return rc;
     n_buckets[i] = dict[i]->n;
     if ((int64_t)nq * n_buckets[i] * 4 > (2ll << 30))
       NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "terms aggregation: batch x distinct values exceeds the 2 GB count table");
@@ -3041,7 +3204,13 @@ static int searcher_aggs(nrtgpu_searcher* s, const char* fn, const BatchRequest&
     AggTables& x = bs[(size_t)l]->agg_tab;
     x = t;
     for (int i = 0; i < n_aggs; ++i)
-      if (dict[i]) { x.codes[i] = dict[i]->codes[(size_t)l]; x.distinct[i] = dict[i]->values.p; }
+      if (dict[i]) {
+        x.codes[i] = dict[i]->codes[(size_t)l]; x.distinct[i] = dict[i]->values.p;
+        if (agg_keyword(aggs[i])) {   // reader-wide ordinals, per doc (SORTED) or per value behind the leaf's doc offsets
+          x.distinct[i] = nullptr;
+          x.offsets[i] = s->leaves[(size_t)l]->kw[(size_t)aggs[i].column]->doc_off.p;
+        }
+      }
     bs[(size_t)l]->agg_shared = true;
   }
   for (int l = 0; l < n_leaves; ++l)

@@ -302,7 +302,8 @@ __device__ __noinline__ void count_role_stats(const ProbeLaunch& L, const SM& sm
 }
 
 // kStats: the profiling instantiation (NRTGPU_DEBUG_MODES=1) keeps cycle counters; the production one has none of their registers
-template <bool kSimple, bool kStats, int kCtas, int kStageT>
+// kMulti: the generic instantiation for launches whose collectors count a SORTED_SET keyword column (agg_collect<true>)
+template <bool kSimple, bool kStats, int kCtas, int kStageT, bool kMulti = false>
 __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __grid_constant__ ProbeLaunch L) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   using ProbeSmem = ProbeSmemT<kStageT>;
@@ -649,7 +650,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
           float score;
           if (have && evaluate_doc(L, sm, d, e.y, &score)) {
             ++my_hits;
-            if (L.aggs) agg_collect(*L.aggs, L.ix, qi, d, score);   // additional collectors see every matching doc
+            if (L.aggs) agg_collect<kMulti>(*L.aggs, L.ix, qi, d, score);   // additional collectors see every matching doc
             if (L.sort_kind == NRTGPU_SORT_RELEVANCE || L.sort_kind == kSortScoreRank) {
               entry = make_key(score, d);
               // [score, ...] order: ties by the order's rank, which takes the doc's place; ordered(-s) == ~ordered(s) for reverse

@@ -5,7 +5,7 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass, field
-from typing import List, Optional
+from typing import List, Optional, Sequence
 
 import numpy as np
 
@@ -32,6 +32,60 @@ class TextField:
 
 
 @dataclass
+class KeywordColumn:
+    """String doc values of one keyword field in one leaf (SortedDocValues / SortedSetDocValues): the leaf's term
+    dictionary, strictly ascending in byte order, and each doc's ordinals into it. SORTED (offsets None): ords is
+    int32[n_docs], -1 for a doc without a value. SORTED_SET: offsets is int64[n_docs+1] and ords the flattened ordinals,
+    strictly ascending within a doc (the set Lucene keeps: each term of a doc once)."""
+    terms: List[bytes]
+    ords: np.ndarray
+    offsets: Optional[np.ndarray] = None
+
+    @staticmethod
+    def from_values(values: Sequence, multi_valued: bool) -> "KeywordColumn":
+        """The column of per-doc values as an adaptor reads them from documents: SORTED, a str / bytes or None per doc;
+        SORTED_SET, an iterable of them per doc (repeats collapse, as in SortedSetDocValues)."""
+        enc = [(None if v is None else _utf8(v)) if not multi_valued else sorted({_utf8(x) for x in v}) for v in values]
+        terms = sorted({t for v in enc for t in ([v] if not multi_valued else v) if t is not None})
+        ord_of = {t: i for i, t in enumerate(terms)}
+        if not multi_valued:
+            return KeywordColumn(terms, np.array([-1 if v is None else ord_of[v] for v in enc], np.int32))
+        off = np.zeros(len(enc) + 1, np.int64)
+        np.cumsum([len(v) for v in enc], out=off[1:])
+        return KeywordColumn(terms, np.array([ord_of[t] for v in enc for t in v], np.int32), off)
+
+    @property
+    def multi_valued(self) -> bool:
+        return self.offsets is not None
+
+    def doc_ords(self, doc: int) -> np.ndarray:
+        if self.offsets is None:
+            o = int(self.ords[doc])
+            return np.zeros(0, np.int32) if o < 0 else np.array([o], np.int32)
+        return self.ords[int(self.offsets[doc]):int(self.offsets[doc + 1])]
+
+    def doc_range(self, lo: int, hi: int) -> "KeywordColumn":
+        """The column of docs [lo, hi) as a segment of them holds it: its own dictionary, only the terms present there,
+        ordinals renumbered."""
+        if self.offsets is None:
+            sub = self.ords[lo:hi]
+        else:
+            sub = self.ords[int(self.offsets[lo]):int(self.offsets[hi])]
+        present = np.unique(sub[sub >= 0])
+        remap = np.full(len(self.terms) + 1, -1, np.int32)
+        remap[present] = np.arange(len(present), dtype=np.int32)
+        ords = np.ascontiguousarray(remap[sub], np.int32)
+        terms = [self.terms[int(t)] for t in present]
+        if self.offsets is None:
+            return KeywordColumn(terms, ords)
+        return KeywordColumn(terms, ords, np.ascontiguousarray(self.offsets[lo:hi + 1] - self.offsets[lo]))
+
+
+def _utf8(v) -> bytes:
+    return v.encode("utf-8") if isinstance(v, str) else bytes(v)
+
+
+@dataclass
 class HostShard:
     n_docs: int
     doc_base: int
@@ -53,6 +107,9 @@ class HostShard:
     # term positions (PostingsEnum.POSITIONS): posting after posting, the post_freqs[p] positions of posting p, ascending;
     # None = indexed without positions (PhraseQuery is refused)
     post_positions: Optional[np.ndarray] = None
+    # keyword columns (string doc values, nrtgpu_index_add_keyword_columns); keyword column k is TermsCollector(k, ...,
+    # field_type="keyword")
+    keyword_columns: List[KeywordColumn] = field(default_factory=list)
 
     @property
     def n_terms(self) -> int:
@@ -105,7 +162,8 @@ class HostShard:
                             for i in range(len(self.columns))],
             column_has=[None if h is None else np.ascontiguousarray(h[lo:hi]) for h in self.column_has],
             live_docs=None if self.live_docs is None else np.ascontiguousarray(self.live_docs[lo:hi]),
-            vectors=sub_vec, vec_similarity=self.vec_similarity, vec_docs=sub_vdocs, post_positions=sub_pos)
+            vectors=sub_vec, vec_similarity=self.vec_similarity, vec_docs=sub_vdocs, post_positions=sub_pos,
+            keyword_columns=[k.doc_range(lo, hi) for k in self.keyword_columns])
 
 
 def _ptr(a: Optional[np.ndarray], typ):
@@ -170,6 +228,16 @@ class PinnedDesc:
             d.vec_element_type = 1 if byte_field else 0
             d.vec_docs = _ptr(arr(sh.vec_docs, np.int32), N.i32p)
         self.desc = d
+        # keyword columns (nrtgpu_index_add_keyword_columns, after the build)
+        self.keyword = (N.KeywordColumn * max(len(sh.keyword_columns), 1))()
+        for i, k in enumerate(sh.keyword_columns):
+            toff = np.zeros(len(k.terms) + 1, np.int64)
+            np.cumsum([len(t) for t in k.terms], out=toff[1:])
+            tb = arr(np.frombuffer(b"".join(k.terms) or b"\0", np.uint8), np.uint8)
+            self.keyword[i] = N.KeywordColumn(len(k.terms), 1 if k.multi_valued else 0, tb.ctypes.data, arr(toff, np.int64).ctypes.data,
+                                              arr(k.ords, np.int32).ctypes.data,
+                                              None if k.offsets is None else arr(k.offsets, np.int64).ctypes.data)
+        self.n_keyword = len(sh.keyword_columns)
 
 
 # ---------------------------------------------------------------- synthetic inputs (Appendix B)

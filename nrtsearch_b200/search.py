@@ -223,7 +223,9 @@ class SortFieldCollector:
 @dataclass(frozen=True)
 class TermsCollector:
     """TermsCollector over a numeric doc-value field ({Int,Long,Float,Double}TermsCollectorManager): `size` buckets ordered
-    by count (BucketOrder COUNT, desc by default). nested: up to 4 (name, MinCollector | MaxCollector | SumCollector |
+    by count (BucketOrder COUNT, desc by default). field_type "keyword": column is a keyword column of the shard
+    (HostShard.keyword_columns, OrdinalTermsCollectorManager), a doc of a multi-valued one counts once per term, and the
+    result's "keys" is an object array of str (None past a query's "n"). nested: up to 4 (name, MinCollector | MaxCollector | SumCollector |
     TopHitsCollector) computed per bucket (Collector.nestedCollectors); order_by: the name of a nested min / max / sum
     that orders the buckets instead of the count (BucketOrder by a nested collector, in the order_desc direction)."""
     column: int
@@ -300,7 +302,34 @@ class FilterCollector:
     nested: tuple = ()
 
 
-_VALUE_TYPE = {"int": 0, "long": 0, "float": 1, "double": 2}
+_VALUE_TYPE = {"int": 0, "long": 0, "float": 1, "double": 2, "keyword": 3}
+
+
+def _keyword_keys(collectors: Sequence[object], outs: Sequence[object], term) -> None:
+    """Turns the ordinal keys of keyword terms collectors (and those nested in filter collectors) into str, in place;
+    term(column, ord) -> bytes"""
+    for c, o in zip(collectors, outs):
+        if isinstance(c, TermsCollector) and c.field_type == "keyword":
+            filled = np.arange(o["keys"].shape[1])[None, :] < np.asarray(o["n"])[:, None]
+            ords, at = np.unique(o["keys"][filled], return_inverse=True)   # one lookup per distinct term of the batch
+            names = np.empty(len(ords), object)
+            names[:] = [term(c.column, int(x)).decode("utf-8") for x in ords]
+            keys = np.full(o["keys"].shape, None, object)
+            keys[filled] = names[at.reshape(-1)]
+            o["keys"] = keys
+        elif isinstance(c, FilterCollector):
+            names = [name for name, x in c.nested]
+            _keyword_keys([x for _, x in c.nested], [o[name] for name in names], term)
+
+
+def _term_bytes(fn, *args) -> bytes:
+    """the bytes of one keyword term through nrtgpu_index_keyword_term / nrtgpu_searcher_keyword_term (fn bound to its
+    handle, column and ordinal)"""
+    n = C.c_int32()
+    check(fn(*args, None, 0, C.byref(n)))
+    buf = (C.c_uint8 * max(n.value, 1))()
+    check(fn(*args, buf, n.value, C.byref(n)))
+    return bytes(buf[:n.value])
 
 
 @dataclass
@@ -514,8 +543,22 @@ class GpuIndex:
         self.handle = h
         self.n_docs, self.doc_base = shard.n_docs, shard.doc_base
         self._orders = {}
+        self._terms = {}
         if shard.post_positions is not None:
             self.add_positions(shard.post_positions)
+        if pinned.n_keyword:
+            try:
+                check(self._lib.nrtgpu_index_add_keyword_columns(self.handle, pinned.keyword, pinned.n_keyword))
+            except Exception:   # a refused column: the image built above is freed, not leaked
+                self.close()
+                raise
+
+    def keyword_term(self, column: int, ord_: int) -> bytes:
+        """term `ord_` of keyword column `column` of this image (nrtgpu_index_keyword_term)"""
+        key = (column, ord_)
+        if key not in self._terms:
+            self._terms[key] = _term_bytes(self._lib.nrtgpu_index_keyword_term, self.handle, column, ord_)
+        return self._terms[key]
 
     def add_positions(self, positions: np.ndarray):
         """Term positions of every posting, posting after posting (HostShard.post_positions): what PhraseQuery needs."""
@@ -958,6 +1001,7 @@ class GpuIndexSearcher:
             fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * 1)(self.index.sort_order(fields, stream).value))
             check(self._lib.nrtgpu_search_bool_aggs_sorted_hits(self.index.handle, carr, ncl, qarr, nq, k, 0, *fr.sorted_args,
                                                                 C.c_void_p(stream), *hits))
+            _keyword_keys(additional, fr.outs, self.index.keyword_term)
             return out, fr.outs
         aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         if n_nested:
@@ -966,6 +1010,7 @@ class GpuIndexSearcher:
         else:
             check(self._lib.nrtgpu_search_bool_aggs(self.index.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
                                                     C.c_void_p(stream), *hits))
+        _keyword_keys(additional, outs, self.index.keyword_term)
         return out, outs
 
     def search_tree_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
@@ -981,6 +1026,7 @@ class GpuIndexSearcher:
         check(self._lib.nrtgpu_search_tree_aggs(self.index.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k, 0,
                                                 *fr.sorted_args, C.c_void_p(stream), out.docs.ctypes.data, out.scores.ctypes.data,
                                                 out.counts.ctypes.data, out.total_hits.ctypes.data))
+        _keyword_keys(additional, fr.outs, self.index.keyword_term)
         return out, fr.outs
 
     def score_docs(self, queries: Sequence[object], docs: np.ndarray, counts: Optional[np.ndarray] = None, stream: int = 0):
@@ -1082,6 +1128,15 @@ class GpuLeafSearcher:
         h = C.c_void_p()
         check(self._lib.nrtgpu_searcher_create(ctx.handle, arr, len(leaves), C.byref(h)))
         self.handle, self.leaves = h, list(leaves)
+        self._terms = {}
+
+    def keyword_term(self, column: int, ord_: int) -> bytes:
+        """reader-wide term `ord_` of keyword column `column`: the byte-order union of the leaves' dictionaries
+        (nrtgpu_searcher_keyword_term)"""
+        key = (column, ord_)
+        if key not in self._terms:
+            self._terms[key] = _term_bytes(lambda *a: self._lib.nrtgpu_searcher_keyword_term(*a, None), self.handle, column, ord_)
+        return self._terms[key]
 
     def search_batch(self, queries: Sequence[object], collector: RelevanceCollector, stream: int = 0,
                      search_after: Optional[Sequence[Optional[ScoreDoc]]] = None) -> BatchResult:
@@ -1195,12 +1250,14 @@ class GpuLeafSearcher:
                                                                          C.c_void_p(stream), out.docs.ctypes.data,
                                                                          out.scores.ctypes.data, out.counts.ctypes.data,
                                                                          out.total_hits.ctypes.data))
+            _keyword_keys(additional, fr.outs, self.keyword_term)
             return out, fr.outs
         aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         check(self._lib.nrtgpu_searcher_search_bool_aggs_nested(self.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
                                                                 narr, n_nested, nres, C.c_void_p(stream), out.docs.ctypes.data,
                                                                 out.scores.ctypes.data, out.counts.ctypes.data,
                                                                 out.total_hits.ctypes.data))
+        _keyword_keys(additional, outs, self.keyword_term)
         return out, outs
 
     def search_tree_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
@@ -1216,6 +1273,7 @@ class GpuLeafSearcher:
         check(self._lib.nrtgpu_searcher_search_tree_aggs(self.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k, 0,
                                                          *fr.sorted_args, C.c_void_p(stream), out.docs.ctypes.data,
                                                          out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data))
+        _keyword_keys(additional, fr.outs, self.keyword_term)
         return out, fr.outs
 
     def close(self):
