@@ -178,6 +178,12 @@ struct alignas(16) DevProbeQuery {
   DevQuery q;
   DevClause cl[kMaxClauses];
   float ubt[256];                  // pure disjunctions: score bound per tf pattern, index sum min(tf_s, 3) * 4^s
+  // pure disjunctions, exact sweep warm-up (TOP_SCORES, every other slot has a plane): the warm-up scores the docs of
+  // warm_slot's list below granule warm_gran exactly and outputs them; the query's other items leave those postings to
+  // it. warm_slot -1 and warm_gran 0: none.
+  int32_t warm_slot;
+  int32_t warm_gran;
+  int32_t reserved[2];
 };
 static_assert(sizeof(DevProbeQuery) % 16 == 0, "DevProbeQuery is copied 16 bytes at a time");
 
@@ -200,9 +206,13 @@ NRT_HD int item_part(int32_t w) { return (item_flags(w) & kItemSweep) ? 0 : ((w 
 NRT_HD int item_lparts(int32_t w) { return (w >> 20) & 0xf; }
 
 // Boundary entries per (query, term slot) (sbounds of slice_bounds_kernel): n_slices * parts_max part boundaries
-// (slice-major), the shard end, the end of the warm-up granules of slice 0.
+// (slice-major), the shard end, the end of the warm-up granules of slice 0, the end of the exact sweep warm-up
+// (DevProbeQuery::warm_gran, a per-query granule).
 NRT_HD int boundary_end_entry(int n_slices, int parts_max) { return n_slices * parts_max; }
 NRT_HD int boundary_warm_entry(int n_slices, int parts_max) { return n_slices * parts_max + 1; }
+NRT_HD int boundary_exact_entry(int n_slices, int parts_max) { return n_slices * parts_max + 2; }
+NRT_HD int boundary_entries(int n_slices, int parts_max) { return n_slices * parts_max + 3; }
+constexpr uint32_t kSweepPostings = 32768;   // postings of the rarest list a sweep warm-up scores (at least, when exact)
 
 // Granules [g_lo, g_hi) of the item inside its slice (g_count granules, parts_max finest parts of `fine` granules each),
 // and the boundary entries e_lo / e_hi that hold its lists' posting bounds. A kItemBehindWarm item also starts at or after

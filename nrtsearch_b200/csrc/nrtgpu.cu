@@ -294,7 +294,7 @@ struct nrtgpu_batch {
   int32_t nq = 0, top_k = 0;
   CompiledBatch cb;            // host copies the async uploads read, kept until the next compilation
   WorkPlan plan;               // (search batches only)
-  DevBuf<uint32_t> sbounds;            // probe kernel: [nq][4][n_slices * parts_max + 2] part-boundary posting offsets
+  DevBuf<uint32_t> sbounds;            // probe kernel: [nq][4][n_slices * parts_max + 3] boundary posting offsets (batch_plan.h)
   DevBuf<v3::DevProbeQuery> pquery;    // probe kernel: [nq] per-query records (probe_query_kernel)
   DevBuf<unsigned int> work_counter;   // probe kernel: queue heads [2]
   DevBuf<unsigned long long> probe_stats;
@@ -353,6 +353,7 @@ struct nrtgpu_batch {
   int64_t ta_scalar = 0;           // terminateAfter (0: none)
   int64_t terminate_after_max_recall = 0;
   DevBuf<unsigned long long> known_hits;        // probe kernel: plan.known_hits
+  DevBuf<int32_t> warm_exact;                   // probe kernel: plan.warm_exact
   DevBuf<uint64_t> theta;
   DevBuf<unsigned long long> total_hits;
   DevBuf<uint64_t> slice_keys;
@@ -878,6 +879,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
   if ((rc = b->work_query.upload_async(p.work_query.data(), p.work_query.size(), st))) return rc;
   if ((rc = b->work_slice.upload_async(p.work_item.data(), p.work_item.size(), st))) return rc;
   if ((rc = b->known_hits.upload_async(p.known_hits.data(), p.known_hits.size(), st))) return rc;
+  if ((rc = b->warm_exact.upload_async(p.warm_exact.data(), p.warm_exact.size(), st))) return rc;
   if (b->cb.sorted) {
     bool any_after = false;
     b->h_after_docs.assign((size_t)nq, 0);
@@ -926,21 +928,23 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
   if ((rc = b->pruned.alloc((size_t)nq))) return rc;
   if ((rc = b->terminated.alloc((size_t)nq))) return rc;
   if (p.n_probe_simple + p.n_probe_generic > 0) {
-    // probe kernel: posting offsets of every (query, term slot) at the part boundaries only (skip data for the long lists,
-    // one lower_bound for the short ones); the granule offsets inside a slice are read from gran_tab by the kernel
-    const int64_t total = (int64_t)nq * v3::kT * ((int64_t)p.n_slices * p.parts_max + 2);
+    // the state of every query that no work item changes, which each item copies instead of deriving it ...
+    if ((rc = b->pquery.alloc((size_t)nq))) return rc;
+    v3::ProbeQueryLaunch Q;
+    Q.ix = ix->view(); Q.clauses = b->clauses.p; Q.queries = b->queries.p; Q.field_min_norm = ix->field_min_norm.p;
+    Q.warm_exact = b->warm_exact.p; Q.n_gran = p.n_gran; Q.out = b->pquery.p;
+    v3::probe_query_kernel<<<(unsigned)nq, v3::kUbt, 0, st>>>(Q);
+    NRT_CUDA_TRY(cudaGetLastError());
+    // ... and the posting offsets of every (query, term slot) at the part boundaries only (skip data for the long lists,
+    // one lower_bound for the short ones) and at the end of an exact warm-up (the records' warm_gran); the granule offsets
+    // inside a slice are read from gran_tab by the kernel
+    const int64_t total = (int64_t)nq * v3::kT * v3::boundary_entries(p.n_slices, p.parts_max);
     if ((rc = b->sbounds.alloc((size_t)total))) return rc;
     if ((rc = b->work_counter.alloc(2))) return rc;
     v3::SliceBoundsLaunch S;
-    S.ix = ix->view(); S.clauses = b->clauses.p; S.queries = b->queries.p; S.nq = nq; S.n_slices = p.n_slices;
+    S.ix = Q.ix; S.clauses = b->clauses.p; S.queries = b->queries.p; S.pquery = b->pquery.p; S.nq = nq; S.n_slices = p.n_slices;
     S.slice_gran = p.slice_docs / v3::kGran; S.n_gran = p.n_gran; S.parts_max = p.parts_max; S.sbounds = b->sbounds.p;
     v3::slice_bounds_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S);
-    NRT_CUDA_TRY(cudaGetLastError());
-    // ... and the state of every query that no work item changes, which each item copies instead of deriving it
-    if ((rc = b->pquery.alloc((size_t)nq))) return rc;
-    v3::ProbeQueryLaunch Q;
-    Q.ix = S.ix; Q.clauses = b->clauses.p; Q.queries = b->queries.p; Q.field_min_norm = ix->field_min_norm.p; Q.out = b->pquery.p;
-    v3::probe_query_kernel<<<(unsigned)nq, v3::kUbt, 0, st>>>(Q);
     NRT_CUDA_TRY(cudaGetLastError());
   }
   if (!b->ev[0][0]) for (auto& r : b->ev) for (auto& e : r) NRT_CUDA_TRY(cudaEventCreate(&e));
@@ -1251,6 +1255,8 @@ int nrtgpu_batch_run(nrtgpu_batch* b, void* stream_) {
                                   "%llu items end with stale roles (%.1f%% of item cycles, %.0f cyc each, %llu driver postings, %llu in lists that turned non-essential; slice 0 %llu, slice 1 %llu)\n",
                                   x[18], 100.0 * (double)x[19] / (double)x[1], x[20], x[21], x[22], 100.0 * (double)x[23] / (double)x[1],
                                   x[22] ? (double)x[23] / x[22] : 0.0, x[24], x[25], x[26], x[27]);
+      if (k == 0 && x[28]) fprintf(stderr, "[nrtgpu probe simple] exact warm-ups: %llu items, %llu driver postings, %.0f cyc each\n",
+                                   x[28], x[29], (double)x[30] / x[28]);
     }
   }
   MergeLaunch M;

@@ -96,7 +96,7 @@ constexpr int kUbt = 4 * 4 * 4 * 4;          // tf-pattern bounds: min(tf, 3) pe
 static_assert(sizeof(DevProbeQuery::ubt) == kUbt * sizeof(float), "one bound per tf pattern");
 constexpr int kWq = 32 * kR;                 // per-warp queue entries: the rounds drain it below 32 after their first push; once
                                              // the buffer is full, the kR - 1 pushes left in the round are not drained
-constexpr int kProbeStats = 28;              // stats words per instantiation (ProbeLaunch::stats)
+constexpr int kProbeStats = 31;              // stats words per instantiation (ProbeLaunch::stats)
 constexpr uint32_t kPiece = 8192;            // bytes per bulk copy
 constexpr uint32_t kTfInexact = 0xFEu;       // tf byte of a plane probe whose 2-bit code saturated (tf >= 3): the exact byte is
                                              // fetched from the byte plane when the doc is scored (rare); >= 3 for the bound table
@@ -108,13 +108,15 @@ struct ProbeLaunch {
   const DevProbeQuery* pquery;   // [nq] per-query records (probe_query_kernel)
   const int32_t* work_query;
   const int32_t* work_slice;     // work-item word (batch_plan.h item_encode)
-  const uint32_t* sbounds;       // [nq][kT][n_slices * parts_max + 2]: postings of the slot's list below every part boundary, the shard end, the warm-up boundary
+  const uint32_t* sbounds;       // [nq][kT][boundary_entries]: postings of the slot's list below every part boundary, the shard end, the
+                                 // warm-up boundary, the end of the exact sweep warm-up
   unsigned int* work_counter;    // queue head
   unsigned long long* stats;     // optional [kProbeStats]: items, item cycles, runs, driver postings, flushes, staged runs, set-up
                                  // cycles, rounds, longest item, CTA busy (sum, max), warm-up items and cycles, flush, TMA wait and
                                  // flush_top_k cycles, queued entries, admitted keys; pure-disjunction items that started with no
                                  // threshold (count, cycles, in slice 0 / 1) and whose MAXSCORE roles went stale (count, cycles,
-                                 // driver postings, postings of the lists that turned non-essential, in slice 0 / 1)
+                                 // driver postings, postings of the lists that turned non-essential, in slice 0 / 1); exact sweep
+                                 // warm-ups (count, driver postings, cycles)
   int32_t n_work, n_lists, n_slices, top_k;
   int32_t parts_max;             // result lists / boundary entries per slice (a heavy (query, slice) is split into up to this many items)
   int32_t slice_docs;            // multiple of kGran, <= kMaxSliceGran * kGran
@@ -178,6 +180,11 @@ struct alignas(128) ProbeSmemT {
   int theta_dec;                   // 1: the item publishes (k-th key - 1) as threshold (sweep warm-up: its candidates are not output)
   unsigned long long theta;
   int dbg_theta0;                  // profiling instantiation: the item started without a threshold
+  // pure disjunctions: a regular item of a query with an exact sweep warm-up
+  int32_t warm_g;                  // the warm-up's end granule, relative to the slice
+  uint32_t warm_own;               // the word byte of the warm-up's list: below warm_g, a doc that holds it is the warm-up's
+  uint32_t s_candrun[kT], s_cntrun[kT];   // s_candbelow / s_cntbefore in the current run: with warm_own in a run below warm_g
+  uint32_t run_drv;                // the lists that lead in the run (drv_mask without the warm-up's list below warm_g)
 };
 static_assert(sizeof(ProbeSmemT<kStageA>) <= 232448 / kCtasA - 1024 && sizeof(ProbeSmemT<kStageB>) <= 232448 / kCtasB - 1024, "ProbeSmem exceeds the per-CTA shared memory budget");
 
@@ -319,7 +326,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
   uint32_t stage_parity = 0;   // phase of stage_bar the next staged run completes (tracked identically by every thread)
   const int gran_per_slice = L.slice_docs >> kLogGran;
   const int fine = (gran_per_slice + L.parts_max - 1) / L.parts_max;   // granules per finest part of a slice
-  const int sb_stride = L.n_slices * L.parts_max + 2;
+  const int sb_stride = boundary_entries(L.n_slices, L.parts_max);
   const long long t_cta = kStats ? clock64() : 0ll;
 
   for (;;) {
@@ -345,6 +352,11 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
     // probing only the lists with tf planes (the other lists count as absent: scores are lower bounds). Nothing is output;
     // the k-th best lower-bound key minus one becomes the query's threshold before any other item of the query runs --
     // the docs that hold the query's rarest term are where its top-k is, a far better sample than the first 32K docs.
+    // EXACT sweep warm-up (the record's warm_slot, TOP_SCORES, every other list has a plane): nothing is absent, so the
+    // keys are true keys. It sweeps the list up to the record's warm_gran (the first granule boundary with 32K postings
+    // below it), counts and outputs those docs like a regular item and publishes the k-th key; in the query's other items
+    // the list leads only from warm_gran on, and below it a doc that holds the list is the warm-up's (run_drv, s_candrun,
+    // s_cntrun).
     const bool sweep_warm = (wflags & kItemSweep) != 0;
     const int warm_slot = item_sweep_slot(item);
     const int g_first = slice * gran_per_slice;
@@ -365,7 +377,8 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       uint4 piece = make_uint4(0u, 0u, 0u, 0u);
       if (tid < n16) piece = __ldg(reinterpret_cast<const uint4*>(L.pquery + qi) + tid);
       unsigned long long theta = 0ull, hits0 = 0ull, known = 0ull;
-      uint32_t ba = 0, bb = 0, bw = 0;
+      uint32_t ba = 0, bb = 0, bw = 0, bx = 0;
+      int exact_slot = -1;
       if (tid == 0) {
         theta = *(volatile unsigned long long*)&L.theta[qi];
         hits0 = *(volatile unsigned long long*)&L.total_hits[qi];
@@ -376,6 +389,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
         ba = sb[span.e_lo];
         bb = sb[span.e_hi];
         if (wflags & kItemBehindWarm) bw = sb[boundary_warm_entry(L.n_slices, L.parts_max)];
+        if (kSimple && sweep_warm) { exact_slot = __ldg(&L.pquery[qi].warm_slot); bx = sb[boundary_exact_entry(L.n_slices, L.parts_max)]; }
       }
       uint32_t gv[kGbIter];
       const uint32_t* row = L.ix.gran_tab + (size_t)max(gran_row, 0) * (size_t)(L.n_gran + 1) + g_first;
@@ -390,7 +404,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       if (tid >= 32 && tid < 32 + kT) {
         const int s = tid - 32;
         const uint32_t a = max(ba, bw);
-        if (sweep_warm && s == warm_slot) bb = min(bb, a + 32768u);
+        if (sweep_warm && s == warm_slot) bb = (s == exact_slot) ? bx : min(bb, a + kSweepPostings);
         sm.s_ia[s] = a; sm.s_ib[s] = max(a, bb); sm.s_ra[s] = 0; sm.s_rb[s] = 0; sm.s_sdelta[s] = 0;
       }
 #pragma unroll
@@ -413,9 +427,11 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       for (int s = 0; s < n_term; ++s) if (sm.pq.kind[s] == kPlane) pm |= 1u << s;
       uint32_t drv, ess;
       int cnt_first = -1;
+      const bool exact_warm = kSimple && sm.pq.warm_slot >= 0;   // the query has an exact sweep warm-up
       if (kSimple && sweep_warm) {
         drv = ess = 1u << warm_slot;
-        if (t < n_term) { sm.s_candbelow[t] = 0u; sm.s_cntbefore[t] = 0xffffffffu; sm.s_need[t] = pm & ~(1u << t); }   // (cntbefore: nothing is counted)
+        // (cntbefore: a lower-bound warm-up counts nothing, an exact one every live doc)
+        if (t < n_term) { sm.s_candbelow[t] = 0u; sm.s_cntbefore[t] = exact_warm ? 0u : 0xffffffffu; sm.s_need[t] = pm & ~(1u << t); }
       } else if (kSimple) {
         ess = all & ~ne;
         if (complete && ne && !L.ix.live_bits) {   // the densest non-essential list with a plane contributes its posting count unread
@@ -454,6 +470,13 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       __syncwarp((1u << kT) - 1u);
       if (t == 0) {
         if (ne && !complete) L.pruned[qi] = 1;
+        if (kSimple) {
+          if (exact_warm && sweep_warm) sm.theta_dec = 0;
+          const int warm_g = (exact_warm && !sweep_warm) ? sm.pq.warm_gran - g_first : 0;
+          sm.warm_g = warm_g;
+          sm.warm_own = exact_warm ? 0xffu << (8 * sm.pq.warm_slot) : 0u;
+          if (exact_warm && !sweep_warm && warm_g >= g_hi) drv &= ~(1u << sm.pq.warm_slot);   // the warm-up swept the list's postings of the item
+        }
         // short lists are staged whole at the first run; what does not fit the reserve is searched in global memory
         int st = 0;
         uint32_t lm = 0, shm = 0, gm = 0;
@@ -508,6 +531,17 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
           return tot <= cap;
         };
         int hi = g_hi, lo = g0 + 1;
+        // no run straddles the end of an exact warm-up: below it, the warm-up's list does not lead (it is still staged and
+        // probed) and a doc that holds it is owned by the warm-up
+        // (the generic instantiation has no exact warm-ups: its items read s_candbelow, s_cntbefore and drv_mask)
+        uint32_t run_drv = drv_mask;
+        if (kSimple) {
+          if (g0 < sm.warm_g && sm.warm_g < hi) hi = sm.warm_g;
+          const uint32_t own = g0 < sm.warm_g ? sm.warm_own : 0u;
+          for (int s = 0; s < kT; ++s) { sm.s_candrun[s] = sm.s_candbelow[s] | own; sm.s_cntrun[s] = sm.s_cntbefore[s] | own; }
+          run_drv &= ~presence4(own);
+          sm.run_drv = run_drv;
+        }
         if (long_mask && hi > lo && !fits(hi)) {
           while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (fits(mid)) lo = mid; else hi = mid; }
           hi = lo;
@@ -582,7 +616,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
             if (((long_mask >> s) & 1u) && sm.s_rb[s] > sm.s_ra[s]) st += stage(s, sm.s_ra[s], sm.s_rb[s], st);
         }
         uint32_t pre = 0;   // prefix of the driver postings
-        for (int s = 0; s < kT; ++s) { sm.s_pre[s] = pre; if (s < n_term && ((drv_mask >> s) & 1u)) pre += sm.s_rb[s] - sm.s_ra[s]; }
+        for (int s = 0; s < kT; ++s) { sm.s_pre[s] = pre; if (s < n_term && ((run_drv >> s) & 1u)) pre += sm.s_rb[s] - sm.s_ra[s]; }
         sm.s_pre[kT] = pre;
       }
       __syncthreads();   // R1: run plan visible
@@ -610,7 +644,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
               sm.s_ra[s] = na; sm.s_rb[s] = (uint32_t)(l - base);
             }
           uint32_t pre = 0;
-          for (int s = 0; s < kT; ++s) { sm.s_pre[s] = pre; if (s < n_term && ((drv_mask >> s) & 1u)) pre += sm.s_rb[s] - sm.s_ra[s]; }
+          for (int s = 0; s < kT; ++s) { sm.s_pre[s] = pre; if (s < n_term && (((kSimple ? sm.run_drv : drv_mask) >> s) & 1u)) pre += sm.s_rb[s] - sm.s_ra[s]; }
           sm.s_pre[kT] = pre;
         }
         __syncthreads();
@@ -686,7 +720,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
         const int ct_end = NRT_KNOCK(8) ? 0 : (dense ? n_term + 1 : n_term);   // dense: one more "list" = every doc of the run
         while (!full && ct < ct_end) {
           const bool t_dense = ct == n_term;
-          const uint32_t n_t = t_dense ? (uint32_t)(sm.run_d1 - sm.run_d0) : (((drv_mask >> ct) & 1u) ? sm.s_rb[ct] - sm.s_ra[ct] : 0u);
+          const uint32_t n_t = t_dense ? (uint32_t)(sm.run_d1 - sm.run_d0) : ((((kSimple ? sm.run_drv : drv_mask) >> ct) & 1u) ? sm.s_rb[ct] - sm.s_ra[ct] : 0u);
           if (cb >= n_t) { ++ct; cb = 0; continue; }
           const int t = t_dense ? 0 : ct;
           const uint32_t need = t_dense ? ((n_term >= 32) ? 0xffffffffu : ((1u << n_term) - 1u)) : sm.s_need[t];
@@ -694,7 +728,8 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
                          need_short = NRT_KNOCK(2) ? 0u : need & short_mask, need_glob = need & global_mask;
           const bool t_staged = !t_dense && (((long_mask | short_mask) >> t) & 1u);
           const bool t_ess = (ess_mask >> t) & 1u;
-          const uint32_t candbelow = t_dense ? 0u : sm.s_candbelow[t], cntbefore = t_dense ? 0u : sm.s_cntbefore[t];
+          const uint32_t candbelow = t_dense ? 0u : (kSimple ? sm.s_candrun[t] : sm.s_candbelow[t]),
+                         cntbefore = t_dense ? 0u : (kSimple ? sm.s_cntrun[t] : sm.s_cntbefore[t]);
           const int32_t dense_d0 = sm.run_d0;
           const int32_t* sdoc_t = sm.sdocs + ((int)sm.s_ra[t] + sm.s_sdelta[t]);   // posting x of the run segment: sdoc_t[x]
           const uint8_t* sf8_t = sm.sf8 + ((int)sm.s_ra[t] + sm.s_sdelta[t]);
@@ -830,13 +865,14 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       if (kStats) dbg_tflush += clock64() - tf;
       if (kStats) ++dbg_flush;
     }
-    const int keep = sweep_warm ? 0 : min(sm.cand_count, L.top_k);
+    const bool lb_warm = kSimple ? sm.theta_dec != 0 : sweep_warm;   // a lower-bound sweep warm-up outputs nothing and counts nothing
+    const int keep = lb_warm ? 0 : min(sm.cand_count, L.top_k);
     const int out_list = item_out_list(item, L.parts_max, L.n_lists);
     uint64_t* out = L.slice_keys + ((size_t)qi * L.n_lists + out_list) * L.top_k;
     for (int i = tid; i < keep; i += kThreads) out[i] = sm.cand[i];
     if (tid == 0) L.slice_cnt[(size_t)qi * L.n_lists + out_list] = keep;
     for (int o = 16; o > 0; o >>= 1) my_hits += __shfl_xor_sync(0xffffffffu, my_hits, o);
-    if (lane == 0 && my_hits && !sweep_warm) atomicAdd(&L.total_hits[qi], (unsigned long long)my_hits);
+    if (lane == 0 && my_hits && !lb_warm) atomicAdd(&L.total_hits[qi], (unsigned long long)my_hits);
     if (kStats) {
       for (int o = 16; o > 0; o >>= 1) dbg_admit += __shfl_xor_sync(0xffffffffu, dbg_admit, o);
       if (lane == 0) { atomicAdd(&L.stats[16], (unsigned long long)dbg_queued); atomicAdd(&L.stats[17], (unsigned long long)dbg_admit); }
@@ -853,6 +889,7 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
       atomicAdd(&L.stats[7], (unsigned long long)dbg_rounds);
       atomicMax(&L.stats[8], cyc);
       if (wflags & (kItemWarmDocs | kItemSweep)) { atomicAdd(&L.stats[11], 1ull); atomicAdd(&L.stats[12], cyc); }
+      if (sweep_warm && !lb_warm) { atomicAdd(&L.stats[28], 1ull); atomicAdd(&L.stats[29], dbg_post); atomicAdd(&L.stats[30], cyc); }
       atomicAdd(&L.stats[13], (unsigned long long)dbg_tflush); atomicAdd(&L.stats[14], (unsigned long long)dbg_twait);
       if (kSimple && !sweep_warm) count_role_stats(L, sm, qi, item_slice(item), ess_mask, cyc, dbg_post);
     }
@@ -864,23 +901,25 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
 }
 
 // postings of every (query, term slot) below each part boundary of every slice (parts_max equal granule ranges per
-// slice), below the end of the shard, and below the warm-up boundary of slice 0
+// slice), below the end of the shard, below the warm-up boundary of slice 0 and below the end of the query's exact sweep
+// warm-up (its record's warm_gran: probe_query_kernel runs first)
 struct SliceBoundsLaunch {
   DevIndexView ix;
   const DevClause* clauses;
   const DevQuery* queries;
+  const DevProbeQuery* pquery;
   int32_t nq, n_slices, slice_gran, n_gran, parts_max;
-  uint32_t* sbounds;   // [nq][kT][n_slices * parts_max + 2]
+  uint32_t* sbounds;   // [nq][kT][boundary_entries]
 };
 
 __global__ void slice_bounds_kernel(SliceBoundsLaunch B) {
-  const int n_b = B.n_slices * B.parts_max;
-  const int per_slot = n_b + 2;
+  const int per_slot = boundary_entries(B.n_slices, B.parts_max);
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)B.nq * kT * per_slot) return;
   const int q = (int)(i / (kT * per_slot)), s = (int)((i / per_slot) % kT), e = (int)(i % per_slot);
   const DevQuery dq = B.queries[q];
-  const int64_t gran = boundary_gran(e, B.n_slices, B.parts_max, B.slice_gran, B.n_gran);
+  const int64_t gran = e == boundary_exact_entry(B.n_slices, B.parts_max) ? (int64_t)B.pquery[q].warm_gran
+                                                                           : boundary_gran(e, B.n_slices, B.parts_max, B.slice_gran, B.n_gran);
   uint32_t out = 0;
   for (int c = 0; c < dq.n_clauses; ++c) {
     const DevClause cl = B.clauses[dq.clause_begin + c];
@@ -903,6 +942,8 @@ struct ProbeQueryLaunch {
   const DevClause* clauses;
   const DevQuery* queries;
   const uint8_t* field_min_norm;
+  const int32_t* warm_exact;   // [nq] the slot of the query's exact sweep warm-up, -1: none (WorkPlan::warm_exact)
+  int32_t n_gran;
   DevProbeQuery* out;   // [nq]
 };
 
@@ -919,6 +960,7 @@ __global__ void __launch_bounds__(kUbt) probe_query_kernel(ProbeQueryLaunch B) {
     r.kind[s] = kAbsent; r.plane[s] = nullptr; r.plane2[s] = nullptr; r.gdocs[s] = nullptr; r.gf8[s] = nullptr;
     r.weight[s] = 0.f; r.ub[s] = 0.f; r.clause[s] = 0; r.field[s] = 0; r.pbm[s] = 0; r.row[s] = -1; r.ord[s] = 0; r.pre[s] = 0.f;
   }
+  if (tid == 0) { r.warm_slot = -1; r.warm_gran = 0; r.reserved[0] = r.reserved[1] = 0; }
   __syncthreads();
   if (tid < ncl && r.cl[tid].kind == NRTGPU_TERM) {   // per-slot descriptors (one thread per clause)
     const DevClause& c = r.cl[tid];
@@ -963,6 +1005,18 @@ __global__ void __launch_bounds__(kUbt) probe_query_kernel(ProbeQueryLaunch B) {
     for (int a = 1; a < n; ++a) { const int x = ord[a]; int b = a - 1; while (b >= 0 && r.ub[ord[b]] > r.ub[x]) { ord[b + 1] = ord[b]; --b; } ord[b + 1] = x; }
     double pre = 0.0;
     for (int a = 0; a < n; ++a) { pre += (double)r.ub[ord[a]]; r.ord[a] = ord[a]; r.pre[a] = (float)pre; }
+    // exact sweep warm-up: every other slot is probed through a plane; it ends at the first granule boundary with
+    // kSweepPostings postings of its list below it (the shard end for a shorter list or one without granule offsets)
+    int w = B.warm_exact[qi];
+    for (int s = 0; s < n_term; ++s) if (w >= 0 && s != w && r.kind[s] != kPlane) w = -1;
+    if (w >= 0) {
+      int lo = 0, hi = B.n_gran;
+      if (r.row[w] >= 0) {
+        const uint32_t* row = B.ix.gran_tab + (size_t)r.row[w] * (size_t)(B.n_gran + 1);
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (__ldg(row + mid) < kSweepPostings) lo = mid + 1; else hi = mid; }
+      }
+      r.warm_slot = w; r.warm_gran = hi;
+    }
   }
   __syncthreads();
   const uint4* src = reinterpret_cast<const uint4*>(&r);
