@@ -246,6 +246,11 @@ int nrtgpu_index_add_keyword_columns(nrtgpu_index* ix, const nrtgpu_keyword_colu
 /* The bytes of term `ord` of keyword column `column` of an image: its length in *len, and its first min(len, cap) bytes
  * in out (out may be NULL when cap is 0). NRTGPU_ERR_INVALID: a column or ordinal out of range, len NULL. */
 int nrtgpu_index_keyword_term(const nrtgpu_index* ix, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len);
+/* The sort code of a term (bytes[0 .. len)) in keyword column `column` of an image (NRTGPU_SORT_KEYWORD values): 2i + 2
+ * when the dictionary holds it as term i, else 2i + 1 where i is the number of terms that sort before it (unsigned-byte
+ * order). A searchAfter term from LastHitInfo becomes an after value this way. NRTGPU_ERR_INVALID: a column out of range,
+ * code NULL, bytes NULL with len > 0, len < 0. */
+int nrtgpu_index_keyword_seek(const nrtgpu_index* ix, int32_t column, const uint8_t* bytes, int32_t len, int64_t* code);
 
 /* Phrase leaves of query trees (PhraseQuery / match_phrase, reference QueryNodeMapper.java:285-291, :397-427). A clause of
  * kind NRTGPU_PHRASE is a leaf whose id indexes phrases[]; its boost is the leaf's folded boost, as for a term leaf. The
@@ -333,28 +338,44 @@ int nrtgpu_search_sorted(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t
  *                       sorts as missing_value; on a MULTI-valued column `selector` picks the doc's smallest (MIN, the
  *                       default) or largest (MAX) value (SortedNumericSelector), ignored on a single-valued one;
  *   NRTGPU_SORT_DOCID   the doc id, ascending unless reverse; the fields after it cannot decide anything and are ignored;
- *   NRTGPU_SORT_SCORE   the BM25 score, higher first unless reverse (RelevanceComparator); FIRST position only.
+ *   NRTGPU_SORT_SCORE   the BM25 score, higher first unless reverse (RelevanceComparator); FIRST position only;
+ *   NRTGPU_SORT_KEYWORD a keyword column `column` (nrtgpu_index_add_keyword_columns) by its term in unsigned-byte order
+ *                       (SortField STRING / SortedSetSortField), ascending unless reverse. On a SORTED_SET column the
+ *                       selector picks one of the doc's n ascending ordinals: MIN ords[0], MAX ords[n-1], MIDDLE_MIN
+ *                       ords[(n-1)/2], MIDDLE_MAX ords[n/2] (SortedSetSelector); it is ignored on a SORTED column.
+ *                       missing_value 0 (STRING_FIRST): a doc without a value sorts before every term; 1 (STRING_LAST):
+ *                       after every term. reverse reverses the whole comparison, the missing position included.
+ *                       Its FieldDoc value (out_sort_values, after_values, nrtgpu_nested_sort.values, packed records) is
+ *                       the term's code in the dictionary of the call: 2i + 2 for term i, 0 for no value (null). On a
+ *                       single image that is the image's dictionary, on a searcher the reader-wide union. After values may
+ *                       also hold 2i + 1 (i in 0..n): a term held by no dictionary, between term i - 1 and term i; any
+ *                       other code is NRTGPU_ERR_INVALID. nrtgpu_index_keyword_seek / nrtgpu_searcher_keyword_seek turn a
+ *                       term into its code; the *_keyword_term calls turn code c back (ordinal c / 2 - 1).
  * The implicit last tie-break is the doc id, ascending. An order (nrtgpu_sort_order) ranks every doc of the image under
  * one Sort once (an O(n log n) device sort on `stream`); it depends on the columns only, so it stays valid across
  * nrtgpu_index_set_live_docs and nrtgpu_index_update_stats: build one per (leaf, Sort) and reuse it for every request.
  * It holds 8 bytes per doc of device memory (nrtgpu_sort_order_device_bytes) and must be closed before its index.
  *   nrtgpu_sort_order_create: NRTGPU_ERR_INVALID for n_fields < 1, a bad kind or selector, a column out of range;
+ *                             for a KEYWORD field also a keyword column out of range, a selector outside MIN..MIDDLE_MAX
+ *                             and a missing_value other than 0 or 1 (MIDDLE_* on a COLUMN field is a bad selector);
  *                             NRTGPU_ERR_UNSUPPORTED for n_fields > 8 or a SCORE after the first position.
+ *   nrtgpu_search_sorted (one field) keeps refusing the KEYWORD kind ("bad sort kind").
  *   nrtgpu_search_sorted_fields: as nrtgpu_search_sorted (exact totalHits, the same limits and refusals) with the order's
  *     Sort. out_sort_values [nq*top_k*n_fields] = FieldDoc.fields of every hit: a column's selected value or missing_value,
  *     the global doc id for DOCID, the score's float bits zero-extended for SCORE (Float.floatToIntBits).
  *     after_values [nq*n_fields] (same encoding) + nrtgpu_query.has_after / after_doc: a hit qualifies iff its field tuple
  *     sorts strictly after the after tuple, or ties with it and has a greater global doc id than after_doc
  *     (PagingFieldCollector); the values need not be held by any doc of this leaf.
- *     NRTGPU_ERR_INVALID: an order of another index, has_after without after_values. */
-enum { NRTGPU_SORT_SCORE = 3 };
-enum { NRTGPU_SELECT_MIN = 0, NRTGPU_SELECT_MAX = 1 };
+ *     NRTGPU_ERR_INVALID: an order of another index, has_after without after_values, a KEYWORD after code outside
+ *     0..2n + 1 (n: the column's terms). */
+enum { NRTGPU_SORT_SCORE = 3, NRTGPU_SORT_KEYWORD = 5 };   /* (4 is taken by an internal kind) */
+enum { NRTGPU_SELECT_MIN = 0, NRTGPU_SELECT_MAX = 1, NRTGPU_SELECT_MIDDLE_MIN = 2, NRTGPU_SELECT_MIDDLE_MAX = 3 };
 typedef struct {
-  int32_t kind;          /* NRTGPU_SORT_COLUMN, NRTGPU_SORT_DOCID or NRTGPU_SORT_SCORE */
-  int32_t column;        /* NRTGPU_SORT_COLUMN: doc-value column id */
+  int32_t kind;          /* NRTGPU_SORT_COLUMN, NRTGPU_SORT_DOCID, NRTGPU_SORT_SCORE or NRTGPU_SORT_KEYWORD */
+  int32_t column;        /* NRTGPU_SORT_COLUMN: doc-value column id; NRTGPU_SORT_KEYWORD: keyword column id */
   int32_t reverse;
-  int32_t selector;      /* NRTGPU_SELECT_MIN / _MAX (multi-valued columns) */
-  int64_t missing_value;
+  int32_t selector;      /* NRTGPU_SELECT_MIN / _MAX (multi-valued columns); MIDDLE_MIN / _MAX: SORTED_SET keyword only */
+  int64_t missing_value; /* NRTGPU_SORT_KEYWORD: 0 STRING_FIRST, 1 STRING_LAST */
 } nrtgpu_sort_field;
 typedef struct nrtgpu_sort_order nrtgpu_sort_order;
 int nrtgpu_sort_order_create(nrtgpu_index* ix, const nrtgpu_sort_field* fields, int32_t n_fields, void* stream,
@@ -379,9 +400,12 @@ int nrtgpu_search_sorted_fields(nrtgpu_index* ix, const nrtgpu_sort_order* order
  *     in the caller-owned DEVICE record d_record; synchronises `stream`. With disallow_partial_results a timeout is
  *     NRTGPU_ERR_TIMEOUT, as on the host path.
  *   nrtgpu_merge_sorted_packed: TopFieldDocs.merge of n_lists records [n_lists][words] of the same Sort into d_out_record,
- *     on `stream` (asynchronous). fields = the Sort's nrtgpu_sort_field records; only kind and reverse are read. Hits
- *     compare field by field: COLUMN and DOCID by the value as a sortable long, ascending unless reverse; SCORE by the float
- *     of its bits, higher first unless reverse; the fields after the first DOCID are ignored; then the global doc id
+ *     on `stream` (asynchronous). fields = the Sort's nrtgpu_sort_field records; kind and reverse are read, and for a
+ *     KEYWORD field missing_value. Hits compare field by field: COLUMN and DOCID by the value as a sortable long, ascending
+ *     unless reverse; SCORE by the float of its bits, higher first unless reverse; KEYWORD by its code, code 0 first
+ *     (missing_value 0) or last (1), the whole reversed with reverse. Keyword codes compare only when every record numbers
+ *     them in one dictionary (a searcher maps its leaves' codes to the reader-wide union before it merges; records of
+ *     different shards do not compare). The fields after the first DOCID are ignored; then the global doc id
  *     ascending. totalHits are summed and the flags ORed. NRTGPU_ERR_INVALID: n_lists < 1, n_fields outside 1..8, a bad
  *     kind, nq <= 0, top_k outside 1..1024, an unaligned record. */
 int64_t nrtgpu_sorted_packed_words(int32_t nq, int32_t top_k, int32_t n_fields);
@@ -785,8 +809,9 @@ int nrtgpu_searcher_close(nrtgpu_searcher* s);
  * terminated_early / relation GTE make the merged query's.
  *   nrtgpu_searcher_search_sorted_fields: nrtgpu_search_sorted_fields over the leaves (TopFieldDocs.merge,
  *     nrtgpu_merge_sorted_packed). orders[n_orders]: one nrtgpu_sort_order per leaf, in leaf order, all of the same Sort (the
- *     same kinds and directions, and for a column field the same column, selector and missing value). after_values /
- *     after_doc are reader-wide and go to every leaf unchanged. A one-field Sort is a one-field order here.
+ *     same kinds and directions, and for a column or keyword field the same column, selector and missing value).
+ *     after_values / after_doc are reader-wide and go to every leaf unchanged, except a KEYWORD field's code, which each
+ *     leaf receives in its own dictionary (nrtgpu_searcher_keyword_seek). A one-field Sort is a one-field order here.
  *     NRTGPU_ERR_INVALID: n_orders != the number of leaves, an order made on another index than its leaf, orders of
  *     different Sorts.
  *   nrtgpu_searcher_search_tree_phrases: nrtgpu_search_tree_phrases over the leaves (n_nodes / n_phrases may be 0);
@@ -838,6 +863,12 @@ int nrtgpu_searcher_search_knn_filtered(nrtgpu_searcher* s, const float* queries
  * NRTGPU_ERR_INVALID: a column some leaf lacks, an ordinal out of range (ord -1 only asks for n_terms), len NULL. */
 int nrtgpu_searcher_keyword_term(nrtgpu_searcher* s, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len,
                                  int32_t* n_terms);
+/* nrtgpu_index_keyword_seek in the reader-wide dictionary of keyword column `column` (built as by
+ * nrtgpu_searcher_keyword_term if no call has yet): the after values of nrtgpu_searcher_search_sorted_fields and the
+ * values it returns for a KEYWORD field are codes of that dictionary. Each leaf is searched with the code its own
+ * dictionary gives the same term, and its hits' codes are mapped to the union on the device before the merge; sorted top
+ * hits over the leaves likewise. NRTGPU_ERR_INVALID: a column some leaf lacks, and the refusals of the image call. */
+int nrtgpu_searcher_keyword_seek(nrtgpu_searcher* s, int32_t column, const uint8_t* bytes, int32_t len, int64_t* code);
 int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
                                             const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
                                             const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,

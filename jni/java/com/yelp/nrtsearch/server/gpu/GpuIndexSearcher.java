@@ -231,7 +231,12 @@ public class GpuIndexSearcher extends MyIndexSearcher {
 
       <T> T toResult(TopDocs topDocs, double queueMs, double searchMs, int batchSize);
 
-      /** SortFieldCollector requests: nrtgpu_sort_field[numSortFields()], or null for relevance. */
+      /**
+       * SortFieldCollector requests: nrtgpu_sort_field[numSortFields()], or null for relevance. A SortField of an AtomFieldDef
+       * (STRING or SortedSetSortField) is kind NrtGpu.SORT_KEYWORD on the field's keyword column, its selector one of
+       * NrtGpu.SELECT_*, missing_value 1 for STRING_LAST; its after value is NrtGpu.keywordSeek of the LastHitInfo string
+       * (searcherKeywordSeek over several leaves), or 0 for NULL_SORT_VALUE.
+       */
       default ByteBuffer sortFields() {
         return null;
       }

@@ -80,6 +80,21 @@ public final class NrtGpu {
   /** keywordTerm for a searcher's reader-wide ordinals; ord -1 returns the number of reader-wide terms. */
   public static native int searcherKeywordTerm(long searcher, int column, int ord, ByteBuffer out, int cap);
 
+  /** nrtgpu_sort_field.kind of a keyword sort field (AtomFieldDef.getSortField); missing_value 0 STRING_FIRST, 1 STRING_LAST. */
+  public static final int SORT_KEYWORD = 5;
+  /** nrtgpu_sort_field.selector (SortedSetSelector.Type); MIDDLE_* only on a SORTED_SET keyword field. */
+  public static final int SELECT_MIN = 0, SELECT_MAX = 1, SELECT_MIDDLE_MIN = 2, SELECT_MIDDLE_MAX = 3;
+
+  /**
+   * The sort code of a keyword term (len bytes of the direct buffer term) in keyword column `column` of an image: 2i + 2
+   * for its term i, 2i + 1 for a term it does not hold. A LastHitInfo string becomes a keyword field's after value this way
+   * (NULL_SORT_VALUE is 0); FieldDoc values c map back to terms with keywordTerm(c / 2 - 1).
+   */
+  public static native long keywordSeek(long index, int column, ByteBuffer term, int len);
+
+  /** keywordSeek in a searcher's reader-wide dictionary (the codes of searcherSearchSortedFields). */
+  public static native long searcherKeywordSeek(long searcher, int column, ByteBuffer term, int len);
+
   /**
    * Query trees with PhraseQuery leaves: phrases = nrtgpu_phrase[nPhrases] referenced by clauses of kind 4 (PHRASE),
    * phraseTerms = nrtgpu_phrase_term[nPhraseTerms] (term id, PhraseQuery position); otherwise as searchTree, which it is

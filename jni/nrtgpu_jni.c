@@ -165,6 +165,21 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherKeyword
     return -1;
   return ord == -1 ? n_terms : len;
 }
+/* the sort code of a keyword term (term: a direct ByteBuffer of len bytes) in an image's dictionary: a LastHitInfo string
+ * as the after value of an NRTGPU_SORT_KEYWORD field; -1 after a refusal (the exception is pending) */
+JNIEXPORT jlong JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_keywordSeek(JNIEnv* env, jclass c, jlong ix, jint column, jobject term,
+                                                                              jint len) {
+  int64_t code = 0;
+  if (fail(env, nrtgpu_index_keyword_seek((const nrtgpu_index*)(intptr_t)ix, column, (const uint8_t*)ADDR(env, term), len, &code))) return -1;
+  return code;
+}
+/* keywordSeek in a searcher's reader-wide dictionary */
+JNIEXPORT jlong JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherKeywordSeek(JNIEnv* env, jclass c, jlong s, jint column,
+                                                                                      jobject term, jint len) {
+  int64_t code = 0;
+  if (fail(env, nrtgpu_searcher_keyword_seek((nrtgpu_searcher*)(intptr_t)s, column, (const uint8_t*)ADDR(env, term), len, &code))) return -1;
+  return code;
+}
 /* phrases / phraseTerms: direct ByteBuffers laid out as nrtgpu_phrase[] / nrtgpu_phrase_term[] (nPhrases 0: searchTree) */
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTreePhrases(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,

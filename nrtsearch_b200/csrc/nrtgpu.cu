@@ -12,6 +12,7 @@
 #include <thrust/unique.h>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <condition_variable>
 #include <deque>
@@ -333,6 +334,8 @@ struct nrtgpu_batch {
   // sorted top hits: FieldDoc values of the results; over several leaves the group's packed sorted records (leaves', then
   // merged) and the key scores of a leaf's selection
   DevBuf<int64_t> nest_svals, nest_rec; DevBuf<float> nest_rscores;
+  // a searcher's leaf: per cb.nested entry, the leaf -> union maps of its Sort's keyword fields (empty: a single image)
+  std::vector<std::array<const uint32_t*, kMaxSortFields>> nest_kw_map;
   DevBuf<AggLaunch> nest_launch;
   DevBuf<unsigned long long> p2_total; DevBuf<int32_t> p2_flags;   // the top-hits run's totalHits / pruned / terminated
   // filter collectors (cb.agg_filters): one row per FILTER aggregation on this image (agg_rows), built by batch_filter_rows
@@ -800,6 +803,28 @@ static void copy_term(const std::vector<uint8_t>& bytes, const std::vector<int64
   if (out && cap > 0 && l > 0) std::memcpy(out, bytes.data() + a, (size_t)std::min<int64_t>(l, cap));
 }
 
+// the sort code of term t[0 .. len) in a host dictionary of n terms (bytes, off): 2i + 2 for term i, else 2i + 1 where i
+// terms sort before it (unsigned bytes, then length: BytesRef order)
+static int64_t keyword_seek_code(const std::vector<uint8_t>& bytes, const std::vector<int64_t>& off, int32_t n, const uint8_t* t,
+                                 int32_t len) {
+  auto cmp = [&](int32_t i) {   // term i against t: < 0, 0, > 0
+    const int64_t a = off[(size_t)i], l = off[(size_t)i + 1] - a, m = std::min<int64_t>(l, len);
+    const int c = m > 0 ? std::memcmp(bytes.data() + a, t, (size_t)m) : 0;
+    return c != 0 ? c : (l < len ? -1 : (l > len ? 1 : 0));
+  };
+  int32_t lo = 0, hi = n;   // the first term that does not sort before t
+  while (lo < hi) { const int32_t m = lo + (hi - lo) / 2; if (cmp(m) < 0) lo = m + 1; else hi = m; }
+  return (lo < n && cmp(lo) == 0) ? 2 * (int64_t)lo + 2 : 2 * (int64_t)lo + 1;
+}
+
+int nrtgpu_index_keyword_seek(const nrtgpu_index* ix, int32_t column, const uint8_t* bytes, int32_t len, int64_t* code) {
+  if (!ix || !code || (!bytes && len > 0) || len < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_seek: bad argument");
+  if (column < 0 || (size_t)column >= ix->kw.size()) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_seek: keyword column out of range");
+  const KeywordColumn& c = *ix->kw[(size_t)column];
+  *code = keyword_seek_code(c.bytes, c.off, c.n_terms, bytes, len);
+  return NRTGPU_OK;
+}
+
 int nrtgpu_index_keyword_term(const nrtgpu_index* ix, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len) {
   if (!ix || !len) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_term: NULL argument");
   if (column < 0 || (size_t)column >= ix->kw.size()) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_term: keyword column out of range");
@@ -855,6 +880,24 @@ static int batch_compile(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& 
 
 static int batch_filter_rows(nrtgpu_batch* b, const BatchRequest& r, cudaStream_t st);
 
+// the KEYWORD after values of the queries with searchAfter: 0 (null) or a code 1 .. 2n + 1 of the column's n terms (n_distinct
+// of the order's field on an image; the caller's n on a searcher)
+static int check_keyword_after(const nrtgpu_sort_order* o, const int64_t* after, const nrtgpu_query* queries, int32_t nq,
+                               const char* fn, const int32_t* n_terms = nullptr) {
+  for (int j = 0; j < o->n_fields; ++j) {
+    if (o->spec[j].kind != NRTGPU_SORT_KEYWORD) continue;
+    const int64_t hi = 2 * (int64_t)(n_terms ? n_terms[j] : o->f[j].n_distinct) + 1;
+    for (int q = 0; q < nq; ++q)
+      if (queries[q].has_after) {
+        const int64_t c = after[(size_t)q * o->n_fields + j];
+        if (c < 0 || c > hi)
+          NRT_FAIL(NRTGPU_ERR_INVALID, std::string(fn) + ": keyword after value " + std::to_string(c) + " of sort field " +
+                                           std::to_string(j) + " is not a code of the column's " + std::to_string(hi / 2) + " terms");
+      }
+  }
+  return NRTGPU_OK;
+}
+
 // a search batch: compile, plan the work list, upload, set up sorted searchAfter, allocate the results, launch
 // slice_bounds_kernel and build the rows of the filter collectors
 static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r, cudaStream_t st) {
@@ -866,6 +909,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
   b->order = sort_order;
   b->ran = false; b->runs_recorded = 0;
   b->agg_shared = false;
+  b->nest_kw_map.clear();
   if (sort_order) {   // fields-only order: the COLUMN key with the rank as its code; [score, ...]: kSortScoreRank
     b->sort_kind = sort_order->score_first ? kSortScoreRank : NRTGPU_SORT_COLUMN; b->sort_column = 0;
     b->sort_reverse = sort_order->score_first ? sort_order->score_reverse : 0; b->sort_missing_value = 0;
@@ -890,6 +934,8 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
       NRT_CUDA_TRY(cudaMemsetAsync(b->sort_missing_code.p, 0, sizeof(uint32_t), st));
       if ((rc = b->after_docs.upload_async(b->h_after_docs.data(), (size_t)nq, st))) return rc;
       const size_t nv = (size_t)nq * sort_order->n_fields;
+      if (r.order_after && any_after)
+        if ((rc = check_keyword_after(sort_order, r.order_after, r.queries, nq, "nrtgpu_search_sorted_fields"))) return rc;
       if (r.order_after) { if ((rc = b->after_values.upload_async(r.order_after, nv, st))) return rc; }
       else if ((rc = b->after_values.alloc(nv))) return rc;
       SortFieldsAfterLaunch A{};
@@ -1359,6 +1405,20 @@ static int sorted_hit_values(const nrtgpu_sort_order* o, int32_t doc_base, int32
   return NRTGPU_OK;
 }
 
+// A searcher's leaf: the FieldDoc values [n][n_fields] of its hits, whose KEYWORD codes number the leaf's dictionary, to
+// codes of the reader-wide union (sort_kw_map_kernel), before the leaves' records merge. maps: per field, NULL where
+// nothing maps (see SortKwMapLaunch); nothing runs when every entry is NULL.
+static int sort_kw_values_to_union(const uint32_t* const* maps, int n_fields, int64_t* values, int64_t n, cudaStream_t st) {
+  SortKwMapLaunch M{};
+  bool any = false;
+  for (int j = 0; j < n_fields; ++j) { M.map[j] = maps[j]; any |= maps[j] != nullptr; }
+  if (!any || n <= 0) return NRTGPU_OK;
+  M.values = values; M.n = n; M.n_fields = n_fields;
+  sort_kw_map_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(M);
+  NRT_CUDA_TRY(cudaGetLastError());
+  return NRTGPU_OK;
+}
+
 // Nested top hits of terms or filter aggregation `parent` (pass 2) over the batches bs[0 .. n_b) that counted into one set of tables
 // (a single image: one batch; a searcher: one per leaf). Each batch's engine runs again (batch_engine_launch: the probe
 // kernel, or the window engine for tree and wide batches) with a collector that only
@@ -1488,6 +1548,9 @@ static int batch_nested_top_hits(nrtgpu_batch* const* bs, int n_b, cudaStream_t 
         NRT_CUDA_TRY(cudaGetLastError());
         if ((rc = sorted_hit_values(o, x->ix->doc_base, r, r + L.counts, b->nest_rscores.p, gs, H.top_hits,
                                     reinterpret_cast<int64_t*>(r + L.values), st))) return rc;
+        if (!x->nest_kw_map.empty() &&   // keyword values in the reader-wide dictionary, so the leaves' lists merge
+            (rc = sort_kw_values_to_union(x->nest_kw_map[th[(size_t)k]].data(), o->n_fields, reinterpret_cast<int64_t*>(r + L.values),
+                                          (int64_t)gs * H.top_hits, st))) return rc;
       }
     }
     for (int k = 0; k < n_th; ++k) {
@@ -1924,6 +1987,13 @@ int nrtgpu_sort_order_create(nrtgpu_index* ix, const nrtgpu_sort_field* fields, 
         f.c64 = ix->col64[c]->p; f.c32 = ix->col32[c]->p; f.has = ix->col_has[c]->p;
         f.codes = ix->col_code[c]->p; f.distinct = ix->col_distinct[c]->p; f.n_distinct = ix->col_n_distinct[c];
       }
+    } else if (s.kind == NRTGPU_SORT_KEYWORD) {
+      if (s.column < 0 || (size_t)s.column >= ix->kw.size()) NRT_FAIL(NRTGPU_ERR_INVALID, "keyword sort column out of range");
+      if (s.selector < NRTGPU_SELECT_MIN || s.selector > NRTGPU_SELECT_MIDDLE_MAX) NRT_FAIL(NRTGPU_ERR_INVALID, "bad sort selector");
+      if (s.missing_value != 0 && s.missing_value != 1)
+        NRT_FAIL(NRTGPU_ERR_INVALID, "keyword sort missing_value must be 0 (STRING_FIRST) or 1 (STRING_LAST)");
+      const KeywordColumn& c = *ix->kw[(size_t)s.column];
+      f.codes = c.codes.p; f.mv_off = c.multi ? c.doc_off.p : nullptr; f.n_distinct = c.n_terms;
     } else if (s.kind == NRTGPU_SORT_SCORE) {
       if (i > 0) NRT_FAIL(NRTGPU_ERR_UNSUPPORTED, "a SCORE sort field is on the GPU path only in first position");
       o->score_first = true; o->score_reverse = s.reverse != 0;
@@ -2001,9 +2071,11 @@ int nrtgpu_merge_sorted_packed(nrtgpu_ctx* ctx, const nrtgpu_sort_field* fields,
   S.n_lists = n_lists; S.nq = nq; S.top_k = top_k; S.n_fields = n_fields; S.n_cmp = n_fields;
   for (int i = n_fields - 1; i >= 0; --i) {   // the fields after the first DOCID cannot decide anything
     const int32_t k = fields[i].kind;
-    if (k != NRTGPU_SORT_COLUMN && k != NRTGPU_SORT_DOCID && k != NRTGPU_SORT_SCORE) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_merge_sorted_packed: bad sort field kind");
+    if (k != NRTGPU_SORT_COLUMN && k != NRTGPU_SORT_DOCID && k != NRTGPU_SORT_SCORE && k != NRTGPU_SORT_KEYWORD)
+      NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_merge_sorted_packed: bad sort field kind");
     if (k == NRTGPU_SORT_DOCID) S.n_cmp = i + 1;
     S.kind[i] = k; S.reverse[i] = fields[i].reverse != 0;
+    if (k == NRTGPU_SORT_KEYWORD && fields[i].missing_value != 0) S.missing_last |= 1 << i;
   }
   NRT_CUDA_TRY(cudaSetDevice(ctx->device));
   sort_merge_kernel<<<(unsigned)nq, kSortMergeThreads, 0, (cudaStream_t)stream>>>(S);
@@ -2725,13 +2797,19 @@ int nrtgpu_rescore_combine(nrtgpu_ctx* ctx, int32_t nq, int32_t n_hits, const in
 // distinct values, and per leaf the codes that number its docs' values in it. A leaf whose dictionary is the union, or
 // which holds no value, counts through its own col_code; every other leaf through a renumbered copy (4 B per doc).
 // A keyword column's reader-wide dictionary is the byte-order union of the leaves' term dictionaries, built on the host
-// (bytes / off); values stays empty, and a leaf's codes (per doc or per value) are renumbered through its ordinal map.
+// (bytes / off); values stays empty, and a leaf's codes (per doc or per value) are renumbered through its ordinal map,
+// which is kept: keyword sorts map the leaf's FieldDoc values to the union through it, and after values back.
 struct ReaderDict {
   DevBuf<uint64_t> values;   // [n] ascending, the sortable domain of col_distinct
   int32_t n = 0;
   std::vector<uint8_t> bytes; std::vector<int64_t> off;   // keyword columns: term g of the union is bytes[off[g], off[g + 1])
   std::vector<std::unique_ptr<DevBuf<uint32_t>>> own;   // per leaf: the renumbered codes (unallocated where col_code serves)
   std::vector<const uint32_t*> codes;                   // per leaf: the codes its docs count through
+  // keyword columns, per leaf: whether its dictionary is the union, else its ordinal map (leaf term i -> union ordinal,
+  // ascending) on the host and on the device (unallocated for a leaf without terms)
+  std::vector<uint8_t> same;
+  std::vector<std::vector<uint32_t>> hmap;
+  std::vector<std::unique_ptr<DevBuf<uint32_t>>> dmap;
 };
 
 struct nrtgpu_searcher {
@@ -2766,22 +2844,28 @@ static int searcher_kw_dict(nrtgpu_searcher* s, int32_t column, cudaStream_t st,
   d->n = (int32_t)uni.size();
   d->off.assign(1, 0);
   for (const std::string& x : uni) { d->bytes.insert(d->bytes.end(), x.begin(), x.end()); d->off.push_back((int64_t)d->bytes.size()); }
-  DevBuf<uint32_t> map;
   int rc;
   for (const nrtgpu_index* ix : s->leaves) {
     const KeywordColumn& c = *ix->kw[(size_t)column];
     d->own.emplace_back(new DevBuf<uint32_t>);
+    d->dmap.emplace_back(new DevBuf<uint32_t>);
+    d->hmap.emplace_back();
+    d->same.push_back(c.n_terms == d->n ? 1 : 0);
     const int64_t n_codes = c.n_values;
-    if (c.n_terms == d->n || c.n_terms == 0 || n_codes == 0) { d->codes.push_back(c.codes.p); continue; }   // already reader-wide, or all 0
-    std::vector<uint32_t> m((size_t)c.n_terms);
+    if (c.n_terms == d->n || c.n_terms == 0) { d->codes.push_back(c.codes.p); continue; }   // already reader-wide, or all 0
+    std::vector<uint32_t>& m = d->hmap.back();
+    m.resize((size_t)c.n_terms);
     for (int32_t t = 0; t < c.n_terms; ++t) m[(size_t)t] = (uint32_t)(std::lower_bound(uni.begin(), uni.end(), term(c, t)) - uni.begin());
+    DevBuf<uint32_t>& map = *d->dmap.back();
+    if ((rc = map.upload_async(m.data(), m.size(), st))) return rc;
+    if (n_codes == 0) { d->codes.push_back(c.codes.p); continue; }
     DevBuf<uint32_t>& own = *d->own.back();
-    if ((rc = map.upload_async(m.data(), m.size(), st)) || (rc = own.alloc((size_t)n_codes))) return rc;
+    if ((rc = own.alloc((size_t)n_codes))) return rc;
     dict_remap_kernel<<<(unsigned)((n_codes + 255) / 256), 256, 0, st>>>(c.codes.p, n_codes, map.p, own.p);   // (per doc or per value)
     NRT_CUDA_TRY(cudaGetLastError());
-    NRT_CUDA_TRY(cudaStreamSynchronize(st));   // the map (and m) are reused by the next leaf
     d->codes.push_back(own.p);
   }
+  NRT_CUDA_TRY(cudaStreamSynchronize(st));
   *out = d.get();
   s->kw_dicts[column] = std::move(d);
   return NRTGPU_OK;
@@ -2791,6 +2875,33 @@ static int searcher_kw_dict(nrtgpu_searcher* s, int32_t column, cudaStream_t st,
 static bool searcher_has_kw(const nrtgpu_searcher* s, int32_t column) {
   for (const nrtgpu_index* ix : s->leaves) if (column < 0 || (size_t)column >= ix->kw.size()) return false;
   return true;
+}
+
+// The reader-wide dictionaries of the KEYWORD fields of a Sort (orders of the leaves of s, all of that Sort; built on st
+// when first asked for): dicts[j] (NULL for the other kinds), and per leaf l maps[l][j], its ordinal map to the union
+// (NULL where the leaf's dictionary is the union, or for the other kinds)
+static int searcher_sort_kw(nrtgpu_searcher* s, const nrtgpu_sort_order* o, cudaStream_t st, const ReaderDict** dicts,
+                            std::vector<std::array<const uint32_t*, kMaxSortFields>>* maps) {
+  maps->assign(s->leaves.size(), std::array<const uint32_t*, kMaxSortFields>{});
+  for (int j = 0; j < o->n_fields; ++j) {
+    dicts[j] = nullptr;
+    if (o->spec[j].kind != NRTGPU_SORT_KEYWORD) continue;
+    if (int rc = searcher_kw_dict(s, o->spec[j].column, st, &dicts[j])) return rc;
+    for (size_t l = 0; l < s->leaves.size(); ++l)
+      if (!dicts[j]->same[l]) (*maps)[l][(size_t)j] = dicts[j]->dmap[l]->p;
+  }
+  return NRTGPU_OK;
+}
+
+// a reader-wide KEYWORD code -> the code that leaf l's dictionary gives the same term (the leaf's terms are a subset of
+// the union, so its map m is ascending): a held union term 2g + 2 is the leaf's 2i + 2 when m[i] == g, else an odd code;
+// the gap 2g + 1 before union term g is the gap before the leaf's first term at or after it
+static int64_t kw_code_to_leaf(const ReaderDict& d, size_t l, int64_t c) {
+  if (c == 0 || d.same[l]) return c;
+  const std::vector<uint32_t>& m = d.hmap[l];
+  const uint32_t g = (uint32_t)((c - 1) / 2);
+  const size_t i = (size_t)(std::lower_bound(m.begin(), m.end(), g) - m.begin());
+  return (c % 2 == 0 && i < m.size() && m[i] == g) ? 2 * (int64_t)i + 2 : 2 * (int64_t)i + 1;
 }
 
 static int32_t ix_n_distinct(const nrtgpu_index* ix, int32_t c) {
@@ -2921,13 +3032,15 @@ static bool searcher_has_vectors(const nrtgpu_searcher* s) {
   return false;
 }
 
-// two sort orders rank by the same Sort: every field's kind and direction, and a column field's column, selector and missing value
+// two sort orders rank by the same Sort: every field's kind and direction, and a column or keyword field's column,
+// selector and missing value
 static bool same_sort(const nrtgpu_sort_order* a, const nrtgpu_sort_order* b) {
   if (a->n_fields != b->n_fields) return false;
   for (int i = 0; i < a->n_fields; ++i) {
     const nrtgpu_sort_field &x = a->spec[i], &y = b->spec[i];
     if (x.kind != y.kind || (x.reverse != 0) != (y.reverse != 0)) return false;
-    if (x.kind == NRTGPU_SORT_COLUMN && (x.column != y.column || x.selector != y.selector || x.missing_value != y.missing_value)) return false;
+    if ((x.kind == NRTGPU_SORT_COLUMN || x.kind == NRTGPU_SORT_KEYWORD) &&
+        (x.column != y.column || x.selector != y.selector || x.missing_value != y.missing_value)) return false;
   }
   return true;
 }
@@ -2947,6 +3060,17 @@ int nrtgpu_searcher_create(nrtgpu_ctx* ctx, nrtgpu_index* const* leaves, int32_t
 }
 
 int nrtgpu_searcher_close(nrtgpu_searcher* s) { delete s; return NRTGPU_OK; }
+
+int nrtgpu_searcher_keyword_seek(nrtgpu_searcher* s, int32_t column, const uint8_t* bytes, int32_t len, int64_t* code) {
+  if (!s || !code || (!bytes && len > 0) || len < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_keyword_seek: bad argument");
+  if (!searcher_has_kw(s, column)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_keyword_seek: keyword column out of range");
+  NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
+  std::lock_guard<std::mutex> g(s->mu);
+  const ReaderDict* d = nullptr;
+  if (int rc = searcher_kw_dict(s, column, nullptr, &d)) return rc;
+  *code = keyword_seek_code(d->bytes, d->off, d->n, bytes, len);
+  return NRTGPU_OK;
+}
 
 int nrtgpu_searcher_keyword_term(nrtgpu_searcher* s, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len,
                                  int32_t* n_terms) {
@@ -3017,10 +3141,33 @@ int nrtgpu_searcher_search_sorted_fields(nrtgpu_searcher* s, const nrtgpu_sort_o
   const int32_t nf = orders[0]->n_fields;
   const SortedRecordLayout L = sorted_record_layout(nq, top_k, nf);
   int rc;
+  // keyword fields: reader-wide after codes are checked against the union, then given to each leaf in its own dictionary,
+  // and each leaf's hit values are mapped to the union before the merge
+  const ReaderDict* kw[kMaxSortFields] = {};
+  std::vector<std::array<const uint32_t*, kMaxSortFields>> kw_maps;
+  if ((rc = searcher_sort_kw(s, orders[0], st, kw, &kw_maps))) return rc;
+  bool any_kw = false;
+  int32_t kw_n[kMaxSortFields] = {};
+  for (int j = 0; j < nf; ++j) if (kw[j]) { any_kw = true; kw_n[j] = kw[j]->n; }
+  if (any_kw && after_values && queries &&
+      (rc = check_keyword_after(orders[0], after_values, queries, nq, "nrtgpu_searcher_search_sorted_fields", kw_n))) return rc;
   if ((rc = s->records.alloc((size_t)L.words * n_leaves)) || (rc = s->merged.alloc((size_t)L.words))) return rc;
-  for (int l = 0; l < n_leaves; ++l)   // every leaf pages after the same reader-wide FieldDoc
-    if ((rc = nrtgpu_search_sorted_fields_packed(s->leaves[(size_t)l], orders[l], clauses, n_clauses, queries, nq, top_k, flags, after_values,
-                                                 limits, stream, s->records.p + (size_t)l * L.words))) return rc;
+  std::vector<int64_t> leaf_after;
+  for (int l = 0; l < n_leaves; ++l) {   // every leaf pages after the same reader-wide FieldDoc
+    const int64_t* av = after_values;
+    if (any_kw && after_values) {
+      leaf_after.assign(after_values, after_values + (size_t)nq * nf);
+      for (int j = 0; j < nf; ++j)
+        if (kw[j])
+          for (int q = 0; q < nq; ++q) leaf_after[(size_t)q * nf + j] = kw_code_to_leaf(*kw[j], (size_t)l, after_values[(size_t)q * nf + j]);
+      av = leaf_after.data();
+    }
+    int32_t* rec = s->records.p + (size_t)l * L.words;
+    if ((rc = nrtgpu_search_sorted_fields_packed(s->leaves[(size_t)l], orders[l], clauses, n_clauses, queries, nq, top_k, flags, av,
+                                                 limits, stream, rec))) return rc;
+    if (any_kw && (rc = sort_kw_values_to_union(kw_maps[(size_t)l].data(), nf, reinterpret_cast<int64_t*>(rec + L.values),
+                                                (int64_t)nq * top_k, st))) return rc;
+  }
   // TopFieldDocs.merge over the leaves
   if ((rc = nrtgpu_merge_sorted_packed(s->ctx, orders[0]->spec, nf, n_leaves, nq, top_k, s->records.p, s->merged.p, stream))) return rc;
   s->host.resize((size_t)L.words);
@@ -3202,6 +3349,19 @@ static int searcher_aggs(nrtgpu_searcher* s, const char* fn, const BatchRequest&
   for (int l = 0; l < n_leaves; ++l) {
     if ((rc = batch_build(bs[(size_t)l], s->leaves[(size_t)l], r, st)) || (rc = batch_set_limits(bs[(size_t)l], nullptr, st)) ||
         (rc = nrtgpu_batch_bind_packed(bs[(size_t)l], s->records.p + (size_t)l * words))) return rc;
+  }
+  // sorted top hits by a Sort with keyword fields: each leaf's hit values are mapped to the reader-wide dictionaries
+  for (int j = 0; j < n_nested && r.nested_sorts && n_leaves > 1; ++j) {
+    const nrtgpu_sort_order* const* orders = r.nested_sorts[j].orders;
+    if (!orders || nested[j].kind != NRTGPU_AGG_TOP_HITS) continue;
+    const ReaderDict* kw[kMaxSortFields] = {};
+    std::vector<std::array<const uint32_t*, kMaxSortFields>> maps;
+    if ((rc = searcher_sort_kw(s, orders[0], st, kw, &maps))) return rc;
+    for (int l = 0; l < n_leaves; ++l) {
+      std::vector<std::array<const uint32_t*, kMaxSortFields>>& m = bs[(size_t)l]->nest_kw_map;
+      m.resize((size_t)n_nested, std::array<const uint32_t*, kMaxSortFields>{});
+      m[(size_t)j] = maps[(size_t)l];
+    }
   }
   // the reader-wide tables live in leaf 0's workspace and are reset once; every leaf counts into them with its own codes
   AggTables t = {};

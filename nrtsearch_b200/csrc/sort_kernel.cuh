@@ -149,10 +149,15 @@ inline int sort_codes_build(const int64_t* c64, const int32_t* c32, const uint8_
 // asc. The posting kernel keys a hit by its rank: hi = ~rank, lo = ~doc (the COLUMN key with the rank as its code), or,
 // for [score, ...], hi = the ordered score, lo = ~rank (kSortScoreRank; the merge decodes the rank as the "doc", and
 // sort_fields_values_kernel maps it back through perm). A score, a tie code and a doc would not fit 64 bits together;
-// the rank holds the doc tie-break, which is why SCORE must lead.
+// the rank holds the doc tie-break, which is why SCORE must lead. A KEYWORD field is one more key pass
+// (sort_order_kw_keys_kernel): the posting kernels read the rank either way, never the field's values.
 constexpr int32_t kSortScoreRank = 4;   // internal sort kind of the posting kernels (beside NRTGPU_SORT_COLUMN / _DOCID)
 constexpr int kMaxSortFields = 8;
 
+// A KEYWORD field (NRTGPU_SORT_KEYWORD) reads a keyword column's codes (2i + 2 for term i of the image's dictionary, 0: no
+// value): `codes` per doc (SORTED), or per value behind the doc offsets `mv_off` (SORTED_SET, ascending within a doc);
+// `missing` is 0 (STRING_FIRST) or 1 (STRING_LAST). Its value is the selected code, so values compare as terms only
+// between codes of one dictionary.
 struct SortFieldDev {
   int32_t kind, reverse, selector, n_distinct;
   int64_t missing;
@@ -162,9 +167,23 @@ struct SortFieldDev {
   const uint64_t* distinct;
 };
 
-// the doc's value of one field: the column value (MIN / MAX selected on a multi-valued column) or missing; the global doc id
+// the keyword code of doc d (0: no value): SORTED its code; SORTED_SET the selector's pick of its n ascending codes
+// (SortedSetSelector: MIN [0], MAX [n-1], MIDDLE_MIN [(n-1)/2], MIDDLE_MAX [n/2])
+__device__ __forceinline__ uint32_t sort_kw_code(const SortFieldDev& f, int32_t d) {
+  if (!f.mv_off) return f.codes[d];
+  const int64_t a = f.mv_off[d], n = f.mv_off[d + 1] - a;
+  if (n == 0) return 0u;
+  const int64_t j = f.selector == NRTGPU_SELECT_MAX ? n - 1
+                  : f.selector == NRTGPU_SELECT_MIDDLE_MIN ? (n - 1) / 2
+                  : f.selector == NRTGPU_SELECT_MIDDLE_MAX ? n / 2 : 0;
+  return f.codes[a + j];
+}
+
+// the doc's value of one field: the column value (MIN / MAX selected on a multi-valued column) or missing; the global doc
+// id; a keyword's selected code
 __device__ __forceinline__ int64_t sort_field_value(const SortFieldDev& f, int32_t d, int32_t doc_base) {
   if (f.kind == NRTGPU_SORT_DOCID) return (int64_t)d + doc_base;
+  if (f.kind == NRTGPU_SORT_KEYWORD) return (int64_t)sort_kw_code(f, d);
   if (f.mv_off) {
     const int64_t a = f.mv_off[d], b = f.mv_off[d + 1];
     return a == b ? f.missing : f.c64[f.selector == NRTGPU_SELECT_MAX ? b - 1 : a];
@@ -172,8 +191,16 @@ __device__ __forceinline__ int64_t sort_field_value(const SortFieldDev& f, int32
   if (f.has && !f.has[d]) return f.missing;
   return f.c32 ? (int64_t)f.c32[d] : f.c64[d];
 }
+// ascending key of a keyword code: code 0 (no value) first or last by the missing rule, then the whole under reverse
+__host__ __device__ __forceinline__ uint64_t sort_kw_key(int32_t reverse, int64_t missing_last, int64_t code) {
+  const uint64_t k = code == 0 ? (missing_last ? ~0ull : 0ull) : (uint64_t)code;
+  return k ^ (reverse ? ~0ull : 0ull);
+}
 // ascending key of a value under the field's direction
-__device__ __forceinline__ uint64_t sort_field_key(const SortFieldDev& f, int64_t v) { return sortable_u64(v) ^ (f.reverse ? ~0ull : 0ull); }
+__device__ __forceinline__ uint64_t sort_field_key(const SortFieldDev& f, int64_t v) {
+  if (f.kind == NRTGPU_SORT_KEYWORD) return sort_kw_key(f.reverse, f.missing, v);
+  return sortable_u64(v) ^ (f.reverse ? ~0ull : 0ull);
+}
 
 // LSD pass keys, in the current perm order: 32-bit codes for single-valued columns, 64-bit keys otherwise
 __global__ void sort_order_keys32_kernel(SortFieldDev f, const int32_t* __restrict__ perm, int32_t n, uint32_t* __restrict__ keys) {
@@ -181,6 +208,14 @@ __global__ void sort_order_keys32_kernel(SortFieldDev f, const int32_t* __restri
   if (i >= n) return;
   uint32_t c = f.codes[perm[i]];
   if (c == 0u) c = sort_code_of(f.distinct, f.n_distinct, f.missing);
+  keys[i] = f.reverse ? ~c : c;
+}
+// keyword pass: the doc's selected code (codes stay below 2^31 + 2), 0 first or last by the missing rule, under reverse
+__global__ void sort_order_kw_keys_kernel(SortFieldDev f, const int32_t* __restrict__ perm, int32_t n, uint32_t* __restrict__ keys) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint32_t c = sort_kw_code(f, perm[i]);
+  if (c == 0u) c = f.missing ? 0xffffffffu : 0u;
   keys[i] = f.reverse ? ~c : c;
 }
 __global__ void sort_order_keys64_kernel(SortFieldDev f, const int32_t* __restrict__ perm, int32_t n, int32_t doc_base,
@@ -208,8 +243,9 @@ inline int sort_order_build(const SortFieldDev* f, int n_f, int32_t n, int32_t d
   sort_order_init_kernel<<<grid, 256, 0, st>>>(n, docid_last && f[n_f - 1].reverse, perm);
   NRT_CUDA_TRY(cudaGetLastError());
   for (int i = n_f - (docid_last ? 2 : 1); i >= 0; --i) {
-    if (f[i].codes) {
-      sort_order_keys32_kernel<<<grid, 256, 0, st>>>(f[i], perm, n, keys32);
+    if (f[i].kind == NRTGPU_SORT_KEYWORD || f[i].codes) {
+      if (f[i].kind == NRTGPU_SORT_KEYWORD) sort_order_kw_keys_kernel<<<grid, 256, 0, st>>>(f[i], perm, n, keys32);
+      else sort_order_keys32_kernel<<<grid, 256, 0, st>>>(f[i], perm, n, keys32);
       NRT_CUDA_TRY(cudaGetLastError());
       thrust::stable_sort_by_key(thrust::cuda::par.on(st), keys32, keys32 + n, perm);
     } else {
@@ -318,6 +354,7 @@ struct SortMergeLaunch {
   int32_t n_lists, nq, top_k, n_fields;
   int32_t n_cmp;                 // fields that decide: up to and including the first DOCID
   int32_t kind[kMaxSortFields], reverse[kMaxSortFields];
+  int32_t missing_last;              // bit f: KEYWORD field f is STRING_LAST (else STRING_FIRST)
 };
 
 // entries of query q in record r (clamped to [0, top_k])
@@ -326,12 +363,14 @@ __device__ __forceinline__ int sort_record_count(const int32_t* r, int64_t count
   return c < 0 ? 0 : (c > K ? K : c);
 }
 
-// ascending merge key of one FieldDoc value: COLUMN / DOCID by the sortable long, SCORE by its float bits, higher first
-__device__ __forceinline__ uint64_t sort_merge_key(int32_t kind, int32_t reverse, int64_t v) {
+// ascending merge key of one FieldDoc value: COLUMN / DOCID by the sortable long, SCORE by its float bits, higher first,
+// KEYWORD by its code under the missing rule (codes of one dictionary: the records' producer maps them there)
+__device__ __forceinline__ uint64_t sort_merge_key(int32_t kind, int32_t reverse, int64_t missing, int64_t v) {
   if (kind == NRTGPU_SORT_SCORE) {
     const uint32_t o = float_to_ordered(__uint_as_float((uint32_t)v));
     return (uint64_t)(reverse ? o : ~o);
   }
+  if (kind == NRTGPU_SORT_KEYWORD) return sort_kw_key(reverse, missing, v);
   return sortable_u64(v) ^ (reverse ? ~0ull : 0ull);
 }
 
@@ -375,7 +414,7 @@ __global__ void __launch_bounds__(kSortMergeThreads) sort_merge_kernel(SortMerge
       const int64_t* v = vals_l + (size_t)i * F;
       uint64_t ke[kMaxSortFields];
 #pragma unroll
-      for (int f = 0; f < kMaxSortFields; ++f) ke[f] = f < S.n_cmp ? sort_merge_key(S.kind[f], S.reverse[f], v[f]) : 0ull;
+      for (int f = 0; f < kMaxSortFields; ++f) ke[f] = f < S.n_cmp ? sort_merge_key(S.kind[f], S.reverse[f], (S.missing_last >> f) & 1, v[f]) : 0ull;
       int pos = i;
       for (int m = 0; m < S.n_lists && pos < K; ++m) {
         if (m == l) continue;
@@ -390,7 +429,7 @@ __global__ void __launch_bounds__(kSortMergeThreads) sort_merge_kernel(SortMerge
 #pragma unroll
           for (int f = 0; f < kMaxSortFields; ++f) {
             if (f < S.n_cmp && c == 0) {
-              const uint64_t k = sort_merge_key(S.kind[f], S.reverse[f], w[f]);
+              const uint64_t k = sort_merge_key(S.kind[f], S.reverse[f], (S.missing_last >> f) & 1, w[f]);
               c = k < ke[f] ? -1 : (k > ke[f] ? 1 : 0);
             }
           }
@@ -405,6 +444,22 @@ __global__ void __launch_bounds__(kSortMergeThreads) sort_merge_kernel(SortMerge
       }
     }
   }
+}
+
+// Over several leaves: the KEYWORD FieldDoc values of a leaf's hits, codes of the leaf's dictionary, become codes of the
+// reader-wide union before the leaves' records merge. map[j]: field j's leaf -> union ordinal map (NULL: not a keyword,
+// or the leaf's dictionary is the union). values [n][n_fields]; 0 (no value, or a slot past the count) stays 0.
+struct SortKwMapLaunch {
+  int64_t* values; int64_t n; int32_t n_fields;
+  const uint32_t* map[kMaxSortFields];
+};
+__global__ void sort_kw_map_kernel(SortKwMapLaunch S) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= S.n) return;
+  int64_t* v = S.values + i * S.n_fields;
+#pragma unroll
+  for (int j = 0; j < kMaxSortFields; ++j)   // (unrolled: map[] stays in parameter space)
+    if (j < S.n_fields && S.map[j] && v[j] != 0) v[j] = 2 * (int64_t)S.map[j][v[j] / 2 - 1] + 2;
 }
 
 // positions [start_hit, start_hit + w) of each list of a merged sorted record ([n][top_k], the leaves' sorted nested top

@@ -181,17 +181,28 @@ class SortType:
     "docid" or "score" (higher scores first unless reverse). field_type picks the missing value exactly as the reference's
     FieldDefs do (IntFieldDef.java:103, LongFieldDef.java:103, FloatFieldDef.java:105, DoubleFieldDef.java:105): MAX /
     +Infinity when missing_last, else MIN / -Infinity -- irrespective of reverse. selector: which value of a multi-valued
-    column sorts the doc, "min" (the default) or "max" (NumberFieldDef.java:266-278, SortedNumericSelector)."""
+    column sorts the doc, "min" (the default) or "max" (NumberFieldDef.java:266-278, SortedNumericSelector).
+    field_type "keyword": field is a keyword column of the shard (HostShard.keyword_columns), sorted by its term in
+    unsigned-byte order (AtomFieldDef.getSortField: SortField STRING, or SortedSetSortField on a multi-valued column,
+    whose selector may also be "middle_min" or "middle_max"); a doc without a value sorts first, or last when missing_last,
+    and reverse reverses the whole order, the missing position included. Its FieldDoc values are str, or None for no
+    value."""
     field: object            # column id, "docid" or "score"
     reverse: bool = False
     missing_last: bool = False
-    field_type: str = "long"   # int | long | float | double
+    field_type: str = "long"   # int | long | float | double | keyword
     selector: str = "min"
+
+    @property
+    def keyword(self) -> bool:
+        return self.field_type == "keyword" and self.field not in ("docid", "score")
 
     def missing_value(self) -> int:
         if self.field in ("docid", "score"):
             return 0
         hi = self.missing_last
+        if self.field_type == "keyword":   # STRING_FIRST 0 / STRING_LAST 1
+            return 1 if hi else 0
         if self.field_type == "int":
             return 2**31 - 1 if hi else -(2**31)
         if self.field_type == "long":
@@ -203,11 +214,83 @@ class SortType:
         raise ValueError(f"field type {self.field_type} does not support sorting")
 
     def c_field(self) -> _native.SortField:
+        if self.keyword:
+            if self.selector not in _SELECTORS:
+                raise ValueError(f"selector must be one of {', '.join(map(repr, _SELECTORS))}, not {self.selector!r}")
+            return _native.SortField(5, int(self.field), 1 if self.reverse else 0, _SELECTORS.index(self.selector),
+                                     self.missing_value())
         if self.selector not in ("min", "max"):
             raise ValueError(f"selector must be 'min' or 'max', not {self.selector!r}")
         kind = 3 if self.field == "score" else 2 if self.field == "docid" else 1
         return _native.SortField(kind, int(self.field) if kind == 1 else 0, 1 if self.reverse else 0,
                                  1 if self.selector == "max" else 0, self.missing_value())
+
+
+_SELECTORS = ("min", "max", "middle_min", "middle_max")   # NRTGPU_SELECT_*: SortedSetSelector.Type of a keyword sort
+
+
+def _keyword_sort_values(fields: Sequence[SortType], values: np.ndarray, names) -> np.ndarray:
+    """FieldDoc values [..., n_fields] of a Sort; with a keyword field, an object array whose keyword entries are str
+    (code 2i + 2: term i, through names(column, ords), a _TermNames) or None (code 0: no value) and whose other entries are
+    int; an all-numeric Sort's int64 array unchanged"""
+    kw = [j for j, f in enumerate(fields) if isinstance(f, SortType) and f.keyword]
+    if not kw:
+        return values
+    out = np.empty(values.shape, object)   # (None everywhere)
+    for j, f in enumerate(fields):
+        codes, col = values[..., j], out[..., j]   # (col: a view of out)
+        if j not in kw:
+            col[...] = codes
+            continue
+        held = codes != 0
+        col[held] = names(int(f.field), codes[held] // 2 - 1)
+    return out
+
+
+class _TermNames:
+    """The str of keyword terms by ordinal, per column, each looked up and decoded once (term(column, ord) -> bytes): a
+    page's keyword values become str by one indexing of the column's array, whatever its number of distinct terms."""
+
+    def __init__(self, term):
+        self.term, self.cols = term, {}
+
+    def __call__(self, column: int, ords: np.ndarray) -> np.ndarray:
+        ords = np.asarray(ords, np.int64)
+        names, have = self.cols.get(column, (np.empty(0, object), np.zeros(0, bool)))
+        hi = int(ords.max()) + 1 if len(ords) else 0
+        if hi > len(names):
+            m = max(hi, 2 * len(names))
+            names = np.concatenate([names, np.empty(m - len(names), object)])
+            have = np.concatenate([have, np.zeros(m - len(have), bool)])
+            self.cols[column] = (names, have)
+        for o in np.unique(ords[~have[ords]]):
+            names[o] = self.term(column, int(o)).decode("utf-8")
+            have[o] = True
+        return names[ords]
+
+
+def _after_row(fields: Sequence[SortType], a: "FieldDoc", seek) -> list:
+    """the int64 after values of FieldDoc a: a keyword field's str (or bytes) becomes its code through seek(column, bytes),
+    None the null code 0; an int is taken as a code already"""
+    vals = list(a.values) if a.values is not None else [a.value]
+    for j, f in enumerate(fields[:len(vals)]):
+        if isinstance(f, SortType) and f.keyword:
+            v = vals[j]
+            vals[j] = 0 if v is None else int(v) if isinstance(v, (int, np.integer)) else seek(int(f.field), _utf8_bytes(v))
+    return vals
+
+
+def _utf8_bytes(v) -> bytes:
+    return v.encode("utf-8") if isinstance(v, str) else bytes(v)
+
+
+def _seek(fn, *args) -> int:
+    """the sort code of one keyword term through nrtgpu_index_keyword_seek / nrtgpu_searcher_keyword_seek (fn bound to
+    its handle and column, args ending with the term's bytes)"""
+    code = C.c_int64()
+    t = args[-1]
+    check(fn(*args[:-1], t, len(t), C.byref(code)))
+    return int(code.value)
 
 
 @dataclass
@@ -305,10 +388,18 @@ class FilterCollector:
 _VALUE_TYPE = {"int": 0, "long": 0, "float": 1, "double": 2, "keyword": 3}
 
 
-def _keyword_keys(collectors: Sequence[object], outs: Sequence[object], term) -> None:
-    """Turns the ordinal keys of keyword terms collectors (and those nested in filter collectors) into str, in place;
-    term(column, ord) -> bytes"""
+def _keyword_keys(collectors: Sequence[object], outs: Sequence[object], term, term_names=None) -> None:
+    """Turns the ordinal keys of keyword terms collectors (and those nested in filter collectors) into str, and the
+    "sort_values" of top hits sorted by a Sort with a keyword field into object arrays (_keyword_sort_values), in place;
+    term(column, ord) -> bytes, term_names: the owner's _TermNames"""
     for c, o in zip(collectors, outs):
+        if isinstance(c, TopHitsCollector):
+            if c.sort is not None and "sort_values" in o:
+                o["sort_values"] = _keyword_sort_values(c.sort_fields(), o["sort_values"], term_names)
+            continue
+        if isinstance(c, TermsCollector) and "nested" in o:
+            tops = [(name, x) for name, x in c.nested if isinstance(x, TopHitsCollector)]
+            _keyword_keys([x for _, x in tops], [o["nested"][name] for name, _ in tops], term, term_names)
         if isinstance(c, TermsCollector) and c.field_type == "keyword":
             filled = np.arange(o["keys"].shape[1])[None, :] < np.asarray(o["n"])[:, None]
             ords, at = np.unique(o["keys"][filled], return_inverse=True)   # one lookup per distinct term of the batch
@@ -318,8 +409,8 @@ def _keyword_keys(collectors: Sequence[object], outs: Sequence[object], term) ->
             keys[filled] = names[at.reshape(-1)]
             o["keys"] = keys
         elif isinstance(c, FilterCollector):
-            names = [name for name, x in c.nested]
-            _keyword_keys([x for _, x in c.nested], [o[name] for name in names], term)
+            nested_names = [name for name, x in c.nested]
+            _keyword_keys([x for _, x in c.nested], [o[name] for name in nested_names], term, term_names)
 
 
 def _term_bytes(fn, *args) -> bytes:
@@ -335,14 +426,15 @@ def _term_bytes(fn, *args) -> bytes:
 @dataclass
 class FieldDoc:
     doc: int
-    value: int = 0   # fields[0], sortable-long domain
-    values: Optional[Tuple[int, ...]] = None   # every field of a multi-field Sort (a row of SortedResult.sort_values)
+    value: object = 0   # fields[0], sortable-long domain; a keyword field's str, or None for no value
+    values: Optional[Tuple[object, ...]] = None   # every field of a multi-field Sort (a row of SortedResult.sort_values)
 
 
 @dataclass
 class SortedResult:
     docs: np.ndarray          # int32 [nq, k]
-    sort_values: np.ndarray   # int64 [nq, k] FieldDoc.fields[0] of every hit; [nq, k, n_fields] for a sequence of SortTypes
+    sort_values: np.ndarray   # int64 [nq, k] FieldDoc.fields[0] of every hit; [nq, k, n_fields] for a sequence of SortTypes;
+                              # object (str / None for keyword fields, int else) when the Sort has a keyword field
     counts: np.ndarray
     total_hits: np.ndarray
     relation: np.ndarray
@@ -544,6 +636,7 @@ class GpuIndex:
         self.n_docs, self.doc_base = shard.n_docs, shard.doc_base
         self._orders = {}
         self._terms = {}
+        self.keyword_names = _TermNames(self.keyword_term)   # str of terms by ordinal (sorted pages' keyword values)
         if shard.post_positions is not None:
             self.add_positions(shard.post_positions)
         if pinned.n_keyword:
@@ -559,6 +652,11 @@ class GpuIndex:
         if key not in self._terms:
             self._terms[key] = _term_bytes(self._lib.nrtgpu_index_keyword_term, self.handle, column, ord_)
         return self._terms[key]
+
+    def keyword_seek(self, column: int, term: bytes) -> int:
+        """the sort code of `term` in keyword column `column` of this image (nrtgpu_index_keyword_seek): 2i + 2 for its
+        term i, 2i + 1 for a term it does not hold"""
+        return _seek(self._lib.nrtgpu_index_keyword_seek, self.handle, column, term)
 
     def add_positions(self, positions: np.ndarray):
         """Term positions of every posting, posting after posting (HostShard.post_positions): what PhraseQuery needs."""
@@ -937,6 +1035,10 @@ class GpuIndexSearcher:
                       search_after: Optional[Sequence[Optional[FieldDoc]]] = None, stream: int = 0) -> SortedResult:
         """IndexSearcher.search(query, TopFieldCollectorManager(sort, numHits, after, threshold)) for a batch."""
         st = collector.sort
+        if isinstance(st, SortType) and st.keyword:   # a one-field keyword Sort: a one-field order, sort_values [nq, k]
+            out = self._search_sorted_fields(queries, collector, [st], search_after, stream)
+            out.sort_values = out.sort_values.reshape(out.sort_values.shape[:2])
+            return out
         if not isinstance(st, SortType) or st.field == "score":
             return self._search_sorted_fields(queries, collector, [st] if isinstance(st, SortType) else list(st), search_after, stream)
         after_sd = None if search_after is None else [None if a is None else ScoreDoc(a.doc, 0.0) for a in search_after]
@@ -973,7 +1075,7 @@ class GpuIndexSearcher:
             av = np.zeros((nq, nf), np.int64)
             for i, a in enumerate(search_after):
                 if a is not None:
-                    av[i] = a.values if a.values is not None else (a.value,)
+                    av[i] = _after_row(fields, a, self.index.keyword_seek)
         lim = None
         if collector.timeout_sec > 0 or collector.terminate_after > 0:
             lim = SearchLimits(collector.timeout_sec, 0.0, 0, collector.terminate_after, 0)
@@ -982,6 +1084,7 @@ class GpuIndexSearcher:
                                                     C.c_void_p(stream), out.docs.ctypes.data, out.sort_values.ctypes.data,
                                                     out.counts.ctypes.data, out.total_hits.ctypes.data, out.relation.ctypes.data,
                                                     out.hit_timeout.ctypes.data, out.terminated_early.ctypes.data))
+        out.sort_values = _keyword_sort_values(fields, out.sort_values, self.index.keyword_names)
         return out
 
     def search_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
@@ -1001,7 +1104,7 @@ class GpuIndexSearcher:
             fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * 1)(self.index.sort_order(fields, stream).value))
             check(self._lib.nrtgpu_search_bool_aggs_sorted_hits(self.index.handle, carr, ncl, qarr, nq, k, 0, *fr.sorted_args,
                                                                 C.c_void_p(stream), *hits))
-            _keyword_keys(additional, fr.outs, self.index.keyword_term)
+            _keyword_keys(additional, fr.outs, self.index.keyword_term, self.index.keyword_names)
             return out, fr.outs
         aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         if n_nested:
@@ -1010,7 +1113,7 @@ class GpuIndexSearcher:
         else:
             check(self._lib.nrtgpu_search_bool_aggs(self.index.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
                                                     C.c_void_p(stream), *hits))
-        _keyword_keys(additional, outs, self.index.keyword_term)
+        _keyword_keys(additional, outs, self.index.keyword_term, self.index.keyword_names)
         return out, outs
 
     def search_tree_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
@@ -1026,7 +1129,7 @@ class GpuIndexSearcher:
         check(self._lib.nrtgpu_search_tree_aggs(self.index.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k, 0,
                                                 *fr.sorted_args, C.c_void_p(stream), out.docs.ctypes.data, out.scores.ctypes.data,
                                                 out.counts.ctypes.data, out.total_hits.ctypes.data))
-        _keyword_keys(additional, fr.outs, self.index.keyword_term)
+        _keyword_keys(additional, fr.outs, self.index.keyword_term, self.index.keyword_names)
         return out, fr.outs
 
     def score_docs(self, queries: Sequence[object], docs: np.ndarray, counts: Optional[np.ndarray] = None, stream: int = 0):
@@ -1129,6 +1232,7 @@ class GpuLeafSearcher:
         check(self._lib.nrtgpu_searcher_create(ctx.handle, arr, len(leaves), C.byref(h)))
         self.handle, self.leaves = h, list(leaves)
         self._terms = {}
+        self.keyword_names = _TermNames(self.keyword_term)   # str of reader-wide terms by ordinal
 
     def keyword_term(self, column: int, ord_: int) -> bytes:
         """reader-wide term `ord_` of keyword column `column`: the byte-order union of the leaves' dictionaries
@@ -1137,6 +1241,10 @@ class GpuLeafSearcher:
         if key not in self._terms:
             self._terms[key] = _term_bytes(lambda *a: self._lib.nrtgpu_searcher_keyword_term(*a, None), self.handle, column, ord_)
         return self._terms[key]
+
+    def keyword_seek(self, column: int, term: bytes) -> int:
+        """the sort code of `term` in the reader-wide dictionary of keyword column `column` (nrtgpu_searcher_keyword_seek)"""
+        return _seek(self._lib.nrtgpu_searcher_keyword_seek, self.handle, column, term)
 
     def search_batch(self, queries: Sequence[object], collector: RelevanceCollector, stream: int = 0,
                      search_after: Optional[Sequence[Optional[ScoreDoc]]] = None) -> BatchResult:
@@ -1174,7 +1282,7 @@ class GpuLeafSearcher:
             av = np.zeros((nq, nf), np.int64)
             for i, a in enumerate(search_after):
                 if a is not None:
-                    av[i] = a.values if a.values is not None else (a.value,)
+                    av[i] = _after_row(fields, a, self.keyword_seek)
         lim = None
         if collector.timeout_sec > 0 or collector.terminate_after > 0:
             lim = SearchLimits(collector.timeout_sec, 0.0, 0, collector.terminate_after, 0)
@@ -1184,6 +1292,7 @@ class GpuLeafSearcher:
                                                              out.docs.ctypes.data, out.sort_values.ctypes.data, out.counts.ctypes.data,
                                                              out.total_hits.ctypes.data, out.relation.ctypes.data,
                                                              out.hit_timeout.ctypes.data, out.terminated_early.ctypes.data))
+        out.sort_values = _keyword_sort_values(fields, out.sort_values, self.keyword_names)
         if isinstance(st, SortType) and st.field != "score":
             out.sort_values = out.sort_values.reshape(nq, k)
         return out
@@ -1250,14 +1359,14 @@ class GpuLeafSearcher:
                                                                          C.c_void_p(stream), out.docs.ctypes.data,
                                                                          out.scores.ctypes.data, out.counts.ctypes.data,
                                                                          out.total_hits.ctypes.data))
-            _keyword_keys(additional, fr.outs, self.keyword_term)
+            _keyword_keys(additional, fr.outs, self.keyword_term, self.keyword_names)
             return out, fr.outs
         aggs, res, narr, nres, n_nested, outs = _collector_records(nq, additional)
         check(self._lib.nrtgpu_searcher_search_bool_aggs_nested(self.handle, carr, ncl, qarr, nq, k, 0, aggs, len(additional), res,
                                                                 narr, n_nested, nres, C.c_void_p(stream), out.docs.ctypes.data,
                                                                 out.scores.ctypes.data, out.counts.ctypes.data,
                                                                 out.total_hits.ctypes.data))
-        _keyword_keys(additional, outs, self.keyword_term)
+        _keyword_keys(additional, outs, self.keyword_term, self.keyword_names)
         return out, outs
 
     def search_tree_with_collectors(self, queries: Sequence[object], collector: RelevanceCollector, additional: Sequence[object],
@@ -1273,7 +1382,7 @@ class GpuLeafSearcher:
         check(self._lib.nrtgpu_searcher_search_tree_aggs(self.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k, 0,
                                                          *fr.sorted_args, C.c_void_p(stream), out.docs.ctypes.data,
                                                          out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data))
-        _keyword_keys(additional, fr.outs, self.keyword_term)
+        _keyword_keys(additional, fr.outs, self.keyword_term, self.keyword_names)
         return out, fr.outs
 
     def close(self):

@@ -114,13 +114,17 @@ class SortedPackedGather:
     """The sorted counterpart of PackedGather: every rank's packed sorted record (docs, counts, flags, totalHits and the
     FieldDoc values of all queries; include/nrtgpu.h nrtgpu_sorted_packed_words), filled by
     nrtgpu_search_sorted_fields_packed, is all-gathered once, then nrtgpu_merge_sorted_packed does TopFieldDocs.merge on
-    every rank. fields: the Sort's SortTypes (search.SortType)."""
+    every rank. fields: the Sort's SortTypes (search.SortType). A Sort with a keyword field is refused: its values are
+    codes of each shard's own term dictionary, which do not compare across shards."""
 
     def __init__(self, nq: int, k: int, fields, world: int, device):
         import torch
         from . import _native
         self.nq, self.k, self.world = nq, k, world
         self.fields = list(fields)
+        if any(getattr(f, "field_type", None) == "keyword" and f.field not in ("docid", "score") for f in self.fields):
+            raise _native.NrtGpuUnsupported(3, "a Sort with a keyword field does not merge across shards: each shard numbers "
+                                               "its own term dictionary")
         self.n_fields = len(self.fields)
         self.words = (int(_native.gpu_lib().nrtgpu_sorted_packed_words(nq, k, self.n_fields)) if device.type == "cuda"
                       else sorted_packed_words(nq, k, self.n_fields))
