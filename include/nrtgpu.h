@@ -98,7 +98,8 @@ typedef struct {
   const int64_t* const* column_offsets; /* NULL, or [n_columns]: a non-NULL entry makes column c MULTI-valued (SORTED_NUMERIC doc
                                        values, reference NumberFieldDef.java multiValued): int64[n_docs+1] offsets into columns[c],
                                        which then holds the flattened values, ascending within a doc. A range clause matches a doc
-                                       when ANY of its values lies in [lo, hi] (SortedNumericDocValuesRangeQuery). nrtgpu_search_sorted,
+                                       when ANY of its values lies in [lo, hi] (SortedNumericDocValuesRangeQuery; keyword
+                                       columns take NRTGPU_KEYWORD_RANGE clauses with the same rule). nrtgpu_search_sorted,
                                        terms / min / max / sum collectors and fetch on such a column answer NRTGPU_ERR_UNSUPPORTED;
                                        nrtgpu_search_sorted_fields sorts on it (MIN / MAX selector). */
 } nrtgpu_shard_desc;
@@ -220,7 +221,8 @@ int nrtgpu_index_add_positions(nrtgpu_index* ix, const int32_t* positions, int64
 
 /* Keyword columns of an image (string doc values of atom / text-with-docValues fields: SortedDocValues and
  * SortedSetDocValues of the leaf). Column k of the call is keyword column k of the image; terms aggregations name it with
- * value_type NRTGPU_AGG_VALUE_KEYWORD. Per column:
+ * value_type NRTGPU_AGG_VALUE_KEYWORD, keyword sorts, NRTGPU_KEYWORD_RANGE clauses and NRTGPU_AGG_FILTER_KEYWORD_SET
+ * filters by its index. Per column:
  *   term_bytes / term_offsets [n_terms + 1]  the leaf's term dictionary, term i = term_bytes[term_offsets[i], term_offsets[i + 1]),
  *            strictly ascending in unsigned-byte order (BytesRef.compareTo); ordinal i is term i;
  *   multi_valued 0 (SORTED)      ords [n_docs]: the doc's ordinal, -1: no value;
@@ -251,6 +253,31 @@ int nrtgpu_index_keyword_term(const nrtgpu_index* ix, int32_t column, int32_t or
  * order). A searchAfter term from LastHitInfo becomes an after value this way. NRTGPU_ERR_INVALID: a column out of range,
  * code NULL, bytes NULL with len > 0, len < 0. */
 int nrtgpu_index_keyword_seek(const nrtgpu_index* ix, int32_t column, const uint8_t* bytes, int32_t len, int64_t* code);
+
+/* Keyword range clauses (TermRangeQuery and SortedSetDocValuesField.newSlowRangeQuery on an atom field, AtomFieldDef.getRangeQuery;
+ * PrefixQuery on an atom field with a constant-score rewrite, AtomFieldDef.getPrefixQuery). A clause of kind
+ * NRTGPU_KEYWORD_RANGE tests keyword column `id` (nrtgpu_index_add_keyword_columns) against the inclusive code range
+ * [lo, hi]: codes of the image's dictionary on an image, of the reader-wide union on a searcher (as keyword sort values).
+ * Ordinals follow unsigned-byte term order, so the terms a range or a prefix matches are one run of codes. A SORTED doc
+ * matches when its code is in [lo, hi], a SORTED_SET doc when any of its codes is; a doc without a value never matches.
+ * The clause is constant-score (score = boost) under every occur, exactly as NRTGPU_RANGE_I64, and every entry point that
+ * takes a range clause takes it (flat and tree batches, sorted search, collectors and their filter queries, kNN filter
+ * queries, the second pass, the micro-batcher). lo > hi is an empty range and matches no doc.
+ *   NRTGPU_ERR_INVALID: "keyword column out of range" (an image without keyword columns included), "keyword code out of
+ *   range" for lo or hi outside [1, 2n + 1] (n: the dictionary's terms).
+ * nrtgpu_index_keyword_range / nrtgpu_searcher_keyword_range turn term bounds into that range. With c = the
+ * nrtgpu_index_keyword_seek code of a bound (2i + 2 for a held term, 2i + 1 for the gap before term i):
+ *   lower inclusive lo = c, exclusive lo = c + 1 when c is even (else c), NO_LOWER lo = 1;
+ *   upper inclusive hi = c, exclusive hi = c - 1 when c is even (else c), NO_UPPER hi = 2n + 1;
+ *   PREFIX: lower is the prefix p (upper is unused): lo = seek(p), and the upper bound is succ(p) exclusive, where succ(p) is
+ *   p with its trailing 0xFF bytes dropped and its last byte incremented; an empty or all-0xFF prefix has no upper bound.
+ * The bounds are bytes as the field indexes them: applying the field's normalizer is the caller's. NRTGPU_ERR_INVALID: a
+ * keyword column out of range, lo or hi NULL, a bound NULL with a length > 0, a negative length, a bad flag. */
+enum { NRTGPU_KEYWORD_RANGE = 5 };
+enum { NRTGPU_KEYWORD_NO_LOWER = 1, NRTGPU_KEYWORD_NO_UPPER = 2, NRTGPU_KEYWORD_LOWER_EXCLUSIVE = 4,
+       NRTGPU_KEYWORD_UPPER_EXCLUSIVE = 8, NRTGPU_KEYWORD_PREFIX = 16 };
+int nrtgpu_index_keyword_range(const nrtgpu_index* ix, int32_t column, const uint8_t* lower, int32_t lower_len,
+                               const uint8_t* upper, int32_t upper_len, int32_t flags, int64_t* lo, int64_t* hi);
 
 /* Phrase leaves of query trees (PhraseQuery / match_phrase, reference QueryNodeMapper.java:285-291, :397-427). A clause of
  * kind NRTGPU_PHRASE is a leaf whose id indexes phrases[]; its boost is the leaf's folded boost, as for a term leaf. The
@@ -542,6 +569,11 @@ int nrtgpu_search_bool_aggs_nested(nrtgpu_index* ix, const nrtgpu_clause* clause
  *                      the set, by bit equality in that domain, so -0.0 != 0.0 and NaN == NaN as in Java's boxed equals.
  *                      Any order, duplicates allowed; n_values == 0 passes nothing. A set of another term type than the
  *                      field's never matches in the reference: the caller passes an empty set.
+ *   NRTGPU_AGG_FILTER_KEYWORD_SET  values[n_values] are keyword codes (nrtgpu_index_keyword_seek; reader-wide codes on a
+ *                      searcher) of keyword column `column` (SetQueryFilter over the TEXTTERMS of an atom field): a doc passes
+ *                      when the code of one of its terms is in the set (String equals). An odd code is a term the dictionary
+ *                      does not hold and matches nothing. NRTGPU_ERR_INVALID: a keyword column out of range, a code outside
+ *                      [1, 2n + 1].
  * Every query of the batch takes the same filters. Deleted docs never pass.
  * nrtgpu_search_bool_aggs_filtered: nrtgpu_search_bool_aggs_nested (every refusal, the same hits and results) plus filter
  * collectors; nrtgpu_search_bool_aggs and _aggs_nested are this call without filter records.
@@ -551,13 +583,13 @@ int nrtgpu_search_bool_aggs_nested(nrtgpu_index* ix, const nrtgpu_clause* clause
  *   The 8-aggregation cap counts the FILTER aggregations. Query trees and wide batches stay NRTGPU_ERR_UNSUPPORTED. A refused
  *   call writes no output. */
 enum { NRTGPU_AGG_FILTER = 6 };
-enum { NRTGPU_AGG_FILTER_QUERY = 1, NRTGPU_AGG_FILTER_VALUE_SET = 2 };
+enum { NRTGPU_AGG_FILTER_QUERY = 1, NRTGPU_AGG_FILTER_VALUE_SET = 2, NRTGPU_AGG_FILTER_KEYWORD_SET = 4 };   /* (3 stays a bad filter kind) */
 typedef struct {
-  int32_t kind;           /* NRTGPU_AGG_FILTER_QUERY / _VALUE_SET */
+  int32_t kind;           /* NRTGPU_AGG_FILTER_QUERY / _VALUE_SET / _KEYWORD_SET */
   int32_t query;          /* QUERY: index into filter_queries */
-  int32_t column;         /* VALUE_SET */
-  int32_t n_values;       /* VALUE_SET */
-  const int64_t* values;  /* VALUE_SET: [n_values] */
+  int32_t column;         /* VALUE_SET: numeric column; KEYWORD_SET: keyword column */
+  int32_t n_values;       /* VALUE_SET, KEYWORD_SET */
+  const int64_t* values;  /* VALUE_SET: [n_values] sortable longs; KEYWORD_SET: [n_values] keyword codes */
 } nrtgpu_agg_filter;
 int nrtgpu_search_bool_aggs_filtered(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses,
                                      const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
@@ -869,6 +901,12 @@ int nrtgpu_searcher_keyword_term(nrtgpu_searcher* s, int32_t column, int32_t ord
  * dictionary gives the same term, and its hits' codes are mapped to the union on the device before the merge; sorted top
  * hits over the leaves likewise. NRTGPU_ERR_INVALID: a column some leaf lacks, and the refusals of the image call. */
 int nrtgpu_searcher_keyword_seek(nrtgpu_searcher* s, int32_t column, const uint8_t* bytes, int32_t len, int64_t* code);
+/* nrtgpu_index_keyword_range in the reader-wide dictionary of keyword column `column`: the code range of an
+ * NRTGPU_KEYWORD_RANGE clause on a searcher. Keyword clauses (in queries, filter queries and kNN filter queries) and keyword
+ * value sets of a searcher carry reader-wide codes; each leaf receives them mapped to its own dictionary. NRTGPU_ERR_INVALID:
+ * a column some leaf lacks, and the refusals of the image call. */
+int nrtgpu_searcher_keyword_range(nrtgpu_searcher* s, int32_t column, const uint8_t* lower, int32_t lower_len,
+                                  const uint8_t* upper, int32_t upper_len, int32_t flags, int64_t* lo, int64_t* hi);
 int nrtgpu_searcher_search_bool_aggs_nested(nrtgpu_searcher* s, const nrtgpu_clause* clauses, int32_t n_clauses,
                                             const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t flags,
                                             const nrtgpu_aggregation* aggs, int32_t n_aggs, const nrtgpu_aggregation_result* results,

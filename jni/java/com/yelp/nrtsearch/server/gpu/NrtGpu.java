@@ -95,6 +95,18 @@ public final class NrtGpu {
   /** keywordSeek in a searcher's reader-wide dictionary (the codes of searcherSearchSortedFields). */
   public static native long searcherKeywordSeek(long searcher, int column, ByteBuffer term, int len);
 
+  /** Keyword range clauses (clause kind 5, KEYWORD_RANGE): flags of keywordRange. */
+  public static final int KEYWORD_NO_LOWER = 1, KEYWORD_NO_UPPER = 2, KEYWORD_LOWER_EXCLUSIVE = 4, KEYWORD_UPPER_EXCLUSIVE = 8,
+      KEYWORD_PREFIX = 16;
+
+  /**
+   * The code range of a TermRangeQuery or PrefixQuery on an atom field: out (two longs) receives [lo, hi] for a KEYWORD_RANGE
+   * clause, in the image's dictionary (searcher 0) or the searcher's reader-wide one. The bounds are the field's normalized
+   * bytes (AtomFieldDef.normalize).
+   */
+  public static native int keywordRange(long index, long searcher, int column, ByteBuffer lower, int lowerLen, ByteBuffer upper,
+                                        int upperLen, int flags, ByteBuffer out);
+
   /**
    * Query trees with PhraseQuery leaves: phrases = nrtgpu_phrase[nPhrases] referenced by clauses of kind 4 (PHRASE),
    * phraseTerms = nrtgpu_phrase_term[nPhraseTerms] (term id, PhraseQuery position); otherwise as searchTree, which it is

@@ -180,6 +180,18 @@ JNIEXPORT jlong JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searcherKeywor
   if (fail(env, nrtgpu_searcher_keyword_seek((nrtgpu_searcher*)(intptr_t)s, column, (const uint8_t*)ADDR(env, term), len, &code))) return -1;
   return code;
 }
+/* the code range [lo, hi] of a keyword range clause (NRTGPU_KEYWORD_RANGE) from term bounds (direct ByteBuffers; flags
+ * NRTGPU_KEYWORD_*: NO_LOWER 1, NO_UPPER 2, LOWER_EXCLUSIVE 4, UPPER_EXCLUSIVE 8, PREFIX 16) into out[0..1] (a direct
+ * ByteBuffer of two longs), in an image's dictionary (searcher == 0) or a searcher's reader-wide one; 0 or the refusal's code */
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_keywordRange(JNIEnv* env, jclass c, jlong ix, jlong s, jint column,
+                                                                              jobject lower, jint lowerLen, jobject upper,
+                                                                              jint upperLen, jint flags, jobject out) {
+  int64_t* o = (int64_t*)ADDR(env, out);
+  const uint8_t* lo = (const uint8_t*)ADDR(env, lower);
+  const uint8_t* hi = (const uint8_t*)ADDR(env, upper);
+  return s ? fail(env, nrtgpu_searcher_keyword_range((nrtgpu_searcher*)(intptr_t)s, column, lo, lowerLen, hi, upperLen, flags, o, o + 1))
+           : fail(env, nrtgpu_index_keyword_range((const nrtgpu_index*)(intptr_t)ix, column, lo, lowerLen, hi, upperLen, flags, o, o + 1));
+}
 /* phrases / phraseTerms: direct ByteBuffers laid out as nrtgpu_phrase[] / nrtgpu_phrase_term[] (nPhrases 0: searchTree) */
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTreePhrases(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,

@@ -161,6 +161,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_search_tree_aggs", "nrtgpu_searcher_search_tree_aggs",
     "nrtgpu_index_add_keyword_columns", "nrtgpu_index_keyword_term", "nrtgpu_searcher_keyword_term",
     "nrtgpu_index_keyword_seek", "nrtgpu_searcher_keyword_seek",
+    "nrtgpu_index_keyword_range", "nrtgpu_searcher_keyword_range",
 ]
 
 _gpu = None
@@ -214,6 +215,9 @@ def gpu_lib() -> C.CDLL:
                                                      C.POINTER(C.c_int32)]
         lib.nrtgpu_index_keyword_seek.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_int64)]
         lib.nrtgpu_searcher_keyword_seek.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_int64)]
+        for fn in (lib.nrtgpu_index_keyword_range, lib.nrtgpu_searcher_keyword_range):
+            fn.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32, C.c_char_p, C.c_int32, C.c_int32, C.POINTER(C.c_int64),
+                           C.POINTER(C.c_int64)]
         lib.nrtgpu_search_tree_phrases.argtypes = [C.c_void_p, C.POINTER(Clause), C.c_int32, C.POINTER(Node), C.c_int32,
                                                    C.POINTER(Phrase), C.c_int32, C.POINTER(PhraseTerm), C.c_int32, C.POINTER(Query),
                                                    C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(SearchLimits), C.c_void_p] + \

@@ -2,7 +2,7 @@
 // KnnUtils.java:135-155), evaluated on the device into one bitmap row per distinct filter of a call:
 // uint32[n_rows][ceil(n_docs / 32)], bit d set iff live doc d matches the filter. Rows are built word-parallel:
 //   * a term clause reads the bitmap of its term, built once per call by scattering the term's postings (cost ~ df);
-//   * a range clause runs range_matches with one lane per doc, a warp ballot forms the word;
+//   * a range clause runs range_matches (a keyword range keyword_matches) with one lane per doc, a warp ballot forms the word;
 //   * match-all is ~0;
 //   * the words combine as eval_clauses (query_eval.cuh) matches: AND of MUST / FILTER, minus the OR of MUST_NOT, and at least
 //     need_should SHOULD clauses per bit (a bit-sliced counter); an empty query gives 0.
@@ -54,6 +54,20 @@ struct KnnFilterRowsLaunch {
   int32_t* row_cnt;             // [n_rows] matching docs, zeroed
 };
 
+// word w0 + lane of a keyword range clause's row, as the range branch of knn_filter_rows_kernel forms it: for word w0 + j
+// lane l tests doc 32 (w0 + j) + l, a warp ballot forms the word (out of line: inlined, it makes the kernel spill)
+__device__ __noinline__ uint32_t keyword_row_word(const uint32_t* codes, const int64_t* off, int32_t n_docs, int64_t lo, int64_t hi,
+                                                  int w0, int lane) {
+  uint32_t x = 0u;
+  for (int j = 0; j < 32; ++j) {
+    const int64_t doc = 32ll * (w0 + j) + lane;
+    const bool m = doc < n_docs && keyword_codes_match(codes, off, (int32_t)doc, lo, hi);
+    const uint32_t b = __ballot_sync(0xffffffffu, m);
+    if (lane == j) x = b;
+  }
+  return x;
+}
+
 // one thread per (row, word); a warp covers 32 consecutive words of one row
 __global__ void __launch_bounds__(256) knn_filter_rows_kernel(KnnFilterRowsLaunch L) {
   const int row = L.row0 + blockIdx.y, lane = threadIdx.x & 31;
@@ -73,6 +87,8 @@ __global__ void __launch_bounds__(256) knn_filter_rows_kernel(KnnFilterRowsLaunc
         const uint32_t b = __ballot_sync(0xffffffffu, m);
         if (lane == j) x = b;
       }
+    } else if (c.kind == NRTGPU_KEYWORD_RANGE) {
+      x = keyword_row_word(L.ix.kw_codes[c.col], L.ix.kw_off[c.col], L.ix.n_docs, c.lo, c.hi, w0, lane);
     } else {
       x = ~0u;
     }
@@ -107,10 +123,12 @@ __global__ void __launch_bounds__(256) knn_filter_rows_kernel(KnnFilterRowsLaunc
 // The row of a filter collector's value set (FilterCollectorManager.SetQueryFilter over a TermInSetQuery): bit d is set iff
 // live doc d has a value of `column` in set[0 .. n_set), sorted and distinct in the column's sortable-long domain, so a
 // match is bit equality (-0.0 != 0.0, NaN == NaN, as Java's boxed equals). One lane per doc and a warp ballot per word, as
-// the range branch above; a multi-valued doc passes when any of its values is in the set.
+// the range branch above; a multi-valued doc passes when any of its values is in the set. A keyword set
+// (NRTGPU_AGG_FILTER_KEYWORD_SET) holds codes of keyword column `column`: a doc passes when one of its terms' codes is in
+// it (a set holds no code 0, so a doc without a value never passes).
 struct AggValueSetLaunch {
   DevIndexView ix;
-  int32_t column, n_set, words;
+  int32_t column, n_set, words, keyword;
   const int64_t* set;
   uint32_t* row;   // [words]
 };
@@ -126,8 +144,12 @@ __global__ void __launch_bounds__(256) agg_value_set_kernel(AggValueSetLaunch L)
   bool m = false;
   if (doc < L.ix.n_docs && L.n_set > 0) {
     const int32_t d = (int32_t)doc;
-    const int64_t* off = L.ix.colmv_off ? L.ix.colmv_off[L.column] : nullptr;
-    if (off) {
+    const int64_t* off = L.keyword ? L.ix.kw_off[L.column] : L.ix.colmv_off ? L.ix.colmv_off[L.column] : nullptr;
+    if (L.keyword) {
+      const uint32_t* v = L.ix.kw_codes[L.column];
+      if (off) for (int64_t j = off[d]; j < off[d + 1] && !m; ++j) m = in_sorted_set(L.set, L.n_set, (int64_t)__ldg(v + j));
+      else m = in_sorted_set(L.set, L.n_set, (int64_t)__ldg(v + d));
+    } else if (off) {
       const int64_t* v = L.ix.colmv_val[L.column];
       for (int64_t j = off[d]; j < off[d + 1] && !m; ++j) m = in_sorted_set(L.set, L.n_set, v[j]);
     } else {

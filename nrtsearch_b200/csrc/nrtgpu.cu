@@ -204,6 +204,8 @@ struct nrtgpu_index {
   std::vector<uint8_t> col_multi;                            // [n_columns] 1 = multi-valued
   std::vector<std::unique_ptr<KeywordColumn>> kw;            // keyword columns (nrtgpu_index_add_keyword_columns)
   std::vector<int32_t> kw_n_terms;
+  DevBuf<const uint32_t*> kw_code_ptrs;                      // [kw] the columns' codes, for the keyword clauses of DevIndexView
+  DevBuf<const int64_t*> kw_off_ptrs;                        // [kw] SORTED_SET doc offsets, NULL for SORTED
   bool kw_added = false;
   DevBuf<uint32_t> live_bits;
   // vectors
@@ -244,6 +246,7 @@ struct nrtgpu_index {
     v.dense_tf = dense_tf.p; v.dense_stride = dense_stride; v.dense_tf2 = dense_tf2.p;
     v.gran_tab = gran_tab.p; v.n_gran = gran_n;
     v.positions = positions.p; v.pos_off = pos_off.p; v.pos_base = pos_base.p;
+    v.kw_codes = kw_code_ptrs.p; v.kw_off = kw_off_ptrs.p;
     return v;
   }
   PlanDict dict() const {   // what batch compilation and planning read
@@ -788,6 +791,11 @@ int nrtgpu_index_add_keyword_columns(nrtgpu_index* ix, const nrtgpu_keyword_colu
     bytes += (int64_t)(x->codes.bytes() + x->doc_off.bytes());
     kw.push_back(std::move(x));
   }
+  if (n > 0) {   // (no image reads these before kw_added is set)
+    std::vector<const uint32_t*> cp; std::vector<const int64_t*> op;
+    for (auto& x : kw) { cp.push_back(x->codes.p); op.push_back(x->multi ? x->doc_off.p : nullptr); }
+    if ((rc = ix->kw_code_ptrs.upload(cp.data(), cp.size())) || (rc = ix->kw_off_ptrs.upload(op.data(), op.size()))) return rc;
+  }
   ix->kw = std::move(kw);
   for (auto& x : ix->kw) ix->kw_n_terms.push_back(x->n_terms);
   ix->kw_added = true;
@@ -803,26 +811,20 @@ static void copy_term(const std::vector<uint8_t>& bytes, const std::vector<int64
   if (out && cap > 0 && l > 0) std::memcpy(out, bytes.data() + a, (size_t)std::min<int64_t>(l, cap));
 }
 
-// the sort code of term t[0 .. len) in a host dictionary of n terms (bytes, off): 2i + 2 for term i, else 2i + 1 where i
-// terms sort before it (unsigned bytes, then length: BytesRef order)
-static int64_t keyword_seek_code(const std::vector<uint8_t>& bytes, const std::vector<int64_t>& off, int32_t n, const uint8_t* t,
-                                 int32_t len) {
-  auto cmp = [&](int32_t i) {   // term i against t: < 0, 0, > 0
-    const int64_t a = off[(size_t)i], l = off[(size_t)i + 1] - a, m = std::min<int64_t>(l, len);
-    const int c = m > 0 ? std::memcmp(bytes.data() + a, t, (size_t)m) : 0;
-    return c != 0 ? c : (l < len ? -1 : (l > len ? 1 : 0));
-  };
-  int32_t lo = 0, hi = n;   // the first term that does not sort before t
-  while (lo < hi) { const int32_t m = lo + (hi - lo) / 2; if (cmp(m) < 0) lo = m + 1; else hi = m; }
-  return (lo < n && cmp(lo) == 0) ? 2 * (int64_t)lo + 2 : 2 * (int64_t)lo + 1;
-}
-
 int nrtgpu_index_keyword_seek(const nrtgpu_index* ix, int32_t column, const uint8_t* bytes, int32_t len, int64_t* code) {
   if (!ix || !code || (!bytes && len > 0) || len < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_seek: bad argument");
   if (column < 0 || (size_t)column >= ix->kw.size()) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_seek: keyword column out of range");
   const KeywordColumn& c = *ix->kw[(size_t)column];
-  *code = keyword_seek_code(c.bytes, c.off, c.n_terms, bytes, len);
+  *code = keyword_seek_code(c.bytes.data(), c.off.data(), c.n_terms, bytes, len);
   return NRTGPU_OK;
+}
+
+int nrtgpu_index_keyword_range(const nrtgpu_index* ix, int32_t column, const uint8_t* lower, int32_t lower_len, const uint8_t* upper,
+                               int32_t upper_len, int32_t flags, int64_t* lo, int64_t* hi) {
+  if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_range: NULL index");
+  if (column < 0 || (size_t)column >= ix->kw.size()) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_keyword_range: keyword column out of range");
+  const KeywordColumn& c = *ix->kw[(size_t)column];
+  return keyword_range_codes(c.bytes.data(), c.off.data(), c.n_terms, lower, lower_len, upper, upper_len, flags, lo, hi);
 }
 
 int nrtgpu_index_keyword_term(const nrtgpu_index* ix, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len) {
@@ -2559,6 +2561,7 @@ static int batch_filter_rows(nrtgpu_batch* b, const BatchRequest& r, cudaStream_
     row_of[(size_t)i] = (int32_t)(row_filter.size() + k);
     AggValueSetLaunch L;
     L.ix = ix->view(); L.column = cb.agg_filters[(size_t)i].column; L.n_set = (int32_t)(set_at[k + 1] - set_at[k]); L.words = words;
+    L.keyword = cb.agg_filters[(size_t)i].kind == NRTGPU_AGG_FILTER_KEYWORD_SET;
     L.set = b->agg_set.p + set_at[k]; L.row = b->agg_rows.p + (size_t)row_of[(size_t)i] * words;
     agg_value_set_kernel<<<(unsigned)(((int64_t)words * 32 + 255) / 256), 256, 0, st>>>(L);
     NRT_CUDA_TRY(cudaGetLastError());
@@ -2904,6 +2907,95 @@ static int64_t kw_code_to_leaf(const ReaderDict& d, size_t l, int64_t c) {
   return (c % 2 == 0 && i < m.size() && m[i] == g) ? 2 * (int64_t)i + 2 : 2 * (int64_t)i + 1;
 }
 
+// Keyword clauses and keyword value sets of a searcher's request carry reader-wide codes; each leaf receives a copy of
+// the clause array (and of the filter records) with its codes mapped by kw_code_to_leaf. That map is monotone and sends a
+// union term the leaf lacks to the leaf's gap code beside it, so an inclusive bound keeps exactly the leaf terms that lie
+// inside the union bound: for a leaf term with union ordinal u, 2u + 2 >= lo iff its leaf code >= the mapped lo (a lo on
+// a held term maps onto that term; one on a missing term or a gap maps onto the gap before the first leaf term above it),
+// and symmetrically for hi. The argument is the one behind the sorted after values. A set code maps to the leaf's code of
+// the same term, or to an odd code, which matches nothing, where the leaf lacks it. Leaves whose dictionary is the union
+// (same[l]) take the caller's arrays.
+struct KwLeafRequest {
+  const ReaderDict* dict[kMaxAggs] = {};                  // per aggregation: the dictionary of a keyword set
+  std::vector<const ReaderDict*> clause_dict, filter_dict;   // per clause / filter clause: a keyword clause's dictionary
+  bool any = false;
+  std::vector<nrtgpu_clause> clauses, filter_clauses;     // leaf copies
+  std::vector<nrtgpu_agg_filter> filters;
+  std::vector<std::vector<int64_t>> sets;
+};
+
+// the reader-wide dictionaries of the keyword clauses of cl[0 .. n), their columns and codes checked against the union
+// with the messages of the single-image call
+static int searcher_kw_clauses(nrtgpu_searcher* s, const nrtgpu_clause* cl, int32_t n, cudaStream_t st,
+                               std::vector<const ReaderDict*>* dicts, bool* any) {
+  dicts->assign((size_t)std::max(n, 0), nullptr);
+  for (int32_t i = 0; cl && i < n; ++i) {
+    if (cl[i].kind != NRTGPU_KEYWORD_RANGE) continue;
+    if (!searcher_has_kw(s, cl[i].id)) NRT_FAIL(NRTGPU_ERR_INVALID, "keyword range: keyword column out of range");
+    const ReaderDict* d = nullptr;
+    if (int rc = searcher_kw_dict(s, cl[i].id, st, &d)) return rc;
+    const int64_t top = 2 * (int64_t)d->n + 1;
+    if (cl[i].lo < 1 || cl[i].lo > top || cl[i].hi < 1 || cl[i].hi > top) NRT_FAIL(NRTGPU_ERR_INVALID, "keyword range: keyword code out of range");
+    (*dicts)[(size_t)i] = d;
+    *any = true;
+  }
+  return NRTGPU_OK;
+}
+
+// the keyword clauses, filter clauses and keyword sets of request r on searcher s (caller holds s->mu)
+static int searcher_kw_request(nrtgpu_searcher* s, const BatchRequest& r, cudaStream_t st, KwLeafRequest* k) {
+  int rc;
+  if ((rc = searcher_kw_clauses(s, r.clauses, r.n_clauses, st, &k->clause_dict, &k->any))) return rc;
+  if ((rc = searcher_kw_clauses(s, r.filter_clauses, r.n_filter_clauses, st, &k->filter_dict, &k->any))) return rc;
+  for (int i = 0; i < std::min(r.n_aggs, kMaxAggs) && r.agg_filters && r.aggs; ++i) {
+    const nrtgpu_agg_filter& f = r.agg_filters[i];
+    if (r.aggs[i].kind != NRTGPU_AGG_FILTER || f.kind != NRTGPU_AGG_FILTER_KEYWORD_SET) continue;
+    if (!searcher_has_kw(s, f.column)) NRT_FAIL(NRTGPU_ERR_INVALID, "filter aggregation: keyword column out of range");
+    if (f.n_values < 0 || (f.n_values > 0 && !f.values)) NRT_FAIL(NRTGPU_ERR_INVALID, "filter aggregation: bad value set");
+    if ((rc = searcher_kw_dict(s, f.column, st, &k->dict[i]))) return rc;
+    for (int32_t v = 0; v < f.n_values; ++v)
+      if (f.values[v] < 1 || f.values[v] > 2 * (int64_t)k->dict[i]->n + 1)
+        NRT_FAIL(NRTGPU_ERR_INVALID, "filter aggregation: keyword code out of range");
+    k->any = true;
+  }
+  return NRTGPU_OK;
+}
+
+// cl[0 .. n) with the keyword codes of leaf l (dicts from searcher_kw_clauses), in buf, or cl itself when nothing changes
+static const nrtgpu_clause* kw_leaf_clauses(const std::vector<const ReaderDict*>& dicts, const nrtgpu_clause* cl, int32_t n, size_t l,
+                                            std::vector<nrtgpu_clause>& buf) {
+  bool change = false;
+  for (int32_t i = 0; i < n; ++i) change |= dicts[(size_t)i] && !dicts[(size_t)i]->same[l];
+  if (!change) return cl;
+  buf.assign(cl, cl + n);
+  for (int32_t i = 0; i < n; ++i)
+    if (const ReaderDict* d = dicts[(size_t)i]) { buf[(size_t)i].lo = kw_code_to_leaf(*d, l, cl[i].lo); buf[(size_t)i].hi = kw_code_to_leaf(*d, l, cl[i].hi); }
+  return buf.data();
+}
+
+// request r as leaf l of the searcher receives it (k from searcher_kw_request)
+static BatchRequest kw_leaf_request(KwLeafRequest& k, const BatchRequest& r, size_t l) {
+  BatchRequest x = r;
+  if (!k.any) return x;
+  x.clauses = kw_leaf_clauses(k.clause_dict, r.clauses, r.n_clauses, l, k.clauses);
+  x.filter_clauses = kw_leaf_clauses(k.filter_dict, r.filter_clauses, r.n_filter_clauses, l, k.filter_clauses);
+  bool sets = false;
+  const int n_aggs = std::min(r.n_aggs, kMaxAggs);
+  for (int i = 0; i < n_aggs; ++i) sets |= k.dict[i] && !k.dict[i]->same[l];
+  if (sets) {
+    k.filters.assign(r.agg_filters, r.agg_filters + r.n_aggs);
+    k.sets.assign((size_t)n_aggs, {});
+    for (int i = 0; i < n_aggs; ++i) {
+      if (!k.dict[i]) continue;
+      nrtgpu_agg_filter& f = k.filters[(size_t)i];
+      for (int32_t v = 0; v < f.n_values; ++v) k.sets[(size_t)i].push_back(kw_code_to_leaf(*k.dict[i], l, f.values[v]));
+      f.values = k.sets[(size_t)i].data();
+    }
+    x.agg_filters = k.filters.data();
+  }
+  return x;
+}
+
 static int32_t ix_n_distinct(const nrtgpu_index* ix, int32_t c) {
   return (size_t)c < ix->col_n_distinct.size() ? ix->col_n_distinct[(size_t)c] : 0;
 }
@@ -3068,8 +3160,19 @@ int nrtgpu_searcher_keyword_seek(nrtgpu_searcher* s, int32_t column, const uint8
   std::lock_guard<std::mutex> g(s->mu);
   const ReaderDict* d = nullptr;
   if (int rc = searcher_kw_dict(s, column, nullptr, &d)) return rc;
-  *code = keyword_seek_code(d->bytes, d->off, d->n, bytes, len);
+  *code = keyword_seek_code(d->bytes.data(), d->off.data(), d->n, bytes, len);
   return NRTGPU_OK;
+}
+
+int nrtgpu_searcher_keyword_range(nrtgpu_searcher* s, int32_t column, const uint8_t* lower, int32_t lower_len, const uint8_t* upper,
+                                  int32_t upper_len, int32_t flags, int64_t* lo, int64_t* hi) {
+  if (!s) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_keyword_range: NULL searcher");
+  if (!searcher_has_kw(s, column)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_keyword_range: keyword column out of range");
+  NRT_CUDA_TRY(cudaSetDevice(s->ctx->device));
+  std::lock_guard<std::mutex> g(s->mu);
+  const ReaderDict* d = nullptr;
+  if (int rc = searcher_kw_dict(s, column, nullptr, &d)) return rc;
+  return keyword_range_codes(d->bytes.data(), d->off.data(), d->n, lower, lower_len, upper, upper_len, flags, lo, hi);
 }
 
 int nrtgpu_searcher_keyword_term(nrtgpu_searcher* s, int32_t column, int32_t ord, uint8_t* out, int32_t cap, int32_t* len,
@@ -3101,9 +3204,15 @@ int nrtgpu_searcher_search_bool(nrtgpu_searcher* s, const nrtgpu_clause* clauses
   const int n_leaves = (int)s->leaves.size();
   int rc;
   if ((rc = s->records.alloc((size_t)words * n_leaves)) || (rc = s->merged.alloc((size_t)words))) return rc;
-  for (int l = 0; l < n_leaves; ++l)   // every leaf runs the whole batch (LeafCollector per segment), results stay on the device
-    if ((rc = nrtgpu_search_bool_packed(s->leaves[(size_t)l], clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags, limits,
+  std::vector<const ReaderDict*> kw;   // keyword clauses: each leaf receives their codes in its own dictionary
+  std::vector<nrtgpu_clause> leaf_clauses;
+  bool any_kw = false;
+  if ((rc = searcher_kw_clauses(s, clauses, n_clauses, st, &kw, &any_kw))) return rc;
+  for (int l = 0; l < n_leaves; ++l) {   // every leaf runs the whole batch (LeafCollector per segment), results stay on the device
+    const nrtgpu_clause* cl = any_kw ? kw_leaf_clauses(kw, clauses, n_clauses, (size_t)l, leaf_clauses) : clauses;
+    if ((rc = nrtgpu_search_bool_packed(s->leaves[(size_t)l], cl, n_clauses, queries, nq, top_k, total_hits_threshold, flags, limits,
                                         stream, s->records.p + (size_t)l * words))) return rc;
+  }
   // TopDocs.merge over the leaves (LazyQueueTopScoreDocCollectorManager.java:137-144)
   if ((rc = nrtgpu_merge_topk_packed(s->ctx, n_leaves, nq, top_k, s->records.p, s->merged.p, stream))) return rc;
   s->host.resize((size_t)words);
@@ -3152,6 +3261,10 @@ int nrtgpu_searcher_search_sorted_fields(nrtgpu_searcher* s, const nrtgpu_sort_o
   if (any_kw && after_values && queries &&
       (rc = check_keyword_after(orders[0], after_values, queries, nq, "nrtgpu_searcher_search_sorted_fields", kw_n))) return rc;
   if ((rc = s->records.alloc((size_t)L.words * n_leaves)) || (rc = s->merged.alloc((size_t)L.words))) return rc;
+  std::vector<const ReaderDict*> kw_cl;   // keyword clauses, mapped per leaf as the after codes are
+  std::vector<nrtgpu_clause> leaf_clauses;
+  bool any_kw_cl = false;
+  if ((rc = searcher_kw_clauses(s, clauses, n_clauses, st, &kw_cl, &any_kw_cl))) return rc;
   std::vector<int64_t> leaf_after;
   for (int l = 0; l < n_leaves; ++l) {   // every leaf pages after the same reader-wide FieldDoc
     const int64_t* av = after_values;
@@ -3163,7 +3276,8 @@ int nrtgpu_searcher_search_sorted_fields(nrtgpu_searcher* s, const nrtgpu_sort_o
       av = leaf_after.data();
     }
     int32_t* rec = s->records.p + (size_t)l * L.words;
-    if ((rc = nrtgpu_search_sorted_fields_packed(s->leaves[(size_t)l], orders[l], clauses, n_clauses, queries, nq, top_k, flags, av,
+    const nrtgpu_clause* cl = any_kw_cl ? kw_leaf_clauses(kw_cl, clauses, n_clauses, (size_t)l, leaf_clauses) : clauses;
+    if ((rc = nrtgpu_search_sorted_fields_packed(s->leaves[(size_t)l], orders[l], cl, n_clauses, queries, nq, top_k, flags, av,
                                                  limits, stream, rec))) return rc;
     if (any_kw && (rc = sort_kw_values_to_union(kw_maps[(size_t)l].data(), nf, reinterpret_cast<int64_t*>(rec + L.values),
                                                 (int64_t)nq * top_k, st))) return rc;
@@ -3193,9 +3307,12 @@ int nrtgpu_searcher_search_tree_phrases(nrtgpu_searcher* s, const nrtgpu_clause*
   BatchRequest r = tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags);
   int rc = phrase_request(&r, phrases, n_phrases, phrase_terms, n_phrase_terms);
   if (rc) return rc;
+  KwLeafRequest kw;
   return searcher_scored(s, "nrtgpu_searcher_search_tree_phrases", nq, top_k, stream, [&](int l, int32_t* d_record) {
+    // (the leaves run in order under the searcher's lock: the first prepares the keyword codes of every leaf)
+    if (l == 0) { if (int rc2 = searcher_kw_request(s, r, (cudaStream_t)stream, &kw)) return rc2; }
     SearchOut o; o.d_record = d_record; o.record_limits = true;
-    return search_bool_impl(s->leaves[(size_t)l], r, limits, stream, o);
+    return search_bool_impl(s->leaves[(size_t)l], kw_leaf_request(kw, r, (size_t)l), limits, stream, o);
   }, out_docs, out_scores, out_counts, out_total_hits, out_relation, out_hit_timeout, out_terminated_early);
 }
 
@@ -3223,10 +3340,16 @@ int nrtgpu_searcher_search_knn_filtered(nrtgpu_searcher* s, const float* queries
   if (!searcher_has_vectors(s)) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn_filtered: no leaf has a vector field");
   if (nq <= 0 || n_filters < 0) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn_filtered: nq must be > 0 and n_filters >= 0");
   if (k <= 0 || k > kMaxTopK) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_searcher_search_knn_filtered: k out of range");
+  std::vector<const ReaderDict*> kw;
+  std::vector<nrtgpu_clause> leaf_clauses;
+  bool any_kw = false;
   return searcher_scored(s, "nrtgpu_searcher_search_knn_filtered", nq, k, stream, [&](int l, int32_t* d_record) {
+    // (the leaves run in order under the searcher's lock: the first checks the keyword clauses against the union)
+    if (l == 0) { if (int rc = searcher_kw_clauses(s, filter_clauses, n_filter_clauses, (cudaStream_t)stream, &kw, &any_kw)) return rc; }
     nrtgpu_index* ix = s->leaves[(size_t)l];
+    const nrtgpu_clause* cl = any_kw ? kw_leaf_clauses(kw, filter_clauses, n_filter_clauses, (size_t)l, leaf_clauses) : filter_clauses;
     return knn_leaf_record(ix, nq, k, stream, d_record, [&](int32_t* d, float* sc, int32_t* c) {
-      return nrtgpu_search_knn_filtered(ix, queries, nq, k, boosts, filter_clauses, n_filter_clauses, filters, n_filters, filter_of,
+      return nrtgpu_search_knn_filtered(ix, queries, nq, k, boosts, cl, n_filter_clauses, filters, n_filters, filter_of,
                                         stream, d, sc, c);
     });
   }, out_docs, out_scores, out_counts, nullptr, nullptr, nullptr, nullptr);
@@ -3320,10 +3443,15 @@ static int searcher_aggs(nrtgpu_searcher* s, const char* fn, const BatchRequest&
   cudaStream_t st = (cudaStream_t)stream;
   std::lock_guard<std::mutex> g(s->mu);
   const int n_leaves = (int)s->leaves.size();
+  KwLeafRequest kw;   // keyword clauses and sets: reader-wide codes, checked against the union, mapped per leaf
+  if ((rc = searcher_kw_request(s, r, st, &kw))) return rc;
+  std::vector<KwLeafRequest> kw_leaf((size_t)n_leaves, kw);   // (each leaf's request points into its own copies)
+  std::vector<BatchRequest> lr;
+  for (int l = 0; l < n_leaves; ++l) lr.push_back(kw_leaf_request(kw_leaf[(size_t)l], r, (size_t)l));
   {   // every refusal of the single-image call, on every leaf's columns, before any batch is built
     CompiledBatch cb;
-    for (nrtgpu_index* ix : s->leaves)
-      if ((rc = compile_batch(ix->dict(), r, &cb))) return rc;
+    for (int l = 0; l < n_leaves; ++l)
+      if ((rc = compile_batch(s->leaves[(size_t)l]->dict(), lr[(size_t)l], &cb))) return rc;
   }
   // the reader-wide dictionaries, and the table limits of the single-image call at their size
   const ReaderDict* dict[kMaxAggs] = {};
@@ -3347,7 +3475,7 @@ static int searcher_aggs(nrtgpu_searcher* s, const char* fn, const BatchRequest&
   const int64_t words = nrtgpu_packed_words(nq, top_k);
   if ((rc = s->records.alloc((size_t)words * n_leaves)) || (rc = s->merged.alloc((size_t)words))) return rc;
   for (int l = 0; l < n_leaves; ++l) {
-    if ((rc = batch_build(bs[(size_t)l], s->leaves[(size_t)l], r, st)) || (rc = batch_set_limits(bs[(size_t)l], nullptr, st)) ||
+    if ((rc = batch_build(bs[(size_t)l], s->leaves[(size_t)l], lr[(size_t)l], st)) || (rc = batch_set_limits(bs[(size_t)l], nullptr, st)) ||
         (rc = nrtgpu_batch_bind_packed(bs[(size_t)l], s->records.p + (size_t)l * words))) return rc;
   }
   // sorted top hits by a Sort with keyword fields: each leaf's hit values are mapped to the reader-wide dictionaries

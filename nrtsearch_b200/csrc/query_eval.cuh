@@ -36,6 +36,10 @@ struct DevIndexView {
   const int32_t* positions;
   const uint32_t* pos_off;       // [P]
   const int64_t* pos_base;       // [n_terms + 1]
+  // keyword columns (nrtgpu_index_add_keyword_columns; NULL without): codes 2i + 2 of ordinal i, 0 = no value, per doc
+  // (SORTED: kw_off[k] NULL) or per value behind the doc offsets kw_off[k] (SORTED_SET, ascending within a doc)
+  const uint32_t* const* kw_codes;
+  const int64_t* const* kw_off;
 };
 
 // numeric range clause on one doc (IndexOrDocValuesQuery's doc-values side, reference IntFieldDef.java:124-158 inclusive
@@ -53,6 +57,35 @@ __device__ __forceinline__ bool range_matches(const DevIndexView& ix, int col, i
   const int64_t x = ix.col32[col] ? (int64_t)__ldg(ix.col32[col] + doc) : __ldg(ix.col64[col] + doc);
   return x >= lo && x <= hi;
 }
+
+// keyword range clause on one doc (NRTGPU_KEYWORD_RANGE: TermRangeQuery / PrefixQuery over ordinals in byte order, lo >= 1
+// as compiled, so a doc without a value -- code 0 -- never matches): SORTED = its code is in [lo, hi]; SORTED_SET = ANY of
+// its codes is, found as range_matches finds a multi-valued value
+__device__ __forceinline__ bool keyword_codes_match(const uint32_t* v, const int64_t* off, int32_t doc, int64_t lo, int64_t hi) {
+  if (off) {
+    int64_t a = off[doc], b = off[doc + 1];
+    const int64_t end = b;
+    while (a < b) { const int64_t m = (a + b) >> 1; if ((int64_t)__ldg(v + m) < lo) a = m + 1; else b = m; }
+    return a < end && (int64_t)__ldg(v + a) <= hi;
+  }
+  const int64_t x = (int64_t)__ldg(v + doc);
+  return x >= lo && x <= hi;
+}
+__device__ __forceinline__ bool keyword_matches(const DevIndexView& ix, int col, int32_t doc, int64_t lo, int64_t hi) {
+  return keyword_codes_match(ix.kw_codes[col], ix.kw_off[col], doc, lo, hi);
+}
+
+// keyword_matches out of line: the flat clause rule's hot loop then keeps the numeric range test as it was, and only a
+// keyword clause pays the call
+__device__ __noinline__ bool keyword_matches_call(const DevIndexView& ix, const DevClause& c, int32_t doc) {
+  return keyword_matches(ix, c.col, doc, c.lo, c.hi);
+}
+
+// a doc-value clause (numeric or keyword range) on one doc
+__device__ __forceinline__ bool dv_clause_matches(const DevIndexView& ix, const DevClause& c, int32_t doc) {
+  return c.kind == NRTGPU_RANGE_I64 ? range_matches(ix, c.col, doc, c.lo, c.hi) : keyword_matches(ix, c.col, doc, c.lo, c.hi);
+}
+__device__ __forceinline__ bool is_dv_clause(int kind) { return kind == NRTGPU_RANGE_I64 || kind == NRTGPU_KEYWORD_RANGE; }
 
 // exact tf of posting (clause c, doc) when the byte saturated: find the posting, then the exception list
 __device__ __noinline__ float exact_freq_slow(const DevIndexView& ix, const DevClause& c, int32_t doc) {
@@ -73,22 +106,23 @@ __device__ __noinline__ float exact_freq_slow(const DevIndexView& ix, const DevC
 //   term_mask: bit s set iff term slot s is present, for an engine that knows it before scoring (a doc missing a required
 //              slot or holding an excluded one is rejected at once); an engine that does not passes q.req_term_mask.
 //   term(c, &s): whether term clause c is present in doc; if it is and c.scoring, sets s to its BM25 float.
-// Doc-value clauses are evaluated before any term is scored: a doc that fails a required range (or holds an excluded one)
-// costs no norm gather, as ConjunctionDISI advances the cheapest iterators first. Ranges have no side effects and the sums
-// stay in clause order, so the order changes no result.
+// Doc-value clauses (numeric and keyword ranges) and match-all clauses are evaluated before any term is scored: a doc that
+// fails a required range (or holds an excluded one) costs no norm gather, as ConjunctionDISI advances the cheapest
+// iterators first. They have no side effects and the sums stay in clause order, so the order changes no result.
 template <class TermScore>
 __device__ __forceinline__ bool eval_clauses(const DevIndexView& ix, const DevQuery& q, const DevClause* cl,
                                              int32_t doc, uint32_t term_mask, TermScore term, float* out_score) {
   if ((term_mask & q.req_term_mask) != q.req_term_mask) return false;
   if (term_mask & q.not_term_mask) return false;
   if (ix.live_bits && !((ix.live_bits[doc >> 5] >> (doc & 31)) & 1u)) return false;
-  uint32_t range_present = 0;
+  uint32_t nonterm_present = 0;   // bit i: clause i is a doc-value clause that matches, or a match-all clause
   if (q.has_nonterm)
     for (int i = 0; i < q.n_clauses; ++i) {
       const DevClause& c = cl[i];
-      if (c.kind != NRTGPU_RANGE_I64) continue;
-      const bool p = range_matches(ix, c.col, doc, c.lo, c.hi);
-      if (p) { if (c.occur == NRTGPU_MUST_NOT) return false; range_present |= 1u << i; }
+      if (c.kind == NRTGPU_TERM) continue;
+      const bool p = c.kind == NRTGPU_RANGE_I64 ? range_matches(ix, c.col, doc, c.lo, c.hi)
+                   : c.kind == NRTGPU_KEYWORD_RANGE ? keyword_matches_call(ix, c, doc) : true;
+      if (p) { if (c.occur == NRTGPU_MUST_NOT) return false; nonterm_present |= 1u << i; }
       else if (c.occur == NRTGPU_MUST || c.occur == NRTGPU_FILTER) return false;
     }
   double must_sum = 0.0, should_sum = 0.0;
@@ -99,11 +133,8 @@ __device__ __forceinline__ bool eval_clauses(const DevIndexView& ix, const DevQu
     float s = 0.0f;
     if (c.kind == NRTGPU_TERM) {
       present = term(c, &s);
-    } else if (c.kind == NRTGPU_RANGE_I64) {
-      present = (range_present >> i) & 1u;
-      s = c.weight;
     } else {
-      present = true;
+      present = (nonterm_present >> i) & 1u;
       s = c.weight;
     }
     if (!present) {
@@ -151,8 +182,8 @@ __device__ __forceinline__ bool eval_node(const DevIndexView& ix, const DevNode&
     float s = 0.0f;
     if (c.kind == NRTGPU_TERM || c.kind == NRTGPU_PHRASE) {
       present = term(c, &s);
-    } else if (c.kind == NRTGPU_RANGE_I64) {
-      present = range_matches(ix, c.col, doc, c.lo, c.hi);
+    } else if (is_dv_clause(c.kind)) {
+      present = dv_clause_matches(ix, c, doc);
       s = c.weight;
     } else if (c.kind == NRTGPU_NODE) {
       present = (node_match >> c.node) & 1u;

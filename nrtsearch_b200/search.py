@@ -54,6 +54,37 @@ class RangeQuery:
 
 
 @dataclass(frozen=True)
+class KeywordRangeQuery:
+    """TermRangeQuery on an atom field (AtomFieldDef.getRangeQuery; SortedSetDocValuesField.newSlowRangeQuery on a field
+    with doc values only): keyword column `column` (HostShard.keyword_columns) has a term in the range, in unsigned-byte
+    order. lower / upper: str (UTF-8) or bytes, already normalized as the field indexes its terms, or None for an open
+    end. Constant-score: a matching doc scores the boost, as RangeQuery does. Usable wherever RangeQuery is; each searcher
+    turns it into a code range of its dictionary (keyword_range)."""
+    column: int
+    lower: object = None
+    upper: object = None
+    include_lower: bool = True
+    include_upper: bool = True
+
+
+@dataclass(frozen=True)
+class KeywordPrefixQuery:
+    """PrefixQuery on an atom field (AtomFieldDef.getPrefixQuery) with a constant-score rewrite: keyword column `column`
+    has a term starting with `prefix` (str or bytes). Usable wherever RangeQuery is, as KeywordRangeQuery."""
+    column: int
+    prefix: object = b""
+
+
+@dataclass(frozen=True)
+class _KeywordCodes:
+    """a KeywordRangeQuery / KeywordPrefixQuery resolved by a searcher: the inclusive code range [lo, hi] of keyword column
+    `column` in its dictionary (an NRTGPU_KEYWORD_RANGE clause)"""
+    column: int
+    lo: int
+    hi: int
+
+
+@dataclass(frozen=True)
 class MatchAllDocsQuery:
     pass
 
@@ -358,7 +389,9 @@ class ValueSetFilter:
     """The set filter of a FilterCollector (FilterCollectorManager.SetQueryFilter over a TermInSetQuery): a doc passes when one
     of its values of `column` (single- or multi-valued) is in `values`, numbers of the field's type compared as Java's boxed
     equals does, by their bits (-0.0 != 0.0, NaN == NaN). A set of another term type than the field's never matches in the
-    reference: the adaptor passes an empty set for it."""
+    reference: the adaptor passes an empty set for it. field_type "keyword": column is a keyword column
+    (HostShard.keyword_columns) and values are its terms (str or bytes), matched as String.equals does (the TEXTTERMS set of
+    an atom field); each searcher turns them into codes of its dictionary."""
     column: int
     values: tuple
     field_type: str = "long"
@@ -386,6 +419,66 @@ class FilterCollector:
 
 
 _VALUE_TYPE = {"int": 0, "long": 0, "float": 1, "double": 2, "keyword": 3}
+
+# nrtgpu_index_keyword_range flags
+_KW_NO_LOWER, _KW_NO_UPPER, _KW_LOWER_EXCLUSIVE, _KW_UPPER_EXCLUSIVE, _KW_PREFIX = 1, 2, 4, 8, 16
+
+
+@dataclass(frozen=True)
+class _KeywordCodeSet:
+    """a keyword ValueSetFilter resolved by a searcher: the codes of its terms in the searcher's dictionary
+    (NRTGPU_AGG_FILTER_KEYWORD_SET)"""
+    column: int
+    codes: tuple
+
+
+def _keyword_range(fn, handle, column: int, q) -> Tuple[int, int]:
+    """the code range of a KeywordRangeQuery / KeywordPrefixQuery through nrtgpu_index_keyword_range /
+    nrtgpu_searcher_keyword_range (fn) on handle"""
+    if isinstance(q, KeywordPrefixQuery):
+        lower, upper, flags = _utf8_bytes(q.prefix), b"", _KW_PREFIX
+    else:
+        flags = 0
+        lower = b"" if q.lower is None else _utf8_bytes(q.lower)
+        upper = b"" if q.upper is None else _utf8_bytes(q.upper)
+        flags |= _KW_NO_LOWER if q.lower is None else (0 if q.include_lower else _KW_LOWER_EXCLUSIVE)
+        flags |= _KW_NO_UPPER if q.upper is None else (0 if q.include_upper else _KW_UPPER_EXCLUSIVE)
+    lo, hi = C.c_int64(), C.c_int64()
+    check(fn(handle, column, lower, len(lower), upper, len(upper), flags, C.byref(lo), C.byref(hi)))
+    return lo.value, hi.value
+
+
+def _resolve_keywords(q, searcher):
+    """q with every KeywordRangeQuery / KeywordPrefixQuery turned into _KeywordCodes and every keyword ValueSetFilter into
+    a _KeywordCodeSet by searcher.keyword_range / keyword_seek (its own dictionary), through BooleanQuery,
+    DisjunctionMaxQuery, BoostQuery and FilterCollector; q itself when it holds none"""
+    if isinstance(q, (KeywordRangeQuery, KeywordPrefixQuery)):
+        return _KeywordCodes(q.column, *searcher.keyword_range(q))
+    if isinstance(q, BoostQuery):
+        sub = _resolve_keywords(q.query, searcher)
+        return q if sub is q.query else BoostQuery(sub, q.boost)
+    if isinstance(q, BooleanQuery):
+        subs = [_resolve_keywords(c.query, searcher) for c in q.clauses]
+        if all(x is c.query for x, c in zip(subs, q.clauses)):
+            return q
+        return BooleanQuery([BooleanClause(x, c.occur) for x, c in zip(subs, q.clauses)], q.minimum_number_should_match)
+    if isinstance(q, DisjunctionMaxQuery):
+        subs = [_resolve_keywords(d, searcher) for d in q.disjuncts]
+        return q if all(x is d for x, d in zip(subs, q.disjuncts)) else DisjunctionMaxQuery(subs, q.tie_breaker)
+    if isinstance(q, ValueSetFilter) and q.field_type == "keyword":
+        return _KeywordCodeSet(q.column, tuple(searcher.keyword_seek(q.column, _utf8_bytes(v)) for v in q.values))
+    if isinstance(q, FilterCollector):
+        f = _resolve_keywords(q.filter, searcher)
+        nested = tuple((name, _resolve_keywords(c, searcher)) for name, c in q.nested)
+        if f is q.filter and all(x is c for (_, x), (_, c) in zip(nested, q.nested)):
+            return q
+        return FilterCollector(f, nested)
+    return q
+
+
+def _resolve_all(items, searcher):
+    """_resolve_keywords over a sequence (None entries kept)"""
+    return None if items is None else [None if x is None else _resolve_keywords(x, searcher) for x in items]
 
 
 def _keyword_keys(collectors: Sequence[object], outs: Sequence[object], term, term_names=None) -> None:
@@ -460,6 +553,10 @@ def _flatten(q, boost: np.float32, out: list, occur: Occur) -> None:
         out.append((int(occur), 1, int(q.column), float(boost), int(q.lower), int(q.upper)))
     elif isinstance(q, MatchAllDocsQuery):
         out.append((int(occur), 2, 0, float(boost), 0, 0))
+    elif isinstance(q, _KeywordCodes):
+        out.append((int(occur), 5, int(q.column), float(boost), int(q.lo), int(q.hi)))
+    elif isinstance(q, (KeywordRangeQuery, KeywordPrefixQuery)):
+        raise ValueError(f"{type(q).__name__} is resolved to codes by a searcher (GpuIndexSearcher / GpuLeafSearcher)")
     else:
         raise NrtGpuUnsupported(3, f"query node {type(q).__name__} is outside the GPU path")
 
@@ -657,6 +754,11 @@ class GpuIndex:
         """the sort code of `term` in keyword column `column` of this image (nrtgpu_index_keyword_seek): 2i + 2 for its
         term i, 2i + 1 for a term it does not hold"""
         return _seek(self._lib.nrtgpu_index_keyword_seek, self.handle, column, term)
+
+    def keyword_range(self, q) -> Tuple[int, int]:
+        """the code range [lo, hi] of a KeywordRangeQuery / KeywordPrefixQuery in this image's dictionary
+        (nrtgpu_index_keyword_range)"""
+        return _keyword_range(self._lib.nrtgpu_index_keyword_range, self.handle, q.column, q)
 
     def add_positions(self, positions: np.ndarray):
         """Term positions of every posting, posting after posting (HostShard.post_positions): what PhraseQuery needs."""
@@ -858,10 +960,13 @@ class _FilteredRecords:
             o = {"doc_count": np.zeros(nq, np.int32)}
             self.res.append(CAggResult(None, None, o["doc_count"].ctypes.data, None, None, None))
             f = a.filter
-            if isinstance(f, ValueSetFilter):
-                vals = np.ascontiguousarray(f.sortable(), np.int64)
+            if isinstance(f, (ValueSetFilter, _KeywordCodeSet)):
+                keyword = isinstance(f, _KeywordCodeSet)
+                if not keyword and f.field_type == "keyword":
+                    raise ValueError("a keyword ValueSetFilter is resolved to codes by a searcher")
+                vals = np.ascontiguousarray(np.array(f.codes, np.int64) if keyword else f.sortable(), np.int64)
                 self.keep.append(vals)
-                self.filters[i] = CAggFilter(2, 0, f.column, len(vals), vals.ctypes.data if len(vals) else None)
+                self.filters[i] = CAggFilter(4 if keyword else 2, 0, f.column, len(vals), vals.ctypes.data if len(vals) else None)
             else:
                 self.filters[i] = CAggFilter(1, len(self.filter_queries), 0, 0, None)
                 self.filter_queries.append(f)
@@ -960,7 +1065,7 @@ class GpuIndexSearcher:
                 search_after: Optional[Sequence[Optional[ScoreDoc]]] = None, flags: int = 0) -> PreparedBatch:
         if search_after is None and collector.search_after is not None:
             search_after = [collector.search_after] * len(queries)
-        carr, ncl, qarr, nq = compile_queries(queries, search_after)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self.index), search_after)
         return PreparedBatch(self.index, carr, ncl, qarr, nq, collector.num_hits_to_collect,
                              collector.total_hits_threshold, flags)
 
@@ -969,7 +1074,7 @@ class GpuIndexSearcher:
         """One call through the C ABI with HOST buffers (nrtgpu_search_bool)."""
         if search_after is None and collector.search_after is not None:
             search_after = [collector.search_after] * len(queries)
-        carr, ncl, qarr, nq = compile_queries(queries, search_after)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self.index), search_after)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, max(k, 1)), np.int32), np.zeros((nq, max(k, 1)), np.float32),
                           np.zeros(nq, np.int32), np.zeros(nq, np.int64), np.zeros(nq, np.uint8),
@@ -987,7 +1092,7 @@ class GpuIndexSearcher:
         """prepare() for queries that may nest BooleanQuery and DisjunctionMaxQuery (nrtgpu_batch_prepare_tree)."""
         if search_after is None and collector.search_after is not None:
             search_after = [collector.search_after] * len(queries)
-        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, search_after, phrase_table=True)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(_resolve_all(queries, self.index), search_after, phrase_table=True)
         return PreparedBatch(self.index, carr, ncl, qarr, nq, collector.num_hits_to_collect, collector.total_hits_threshold, flags,
                              nodes=(narr, nn), phrases=(parr, n_ph, tarr, n_pt) if n_ph else None)
 
@@ -997,7 +1102,7 @@ class GpuIndexSearcher:
         nested query or a PhraseQuery runs on the window engine (phrases: nrtgpu_search_tree_phrases)."""
         if search_after is None and collector.search_after is not None:
             search_after = [collector.search_after] * len(queries)
-        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, search_after, phrase_table=True)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(_resolve_all(queries, self.index), search_after, phrase_table=True)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, max(k, 1)), np.int32), np.zeros((nq, max(k, 1)), np.float32),
                           np.zeros(nq, np.int32), np.zeros(nq, np.int64), np.zeros(nq, np.uint8),
@@ -1042,7 +1147,7 @@ class GpuIndexSearcher:
         if not isinstance(st, SortType) or st.field == "score":
             return self._search_sorted_fields(queries, collector, [st] if isinstance(st, SortType) else list(st), search_after, stream)
         after_sd = None if search_after is None else [None if a is None else ScoreDoc(a.doc, 0.0) for a in search_after]
-        carr, ncl, qarr, nq = compile_queries(queries, after_sd)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self.index), after_sd)
         k = collector.num_hits_to_collect
         out = SortedResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.int64), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                            np.zeros(nq, np.uint8))
@@ -1066,7 +1171,7 @@ class GpuIndexSearcher:
         order = self.index.sort_order(fields, stream)
         nf = len(fields)
         after_sd = None if search_after is None else [None if a is None else ScoreDoc(a.doc, 0.0) for a in search_after]
-        carr, ncl, qarr, nq = compile_queries(queries, after_sd)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self.index), after_sd)
         k = collector.num_hits_to_collect
         out = SortedResult(np.zeros((nq, k), np.int32), np.zeros((nq, k, nf), np.int64), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                            np.zeros(nq, np.uint8), np.zeros(nq, np.uint8), np.zeros(nq, np.uint8))
@@ -1095,13 +1200,13 @@ class GpuIndexSearcher:
         top_hits - start_hit], "counts", "total_hits" [nq, size][, "sort_values" [nq, size, top_hits - start_hit, n_fields]]}
         (top hits)}, per returned bucket. A FilterCollector's and a top-level TopHitsCollector's results are the dicts their
         docstrings describe (nrtgpu_search_bool_aggs_sorted_hits)."""
-        carr, ncl, qarr, nq = compile_queries(queries)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self.index))
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
         hits = (out.docs.ctypes.data, out.scores.ctypes.data, out.counts.ctypes.data, out.total_hits.ctypes.data)
         if _has_filter(additional):   # filter collectors, top-level or sorted top hits: the records of _FilteredRecords
-            fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * 1)(self.index.sort_order(fields, stream).value))
+            fr = _FilteredRecords(nq, _resolve_all(additional, self.index), lambda fields: (C.c_void_p * 1)(self.index.sort_order(fields, stream).value))
             check(self._lib.nrtgpu_search_bool_aggs_sorted_hits(self.index.handle, carr, ncl, qarr, nq, k, 0, *fr.sorted_args,
                                                                 C.c_void_p(stream), *hits))
             _keyword_keys(additional, fr.outs, self.index.keyword_term, self.index.keyword_names)
@@ -1121,11 +1226,11 @@ class GpuIndexSearcher:
         """search_with_collectors() for the queries of search_tree(): nested BooleanQuery and DisjunctionMaxQuery, PhraseQuery
         leaves, and flat batches of any width (nrtgpu_search_tree_aggs). The same collectors, the same (BatchResult, results)
         return; a batch with a nested query or a phrase, or a wide one, is collected by the window engine."""
-        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, phrase_table=True)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(_resolve_all(queries, self.index), phrase_table=True)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
-        fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * 1)(self.index.sort_order(fields, stream).value))
+        fr = _FilteredRecords(nq, _resolve_all(additional, self.index), lambda fields: (C.c_void_p * 1)(self.index.sort_order(fields, stream).value))
         check(self._lib.nrtgpu_search_tree_aggs(self.index.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k, 0,
                                                 *fr.sorted_args, C.c_void_p(stream), out.docs.ctypes.data, out.scores.ctypes.data,
                                                 out.counts.ctypes.data, out.total_hits.ctypes.data))
@@ -1134,7 +1239,7 @@ class GpuIndexSearcher:
 
     def score_docs(self, queries: Sequence[object], docs: np.ndarray, counts: Optional[np.ndarray] = None, stream: int = 0):
         """Second pass of QueryRescorer: query q on its own hit list -> (matches uint8 [nq, n], scores float32 [nq, n])."""
-        carr, ncl, qarr, nq = compile_queries(queries)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self.index))
         d = np.ascontiguousarray(docs, np.int32)
         cn = None if counts is None else np.ascontiguousarray(counts, np.int32)
         m, s = np.zeros(d.shape, np.uint8), np.zeros(d.shape, np.float32)
@@ -1145,7 +1250,7 @@ class GpuIndexSearcher:
     def rescore_query(self, queries: Sequence[object], docs: np.ndarray, scores: np.ndarray, counts: np.ndarray, window: int,
                       query_weight: float, rescore_weight: float, stream: int = 0):
         """QueryRescore (QueryRescore.java:39-57) end to end on the device: returns docs, scores, counts of the rescored lists."""
-        carr, ncl, qarr, nq = compile_queries(queries)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self.index))
         d = np.ascontiguousarray(docs, np.int32).copy()
         s = np.ascontiguousarray(scores, np.float32).copy()
         cn = np.ascontiguousarray(counts, np.int32)
@@ -1157,7 +1262,7 @@ class GpuIndexSearcher:
     def score_docs_tree(self, queries: Sequence[object], docs: np.ndarray, counts: Optional[np.ndarray] = None, stream: int = 0):
         """score_docs() for rescore queries that may nest BooleanQuery and DisjunctionMaxQuery or hold PhraseQuery leaves
         (nrtgpu_score_docs_tree): the queries search_tree takes."""
-        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, phrase_table=True)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(_resolve_all(queries, self.index), phrase_table=True)
         d = np.ascontiguousarray(docs, np.int32)
         cn = None if counts is None else np.ascontiguousarray(counts, np.int32)
         m, s = np.zeros(d.shape, np.uint8), np.zeros(d.shape, np.float32)
@@ -1170,7 +1275,7 @@ class GpuIndexSearcher:
                            query_weight: float, rescore_weight: float, stream: int = 0):
         """rescore_query() for rescore queries that may nest BooleanQuery and DisjunctionMaxQuery or hold PhraseQuery leaves
         (nrtgpu_rescore_query_tree): returns docs, scores, counts of the rescored lists."""
-        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, phrase_table=True)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(_resolve_all(queries, self.index), phrase_table=True)
         d = np.ascontiguousarray(docs, np.int32).copy()
         s = np.ascontiguousarray(scores, np.float32).copy()
         cn = np.ascontiguousarray(counts, np.int32)
@@ -1209,7 +1314,7 @@ class GpuIndexSearcher:
         if filter_queries is not None:
             if filter_docs is not None:
                 raise ValueError("pass filter_docs or filter_queries, not both")
-            carr, ncl, qarr, nf, filter_of = compile_filters(filter_queries, nq)
+            carr, ncl, qarr, nf, filter_of = compile_filters(_resolve_all(filter_queries, self.index), nq)
             check(self._lib.nrtgpu_search_knn_filtered(self.index.handle, q.ctypes.data, nq, k, None if b is None else b.ctypes.data,
                                                        carr, ncl, qarr, nf, filter_of.ctypes.data, C.c_void_p(stream),
                                                        docs.ctypes.data, scores.ctypes.data, counts.ctypes.data))
@@ -1246,12 +1351,17 @@ class GpuLeafSearcher:
         """the sort code of `term` in the reader-wide dictionary of keyword column `column` (nrtgpu_searcher_keyword_seek)"""
         return _seek(self._lib.nrtgpu_searcher_keyword_seek, self.handle, column, term)
 
+    def keyword_range(self, q) -> Tuple[int, int]:
+        """the code range [lo, hi] of a KeywordRangeQuery / KeywordPrefixQuery in the reader-wide dictionary
+        (nrtgpu_searcher_keyword_range)"""
+        return _keyword_range(self._lib.nrtgpu_searcher_keyword_range, self.handle, q.column, q)
+
     def search_batch(self, queries: Sequence[object], collector: RelevanceCollector, stream: int = 0,
                      search_after: Optional[Sequence[Optional[ScoreDoc]]] = None) -> BatchResult:
         """search_after: one reader-wide ScoreDoc (or None) per query; every leaf pages after it (TopDocs.merge of the pages)."""
         if search_after is None and collector.search_after is not None:
             search_after = [collector.search_after] * len(queries)
-        carr, ncl, qarr, nq = compile_queries(queries, search_after)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self), search_after)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
@@ -1273,7 +1383,7 @@ class GpuLeafSearcher:
         orders = (C.c_void_p * len(self.leaves))(*[l.sort_order(fields, stream).value for l in self.leaves])
         nf = len(fields)
         after_sd = None if search_after is None else [None if a is None else ScoreDoc(a.doc, 0.0) for a in search_after]
-        carr, ncl, qarr, nq = compile_queries(queries, after_sd)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self), after_sd)
         k = collector.num_hits_to_collect
         out = SortedResult(np.zeros((nq, k), np.int32), np.zeros((nq, k, nf), np.int64), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                            np.zeros(nq, np.uint8), np.zeros(nq, np.uint8), np.zeros(nq, np.uint8))
@@ -1303,7 +1413,7 @@ class GpuLeafSearcher:
         leaves' pages merged on the device (TopDocs.merge)."""
         if search_after is None and collector.search_after is not None:
             search_after = [collector.search_after] * len(queries)
-        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, search_after, phrase_table=True)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(_resolve_all(queries, self), search_after, phrase_table=True)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, max(k, 1)), np.int32), np.zeros((nq, max(k, 1)), np.float32),
                           np.zeros(nq, np.int32), np.zeros(nq, np.int64), np.zeros(nq, np.uint8),
@@ -1331,7 +1441,7 @@ class GpuLeafSearcher:
         if filter_queries is not None:
             if filter_docs is not None:
                 raise ValueError("pass filter_docs or filter_queries, not both")
-            carr, ncl, qarr, nf, filter_of = compile_filters(filter_queries, nq)
+            carr, ncl, qarr, nf, filter_of = compile_filters(_resolve_all(filter_queries, self), nq)
             check(self._lib.nrtgpu_searcher_search_knn_filtered(self.handle, q.ctypes.data, nq, k, None if b is None else b.ctypes.data,
                                                                 carr, ncl, qarr, nf, filter_of.ctypes.data, C.c_void_p(stream),
                                                                 docs.ctypes.data, scores.ctypes.data, counts.ctypes.data))
@@ -1348,12 +1458,12 @@ class GpuLeafSearcher:
         into reader-wide tables, buckets by value (the searcher's reader-wide dictionary of each terms column, built by the
         column's first aggregation), and the buckets, nested values and nested top hits are selected once from them; the
         leaves' pages are merged on the device (TopDocs.merge). Returns what the single-image method returns."""
-        carr, ncl, qarr, nq = compile_queries(queries)
+        carr, ncl, qarr, nq = compile_queries(_resolve_all(queries, self))
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
         if _has_filter(additional):
-            fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * len(self.leaves))(
+            fr = _FilteredRecords(nq, _resolve_all(additional, self), lambda fields: (C.c_void_p * len(self.leaves))(
                 *[l.sort_order(fields, stream).value for l in self.leaves]))
             check(self._lib.nrtgpu_searcher_search_bool_aggs_sorted_hits(self.handle, carr, ncl, qarr, nq, k, 0, *fr.sorted_args,
                                                                          C.c_void_p(stream), out.docs.ctypes.data,
@@ -1373,11 +1483,11 @@ class GpuLeafSearcher:
                                     stream: int = 0):
         """GpuIndexSearcher.search_tree_with_collectors over the leaves (nrtgpu_searcher_search_tree_aggs), with the reader-wide
         tables and merges of search_with_collectors. Returns what the single-image method returns."""
-        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(queries, phrase_table=True)
+        carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq = compile_tree(_resolve_all(queries, self), phrase_table=True)
         k = collector.num_hits_to_collect
         out = BatchResult(np.zeros((nq, k), np.int32), np.zeros((nq, k), np.float32), np.zeros(nq, np.int32), np.zeros(nq, np.int64),
                           np.zeros(nq, np.uint8))
-        fr = _FilteredRecords(nq, additional, lambda fields: (C.c_void_p * len(self.leaves))(
+        fr = _FilteredRecords(nq, _resolve_all(additional, self), lambda fields: (C.c_void_p * len(self.leaves))(
             *[l.sort_order(fields, stream).value for l in self.leaves]))
         check(self._lib.nrtgpu_searcher_search_tree_aggs(self.handle, carr, ncl, narr, nn, parr, n_ph, tarr, n_pt, qarr, nq, k, 0,
                                                          *fr.sorted_args, C.c_void_p(stream), out.docs.ctypes.data,
@@ -1400,11 +1510,11 @@ class GpuBatcher:
         self._lib = _native.gpu_lib()
         h = C.c_void_p()
         check(self._lib.nrtgpu_batcher_create(index.handle, max_batch, max_wait_us, C.byref(h)))
-        self.handle = h
+        self.handle, self.index = h, index
 
     def submit(self, query, collector: RelevanceCollector):
         """Blocking: returns (TopDocs, Diagnostics) of the one query."""
-        carr, ncl, qarr, _ = compile_queries([query])
+        carr, ncl, qarr, _ = compile_queries([_resolve_keywords(query, self.index)])
         k = collector.num_hits_to_collect
         docs, scores = np.zeros(k, np.int32), np.zeros(k, np.float32)
         cnt, tot, rel = C.c_int32(), C.c_int64(), C.c_uint8()
