@@ -113,7 +113,10 @@ typedef struct {
   int32_t occur;  /* NRTGPU_SHOULD.. */
   int32_t kind;   /* NRTGPU_TERM.. */
   int32_t id;     /* term id or column id */
-  float boost;    /* product of enclosing BoostQuery boosts (weight = boost * idf) */
+  float boost;    /* product of enclosing BoostQuery boosts (weight = boost * idf). Every entry point that compiles
+                     clauses refuses, with NRTGPU_ERR_INVALID and no output written, a boost < 0 ("Boost must be a
+                     positive number", QueryNodeMapper.java:127) and a NaN or infinite one ("Boost must be a finite
+                     number", as Lucene's BoostQuery refuses it). 0 is a weight of 0. */
   int64_t lo, hi; /* inclusive range bounds */
 } nrtgpu_clause;
 

@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import ctypes as C
 import enum
+import math
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence, Tuple
 
@@ -542,11 +543,7 @@ def _f32(x: float) -> np.float32:
 def _flatten(q, boost: np.float32, out: list, occur: Occur) -> None:
     """One clause of the flat BooleanQuery; BoostQuery boosts multiply outermost-first in float
     (BoostQuery.createWeight passes boost * this.boost down)."""
-    while isinstance(q, BoostQuery):
-        if q.boost < 0:
-            raise ValueError("Boost must be a positive number")  # QueryNodeMapper.java:127
-        boost = _f32(boost * _f32(q.boost))
-        q = q.query
+    q, boost = _unboost(q, boost)
     if isinstance(q, TermQuery):
         out.append((int(occur), 0, int(q.term), float(boost), 0, 0))
     elif isinstance(q, RangeQuery):
@@ -566,12 +563,7 @@ def compile_queries(queries: Sequence[object], search_after: Optional[Sequence[O
     (Lucene rewrites a one-clause BooleanQuery to its clause; scores are identical)."""
     flat, qs = [], []
     for i, q in enumerate(queries):
-        boost = _f32(1.0)
-        while isinstance(q, BoostQuery):
-            if q.boost < 0:
-                raise ValueError("Boost must be a positive number")
-            boost = _f32(boost * _f32(q.boost))
-            q = q.query
+        q, boost = _unboost(q, _f32(1.0))
         begin = len(flat)
         msm = 0
         if isinstance(q, BooleanQuery):
@@ -595,10 +587,13 @@ def compile_queries(queries: Sequence[object], search_after: Optional[Sequence[O
 
 
 def _unboost(q, boost: np.float32):
-    """(the query under any BoostQuerys, the boost folded outermost first in float)"""
+    """(the query under any BoostQuerys, the boost folded outermost first in float). A boost < 0 is refused as the
+    reference refuses it (QueryNodeMapper.java:127), a NaN or infinite one as Lucene's BoostQuery does."""
     while isinstance(q, BoostQuery):
         if q.boost < 0:
             raise ValueError("Boost must be a positive number")
+        if not math.isfinite(q.boost):
+            raise ValueError(f"Boost must be a finite number, got {q.boost}")
         boost = _f32(boost * _f32(q.boost))
         q = q.query
     return q, boost
