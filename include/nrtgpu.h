@@ -186,23 +186,39 @@ int nrtgpu_search_bool_ex(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_
  *   BOOL node:   the rule of a flat BooleanQuery, a child node counting as a clause that scores the child's float;
  *   DISMAX node: matches if any disjunct does, scores (float)((double)max + others * (double)tie_breaker), where others is
  *                the double sum of the other matching disjuncts (DisjunctionMaxScorer, Lucene 10).
- * Subtrees under FILTER and MUST_NOT only match. Boosts are folded into the leaves (outermost first, in float): a node
- * clause has boost 1. Every tree batch runs on the window engine (as a batch with more than 4 term clauses does).
+ *   CONSTANT node (ConstantScoreQuery; ExistsQuery is one over the term of its field in the _field_names field): matches
+ *                when its clause does and scores its boost; nothing below it scores (a phrase stops at its first match);
+ *   MIN_SCORE node (MinScoreQuery, the reference's MinThresholdQuery): its clause is scored with boost 1 below the node
+ *                (boosts below it still fold into its leaves) and always scores, even under FILTER, MUST_NOT or CONSTANT;
+ *                with s its float score the node matches iff s >= min_score in float (a NaN threshold matches nothing)
+ *                and scores __fmul_rn(s, boost). A threshold of 0 is an ordinary threshold here: the reference returns
+ *                the inner query unwrapped at 0, boosts folded into its leaves, which the caller compiles as that query.
+ *                Both kinds hold exactly one clause, whose occur is MUST (any leaf kind or a node clause). Their boost
+ *                is the float product, outermost first, of the BoostQuerys above the node.
+ * Subtrees under FILTER, MUST_NOT and CONSTANT only match, unless a MIN_SCORE node below scores its own. Boosts are
+ * folded into the leaves (outermost first, in float), stopping at a CONSTANT or MIN_SCORE node, which takes them as its
+ * boost: a node clause has boost 1. A CONSTANT or MIN_SCORE query at the root is a root with one MUST node clause.
+ * Every tree batch runs on the window engine (as a batch with more than 4 term clauses does).
  *   NRTGPU_ERR_INVALID:     a node id out of range, a node referenced twice or from a cycle, a bad node kind or clause
  *                           range, a DISMAX clause whose occur is not SHOULD, tie_breaker outside [0, 1], a node clause
- *                           whose boost is not 1, msm < 0, and every check of nrtgpu_search_bool_ex.
+ *                           whose boost is not 1, msm < 0, a CONSTANT or MIN_SCORE node without exactly one clause or
+ *                           whose clause is not MUST, a CONSTANT or MIN_SCORE boost < 0, NaN or infinite, a min_score < 0
+ *                           ("MinScoreQuery.min_score must be a non-negative number"), and every check of
+ *                           nrtgpu_search_bool_ex.
  *   NRTGPU_ERR_UNSUPPORTED: more than 8 term leaves, 8 nodes or 32 clauses in one tree, more than 4 levels of queries
- *                           (the root counts as one), top_k > 1024.
+ *                           (the root counts as one), top_k > 1024. CONSTANT and MIN_SCORE nodes count as nodes and
+ *                           levels, their clause as a clause.
  * With n_nodes == 0 nrtgpu_search_tree is nrtgpu_search_bool_ex (same compile, same engine); the other entry points
- * reject NRTGPU_NODE clauses as a bad clause kind. */
+ * reject NRTGPU_NODE clauses as a bad clause kind. Node kind 2 is not a kind. */
 enum { NRTGPU_NODE = 3 };
-enum { NRTGPU_NODE_BOOL = 0, NRTGPU_NODE_DISMAX = 1 };
+enum { NRTGPU_NODE_BOOL = 0, NRTGPU_NODE_DISMAX = 1, NRTGPU_NODE_CONSTANT = 3, NRTGPU_NODE_MIN_SCORE = 4 };
 typedef struct {
-  int32_t kind;                      /* NRTGPU_NODE_BOOL / NRTGPU_NODE_DISMAX */
+  int32_t kind;                      /* NRTGPU_NODE_BOOL / _DISMAX / _CONSTANT / _MIN_SCORE */
   int32_t clause_begin, clause_end;  /* its clauses in the same clauses[] array */
   int32_t min_should_match;          /* BOOL */
   float tie_breaker;                 /* DISMAX: tieBreakerMultiplier, in [0, 1] */
-  int32_t reserved;
+  float boost;                       /* CONSTANT / MIN_SCORE (BOOL and DISMAX do not read it) */
+  float min_score;                   /* MIN_SCORE: the threshold, >= 0 or NaN */
 } nrtgpu_node;
 int nrtgpu_search_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,
                        int32_t n_nodes, const nrtgpu_query* queries, int32_t nq, int32_t top_k,

@@ -50,8 +50,10 @@ public final class NrtGpu {
       ByteBuffer outHitTimeout, ByteBuffer outTerminatedEarly);
 
   /**
-   * Query trees (nested BooleanQuery / DisjunctionMaxQuery): nodes = nrtgpu_node[nNodes], referenced by clauses of kind 3
-   * (NODE); otherwise as searchBoolEx, which it is with nNodes == 0.
+   * Query trees (nested BooleanQuery / DisjunctionMaxQuery / ConstantScoreQuery / MinScoreQuery): nodes =
+   * nrtgpu_node[nNodes] (28 bytes each: int kind (0 BOOL, 1 DISMAX, 3 CONSTANT, 4 MIN_SCORE), clauseBegin, clauseEnd,
+   * minShouldMatch, float tieBreaker, boost, minScore), referenced by clauses of kind 3 (NODE); otherwise as
+   * searchBoolEx, which it is with nNodes == 0.
    */
   public static native int searchTree(
       long index, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer queries, int nq,

@@ -95,7 +95,8 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchBoolEx(
                                          (int64_t*)ADDR(env, outTotalHits), (uint8_t*)ADDR(env, outRelation),
                                          (uint8_t*)ADDR(env, outHitTimeout), (uint8_t*)ADDR(env, outTerminatedEarly)));
 }
-/* nodes: a direct ByteBuffer laid out as nrtgpu_node[] (null with nNodes 0: the search of searchBoolEx) */
+/* nodes: a direct ByteBuffer laid out as nrtgpu_node[] (28 bytes each: kind, clause_begin, clause_end, min_should_match,
+ * tie_breaker, boost, min_score; null with nNodes 0: the search of searchBoolEx) */
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTree(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject queries, jint nq,
     jint topK, jint totalHitsThreshold, jint flags, jobject limits, jobject outDocs, jobject outScores, jobject outCounts,

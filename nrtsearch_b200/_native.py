@@ -125,9 +125,10 @@ class Query(C.Structure):
 
 
 class Node(C.Structure):
-    """nrtgpu_node: a nested BooleanQuery (kind 0) or DisjunctionMaxQuery (kind 1) of a query tree."""
+    """nrtgpu_node: a nested BooleanQuery (kind 0), DisjunctionMaxQuery (kind 1), ConstantScoreQuery (kind 3) or
+    MinScoreQuery (kind 4) of a query tree; boost is that of kinds 3 and 4, min_score that of kind 4."""
     _fields_ = [("kind", C.c_int32), ("clause_begin", C.c_int32), ("clause_end", C.c_int32), ("min_should_match", C.c_int32),
-                ("tie_breaker", C.c_float), ("reserved", C.c_int32)]
+                ("tie_breaker", C.c_float), ("boost", C.c_float), ("min_score", C.c_float)]
 
 
 class Phrase(C.Structure):

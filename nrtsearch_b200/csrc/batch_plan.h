@@ -61,14 +61,22 @@ constexpr int kMaxTreeClauses = 32;   // clauses of one tree, nodes and leaves
 constexpr int kMaxTreeNodes = 9;      // the root and up to 8 nested nodes
 constexpr int kMaxTreeDepth = 4;      // levels of queries, the root included
 
+// CONSTANT and MIN_SCORE nodes (one MUST clause: n_req 1, need_should 0) read no msm or tie breaker, so their boost and
+// threshold share those words and the record keeps its size.
 struct DevNode {
-  int32_t kind;           // NRTGPU_NODE_BOOL / NRTGPU_NODE_DISMAX
+  int32_t kind;           // NRTGPU_NODE_BOOL / _DISMAX / _CONSTANT / _MIN_SCORE
   int32_t clause_begin;   // relative to the query's clause_begin
   int32_t n_clauses;
   int32_t n_req;          // BOOL: MUST + FILTER clauses
   int32_t need_should;    // BOOL: minimum matching SHOULD clauses (DISMAX: 1)
-  int32_t msm;            // BOOL: minimumNumberShouldMatch as given
-  float tie_breaker;      // DISMAX
+  union {
+    int32_t msm;          // BOOL: minimumNumberShouldMatch as given
+    float min_score;      // MIN_SCORE
+  };
+  union {
+    float tie_breaker;    // DISMAX
+    float boost;          // CONSTANT / MIN_SCORE
+  };
   int32_t empty;          // 1: can match nothing
 };
 static_assert(sizeof(DevNode) == 32, "DevNode layout");

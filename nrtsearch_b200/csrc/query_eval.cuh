@@ -168,7 +168,10 @@ __device__ __forceinline__ bool eval_clauses(const DevIndexView& ix, const DevQu
 //   BOOL:   eval_clauses's rule, a child node counting as a clause that is present when it matched and scores its float;
 //   DISMAX: matches if any disjunct does; DisjunctionMaxScorer's float max and double sum of the others, streamed in clause
 //           order as Lucene 10 streams its disjuncts (a new max moves the old one into the sum), scored
-//           (float)((double)max + others * (double)tie_breaker).
+//           (float)((double)max + others * (double)tie_breaker);
+//   CONSTANT: its one MUST clause matches; scores the node's boost (the clause was compiled non-scoring);
+//   MIN_SCORE: its one MUST clause matches with a float s >= min_score (MinThresholdQuery / MinScoreWrapper); scores
+//           s * boost in float.
 // term(c, &s) as for eval_clauses, for term and phrase leaves alike. Liveness is the caller's.
 template <class TermScore>
 __device__ __forceinline__ bool eval_node(const DevIndexView& ix, const DevNode& nd, const DevClause* cl, int32_t doc,
@@ -212,6 +215,12 @@ __device__ __forceinline__ bool eval_node(const DevIndexView& ix, const DevNode&
   if (n_should < nd.need_should) return false;
   float score;
   if (nd.kind == NRTGPU_NODE_DISMAX) score = (float)((double)max_s + should_sum * (double)nd.tie_breaker);
+  else if (nd.kind == NRTGPU_NODE_CONSTANT) score = nd.boost;
+  else if (nd.kind == NRTGPU_NODE_MIN_SCORE) {
+    const float s = (float)must_sum;   // its one MUST clause's float
+    if (!(s >= nd.min_score)) return false;   // hasPassedMinScore: s > min || s == min (NaN: never)
+    score = __fmul_rn(s, nd.boost);
+  }
   else if (nd.n_req == 0) score = (float)should_sum;
   else {
     const float req = (float)must_sum;

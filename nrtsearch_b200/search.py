@@ -104,6 +104,25 @@ class DisjunctionMaxQuery:
     tie_breaker: float = 0.0
 
 
+@dataclass(frozen=True)
+class ConstantScoreQuery:
+    """ConstantScoreQuery(filter) (QueryNodeMapper.java:194, :635-640): a doc matches when `filter` does and scores the
+    product of the BoostQuerys around this query (1 without them); nothing inside it scores. ExistsQuery(field) is one
+    over the _field_names term of the field (INTEGRATION.md). A node of a query tree (GpuIndexSearcher.search_tree)."""
+    filter: object
+
+
+@dataclass(frozen=True)
+class MinScoreQuery:
+    """MinScoreQuery(query, min_score), built by the reference as MinThresholdQuery (QueryNodeMapper.java:199, :642-656):
+    a doc matches when `query` does with a float score s >= min_score, and scores s times the product of the BoostQuerys
+    around this query; `query` is scored with boost 1 (its own BoostQuerys still apply), even where the tree only
+    filters. min_score < 0 is refused; 0 returns `query` itself with the outer boosts folded into it, as the reference
+    does; NaN matches nothing. A node of a query tree (GpuIndexSearcher.search_tree)."""
+    query: object
+    min_score: float
+
+
 @dataclass
 class PhraseQuery:
     """PhraseQuery(slop, terms, positions): what match_phrase maps to (QueryNodeMapper.java:285-291, :397-427). All terms on
@@ -452,7 +471,7 @@ def _keyword_range(fn, handle, column: int, q) -> Tuple[int, int]:
 def _resolve_keywords(q, searcher):
     """q with every KeywordRangeQuery / KeywordPrefixQuery turned into _KeywordCodes and every keyword ValueSetFilter into
     a _KeywordCodeSet by searcher.keyword_range / keyword_seek (its own dictionary), through BooleanQuery,
-    DisjunctionMaxQuery, BoostQuery and FilterCollector; q itself when it holds none"""
+    DisjunctionMaxQuery, ConstantScoreQuery, MinScoreQuery, BoostQuery and FilterCollector; q itself when it holds none"""
     if isinstance(q, (KeywordRangeQuery, KeywordPrefixQuery)):
         return _KeywordCodes(q.column, *searcher.keyword_range(q))
     if isinstance(q, BoostQuery):
@@ -466,6 +485,12 @@ def _resolve_keywords(q, searcher):
     if isinstance(q, DisjunctionMaxQuery):
         subs = [_resolve_keywords(d, searcher) for d in q.disjuncts]
         return q if all(x is d for x, d in zip(subs, q.disjuncts)) else DisjunctionMaxQuery(subs, q.tie_breaker)
+    if isinstance(q, ConstantScoreQuery):
+        sub = _resolve_keywords(q.filter, searcher)
+        return q if sub is q.filter else ConstantScoreQuery(sub)
+    if isinstance(q, MinScoreQuery):
+        sub = _resolve_keywords(q.query, searcher)
+        return q if sub is q.query else MinScoreQuery(sub, q.min_score)
     if isinstance(q, ValueSetFilter) and q.field_type == "keyword":
         return _KeywordCodeSet(q.column, tuple(searcher.keyword_seek(q.column, _utf8_bytes(v)) for v in q.values))
     if isinstance(q, FilterCollector):
@@ -602,10 +627,12 @@ def _unboost(q, boost: np.float32):
 def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Optional[ScoreDoc]]] = None,
                  phrase_table: bool = False):
     """Query trees -> (Clause[], n_clauses, Node[], n_nodes, Query[], nq) for nrtgpu_search_tree. The root of a query is a
-    BooleanQuery (a bare leaf or DisjunctionMaxQuery becomes its single MUST clause); every BooleanQuery or
-    DisjunctionMaxQuery below it is a node, numbered in pre-order over the batch, whose clauses are one range of the clause
-    array. BoostQuery boosts are folded through the nodes into the leaves, outermost first in float, so node clauses carry
-    boost 1 (BoostQuery.createWeight passes boost * this.boost down).
+    BooleanQuery (a bare leaf, DisjunctionMaxQuery, ConstantScoreQuery or MinScoreQuery becomes its single MUST clause);
+    every BooleanQuery, DisjunctionMaxQuery, ConstantScoreQuery or MinScoreQuery below it is a node, numbered in pre-order
+    over the batch, whose clauses are one range of the clause array. BoostQuery boosts are folded through the nodes into
+    the leaves, outermost first in float, so node clauses carry boost 1 (BoostQuery.createWeight passes boost * this.boost
+    down). A ConstantScoreQuery or MinScoreQuery node takes the boost folded down to it as its own and the fold starts again
+    at 1 below it; MinScoreQuery(q, 0) is compiled as q, and a min_score < 0 raises ValueError.
     phrase_table: return (Clause[], n_clauses, Node[], n_nodes, Phrase[], n_phrases, PhraseTerm[], n_phrase_terms, Query[],
     nq) for nrtgpu_search_tree_phrases instead: a PhraseQuery leaf is a clause of kind 4 whose id indexes the phrase table.
     Without it a PhraseQuery is refused."""
@@ -623,36 +650,55 @@ def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Opti
         else:
             _flatten(sub, sb, flat, occ)
 
-    def parts(q):
+    def unwrap(q, b):
+        """_unboost, through MinScoreQuerys of threshold 0 (QueryNodeMapper returns their query unwrapped)"""
+        while True:
+            q, b = _unboost(q, b)
+            if not isinstance(q, MinScoreQuery):
+                return q, b
+            if q.min_score < 0:
+                raise ValueError("MinScoreQuery.min_score must be a non-negative number")
+            if q.min_score != 0:
+                return q, b
+            q = q.query
+
+    one = _f32(1.0)
+
+    def parts(q, b):
+        """(kind, clauses, msm, tie, the boost its clauses fold from, node boost, min_score) of a node reached with boost b"""
         if isinstance(q, BooleanQuery):
-            return 0, [(c.query, c.occur) for c in q.clauses], q.minimum_number_should_match, 0.0
-        return 1, [(d, Occur.SHOULD) for d in q.disjuncts], 0, float(q.tie_breaker)
+            return 0, [(c.query, c.occur) for c in q.clauses], q.minimum_number_should_match, 0.0, b, 0.0, 0.0
+        if isinstance(q, DisjunctionMaxQuery):
+            return 1, [(d, Occur.SHOULD) for d in q.disjuncts], 0, float(q.tie_breaker), b, 0.0, 0.0
+        if isinstance(q, ConstantScoreQuery):
+            return 3, [(q.filter, Occur.MUST)], 0, 0.0, one, float(b), 0.0
+        return 4, [(q.query, Occur.MUST)], 0, 0.0, one, float(b), float(q.min_score)
 
     for i, q in enumerate(queries):
-        q, boost = _unboost(q, _f32(1.0))
+        q, boost = unwrap(q, one)
         if isinstance(q, BooleanQuery):
-            root = (0, [(c.query, c.occur) for c in q.clauses], q.minimum_number_should_match, 0.0)
+            root = (0, [(c.query, c.occur) for c in q.clauses], q.minimum_number_should_match, 0.0, boost, 0.0, 0.0)
         else:
-            root = (0, [(q, Occur.MUST)], 0, 0.0)
-        order = []   # pre-order: [kind, [(leaf, boost, occur) | (node position, None, occur)], msm, tie]
+            root = (0, [(q, Occur.MUST)], 0, 0.0, boost, 0.0, 0.0)
+        order = []   # pre-order: [kind, [(leaf, boost, occur) | (node position, None, occur)], msm, tie, node boost, min_score]
 
-        def visit(kind, cls, msm, tie, b):
+        def visit(kind, cls, msm, tie, b, nb, ms):
             pos = len(order)
             order.append(None)
             children = []
             for sub, occ in cls:
-                s, sb = _unboost(sub, b)
-                if isinstance(s, (BooleanQuery, DisjunctionMaxQuery)):
-                    children.append((visit(*parts(s), sb), None, occ))
+                s, sb = unwrap(sub, b)
+                if isinstance(s, (BooleanQuery, DisjunctionMaxQuery, ConstantScoreQuery, MinScoreQuery)):
+                    children.append((visit(*parts(s, sb)), None, occ))
                 else:
                     children.append((s, sb, occ))
-            order[pos] = (kind, children, msm, tie)
+            order[pos] = (kind, children, msm, tie, nb, ms)
             return pos
 
-        visit(*root, boost)
+        visit(*root)
         base = len(nodes) - 1   # node id of pre-order position p > 0: base + p
         begin_end = []
-        for kind, children, msm, tie in order:
+        for kind, children, msm, tie, nb, ms in order:
             begin = len(flat)
             for sub, sb, occ in children:
                 if sb is None:
@@ -661,8 +707,8 @@ def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Opti
                     leaf(sub, sb, occ)
             begin_end.append((begin, len(flat)))
         for p in range(1, len(order)):
-            kind, _, msm, tie = order[p]
-            nodes.append((kind, begin_end[p][0], begin_end[p][1], msm, tie, 0))
+            kind, _, msm, tie, nb, ms = order[p]
+            nodes.append((kind, begin_end[p][0], begin_end[p][1], msm, tie, nb, ms))
         after = search_after[i] if search_after is not None else None
         qs.append((begin_end[0][0], begin_end[0][1], root[2], 1 if after is not None else 0,
                    after.doc if after is not None else 0, after.score if after is not None else 0.0))
