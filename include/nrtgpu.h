@@ -321,8 +321,36 @@ int nrtgpu_index_keyword_range(const nrtgpu_index* ix, int32_t column, const uin
  *                           groups), every limit of nrtgpu_search_tree.
  * With n_phrases == 0 these are nrtgpu_search_tree / nrtgpu_batch_prepare_tree. A batch holding a phrase is a tree batch
  * even without nodes (a bare PhraseQuery is a root with one MUST phrase clause). Every other entry point rejects
- * NRTGPU_PHRASE clauses as a bad clause kind. */
-enum { NRTGPU_PHRASE = 4 };
+ * NRTGPU_PHRASE clauses as a bad clause kind.
+ *
+ * Multi-phrase leaves (MultiPhraseQuery: match_phrase_prefix, multi_match PHRASE_PREFIX, match_phrase over stacked
+ * synonyms). A clause of kind NRTGPU_MULTI_PHRASE is a leaf whose id indexes phrases[] as for NRTGPU_PHRASE; its
+ * phrase_terms share positions (given in non-decreasing order), and terms that share a position are ALTERNATIVES: a doc
+ * matches a position when any of them occurs there. The positions of a position are the merged positions of its terms,
+ * repeats kept (UnionPostingsEnum). Prefix expansion is the caller's: it passes the expanded terms' ids. Semantics:
+ *   weight:  boost * (float) of the double sum of the float idf of every term with df > 0 over all positions, a term
+ *            repeated at several positions counted each time (MultiPhraseQuery.createWeight), summed position after
+ *            position, ascending term id within one; no such term: the leaf matches nothing. Score as for NRTGPU_PHRASE; slop 0
+ *            is ExactPhraseMatcher over the merged positions, slop > 0 SloppyPhraseMatcher;
+ *   one position (MultiPhraseQuery.rewrite): a BooleanQuery of SHOULD TermQuerys over its alternatives: matches a doc
+ *            holding any of them and scores (float) of the double sum of each present alternative's BM25 at weight
+ *            boost * idf of that term, summed in ascending term id order (one alternative: that TermQuery);
+ *   no positions: matches nothing. Under FILTER, MUST_NOT and inside a CONSTANT node it only has to match.
+ * Limits: every position takes ONE term slot, however many alternatives it has (<= 8 slots per tree, term leaves,
+ * phrase terms and multi-phrase positions together); at most 128 alternatives per position; per call the distinct
+ * alternative sets of a position (deduplicated over the batch's queries; a one-position leaf's set is keyed by its
+ * boost too) gather at most 2^25 postings (52 bytes of device scratch each, 1.75 GB) and merge at most 2^27
+ * positions (4 bytes each, 512 MB). The unions are built on the device by each call (and once by a prepared batch). The
+ * scratch belongs to the batch that runs the call (an index's reused search workspace for the one-shot calls) and, like
+ * that batch's other buffers, only grows: after a call near the caps up to 2.25 GB stay allocated until the index (or the
+ * prepared batch) is freed. NRTGPU_UNION_POSTINGS, read when the context is created, lowers the postings cap (> 0).
+ *   NRTGPU_ERR_INVALID:     as for NRTGPU_PHRASE (an image without positions only with two or more positions);
+ *   NRTGPU_ERR_UNSUPPORTED: more than 8 term slots, more than 128 terms at one position, a sloppy multi-phrase in
+ *                           which one term appears at two positions, the union postings or positions cap.
+ * A refused call writes no output. Accepted by nrtgpu_search_tree_phrases, nrtgpu_batch_prepare_tree_phrases,
+ * nrtgpu_search_tree_aggs, nrtgpu_searcher_search_tree_phrases and nrtgpu_searcher_search_tree_aggs; every other entry
+ * point, tree rescoring (nrtgpu_score_docs_tree, nrtgpu_rescore_query_tree) included, rejects it as a bad clause kind. */
+enum { NRTGPU_PHRASE = 4, NRTGPU_MULTI_PHRASE = 6 };
 typedef struct { int32_t term_begin, term_end; int32_t slop; int32_t reserved; } nrtgpu_phrase;
 typedef struct { int32_t term; int32_t position; } nrtgpu_phrase_term;
 int nrtgpu_search_tree_phrases(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_t n_clauses, const nrtgpu_node* nodes,

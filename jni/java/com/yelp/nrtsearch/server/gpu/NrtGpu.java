@@ -110,9 +110,10 @@ public final class NrtGpu {
                                         int upperLen, int flags, ByteBuffer out);
 
   /**
-   * Query trees with PhraseQuery leaves: phrases = nrtgpu_phrase[nPhrases] referenced by clauses of kind 4 (PHRASE),
-   * phraseTerms = nrtgpu_phrase_term[nPhraseTerms] (term id, PhraseQuery position); otherwise as searchTree, which it is
-   * with nPhrases == 0.
+   * Query trees with PhraseQuery leaves: phrases = nrtgpu_phrase[nPhrases] referenced by clauses of kind 4 (PHRASE)
+   * or kind 6 (MULTI_PHRASE: MultiPhraseQuery, match_phrase_prefix with its prefix expanded by the caller; terms that
+   * share a position are alternatives), phraseTerms = nrtgpu_phrase_term[nPhraseTerms] (term id, position); otherwise
+   * as searchTree, which it is with nPhrases == 0.
    */
   public static native int searchTreePhrases(
       long index, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer phrases, int nPhrases,

@@ -193,7 +193,8 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_keywordRange(JN
   return s ? fail(env, nrtgpu_searcher_keyword_range((nrtgpu_searcher*)(intptr_t)s, column, lo, lowerLen, hi, upperLen, flags, o, o + 1))
            : fail(env, nrtgpu_index_keyword_range((const nrtgpu_index*)(intptr_t)ix, column, lo, lowerLen, hi, upperLen, flags, o, o + 1));
 }
-/* phrases / phraseTerms: direct ByteBuffers laid out as nrtgpu_phrase[] / nrtgpu_phrase_term[] (nPhrases 0: searchTree) */
+/* phrases / phraseTerms: direct ByteBuffers laid out as nrtgpu_phrase[] / nrtgpu_phrase_term[] (nPhrases 0: searchTree),
+ * for clauses of kind NRTGPU_PHRASE and NRTGPU_MULTI_PHRASE */
 JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_searchTreePhrases(
     JNIEnv* env, jclass c, jlong ix, jobject clauses, jint nClauses, jobject nodes, jint nNodes, jobject phrases, jint nPhrases,
     jobject phraseTerms, jint nPhraseTerms, jobject queries, jint nq, jint topK, jint totalHitsThreshold, jint flags,

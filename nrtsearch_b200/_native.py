@@ -132,12 +132,13 @@ class Node(C.Structure):
 
 
 class Phrase(C.Structure):
-    """nrtgpu_phrase: a PhraseQuery leaf of a query tree, its terms phrase_terms[term_begin:term_end]."""
+    """nrtgpu_phrase: a PhraseQuery leaf (clause kind 4) or a MultiPhraseQuery leaf (clause kind 6, NRTGPU_MULTI_PHRASE:
+    terms that share a position are alternatives) of a query tree, its terms phrase_terms[term_begin:term_end]."""
     _fields_ = [("term_begin", C.c_int32), ("term_end", C.c_int32), ("slop", C.c_int32), ("reserved", C.c_int32)]
 
 
 class PhraseTerm(C.Structure):
-    """nrtgpu_phrase_term: a term of a phrase and its PhraseQuery position."""
+    """nrtgpu_phrase_term: a term of a phrase and its PhraseQuery / MultiPhraseQuery position."""
     _fields_ = [("term", C.c_int32), ("position", C.c_int32)]
 
 

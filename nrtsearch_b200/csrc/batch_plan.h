@@ -99,6 +99,18 @@ struct DevPhrase {
 };
 static_assert(sizeof(DevPhrase) == 64, "DevPhrase layout");
 
+// Multi-phrase leaves of tree batches (NRTGPU_MULTI_PHRASE, nrtgpu_search_tree_phrases). A position that holds several
+// alternative terms takes ONE term slot whose list is a union built on the device for the call (union_kernel.cuh): a
+// term clause (kind NRTGPU_TERM) with plane kUnionList, post_base / n_post its range of the call's union entries (the
+// host writes the union's index into post_base, union_patch_kernel the range). A one-position multi-phrase is such a
+// slot on its own, scored from the union's per-entry score (SHOULD TermQuerys over the alternatives); a longer one is a
+// DevPhrase whose union positions read the union's merged positions. Only the kUnion instantiations of the window
+// engine read plane there; every other engine refuses the kind.
+constexpr int32_t kUnionList = -2;
+constexpr int kMaxUnionAlternatives = 128;        // alternatives of one multi-phrase position
+constexpr int64_t kMaxUnionPostings = 1ll << 25;  // postings the distinct unions of one call gather (52 B each of scratch)
+constexpr int64_t kMaxUnionPositions = 1ll << 27; // positions the distinct phrase-position unions of one call merge (4 B each)
+
 struct DevQuery {
   int32_t clause_begin, n_clauses;
   int32_t n_term;          // number of term clauses (= slots used)

@@ -23,10 +23,14 @@
 // cover (batch_plan.inc compile_tree), and a doc is evaluated node by node (eval_node) instead of by one clause list.
 // Additional collectors (nrtgpu_search_tree_aggs, bool_window_kernel<kTree, true>): every matching doc is also handed to
 // agg_collect with its score, where pass 2 counts it, as the probe kernel's generic instantiation does.
+// Multi-phrase unions (tree batches whose term slots include call unions, bool_window_union_kernel): a union slot's list is
+// the call's union entries (union_kernel.cuh) instead of the image's postings, a presence byte in pass 1; the phrase
+// matcher reads its merged positions and a scoring one-position slot its entry's score (query_eval.cuh SmemUnions).
 #pragma once
 #include <type_traits>
 #include "query_eval.cuh"
 #include "collect_kernel.cuh"
+#include "union_kernel.cuh"
 
 namespace nrtgpu {
 
@@ -82,6 +86,23 @@ struct BoolTreeSmem : BoolSmemT<true> {
   int n_nodes;
   int n_phrases;
 };
+// tree batches with multi-phrase unions: the call's union entries
+struct BoolLaunchU : BoolLaunch {
+  UnionView u;
+};
+struct BoolTreeSmemU : BoolTreeSmem {
+  UnionView u;
+};
+template <> struct SmemUnions<BoolTreeSmemU> : std::true_type {};
+
+// the list of a term slot: the image's postings, or (kUnion) the call's union entries
+template <bool kUnion, class Launch>
+__device__ __forceinline__ const int32_t* list_docs(const Launch& L, const DevClause& c) {
+  if constexpr (kUnion) {
+    if (c.plane == kUnionList) return L.u.docs + c.post_base;
+  }
+  return L.ix.post_docs + c.post_base;
+}
 
 // the clauses of sm.q on one candidate doc; slot holds the doc's tf byte of every term slot
 __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolSmem& sm, int32_t doc,
@@ -109,19 +130,31 @@ __device__ __forceinline__ uint32_t phrase_posting(const DevIndexView& ix, const
   return lo;
 }
 
+// ... of a slot that may be a union
+__device__ __forceinline__ uint32_t phrase_posting(const DevIndexView& ix, const BoolTreeSmemU& sm, const DevClause& t, int32_t doc) {
+  const int w = (doc & (kWideSliceDocs - 1)) / kWindowDocs;
+  const int32_t* docs = (t.plane == kUnionList ? sm.u.docs : ix.post_docs) + t.post_base;
+  uint32_t lo = sm.bounds[t.slot][w], hi = sm.bounds[t.slot][w + 1];
+  while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (__ldg(docs + m) < doc) lo = m + 1; else hi = m; }
+  return lo;
+}
+
 // the query tree of sm on one candidate doc
 __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolTreeSmem& sm, int32_t doc, uint64_t slot,
+                                             float* out_score) {
+  return eval_tree(ix, sm, doc, slot, out_score);
+}
+__device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolTreeSmemU& sm, int32_t doc, uint64_t slot,
                                              float* out_score) {
   return eval_tree(ix, sm, doc, slot, out_score);
 }
 
 // kTree: a tree batch (sm holds the query's nodes, evaluate_doc walks them); otherwise flat BooleanQuerys.
 // kAggs: every matching doc also goes to the collectors of L.aggs (the other instantiations never read it); kMulti: they
-// count a SORTED_SET keyword column (agg_collect<true>)
-template <bool kTree, bool kAggs, bool kMulti = false>
-__global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_constant__ BoolLaunch L) {
-  using Smem = typename std::conditional<kTree, BoolTreeSmem, BoolSmem>::type;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
+// count a SORTED_SET keyword column (agg_collect<true>); kUnion (tree batches): term slots may be call unions (L.u)
+template <bool kTree, bool kAggs, bool kMulti, bool kUnion, class Launch>
+__device__ __forceinline__ void bool_window_body(const Launch& L, unsigned char* smem_raw) {
+  using Smem = typename std::conditional<kUnion, BoolTreeSmemU, typename std::conditional<kTree, BoolTreeSmem, BoolSmem>::type>::type;
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
   const int tid = threadIdx.x;
   const int lane = tid & 31;
@@ -140,6 +173,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
         sm.n_nodes = L.node_begin[qi + 1] - L.node_begin[qi];
         sm.n_phrases = L.phrase_begin ? L.phrase_begin[qi + 1] - L.phrase_begin[qi] : 0;
       }
+      if constexpr (kUnion) sm.u = L.u;
     }
     __syncthreads();
     if (sm.skip) continue;   // (CTA-uniform) slice_cnt stays 0: the slice contributes no keys
@@ -166,7 +200,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
       if (sm.cl[c].kind != NRTGPU_TERM) continue;
       int64_t target64 = (int64_t)slice_base + (int64_t)w * kWindowDocs;
       int32_t target = target64 > (int64_t)slice_end ? slice_end : (int32_t)target64;
-      const int32_t* docs = L.ix.post_docs + sm.cl[c].post_base;
+      const int32_t* docs = list_docs<kUnion>(L, sm.cl[c]);
       int lo = 0, hi = sm.cl[c].n_post;
       while (lo < hi) { int mid = (lo + hi) >> 1; if (__ldg(docs + mid) < target) lo = mid + 1; else hi = mid; }
       sm.bounds[sm.cl[c].slot][w] = (uint32_t)lo;
@@ -189,9 +223,10 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
         const int s = sm.cl[c].slot;
         const uint32_t b0 = sm.bounds[s][w], b1 = sm.bounds[s][w + 1];
         if (b1 > b0) any = true;
-        const int32_t* docs = L.ix.post_docs + sm.cl[c].post_base;
+        const int32_t* docs = list_docs<kUnion>(L, sm.cl[c]);
         const uint8_t* f8 = L.ix.post_f8 + sm.cl[c].post_base;
-        const bool scoring = sm.cl[c].scoring != 0;
+        bool scoring = sm.cl[c].scoring != 0;
+        if constexpr (kUnion) scoring = scoring && sm.cl[c].plane != kUnionList;   // a union slot: a presence byte
         unsigned char* slot_bytes = reinterpret_cast<unsigned char*>(sm.slots);
         for (uint32_t p = b0 + tid; p < b1; p += kThreads) {
           int32_t d = docs[p] - wbase;
@@ -239,7 +274,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
           for (int j = 0; j < s; ++j) if ((sm.q.driver_mask >> j) & 1u) below |= (uint64_t)0xff << (8 * j);
           const uint64_t own = (uint64_t)0xff << (8 * s);
           const uint32_t b0 = sm.bounds[s][w], b1 = sm.bounds[s][w + 1];
-          const int32_t* docs = L.ix.post_docs + sm.cl[c].post_base;
+          const int32_t* docs = list_docs<kUnion>(L, sm.cl[c]);
           for (uint32_t p0 = b0; p0 < b1; p0 += kThreads) {
             uint32_t p = p0 + tid;
             bool matched = false; int32_t doc = 0; float score = 0.0f;
@@ -278,7 +313,7 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
           const int s = sm.cl[c].slot;
           if ((sm.q.driver_mask >> s) & 1u) continue;
           const uint32_t b0 = sm.bounds[s][w], b1 = sm.bounds[s][w + 1];
-          const int32_t* docs = L.ix.post_docs + sm.cl[c].post_base;
+          const int32_t* docs = list_docs<kUnion>(L, sm.cl[c]);
           for (uint32_t p = b0 + tid; p < b1; p += kThreads) sm.slots[docs[p] - wbase] = 0;
         }
         __syncthreads();
@@ -294,6 +329,19 @@ __global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_c
     for (int o = 16; o > 0; o >>= 1) my_hits += __shfl_xor_sync(0xffffffffu, my_hits, o);
     if (lane == 0 && my_hits) atomicAdd(&L.total_hits[qi], my_hits);
   }
+}
+
+template <bool kTree, bool kAggs, bool kMulti = false>
+__global__ void __launch_bounds__(kThreads, 2) bool_window_kernel(const __grid_constant__ BoolLaunch L) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  bool_window_body<kTree, kAggs, kMulti, false>(L, smem_raw);
+}
+
+// tree batches with multi-phrase unions (shared memory: sizeof(BoolTreeSmemU))
+template <bool kAggs, bool kMulti = false>
+__global__ void __launch_bounds__(kThreads, 2) bool_window_union_kernel(const __grid_constant__ BoolLaunchU L) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  bool_window_body<true, kAggs, kMulti, true>(L, smem_raw);
 }
 
 // ---- per-query merge of the slice lists (TopDocs.merge semantics: key order is total) ----

@@ -180,6 +180,7 @@ struct nrtgpu_index {
   DevBuf<int32_t> positions;        // term positions, posting after posting (nrtgpu_index_add_positions)
   DevBuf<uint32_t> pos_off;         // [P] first position of each posting, relative to its term's base
   DevBuf<int64_t> pos_base;         // [n_terms + 1] first position of each term
+  std::vector<int64_t> h_pos_base;  // ... its host copy (the multi-phrase unions' positions cap)
   std::vector<std::unique_ptr<DevBuf<uint8_t>>> norms;
   DevBuf<const uint8_t*> norms_ptrs;
   DevBuf<float> caches;
@@ -257,6 +258,8 @@ struct nrtgpu_index {
     d.col_multi = col_multi.data(); d.col_n_distinct = col_n_distinct.data(); d.has_deletes = live_bits.p != nullptr;
     d.has_positions = has_positions;
     d.n_keyword = (int32_t)kw.size(); d.kw_n_terms = kw_n_terms.data();
+    d.term_pos = has_positions ? h_pos_base.data() : nullptr;
+    d.max_union_postings = ctx->plan.union_postings;
     return d;
   }
   KnnCorpus knn_corpus() const {   // what the kNN stages read; NRTGPU_KNN_SIMT, read on every call, forces the fp32 SIMT stage
@@ -309,6 +312,16 @@ struct nrtgpu_batch {
   DevBuf<DevPhrase> phrases;      // tree batches: cb.phrases
   DevBuf<int32_t> phrase_begin;   // tree batches: cb.phrase_begin
   DevBuf<int32_t> work_query, work_slice;
+  // multi-phrase unions of the batch (union_kernel.cuh), rebuilt by every batch_build that has some: the alternatives, the
+  // sort's keys and values (double buffers), the run heads and their scan, the entries and their positions
+  DevBuf<int64_t> u_alt_gstart, u_alt_post;
+  DevBuf<int32_t> u_alt_term, u_alt_union, u_alt_field, u_clause;
+  DevBuf<float> u_alt_weight;
+  DevBuf<uint8_t> u_mode, u_temp;
+  DevBuf<uint64_t> u_keys[2];
+  DevBuf<int32_t> u_vals[2], u_head, u_incl, u_docs, u_first, u_npos, u_pos_off, u_positions;
+  DevBuf<float> u_score;
+  UnionView u_view = {};
   DevBuf<int32_t> pruned;    // [nq] relation GTE flags
   DevBuf<int32_t> terminated; // [nq] terminateAfter cut the query short
   DevBuf<int32_t> timed_out;  // [nq] a work item of the query was skipped because the deadline had passed
@@ -442,12 +455,16 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   { const char* e = getenv("NRTGPU_ITEM_POSTINGS"); if (e && atoll(e) > 0) c->plan.item_postings = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE"); if (e && atoll(e) > 0) c->plan.item_share = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE_FULL"); if (e && atoll(e) > 0) c->plan.item_share_full = atoll(e); }
+  { const char* e = getenv("NRTGPU_UNION_POSTINGS"); if (e && atoll(e) > 0) c->plan.union_postings = std::min<int64_t>(atoll(e), kMaxUnionPostings); }
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_union_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmemU)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_union_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmemU)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_union_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmemU)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<false, false, v3::kCtasA, v3::kStageA, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)sizeof(v3::ProbeSmemT<v3::kStageA>)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<false, false, v3::kCtasB, v3::kStageB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -763,6 +780,7 @@ int nrtgpu_index_add_positions(nrtgpu_index* ix, const int32_t* positions, int64
   if ((rc = ix->pos_off.upload(off.data(), off.size()))) return rc;
   if ((rc = ix->pos_base.upload(base.data(), base.size()))) return rc;
   ix->device_bytes += (int64_t)(ix->positions.bytes() + ix->pos_off.bytes() + ix->pos_base.bytes()) - old_bytes;
+  ix->h_pos_base = std::move(base);
   ix->has_positions = true;
   return NRTGPU_OK;
 }
@@ -882,6 +900,83 @@ static int batch_compile(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& 
 
 static int batch_filter_rows(nrtgpu_batch* b, const BatchRequest& r, cudaStream_t st);
 
+// The multi-phrase unions of a compiled batch (union_kernel.cuh) into the batch's buffers, and every union clause's entry
+// range into its uploaded clauses; asynchronous on `st`. The scratch is sized by the postings the unions gather
+// (CompiledBatch::union_postings, capped by compile_tree) and the positions they merge.
+static int union_build(nrtgpu_batch* b, nrtgpu_index* ix, cudaStream_t st) {
+  const CompiledBatch& cb = b->cb;
+  const int32_t n_alts = (int32_t)cb.union_term.size();
+  std::vector<int64_t> gstart((size_t)n_alts + 1, 0), post((size_t)n_alts);
+  std::vector<int32_t> au((size_t)n_alts), af((size_t)n_alts);
+  for (int32_t u = 0; u < cb.n_unions(); ++u)
+    for (int32_t a = cb.union_begin[(size_t)u]; a < cb.union_begin[(size_t)u + 1]; ++a) {
+      const int32_t t = cb.union_term[(size_t)a];
+      post[(size_t)a] = ix->term_off[(size_t)t];
+      gstart[(size_t)a + 1] = gstart[(size_t)a] + (ix->term_off[(size_t)t + 1] - ix->term_off[(size_t)t]);
+      au[(size_t)a] = u; af[(size_t)a] = ix->term_field[(size_t)t];
+    }
+  const int64_t S = gstart[(size_t)n_alts];
+  int rc;
+  if ((rc = b->u_alt_gstart.upload_async(gstart.data(), gstart.size(), st)) || (rc = b->u_alt_post.upload_async(post.data(), post.size(), st)) ||
+      (rc = b->u_alt_term.upload_async(cb.union_term.data(), cb.union_term.size(), st)) ||
+      (rc = b->u_alt_union.upload_async(au.data(), au.size(), st)) || (rc = b->u_alt_field.upload_async(af.data(), af.size(), st)) ||
+      (rc = b->u_alt_weight.upload_async(cb.union_weight.data(), cb.union_weight.size(), st)) ||
+      (rc = b->u_mode.upload_async(cb.union_scored.data(), cb.union_scored.size(), st)) ||
+      (rc = b->u_clause.upload_async(cb.union_clause.data(), cb.union_clause.size(), st))) return rc;
+  const size_t n1 = (size_t)std::max<int64_t>(S, 1);
+  for (int i = 0; i < 2; ++i) if ((rc = b->u_keys[i].alloc(n1)) || (rc = b->u_vals[i].alloc(n1))) return rc;
+  if ((rc = b->u_head.alloc(n1)) || (rc = b->u_incl.alloc(n1)) || (rc = b->u_docs.alloc(n1)) || (rc = b->u_first.alloc(n1)) ||
+      (rc = b->u_score.alloc(n1)) || (rc = b->u_npos.alloc(n1 + 1)) || (rc = b->u_pos_off.alloc(n1 + 1)) ||
+      (rc = b->u_positions.alloc((size_t)std::max<int64_t>(cb.union_positions, 1)))) return rc;
+  NRT_CUDA_TRY(cudaMemsetAsync(b->u_npos.p, 0, (n1 + 1) * sizeof(int32_t), st));
+  UnionBuildLaunch U{};
+  U.ix = ix->view(); U.n_alts = n_alts; U.alt_gstart = b->u_alt_gstart.p; U.alt_post = b->u_alt_post.p; U.alt_term = b->u_alt_term.p;
+  U.alt_union = b->u_alt_union.p; U.alt_field = b->u_alt_field.p; U.alt_weight = b->u_alt_weight.p; U.union_mode = b->u_mode.p;
+  U.n_gather = S; U.head = b->u_head.p; U.incl = b->u_incl.p; U.docs = b->u_docs.p; U.score = b->u_score.p; U.first = b->u_first.p;
+  U.npos = b->u_npos.p; U.pos_off = b->u_pos_off.p; U.positions = b->u_positions.p;
+  U.clauses = b->clauses.p; U.union_clause = b->u_clause.p; U.n_union_clauses = (int32_t)cb.union_clause.size();
+  const unsigned grid = (unsigned)((S + 255) / 256);
+  if (S > 0) {
+    union_gather_kernel<<<grid, 256, 0, st>>>(U, b->u_keys[0].p, b->u_vals[0].p);
+    NRT_CUDA_TRY(cudaGetLastError());
+    int end_bit = 32;
+    while (end_bit < 64 && (1ll << (end_bit - 32)) < (int64_t)cb.n_unions()) ++end_bit;
+    cub::DoubleBuffer<uint64_t> keys(b->u_keys[0].p, b->u_keys[1].p);
+    cub::DoubleBuffer<int32_t> vals(b->u_vals[0].p, b->u_vals[1].p);
+    size_t tb = 0, ts = 0;
+    NRT_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, vals, (int)S, 0, end_bit, st));
+    NRT_CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, ts, b->u_head.p, b->u_incl.p, thrust::plus<void>(), (int)S, st));
+    size_t tp = 0;
+    NRT_CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, tp, b->u_npos.p, b->u_pos_off.p + 1, thrust::plus<void>(), (int)S, st));
+    if ((rc = b->u_temp.alloc(std::max(std::max(tb, ts), tp)))) return rc;
+    tb = b->u_temp.bytes();
+    NRT_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b->u_temp.p, tb, keys, vals, (int)S, 0, end_bit, st));
+    U.keys = keys.Current(); U.vals = vals.Current();
+    union_head_kernel<<<grid, 256, 0, st>>>(U);
+    NRT_CUDA_TRY(cudaGetLastError());
+    ts = b->u_temp.bytes();
+    NRT_CUDA_TRY(cub::DeviceScan::InclusiveScan(b->u_temp.p, ts, b->u_head.p, b->u_incl.p, thrust::plus<void>(), (int)S, st));
+    union_entry_kernel<<<grid, 256, 0, st>>>(U);
+    NRT_CUDA_TRY(cudaGetLastError());
+    if (cb.union_positions > 0) {
+      tp = b->u_temp.bytes();
+      // the exclusive scan of the position counts as pos_off[0] = 0 and the inclusive one behind it: both scans are the
+      // int scan with thrust::plus that the library already instantiates (cub's InclusiveSum / ExclusiveSum kernels for
+      // int spill 4 bytes on sm_90a)
+      NRT_CUDA_TRY(cudaMemsetAsync(b->u_pos_off.p, 0, sizeof(int32_t), st));
+      NRT_CUDA_TRY(cub::DeviceScan::InclusiveScan(b->u_temp.p, tp, b->u_npos.p, b->u_pos_off.p + 1, thrust::plus<void>(), (int)S, st));
+      union_positions_kernel<<<grid, 256, 0, st>>>(U);
+      NRT_CUDA_TRY(cudaGetLastError());
+    }
+  }
+  if (U.n_union_clauses > 0) {
+    union_patch_kernel<<<(unsigned)((U.n_union_clauses + 127) / 128), 128, 0, st>>>(U);
+    NRT_CUDA_TRY(cudaGetLastError());
+  }
+  b->u_view = UnionView{b->u_docs.p, b->u_score.p, b->u_pos_off.p, b->u_positions.p};
+  return NRTGPU_OK;
+}
+
 // the KEYWORD after values of the queries with searchAfter: 0 (null) or a code 1 .. 2n + 1 of the column's n terms (n_distinct
 // of the order's field on an image; the caller's n on a searcher)
 static int check_keyword_after(const nrtgpu_sort_order* o, const int64_t* after, const nrtgpu_query* queries, int32_t nq,
@@ -920,6 +1015,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
     b->sort_kind = sorted ? sort->kind : 0; b->sort_column = sorted ? sort->column : 0; b->sort_reverse = sorted ? (sort->reverse != 0) : 0;
     b->sort_missing_value = sorted ? sort->missing_value : 0;
   }
+  if (b->cb.n_unions() > 0 && (rc = union_build(b, ix, st))) return rc;
   WorkPlan& p = b->plan;
   plan_work(ix->dict(), ix->ctx->plan, b->cb, &p);
   if ((rc = b->work_query.upload_async(p.work_query.data(), p.work_query.size(), st))) return rc;
@@ -1039,6 +1135,7 @@ int nrtgpu_batch_prepare_tree_phrases(nrtgpu_index* ix, const nrtgpu_clause* cla
   BatchRequest r = tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags);
   int rc = phrase_request(&r, phrases, n_phrases, phrase_terms, n_phrase_terms);
   if (rc) return rc;
+  r.unions = true;
   std::unique_ptr<nrtgpu_batch> b(new nrtgpu_batch);
   if ((rc = batch_build(b.get(), ix, r, (cudaStream_t)0))) return rc;
   NRT_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)0));
@@ -1133,7 +1230,15 @@ static int batch_engine_launch(nrtgpu_batch* b, const AggLaunch* aggs, bool mult
   L.deadline_ns = (!p2 && b->limits_active) ? b->deadline_ns : 0; L.clock0 = b->clock0.p; L.timed_out = b->timed_out.p;
   L.aggs = aggs;
   const unsigned grid = (unsigned)b->plan.n_work();
-  if (b->cb.tree) {
+  if (b->cb.tree && b->cb.n_unions() > 0) {
+    BoolLaunchU LU;
+    static_cast<BoolLaunch&>(LU) = L;
+    LU.nodes = b->nodes.p; LU.node_begin = b->node_begin.p; LU.phrases = b->phrases.p; LU.phrase_begin = b->phrase_begin.p;
+    LU.u = b->u_view;
+    if (multi) bool_window_union_kernel<true, true><<<grid, kThreads, sizeof(BoolTreeSmemU), st>>>(LU);
+    else if (aggs) bool_window_union_kernel<true><<<grid, kThreads, sizeof(BoolTreeSmemU), st>>>(LU);
+    else bool_window_union_kernel<false><<<grid, kThreads, sizeof(BoolTreeSmemU), st>>>(LU);
+  } else if (b->cb.tree) {
     L.nodes = b->nodes.p; L.node_begin = b->node_begin.p; L.phrases = b->phrases.p; L.phrase_begin = b->phrase_begin.p;
     if (multi) bool_window_kernel<true, true, true><<<grid, kThreads, sizeof(BoolTreeSmem), st>>>(L);
     else if (aggs) bool_window_kernel<true, true><<<grid, kThreads, sizeof(BoolTreeSmem), st>>>(L);
@@ -1950,6 +2055,7 @@ int nrtgpu_search_tree_phrases(nrtgpu_index* ix, const nrtgpu_clause* clauses, i
   BatchRequest r = tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags);
   int rc = phrase_request(&r, phrases, n_phrases, phrase_terms, n_phrase_terms);
   if (rc) return rc;
+  r.unions = true;
   SearchOut o; o.docs = out_docs; o.scores = out_scores; o.counts = out_counts; o.total_hits = out_total_hits; o.relation = out_relation;
   o.hit_timeout = out_hit_timeout; o.terminated_early = out_terminated_early;
   return search_bool_impl(ix, r, limits, stream, o);
@@ -2190,6 +2296,7 @@ static int tree_aggs_request(BatchRequest* r, const nrtgpu_clause* clauses, int3
   if (rc || (rc = aggs_request(r, aggs, n_aggs, results, nested, n_nested, nested_results, nested_sorts, agg_filters, filter_clauses,
                                n_filter_clauses, filter_queries, n_filter_queries))) return rc;
   r->window_collectors = true;
+  r->unions = true;
   return NRTGPU_OK;
 }
 
@@ -3307,6 +3414,7 @@ int nrtgpu_searcher_search_tree_phrases(nrtgpu_searcher* s, const nrtgpu_clause*
   BatchRequest r = tree_request(clauses, n_clauses, nodes, n_nodes, queries, nq, top_k, total_hits_threshold, flags);
   int rc = phrase_request(&r, phrases, n_phrases, phrase_terms, n_phrase_terms);
   if (rc) return rc;
+  r.unions = true;
   KwLeafRequest kw;
   return searcher_scored(s, "nrtgpu_searcher_search_tree_phrases", nq, top_k, stream, [&](int l, int32_t* d_record) {
     // (the leaves run in order under the searcher's lock: the first prepares the keyword codes of every leaf)

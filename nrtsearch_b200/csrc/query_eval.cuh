@@ -4,10 +4,16 @@
 // the window engine's tree instantiation and the second pass of tree batches. The engines differ only in how they find a
 // term's tf and norm, and a phrase term's posting; each passes that in.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 #include "../../include/nrtgpu.h"
 
 namespace nrtgpu {
+
+// Whether a tree engine's shared state (Smem) may hold term slots whose lists are call unions (batch_plan.h kUnionList):
+// only the kUnion instantiations of the window engine (bool_kernel.cuh BoolTreeSmemU), which specialise it. Every other
+// engine compiles the code below without the union branches.
+template <class Smem> struct SmemUnions : std::false_type {};
 
 struct DevIndexView {
   int32_t n_docs;
@@ -254,26 +260,41 @@ __device__ __forceinline__ uint32_t presence_mask(uint64_t s) {
 template <class Smem>
 __device__ __noinline__ float phrase_freq(const DevIndexView& ix, const Smem& sm, const DevPhrase& ph, int32_t doc,
                                           bool first_only) {
+  constexpr bool kUnions = SmemUnions<Smem>::value;
   const int n = ph.n_terms;
   int64_t cur[kMaxTermSlots], end[kMaxTermSlots];
+  const int32_t* P = ix.positions;
+  uint32_t in_union = 0;   // (kUnions) bit i: term i's positions are sm.u.positions[cur[i] .. end[i]), else P's
+  auto at = [&](int i, int64_t k) {   // position k of term i
+    if constexpr (kUnions) return __ldg(((in_union >> i) & 1u ? sm.u.positions : P) + k);
+    else return __ldg(P + k);
+  };
   for (int i = 0; i < n; ++i) {
     const DevClause& t = sm.cl[ph.clause0 + i];
     const uint32_t lo = phrase_posting(ix, sm, t, doc);
+    if constexpr (kUnions) {
+      if (t.plane == kUnionList) {   // a union slot: its entry's merged positions
+        const int64_t e = t.post_base + lo;
+        in_union |= 1u << i;
+        cur[i] = __ldg(sm.u.pos_off + e);
+        end[i] = __ldg(sm.u.pos_off + e + 1);
+        continue;
+      }
+    }
     const int64_t gp = t.post_base + lo, base = __ldg(ix.pos_base + t.col);
     cur[i] = base + __ldg(ix.pos_off + gp);
     end[i] = (int64_t)lo + 1 < (int64_t)t.n_post ? base + __ldg(ix.pos_off + gp + 1) : __ldg(ix.pos_base + t.col + 1);
   }
-  const int32_t* P = ix.positions;
   float freq = 0.0f;
   if (ph.slop == 0) {
     for (int64_t a = cur[0]; a < end[0]; ++a) {
-      const int32_t phrase_pos = __ldg(P + a) - ph.offset[0];
+      const int32_t phrase_pos = at(0, a) - ph.offset[0];
       bool ok = true;
       for (int j = 1; j < n && ok; ++j) {
         const int32_t want = phrase_pos + ph.offset[j];
-        while (cur[j] < end[j] && __ldg(P + cur[j]) < want) ++cur[j];
+        while (cur[j] < end[j] && at(j, cur[j]) < want) ++cur[j];
         if (cur[j] == end[j]) return freq;   // term j has no position left: no later lead position can match
-        ok = __ldg(P + cur[j]) == want;
+        ok = at(j, cur[j]) == want;
       }
       if (ok) { freq = __fadd_rn(freq, 1.0f); if (first_only) return freq; }
     }
@@ -283,7 +304,7 @@ __device__ __noinline__ float phrase_freq(const DevIndexView& ix, const Smem& sm
   int32_t end_pos = INT_MIN;
   uint32_t inq = 0;
   for (int i = 0; i < n; ++i) {
-    pos[i] = __ldg(P + cur[i]) - ph.offset[i]; ++cur[i];
+    pos[i] = at(i, cur[i]) - ph.offset[i]; ++cur[i];
     end_pos = max(end_pos, pos[i]);
     inq |= 1u << i;
   }
@@ -303,7 +324,7 @@ __device__ __noinline__ float phrase_freq(const DevIndexView& ix, const Smem& sm
     bool positioned = true, matched = false;
     for (;;) {
       if (cur[pp] >= end[pp]) { positioned = false; matched = match_len <= ph.slop; break; }
-      pos[pp] = __ldg(P + cur[pp]) - ph.offset[pp]; ++cur[pp];
+      pos[pp] = at(pp, cur[pp]) - ph.offset[pp]; ++cur[pp];
       end_pos = max(end_pos, pos[pp]);
       if (pos[pp] > next) {   // done minimising the current match length
         inq |= 1u << pp;
@@ -326,7 +347,7 @@ __device__ __noinline__ float phrase_freq(const DevIndexView& ix, const Smem& sm
 // terms that do not score: 1): the root's required and excluded slots, liveness, then the nodes bottom-up (reverse
 // pre-order: children before parents) through eval_node, no recursion. sm holds the query (q), its clauses (cl), nodes
 // (nodes, n_nodes), phrase records (phrases) and the per-slot BM25 caches (cache[slot][norm byte]); phrase_posting(ix, sm, ...)
-// is the engine's.
+// is the engine's. A union slot that scores (a one-position multi-phrase) reads its entry's score (SmemUnions).
 template <class Smem>
 __device__ __forceinline__ bool eval_tree(const DevIndexView& ix, const Smem& sm, int32_t doc, uint64_t slot, float* out_score) {
   const uint32_t mask = presence_mask(slot);
@@ -350,6 +371,9 @@ __device__ __forceinline__ bool eval_tree(const DevIndexView& ix, const Smem& sm
     const uint32_t b = (uint32_t)((slot >> (8 * c.slot)) & 0xff);
     if (b == 0) return false;
     if (c.scoring) {
+      if constexpr (SmemUnions<Smem>::value) {
+        if (c.plane == kUnionList) { *s = __ldg(sm.u.score + c.post_base + phrase_posting(ix, sm, c, doc)); return true; }
+      }
       const float f = (b == 255u) ? exact_freq_slow(ix, c, doc) : (float)b;
       const uint8_t* nrm = ix.norms[c.field];
       const uint32_t nb = nrm ? (uint32_t)nrm[doc] : 1u;

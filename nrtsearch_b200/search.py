@@ -139,6 +139,47 @@ class PhraseQuery:
         return [(int(t), int(p)) for t, p in zip(self.terms, pos)]
 
 
+@dataclass
+class MultiPhraseQuery:
+    """MultiPhraseQuery(terms, positions, slop): a phrase whose position i holds any of the alternative terms terms[i]
+    (match_phrase over stacked synonyms; the query MatchPhrasePrefixQuery rewrites to). All terms on one text field, term
+    ids as for PhraseQuery; positions default to 0, 1, 2, ... and must ascend. A doc matches position i when any of
+    terms[i] occurs there; one position is the BooleanQuery of SHOULD TermQuerys over its alternatives, no position (or an
+    empty one) matches nothing. Runs on the window engine as a leaf of a query tree (GpuIndexSearcher.search_tree), the
+    alternatives of a position merged on the device (nrtgpu.h NRTGPU_MULTI_PHRASE)."""
+    terms: List[List[int]] = field(default_factory=list)
+    positions: Optional[List[int]] = None
+    slop: int = 0
+
+    def term_positions(self) -> List[Tuple[int, int]]:
+        """(term, position) of every alternative, position after position; [] when the query matches nothing"""
+        pos = list(range(len(self.terms))) if self.positions is None else [int(p) for p in self.positions]
+        if len(pos) != len(self.terms):
+            raise ValueError("MultiPhraseQuery: one position per term array")
+        if len(set(pos)) != len(pos):
+            raise ValueError("MultiPhraseQuery: one term array per position")
+        if any(len(alts) == 0 for alts in self.terms):
+            return []
+        return [(int(t), p) for alts, p in zip(self.terms, pos) for t in alts]
+
+
+@dataclass
+class MatchPhrasePrefixQuery:
+    """match_phrase_prefix (reference MatchPhrasePrefixQuery.java): terms[i] are the analyzed tokens at position i (several
+    at one position: stacked synonyms) and `expansions` the indexed terms the last token's prefix expands to, which the
+    adaptor finds in the term dictionary (at most max_expansions, default 50; INTEGRATION.md). It rewrites as the
+    reference does: no expansion matches nothing; otherwise a MultiPhraseQuery of terms followed by the expansions, so a
+    one-token query is the disjunction of its expansions. Term ids as for PhraseQuery."""
+    terms: List[List[int]] = field(default_factory=list)
+    expansions: List[int] = field(default_factory=list)
+    slop: int = 0
+
+    def rewrite(self) -> MultiPhraseQuery:
+        if not self.expansions:
+            return MultiPhraseQuery([], None, int(self.slop))
+        return MultiPhraseQuery([list(t) for t in self.terms] + [list(self.expansions)], None, int(self.slop))
+
+
 @dataclass(frozen=True)
 class BooleanClause:
     query: object
@@ -634,13 +675,22 @@ def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Opti
     down). A ConstantScoreQuery or MinScoreQuery node takes the boost folded down to it as its own and the fold starts again
     at 1 below it; MinScoreQuery(q, 0) is compiled as q, and a min_score < 0 raises ValueError.
     phrase_table: return (Clause[], n_clauses, Node[], n_nodes, Phrase[], n_phrases, PhraseTerm[], n_phrase_terms, Query[],
-    nq) for nrtgpu_search_tree_phrases instead: a PhraseQuery leaf is a clause of kind 4 whose id indexes the phrase table.
-    Without it a PhraseQuery is refused."""
+    nq) for nrtgpu_search_tree_phrases instead: a PhraseQuery leaf is a clause of kind 4 whose id indexes the phrase table,
+    a MultiPhraseQuery (or MatchPhrasePrefixQuery, rewritten) one of kind 6. Without it either is refused."""
     flat, nodes, qs = [], [], []
     phrases, pterms = [], []
 
     def leaf(sub, sb, occ):
-        if isinstance(sub, PhraseQuery):
+        if isinstance(sub, MatchPhrasePrefixQuery):
+            sub = sub.rewrite()
+        if isinstance(sub, MultiPhraseQuery):
+            if not phrase_table:
+                raise NrtGpuUnsupported(3, "MultiPhraseQuery needs compile_tree(..., phrase_table=True)")
+            begin = len(pterms)
+            pterms.extend(sub.term_positions())
+            phrases.append((begin, len(pterms), int(sub.slop), 0))
+            flat.append((int(occ), 6, len(phrases) - 1, float(sb), 0, 0))
+        elif isinstance(sub, PhraseQuery):
             if not phrase_table:
                 raise NrtGpuUnsupported(3, "PhraseQuery needs compile_tree(..., phrase_table=True)")
             begin = len(pterms)
