@@ -724,79 +724,187 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
           if (cb >= n_t) { ++ct; cb = 0; continue; }
           const int t = t_dense ? 0 : ct;
           const uint32_t need = t_dense ? ((n_term >= 32) ? 0xffffffffu : ((1u << n_term) - 1u)) : sm.s_need[t];
-          const uint32_t need_plane = NRT_KNOCK(1) ? 0u : need & plane_mask, need_long = NRT_KNOCK(2) ? 0u : need & long_mask,
-                         need_short = NRT_KNOCK(2) ? 0u : need & short_mask, need_glob = need & global_mask;
           const bool t_staged = !t_dense && (((long_mask | short_mask) >> t) & 1u);
           const bool t_ess = (ess_mask >> t) & 1u;
           const uint32_t candbelow = t_dense ? 0u : (kSimple ? sm.s_candrun[t] : sm.s_candbelow[t]),
                          cntbefore = t_dense ? 0u : (kSimple ? sm.s_cntrun[t] : sm.s_cntbefore[t]);
           const int32_t dense_d0 = sm.run_d0;
-          const int32_t* sdoc_t = sm.sdocs + ((int)sm.s_ra[t] + sm.s_sdelta[t]);   // posting x of the run segment: sdoc_t[x]
-          const uint8_t* sf8_t = sm.sf8 + ((int)sm.s_ra[t] + sm.s_sdelta[t]);
-          const int32_t* gdoc_t = sm.pq.gdocs[t] + sm.s_ra[t];
-          const uint8_t* gf8_t = sm.pq.gf8[t] + sm.s_ra[t];
           const uint32_t tshift = t_dense ? 0u : 8u * (uint32_t)t;
-          // software pipeline: the postings of the NEXT round are fetched before the current round is processed
-          // (generic pointers: one load path for staged -- shared memory -- and plane / global -- HBM -- driver lists)
-          const int32_t* dptr = t_staged ? sdoc_t : gdoc_t;
-          const uint8_t* fptr = t_staged ? sf8_t : gf8_t;
-          int32_t nd[kR]; uint32_t nf[kR];
+          constexpr uint32_t kRound = kR * kThreads;
+          constexpr int kP = kT - 1;   // slots a driver posting of a pure disjunction probes (every slot but its own)
+          int32_t doc[kR], nd[kR]; uint32_t df[kR], nf[kR];
+          uint32_t gq[kR][kP];         // (simple) the plane bytes of round r, gathered one round ahead
+          // The simple instantiations read the driver list in one of two forms, fixed for all its rounds: staged (posting
+          // x of the run segment at sdocs / sf8[sbase + x]) or in place (gdoc / gf8[x], read-only global loads).
+          const int sbase = (int)sm.s_ra[t] + sm.s_sdelta[t];
+          const int32_t* gdoc = sm.pq.gdocs[t] + sm.s_ra[t];
+          const uint8_t* gf8 = sm.pq.gf8[t] + sm.s_ra[t];
+          // The probe plan of a pure disjunction's driver list, built once per driver list and kept in registers for all
+          // its rounds (the rounds store to shared memory, so the compiler would otherwise reload it per posting):
+          // entries [0, np) are the slots gathered from a tf plane, pw = the plane's 2-bit codes; entries [np, n_probe)
+          // the slots searched, pw = posting range a | b << 32 with pd = the shared-memory index of posting 0 (long: a
+          // granule of [a, b) is searched; short: the whole range; global: [a, b) of the list in global memory). Byte i
+          // of pslot: the slot of entry i and, for a search, its kind << 2. A search of an empty range finds nothing, so
+          // such a slot is left out.
+          uint64_t pw[kP]; int32_t pd[kP];
+          uint32_t pslot = 0u;
+          int np = 0, n_probe = 0;
+          // postings of the round that starts at b0 (doc -1: no posting)
+          auto fetch = [&](uint32_t b0, int32_t (&d)[kR], uint32_t (&f)[kR]) {
 #pragma unroll
-          for (int j = 0; j < kR; ++j) {
-            const uint32_t x = cb + (uint32_t)(j * kThreads + tid);
-            nd[j] = -1; nf[j] = 0;   // doc -1: no posting
-            if (x < n_t) {
-              if (t_dense) nd[j] = dense_d0 + (int32_t)x; else { nd[j] = dptr[x]; nf[j] = fptr[x]; }
+            for (int j = 0; j < kR; ++j) {
+              const uint32_t x = b0 + (uint32_t)(j * kThreads + tid);
+              d[j] = -1; f[j] = 0u;
+              if (x < n_t) {
+                if (t_staged) { d[j] = sm.sdocs[sbase + (int)x]; f[j] = sm.sf8[sbase + (int)x]; }
+                else { d[j] = __ldg(gdoc + x); f[j] = __ldg(gf8 + x); }
+              }
+            }
+          };
+          // plane gathers of the postings of a round (2-bit tf codes, all in flight together; lanes without a posting
+          // gather byte 0 of the plane: harmless, and the branches stay warp-uniform)
+          auto gather = [&](const int32_t (&d)[kR], uint32_t (&g)[kR][kP]) {
+#pragma unroll
+            for (int j = 0; j < kR; ++j) {
+              const uint32_t d4 = (uint32_t)max(d[j], 0) >> 2;
+#pragma unroll
+              for (int i = 0; i < kP; ++i) g[j][i] = i < np ? (uint32_t)__ldg(reinterpret_cast<const uint8_t*>(pw[i]) + d4) : 0u;
+            }
+          };
+          // The generic instantiations keep the mask-driven round: what each slot is probed by, tested per posting, one
+          // generic load path for staged (shared memory) and in-place (global memory) driver lists, postings one round
+          // ahead and the round's gathers issued as it starts. With the plan they ran slower (DESIGN.md §4.1 Rounds):
+          // their drains call the clause evaluation with every live register saved around the call.
+          const uint32_t need_plane = NRT_KNOCK(1) ? 0u : need & plane_mask, need_long = NRT_KNOCK(2) ? 0u : need & long_mask,
+                         need_short = NRT_KNOCK(2) ? 0u : need & short_mask, need_glob = need & global_mask;
+          const int32_t* dptr = t_staged ? sm.sdocs + sbase : gdoc;
+          const uint8_t* fptr = t_staged ? sm.sf8 + sbase : gf8;
+          if constexpr (kSimple) {
+            uint32_t rest_p = NRT_KNOCK(1) ? 0u : need & plane_mask;
+            uint32_t rest_s = (NRT_KNOCK(2) ? 0u : need & (long_mask | short_mask)) | (need & global_mask);
+            for (int u = 0; u < kT; ++u) if (((rest_s >> u) & 1u) && sm.s_rb[u] <= sm.s_ra[u]) rest_s &= ~(1u << u);
+            np = __popc(rest_p);
+            n_probe = np + __popc(rest_s);
+#pragma unroll
+            for (int i = 0; i < kP; ++i) {
+              pw[i] = 0ull; pd[i] = 0;
+              if (rest_p) {
+                const int u = __ffs(rest_p) - 1;
+                rest_p &= rest_p - 1u;
+                pw[i] = reinterpret_cast<uint64_t>(sm.pq.plane2[u]);
+                pslot |= (uint32_t)u << (8 * i);
+              } else if (rest_s) {
+                const int u = __ffs(rest_s) - 1;
+                rest_s &= rest_s - 1u;
+                const uint32_t kind = ((long_mask >> u) & 1u) ? kLong : (((short_mask >> u) & 1u) ? kShort : kGlobal);
+                pw[i] = (uint64_t)sm.s_ra[u] | ((uint64_t)sm.s_rb[u] << 32);
+                pd[i] = sm.s_sdelta[u];
+                pslot |= ((uint32_t)u | (kind << 2)) << (8 * i);
+              }
+            }
+            // Software pipeline, restarted from cb for every driver list and after every flush (nothing of it outlives a
+            // round that did not complete): the postings of round r + 2 are fetched and the plane gathers of round r + 1
+            // issued before round r is searched, tested and queued, so the gathers of a warp overlap its own searches.
+            fetch(cb, doc, df);
+            gather(doc, gq);
+            fetch(cb + kRound, nd, nf);
+          } else {
+            np = need_plane != 0u;
+#pragma unroll
+            for (int j = 0; j < kR; ++j) {
+              const uint32_t x = cb + (uint32_t)(j * kThreads + tid);
+              nd[j] = -1; nf[j] = 0;   // doc -1: no posting
+              if (x < n_t) {
+                if (t_dense) nd[j] = dense_d0 + (int32_t)x; else { nd[j] = dptr[x]; nf[j] = fptr[x]; }
+              }
             }
           }
           while (!full && cb < n_t) {
             const unsigned long long theta = sm.theta;
             const float theta_s = theta ? key_score(theta) : -INFINITY;
-            int32_t doc[kR]; uint32_t word[kR];
-            uint32_t pbyte[kR][kT];
+            uint32_t word[kR];
+            uint32_t pbyte[kR][kT];   // (generic) the plane bytes of the round, by slot
+            uint32_t ngq[kR][kP]; int32_t nnd[kR]; uint32_t nnf[kR];   // (simple) the next stages of the pipeline
+            if constexpr (kSimple) {
+              if (cb + kRound < n_t) gather(nd, ngq);
+              else {
 #pragma unroll
-            for (int j = 0; j < kR; ++j) { doc[j] = nd[j]; word[j] = nf[j] << tshift; }
-            // plane gathers of every posting of the round (2-bit tf codes, all in flight together)
-            // (lanes without a posting gather byte 0 of the plane: harmless, and the branches stay CTA-uniform)
+                for (int j = 0; j < kR; ++j)
 #pragma unroll
-            for (int j = 0; j < kR; ++j) {
-              const uint32_t d4 = (uint32_t)max(doc[j], 0) >> 2;
-              pbyte[j][0] = 0u; pbyte[j][1] = 0u; pbyte[j][2] = 0u; pbyte[j][3] = 0u;
-              if (need_plane & 1u) pbyte[j][0] = (uint32_t)__ldg(sm.pq.plane2[0] + d4);
-              if (need_plane & 2u) pbyte[j][1] = (uint32_t)__ldg(sm.pq.plane2[1] + d4);
-              if (need_plane & 4u) pbyte[j][2] = (uint32_t)__ldg(sm.pq.plane2[2] + d4);
-              if (need_plane & 8u) pbyte[j][3] = (uint32_t)__ldg(sm.pq.plane2[3] + d4);
-            }
-            // next round's postings
-            {
-              const uint32_t nb = cb + (uint32_t)(kR * kThreads);
+                  for (int i = 0; i < kP; ++i) ngq[j][i] = 0u;
+              }
+              fetch(cb + 2 * kRound, nnd, nnf);
 #pragma unroll
-              for (int j = 0; j < kR; ++j) {
-                const uint32_t x = nb + (uint32_t)(j * kThreads + tid);
-                nd[j] = -1; nf[j] = 0;
-                if (x < n_t) {
-                  if (t_dense) nd[j] = dense_d0 + (int32_t)x; else { nd[j] = dptr[x]; nf[j] = fptr[x]; }
+              for (int j = 0; j < kR; ++j) word[j] = df[j] << tshift;
+              // searches (staged lists in shared memory)
+              if (n_probe > np) {
+#pragma unroll
+                for (int j = 0; j < kR; ++j) {
+                  if (doc[j] < 0) continue;
+                  const int g = (doc[j] - slice_base) >> kLogGran;
+#pragma unroll
+                  for (int i = 0; i < kP; ++i) {
+                    if (i < np || i >= n_probe) continue;
+                    const uint32_t u = (pslot >> (8 * i)) & 3u, kind = (pslot >> (8 * i + 2)) & 7u;
+                    const uint32_t a = (uint32_t)pw[i], b = (uint32_t)(pw[i] >> 32);
+                    uint32_t r = 0;
+                    if (kind == kLong) {
+                      const uint32_t lo = max(sm.gb[u][g], a), hi = min(sm.gb[u][g + 1], b);
+                      if (hi > lo) r = probe_smem(sm, (int)lo + pd[i], (int)hi + pd[i], doc[j]);
+                    } else if (kind == kShort) {
+                      r = probe_smem(sm, (int)a + pd[i], (int)b + pd[i], doc[j]);
+                    } else {
+                      r = probe_global(sm.pq.gdocs[u], sm.pq.gf8[u], a, b, doc[j]);
+                    }
+                    word[j] |= r << (8 * u);
+                  }
                 }
               }
-            }
-            // searches of the staged lists (shared memory; overlaps the gathers)
-            if (need_long | need_short | need_glob) {
+            } else {
+#pragma unroll
+              for (int j = 0; j < kR; ++j) { doc[j] = nd[j]; word[j] = nf[j] << tshift; }
+              // plane gathers of every posting of the round (2-bit tf codes, all in flight together)
+              // (lanes without a posting gather byte 0 of the plane: harmless, and the branches stay CTA-uniform)
 #pragma unroll
               for (int j = 0; j < kR; ++j) {
-                if (doc[j] < 0) continue;
-                const int g = (doc[j] - slice_base) >> kLogGran;
+                const uint32_t d4 = (uint32_t)max(doc[j], 0) >> 2;
+                pbyte[j][0] = 0u; pbyte[j][1] = 0u; pbyte[j][2] = 0u; pbyte[j][3] = 0u;
+                if (need_plane & 1u) pbyte[j][0] = (uint32_t)__ldg(sm.pq.plane2[0] + d4);
+                if (need_plane & 2u) pbyte[j][1] = (uint32_t)__ldg(sm.pq.plane2[1] + d4);
+                if (need_plane & 4u) pbyte[j][2] = (uint32_t)__ldg(sm.pq.plane2[2] + d4);
+                if (need_plane & 8u) pbyte[j][3] = (uint32_t)__ldg(sm.pq.plane2[3] + d4);
+              }
+              // next round's postings
+              {
+                const uint32_t nb = cb + kRound;
 #pragma unroll
-                for (int u = 0; u < kT; ++u) {
-                  uint32_t b = 0;
-                  if ((need_long >> u) & 1u) {
-                    const uint32_t lo = max(sm.gb[u][g], sm.s_ra[u]), hi = min(sm.gb[u][g + 1], sm.s_rb[u]);
-                    if (hi > lo) b = probe_smem(sm, (int)lo + sm.s_sdelta[u], (int)hi + sm.s_sdelta[u], doc[j]);
-                  } else if ((need_short >> u) & 1u) {
-                    if (sm.s_rb[u] > sm.s_ra[u]) b = probe_smem(sm, (int)sm.s_ra[u] + sm.s_sdelta[u], (int)sm.s_rb[u] + sm.s_sdelta[u], doc[j]);
-                  } else if ((need_glob >> u) & 1u) {
-                    if (sm.s_rb[u] > sm.s_ra[u]) b = probe_global(sm.pq.gdocs[u], sm.pq.gf8[u], sm.s_ra[u], sm.s_rb[u], doc[j]);
+                for (int j = 0; j < kR; ++j) {
+                  const uint32_t x = nb + (uint32_t)(j * kThreads + tid);
+                  nd[j] = -1; nf[j] = 0;
+                  if (x < n_t) {
+                    if (t_dense) nd[j] = dense_d0 + (int32_t)x; else { nd[j] = dptr[x]; nf[j] = fptr[x]; }
                   }
-                  word[j] |= b << (8 * u);
+                }
+              }
+              // searches of the staged lists (shared memory; overlaps the gathers)
+              if (need_long | need_short | need_glob) {
+#pragma unroll
+                for (int j = 0; j < kR; ++j) {
+                  if (doc[j] < 0) continue;
+                  const int g = (doc[j] - slice_base) >> kLogGran;
+#pragma unroll
+                  for (int u = 0; u < kT; ++u) {
+                    uint32_t b = 0;
+                    if ((need_long >> u) & 1u) {
+                      const uint32_t lo = max(sm.gb[u][g], sm.s_ra[u]), hi = min(sm.gb[u][g + 1], sm.s_rb[u]);
+                      if (hi > lo) b = probe_smem(sm, (int)lo + sm.s_sdelta[u], (int)hi + sm.s_sdelta[u], doc[j]);
+                    } else if ((need_short >> u) & 1u) {
+                      if (sm.s_rb[u] > sm.s_ra[u]) b = probe_smem(sm, (int)sm.s_ra[u] + sm.s_sdelta[u], (int)sm.s_rb[u] + sm.s_sdelta[u], doc[j]);
+                    } else if ((need_glob >> u) & 1u) {
+                      if (sm.s_rb[u] > sm.s_ra[u]) b = probe_global(sm.pq.gdocs[u], sm.pq.gf8[u], sm.s_ra[u], sm.s_rb[u], doc[j]);
+                    }
+                    word[j] |= b << (8 * u);
+                  }
                 }
               }
             }
@@ -806,11 +914,17 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
 #pragma unroll
             for (int j = 0; j < kR; ++j) {
               uint32_t v = word[j];
-              if (need_plane) {
-                // the four gathered bytes side by side; the doc's 2-bit code of every plane with one shift and one mask
+              if (np) {
+                // the gathered bytes side by side; the doc's 2-bit code of every plane with one shift and one mask
                 // (bits shifted in from the neighbouring byte fall outside the mask); code 3 = "three or more" becomes
                 // kTfInexact (resolved when the doc is scored)
-                const uint32_t raw = pbyte[j][0] | (pbyte[j][1] << 8) | (pbyte[j][2] << 16) | (pbyte[j][3] << 24);
+                uint32_t raw = 0u;
+                if constexpr (kSimple) {
+#pragma unroll
+                  for (int i = 0; i < kP; ++i) raw |= gq[j][i] << (8u * ((pslot >> (8 * i)) & 3u));
+                } else {
+                  raw = pbyte[j][0] | (pbyte[j][1] << 8) | (pbyte[j][2] << 16) | (pbyte[j][3] << 24);
+                }
                 const uint32_t codes = (raw >> (((uint32_t)max(doc[j], 0) & 3u) * 2u)) & 0x03030303u;
                 const uint32_t sat = __vcmpeq4(codes, 0x03030303u);   // 0xff where the code saturated
                 v |= (codes & ~sat) | (sat & (kTfInexact * 0x01010101u));
@@ -839,7 +953,15 @@ __global__ void __launch_bounds__(kThreads, kCtas) posting_probe_kernel(const __
               if (kStats && lane == 0) dbg_queued += __popc(bal);
               while (!full && qn >= 32) full = __any_sync(0xffffffffu, drain(32));   // (a parked key stops the warp: park is free whenever drain runs)
             }
-            cb += kR * kThreads;
+            if constexpr (kSimple) {
+#pragma unroll
+              for (int j = 0; j < kR; ++j) {
+                doc[j] = nd[j]; df[j] = nf[j]; nd[j] = nnd[j]; nf[j] = nnf[j];
+#pragma unroll
+                for (int i = 0; i < kP; ++i) gq[j][i] = ngq[j][i];
+              }
+            }
+            cb += kRound;
             if (kStats && tid == 0) ++dbg_rounds;
           }
         }
