@@ -209,13 +209,48 @@ int nrtgpu_search_bool_ex(nrtgpu_index* ix, const nrtgpu_clause* clauses, int32_
  *                           (the root counts as one), top_k > 1024. CONSTANT and MIN_SCORE nodes count as nodes and
  *                           levels, their clause as a clause.
  * With n_nodes == 0 nrtgpu_search_tree is nrtgpu_search_bool_ex (same compile, same engine); the other entry points
- * reject NRTGPU_NODE clauses as a bad clause kind. Node kind 2 is not a kind. */
+ * reject NRTGPU_NODE clauses as a bad clause kind. Node kinds 2 and 5 are not kinds.
+ *
+ * NESTED node (NestedQuery, reference QueryNodeMapper.getNestedQuery: Lucene 10 ToParentBlockJoinQuery): a block join.
+ * The image stores each parent as a block, its child docs first and the parent last; the parents are the docs of one
+ * term (nrtgpu_index_add_parents, the _nested_path:_root term). The node holds exactly one MUST clause, the child query,
+ * which the caller builds as the reference does: a BOOL node {FILTER _nested_path:<path>, MUST child}. min_should_match
+ * holds the score mode (the proto's NestedQuery.ScoreMode): NONE 0, AVG 1, MAX 2, MIN 3, SUM 4; tie_breaker, boost and
+ * min_score are not read. The child query is evaluated WITHOUT live docs (the child scorer does not read acceptDocs); a
+ * matching child c joins the smallest parent doc > c, and joins nothing when it is itself a parent or follows the image's
+ * last parent. A parent with n >= 1 joined children of float scores s_1..s_n (child doc order) matches and scores
+ *   NONE: 0.0f;  SUM: (float) of the double sum in child order;  AVG: (float)(double sum / n);  MAX / MIN: the largest /
+ *   smallest s_i,
+ * and is then a hit as any doc is (its own liveness applies). Boosts above the node fold through it into the child query's
+ * leaves; the node has no boost of its own. Under FILTER, MUST_NOT or CONSTANT, or with NONE, the child query only has to
+ * match (a MIN_SCORE node inside it still scores its own subtree). Joins may appear at any depth and under every occur,
+ * but not inside a child query. Each join is built on the device by the call (once by a prepared batch): the child query
+ * runs over every slice, its matches are sorted and folded into one (parent, score) list per join, and the parent query
+ * reads that list as a term slot. Like the multi-phrase unions' build, this runs when the batch is built and does not
+ * check the search deadline, and the child matches count toward no totalHits or terminateAfter.
+ * Limits: the tree limits (8 term slots, 8 nodes, 32 clauses, 4 levels) apply to the parent tree, where each join takes
+ * one term slot and one clause, and separately to each child tree, rooted at the join's clause. Before any launch, each
+ * join's child matches are bounded by the postings of its child query's driver lists (a multi-phrase union slot at its
+ * gathered postings; a query without a driver list at the image's doc count); a call whose bounds sum to more than 2^26
+ * is refused. The join scratch takes 40 bytes per bounded child (sort keys and scores, double-buffered; run heads and
+ * their scan; the entries behind the union entries), plus the sort's temporary storage. It belongs to the batch that runs the call and, like the union scratch, only grows.
+ * NRTGPU_JOIN_CHILDREN, read when the context is created, lowers the cap (> 0).
+ *   NRTGPU_ERR_INVALID:     a NESTED node without exactly one clause or whose clause is not MUST, a score mode outside
+ *                           0..4, an image without parents ("index has no parent docs: nrtgpu_index_add_parents");
+ *   NRTGPU_ERR_UNSUPPORTED: a NESTED node inside a join's child query, the join cap, a tree limit of the parent tree or
+ *                           of a child tree.
+ * A refused call writes no output and launches nothing. Accepted by nrtgpu_search_tree, nrtgpu_search_tree_phrases,
+ * nrtgpu_batch_prepare_tree[_phrases], nrtgpu_search_tree_aggs, nrtgpu_searcher_search_tree_phrases and
+ * nrtgpu_searcher_search_tree_aggs (every leaf with its own parents: blocks never straddle leaves); tree rescoring
+ * (nrtgpu_score_docs_tree, nrtgpu_rescore_query_tree) answers "bad node kind". */
 enum { NRTGPU_NODE = 3 };
-enum { NRTGPU_NODE_BOOL = 0, NRTGPU_NODE_DISMAX = 1, NRTGPU_NODE_CONSTANT = 3, NRTGPU_NODE_MIN_SCORE = 4 };
+enum { NRTGPU_NODE_BOOL = 0, NRTGPU_NODE_DISMAX = 1, NRTGPU_NODE_CONSTANT = 3, NRTGPU_NODE_MIN_SCORE = 4,
+       NRTGPU_NODE_NESTED = 6 };
+enum { NRTGPU_NESTED_NONE = 0, NRTGPU_NESTED_AVG = 1, NRTGPU_NESTED_MAX = 2, NRTGPU_NESTED_MIN = 3, NRTGPU_NESTED_SUM = 4 };
 typedef struct {
-  int32_t kind;                      /* NRTGPU_NODE_BOOL / _DISMAX / _CONSTANT / _MIN_SCORE */
+  int32_t kind;                      /* NRTGPU_NODE_BOOL / _DISMAX / _CONSTANT / _MIN_SCORE / _NESTED */
   int32_t clause_begin, clause_end;  /* its clauses in the same clauses[] array */
-  int32_t min_should_match;          /* BOOL */
+  int32_t min_should_match;          /* BOOL; NESTED: the score mode */
   float tie_breaker;                 /* DISMAX: tieBreakerMultiplier, in [0, 1] */
   float boost;                       /* CONSTANT / MIN_SCORE (BOOL and DISMAX do not read it) */
   float min_score;                   /* MIN_SCORE: the threshold, >= 0 or NaN */
@@ -237,6 +272,12 @@ int nrtgpu_batch_prepare_tree(nrtgpu_index* ix, const nrtgpu_clause* clauses, in
  * 4 B per posting and 8 B per term). NRTGPU_ERR_INVALID: a wrong count, a negative position, positions that descend
  * within a posting. */
 int nrtgpu_index_add_positions(nrtgpu_index* ix, const int32_t* positions, int64_t n_positions);
+
+/* The parent docs of an image's blocks (NRTGPU_NODE_NESTED): the docs of term root_term (the _nested_path:_root term,
+ * QueryBitSetProducer of the reference's IndexState), as a bitset on the device (N / 8 bytes, counted by
+ * nrtgpu_index_device_bytes). It stays valid across nrtgpu_index_set_live_docs and nrtgpu_index_update_stats; a second
+ * call replaces it. NRTGPU_ERR_INVALID: a term out of range. */
+int nrtgpu_index_add_parents(nrtgpu_index* ix, int32_t root_term);
 
 /* Keyword columns of an image (string doc values of atom / text-with-docValues fields: SortedDocValues and
  * SortedSetDocValues of the leaf). Column k of the call is keyword column k of the image; terms aggregations name it with

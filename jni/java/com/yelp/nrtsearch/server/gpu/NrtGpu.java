@@ -50,10 +50,11 @@ public final class NrtGpu {
       ByteBuffer outHitTimeout, ByteBuffer outTerminatedEarly);
 
   /**
-   * Query trees (nested BooleanQuery / DisjunctionMaxQuery / ConstantScoreQuery / MinScoreQuery): nodes =
-   * nrtgpu_node[nNodes] (28 bytes each: int kind (0 BOOL, 1 DISMAX, 3 CONSTANT, 4 MIN_SCORE), clauseBegin, clauseEnd,
-   * minShouldMatch, float tieBreaker, boost, minScore), referenced by clauses of kind 3 (NODE); otherwise as
-   * searchBoolEx, which it is with nNodes == 0.
+   * Query trees (nested BooleanQuery / DisjunctionMaxQuery / ConstantScoreQuery / MinScoreQuery / NestedQuery): nodes =
+   * nrtgpu_node[nNodes] (28 bytes each: int kind (0 BOOL, 1 DISMAX, 3 CONSTANT, 4 MIN_SCORE, 6 NESTED), clauseBegin,
+   * clauseEnd, minShouldMatch (NESTED: the score mode, 0 NONE 1 AVG 2 MAX 3 MIN 4 SUM), float tieBreaker, boost,
+   * minScore), referenced by clauses of kind 3 (NODE); a NESTED node holds one MUST clause, the child query
+   * {FILTER _nested_path:path, MUST child}, and needs addParents; otherwise as searchBoolEx, which it is with nNodes == 0.
    */
   public static native int searchTree(
       long index, ByteBuffer clauses, int nClauses, ByteBuffer nodes, int nNodes, ByteBuffer queries, int nq,
@@ -66,6 +67,12 @@ public final class NrtGpu {
    * positions of each posting ascending (PostingsEnum.nextPosition() with PostingsEnum.POSITIONS).
    */
   public static native int addPositions(long index, ByteBuffer positions, long nPositions);
+
+  /**
+   * The parent docs of the image's blocks (NESTED nodes): the docs of term rootTerm (_nested_path:_root), kept as a
+   * bitset on the device across live-doc and statistics refreshes.
+   */
+  public static native int addParents(long index, int rootTerm);
 
   /**
    * Keyword columns of an image, read per leaf from SortedDocValues / SortedSetDocValues when the image is built: column k

@@ -113,6 +113,9 @@ JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_addPositions(JN
                                                                                jlong nPositions) {
   return fail(env, nrtgpu_index_add_positions((nrtgpu_index*)(intptr_t)ix, (const int32_t*)ADDR(env, positions), nPositions));
 }
+JNIEXPORT jint JNICALL Java_com_yelp_nrtsearch_server_gpu_NrtGpu_addParents(JNIEnv* env, jclass c, jlong ix, jint rootTerm) {
+  return fail(env, nrtgpu_index_add_parents((nrtgpu_index*)(intptr_t)ix, rootTerm));
+}
 /* keyword columns (SortedDocValues / SortedSetDocValues of the leaf), column k from element k of each array: termBytes,
  * termOffsets (int64[nTerms + 1]), ords (int32) and docOffsets (int64[maxDoc + 1], SORTED_SET; null for SORTED) are direct
  * ByteBuffers */

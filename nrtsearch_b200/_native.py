@@ -125,8 +125,9 @@ class Query(C.Structure):
 
 
 class Node(C.Structure):
-    """nrtgpu_node: a nested BooleanQuery (kind 0), DisjunctionMaxQuery (kind 1), ConstantScoreQuery (kind 3) or
-    MinScoreQuery (kind 4) of a query tree; boost is that of kinds 3 and 4, min_score that of kind 4."""
+    """nrtgpu_node: a nested BooleanQuery (kind 0), DisjunctionMaxQuery (kind 1), ConstantScoreQuery (kind 3),
+    MinScoreQuery (kind 4) or NestedQuery (kind 6, a block join whose score mode is min_should_match) of a query tree;
+    boost is that of kinds 3 and 4, min_score that of kind 4."""
     _fields_ = [("kind", C.c_int32), ("clause_begin", C.c_int32), ("clause_end", C.c_int32), ("min_should_match", C.c_int32),
                 ("tie_breaker", C.c_float), ("boost", C.c_float), ("min_score", C.c_float)]
 
@@ -152,7 +153,7 @@ NRTGPU_SYMBOLS = [
     "nrtgpu_search_knn_filtered", "nrtgpu_knn_filter_stats",
     "nrtgpu_sort_order_create", "nrtgpu_sort_order_device_bytes", "nrtgpu_sort_order_close", "nrtgpu_search_sorted_fields",
     "nrtgpu_search_tree", "nrtgpu_batch_prepare_tree",
-    "nrtgpu_index_add_positions", "nrtgpu_search_tree_phrases", "nrtgpu_batch_prepare_tree_phrases",
+    "nrtgpu_index_add_positions", "nrtgpu_index_add_parents", "nrtgpu_search_tree_phrases", "nrtgpu_batch_prepare_tree_phrases",
     "nrtgpu_score_docs_tree", "nrtgpu_rescore_query_tree",
     "nrtgpu_search_bool_aggs_nested",
     "nrtgpu_sorted_packed_words", "nrtgpu_search_sorted_fields_packed", "nrtgpu_merge_sorted_packed",
@@ -211,6 +212,7 @@ def gpu_lib() -> C.CDLL:
                                                   C.POINTER(Query), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                                   C.POINTER(C.c_void_p)]
         lib.nrtgpu_index_add_positions.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+        lib.nrtgpu_index_add_parents.argtypes = [C.c_void_p, C.c_int32]
         lib.nrtgpu_index_add_keyword_columns.argtypes = [C.c_void_p, C.POINTER(KeywordColumn), C.c_int32]
         lib.nrtgpu_index_keyword_term.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]
         lib.nrtgpu_searcher_keyword_term.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32),

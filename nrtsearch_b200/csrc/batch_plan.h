@@ -111,6 +111,13 @@ constexpr int kMaxUnionAlternatives = 128;        // alternatives of one multi-p
 constexpr int64_t kMaxUnionPostings = 1ll << 25;  // postings the distinct unions of one call gather (52 B each of scratch)
 constexpr int64_t kMaxUnionPositions = 1ll << 27; // positions the distinct phrase-position unions of one call merge (4 B each)
 
+// Block joins of tree batches (NRTGPU_NODE_NESTED). compile_tree compiles each join's child query as an extra query of the
+// batch, after the request's nq (query nq + j is join j's), and the clause that referenced the join as a term slot of
+// plane kUnionList whose list is the join's (parent, score) entries, built on the device behind the union entries
+// (join_kernel.cuh; the host writes the join's index into post_base, join_patch_kernel the range). Each join's child
+// matches are bounded by the postings of its child query's driver lists, and the bounds of one call by kMaxJoinChildren.
+constexpr int64_t kMaxJoinChildren = 1ll << 26;   // bounded child matches of one call (40 B each of scratch)
+
 struct DevQuery {
   int32_t clause_begin, n_clauses;
   int32_t n_term;          // number of term clauses (= slots used)

@@ -25,7 +25,11 @@
 // agg_collect with its score, where pass 2 counts it, as the probe kernel's generic instantiation does.
 // Multi-phrase unions (tree batches whose term slots include call unions, bool_window_union_kernel): a union slot's list is
 // the call's union entries (union_kernel.cuh) instead of the image's postings, a presence byte in pass 1; the phrase
-// matcher reads its merged positions and a scoring one-position slot its entry's score (query_eval.cuh SmemUnions).
+// matcher reads its merged positions and a scoring one-position slot its entry's score (query_eval.cuh SmemUnions). A
+// block join's (parent, score) entries (join_kernel.cuh) are read the same way.
+// Child pass of block joins (bool_window_emit_kernel): the tree, union-capable body with kEmit, run over the joins' child
+// queries; every match is appended to the call's join keys instead of offered to a top-k, with no theta, no slice lists,
+// no totalHits and no deadline (it runs when the batch is built, as the union build does).
 #pragma once
 #include <type_traits>
 #include "query_eval.cuh"
@@ -94,6 +98,14 @@ struct BoolTreeSmemU : BoolTreeSmem {
   UnionView u;
 };
 template <> struct SmemUnions<BoolTreeSmemU> : std::true_type {};
+// the child pass of block joins: where its matches go (query q is join q - join_q0's child query)
+struct BoolLaunchJ : BoolLaunchU {
+  uint64_t* emit_keys;          // [emit_cap] (join << 32 | child doc)
+  float* emit_scores;           // [emit_cap]
+  unsigned int* emit_count;
+  int64_t emit_cap;
+  int32_t join_q0;
+};
 
 // the list of a term slot: the image's postings, or (kUnion) the call's union entries
 template <bool kUnion, class Launch>
@@ -151,8 +163,9 @@ __device__ __forceinline__ bool evaluate_doc(const DevIndexView& ix, const BoolT
 
 // kTree: a tree batch (sm holds the query's nodes, evaluate_doc walks them); otherwise flat BooleanQuerys.
 // kAggs: every matching doc also goes to the collectors of L.aggs (the other instantiations never read it); kMulti: they
-// count a SORTED_SET keyword column (agg_collect<true>); kUnion (tree batches): term slots may be call unions (L.u)
-template <bool kTree, bool kAggs, bool kMulti, bool kUnion, class Launch>
+// count a SORTED_SET keyword column (agg_collect<true>); kUnion (tree batches): term slots may be call unions (L.u);
+// kEmit (the child pass of block joins, BoolLaunchJ): every match is appended to L.emit_* instead
+template <bool kTree, bool kAggs, bool kMulti, bool kUnion, class Launch, bool kEmit = false>
 __device__ __forceinline__ void bool_window_body(const Launch& L, unsigned char* smem_raw) {
   using Smem = typename std::conditional<kUnion, BoolTreeSmemU, typename std::conditional<kTree, BoolTreeSmem, BoolSmem>::type>::type;
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
@@ -166,9 +179,13 @@ __device__ __forceinline__ void bool_window_body(const Launch& L, unsigned char*
     if (tid == 0) {
       sm.q = L.queries[qi];
       sm.cand_count = 0;
-      sm.theta = *(volatile unsigned long long*)&L.theta[qi];
-      sm.skip = L.deadline_ns && deadline_passed(L.deadline_ns, L.clock0);
-      if (sm.skip) L.timed_out[qi] = 1;
+      if constexpr (kEmit) {
+        sm.theta = 0ull; sm.skip = 0;
+      } else {
+        sm.theta = *(volatile unsigned long long*)&L.theta[qi];
+        sm.skip = L.deadline_ns && deadline_passed(L.deadline_ns, L.clock0);
+        if (sm.skip) L.timed_out[qi] = 1;
+      }
       if constexpr (kTree) {
         sm.n_nodes = L.node_begin[qi + 1] - L.node_begin[qi];
         sm.n_phrases = L.phrase_begin ? L.phrase_begin[qi + 1] - L.phrase_begin[qi] : 0;
@@ -239,6 +256,20 @@ __device__ __forceinline__ void bool_window_body(const Launch& L, unsigned char*
       // ---------------- pass 2: emit
       auto offer = [&](bool matched, int32_t doc, float score) {
         // converged call (all lanes of the warp)
+        if constexpr (kEmit) {   // a warp-aggregated append of the warp's matches
+          const unsigned bal = __ballot_sync(0xffffffffu, matched);
+          if (bal) {
+            unsigned int base = 0;
+            if (lane == 0) base = atomicAdd(L.emit_count, (unsigned int)__popc(bal));
+            base = __shfl_sync(0xffffffffu, base, 0);
+            const int64_t at = (int64_t)base + __popc(bal & ((1u << lane) - 1));
+            if (matched && at < L.emit_cap) {
+              L.emit_keys[at] = ((uint64_t)(uint32_t)(qi - L.join_q0) << 32) | (uint32_t)doc;
+              L.emit_scores[at] = score;
+            }
+          }
+          return;
+        }
         bool is_cand = false;
         uint64_t key = 0;
         if (matched) {
@@ -256,6 +287,7 @@ __device__ __forceinline__ void bool_window_body(const Launch& L, unsigned char*
         }
       };
       auto round_end = [&]() {
+        if constexpr (kEmit) return;
         cand_ub += kThreads;
         if (cand_ub > kCandCap - kThreads) {
           __syncthreads();
@@ -320,6 +352,7 @@ __device__ __forceinline__ void bool_window_body(const Launch& L, unsigned char*
       }
     }
     // ---------------- finish the work item
+    if constexpr (kEmit) continue;
     flush_top_k(sm.cand, sm.cand_count, kCandCap, L.top_k, 0ull, &L.theta[qi], sm.theta);
     const int keep = sm.cand_count;
     uint64_t* out = L.slice_keys + ((size_t)qi * L.n_slices + slice) * L.top_k;
@@ -342,6 +375,12 @@ template <bool kAggs, bool kMulti = false>
 __global__ void __launch_bounds__(kThreads, 2) bool_window_union_kernel(const __grid_constant__ BoolLaunchU L) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   bool_window_body<true, kAggs, kMulti, true>(L, smem_raw);
+}
+
+// the child pass of block joins (shared memory: sizeof(BoolTreeSmemU))
+__global__ void __launch_bounds__(kThreads, 2) bool_window_emit_kernel(const __grid_constant__ BoolLaunchJ L) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  bool_window_body<true, false, false, true, BoolLaunchJ, true>(L, smem_raw);
 }
 
 // ---- per-query merge of the slice lists (TopDocs.merge semantics: key order is total) ----

@@ -2,6 +2,7 @@
 // batch compilation, kernel launches. No CPU fallback: every entry point needs a CUDA device.
 #include "../../include/nrtgpu.h"
 #include "bool_kernel.cuh"
+#include "join_kernel.cuh"
 #include "probe_kernel.cuh"
 #include "sort_kernel.cuh"
 #include "collect_kernel.cuh"
@@ -181,6 +182,9 @@ struct nrtgpu_index {
   DevBuf<uint32_t> pos_off;         // [P] first position of each posting, relative to its term's base
   DevBuf<int64_t> pos_base;         // [n_terms + 1] first position of each term
   std::vector<int64_t> h_pos_base;  // ... its host copy (the multi-phrase unions' positions cap)
+  DevBuf<uint32_t> parent_bits;     // the parent docs of the image's blocks (nrtgpu_index_add_parents)
+  bool has_parents = false;
+  int64_t n_parents = 0;
   std::vector<std::unique_ptr<DevBuf<uint8_t>>> norms;
   DevBuf<const uint8_t*> norms_ptrs;
   DevBuf<float> caches;
@@ -260,6 +264,7 @@ struct nrtgpu_index {
     d.n_keyword = (int32_t)kw.size(); d.kw_n_terms = kw_n_terms.data();
     d.term_pos = has_positions ? h_pos_base.data() : nullptr;
     d.max_union_postings = ctx->plan.union_postings;
+    d.has_parents = has_parents; d.n_parents = n_parents; d.max_join_children = ctx->plan.join_children;
     return d;
   }
   KnnCorpus knn_corpus() const {   // what the kNN stages read; NRTGPU_KNN_SIMT, read on every call, forces the fp32 SIMT stage
@@ -322,6 +327,14 @@ struct nrtgpu_batch {
   DevBuf<int32_t> u_vals[2], u_head, u_incl, u_docs, u_first, u_npos, u_pos_off, u_positions;
   DevBuf<float> u_score;
   UnionView u_view = {};
+  int64_t u_gathered = 0;         // the union postings gathered: the join entries start there in u_docs / u_score
+  // block joins of the batch (join_kernel.cuh), rebuilt by every batch_build that has some: the child pass's work items,
+  // the joins' modes and clauses, the emitted keys and scores (double buffers), the run heads and their scan
+  DevBuf<int32_t> j_work_query, j_work_slice, j_clause, j_head, j_incl;
+  DevBuf<uint8_t> j_mode, j_temp;
+  DevBuf<uint64_t> j_keys[2];
+  DevBuf<float> j_scores[2];
+  DevBuf<unsigned int> j_count;
   DevBuf<int32_t> pruned;    // [nq] relation GTE flags
   DevBuf<int32_t> terminated; // [nq] terminateAfter cut the query short
   DevBuf<int32_t> timed_out;  // [nq] a work item of the query was skipped because the deadline had passed
@@ -456,6 +469,7 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   { const char* e = getenv("NRTGPU_ITEM_SHARE"); if (e && atoll(e) > 0) c->plan.item_share = atoll(e); }
   { const char* e = getenv("NRTGPU_ITEM_SHARE_FULL"); if (e && atoll(e) > 0) c->plan.item_share_full = atoll(e); }
   { const char* e = getenv("NRTGPU_UNION_POSTINGS"); if (e && atoll(e) > 0) c->plan.union_postings = std::min<int64_t>(atoll(e), kMaxUnionPostings); }
+  { const char* e = getenv("NRTGPU_JOIN_CHILDREN"); if (e && atoll(e) > 0) c->plan.join_children = std::min<int64_t>(atoll(e), kMaxJoinChildren); }
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmem)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolSmem)));
@@ -465,6 +479,7 @@ int nrtgpu_init(int device_id, nrtgpu_ctx** out) {
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_union_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmemU)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_union_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmemU)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_union_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmemU)));
+  NRT_CUDA_TRY(cudaFuncSetAttribute(bool_window_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BoolTreeSmemU)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<false, false, v3::kCtasA, v3::kStageA, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)sizeof(v3::ProbeSmemT<v3::kStageA>)));
   NRT_CUDA_TRY(cudaFuncSetAttribute(v3::posting_probe_kernel<false, false, v3::kCtasB, v3::kStageB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -785,6 +800,26 @@ int nrtgpu_index_add_positions(nrtgpu_index* ix, const int32_t* positions, int64
   return NRTGPU_OK;
 }
 
+int nrtgpu_index_add_parents(nrtgpu_index* ix, int32_t root_term) {
+  if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_parents: NULL index");
+  if (root_term < 0 || root_term >= ix->n_terms) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_parents: term id out of range");
+  NRT_CUDA_TRY(cudaSetDevice(ix->ctx->device));
+  NRT_CUDA_TRY(cudaDeviceSynchronize());   // searches in flight on this image finish against the old parents
+  const int64_t old_bytes = (int64_t)ix->parent_bits.bytes();
+  const size_t words = std::max<size_t>(((size_t)ix->n_docs + 31) / 32, 1);
+  int rc;
+  if ((rc = ix->parent_bits.alloc(words))) return rc;
+  NRT_CUDA_TRY(cudaMemset(ix->parent_bits.p, 0, words * sizeof(uint32_t)));
+  const int64_t p0 = ix->term_off[(size_t)root_term], np = ix->term_off[(size_t)root_term + 1] - p0;
+  if (np > 0) parent_bits_kernel<<<(unsigned)((np + 255) / 256), 256>>>(ix->post_docs.p + p0, np, ix->parent_bits.p);
+  NRT_CUDA_TRY(cudaGetLastError());
+  NRT_CUDA_TRY(cudaDeviceSynchronize());
+  ix->device_bytes += (int64_t)ix->parent_bits.bytes() - old_bytes;
+  ix->n_parents = np;
+  ix->has_parents = true;
+  return NRTGPU_OK;
+}
+
 int nrtgpu_index_add_keyword_columns(nrtgpu_index* ix, const nrtgpu_keyword_column* cols, int32_t n) {
   if (!ix) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_keyword_columns: NULL index");
   if (ix->kw_added) NRT_FAIL(NRTGPU_ERR_INVALID, "nrtgpu_index_add_keyword_columns: the image already has its keyword columns");
@@ -925,8 +960,9 @@ static int union_build(nrtgpu_batch* b, nrtgpu_index* ix, cudaStream_t st) {
       (rc = b->u_clause.upload_async(cb.union_clause.data(), cb.union_clause.size(), st))) return rc;
   const size_t n1 = (size_t)std::max<int64_t>(S, 1);
   for (int i = 0; i < 2; ++i) if ((rc = b->u_keys[i].alloc(n1)) || (rc = b->u_vals[i].alloc(n1))) return rc;
-  if ((rc = b->u_head.alloc(n1)) || (rc = b->u_incl.alloc(n1)) || (rc = b->u_docs.alloc(n1)) || (rc = b->u_first.alloc(n1)) ||
-      (rc = b->u_score.alloc(n1)) || (rc = b->u_npos.alloc(n1 + 1)) || (rc = b->u_pos_off.alloc(n1 + 1)) ||
+  // (the entries of the batch's joins follow the union entries: join_build)
+  if ((rc = b->u_head.alloc(n1)) || (rc = b->u_incl.alloc(n1)) || (rc = b->u_docs.alloc(n1 + cb.join_bound)) || (rc = b->u_first.alloc(n1)) ||
+      (rc = b->u_score.alloc(n1 + cb.join_bound)) || (rc = b->u_npos.alloc(n1 + 1)) || (rc = b->u_pos_off.alloc(n1 + 1)) ||
       (rc = b->u_positions.alloc((size_t)std::max<int64_t>(cb.union_positions, 1)))) return rc;
   NRT_CUDA_TRY(cudaMemsetAsync(b->u_npos.p, 0, (n1 + 1) * sizeof(int32_t), st));
   UnionBuildLaunch U{};
@@ -974,6 +1010,76 @@ static int union_build(nrtgpu_batch* b, nrtgpu_index* ix, cudaStream_t st) {
     NRT_CUDA_TRY(cudaGetLastError());
   }
   b->u_view = UnionView{b->u_docs.p, b->u_score.p, b->u_pos_off.p, b->u_positions.p};
+  b->u_gathered = S;
+  return NRTGPU_OK;
+}
+
+// The block joins of a compiled batch (join_kernel.cuh) into the entry arrays behind its union entries (union_build ran
+// first and sized them), and every join clause's entry range into its uploaded clauses; asynchronous on `st`. The child
+// pass reads the image without its live docs and runs when the batch is built, without the search deadline. The scratch
+// is sized by the joins' bounded child matches (CompiledBatch::join_bound, capped by compile_tree): the keys beyond the
+// matches keep the sentinel ~0, which sorts after every real key, so the host never reads the match count back.
+static int join_build(nrtgpu_batch* b, nrtgpu_index* ix, cudaStream_t st) {
+  const CompiledBatch& cb = b->cb;
+  const WorkPlan& p = b->plan;
+  const int64_t n = cb.join_bound;
+  const size_t n1 = (size_t)std::max<int64_t>(n, 1);
+  const int64_t base = cb.n_unions() > 0 ? b->u_gathered : 0;
+  int rc;
+  if (cb.n_unions() == 0) {
+    if ((rc = b->u_docs.alloc(n1)) || (rc = b->u_score.alloc(n1))) return rc;
+    b->u_view = UnionView{b->u_docs.p, b->u_score.p, nullptr, nullptr};
+  }
+  if ((rc = b->j_work_query.upload_async(p.join_query.data(), p.join_query.size(), st)) ||
+      (rc = b->j_work_slice.upload_async(p.join_slice.data(), p.join_slice.size(), st)) ||
+      (rc = b->j_clause.upload_async(cb.join_clause.data(), cb.join_clause.size(), st)) ||
+      (rc = b->j_mode.upload_async(cb.join_mode.data(), cb.join_mode.size(), st))) return rc;
+  for (int i = 0; i < 2; ++i) if ((rc = b->j_keys[i].alloc(n1)) || (rc = b->j_scores[i].alloc(n1))) return rc;
+  if ((rc = b->j_head.alloc(n1)) || (rc = b->j_incl.alloc(n1)) || (rc = b->j_count.alloc(1))) return rc;
+  NRT_CUDA_TRY(cudaMemsetAsync(b->j_keys[0].p, 0xff, n1 * sizeof(uint64_t), st));
+  NRT_CUDA_TRY(cudaMemsetAsync(b->j_count.p, 0, sizeof(unsigned int), st));
+  if (!p.join_query.empty()) {   // the child pass
+    BoolLaunchJ L{};
+    L.ix = ix->view(); L.ix.live_bits = nullptr;
+    L.clauses = b->clauses.p; L.queries = b->queries.p;
+    L.work_query = b->j_work_query.p; L.work_slice = b->j_work_slice.p; L.n_work = (int32_t)p.join_query.size();
+    L.n_slices = p.n_slices; L.top_k = b->top_k;
+    L.nodes = b->nodes.p; L.node_begin = b->node_begin.p; L.phrases = b->phrases.p; L.phrase_begin = b->phrase_begin.p;
+    L.aggs = nullptr;
+    L.u = b->u_view;
+    L.emit_keys = b->j_keys[0].p; L.emit_scores = b->j_scores[0].p; L.emit_count = b->j_count.p; L.emit_cap = n;
+    L.join_q0 = cb.nq;
+    bool_window_emit_kernel<<<(unsigned)L.n_work, kThreads, sizeof(BoolTreeSmemU), st>>>(L);
+    NRT_CUDA_TRY(cudaGetLastError());
+  }
+  JoinBuildLaunch J{};
+  J.parent_bits = ix->parent_bits.p; J.n_words = (int32_t)((ix->n_docs + 31) / 32); J.n_joins = cb.n_joins(); J.n = n;
+  J.head = b->j_head.p; J.incl = b->j_incl.p; J.mode = b->j_mode.p; J.base = base;
+  J.docs = b->u_docs.p; J.score = b->u_score.p; J.clauses = b->clauses.p; J.join_clause = b->j_clause.p;
+  J.keys = b->j_keys[0].p; J.scores = b->j_scores[0].p;
+  if (n > 0) {
+    int end_bit = 33;   // the join bits hold every join and the sentinel's all-ones above them
+    while (end_bit < 64 && (1ll << (end_bit - 32)) <= (int64_t)cb.n_joins()) ++end_bit;
+    cub::DoubleBuffer<uint64_t> keys(b->j_keys[0].p, b->j_keys[1].p);
+    cub::DoubleBuffer<float> vals(b->j_scores[0].p, b->j_scores[1].p);
+    size_t tb = 0, ts = 0;
+    NRT_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, vals, (int)n, 0, end_bit, st));
+    NRT_CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, ts, b->j_head.p, b->j_incl.p, thrust::plus<void>(), (int)n, st));
+    if ((rc = b->j_temp.alloc(std::max(tb, ts)))) return rc;
+    tb = b->j_temp.bytes();
+    NRT_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b->j_temp.p, tb, keys, vals, (int)n, 0, end_bit, st));
+    J.keys = keys.Current(); J.scores = vals.Current();
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    join_head_kernel<<<grid, 256, 0, st>>>(J);
+    NRT_CUDA_TRY(cudaGetLastError());
+    ts = b->j_temp.bytes();
+    // (the int scan with thrust::plus that the library already instantiates: cub's InclusiveSum kernels for int spill)
+    NRT_CUDA_TRY(cub::DeviceScan::InclusiveScan(b->j_temp.p, ts, b->j_head.p, b->j_incl.p, thrust::plus<void>(), (int)n, st));
+    join_entry_kernel<<<grid, 256, 0, st>>>(J);
+    NRT_CUDA_TRY(cudaGetLastError());
+  }
+  join_patch_kernel<<<(unsigned)((cb.n_joins() + 127) / 128), 128, 0, st>>>(J);
+  NRT_CUDA_TRY(cudaGetLastError());
   return NRTGPU_OK;
 }
 
@@ -1018,6 +1124,7 @@ static int batch_build(nrtgpu_batch* b, nrtgpu_index* ix, const BatchRequest& r,
   if (b->cb.n_unions() > 0 && (rc = union_build(b, ix, st))) return rc;
   WorkPlan& p = b->plan;
   plan_work(ix->dict(), ix->ctx->plan, b->cb, &p);
+  if (b->cb.n_joins() > 0 && (rc = join_build(b, ix, st))) return rc;
   if ((rc = b->work_query.upload_async(p.work_query.data(), p.work_query.size(), st))) return rc;
   if ((rc = b->work_slice.upload_async(p.work_item.data(), p.work_item.size(), st))) return rc;
   if ((rc = b->known_hits.upload_async(p.known_hits.data(), p.known_hits.size(), st))) return rc;
@@ -1230,7 +1337,7 @@ static int batch_engine_launch(nrtgpu_batch* b, const AggLaunch* aggs, bool mult
   L.deadline_ns = (!p2 && b->limits_active) ? b->deadline_ns : 0; L.clock0 = b->clock0.p; L.timed_out = b->timed_out.p;
   L.aggs = aggs;
   const unsigned grid = (unsigned)b->plan.n_work();
-  if (b->cb.tree && b->cb.n_unions() > 0) {
+  if (b->cb.tree && (b->cb.n_unions() > 0 || b->cb.n_joins() > 0)) {   // union or join slots
     BoolLaunchU LU;
     static_cast<BoolLaunch&>(LU) = L;
     LU.nodes = b->nodes.p; LU.node_begin = b->node_begin.p; LU.phrases = b->phrases.p; LU.phrase_begin = b->phrase_begin.p;
@@ -2022,6 +2129,7 @@ static BatchRequest tree_request(const nrtgpu_clause* clauses, int32_t n_clauses
                                  const nrtgpu_query* queries, int32_t nq, int32_t top_k, int32_t total_hits_threshold, int32_t flags) {
   BatchRequest r{clauses, n_clauses, queries, nq, top_k, total_hits_threshold, flags};
   if (n_nodes > 0) { r.nodes = nodes; r.n_nodes = n_nodes; }
+  r.joins = true;
   return r;
 }
 

@@ -110,6 +110,9 @@ class HostShard:
     # keyword columns (string doc values, nrtgpu_index_add_keyword_columns); keyword column k is TermsCollector(k, ...,
     # field_type="keyword")
     keyword_columns: List[KeywordColumn] = field(default_factory=list)
+    # block joins (NestedQuery): the term every parent doc holds (_nested_path:_root); each parent follows its child docs.
+    # None = an index without nested documents (NestedQuery is refused)
+    parent_term: Optional[int] = None
 
     @property
     def n_terms(self) -> int:
@@ -163,7 +166,7 @@ class HostShard:
             column_has=[None if h is None else np.ascontiguousarray(h[lo:hi]) for h in self.column_has],
             live_docs=None if self.live_docs is None else np.ascontiguousarray(self.live_docs[lo:hi]),
             vectors=sub_vec, vec_similarity=self.vec_similarity, vec_docs=sub_vdocs, post_positions=sub_pos,
-            keyword_columns=[k.doc_range(lo, hi) for k in self.keyword_columns])
+            keyword_columns=[k.doc_range(lo, hi) for k in self.keyword_columns], parent_term=self.parent_term)
 
 
 def _ptr(a: Optional[np.ndarray], typ):

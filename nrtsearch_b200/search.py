@@ -123,6 +123,30 @@ class MinScoreQuery:
     min_score: float
 
 
+_NESTED_SCORE_MODES = {"none": 0, "avg": 1, "max": 2, "min": 3, "sum": 4}
+
+
+@dataclass(frozen=True)
+class NestedQuery:
+    """NestedQuery(query, path_term, score_mode) (QueryNodeMapper.getNestedQuery): a block join. `query` runs over the
+    child docs of the nested path whose _nested_path term is `path_term` (the adaptor's term id), without live docs; each
+    parent doc (HostShard.parent_term, the _nested_path:_root term) that follows matching children matches and scores
+    the fold of their scores: "none" 0, "sum" the double sum in child order, "avg" that sum / n, "max" / "min" the largest /
+    smallest. BoostQuerys around it fold into `query`'s leaves. A node of a query tree (GpuIndexSearcher.search_tree)
+    whose child query is BooleanQuery{FILTER TermQuery(path_term), MUST query}, as the reference builds it."""
+    query: object
+    path_term: int
+    score_mode: str = "none"
+
+    def mode(self) -> int:
+        if self.score_mode not in _NESTED_SCORE_MODES:
+            raise ValueError(f"NestedQuery: unknown score_mode {self.score_mode!r}")
+        return _NESTED_SCORE_MODES[self.score_mode]
+
+    def child_query(self) -> "BooleanQuery":
+        return BooleanQuery().add(TermQuery(int(self.path_term)), Occur.FILTER).add(self.query, Occur.MUST)
+
+
 @dataclass
 class PhraseQuery:
     """PhraseQuery(slop, terms, positions): what match_phrase maps to (QueryNodeMapper.java:285-291, :397-427). All terms on
@@ -532,6 +556,9 @@ def _resolve_keywords(q, searcher):
     if isinstance(q, MinScoreQuery):
         sub = _resolve_keywords(q.query, searcher)
         return q if sub is q.query else MinScoreQuery(sub, q.min_score)
+    if isinstance(q, NestedQuery):
+        sub = _resolve_keywords(q.query, searcher)
+        return q if sub is q.query else NestedQuery(sub, q.path_term, q.score_mode)
     if isinstance(q, ValueSetFilter) and q.field_type == "keyword":
         return _KeywordCodeSet(q.column, tuple(searcher.keyword_seek(q.column, _utf8_bytes(v)) for v in q.values))
     if isinstance(q, FilterCollector):
@@ -673,7 +700,9 @@ def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Opti
     over the batch, whose clauses are one range of the clause array. BoostQuery boosts are folded through the nodes into
     the leaves, outermost first in float, so node clauses carry boost 1 (BoostQuery.createWeight passes boost * this.boost
     down). A ConstantScoreQuery or MinScoreQuery node takes the boost folded down to it as its own and the fold starts again
-    at 1 below it; MinScoreQuery(q, 0) is compiled as q, and a min_score < 0 raises ValueError.
+    at 1 below it; MinScoreQuery(q, 0) is compiled as q, and a min_score < 0 raises ValueError. A NestedQuery is a node of
+    kind 6 (its score mode in min_should_match) over one MUST node, its child query BooleanQuery{FILTER path term, MUST
+    query}; the boost folds through it.
     phrase_table: return (Clause[], n_clauses, Node[], n_nodes, Phrase[], n_phrases, PhraseTerm[], n_phrase_terms, Query[],
     nq) for nrtgpu_search_tree_phrases instead: a PhraseQuery leaf is a clause of kind 4 whose id indexes the phrase table,
     a MultiPhraseQuery (or MatchPhrasePrefixQuery, rewritten) one of kind 6. Without it either is refused."""
@@ -722,6 +751,8 @@ def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Opti
             return 1, [(d, Occur.SHOULD) for d in q.disjuncts], 0, float(q.tie_breaker), b, 0.0, 0.0
         if isinstance(q, ConstantScoreQuery):
             return 3, [(q.filter, Occur.MUST)], 0, 0.0, one, float(b), 0.0
+        if isinstance(q, NestedQuery):   # ToParentBlockJoinQuery.createWeight passes its boost to the child weight
+            return 6, [(q.child_query(), Occur.MUST)], q.mode(), 0.0, b, 0.0, 0.0
         return 4, [(q.query, Occur.MUST)], 0, 0.0, one, float(b), float(q.min_score)
 
     for i, q in enumerate(queries):
@@ -738,7 +769,7 @@ def compile_tree(queries: Sequence[object], search_after: Optional[Sequence[Opti
             children = []
             for sub, occ in cls:
                 s, sb = unwrap(sub, b)
-                if isinstance(s, (BooleanQuery, DisjunctionMaxQuery, ConstantScoreQuery, MinScoreQuery)):
+                if isinstance(s, (BooleanQuery, DisjunctionMaxQuery, ConstantScoreQuery, MinScoreQuery, NestedQuery)):
                     children.append((visit(*parts(s, sb)), None, occ))
                 else:
                     children.append((s, sb, occ))
@@ -827,6 +858,8 @@ class GpuIndex:
         self.keyword_names = _TermNames(self.keyword_term)   # str of terms by ordinal (sorted pages' keyword values)
         if shard.post_positions is not None:
             self.add_positions(shard.post_positions)
+        if shard.parent_term is not None:
+            self.add_parents(shard.parent_term)
         if pinned.n_keyword:
             try:
                 check(self._lib.nrtgpu_index_add_keyword_columns(self.handle, pinned.keyword, pinned.n_keyword))
@@ -855,6 +888,10 @@ class GpuIndex:
         """Term positions of every posting, posting after posting (HostShard.post_positions): what PhraseQuery needs."""
         p = np.ascontiguousarray(positions, np.int32)
         check(self._lib.nrtgpu_index_add_positions(self.handle, p.ctypes.data if len(p) else None, len(p)))
+
+    def add_parents(self, root_term: int):
+        """The parent docs of the image's blocks: the docs of `root_term` (HostShard.parent_term), what NestedQuery needs."""
+        check(self._lib.nrtgpu_index_add_parents(self.handle, int(root_term)))
 
     def sort_order(self, fields: Sequence[SortType], stream: int = 0) -> C.c_void_p:
         """The nrtgpu_sort_order of a Sort, built on first use and kept until close(): it depends on the columns only, so
